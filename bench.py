@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — frames/s of MaGNet's multi-view matching hot path on B200 (BASELINE.json metric).
+"""bench.py — frames/s of MaGNet's multi-view matching hot path on H100 (BASELINE.json metric).
 
 One *step* = one pass of the hot path over one batch of synthetic frames per GPU:
     source repack (NCHW -> PIXC: pixel-major features + Gaussians) + camera table  [once per batch, timed]
@@ -15,9 +15,11 @@ scaling (each rank owns its own batch of 8; the path has no data-path collective
             timed region
   roofline  dominant kernel (cost volume): algorithmic bytes / its CUDA-event duration vs measured HBM peak
   cpu_baseline / --impl reference
-            the reference's CPU path — the unmodified est_costvolume_CW from the vendored baseline/_ref (git-ignored copy of
-            /root/reference made by scripts/vendor_ref.sh; travels with the snapshot), else its bit-identical ATen port —
-            timed on this box's host cores on a bounded sample (1-frame batches)
+            the reference's CPU path — its operator sequence through the bit-identical ATen port oracle/torch_ref.py —
+            timed on the host cores on a bounded sample (1-frame batches)
+
+--dump-outputs DIR writes what the last timed step computed (the updated Gaussians and the last cost volume) as
+float32 .npy files; the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -53,18 +55,7 @@ def measured_peak():
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic(workload, kind=""):
-    """DRAM bytes per launch of the timed cost kernel from the committed ncu --set full capture (profiles/traffic.json:
-    keys "<config>:mma" for the tensor-core kernel, "<config>" for the global-gather kernel, "<config>:tma" for the
-    TMA-staged one), or None."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            return json.load(f).get(workload + (":" + kind if kind else ""))
-    except Exception:
-        return None
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 class ClockSampler:
@@ -159,16 +150,11 @@ def pin_to_gpu_cpus(index):
 
 
 def reference_ops():
-    """The reference's cost-volume function for the baseline legs: the UNMODIFIED models.submodules.homography
-    .est_costvolume_CW (from /root/reference, or its vendored copy baseline/_ref made by scripts/vendor_ref.sh) when
-    available — kind "reference" — else its bit-identical ATen port oracle/torch_ref.py — kind "port".  The sampler
-    (MAGNET.py:154-156) and the update (MAGNET.py:60-69) are inlined in the reference's forward; they are issued here as
-    the same ATen expressions (oracle/torch_ref.py)."""
+    """The reference's cost-volume function for the baseline legs: its bit-identical ATen port oracle/torch_ref.py
+    (tests/test_oracle_golden.py pins it to outputs of the unmodified reference).  The sampler (MAGNET.py:154-156) and
+    the update (MAGNET.py:60-69) are inlined in the reference's forward; they are issued here as the same ATen
+    expressions (oracle/torch_ref.py)."""
     from oracle import torch_ref
-    from oracle.ref_loader import load_reference
-    ref = load_reference()
-    if ref is not None:
-        return ref.homography.est_costvolume_CW, "reference", ref.root
     return torch_ref.cost_volume_cw, "port", "oracle/torch_ref.py"
 
 
@@ -217,8 +203,7 @@ def cpu_reference_frames(frames_cfg, steps, warmup, threads=None, budget_s=None)
             if budget_s is not None and time.perf_counter() - t0 > budget_s:
                 break
         dt = time.perf_counter() - t0
-    what = ("unmodified models.submodules.homography.est_costvolume_CW (%s)" % where if kind == "reference"
-            else "ATen port of the reference operator sequence (%s)" % where)
+    what = "ATen port of the reference operator sequence (%s)" % where
     info = {"cores": cores, "os_cpu_count": os.cpu_count(), "frames": done, "seconds": dt, "kind": kind,
             "sample": f"{done} x 1-frame batch of {WORKLOADS[frames_cfg]} (B=1), {N_ITER} iterations each, "
                       f"{what}, {cores} threads"}
@@ -251,6 +236,8 @@ def main():
     ap.add_argument("--variant", default="auto", choices=["auto", "direct", "cells", "cells_noreuse", "tma", "mma"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gnet", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy (float32)")
     args = ap.parse_args()
 
     from magnet_b200 import dist as md
@@ -273,9 +260,8 @@ def main():
                "cells_noreuse": _lib.VARIANT_CELLS_NOREUSE, "tma": _lib.VARIANT_TMA, "mma": _lib.VARIANT_MMA}[args.variant]
 
     # Weak scaling = the SAME work on every GPU: all ranks build the same seeded batch (each owns its own copy).  With
-    # per-rank seeds the step time followed the poses drawn (the kernel's cost depends on how many bilinear cells a
-    # depth range crosses): +4 % on rank 1, +10 % on one of ranks 2-3 at the same 1965 MHz — that data variance, not
-    # the software, was the 0.91 "scaling efficiency" of round 1 (profiles/r2_scaling.md).
+    # per-rank seeds the step time would follow the poses drawn (the kernel's cost depends on how many bilinear cells a
+    # depth range crosses), not the software.
     inp = make_config(args.config, seed=1)
     B, V, D = inp.B, inp.V, inp.D
     C, H, Wd = inp.ref_feat.shape[1], inp.ref_feat.shape[2], inp.ref_feat.shape[3]
@@ -293,7 +279,6 @@ def main():
     split = variant == _lib.VARIANT_MMA or (variant == _lib.VARIANT_AUTO and C == 64 and V <= 16)
     pixc = variant == _lib.VARIANT_TMA
     layout = _lib.SRC_SPLIT16 if split else (_lib.SRC_PIXC if pixc else _lib.SRC_TILED32)
-    kind = "mma" if split else ("tma" if pixc else "")
     ref_split = None
     if split:
         src_packed = torch.empty(int(_lib.lib().magnet_split16_bytes(V * B, H, Wd)), device=dev, dtype=torch.uint8)
@@ -380,6 +365,13 @@ def main():
         torch.cuda.synchronize()
         graph_ok = bool(torch.equal(graph_pred, eager_pred))
         ms_total = timed(graph.replay, K, sampler)
+        if args.dump_outputs and rank == 0:
+            # what the last replay computed: the Gaussians after N_ITER updates and the last iteration's cost volume
+            # (B x D x H x W fp32 = 39 MB at cfg2, 27 MB at cfg3)
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for name, t in (("gaussians", graph_pred), ("cost_volume", cv)):
+                np.save(os.path.join(args.dump_outputs, name + ".npy"), t.float().cpu().numpy())
         own_ms_step = own["ms"] / K
         launches = launches_per_step * K
         # spread: the same K-step region repeated (median / min / max of the max-over-ranks time per step)
@@ -530,7 +522,7 @@ def main():
     info_variant = _lib.VARIANT_MMA if split else (_lib.VARIANT_CELLS if variant in (_lib.VARIANT_CELLS_NOREUSE, _lib.VARIANT_AUTO) else variant)
     grid, block, smem = ops.cost_launch_info(B, V, D, C, H, Wd, variant=info_variant)
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": ncu_traffic(args.config, kind), "kernel": "cost_mma_kernel<GAUSS,CW> (SPLIT16 planes, tcgen05.mma + TMA windows)" if split else {_lib.VARIANT_DIRECT: "cost_direct_kernel<CW>", _lib.VARIANT_CELLS: "cost_cells_kernel<64,GAUSS,CW> (TILED32 gather)",
+                "kernel": "cost_mma_kernel<GAUSS,CW> (SPLIT16 planes, wgmma + TMA windows)" if split else {_lib.VARIANT_DIRECT: "cost_direct_kernel<CW>", _lib.VARIANT_CELLS: "cost_cells_kernel<64,GAUSS,CW> (TILED32 gather)",
                            _lib.VARIANT_CELLS_NOREUSE: "cost_cells_kernel<64,GAUSS,CW,noreuse>",
                            _lib.VARIANT_TMA: "cost_tma_kernel<64,GAUSS,CW> (PIXC layout, TMA-staged window)"}.get(
                                variant, "cost_cells_kernel<64,GAUSS,CW> (TILED32 gather)"),
@@ -542,7 +534,7 @@ def main():
                 "algorithmic_bytes_per_launch": abytes, "peak_source": peak_src,
                 "launch": {"grid": grid, "block": block, "smem_bytes": smem}}
     # ---- reference-CUDA baseline (north_star / BASELINE.md §2): the reference's operator sequence (repeat,
-    # grid_sample, mul, sum ... — ATen port, bit-identical to the reference on CPU) on the same B200, same inputs
+    # grid_sample, mul, sum ... — ATen port, bit-identical to the reference on CPU) on the same GPU, same inputs
     reference_cuda = None
     if world == 1 and not args.no_cpu_baseline:
         ref_cost_fn, ref_kind, _ = reference_ops()
@@ -596,7 +588,7 @@ def main():
         "data": "synthetic",
         "config": {"workload": WORKLOADS[args.config], "frames_per_step_per_gpu": B, "n_iter": N_ITER, "views": V,
                    "hypotheses": D, "channels": C, "grid": [H, Wd], "depth": inp.meta["depth"], "variant": args.variant,
-                   "cache": "inputs_larger_than_l2 (%.0f MB resident per step vs 126 MB L2)" % ((abytes + 4 * V * B * C * HW) / 1e6),
+                   "cache": "inputs_larger_than_l2 (%.0f MB resident per step vs 50 MB L2)" % ((abytes + 4 * V * B * C * HW) / 1e6),
                    "step": "repack + camera table + %d x (fused cost kernel + update kernel), one CUDA graph per rank, "
                            "K replays timed" % N_ITER},
         "clocks": own_clock,

@@ -11,7 +11,7 @@ upsampled predictions (utils/losses.py:34-50), AdamW, gradient clipping at 1.0, 
 all-reduce per step (magnet_b200.dist.FlatGradAllReduce) instead of DistributedDataParallel.  The frozen
 D-Net / F-Net are replaced by fixed random tensors of their output shapes (they need torch.hub + checkpoints in
 the reference and are out of scope): features (B,64,h,w) / (V*B,64,h,w), Gaussians, x_d3 (B,256,h,w).
-The matching loop runs on the B200 kernels (sampler fused, update kernel with backward)."""
+The matching loop runs on the H100 kernels (sampler fused, update kernel with backward)."""
 import argparse, json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,5 +1,5 @@
 /*
- * magnet_b200.h — C ABI of the B200-native multi-view matching hot path of MaGNet.
+ * magnet_b200.h — C ABI of the H100-native multi-view matching hot path of MaGNet.
  *
  * The reference (baegwangbin/MaGNet) has no FFI layer: its boundary is two Python
  * module-level functions and two inlined blocks (SURVEY §8 b).  Every entry point
@@ -74,7 +74,7 @@ typedef enum magnet_variant {
   MAGNET_VARIANT_TMA = 4,    /* CUDA-core tap-sharing kernel, 4 lanes per pixel, the CTA's source window
                                 staged in shared memory by TMA (MAGNET_SRC_PIXC only)          */
   MAGNET_VARIANT_MMA = 5     /* tensor-core kernel: all (reference pixel, window cell) channel dot products of an
-                                8x8 tile by tcgen05.mma into tensor memory (MAGNET_SRC_SPLIT16 only) */
+                                8x8 tile by wgmma tensor-core MMA (MAGNET_SRC_SPLIT16 only) */
 } magnet_variant;
 
 /* Per (batch element, view) camera constants, 16 floats, produced by magnet_pack_cameras_f32.

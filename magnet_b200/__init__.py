@@ -1,7 +1,7 @@
-"""magnet_b200 — B200-native multi-view matching hot path of MaGNet (baegwangbin/MaGNet).
+"""magnet_b200 — H100-native multi-view matching hot path of MaGNet (baegwangbin/MaGNet).
 
 Only the hot path of SURVEY §8: depth-candidate sampler, plane-sweep warp + bilinear feature
-sampling + depth-consistency weighting + view fusion (one fused sm_100a kernel), Gaussian update,
+sampling + depth-consistency weighting + view fusion (one fused sm_90a kernel), Gaussian update,
 and their reference-facing wrappers.  The CUDA library is mandatory; there is no CPU fallback.
 """
 from . import _lib

@@ -1,7 +1,7 @@
-"""In-tree build of libmagnet_b200.so (sm_100a) with plain nvcc — no torch extension machinery.
+"""In-tree build of libmagnet_b200.so (sm_90a, H100) with plain nvcc — no torch extension machinery.
 
 The C-ABI library has no torch dependency, so it is compiled straight from magnet_b200/csrc/*.cu
-into magnet_b200/libmagnet_b200.so; the built file travels to the GPU box with the repo snapshot.
+into magnet_b200/libmagnet_b200.so (object files and logs under magnet_b200/_build/).
 """
 from __future__ import annotations
 
@@ -19,7 +19,8 @@ BUILD = PKG / "_build"
 LIB = PKG / "libmagnet_b200.so"
 SOURCES = ["api.cu", "cost_mma.cu", "cost_tma.cu", "cost_cells.cu", "cost_direct.cu", "cost_f_bwd.cu", "aux_kernels.cu"]
 HEADERS = [CSRC / "common.cuh", CSRC / "cells_common.cuh", CSRC / "tma_common.cuh", PKG.parent / "include" / "magnet_b200.h"]
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+ARCH = "arch=compute_90a,code=sm_90a"
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", ARCH, "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 
 
@@ -39,7 +40,7 @@ def _digest() -> str:
 
 
 def build(force: bool = False, verbose: bool = False, defines=(), tag: str = "") -> Path:
-    """Compile every .cu for sm_100a and link the shared library.  No-op when up to date.
+    """Compile every .cu for sm_90a and link the shared library.  No-op when up to date.
     ``defines`` / ``tag`` build a tuning variant (e.g. defines=("MAGNET_NCELL=4",), tag="nc4") into
     libmagnet_b200_<tag>.so, selectable at run time with the MAGNET_B200_LIB environment variable."""
     BUILD.mkdir(exist_ok=True)
@@ -64,7 +65,7 @@ def build(force: bool = False, verbose: bool = False, defines=(), tag: str = "")
 
     with ThreadPoolExecutor(max_workers=len(SOURCES)) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(lib), *map(str, objs)]
+    cmd = [nvcc, "-shared", "-gencode", ARCH, "-o", str(lib), *map(str, objs)]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

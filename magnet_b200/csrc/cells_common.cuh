@@ -42,15 +42,15 @@ struct Tap {
   float f, m, s;   // <ref, src>, source mu, source sigma at one integer source pixel (0 when outside)
 };
 
-// <ref, src[tap]> over C channels: C/4 LDG.128 at immediate offsets from one address, packed FMAs.
+// <ref, src[tap]> over C channels: C/4 LDG.128 at immediate offsets from one address, two FMA chains (even / odd channels).
 template <int C>
 __device__ __forceinline__ float tap_dot(const float4* __restrict__ s, const float2 (&ref2)[C / 2]) {
   float2 s0 = make_float2(0.f, 0.f), s1 = make_float2(0.f, 0.f);
 #pragma unroll
   for (int c4 = 0; c4 < C / 4; ++c4) {
     const float4 t = __ldg(s + c4 * 32);
-    s0 = __ffma2_rn(ref2[2 * c4 + 0], make_float2(t.x, t.y), s0);
-    s1 = __ffma2_rn(ref2[2 * c4 + 1], make_float2(t.z, t.w), s1);
+    s0 = ffma2_rn(ref2[2 * c4 + 0], make_float2(t.x, t.y), s0);
+    s1 = ffma2_rn(ref2[2 * c4 + 1], make_float2(t.z, t.w), s1);
   }
   return (s0.x + s0.y) + (s1.x + s1.y);
 }
@@ -72,10 +72,10 @@ __device__ __forceinline__ void tap_dot2(const float4* __restrict__ sa, const fl
     }
 #pragma unroll
     for (int q = 0; q < QB; ++q) {
-      a0 = __ffma2_rn(ref2[2 * (q0 + q) + 0], make_float2(ta[q].x, ta[q].y), a0);
-      a1 = __ffma2_rn(ref2[2 * (q0 + q) + 1], make_float2(ta[q].z, ta[q].w), a1);
-      b0 = __ffma2_rn(ref2[2 * (q0 + q) + 0], make_float2(tb[q].x, tb[q].y), b0);
-      b1 = __ffma2_rn(ref2[2 * (q0 + q) + 1], make_float2(tb[q].z, tb[q].w), b1);
+      a0 = ffma2_rn(ref2[2 * (q0 + q) + 0], make_float2(ta[q].x, ta[q].y), a0);
+      a1 = ffma2_rn(ref2[2 * (q0 + q) + 1], make_float2(ta[q].z, ta[q].w), a1);
+      b0 = ffma2_rn(ref2[2 * (q0 + q) + 0], make_float2(tb[q].x, tb[q].y), b0);
+      b1 = ffma2_rn(ref2[2 * (q0 + q) + 1], make_float2(tb[q].z, tb[q].w), b1);
     }
   }
   fa = (a0.x + a0.y) + (a1.x + a1.y);

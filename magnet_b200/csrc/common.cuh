@@ -1,4 +1,4 @@
-// Shared device helpers for the MaGNet matching kernels (sm_100a).
+// Shared device helpers for the MaGNet matching kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -52,25 +52,31 @@ __device__ __forceinline__ float rcp_nr(float x) {
 
 __device__ __forceinline__ float ldg_f(const float* p) { return __ldg(p); }
 
-// Two hypotheses at once with packed f32x2 instructions (FFMA2 / FADD2 / FMUL2): continuous sample position
-// (ix, iy) = projected pixel - 0.5 (SURVEY A.2 / A.5 #1) and z = depth in the source camera.  Element by element the
-// same IEEE operations as the scalar project() of cells_common.cuh (z = a2 + q2*d separately rounded, 1/(z + 1e-10) =
-// MUFU.RCP + one Newton step), so results are bit-identical to evaluating the two hypotheses one after the other.
+// Element-wise float2 arithmetic, each element one IEEE round-to-nearest operation (sm_90 has no packed f32x2 FMA):
+// the kernels evaluate two hypotheses / two channel partial sums side by side with these.
+__device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+__device__ __forceinline__ float2 fadd2_rn(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+
+// Two hypotheses at once: continuous sample position (ix, iy) = projected pixel - 0.5 (SURVEY A.2 / A.5 #1) and z =
+// depth in the source camera.  Element by element the same IEEE operations as the scalar project() of cells_common.cuh
+// (z = a2 + q2*d separately rounded, 1/(z + 1e-10) = MUFU.RCP + one Newton step), so results are bit-identical to
+// evaluating the two hypotheses one after the other.
 __device__ __forceinline__ void project2(const float2 d, float a0, float a1, float a2, float q0, float q1, float q2,
                                          float2& ix, float2& iy, float2& z) {
-  const float2 P0 = __ffma2_rn(make_float2(q0, q0), d, make_float2(a0, a0));
-  const float2 P1 = __ffma2_rn(make_float2(q1, q1), d, make_float2(a1, a1));
-  // the products are rounded by scalar __fmul_rn: a packed __fmul2_rn feeding __fadd2_rn is contracted into one FFMA2
-  // by the compiler (no FMUL2 in SASS), which would round z once instead of twice
-  z = __fadd2_rn(make_float2(a2, a2), make_float2(__fmul_rn(q2, d.x), __fmul_rn(q2, d.y)));
-  const float2 zp = __fadd2_rn(z, make_float2(1e-10f, 1e-10f));
+  const float2 P0 = ffma2_rn(make_float2(q0, q0), d, make_float2(a0, a0));
+  const float2 P1 = ffma2_rn(make_float2(q1, q1), d, make_float2(a1, a1));
+  // the products are rounded by __fmul_rn, never contracted into an FMA: z is rounded twice, as in the reference
+  z = fadd2_rn(make_float2(a2, a2), make_float2(__fmul_rn(q2, d.x), __fmul_rn(q2, d.y)));
+  const float2 zp = fadd2_rn(z, make_float2(1e-10f, 1e-10f));
   float2 r;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r.x) : "f"(zp.x));
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r.y) : "f"(zp.y));
-  const float2 e = __ffma2_rn(make_float2(-zp.x, -zp.y), r, make_float2(1.0f, 1.0f));
-  r = __ffma2_rn(r, e, r);
-  ix = __ffma2_rn(P0, r, make_float2(-0.5f, -0.5f));
-  iy = __ffma2_rn(P1, r, make_float2(-0.5f, -0.5f));
+  const float2 e = ffma2_rn(make_float2(-zp.x, -zp.y), r, make_float2(1.0f, 1.0f));
+  r = ffma2_rn(r, e, r);
+  ix = ffma2_rn(P0, r, make_float2(-0.5f, -0.5f));
+  iy = ffma2_rn(P1, r, make_float2(-0.5f, -0.5f));
 }
 
 }  // namespace magnet

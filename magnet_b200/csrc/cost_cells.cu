@@ -12,7 +12,7 @@
 // gathers of neighbouring lanes hit neighbouring addresses and the CTA's source footprint stays compact)
 // and owns ONE chunk of JCHUNK = 32 hypotheses (the chunks of a tile are adjacent CTAs).  Per view the work is
 // split into three phases that every lane of a warp executes in LOCKSTEP — a run-per-cell loop would diverge
-// 2.2x on the bench workload (measured by simulation, see DESIGN.md):
+// on the bench workload, where neighbouring pixels cross different numbers of cells:
 //   A  cell list: analytic walk from grid line to grid line in depth space + binary search for the first
 //      hypothesis of each cell (cells_common.cuh: cell_list); exact per-hypothesis walk as the fallback
 //      (d_volume mode, points behind the camera, unsorted k).  Headers in shared memory, at most NCELL per
@@ -34,7 +34,7 @@
 //
 // Numerics (DESIGN.md "parity"): same formulas as the reference, but (i) 1/Zp via MUFU.RCP + one
 // Newton step and ix = P0/Zp - 0.5 folded into one FMA instead of the normalise / clamp /
-// unnormalise round trip, (ii) channel sums re-associated (dot-then-blend, packed f32x2 FMAs),
+// unnormalise round trip, (ii) channel sums re-associated (dot-then-blend, even / odd channel FMA chains),
 // (iii) bilinear polynomial instead of 4 explicit weights, (iv) fp32 view accumulation.  Each
 // changes results at the 1e-6 relative level; the hard consistency threshold can flip for elements
 // within ~1e-5 of it (the reference's own fp32-vs-fp64 flips have the same margins).
@@ -161,8 +161,8 @@ cost_cells_kernel(const __grid_constant__ CostParams p, const int chunk, const i
       const int nmax = __reduce_max_sync(FULL, ncell);
 
       // ---------------- phase B: per-cell records ----------------------------------------------
-      // (A variant where every lane walks its own list of new taps, one or two per iteration, was measured:
-      // same number of gathers within 10 %, less memory-level parallelism, 12 % slower — see DESIGN.md.)
+      // (every lane computes the same tap slot per iteration: its gathers are issued together, which gives more
+      // memory-level parallelism than each lane walking its own list of new taps)
       for (int i = 0; i < nmax; ++i) {
         if (i < ncell) {
           const float2 h = hdr[i * NT + tid];
@@ -233,7 +233,7 @@ cost_cells_kernel(const __grid_constant__ CostParams p, const int chunk, const i
         };
         int j = j_lo;
 #pragma unroll 2
-        for (; j + 1 < j_end; j += 2, ap += 2 * NT, starts >>= 2) {      // two hypotheses per packed (f32x2) projection
+        for (; j + 1 < j_end; j += 2, ap += 2 * NT, starts >>= 2) {      // two hypotheses per float2 projection
           float2 ix2, iy2, z2;
           project2(make_float2(depth_of<MODE>(p, ds, j), depth_of<MODE>(p, ds, j + 1)), a0, a1, a2, q0, q1, q2, ix2, iy2, z2);
           eval(ix2.x, iy2.x, z2.x, (starts & 1u) != 0u, ap);

@@ -1,5 +1,5 @@
 // MAGNET_VARIANT_MMA — tensor-core kernel: fused warp + sample + consistency + view fusion with the channel dot
-// products of a whole (tile, view) computed by tcgen05.mma into tensor memory.
+// products of a whole (tile, view) computed by wgmma (fp32 accumulators in registers).
 //
 // Replaces homography.py:79-161 (and :10-75 with CW == false); absorbs the sampler of MAGNET.py:154-156.
 //
@@ -16,22 +16,23 @@
 //     significant bits per factor, products are exact in the fp32 accumulator (MAGNET_SRC_SPLIT16,
 //     magnet_repack_split16_f32).
 //   * the planes are (image, plane, y, x, 64 channels) fp16 = 128-byte rows: an 8-pixel x 2-plane TMA box with
-//     CU_TENSOR_MAP_SWIZZLE_128B lands as one canonical K-major UMMA atom per plane; the window of a (tile, view) is the
+//     CU_TENSOR_MAP_SWIZZLE_128B lands as one canonical K-major wgmma atom per plane; the window of a (tile, view) is the
 //     bounding box of the tile's sample positions cut into such 8-cell segments (zero fill outside the image =
 //     grid_sample's padding_mode='zeros'), cell index = B-operand row = accumulator column.  The reference tile is the
-//     A operand (rows 0..63 of an M = 128 instruction; rows 64..127 read whatever follows and are never looked at).
+//     A operand (M = 64); warpgroup g computes accumulator columns [128 g, 128 g + 128).
 //   * one warp per tile row (8 pixels in turn), one LANE per hypothesis (lane j: hypotheses j and j + 32 of the
-//     64-hypothesis chunk, packed f32x2 arithmetic across the two): the pixel's constants are warp-uniform (per-warp table
+//     64-hypothesis chunk, evaluated side by side as float2 pairs): the pixel's constants are warp-uniform (per-warp table
 //     in shared memory), the 32 lanes read a handful of neighbouring cells of ONE accumulator row (broadcast /
 //     conflict-free); lanes beyond the last hypothesis replicate it, so there are no activity predicates.
-//   * per view: project all hypotheses (positions cached in registers, exact bounding box) -> TMA window + paired
-//     (mu, sigma) table -> 12 x tcgen05.mma (3 products x 4 K steps) committed to an mbarrier -> tcgen05.ld the 64
-//     accumulator rows into shared memory (over the window, which is dead by then) -> per-hypothesis phase.  The view
+//   * per view: project all hypotheses (exact bounding box) -> TMA window + paired (mu, sigma) table -> 12 x wgmma
+//     m64n128k16 per warpgroup (3 products x 4 K steps) -> the 64 accumulator rows into shared memory (over the window,
+//     which is dead by then) -> per-hypothesis phase, which projects again from the per-warp pixel table (the 32
+//     positions do not fit the registers next to the 64 accumulators).  The view
 //     accumulators live in shared memory (hypothesis-major: the layout the coalesced epilogue reads).
 //   * a window that does not fit 256 cells is cut into sub-windows of <= 32 segments that overlap by one cell column /
 //     row; a hypothesis is evaluated in the sub-window that holds its cell origin.  Same code for any depth distribution.
 //   * persistent CTAs (two per SM): work items (batch element, tile, 64-hypothesis chunk) come from a global counter in a
-//     per-launch slot that the last CTA re-arms (graph-replay safe); barriers and tensor memory are set up once per CTA.
+//     per-launch slot that the last CTA re-arms (graph-replay safe); barriers are set up once per CTA.
 //
 // Numerics: the per-view channel sum is the tensor core's fp32 accumulation of exact products of the split factors
 // (relative error ~2^-21 of sum |ref||src|, the same order as an fp32 FMA chain); everything else — projection, weights,
@@ -55,24 +56,23 @@ constexpr int MPX = MTW * MTH;         // 64 = rows of the accumulator that are 
 constexpr int MCH = 64;                // hypotheses per CTA (two per lane)
 constexpr int MSEG = 32;               // 8-cell segments per window: N <= 256 accumulator columns
 constexpr int MMAXV = 16;              // views whose camera constants are staged in shared memory
-constexpr int M_TMEM_COLS = 256;
 constexpr int SEG_BYTES = 2048;        // hi atom (8 cells x 128 B) + lo atom
 constexpr int META_SEG_BYTES = 128;    // 8 cells x (mu, sigma of the cell and of its right neighbour)
 
 // shared-memory map (bytes from the 1024-aligned base)
 constexpr int MOFF_A = 0;                                   // reference tile: hi 8 KB | lo 8 KB
 constexpr int MOFF_R = 16384;                               // window segments, later the accumulator rows G[64][GP]
-constexpr int MR_BYTES = 67584;                             //   >= 32 * 2048 and >= 64 * 260 * 4
+constexpr int MR_BYTES = 67584;                             //   >= 32 * 2048 and >= 64 * 264 * 4
 constexpr int MOFF_META = MOFF_R + MR_BYTES;                // float4[256] (mu, sigma)[c], (mu, sigma)[c + 1] per window cell
 constexpr int MOFF_CAM = MOFF_META + MSEG * META_SEG_BYTES; // magnet_camera[MMAXV]
 constexpr int MOFF_KS = MOFF_CAM + MMAXV * 64;              // float[MCH]
 constexpr int MOFF_BBOX = MOFF_KS + MCH * 4;                // int[2 slots][4]
-constexpr int MOFF_BAR = MOFF_BBOX + 64;                    // 3 mbarriers, TMEM base address
+constexpr int MOFF_BAR = MOFF_BBOX + 64;                    // 2 mbarriers, next work item
 constexpr int MOFF_ACC = MOFF_BAR + 64;                     // float[MCH][65]: view accumulators, hypothesis-major
 constexpr int MOFF_PIX = MOFF_ACC + MCH * 65 * 4;           // float4[8 warps][8 pixels][2]: (q0,q1,q2,-) (q2,mu,sigma,-)
 constexpr int M_SMEM_USED = MOFF_PIX + 8 * 8 * 32;
 constexpr int M_SMEM_TOTAL = M_SMEM_USED + 1024;            // slack for the 1024-byte alignment of the base
-static_assert(MR_BYTES >= MSEG * SEG_BYTES && MR_BYTES >= MPX * 260 * 4 && MR_BYTES >= MCH * 65 * 4, "region R");
+static_assert(MR_BYTES >= MSEG * SEG_BYTES && MR_BYTES >= MPX * 264 * 4 && MR_BYTES >= MCH * 65 * 4, "region R");
 static_assert(2 * (M_SMEM_TOTAL + 1024) <= 227 * 1024, "two CTAs per SM");
 
 // header of a MAGNET_SRC_SPLIT16 buffer (256 bytes)
@@ -120,14 +120,14 @@ __device__ __forceinline__ float4 lds_f32x4(uint32_t a) {
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
   return v;
 }
-// bilinear interpolation of a (mu, sigma) pair with packed f32x2 instructions; v01 - v00 as fma(v00, -1, v01) (exact
-// product, one rounding = the subtraction)
+// bilinear interpolation of a (mu, sigma) pair; v01 - v00 as fma(v00, -1, v01) (exact product, one rounding = the
+// subtraction)
 __device__ __forceinline__ float2 lerp2d_x2(float4 top, float4 bot, float fx, float fy) {
   const float2 v00 = make_float2(top.x, top.y), v01 = make_float2(top.z, top.w);
   const float2 v10 = make_float2(bot.x, bot.y), v11 = make_float2(bot.z, bot.w);
   const float2 m1 = make_float2(-1.0f, -1.0f), fx2 = make_float2(fx, fx), fy2 = make_float2(fy, fy);
-  const float2 t = __ffma2_rn(fx2, __ffma2_rn(v00, m1, v01), v00), u = __ffma2_rn(fx2, __ffma2_rn(v10, m1, v11), v10);
-  return __ffma2_rn(fy2, __ffma2_rn(t, m1, u), t);
+  const float2 t = ffma2_rn(fx2, ffma2_rn(v00, m1, v01), v00), u = ffma2_rn(fx2, ffma2_rn(v10, m1, v11), v10);
+  return ffma2_rn(fy2, ffma2_rn(t, m1, u), t);
 }
 
 template <int MODE, bool CW>
@@ -144,7 +144,7 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
   float* ks = reinterpret_cast<float*>(smem + MOFF_KS);
   int* bbox = reinterpret_cast<int*>(smem + MOFF_BBOX);
   float* regR = reinterpret_cast<float*>(smem + MOFF_R);
-  const uint32_t bar_tma = sbase + MOFF_BAR, bar_mma = sbase + MOFF_BAR + 8, bar_cam = sbase + MOFF_BAR + 24;
+  const uint32_t bar_tma = sbase + MOFF_BAR, bar_cam = sbase + MOFF_BAR + 24;
   float* acc_s = reinterpret_cast<float*>(smem + MOFF_ACC);
   const unsigned FULL = 0xffffffffu;
 
@@ -159,23 +159,18 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
   const Split16Header* hdr_src = reinterpret_cast<const Split16Header*>(srcbuf);
   volatile int* next_item = reinterpret_cast<volatile int*>(smem + MOFF_BAR + 40);
 
-  // ---- once per CTA: barriers, tensor memory -----------------------------------------------------------------
+  // ---- once per CTA: barriers ---------------------------------------------------------------------------------
   if (tid == 0) {
     mbar_init(bar_tma, 1);
-    mbar_init(bar_mma, 1);
     mbar_init(bar_cam, 1);
     fence_mbar_init();
     prefetch_tmap(&tm_ref);
     prefetch_tmap(&tm_src);
     prefetch_tmap(&tm_meta);
   }
-  if (warp == 1) tmem_alloc(sbase + MOFF_BAR + 32, M_TMEM_COLS);
   if (tid < 8) bbox[tid] = (tid & 1) ? -(1 << 28) : (1 << 28);       // [slot][x_lo, x_hi, y_lo, y_hi]
-  tmem_fence_before_sync();
   __syncthreads();
-  tmem_fence_after_sync();
-  const uint32_t tmem_base = *reinterpret_cast<const volatile uint32_t*>(smem + MOFF_BAR + 32);
-  uint32_t ph_tma = 0, ph_mma = 0, ph_cam = 0;
+  uint32_t ph_tma = 0, ph_cam = 0;
   int it = 0;
   int cur_b = -1;
   const float xmax = (float)W + 1.0f, ymax = (float)H + 1.0f;
@@ -184,7 +179,7 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
 
   // ---- persistent CTA: work items (batch element, tile, hypothesis chunk) are handed out dynamically -----------
   // (the first one is the block index, the others come from a global counter: no tail of a partial last wave, barriers
-  // and tensor memory set up once per SM slot)
+  // set up once per SM slot)
   int item = blockIdx.x;
   while (item < n_items) {
   const int b = item / items_per_b;
@@ -230,7 +225,7 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
   }
   // my two hypotheses of every pixel of the row: (hypothesis jc + lane, hypothesis jc + 32 + lane).  Read from the
   // depth volume they stay in registers; sampled (MAGNET.py:155: multiply, then add) or plane depths are recomputed
-  // from the pixel's Gaussian where needed (2 shuffles + 2 packed instructions instead of 16 registers).
+  // from the pixel's Gaussian where needed (a few instructions instead of 16 registers).
   float2 dvol[MODE == MAGNET_DEPTH_VOLUME ? MTW : 1];
   float2 k2 = make_float2(0.f, 0.f);
   if (MODE == MAGNET_DEPTH_VOLUME) {                       // coalesced read, transposed through shared memory
@@ -248,12 +243,12 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
   } else {
     k2 = make_float2(ks[lane], ks[lane + 32]);
   }
-  // (mu, sigma) come from the warp's pixel table; the product is rounded by scalar __fmul_rn (a packed multiply feeding
-  // a packed add would be contracted into one FFMA2)
+  // (mu, sigma) come from the warp's pixel table; the product is rounded by __fmul_rn so that it is never contracted
+  // into an FMA with the add (the reference rounds twice)
   auto depth2 = [&](const int i, const float mu, const float sg) -> float2 {
     if (MODE == MAGNET_DEPTH_VOLUME) return dvol[i];
     if (MODE == MAGNET_DEPTH_PLANES) return k2;
-    return __fadd2_rn(make_float2(mu, mu), make_float2(__fmul_rn(sg, k2.x), __fmul_rn(sg, k2.y)));
+    return fadd2_rn(make_float2(mu, mu), make_float2(__fmul_rn(sg, k2.x), __fmul_rn(sg, k2.y)));
   };
   float4* pixt = reinterpret_cast<float4*>(smem + MOFF_PIX) + warp * 16;
 
@@ -279,21 +274,23 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
     }
     __syncwarp();
     const int vb = v * p.B + b;
+    // sample position of my two hypotheses of pixel i of the row, clamped: anything left of -1 / right of W (above /
+    // below likewise) has all four taps out of the image, so cells stay near the image and NaN (fmaxf drops it) maps to
+    // "out of bounds"; z = depth in the source camera
+    auto project_px = [&](const int i, float2& ix, float2& iy, float2& z) {
+      const float4 t1 = pixt[2 * i], t2 = pixt[2 * i + 1];   // same address on every lane: broadcast
+      project2(depth2(i, t2.y, t2.z), a0, a1, a2, t1.x, t1.y, t1.z, ix, iy, z);
+      ix.x = fminf(fmaxf(ix.x, -2.0f), xmax); ix.y = fminf(fmaxf(ix.y, -2.0f), xmax);
+      iy.x = fminf(fmaxf(iy.x, -2.0f), ymax); iy.y = fminf(fmaxf(iy.y, -2.0f), ymax);
+    };
 
     // ---------------- projection of every hypothesis, bounding box of the tile's sample positions -------------
-    float2 cix[MTW], ciy[MTW];
+    // (phase C projects again from the pixel table: holding the 32 positions across the MMA would not fit the registers)
     float xl = 1e9f, xh = -1e9f, yl = 1e9f, yh = -1e9f;
 #pragma unroll
     for (int i = 0; i < MTW; ++i) {
-      const float4 t1 = pixt[2 * i], t2 = pixt[2 * i + 1];   // same address on every lane: broadcast
       float2 ix, iy, z;
-      project2(depth2(i, t2.y, t2.z), a0, a1, a2, t1.x, t1.y, t1.z, ix, iy, z);
-      // anything left of -1 / right of W (above / below likewise) has all four taps out of the image: clamp so that
-      // cells stay near the image and NaN (fmaxf drops it) maps to "out of bounds"
-      ix.x = fminf(fmaxf(ix.x, -2.0f), xmax); ix.y = fminf(fmaxf(ix.y, -2.0f), xmax);
-      iy.x = fminf(fmaxf(iy.x, -2.0f), ymax); iy.y = fminf(fmaxf(iy.y, -2.0f), ymax);
-      cix[i] = ix;
-      ciy[i] = iy;
+      project_px(i, ix, iy, z);
       if ((livemask >> i) & 1u) {                          // warp-uniform
         xl = fminf(xl, fminf(ix.x, ix.y)); xh = fmaxf(xh, fmaxf(ix.x, ix.y));
         yl = fminf(yl, fminf(iy.x, iy.y)); yh = fmaxf(yh, fmaxf(iy.x, iy.y));
@@ -336,46 +333,45 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
         }
         __syncwarp();
         const int npad = (nsegs * 8 + 15) & ~15;           // accumulator columns (N % 16 == 0)
-        const int gp = (((npad + 27) >> 5) << 5) + 4;      // row pitch of G in floats: % 32 == 4 (conflict-free stores)
+        const int gp = ((npad + 23) & ~31) + 8;            // row pitch of G in floats: >= npad, % 32 == 8
         mbar_wait_or_trap(bar_tma, ph_tma);                // every thread observes the copies (it reads the table)
         ph_tma ^= 1u;
-        // ---------------- G = ref x window^T: 3 products x 4 K steps, one thread -------------------------------
-        if (warp == 0) {
-          tmem_fence_after_sync();
-          if (lane == 0) {
-            const uint32_t idesc = umma_idesc_f16(128, (uint32_t)npad);
-            const uint64_t a_hi = umma_desc_sw128(sbase + MOFF_A, 1024), a_lo = umma_desc_sw128(sbase + MOFF_A + 8192, 1024);
-            const uint64_t b_hi = umma_desc_sw128(sbase + MOFF_R, SEG_BYTES), b_lo = umma_desc_sw128(sbase + MOFF_R + 1024, SEG_BYTES);
-            uint32_t accum = 0;
+        // ---------------- G = ref x window^T: warpgroup g computes columns [128 g, 128 g + 128) -----------------
+        // (3 products x 4 K steps of m64n128k16; the whole fence .. wait sequence sits inside the warpgroup-uniform
+        // branch, so ptxas keeps the wgmma pipelined)
+        {
+          const int wg = warp >> 2;
+          float acc[64];
+#pragma unroll
+          for (int e = 0; e < 64; ++e) acc[e] = 0.0f;
+          const uint32_t bseg = sbase + MOFF_R + (uint32_t)(wg * 16 * SEG_BYTES);
+          const uint64_t a_hi = gmma_desc_sw128(sbase + MOFF_A, 1024), a_lo = gmma_desc_sw128(sbase + MOFF_A + 8192, 1024);
+          const uint64_t b_hi = gmma_desc_sw128(bseg, SEG_BYTES), b_lo = gmma_desc_sw128(bseg + 1024, SEG_BYTES);
+          __syncwarp();                                      // wgmma is warp-synchronous (.aligned)
+          if (wg == 0 || npad > 128) {                       // CTA-uniform: warpgroup 1 idles on a narrow window
+            wgmma_fence();
 #pragma unroll
             for (int pr = 0; pr < 3; ++pr) {                // small cross terms first
               const uint64_t ad = pr == 0 ? a_lo : a_hi, bd = pr == 1 ? b_lo : b_hi;
 #pragma unroll
-              for (int kk = 0; kk < 4; ++kk) {
-                umma_f16(tmem_base, ad + 2u * kk, bd + 2u * kk, idesc, accum);
-                accum = 1;
-              }
+              for (int kk = 0; kk < 4; ++kk) wgmma_m64n128k16_f16(acc, ad + 2u * kk, bd + 2u * kk, (pr | kk) != 0);
             }
-            umma_commit(bar_mma);
+            wgmma_commit();
+            wgmma_wait_all();
           }
-          __syncwarp();
-        }
-        mbar_wait_or_trap(bar_mma, ph_mma);
-        ph_mma ^= 1u;
-        tmem_fence_after_sync();
-        // ---------------- accumulator rows 0..63 -> shared memory (over the window) ---------------------------
-        if ((warp & 3) < 2) {
-          const int row = (warp & 3) * 32 + lane;
-          float4* grow = reinterpret_cast<float4*>(regR + (size_t)row * gp);
-          for (int cc = warp >> 2; cc * 16 < npad; cc += 2) {
-            float t[16];
-            tmem_ld16(tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(cc * 16), t);
+          __syncthreads();                                   // both warpgroups have read the window: G may overwrite it
+          // accumulator fragment -> G rows (pixels) x columns (cells); gp % 32 == 8 keeps the 8-byte stores conflict-free
+          const int r0 = ((warp & 3) << 4) + (lane >> 2);
+          float* g0 = regR + (size_t)r0 * gp + wg * 128 + 2 * (lane & 3);
 #pragma unroll
-            for (int e = 0; e < 4; ++e) grow[cc * 4 + e] = make_float4(t[4 * e], t[4 * e + 1], t[4 * e + 2], t[4 * e + 3]);
+          for (int j = 0; j < 16; ++j) {
+            if (wg * 128 + 8 * j < npad) {                   // warp-uniform
+              *reinterpret_cast<float2*>(g0 + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
+              *reinterpret_cast<float2*>(g0 + 8 * gp + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+            }
           }
+          __syncthreads();
         }
-        tmem_fence_before_sync();
-        __syncthreads();
 #ifdef MAGNET_MMA_DEBUG
         if (dbg != nullptr && item == 0 && v == 0 && sy == wy0 && sx == wx0) {
           if (tid == 0) {
@@ -402,16 +398,14 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
 #pragma unroll
           for (int i = 0; i < MTW; ++i, rowaddr += (uint32_t)gp * 4u) {
             if (!((livemask >> i) & 1u)) continue;         // warp-uniform
-            // opaque to the optimiser: otherwise floor / fraction of all 8 pixels are hoisted out of the window loop
-            // (they do not depend on it) and held in 64 registers instead of recomputed with 6 instructions
-            asm volatile("" : "+f"(cix[i].x), "+f"(cix[i].y), "+f"(ciy[i].x), "+f"(ciy[i].y));
-            const float2 x = cix[i], y = ciy[i];
+            float2 x, y, z;
+            project_px(i, x, y, z);
             const float2 x0 = make_float2(floorf(x.x), floorf(x.y)), y0 = make_float2(floorf(y.x), floorf(y.y));
             const float2 m1 = make_float2(-1.0f, -1.0f);
-            const float2 fx = __ffma2_rn(x0, m1, x), fy = __ffma2_rn(y0, m1, y);       // x - floor(x), exact
+            const float2 fx = ffma2_rn(x0, m1, x), fy = ffma2_rn(y0, m1, y);       // x - floor(x), exact
             // byte offset of the cell in a G row = 4 * ((y0 - sy) * pitch + (x0 - sx)), in fp32 (small integers, exact)
             // on top of 1.5 * 2^23 so that the integer sits in the mantissa
-            const float2 o = __ffma2_rn(y0, make_float2(pitch4f, pitch4f), __ffma2_rn(x0, make_float2(4.0f, 4.0f), make_float2(c0f, c0f)));
+            const float2 o = ffma2_rn(y0, make_float2(pitch4f, pitch4f), ffma2_rn(x0, make_float2(4.0f, 4.0f), make_float2(c0f, c0f)));
             uint32_t ca = __float_as_uint(o.x) & 0x3fffffu, cb = __float_as_uint(o.y) & 0x3fffffu;
             bool pa = true, pb = true;
             if (!SINGLE) {                                 // evaluated in the sub-window that holds the cell origin
@@ -424,8 +418,8 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
             const float2 g00 = make_float2(lds_f32(ga), lds_f32(gb)), g01 = make_float2(lds_f32(ga + 4), lds_f32(gb + 4));
             const float2 g10 = make_float2(lds_f32(ga + pitch4), lds_f32(gb + pitch4));
             const float2 g11 = make_float2(lds_f32(ga + pitch4 + 4), lds_f32(gb + pitch4 + 4));
-            const float2 ct = __ffma2_rn(fx, __ffma2_rn(g00, m1, g01), g00), cu = __ffma2_rn(fx, __ffma2_rn(g10, m1, g11), g10);
-            const float2 cost = __ffma2_rn(fy, __ffma2_rn(ct, m1, cu), ct);            // both hypotheses at once
+            const float2 ct = ffma2_rn(fx, ffma2_rn(g00, m1, g01), g00), cu = ffma2_rn(fx, ffma2_rn(g10, m1, g11), g10);
+            const float2 cost = ffma2_rn(fy, ffma2_rn(ct, m1, cu), ct);            // both hypotheses at once
             const float costa = cost.x, costb = cost.y;
             bool oka, okb;
             if (CW) {
@@ -433,9 +427,6 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
               // table entry of a cell = (mu, sigma) of the cell and of its right neighbour: two 16-byte reads per hypothesis
               const float2 msa = lerp2d_x2(lds_f32x4(ma), lds_f32x4(ma + pitch4 * 4u), fx.x, fy.x);
               const float2 msb = lerp2d_x2(lds_f32x4(mb), lds_f32x4(mb + pitch4 * 4u), fx.y, fy.y);
-              const float4 t2 = pixt[2 * i + 1];           // (q2, mu, sigma) of the pixel: broadcast
-              const float2 dd = depth2(i, t2.y, t2.z);
-              const float2 z = __fadd2_rn(make_float2(a2, a2), make_float2(__fmul_rn(t2.x, dd.x), __fmul_rn(t2.x, dd.y)));
               // homography.py:157-158: |z - mu~| < sigma~ * kappa, strict
               oka = fabsf(__fsub_rn(z.x, msa.x)) < __fmul_rn(msa.y, kappa);
               okb = fabsf(__fsub_rn(z.y, msb.x)) < __fmul_rn(msb.y, kappa);
@@ -451,7 +442,6 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
         if (single) phase_c(std::true_type{});
         else phase_c(std::false_type{});
         fence_proxy_async();
-        tmem_fence_before_sync();
         __syncthreads();                                   // G / table dead: the next copies and MMAs may overwrite
       }
     }
@@ -499,9 +489,6 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
       __threadfence();
     }
   }
-  tmem_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, M_TMEM_COLS);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -610,6 +597,17 @@ __global__ void __launch_bounds__(256) split16_repack_kernel(const float* __rest
   }
 }
 
+static int sm_count(int dev) {
+  static int cached[64] = {0};
+  int& c = cached[dev & 63];
+  if (c == 0) {
+    int n = 0;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+    c = n;
+  }
+  return c;
+}
+
 cudaError_t launch_repack_split16(const float* src, const float* gmm, void* dst, int N, int C, int H, int W,
                                   cudaStream_t st, int* launches) {
   if (C != 64) return cudaErrorInvalidValue;
@@ -618,7 +616,9 @@ cudaError_t launch_repack_split16(const float* src, const float* gmm, void* dst,
   cudaError_t e = cudaMemsetAsync(dst, 0, SPLIT16_HEADER, st);
   if (e != cudaSuccess) return e;
   const size_t n4 = n / 4;
-  const int blocks = (int)std::min<size_t>(148 * 8, (n4 + 255) / 256 + 1);
+  int dev = 0;
+  if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
+  const int blocks = (int)std::min<size_t>((size_t)sm_count(dev) * 8, (n4 + 255) / 256 + 1);
   absmax_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const float4*>(src), n4, src + n4 * 4, (int)(n - n4 * 4),
                                         reinterpret_cast<unsigned*>(static_cast<unsigned char*>(dst) + offsetof(Split16Header, absmax)));
   dim3 block(256);
@@ -642,7 +642,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 EncodeTiledFn encode_tiled_fn();   // cost_tma.cu
 
 // rank-5 map over the fp16 planes: (64 channels, W, H, 2 planes, N); box = 8 pixels of one row (window segment) or an
-// 8x8 tile (reference), both planes; 128-byte swizzle = the canonical K-major UMMA layout
+// 8x8 tile (reference), both planes; 128-byte swizzle = the canonical K-major wgmma layout
 static cudaError_t make_planes_map(CUtensorMap* tm, const void* planes, int N, int H, int W, int box_rows) {
   EncodeTiledFn enc = encode_tiled_fn();
   if (!enc) return cudaErrorNotSupported;
@@ -674,17 +674,6 @@ static cudaError_t make_meta_map(CUtensorMap* tm, const void* meta, int N, int H
 static float* g_mma_dbg = nullptr;
 void mma_set_debug_buffer(float* p) { g_mma_dbg = p; }
 #endif
-
-static int sm_count(int dev) {
-  static int cached[64] = {0};
-  int& c = cached[dev & 63];
-  if (c == 0) {
-    int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
-    c = n;
-  }
-  return c;
-}
 
 template <int MODE, bool CW>
 static cudaError_t launch_mma_mw(const CostParams& p, cudaStream_t st) {

@@ -1,7 +1,7 @@
 // MAGNET_VARIANT_TMA — TMA-staged CUDA-core kernel (MAGNET_SRC_PIXC; AUTO uses it for the drop-in path with few
 // hypotheses or C in {16, 32} — cost_mma.cu is the production kernel for C == 64): tap-sharing fused warp + sample + consistency + view fusion
 // with the CTA's source window staged in shared memory by TMA (cp.async.bulk.tensor, mbarrier completion) and the
-// per-hypothesis state held in tensor memory.
+// per-hypothesis state held in a per-thread shared-memory scratch.
 //
 // Replaces homography.py:79-161 (and :10-75 with CW == false); absorbs the sampler of MAGNET.py:154-156.
 // Same identity as cost_cells.cu — sum_c ref_c (sum_t w_t src_tc) = sum_t w_t <ref, src_t>, each bilinear cell of a
@@ -15,12 +15,12 @@
 //     padding_mode='zeros' for free, no bounds checks), and the 272-byte pixel pitch makes the 16-byte tap reads of 8
 //     neighbouring pixels bank-conflict free.  The camera table of the batch element is staged by cp.async.bulk.
 //   * FOUR lanes per reference pixel: lane h holds 16 of the 64 reference channels (16 registers instead of 64) and a
-//     contiguous quarter of the hypotheses.  A tap is 4 LDS.128 + 8 FFMA2 per lane and a 2-step butterfly; the
+//     contiguous quarter of the hypotheses.  A tap is 4 LDS.128 + 16 FFMA per lane and a 2-step butterfly; the
 //     hypothesis phases need no cross-lane traffic.  CTA = 16x4 pixel tile = 256 threads, two CTAs per SM = 16 warps.
-//   * the lane's 16 depth hypotheses and 16 view accumulators live in TENSOR MEMORY (tcgen05.ld / tcgen05.st, one
-//     column per value, 64 columns per CTA): the column index may be a run-time value, so the per-hypothesis loops stay
-//     rolled (small code, no register arrays, no spills) — with the arrays in registers the fully unrolled phases
-//     needed > 255 registers.
+//   * the lane's 16 depth hypotheses and 16 view accumulators live in a per-thread SHARED-MEMORY scratch (32 KB per
+//     CTA, 16-byte groups interleaved across the threads: conflict-free): the index may be a run-time value, so the
+//     per-hypothesis loops stay rolled (small code, no register arrays, no spills) — with the arrays in registers the
+//     fully unrolled phases needed > 255 registers.
 //   * per view: A  every lane walks ITS hypotheses exactly (no sortedness assumption, identical for d_volume /
 //                  Gaussian / plane depths), flags the ones that enter a new bilinear cell; the 4 lanes of a pixel
 //                  splice their lists (shuffles) into <= NORG cell origins in shared memory + the CTA bounding box;
@@ -51,20 +51,20 @@ constexpr int KL = 6;                  // cells one lane may contribute per walk
 constexpr int TJL = 16;                // hypotheses per lane
 constexpr int TCH = 4 * TJL;           // hypotheses per CTA (chunk)
 constexpr int TMAXV = 16;              // views whose camera constants are staged in shared memory
-constexpr int TMEM_COLS = 64;          // 2 warp groups x (16 depths + 16 accumulators)
+constexpr int SCR_COLS = 32;           // scratch floats per thread: 16 depths + 16 accumulators
 
 // shared-memory map (bytes)
 constexpr int OFF_BAR = 0;                                   // mbarrier
-constexpr int OFF_TMEM = 8;                                  // TMEM base address written by tcgen05.alloc
 constexpr int OFF_BBOX = 16;                                 // int[2][4]  x_lo, x_hi, y_lo, y_hi of the cell origins
 constexpr int OFF_KS = 64;                                   // float[TCH] sampler offsets / plane depths of the chunk
 constexpr int OFF_CAM = OFF_KS + TCH * 4;                    // magnet_camera[TMAXV]
 constexpr int OFF_ORG = OFF_CAM + TMAXV * 64;                // float2[NORG][TPX]  cell origins
 constexpr int OFF_REC = OFF_ORG + NORG * TPX * 8;            // float4[3][NCP][TPX] records; every warp's own rows double
-constexpr int OFF_WIN = ((OFF_REC + 3 * NCP * TPX * 16 + 127) / 128) * 128;   //   as its float2 staging slots in phase A
+constexpr int OFF_SCR = ((OFF_REC + 3 * NCP * TPX * 16 + 127) / 128) * 128;   //   as its float2 staging slots in phase A
+constexpr int OFF_WIN = OFF_SCR + SCR_COLS * TNT * 4;        // float4[SCR_COLS / 4][TNT] per-thread scratch
 constexpr int TMA_SMEM_TOTAL = (228 * 1024 - 2 * 1024) / 2;  // two CTAs per SM (1 KB per CTA is reserved by the driver)
 static_assert(4 * KL <= 3 * NCP, "one staging slot per record row (see phase_a)");
-static_assert(OFF_CAM % 16 == 0 && OFF_ORG % 16 == 0 && OFF_REC % 16 == 0, "alignment");
+static_assert(OFF_CAM % 16 == 0 && OFF_ORG % 16 == 0 && OFF_REC % 16 == 0 && OFF_SCR % 16 == 0, "alignment");
 
 __host__ __device__ constexpr int pix_floats(int C) { return C + 4; }
 __host__ __device__ constexpr int tma_box_bytes(int C) { return 8 * pix_floats(C) * 4; }
@@ -75,7 +75,7 @@ struct ViewGeom {
 };
 
 __device__ __forceinline__ void project2(const float2 d, const ViewGeom& g, float2& ix, float2& iy, float2& z) {
-  project2(d, g.a0, g.a1, g.a2, g.q0, g.q1, g.q2, ix, iy, z);   // common.cuh: two hypotheses per packed instruction
+  project2(d, g.a0, g.a1, g.a2, g.q0, g.q1, g.q2, ix, iy, z);   // common.cuh: two hypotheses side by side
 }
 
 // predicated shared-memory loads (the destination keeps its value when the predicate is false): phase C reloads the
@@ -94,6 +94,10 @@ __device__ __forceinline__ float4 bilinear_poly4(float v00, float v01, float v10
   return make_float4(v00, v01 - v00, v10 - v00, (v00 - v01) - (v10 - v11));
 }
 
+// Per-thread scratch: column c (a multiple of 4; columns 8q .. 8q+3 = depths 4q .. 4q+3, 8q+4 .. 8q+7 = their
+// accumulators) is one float4 at scr[(c / 4) * TNT], scr = the thread's slot of the OFF_SCR array.
+__device__ __forceinline__ float4& scr_at(float4* scr, int c) { return scr[(c >> 2) * TNT]; }
+
 // Per-lane result of phase A (pixel-wide quantities are identical on the 4 lanes of a pixel).
 struct LaneCells {
   unsigned mask;   // bit m: my hypothesis m starts a cell that this walk keeps
@@ -104,13 +108,13 @@ struct LaneCells {
 };
 
 // ---------------------------------------------------------------------------------------------------------------
-// Phase A: hypotheses >= jlo of the pixel are pending.  TMEM columns tm + 8q .. 8q+3 hold my depths 4q .. 4q+3;
+// Phase A: hypotheses >= jlo of the pixel are pending.  Scratch columns 8q .. 8q+3 hold my depths 4q .. 4q+3;
 // depths beyond my last hypothesis replicate it (so they never start a cell and need no predicate).
 // Every lane projects each of its hypotheses and records the changes of cell: exact for any depth order and sign of z.
-// (The analytic grid-line walk of cost_cells.cu was tried here over each lane's quarter of the hypotheses: with 32
-// lanes walking in lockstep and a binary search per step it measured 6 % SLOWER than this loop — profiles/r2_*.md.)
+// (The analytic grid-line walk of cost_cells.cu over each lane's quarter of the hypotheses would walk 32 lanes in
+// lockstep with a binary search per step; this loop has no data-dependent trip count.)
 // ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ LaneCells phase_a(const ViewGeom& g, const uint32_t tm, const int mend, const int nj,
+__device__ __forceinline__ LaneCells phase_a(const ViewGeom& g, float4* __restrict__ scr, const int mend, const int nj,
                                              const int jb, const int jlo, const int Dc, const int W, const int H,
                                              const int lane, const int pxl, float2* __restrict__ stg,
                                              float2* __restrict__ org, int (&box)[4]) {
@@ -131,12 +135,11 @@ __device__ __forceinline__ LaneCells phase_a(const ViewGeom& g, const uint32_t t
   constexpr int SK = 2 * TPX;                             // float2 stride between consecutive staging slots
   {
 #pragma unroll 1
-    for (int m = 0; m < mend; m += 4) {                   // 4 hypotheses per trip: two independent packed projections
-      float d0, d1, d2, d3;
-      tmem_ld4(tm + 2 * m, d0, d1, d2, d3);
+    for (int m = 0; m < mend; m += 4) {                   // 4 hypotheses per trip: two independent float2 projections
+      const float4 d = scr_at(scr, 2 * m);
       float2 ixa, iya, za, ixb, iyb, zb;
-      project2(make_float2(d0, d1), g, ixa, iya, za);
-      project2(make_float2(d2, d3), g, ixb, iyb, zb);
+      project2(make_float2(d.x, d.y), g, ixa, iya, za);
+      project2(make_float2(d.z, d.w), g, ixb, iyb, zb);
       // anything left of -1 / right of W (above / below likewise) has all four taps out of the image: clamp so that
       // cell coordinates stay small and NaN (fmaxf drops it) maps to "out of bounds"
       float cx[4], cy[4];
@@ -266,8 +269,8 @@ __device__ __forceinline__ void phase_b(const float2 (&ref2)[C / 8], const int n
 #pragma unroll
     for (int q = 0; q < QL; ++q) {
       const float4 t = STAGED ? s[q] : __ldg(s + q);
-      s0 = __ffma2_rn(ref2[2 * q + 0], make_float2(t.x, t.y), s0);
-      s1 = __ffma2_rn(ref2[2 * q + 1], make_float2(t.z, t.w), s1);
+      s0 = ffma2_rn(ref2[2 * q + 0], make_float2(t.x, t.y), s0);
+      s1 = ffma2_rn(ref2[2 * q + 1], make_float2(t.z, t.w), s1);
     }
     TapV r;
     r.f = (s0.x + s0.y) + (s1.x + s1.y);
@@ -338,10 +341,10 @@ __device__ __forceinline__ void phase_b(const float2 (&ref2)[C / 8], const int n
 
 // ---------------------------------------------------------------------------------------------------------------
 // Phase C: every lane evaluates its pending hypotheses whose cell index lies in [i0, i0 + NCP) from the records and
-// adds them to its accumulators (TMEM columns tm + 8q + 4 .. 8q + 7).
+// adds them to its accumulators (scratch columns 8q + 4 .. 8q + 7).
 // ---------------------------------------------------------------------------------------------------------------
 template <bool CW>
-__device__ __forceinline__ void phase_c(const ViewGeom& g, const uint32_t tm, const int mend, const LaneCells& lc,
+__device__ __forceinline__ void phase_c(const ViewGeom& g, float4* __restrict__ scr, const int mend, const LaneCells& lc,
                                         const int jb, const int i0, const float kappa, const int pxl,
                                         const float2* __restrict__ org, const float4* __restrict__ rec) {
   const int mhi = min(max(lc.jstop - jb, 0), TJL);
@@ -353,8 +356,8 @@ __device__ __forceinline__ void phase_c(const ViewGeom& g, const uint32_t tm, co
   unsigned msk = lc.mask;
 #pragma unroll 1
   for (int m = 0; m < mend; m += 4) {                     // 4 hypotheses per trip (instruction-level parallelism)
-    float v[8];                                           // my depths m..m+3 and their accumulators
-    tmem_ld8(tm + 2 * m, v);
+    const float4 dv = scr_at(scr, 2 * m), av = scr_at(scr, 2 * m + 4);
+    float v[8] = {dv.x, dv.y, dv.z, dv.w, av.x, av.y, av.z, av.w};   // my depths m..m+3 and their accumulators
     float2 ix2[2], iy2[2], z2[2];
     project2(make_float2(v[0], v[1]), g, ix2[0], iy2[0], z2[0]);
     project2(make_float2(v[2], v[3]), g, ix2[1], iy2[1], z2[1]);
@@ -390,9 +393,8 @@ __device__ __forceinline__ void phase_c(const ViewGeom& g, const uint32_t tm, co
       }
       v[4 + e] += (ok && inr) ? cost : 0.0f;
     }
-    tmem_st4(tm + 2 * m + 4, v[4], v[5], v[6], v[7]);
+    scr_at(scr, 2 * m + 4) = make_float4(v[4], v[5], v[6], v[7]);
   }
-  tmem_wait_st();
 }
 
 template <int C, int MODE, bool CW>
@@ -430,7 +432,6 @@ cost_tma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
   const bool live = px < W && py < H;
   const int n = min(py, H - 1) * W + min(px, W - 1);       // dead lanes shadow the nearest pixel of the image, never store
 
-  if (warp == 0) tmem_alloc(smem_u32(smem + OFF_TMEM), TMEM_COLS);
   if (tid == 0) {
     mbar_init(bar, 1);
     fence_mbar_init();
@@ -439,16 +440,13 @@ cost_tma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
     prefetch_tmap(&tmap);
   }
   if (tid < TCH) ks[tid] = (MODE != MAGNET_DEPTH_VOLUME && jc + tid < D) ? p.k[jc + tid] : 0.0f;
-  tmem_fence_before_sync();
   __syncthreads();
-  tmem_fence_after_sync();
   if (tid == 0) {                                          // camera constants of this batch element: one bulk copy
     mbar_arrive_expect_tx(bar, (uint32_t)V * 64u);
     bulk_load(smem_u32(smem + OFF_CAM), p.cams + (size_t)b * V, (uint32_t)V * 64u, bar);
   }
-  // my TMEM window: lanes 32*(warp%4).., 32 columns per warp group; columns 8q+{0..3} depths, 8q+{4..7} accumulators
-  const uint32_t tmem_base = *reinterpret_cast<const volatile uint32_t*>(smem + OFF_TMEM);
-  const uint32_t tm = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)((warp >> 2) * 32);
+  // my scratch: columns 8q+{0..3} depths, 8q+{4..7} accumulators
+  float4* scr = reinterpret_cast<float4*>(smem + OFF_SCR) + tid;
 
   // ---- per-lane constants: 16 reference channels, the ray, my depth hypotheses -------------------------------
   float2 ref2[C / 8];
@@ -480,10 +478,9 @@ cost_tma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
         }
         d[e] = v;
       }
-      tmem_st4(tm + 2 * m, d[0], d[1], d[2], d[3]);
-      tmem_st4(tm + 2 * m + 4, 0.0f, 0.0f, 0.0f, 0.0f);
+      scr_at(scr, 2 * m) = make_float4(d[0], d[1], d[2], d[3]);
+      scr_at(scr, 2 * m + 4) = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
     }
-    tmem_wait_st();
   }
   mbar_wait(bar, 0);                                       // camera table landed
   uint32_t phase = 1;
@@ -502,7 +499,7 @@ cost_tma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
 
     // ---------------- phase A + bounding box of the CTA's cells ---------------------------------------------
     int box[4];
-    LaneCells lc = phase_a(g, tm, mend, nj, jb, 0, Dc, W, H, lane, pxl, stg, org, box);
+    LaneCells lc = phase_a(g, scr, mend, nj, jb, 0, Dc, W, H, lane, pxl, stg, org, box);
     int* bb = bbox + (it & 1) * 4;
     if (lane == 0) {
       atomicMin(bb + 0, box[0]); atomicMax(bb + 1, box[1]); atomicMin(bb + 2, box[2]); atomicMax(bb + 3, box[3]);
@@ -550,11 +547,11 @@ cost_tma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
           phase_b<C, CW, true>(ref2, lc.ncell, i0, i1, cs, lane, pxl, org, rec, smem, cbase, img, row_bytes, wx0, wy0, W, H);
         else
           phase_b<C, CW, false>(ref2, lc.ncell, i0, i1, cs, lane, pxl, org, rec, smem, 0, img, W * PS, 0, 0, W, H);
-        phase_c<CW>(g, tm, mend, lc, jb, i0, p.kappa, pxl, org, rec);
+        phase_c<CW>(g, scr, mend, lc, jb, i0, p.kappa, pxl, org, rec);
       }
       if (!__any_sync(FULL, lc.jstop < Dc)) break;
       jlo = lc.jstop;                                      // restart the walk behind the last covered hypothesis;
-      lc = phase_a(g, tm, mend, nj, jb, jlo, Dc, W, H, lane, pxl, stg, org, box);   // (the window only covers the
+      lc = phase_a(g, scr, mend, nj, jb, jlo, Dc, W, H, lane, pxl, stg, org, box);   // (the window only covers the
                                                                                       //  first walk's cells: global taps)
     }
   }
@@ -565,16 +562,13 @@ cost_tma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
     const bool exact = p.inv_v_exact != 0.0f;              // V a power of two: the division is an exact scaling
 #pragma unroll 1
     for (int m = 0; m < mend; m += 4) {
-      float a[4];
-      tmem_ld4(tm + 2 * m + 4, a[0], a[1], a[2], a[3]);
+      const float4 av = scr_at(scr, 2 * m + 4);
+      const float a[4] = {av.x, av.y, av.z, av.w};
 #pragma unroll
       for (int e = 0; e < 4; ++e)
         if (live && m + e < nj) outp[(size_t)(m + e) * HW] = exact ? a[e] * p.inv_v_exact : __fdiv_rn(a[e], p.vf);
     }
   }
-  tmem_fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 // (N, C, H, W) [+ (N, 2, H, W) Gaussians] -> MAGNET_SRC_PIXC (N, H, W, C+4).  One CTA per 32 pixels of one image:

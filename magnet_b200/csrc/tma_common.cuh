@@ -1,5 +1,5 @@
-// sm_100a primitives as inline PTX: mbarrier + TMA (cp.async.bulk[.tensor]) for cost_tma.cu / cost_mma.cu, tensor memory
-// and tcgen05.mma (UMMA) for cost_mma.cu.
+// sm_90a primitives as inline PTX: mbarrier + TMA (cp.async.bulk[.tensor]) for cost_tma.cu / cost_mma.cu, and
+// warpgroup MMA (wgmma.mma_async) for cost_mma.cu.
 #pragma once
 #include <cuda.h>   // CUtensorMap and its enums (types only — cuTensorMapEncodeTiled is resolved at run time)
 #include <stdint.h>
@@ -48,7 +48,7 @@ __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* tma
       ::"r"(dst), "l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4), "r"(bar) : "memory");
 }
 
-// order generic-proxy accesses of shared memory (ld/st.shared) before later async-proxy accesses (TMA writes, UMMA reads)
+// order generic-proxy accesses of shared memory (ld/st.shared) before later async-proxy accesses (TMA writes, wgmma reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // 1-D bulk copy global -> shared (UBLKCP); bytes % 16 == 0, both addresses 16-byte aligned
@@ -61,91 +61,31 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
 }
 
-// ---- tensor memory (TMEM) as per-thread scratch ---------------------------------------------------------------
-// 32x32b shape: thread i of warp w owns TMEM lane 32*(w%4)+i; a column holds one 32-bit word per lane.  The column
-// index may be a run-time (warp-uniform) value, which lets the per-hypothesis loops stay ROLLED while their
-// accumulators live outside the register file.  Loads are completed (wait::ld) inside the same asm statement, so the
-// results cannot be consumed early.
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld2(uint32_t taddr, float& a, float& b) {
-  uint32_t x, y;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0, %1}, [%2];\ntcgen05.wait::ld.sync.aligned;"
-               : "=r"(x), "=r"(y) : "r"(taddr) : "memory");
-  a = __uint_as_float(x);
-  b = __uint_as_float(y);
-}
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, float& a, float& b, float& c, float& d) {
-  uint32_t x, y, z, w;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];\ntcgen05.wait::ld.sync.aligned;"
-               : "=r"(x), "=r"(y), "=r"(z), "=r"(w) : "r"(taddr) : "memory");
-  a = __uint_as_float(x);
-  b = __uint_as_float(y);
-  c = __uint_as_float(z);
-  d = __uint_as_float(w);
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];\ntcgen05.wait::ld.sync.aligned;"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr) : "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-// 16 consecutive accumulator columns of my TMEM lane (epilogue of cost_mma.cu)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr) : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// ---- tcgen05.mma (UMMA), one CTA, fp16 operands from shared memory, fp32 accumulator in tensor memory ------------
+// ---- wgmma: one warpgroup (128 threads), fp16 operands from shared memory, fp32 accumulator in registers ----------
 // Shared-memory matrix descriptor of a K-major operand in the canonical 128-byte-swizzle layout (what TMA's
 // CU_TENSOR_MAP_SWIZZLE_128B writes): rows of 128 bytes (64 fp16 of K), 8-row atoms of 1024 bytes, `sbo` bytes between
-// consecutive atoms.  Bit fields as cute::UMMA::SmemDescriptor: start address >> 4 [0,14), leading byte offset >> 4
-// [16,30) (unused for swizzled K-major, set to 1), stride byte offset >> 4 [32,46), version 1 [46,48), layout type
-// SWIZZLE_128B = 2 [61,64).  A K step of 16 fp16 (32 bytes) inside the swizzle row is start address + 2.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr, uint32_t sbo) {
+// consecutive atoms.  Bit fields as cute::GMMA::GmmaDescriptor: start address >> 4 [0,14), leading byte offset >> 4
+// [16,30) (unused for swizzled K-major, set to 1), stride byte offset >> 4 [32,46), base offset [49,52) = 0 (atoms are
+// 1024-byte aligned), layout type SWIZZLE_128B = 1 [62,64).  A K step of 16 fp16 (32 bytes) inside the swizzle row is
+// start address + 2.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t sbo) {
   return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
+         ((uint64_t)1 << 62);
 }
-// Instruction descriptor, kind::f16 (cute::UMMA::InstrDescriptor): D fp32 [4,6) = 1, A / B fp16 [7,10) / [10,13) = 0,
-// both K-major [15] / [16] = 0, N >> 3 at [17,23), M >> 4 at [24,29).
-__device__ __forceinline__ uint32_t umma_idesc_f16(uint32_t M, uint32_t N) {
-  return (1u << 4) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, issued by ONE thread
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// orders this warpgroup's register / shared-memory accesses before the wgmma instructions that follow
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, both K-major in shared memory.  Accumulator fragment of thread t of the
+// warpgroup: d[4j + {0,1}] = D[16 (t/32) + (t%32)/4][8j + 2 (t%4) + {0,1}], d[4j + {2,3}] = the same columns 8 rows down.
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
+      : "memory");
 }
-// arrive on `bar` when all tcgen05.mma issued so far by this thread have completed (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_st2(uint32_t taddr, float a, float b) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x2.b32 [%0], {%1, %2};" ::"r"(taddr), "r"(__float_as_uint(a)),
-               "r"(__float_as_uint(b)) : "memory");
-}
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, float a, float b, float c, float d) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(__float_as_uint(a)),
-               "r"(__float_as_uint(b)), "r"(__float_as_uint(c)), "r"(__float_as_uint(d)) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 }  // namespace magnet

@@ -120,7 +120,7 @@ def _camera_table(cam_intrins, R, t, is_valid, device):
     return _cache.put("cams", src, ops.pack_cameras(intM_d, R, t, valid_d), extra)
 
 
-MMA_MIN_PLANES = 32   # below half a 64-hypothesis chunk the all-pairs GEMM is wasted: the gather kernel is faster (profiles/r2_ship_point.md)
+MMA_MIN_PLANES = 32   # below half a 64-hypothesis chunk the all-pairs GEMM is wasted: the gather kernel does only the needed taps
 
 
 def _wants_split16(C: int, V: int, variant: int, D: int) -> bool:

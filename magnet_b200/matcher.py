@@ -1,4 +1,4 @@
-"""B200-native matching loop: the iteration of models/MAGNET.py:150-169 with the sampler fused into
+"""H100-native matching loop: the iteration of models/MAGNET.py:150-169 with the sampler fused into
 the cost kernel and the Gaussian update as one kernel, prepared once per forward.
 
 The reference inlines the sampler (MAGNET.py:154-156) and the update (inside GNET.forward, :60-69),
@@ -74,8 +74,8 @@ class MatchingPlan:
         self._packed = {}
         self._ref_split = None
         # Production: the tensor-core kernel on the fp16 hi/lo planes (C == 64 and at least half a chunk of hypotheses,
-        # decided per cost() call); otherwise the global-gather kernel (TILED32), the faster CUDA-core one at every
-        # measured size (profiles/r2_kernels.md).  Pass src_layout=SRC_PIXC / variant=VARIANT_TMA for the TMA-staged
+        # decided per cost() call); otherwise the global-gather kernel (TILED32), which needs no staging window and
+        # no per-thread scratch.  Pass src_layout=SRC_PIXC / variant=VARIANT_TMA for the TMA-staged
         # CUDA-core kernel.  Layouts are packed on first use.
         if src_layout == _lib.SRC_SPLIT16 and not (self.C == 64 and self.V <= 16):
             src_layout = _lib.SRC_TILED32
@@ -182,7 +182,7 @@ class MagnetHead(nn.Module):
 
 
 class MAGNET(nn.Module):
-    """The reference's ``MAGNET`` (models/MAGNET.py:73-175) with the matching loop on the B200 kernels.
+    """The reference's ``MAGNET`` (models/MAGNET.py:73-175) with the matching loop on the H100 kernels.
 
     Same forward signature and return value: ``forward(ref_img, nghbr_imgs, nghbr_poses, is_valid, cam_intrins,
     mode)`` -> list of N_iter upsampled (B,2,H,W) Gaussians.  The backbones are passed in (the reference builds
@@ -224,7 +224,7 @@ class MAGNET(nn.Module):
 
 
 def install(homography_module=None) -> None:
-    """Rebind the reference's operators to the B200 kernels so that ``MAGNET.forward`` /
+    """Rebind the reference's operators to the H100 kernels so that ``MAGNET.forward`` /
     ``MAGNET_F.forward`` / ``test_MaGNet.py`` run unchanged:
 
         import models.submodules.homography as homography   # the reference's module

@@ -8,7 +8,7 @@ units) that bound bin ``j``.  Host-side, fp64, evaluated once.
 The normal quantile is evaluated with ``scipy.special.ndtri`` when scipy is
 importable (the reference uses ``scipy.stats.norm.ppf``, which is ndtri) and with
 a self-contained fp64 Newton refinement of ``erfinv`` otherwise, so the package
-has no hard scipy dependency on the GPU box.
+has no hard scipy dependency.
 """
 from __future__ import annotations
 

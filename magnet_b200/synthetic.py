@@ -9,7 +9,7 @@ source-camera coordinates (utils/utils.py:92), source tensors stacked view-major
 CPU tensors (test_MaGNet.py:36-50).
 
 Everything is generated with numpy (fp64 -> fp32) from an explicit seed so that the
-same arrays can be rebuilt on the GPU box without shipping fixtures.
+same arrays can be rebuilt on any machine without shipping fixtures.
 """
 from __future__ import annotations
 

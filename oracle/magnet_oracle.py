@@ -22,7 +22,7 @@ element by element in the reference's fp32 operation order (SURVEY Appendix A.2)
 
 PIN STATUS: the reference ships no tests, golden vectors or fixtures for this path
 (SURVEY §4, §8c).  The pin is therefore (i) outputs of the reference's own functions,
-imported from /root/reference in the build container and frozen under tests/golden/
+run on an unmodified checkout of the reference and frozen under tests/golden/
 by tests/golden/make_golden.py, and (ii) the analytic known-answer tests of SURVEY B.1.
 ``tests/test_oracle_golden.py`` checks this oracle against both.
 

@@ -5,14 +5,13 @@ Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py`` (``cpu_baseline`` 
 
 Why a second oracle next to ``magnet_oracle.py``: the reference is pure PyTorch, so its
 "CPU implementation" *is* a sequence of stock ATen kernels (matmul, repeat, grid_sample,
-mul, sum ...).  /root/reference cannot travel to the GPU box, so the two baselines that
-BASELINE.md asks for — reference-CPU on the box's host cores and reference-CUDA
-(``grid_sample``) on the B200 — are produced by this port, which issues the same ATen
-operator sequence with the same temporaries (including the D-fold ``repeat``
-materialisations that dominate the reference's cost, homography.py:92-93,105-110).
-``tests/test_oracle_golden.py`` checks, in the build container where /root/reference is
-importable, that this port is BIT-IDENTICAL to the reference functions on CPU; the frozen
-outputs in tests/golden/ carry that pin to the GPU box.
+mul, sum ...).  The reference is not part of this repository, so the two baselines that
+BASELINE.md asks for — reference-CPU on the host cores and reference-CUDA (``grid_sample``)
+on the GPU — are produced by this port, which issues the same ATen operator sequence with
+the same temporaries (including the D-fold ``repeat`` materialisations that dominate the
+reference's cost, homography.py:92-93,105-110).  ``tests/test_oracle_golden.py`` checks that
+this port is BIT-IDENTICAL on CPU to outputs of the reference functions frozen under
+tests/golden/ by tests/golden/make_golden.py.
 
 Restated from: models/submodules/homography.py:10-161 (cost volumes),
 models/MAGNET.py:15-27 (convex upsampling), :58-70 (Gaussian update), :154-156 (sampler).

@@ -1,4 +1,4 @@
-"""Build tuning variants of the library for one-call A/B runs on the GPU box.
+"""Build tuning variants of the library for A/B runs on the GPU.
 usage: python scripts/build_tuning.py "NCELL=4,JCHUNK=32,TILE_W=16:tag" ..."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

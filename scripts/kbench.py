@@ -1,4 +1,4 @@
-"""Kernel-only timing of the cost kernel for quick A/B runs on the GPU box.
+"""Kernel-only timing of the cost kernel for quick A/B runs on the GPU.
 usage: [MAGNET_B200_LIB=...] python scripts/kbench.py [cfg2|cfg3] [variant] [reps] [gauss|volume]   (volume = drop-in d_volume mode)"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,7 +1,5 @@
-"""Generate tests/golden/*.npz by running the UNMODIFIED reference (imported from /root/reference).
-
-Run in the build container only (the GPU box has no /root/reference):
-    python tests/golden/make_golden.py
+"""Generate tests/golden/*.npz by running the UNMODIFIED reference (a checkout of baegwangbin/MaGNet):
+    MAGNET_REFERENCE=<path of the checkout> python tests/golden/make_golden.py
 
 Inputs are not stored: they are rebuilt from the seed by magnet_b200.synthetic (numpy Generator
 streams are version-stable); each file carries a sha256 of the inputs so a drifting generator is
@@ -12,7 +10,6 @@ Reference entry points exercised:
   models/MAGNET.py                 GNET.forward update equations (:58-70), upsample_depth_via_mask (:15-27),
                                    MAGNET.depth_sampling (:120-128), the sampler expression (:154-156)
 """
-import hashlib
 import os
 import sys
 import types
@@ -22,8 +19,10 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = "/root/reference"
+REF = os.environ.get("MAGNET_REFERENCE", "")
 sys.path.insert(0, ROOT)
+
+from tests.util import input_digest  # noqa: E402
 
 CASES = {
     # name: (make_inputs kwargs)
@@ -36,14 +35,6 @@ CASES = {
 F_PLANES = 12
 
 
-def input_digest(inp) -> str:
-    h = hashlib.sha256()
-    for tsr in (inp.ref_feat, inp.nghbr_feat, inp.ref_gmms, inp.nghbr_gmms, inp.nghbr_poses, inp.is_valid,
-                inp.cam_intrins['intM'], inp.cam_intrins['unit_ray_array_2D'], inp.k):
-        h.update(np.ascontiguousarray(tsr.numpy()).tobytes())
-    return h.hexdigest()
-
-
 def f_planes(n=F_PLANES, d_min=0.5, d_max=8.0):
     """SID plane centres as train_FNet.py:56-66 builds them (n planes instead of 80)."""
     idx = np.arange(n + 1)
@@ -52,15 +43,45 @@ def f_planes(n=F_PLANES, d_min=0.5, d_max=8.0):
     return ((bounds[:-1] + bounds[1:]) / 2).astype(np.float32)
 
 
-def main():
-    if not os.path.isdir(REF):
-        raise SystemExit("/root/reference not present: golden vectors can only be generated in the build container")
+def _import_reference():
+    if not os.path.isdir(os.path.join(REF, "models")):
+        raise SystemExit("set MAGNET_REFERENCE to a checkout of the reference (baegwangbin/MaGNet)")
     sys.path.insert(0, REF)
     # utils/utils.py:5-7 imports matplotlib, which is absent; the hot path never touches it.
     for name in ("matplotlib", "matplotlib.pyplot"):
         m = types.ModuleType(name)
         m.use = lambda *a, **k: None
         sys.modules.setdefault(name, m)
+
+
+def live_reference_cases(refh):
+    """Outputs of the reference's est_costvolume_CW / est_costvolume_F (CPU) on the inputs of the bit-identity test of
+    oracle/torch_ref.py and of the drop-in F-volume test (tests/test_oracle_golden.py, tests/test_gpu_reference_module.py)."""
+    from magnet_b200.synthetic import make_inputs
+    threads = torch.get_num_threads()
+    torch.set_num_threads(1)          # the softmax of the F volume reduces in a thread-count dependent order
+    out = {}
+    for seed, depth in ((11, "random"), (12, "smooth")):
+        inp = make_inputs(B=2, V=2, D=6, H=20, W=28, C=8, seed=seed, depth=depth, invalid=[(0, 1)])
+        dv = inp.depth_volume()
+        out[f"cw_{seed}"] = refh.est_costvolume_CW(dv, inp.ref_feat, inp.nghbr_feat, inp.ref_gmms, inp.nghbr_gmms, inp.R,
+                                                   inp.t, inp.is_valid, inp.cam_intrins, 5).numpy()
+        dc = torch.linspace(0.5, 7, 9).view(1, 9, 1, 1)
+        out[f"f_{seed}"] = refh.est_costvolume_F(dc, inp.ref_feat, inp.nghbr_feat, inp.R, inp.t, inp.is_valid,
+                                                 inp.cam_intrins).numpy()
+        out[f"digest_{seed}"] = np.array(input_digest(inp))
+    inp = make_inputs(B=2, V=2, D=8, H=20, W=28, C=16, seed=98, depth="smooth")
+    d_center = torch.linspace(0.8, 6.0, 12).view(1, -1, 1, 1)
+    out["install_f"] = refh.est_costvolume_F(d_center, inp.ref_feat, inp.nghbr_feat, inp.R, inp.t, inp.is_valid,
+                                             inp.cam_intrins).numpy()
+    out["digest_98"] = np.array(input_digest(inp))
+    np.savez_compressed(os.path.join(HERE, "live_reference.npz"), **out)
+    torch.set_num_threads(threads)
+    print("live reference cases written:", sorted(out))
+
+
+def main():
+    _import_reference()
     import models.submodules.homography as refh
     from models.MAGNET import GNET, MAGNET, upsample_depth_via_mask
     from magnet_b200.synthetic import make_inputs
@@ -108,6 +129,7 @@ def main():
                         depth=depth.numpy(), mask=mask.numpy(), up=up.numpy(), **ks)
     print("update / upsample / k_list written")
     camera_prep_and_loss(g)
+    live_reference_cases(refh)
 
 
 def _camera_prep_case():

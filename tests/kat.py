@@ -1,6 +1,6 @@
 """Analytic known-answer cases for the CW / F cost volumes (SURVEY Appendix B.1).  Each builder returns
 (inputs, d_volume, expected, rel_tol); the same cases are run against the oracle on CPU and against the
-CUDA kernels on the GPU box."""
+CUDA kernels on the GPU."""
 import numpy as np
 import torch
 

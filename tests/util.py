@@ -1,5 +1,6 @@
 """Shared helpers for the parity tests (oracle = checker; nothing here is product code)."""
 import ast
+import hashlib
 import os
 
 import numpy as np
@@ -17,6 +18,15 @@ MARGIN_TOL = 1e-4
 FLIP_BUDGET = 5e-5
 
 
+def input_digest(inp) -> str:
+    """sha256 of the seeded inputs a golden case was generated from (tests/golden/make_golden.py)."""
+    h = hashlib.sha256()
+    for tsr in (inp.ref_feat, inp.nghbr_feat, inp.ref_gmms, inp.nghbr_gmms, inp.nghbr_poses, inp.is_valid,
+                inp.cam_intrins['intM'], inp.cam_intrins['unit_ray_array_2D'], inp.k):
+        h.update(np.ascontiguousarray(tsr.numpy()).tobytes())
+    return h.hexdigest()
+
+
 def load_golden(name):
     z = np.load(os.path.join(GOLDEN, name + ".npz"), allow_pickle=False)
     kw = ast.literal_eval(str(z["kwargs"])) if "kwargs" in z.files else None
@@ -25,9 +35,6 @@ def load_golden(name):
 
 def golden_inputs(name):
     """Rebuild the seeded inputs of a golden case and verify them against the stored digest."""
-    import sys
-    sys.path.insert(0, GOLDEN)
-    from make_golden import input_digest
     from magnet_b200.synthetic import make_inputs
     z, kw = load_golden(name)
     inp = make_inputs(**kw)
