@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define MAGNET_ABI_VERSION 3
+#define MAGNET_ABI_VERSION 4
 #define MAGNET_MAX_PLANES 256   /* max depth hypotheses / planes per call (D) */
 
 typedef enum magnet_status {
@@ -129,8 +129,12 @@ int magnet_cost_volume_f32(const magnet_cost_args* args, void* stream);
  * Backward of the plane-sweep volume (est_costvolume_F) w.r.t. both feature maps — what autograd derives for
  * homography.py:10-75 during F-Net training (train_FNet.py:95-114): through the softmax, the 1/V mean, the channel
  * dot product and grid_sample's bilinear gather (scatter-add into the source features).
- * Geometry fields of `fwd` as in the forward call (consistency must be 0, depth_mode MAGNET_DEPTH_PLANES,
- * src_layout MAGNET_SRC_NCHW, C in {8,16,32,64}); `fwd->out` is ignored.
+ * Geometry fields of `fwd` as in the forward call (consistency must be 0, depth_mode MAGNET_DEPTH_PLANES); `fwd->out` is
+ * ignored.  Two forms:
+ *   - src_layout MAGNET_SRC_NCHW, C in {8,16,32,64}: ref_feat / src_feat are the NCHW feature maps (CUDA-core kernel);
+ *   - src_layout MAGNET_SRC_SPLIT16, variant AUTO or MMA, C == 64, V <= 16: ref_feat / src_feat are the split buffers
+ *     the forward read (tensor-core kernel: both gradients as GEMMs on the fp16 hi/lo planes).
+ * grad_src is accumulated with atomics in either form, so results are not bit-deterministic from run to run.
  */
 typedef struct magnet_cost_f_bwd_args {
   const magnet_cost_args* fwd;
@@ -240,6 +244,25 @@ int magnet_upsample_nll_fwd_f32(const float* depth, const float* up_mask, const 
 int magnet_upsample_nll_bwd_f32(const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
                                 float scale, int32_t B, int32_t H, int32_t W, int32_t k, float* grad_depth,
                                 float* grad_mask, void* stream);
+
+/*
+ * F-Net training loss, fused — replaces train_FNet.py:96-108 on the 1/V-averaged scores of the plane-sweep volume
+ * (magnet_cost_volume_f32 with softmax == 0, depth_mode MAGNET_DEPTH_PLANES):
+ *   prob = softmax over the D planes, pred = sum_j prob_j * planes_host[j], l1 = |pred - gt| where mask != 0.
+ * scores (B,D,H,W); planes_host: HOST pointer, D floats; gt (B,1,H,W) quarter-resolution depth; mask (B,1,H,W) uint8.
+ * Neither the probability volume nor the prediction is materialised.
+ * forward: partial[magnet_fnet_l1_partials(B,H,W)] receives one partial sum of l1 per CTA (the caller adds them and
+ *   divides by the number of supervised pixels).
+ * backward: grad_scores (B,D,H,W) is WRITTEN with prob_j (d_j - pred) sign(pred - gt) mask scale, sign(0) = 0;
+ *   scale = upstream gradient / number of supervised pixels, multiplied by *grad_scale (a DEVICE scalar) when
+ *   grad_scale is not NULL, so that a captured CUDA graph can take the upstream gradient from memory.
+ */
+int magnet_fnet_l1_partials(int32_t B, int32_t H, int32_t W);
+int magnet_fnet_l1_fwd_f32(const float* scores, const float* planes_host, const float* gt, const uint8_t* mask, int32_t B,
+                           int32_t D, int32_t H, int32_t W, float* partial, void* stream);
+int magnet_fnet_l1_bwd_f32(const float* scores, const float* planes_host, const float* gt, const uint8_t* mask,
+                           float scale, const float* grad_scale, int32_t B, int32_t D, int32_t H, int32_t W,
+                           float* grad_scores, void* stream);
 
 #ifdef __cplusplus
 }

@@ -7,9 +7,9 @@ and their reference-facing wrappers.  The CUDA library is mandatory; there is no
 from . import _lib
 from .sampling import depth_sampling, k_offsets_f32
 from .homography import est_costvolume_CW, est_costvolume_F, clear_cache, prep_cache
-from .matcher import GNET, MAGNET, MagnetHead, MatchingPlan, matching_loop, install
+from .matcher import GNET, MAGNET, MagnetF, MagnetHead, MatchingPlan, matching_loop, install, sid_planes
 
 __all__ = [
     "depth_sampling", "k_offsets_f32", "est_costvolume_CW", "est_costvolume_F", "clear_cache", "prep_cache",
-    "GNET", "MAGNET", "MagnetHead", "MatchingPlan", "matching_loop", "install",
+    "GNET", "MAGNET", "MagnetF", "MagnetHead", "MatchingPlan", "matching_loop", "install", "sid_planes",
 ]

@@ -15,7 +15,7 @@ PKG = Path(__file__).resolve().parent
 # MAGNET_B200_LIB selects a tuning build (magnet_b200.build.build(defines=..., tag=...)); default = production
 LIB_PATH = Path(os.environ["MAGNET_B200_LIB"]) if os.environ.get("MAGNET_B200_LIB") else PKG / "libmagnet_b200.so"
 
-MAGNET_ABI_VERSION = 3
+MAGNET_ABI_VERSION = 4
 MAGNET_MAX_PLANES = 256
 
 OK, ERR_NULL, ERR_SHAPE, ERR_UNSUPPORTED, ERR_CUDA, ERR_ALIGN = 0, -1, -2, -3, -4, -5
@@ -31,6 +31,7 @@ EXPORTS = (
     "magnet_gaussian_update_bwd_f32", "magnet_convex_upsample_fwd_f32", "magnet_convex_upsample_bwd_f32",
     "magnet_relative_poses_f32", "magnet_camera_rays_f32",
     "magnet_upsample_nll_partials", "magnet_upsample_nll_fwd_f32", "magnet_upsample_nll_bwd_f32",
+    "magnet_fnet_l1_partials", "magnet_fnet_l1_fwd_f32", "magnet_fnet_l1_bwd_f32",
 )
 
 
@@ -121,6 +122,14 @@ def lib() -> C.CDLL:
     L.magnet_upsample_nll_bwd_f32.restype = C.c_int
     L.magnet_upsample_nll_bwd_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int32, C.c_int32,
                                               C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.magnet_fnet_l1_partials.restype = C.c_int
+    L.magnet_fnet_l1_partials.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+    L.magnet_fnet_l1_fwd_f32.restype = C.c_int
+    L.magnet_fnet_l1_fwd_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                         C.c_int32, C.c_void_p, C.c_void_p]
+    L.magnet_fnet_l1_bwd_f32.restype = C.c_int
+    L.magnet_fnet_l1_bwd_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int32,
+                                         C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     if L.magnet_abi_version() != MAGNET_ABI_VERSION:
         raise MagnetError(f"ABI version mismatch: library {L.magnet_abi_version()} != binding {MAGNET_ABI_VERSION}")
     _lib = L

@@ -44,6 +44,17 @@ cudaError_t launch_upsample_fwd(const float* depth, const float* mask, int B, in
 cudaError_t launch_upsample_bwd(const float* gout, const float* depth, const float* mask, int B, int CH, int H, int W,
                                 int k, float* gdepth, float* gmask, cudaStream_t st);
 cudaError_t launch_cost_f_bwd(const BwdParams& p, cudaStream_t st, int* launches);
+cudaError_t launch_cost_f_bwd_mma(const BwdParams& p, cudaStream_t st, int* launches);
+bool f_bwd_mma_supports(int C, int V);
+#ifdef MAGNET_MMA_DEBUG
+void f_bwd_mma_set_debug_buffer(float* p);
+#endif
+int fnet_l1_partials(int B, int HW);
+cudaError_t launch_fnet_l1_fwd(const float* scores, const float* planes, const float* gt, const uint8_t* mask, int B,
+                               int D, int HW, float* partial, cudaStream_t st);
+cudaError_t launch_fnet_l1_bwd(const float* scores, const float* planes, const float* gt, const uint8_t* mask,
+                               float scale, const float* grad_scale, int B, int D, int HW, float* grad_scores,
+                               cudaStream_t st);
 cudaError_t launch_upsample_nll_fwd(const float* depth, const float* mask, const float* gt, const uint8_t* gtm, int B,
                                     int H, int W, int k, float* partial, cudaStream_t st);
 cudaError_t launch_upsample_nll_bwd(const float* depth, const float* mask, const float* gt, const uint8_t* gtm, float scale,
@@ -201,9 +212,17 @@ int magnet_cost_volume_f_bwd_f32(const magnet_cost_f_bwd_args* b, void* stream) 
   if (!a->ref_feat || !a->src_feat || !a->rays || !a->cams || !a->k_host) return MAGNET_ERR_NULL;
   if (!b->grad_out || !b->workspace || !b->grad_ref || !b->grad_src) return MAGNET_ERR_NULL;
   if (a->softmax && !b->prob) return MAGNET_ERR_NULL;
-  if (a->consistency || a->depth_mode != MAGNET_DEPTH_PLANES || a->src_layout != MAGNET_SRC_NCHW)
-    return MAGNET_ERR_UNSUPPORTED;
-  if (a->C != 8 && a->C != 16 && a->C != 32 && a->C != 64) return MAGNET_ERR_UNSUPPORTED;
+  if (a->consistency || a->depth_mode != MAGNET_DEPTH_PLANES) return MAGNET_ERR_UNSUPPORTED;
+  const bool mma = a->src_layout == MAGNET_SRC_SPLIT16;
+  if (mma) {                                   // tensor-core backward on the forward's split buffers
+    if (a->variant != MAGNET_VARIANT_AUTO && a->variant != MAGNET_VARIANT_MMA) return MAGNET_ERR_UNSUPPORTED;
+    if (!magnet::f_bwd_mma_supports(a->C, a->V)) return MAGNET_ERR_UNSUPPORTED;
+    if (reinterpret_cast<uintptr_t>(a->src_feat) % 16 != 0 || reinterpret_cast<uintptr_t>(a->ref_feat) % 16 != 0)
+      return MAGNET_ERR_ALIGN;
+  } else {
+    if (a->src_layout != MAGNET_SRC_NCHW) return MAGNET_ERR_UNSUPPORTED;
+    if (a->C != 8 && a->C != 16 && a->C != 32 && a->C != 64) return MAGNET_ERR_UNSUPPORTED;
+  }
   magnet::BwdParams p;
   p.B = a->B; p.V = a->V; p.D = a->D; p.C = a->C; p.H = a->H; p.W = a->W; p.HW = a->H * a->W;
   p.softmax = a->softmax != 0;
@@ -212,7 +231,8 @@ int magnet_cost_volume_f_bwd_f32(const magnet_cost_f_bwd_args* b, void* stream) 
   p.prob = b->prob; p.grad_out = b->grad_out; p.g_score = b->workspace; p.grad_ref = b->grad_ref; p.grad_src = b->grad_src;
   for (int j = 0; j < MAGNET_MAX_PLANES; ++j) p.k[j] = j < a->D ? a->k_host[j] : 0.0f;
   int launches = 0;
-  cudaError_t e = magnet::launch_cost_f_bwd(p, (cudaStream_t)stream, &launches);
+  cudaError_t e = mma ? magnet::launch_cost_f_bwd_mma(p, (cudaStream_t)stream, &launches)
+                      : magnet::launch_cost_f_bwd(p, (cudaStream_t)stream, &launches);
   if (e != cudaSuccess) return cuda_fail(e);
   g_launches += launches;
   return MAGNET_OK;
@@ -275,6 +295,7 @@ int magnet_repack_split16_f32(const float* src_nchw, const float* src_gmm, void*
 
 #ifdef MAGNET_MMA_DEBUG
 void magnet_mma_debug_buffer(float* p) { magnet::mma_set_debug_buffer(p); }
+void magnet_f_bwd_mma_debug_buffer(float* p) { magnet::f_bwd_mma_set_debug_buffer(p); }
 #endif
 
 int magnet_sample_depths_f32(const float* gmm, const float* k_host, int32_t B, int32_t D, int32_t HW,
@@ -374,6 +395,46 @@ int magnet_upsample_nll_bwd_f32(const float* depth, const float* up_mask, const 
   if (B <= 0 || H <= 0 || W <= 0 || k <= 0 || B > 65535 || H * k > 65535) return MAGNET_ERR_SHAPE;
   cudaError_t e = magnet::launch_upsample_nll_bwd(depth, up_mask, gt, gt_mask, scale, B, H, W, k, grad_depth, grad_mask,
                                                   (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 1;
+  return MAGNET_OK;
+}
+
+int magnet_fnet_l1_partials(int32_t B, int32_t H, int32_t W) {
+  if (B <= 0 || H <= 0 || W <= 0) return MAGNET_ERR_SHAPE;
+  return magnet::fnet_l1_partials(B, H * W);
+}
+
+namespace {
+int validate_fnet_l1(const float* scores, const float* planes_host, const float* gt, const uint8_t* mask, int32_t B,
+                     int32_t D, int32_t H, int32_t W) {
+  if (!scores || !planes_host || !gt || !mask) return MAGNET_ERR_NULL;
+  if (B <= 0 || D <= 0 || H <= 0 || W <= 0 || B > 65535) return MAGNET_ERR_SHAPE;
+  if ((int64_t)H * W > (1 << 26)) return MAGNET_ERR_SHAPE;
+  if (D > MAGNET_MAX_PLANES) return MAGNET_ERR_UNSUPPORTED;
+  return MAGNET_OK;
+}
+}  // namespace
+
+int magnet_fnet_l1_fwd_f32(const float* scores, const float* planes_host, const float* gt, const uint8_t* mask, int32_t B,
+                           int32_t D, int32_t H, int32_t W, float* partial, void* stream) {
+  const int st = validate_fnet_l1(scores, planes_host, gt, mask, B, D, H, W);
+  if (st != MAGNET_OK) return st;
+  if (!partial) return MAGNET_ERR_NULL;
+  cudaError_t e = magnet::launch_fnet_l1_fwd(scores, planes_host, gt, mask, B, D, H * W, partial, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 1;
+  return MAGNET_OK;
+}
+
+int magnet_fnet_l1_bwd_f32(const float* scores, const float* planes_host, const float* gt, const uint8_t* mask,
+                           float scale, const float* grad_scale, int32_t B, int32_t D, int32_t H, int32_t W,
+                           float* grad_scores, void* stream) {
+  const int st = validate_fnet_l1(scores, planes_host, gt, mask, B, D, H, W);
+  if (st != MAGNET_OK) return st;
+  if (!grad_scores) return MAGNET_ERR_NULL;
+  cudaError_t e = magnet::launch_fnet_l1_bwd(scores, planes_host, gt, mask, scale, grad_scale, B, D, H * W, grad_scores,
+                                             (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e);
   g_launches += 1;
   return MAGNET_OK;

@@ -107,9 +107,14 @@ cost_f_bwd_kernel(const __grid_constant__ BwdParams p) {
   for (int c = 0; c < C; ++c) p.grad_ref[((size_t)b * C + c) * HW + n] = gref[c];
 }
 
-cudaError_t launch_cost_f_bwd(const BwdParams& p, cudaStream_t st, int* launches) {
+// g_score into the workspace (also the first launch of the tensor-core backward, cost_f_bwd_mma.cu)
+cudaError_t launch_score_grad(const BwdParams& p, cudaStream_t st) {
   score_grad_kernel<<<dim3((p.HW + 127) / 128, p.B), 128, 0, st>>>(p);
-  cudaError_t e = cudaGetLastError();
+  return cudaGetLastError();
+}
+
+cudaError_t launch_cost_f_bwd(const BwdParams& p, cudaStream_t st, int* launches) {
+  cudaError_t e = launch_score_grad(p, st);
   if (e != cudaSuccess) return e;
   dim3 grid((p.HW + 127) / 128, p.B);
   switch (p.C) {

@@ -75,31 +75,10 @@ constexpr int M_SMEM_TOTAL = M_SMEM_USED + 1024;            // slack for the 102
 static_assert(MR_BYTES >= MSEG * SEG_BYTES && MR_BYTES >= MPX * 264 * 4 && MR_BYTES >= MCH * 65 * 4, "region R");
 static_assert(2 * (M_SMEM_TOTAL + 1024) <= 227 * 1024, "two CTAs per SM");
 
-// header of a MAGNET_SRC_SPLIT16 buffer (256 bytes)
-struct Split16Header {
-  float scale;       // s = 2^k
-  float inv_scale;   // 2^-k
-  unsigned absmax;   // bits of max |x|
-};
-constexpr size_t SPLIT16_HEADER = 256;
-
 // header | fp16 planes (N, 2, H, W, 64) | table (N, H, W + 1, 4): entry x + 1 of a row = (mu, sigma)[x], (mu, sigma)[x + 1]
 // with zeros outside the row — both horizontal taps of a bilinear cell in ONE 16-byte read
 __host__ __device__ inline size_t split16_bytes(size_t N, size_t H, size_t W) {
   return SPLIT16_HEADER + N * H * W * 256 + N * H * (W + 1) * 16;
-}
-
-__device__ __forceinline__ void mbar_wait_or_trap(uint32_t bar, uint32_t parity) {
-  // bounded spin: a protocol error must surface as a launch failure, not as a hung GPU
-#pragma unroll 1
-  for (int it = 0; it < (1 << 22); ++it) {
-    uint32_t done;
-    // the suspend-time hint lets the hardware park the warp instead of spinning on issue slots the other CTA needs
-    asm volatile("{\n.reg .pred P1;\nmbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2, %3;\nselp.u32 %0, 1, 0, P1;\n}"
-                 : "=r"(done) : "r"(bar), "r"(parity), "r"(20000u) : "memory");
-    if (done) return;
-  }
-  __trap();
 }
 
 // work counters of the persistent kernel: one slot per launch in flight (host ticket), re-armed by the last CTA of the
@@ -597,7 +576,7 @@ __global__ void __launch_bounds__(256) split16_repack_kernel(const float* __rest
   }
 }
 
-static int sm_count(int dev) {
+int sm_count(int dev) {
   static int cached[64] = {0};
   int& c = cached[dev & 63];
   if (c == 0) {
@@ -642,8 +621,9 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 EncodeTiledFn encode_tiled_fn();   // cost_tma.cu
 
 // rank-5 map over the fp16 planes: (64 channels, W, H, 2 planes, N); box = 8 pixels of one row (window segment) or an
-// 8x8 tile (reference), both planes; 128-byte swizzle = the canonical K-major wgmma layout
-static cudaError_t make_planes_map(CUtensorMap* tm, const void* planes, int N, int H, int W, int box_rows) {
+// 8x8 tile (reference), both planes; 128-byte swizzle = the canonical K-major wgmma layout (cost_f_bwd_mma.cu reads
+// the same boxes as MN-major operands)
+cudaError_t make_planes_map(CUtensorMap* tm, const void* planes, int N, int H, int W, int box_rows) {
   EncodeTiledFn enc = encode_tiled_fn();
   if (!enc) return cudaErrorNotSupported;
   const cuuint64_t dims[5] = {64, (cuuint64_t)W, (cuuint64_t)H, 2, (cuuint64_t)N};

@@ -31,6 +31,27 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "}" ::"r"(bar), "r"(parity) : "memory");
 }
 
+__device__ __forceinline__ void mbar_wait_or_trap(uint32_t bar, uint32_t parity) {
+  // bounded spin: a protocol error must surface as a launch failure, not as a hung GPU
+#pragma unroll 1
+  for (int it = 0; it < (1 << 22); ++it) {
+    uint32_t done;
+    // the suspend-time hint lets the hardware park the warp instead of spinning on issue slots the other CTA needs
+    asm volatile("{\n.reg .pred P1;\nmbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2, %3;\nselp.u32 %0, 1, 0, P1;\n}"
+                 : "=r"(done) : "r"(bar), "r"(parity), "r"(20000u) : "memory");
+    if (done) return;
+  }
+  __trap();
+}
+
+// header of a MAGNET_SRC_SPLIT16 buffer (256 bytes)
+struct Split16Header {
+  float scale;       // s = 2^k
+  float inv_scale;   // 2^-k
+  unsigned absmax;   // bits of max |x|
+};
+constexpr size_t SPLIT16_HEADER = 256;
+
 // TMA tiled load of one box of a rank-4 tensor map into shared memory (UTMALDG); out-of-range elements are
 // zero-filled by the copy engine, coordinates are signed.
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tmap, uint32_t bar, int c0, int c1, int c2,
@@ -85,6 +106,19 @@ __device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t ad
       "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(adesc), "l"(bdesc), "r"(accumulate)
+      : "memory");
+}
+
+// D[64 x 64] += A[64 x 16] * B[16 x 64] with either operand K-major (TA / TB = 0) or MN-major (= 1, the transposed
+// form: rows of the 128-byte-swizzle atom are K indices holding 64 contiguous M / N elements; the descriptor's stride
+// byte offset is then the distance between consecutive 8-row K groups).  Accumulator fragment as m64n128k16, j < 8.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_f16(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %34, %35;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB)
       : "memory");
 }
 

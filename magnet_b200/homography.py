@@ -218,6 +218,44 @@ class _CostVolumeF(torch.autograd.Function):
         return g_ref, g_src, None, None, None, None, None
 
 
+class _PlaneSweepF(torch.autograd.Function):
+    """Plane-sweep volume of ``MagnetF`` — the 1/V-averaged scores (``softmax=False``, what the fused F-Net loss reads)
+    or the probabilities — differentiable in both feature maps.  The backward runs on the tensor cores whenever the
+    forward read SPLIT16 buffers (C == 64, V <= 16, at least MMA_MIN_PLANES planes), on the same buffers; otherwise
+    the CUDA-core kernel reads the NCHW maps."""
+
+    @staticmethod
+    def forward(ctx, ref_feat, nghbr_feat, planes, rays_d, cams, V, softmax):
+        src, layout, ref_split = _packed_source(nghbr_feat, None, V, _lib.VARIANT_AUTO, ref_feat, len(planes))
+        out = ops.cost_volume(ref_feat.detach(), src, rays_d, cams, V=V, src_layout=layout, consistency=False,
+                              k=planes, planes=True, softmax=softmax, ref_split=ref_split)
+        ctx.save_for_backward(ref_feat.detach(), nghbr_feat.detach(), out if softmax else None, rays_d, cams)
+        ctx.splits = (ref_split, src) if layout == _lib.SRC_SPLIT16 else (None, None)
+        ctx.planes, ctx.V, ctx.softmax = planes, V, softmax
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        ref_feat, nghbr_feat, out, rays_d, cams = ctx.saved_tensors
+        ref_split, src_split = ctx.splits
+        g_ref, g_src = ops.cost_volume_f_bwd(ref_feat, nghbr_feat, rays_d, cams, ctx.planes, ctx.V, out,
+                                             grad_out.contiguous(), softmax=ctx.softmax, ref_split=ref_split,
+                                             src_split=src_split)
+        return g_ref, g_src, None, None, None, None, None
+
+
+def plane_sweep_f(d_center, ref_feat, nghbr_feat, R, t, is_valid, cam_intrins, softmax=True):
+    """The F volume of est_costvolume_F (softmax=True) or its 1/V-averaged scores (softmax=False), with the
+    tensor-core backward where the forward ran on the tensor cores (MagnetF's path; est_costvolume_F keeps the
+    CUDA-core backward)."""
+    device = ref_feat.device
+    V = int(nghbr_feat.shape[0] / ref_feat.shape[0])
+    planes = _plane_list(d_center)
+    _, rays_d = _device_intrinsics(cam_intrins, device)
+    cams = _camera_table(cam_intrins, R, t, is_valid, device)
+    return _PlaneSweepF.apply(ref_feat, nghbr_feat, planes, rays_d, cams, V, softmax)
+
+
 def est_costvolume_F(d_center, ref_feat, nghbr_feat, R, t, is_valid, cam_intrins, variant=_lib.VARIANT_AUTO):
     """Fronto-parallel plane-sweep volume with softmax over planes — drop-in (forward) for
     homography.est_costvolume_F.  d_center (1,D,1,1); the rest as in est_costvolume_CW."""

@@ -223,6 +223,52 @@ class MAGNET(nn.Module):
                          is_valid, cam_intrins)
 
 
+def sid_planes(min_depth: float, max_depth: float, n: int = 80, device=None) -> torch.Tensor:
+    """The F-Net plane depths of train_FNet.py:56-66: centres of n spacing-increasing-discretisation (SID) bins on
+    [min_depth, max_depth], evaluated in float64 and rounded to float32, shape (1, n, 1, 1)."""
+    import numpy as np
+    idx = np.arange(n + 1)
+    gamma = 1 - min_depth
+    bounds = np.exp(np.log(max_depth + gamma) * idx / n) - gamma
+    centre = (bounds[:-1] + bounds[1:]) / 2
+    return torch.from_numpy(centre.astype(np.float32)).view(1, n, 1, 1).to(device)
+
+
+class MagnetF(nn.Module):
+    """The reference's ``MAGNET_F`` (models/MAGNET.py:179-202) — F-Net + plane-sweep volume — with the volume, its
+    backward and the training loss on the H100 kernels.  The attribute is ``f_net``, so a reference F-Net state dict
+    loads; ``f_net(imgs) -> (N, C, h, w)`` as F_psmnet.py:122-124 (cuDNN, trained)."""
+
+    def __init__(self, f_net: nn.Module):
+        super().__init__()
+        self.f_net = f_net
+
+    def _features(self, ref_img, nghbr_imgs):
+        B = ref_img.shape[0]
+        feat = self.f_net(torch.cat((ref_img, nghbr_imgs), dim=0))
+        return feat[:B], feat[B:]
+
+    def forward(self, ref_img, nghbr_imgs, nghbr_poses, is_valid, cam_intrins, d_center):
+        """(B, D, h, w) probability volume over the planes ``d_center`` (1, D, 1, 1), the reference's contract."""
+        from .homography import plane_sweep_f
+        ref_feat, nghbr_feat = self._features(ref_img, nghbr_imgs)
+        return plane_sweep_f(d_center, ref_feat, nghbr_feat, nghbr_poses[:, :, :3, :3], nghbr_poses[:, :, :3, 3],
+                             is_valid, cam_intrins, softmax=True)
+
+    def loss(self, ref_img, nghbr_imgs, nghbr_poses, is_valid, cam_intrins, d_center, gt_dmap, min_depth: float,
+             max_depth: float):
+        """The L1 loss of train_FNet.py:87-108: gt above max_depth is zeroed, gt is nearest-resized to the volume's
+        grid and supervises where it exceeds min_depth; the soft-argmin depth comes from the fused loss kernel on the
+        plane-sweep scores (no probability volume, no prediction map), and both backwards run in CUDA kernels."""
+        from .homography import _plane_list, plane_sweep_f
+        ref_feat, nghbr_feat = self._features(ref_img, nghbr_imgs)
+        scores = plane_sweep_f(d_center, ref_feat, nghbr_feat, nghbr_poses[:, :, :3, :3], nghbr_poses[:, :, :3, 3],
+                               is_valid, cam_intrins, softmax=False)
+        gt = torch.where(gt_dmap > max_depth, torch.zeros_like(gt_dmap), gt_dmap)
+        gt = nn.functional.interpolate(gt, size=[scores.shape[2], scores.shape[3]], mode='nearest')
+        return ops.fnet_l1_loss(scores, _plane_list(d_center), gt.contiguous(), gt > min_depth)
+
+
 def install(homography_module=None) -> None:
     """Rebind the reference's operators to the H100 kernels so that ``MAGNET.forward`` /
     ``MAGNET_F.forward`` / ``test_MaGNet.py`` run unchanged:

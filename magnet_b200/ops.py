@@ -233,36 +233,52 @@ def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tens
     return out
 
 
-def cost_volume_f_bwd(ref_feat, src_feat_nchw, rays, cams, planes, V, prob, grad_out, softmax=True):
+def cost_volume_f_bwd(ref_feat, src_feat_nchw, rays, cams, planes, V, prob, grad_out, softmax=True,
+                      ref_split=None, src_split=None):
     """Gradients of the plane-sweep volume w.r.t. (ref_feat, src_feat) — one magnet_cost_volume_f_bwd_f32 call.
-    src_feat_nchw (V*B,C,H,W) view-major; prob = forward output; returns (grad_ref, grad_src) in NCHW."""
+    src_feat_nchw (V*B,C,H,W) view-major; prob = forward output (read only when ``softmax``); grad_out = gradient w.r.t.
+    the forward output (the probabilities, or the 1/V-averaged scores with ``softmax=False``).  Returns (grad_ref,
+    grad_src) in NCHW.  With ``ref_split`` / ``src_split`` — the repack_split16 buffers the forward read (C == 64,
+    V <= 16) — the tensor-core kernel computes both gradients and the NCHW maps only supply the shapes; without them
+    the CUDA-core kernel reads the NCHW maps (C in {8, 16, 32, 64})."""
     ref_feat = _need_cuda_f32("ref_feat", ref_feat)
     src = _need_cuda_f32("src_feat", src_feat_nchw)
     rays = _need_cuda_f32("rays", rays)
     cams = _need_cuda_f32("cams", cams)
-    prob = _need_cuda_f32("prob", prob)
     grad_out = _need_cuda_f32("grad_out", grad_out)
     B, Cc, H, W = ref_feat.shape
     karr = planes if isinstance(planes, C.Array) else k_array(planes)
     _expect("src_feat", src, (V * B, Cc, H, W))
     _expect("rays", rays, (B, 3, H * W))
-    _expect("prob", prob, (B, len(karr), H, W))
     _expect("grad_out", grad_out, (B, len(karr), H, W))
+    if softmax:
+        prob = _need_cuda_f32("prob", prob)
+        _expect("prob", prob, (B, len(karr), H, W))
     if cams.numel() != B * V * 16:
         raise _lib.MagnetError(f"cams must hold B*V = {B * V} camera records of 16 floats, got {tuple(cams.shape)}")
-    dev = _same_device(("ref_feat", ref_feat), ("src_feat", src), ("rays", rays), ("cams", cams), ("prob", prob),
-                       ("grad_out", grad_out))
+    split = ref_split is not None or src_split is not None
+    if split:
+        for nm, buf, n in (("src_split", src_split, V * B), ("ref_split", ref_split, B)):
+            if not (isinstance(buf, torch.Tensor) and buf.is_cuda and buf.dtype == torch.uint8 and buf.is_contiguous()):
+                raise _lib.MagnetError(f"{nm} must be a contiguous uint8 CUDA buffer from repack_split16")
+            _expect(nm, buf, (int(lib().magnet_split16_bytes(n, H, W)),))
+    dev = _same_device(("ref_feat", ref_feat), ("src_feat", src), ("rays", rays), ("cams", cams),
+                       ("prob", prob if softmax else None), ("grad_out", grad_out), ("ref_split", ref_split),
+                       ("src_split", src_split))
     a = CostArgs()
     a.B, a.V, a.D, a.C, a.H, a.W = B, V, len(karr), Cc, H, W
-    a.depth_mode, a.src_layout, a.consistency, a.softmax = _lib.DEPTH_PLANES, _lib.SRC_NCHW, 0, 1 if softmax else 0
-    a.ref_feat, a.src_feat, a.rays, a.cams = ref_feat.data_ptr(), src.data_ptr(), rays.data_ptr(), cams.data_ptr()
+    a.depth_mode, a.consistency, a.softmax = _lib.DEPTH_PLANES, 0, 1 if softmax else 0
+    a.src_layout = _lib.SRC_SPLIT16 if split else _lib.SRC_NCHW
+    a.ref_feat, a.src_feat = (ref_split.data_ptr(), src_split.data_ptr()) if split else (ref_feat.data_ptr(), src.data_ptr())
+    a.rays, a.cams = rays.data_ptr(), cams.data_ptr()
     a.k_host = C.cast(karr, C.c_void_p)
-    work = torch.empty_like(prob)
+    work = torch.empty_like(grad_out)
     g_ref = torch.empty_like(ref_feat)
     g_src = torch.zeros_like(src)
     bw = _lib.CostFBwdArgs()
     bw.fwd = C.pointer(a)
-    bw.prob, bw.grad_out, bw.workspace = prob.data_ptr(), grad_out.data_ptr(), work.data_ptr()
+    bw.prob = prob.data_ptr() if softmax else None
+    bw.grad_out, bw.workspace = grad_out.data_ptr(), work.data_ptr()
     bw.grad_ref, bw.grad_src = g_ref.data_ptr(), g_src.data_ptr()
     with torch.cuda.device(dev):
         check(lib().magnet_cost_volume_f_bwd_f32(C.byref(bw), _stream(dev)), "magnet_cost_volume_f_bwd_f32")
@@ -408,6 +424,65 @@ def magnet_loss(pred_list, up_mask, gt, gt_mask, k: int, gamma: float = 0.8):
     for i, pred in enumerate(pred_list):
         loss = loss + gamma ** (n - i - 1) * UpsampleNLL.apply(pred, up_mask, gt, gtm, k, count)
     return loss
+
+
+class FnetL1Loss(torch.autograd.Function):
+    """train_FNet.py:96-108 — soft-argmin over the planes of the 1/V-averaged scores, then the mean over the supervised
+    pixels of |pred - gt| — one kernel each way; the probability volume and the prediction never reach memory.
+    Differentiable in the scores.  ``count`` is the number of supervised pixels (int, or a 0-dim device tensor)."""
+
+    @staticmethod
+    def forward(ctx, scores, planes, gt, mask_u8, count):
+        scores = _need_cuda_f32("scores", scores)
+        gt = _need_cuda_f32("gt", gt)
+        if scores.dim() != 4:
+            raise _lib.MagnetError(f"scores must be (B,D,H,W), got {tuple(scores.shape)}")
+        B, D, H, W = scores.shape
+        karr = planes if isinstance(planes, C.Array) else k_array(planes)
+        if len(karr) != D:
+            raise _lib.MagnetError(f"{len(karr)} plane depths for {D} score planes")
+        _expect("gt", gt, (B, 1, H, W))
+        if mask_u8.dtype != torch.uint8 or not mask_u8.is_cuda or tuple(mask_u8.shape) != (B, 1, H, W):
+            raise _lib.MagnetError("mask must be a CUDA uint8 tensor of shape (B,1,H,W)")
+        mask_u8 = mask_u8.contiguous()
+        dev = _same_device(("scores", scores), ("gt", gt), ("mask", mask_u8))
+        partial = torch.empty(lib().magnet_fnet_l1_partials(B, H, W), device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            check(lib().magnet_fnet_l1_fwd_f32(scores.data_ptr(), C.cast(karr, C.c_void_p), gt.data_ptr(),
+                                               mask_u8.data_ptr(), B, D, H, W, partial.data_ptr(), _stream(dev)),
+                  "magnet_fnet_l1_fwd_f32")
+        ctx.save_for_backward(scores, gt, mask_u8)
+        ctx.karr, ctx.count = karr, count
+        return partial.sum(dtype=torch.float64).to(torch.float32) / count
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        scores, gt, mask_u8 = ctx.saved_tensors
+        B, D, H, W = scores.shape
+        g = torch.empty_like(scores)
+        # the upstream gradient stays on the device (no host read: the step can be captured in a CUDA graph)
+        if isinstance(ctx.count, torch.Tensor):
+            gs, scale = (grad_out / ctx.count).to(torch.float32).contiguous(), 1.0
+        else:
+            gs, scale = grad_out.to(torch.float32).contiguous(), 1.0 / float(ctx.count)
+        with torch.cuda.device(scores.device):
+            check(lib().magnet_fnet_l1_bwd_f32(scores.data_ptr(), C.cast(ctx.karr, C.c_void_p), gt.data_ptr(),
+                                               mask_u8.data_ptr(), scale, gs.data_ptr(), B, D, H, W, g.data_ptr(),
+                                               _stream(scores.device)), "magnet_fnet_l1_bwd_f32")
+        return g, None, None, None, None
+
+
+def fnet_l1_loss(scores, planes, gt_q, mask_q, count=None):
+    """F-Net's L1 loss (train_FNet.py:96-108) on the 1/V-averaged plane-sweep scores (B,D,H,W): softmax over the D
+    planes, soft-argmin depth with the plane depths ``planes``, mean |pred - gt_q| where ``mask_q`` (B,1,H,W) is set.
+    ``count`` = number of supervised pixels; by default it is read from the mask (one host read, which also rejects an
+    empty mask — pass it explicitly to capture the step in a CUDA graph)."""
+    mask_u8 = mask_q.to(torch.uint8)
+    if count is None:
+        count = int(mask_u8.sum().item())
+        if count == 0:
+            raise _lib.MagnetError("mask_q selects no pixel")
+    return FnetL1Loss.apply(scores, planes, gt_q, mask_u8, count)
 
 
 def relative_poses(ext_ref: torch.Tensor, ext_nghbr: torch.Tensor):
