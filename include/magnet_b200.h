@@ -147,6 +147,35 @@ typedef struct magnet_cost_f_bwd_args {
 int magnet_cost_volume_f_bwd_f32(const magnet_cost_f_bwd_args* args, void* stream);
 
 /*
+ * Backward of the cost volume with per-pixel depths (est_costvolume_CW, homography.py:79-161; consistency 0 or 1) w.r.t.
+ * both feature maps and the depth hypotheses — what autograd derives for the reference, through the 1/V mean, the
+ * consistency mask (piecewise constant: the source Gaussians get no gradient), the channel dot product and
+ * grid_sample's bilinear gather, including its derivative in the sample position.
+ * `fwd` is the forward call (depth_mode MAGNET_DEPTH_VOLUME or MAGNET_DEPTH_GAUSS); its src_layout and variant name the
+ * forward kernel, whose consistency mask the backward reproduces bit for bit.  Two forms:
+ *   - src_layout MAGNET_SRC_SPLIT16, variant AUTO or MMA (C == 64, V <= 16): fwd->ref_feat / fwd->src_feat are the split
+ *     buffers the forward read; grad_ref and grad_src come from the tensor-core kernel (two GEMMs on the fp16 hi/lo
+ *     planes).  The NCHW maps below are needed only for grad_depth.  With fwd->ref_feat and fwd->src_feat both NULL,
+ *     every gradient comes from the CUDA-core kernel on the NCHW maps, still with the tensor-core forward's mask;
+ *   - variant MAGNET_VARIANT_DIRECT (src_layout NCHW or TILED32): everything from the NCHW maps below, C <= 64.
+ * Other forward kernels (CELLS, TMA) are rejected with MAGNET_ERR_UNSUPPORTED.  The depth gradient always comes from
+ * the CUDA-core kernel; fwd->out is ignored.  Each of grad_ref, grad_src and grad_depth may be NULL when it is not wanted.
+ * grad_src is accumulated with atomics, so results are not bit-deterministic from run to run.
+ */
+typedef struct magnet_cost_bwd_args {
+  const magnet_cost_args* fwd;
+  const float* ref_feat;  /* (B,C,H,W) NCHW                                                                       */
+  const float* src_feat;  /* (V*B,C,H,W) NCHW, view-major                                                         */
+  const float* src_gmm;   /* (V*B,2,H,W) [mu, sigma]; required when fwd->consistency == 1                         */
+  const float* grad_out;  /* (B,D,H,W) gradient w.r.t. the forward output                                         */
+  float* workspace;       /* (B,D,H,W) scratch                                                                    */
+  float* grad_ref;        /* (B,C,H,W)   written, or NULL                                                         */
+  float* grad_src;        /* (V*B,C,H,W) ACCUMULATED with atomics (the caller zeroes it), or NULL                 */
+  float* grad_depth;      /* VOLUME: (B,D,H,W) w.r.t. d_volume; GAUSS: (B,2,H,W) w.r.t. ref_gmm; written, or NULL */
+} magnet_cost_bwd_args;
+int magnet_cost_volume_bwd_f32(const magnet_cost_bwd_args* args, void* stream);
+
+/*
  * Camera constants.  Replaces homography.py:89,98-102 (IntM/R/t products, done there per pair per
  * iteration).  intM (B,3,3) dense; R and t are addressed with element strides so that the
  * non-contiguous views nghbr_poses[:,:,:3,:3] / [:,:,:3,3] of MAGNET.py:147-148 can be passed as is:

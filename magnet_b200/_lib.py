@@ -26,7 +26,8 @@ VARIANT_AUTO, VARIANT_DIRECT, VARIANT_CELLS, VARIANT_CELLS_NOREUSE, VARIANT_TMA,
 # every symbol include/magnet_b200.h declares (tests check the library exports all of them)
 EXPORTS = (
     "magnet_abi_version", "magnet_strerror", "magnet_last_cuda_error", "magnet_launch_count",
-    "magnet_cost_launch_info", "magnet_cost_volume_f32", "magnet_cost_volume_f_bwd_f32", "magnet_pack_cameras_f32",
+    "magnet_cost_launch_info", "magnet_cost_volume_f32", "magnet_cost_volume_f_bwd_f32", "magnet_cost_volume_bwd_f32",
+    "magnet_pack_cameras_f32",
     "magnet_repack_tiled32_f32", "magnet_repack_pixc_f32", "magnet_repack_split16_f32", "magnet_split16_bytes", "magnet_sample_depths_f32", "magnet_gaussian_update_fwd_f32",
     "magnet_gaussian_update_bwd_f32", "magnet_convex_upsample_fwd_f32", "magnet_convex_upsample_bwd_f32",
     "magnet_relative_poses_f32", "magnet_camera_rays_f32",
@@ -51,6 +52,13 @@ class CostFBwdArgs(C.Structure):
     """Mirror of ``struct magnet_cost_f_bwd_args``."""
     _fields_ = [("fwd", C.POINTER(CostArgs)), ("prob", C.c_void_p), ("grad_out", C.c_void_p), ("workspace", C.c_void_p),
                 ("grad_ref", C.c_void_p), ("grad_src", C.c_void_p)]
+
+
+class CostBwdArgs(C.Structure):
+    """Mirror of ``struct magnet_cost_bwd_args``."""
+    _fields_ = [("fwd", C.POINTER(CostArgs)), ("ref_feat", C.c_void_p), ("src_feat", C.c_void_p), ("src_gmm", C.c_void_p),
+                ("grad_out", C.c_void_p), ("workspace", C.c_void_p), ("grad_ref", C.c_void_p), ("grad_src", C.c_void_p),
+                ("grad_depth", C.c_void_p)]
 
 
 class MagnetError(RuntimeError):
@@ -84,6 +92,8 @@ def lib() -> C.CDLL:
     L.magnet_cost_volume_f32.argtypes = [C.POINTER(CostArgs), C.c_void_p]
     L.magnet_cost_volume_f_bwd_f32.restype = C.c_int
     L.magnet_cost_volume_f_bwd_f32.argtypes = [C.POINTER(CostFBwdArgs), C.c_void_p]
+    L.magnet_cost_volume_bwd_f32.restype = C.c_int
+    L.magnet_cost_volume_bwd_f32.argtypes = [C.POINTER(CostBwdArgs), C.c_void_p]
     L.magnet_pack_cameras_f32.restype = C.c_int
     L.magnet_pack_cameras_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
                                           C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int32,

@@ -46,6 +46,9 @@ cudaError_t launch_upsample_bwd(const float* gout, const float* depth, const flo
 cudaError_t launch_cost_f_bwd(const BwdParams& p, cudaStream_t st, int* launches);
 cudaError_t launch_cost_f_bwd_mma(const BwdParams& p, cudaStream_t st, int* launches);
 bool f_bwd_mma_supports(int C, int V);
+cudaError_t launch_cost_cw_bwd(const CwBwdParams& p, const CwBwdParams* split, int C, int mode, bool mask_mma,
+                               const float* grad_out, cudaStream_t st, int* launches);
+bool cw_bwd_supports(int C);
 #ifdef MAGNET_MMA_DEBUG
 void f_bwd_mma_set_debug_buffer(float* p);
 #endif
@@ -233,6 +236,62 @@ int magnet_cost_volume_f_bwd_f32(const magnet_cost_f_bwd_args* b, void* stream) 
   int launches = 0;
   cudaError_t e = mma ? magnet::launch_cost_f_bwd_mma(p, (cudaStream_t)stream, &launches)
                       : magnet::launch_cost_f_bwd(p, (cudaStream_t)stream, &launches);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += launches;
+  return MAGNET_OK;
+}
+
+int magnet_cost_volume_bwd_f32(const magnet_cost_bwd_args* b, void* stream) {
+  if (!b || !b->fwd) return MAGNET_ERR_NULL;
+  const magnet_cost_args* a = b->fwd;
+  if (a->B <= 0 || a->V <= 0 || a->D <= 0 || a->C <= 0 || a->H <= 0 || a->W <= 0) return MAGNET_ERR_SHAPE;
+  if ((int64_t)a->H * a->W > (1 << 26) || a->B > 65535) return MAGNET_ERR_SHAPE;
+  if (a->D > MAGNET_MAX_PLANES) return MAGNET_ERR_UNSUPPORTED;
+  if (!a->rays || !a->cams || !b->grad_out || !b->workspace) return MAGNET_ERR_NULL;
+  if (a->softmax) return MAGNET_ERR_UNSUPPORTED;
+  switch (a->depth_mode) {
+    case MAGNET_DEPTH_VOLUME: if (!a->d_volume) return MAGNET_ERR_NULL; break;
+    case MAGNET_DEPTH_GAUSS: if (!a->ref_gmm || !a->k_host) return MAGNET_ERR_NULL; break;
+    default: return MAGNET_ERR_UNSUPPORTED;
+  }
+  const bool mask_mma = a->src_layout == MAGNET_SRC_SPLIT16;   // the tensor-core forward's mask
+  // its split buffers given: feature gradients on the tensor cores; both NULL: everything on the CUDA cores
+  const bool split = mask_mma && (a->ref_feat || a->src_feat);
+  if (mask_mma) {
+    if (a->variant != MAGNET_VARIANT_AUTO && a->variant != MAGNET_VARIANT_MMA) return MAGNET_ERR_UNSUPPORTED;
+    if (!magnet::mma_supports(a->C, a->D, a->V, a->src_layout) || !magnet::f_bwd_mma_supports(a->C, a->V))
+      return MAGNET_ERR_UNSUPPORTED;
+  }
+  if (split) {
+    if (!a->ref_feat || !a->src_feat) return MAGNET_ERR_NULL;
+    if (reinterpret_cast<uintptr_t>(a->src_feat) % 16 != 0 || reinterpret_cast<uintptr_t>(a->ref_feat) % 16 != 0)
+      return MAGNET_ERR_ALIGN;
+  } else if (!mask_mma && (a->variant != MAGNET_VARIANT_DIRECT ||
+             (a->src_layout != MAGNET_SRC_NCHW && a->src_layout != MAGNET_SRC_TILED32))) {
+    return MAGNET_ERR_UNSUPPORTED;                 // only the tensor-core and DIRECT forwards' masks are reproduced
+  }
+  // the CUDA-core kernel reads the NCHW maps: for every gradient without split buffers, for the depth gradient always
+  const bool nchw = !split || b->grad_depth != nullptr;
+  if (nchw) {
+    if (!b->ref_feat || !b->src_feat) return MAGNET_ERR_NULL;
+    if (a->consistency && !b->src_gmm) return MAGNET_ERR_NULL;
+    if (!magnet::cw_bwd_supports(a->C)) return MAGNET_ERR_UNSUPPORTED;
+  }
+  magnet::CwBwdParams p;
+  p.B = a->B; p.V = a->V; p.D = a->D; p.H = a->H; p.W = a->W; p.HW = a->H * a->W;
+  p.cw = a->consistency != 0;
+  p.kappa = a->kappa;
+  p.ref_feat = b->ref_feat; p.src_feat = b->src_feat; p.src_gmm = b->src_gmm; p.rays = a->rays; p.cams = a->cams;
+  p.d_volume = a->d_volume; p.ref_gmm = a->ref_gmm;
+  p.g_score = b->workspace;
+  p.grad_ref = b->grad_ref; p.grad_src = b->grad_src; p.grad_depth = b->grad_depth;
+  for (int j = 0; j < MAGNET_MAX_PLANES; ++j)
+    p.k[j] = (a->depth_mode == MAGNET_DEPTH_GAUSS && j < a->D) ? a->k_host[j] : 0.0f;
+  magnet::CwBwdParams ps = p;
+  ps.ref_feat = a->ref_feat; ps.src_feat = a->src_feat; ps.src_gmm = nullptr; ps.grad_depth = nullptr;
+  int launches = 0;
+  cudaError_t e = magnet::launch_cost_cw_bwd(p, split ? &ps : nullptr, a->C, a->depth_mode, mask_mma, b->grad_out,
+                                             (cudaStream_t)stream, &launches);
   if (e != cudaSuccess) return cuda_fail(e);
   g_launches += launches;
   return MAGNET_OK;

@@ -42,6 +42,25 @@ struct BwdParams {
   float k[MAGNET_MAX_PLANES];
 };
 
+// Kernel-side arguments of the CW-volume backward (magnet_cost_bwd_args + the geometry of its forward call).
+struct CwBwdParams {
+  int B, V, D, H, W, HW;
+  int cw;                                  // 1: consistency-weighted (the mask is applied), 0: plain sweep
+  float kappa;
+  const float* __restrict__ ref_feat;      // (B,C,H,W) NCHW
+  const float* __restrict__ src_feat;      // (V*B,C,H,W) NCHW
+  const float* __restrict__ src_gmm;       // (V*B,2,H,W)
+  const float* __restrict__ rays;
+  const magnet_camera* __restrict__ cams;
+  const float* __restrict__ d_volume;      // (B,D,H,W), MAGNET_DEPTH_VOLUME
+  const float* __restrict__ ref_gmm;       // (B,2,H,W), MAGNET_DEPTH_GAUSS
+  const float* __restrict__ g_score;       // (B,D,H,W) = grad_out / V
+  float* __restrict__ grad_ref;            // (B,C,H,W) written, or NULL
+  float* __restrict__ grad_src;            // (V*B,C,H,W) accumulated with atomics, or NULL
+  float* __restrict__ grad_depth;          // VOLUME (B,D,H,W) / GAUSS (B,2,H,W) written, or NULL
+  float k[MAGNET_MAX_PLANES];
+};
+
 // 1/x to <1 ulp: MUFU.RCP + one Newton step.  x == 0 -> NaN/inf, which the callers'
 // coordinate clamp turns into "out of bounds" (same outcome as the reference's +-10 clamp).
 __device__ __forceinline__ float rcp_nr(float x) {

@@ -1,6 +1,7 @@
 // Tensor-core backward of the fronto-parallel plane-sweep volume (homography.est_costvolume_F, homography.py:10-75)
 // w.r.t. both feature maps, on the MAGNET_SRC_SPLIT16 operands of the forward (cost_mma.cu) — F-Net training
-// (train_FNet.py:95-114).
+// (train_FNet.py:95-114).  The same kernel, instantiated with per-pixel depths and the consistency mask, gives the feature
+// gradients of the CW volume (est_costvolume_CW) after a tensor-core forward (DESIGN §3.5).
 //
 // With g = dL/dscore (the workspace of score_grad_kernel, already divided by V) and w_t(p, j) the bilinear weights of
 // plane j at reference pixel p in source view v, the gradients are the transpose of the forward's all-pairs product
@@ -43,6 +44,7 @@
 #include <mutex>
 
 #include "cells_common.cuh"
+#include "cw_mask.cuh"
 #include "tma_common.cuh"
 
 namespace magnet {
@@ -75,8 +77,27 @@ __device__ unsigned g_fbwd_done[FB_SLOTS];
 constexpr int FDBG_GC = 16, FDBG_G2 = FDBG_GC + 128 * 64, FDBG_G1 = FDBG_G2 + 128 * 64;   // FDBG_G1 + 2 * 64 * 64 floats in all
 #endif
 
+// The forward's consistency test (cost_mma.cu) of a sample at (ix, iy) with source depth z, cell (x0, y0) touching the
+// image: (mu, sigma) taps from the split buffer's paired table of the view (entry x0 + 1 <-> cell x0, zeros outside),
+// the helpers of cw_mask.cuh.  Not inlined: the call keeps the mask's temporaries out of the GEMM loop's registers.
+__device__ __noinline__ bool table_keep(const float4* __restrict__ meta, float ix, float iy, float z, int x0, int y0,
+                                        int W, int H, float kappa) {
+  float xf, yf, fx, fy;
+  cell_split(ix, xf, fx);
+  cell_split(iy, yf, fy);
+  const float4* row = meta + (size_t)y0 * (W + 1) + (x0 + 1);
+  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+  const float4 top = y0 >= 0 ? __ldg(row) : zero, bot = y0 + 1 < H ? __ldg(row + (W + 1)) : zero;
+  return cw_keep(z, lerp2d_x2(top, bot, fx, fy), kappa);
+}
+
+// P = BwdParams, MODE = PLANES, CW = false: the F volume.  P = CwBwdParams (MODE VOLUME or GAUSS, CW = true): the CW
+// volume, whose depths are per pixel and whose (pixel, hypothesis) pairs count only where the forward's consistency
+// mask kept them (p.cw == 1): the mask is evaluated with the helpers of cw_mask.cuh on the (mu, sigma) table of the
+// source SPLIT16 buffer, exactly as cost_mma.cu evaluates it.
+template <class P, int MODE, bool CW>
 __global__ void __launch_bounds__(BNT, 2)
-cost_f_bwd_mma_kernel(const __grid_constant__ BwdParams p, const __grid_constant__ CUtensorMap tm_ref,
+cost_f_bwd_mma_kernel(const __grid_constant__ P p, const __grid_constant__ CUtensorMap tm_ref,
                       const __grid_constant__ CUtensorMap tm_src, const int n_items, const int slot,
                       float* __restrict__ dbg) {
   extern __shared__ unsigned char smem_raw[];
@@ -165,15 +186,28 @@ cost_f_bwd_mma_kernel(const __grid_constant__ BwdParams p, const __grid_constant
     const float q1 = __fmaf_rn(cam->A[5], r2, __fmaf_rn(cam->A[4], r1, __fmul_rn(cam->A[3], r0)));
     const float q2 = __fmaf_rn(cam->A[8], r2, __fmaf_rn(cam->A[7], r1, __fmul_rn(cam->A[6], r0)));
     const int vb = v * p.B + b;
+    const float4* meta = nullptr;                          // (mu, sigma) table of the source split buffer (CW)
+    if constexpr (CW)
+      meta = reinterpret_cast<const float4*>(reinterpret_cast<const unsigned char*>(p.src_feat) + SPLIT16_HEADER +
+                                             (size_t)p.B * V * HW * 256);
     // cell origin of plane j at my pixel, and whether it can contribute (a tap in the image, g != 0)
     auto cell = [&](const int j, float& g, float& ix, float& iy, int& x0, int& y0) -> bool {
       g = ldg_f(gs + (size_t)j * HW);
-      float z;
-      project(p.k[j], a0, a1, a2, q0, q1, q2, ix, iy, z);
+      float z, d;
+      if constexpr (MODE == MAGNET_DEPTH_VOLUME) d = ldg_f(p.d_volume + ((size_t)b * D + j) * HW + n);
+      else if constexpr (MODE == MAGNET_DEPTH_GAUSS)     // MAGNET.py:155 (the pixel's Gaussian is re-read: registers)
+        d = __fadd_rn(ldg_f(p.ref_gmm + ((size_t)b * 2 + 0) * HW + n),
+                      __fmul_rn(ldg_f(p.ref_gmm + ((size_t)b * 2 + 1) * HW + n), p.k[j]));
+      else d = p.k[j];
+      project(d, a0, a1, a2, q0, q1, q2, ix, iy, z);
       clamp_pos(ix, iy, xmax, ymax);
       x0 = (int)floorf(ix);
       y0 = (int)floorf(iy);
-      return live && g != 0.0f && x0 >= -1 && x0 < W && y0 >= -1 && y0 < H;
+      bool ok = live && g != 0.0f && x0 >= -1 && x0 < W && y0 >= -1 && y0 < H;
+      if constexpr (CW) {
+        if (ok && p.cw) ok = table_keep(meta + (size_t)vb * H * (W + 1), ix, iy, z, x0, y0, W, H, p.kappa);
+      }
+      return ok;
     };
 
     // ---------------- pass 1: bounding box of the contributing cell origins ----------------------------------------
@@ -347,7 +381,7 @@ cost_f_bwd_mma_kernel(const __grid_constant__ BwdParams p, const __grid_constant
         dumped = dumped || dump;
 #endif
         // ---------------- g_src epilogue: cells inside the image, red.global.add, 1 / (s_G s_ref) -------------------
-        if (m_on) {
+        if (m_on && (!CW || p.grad_src != nullptr)) {
           const float sc = hdr_ref->inv_scale * inv_sg;
           float* gsrc = p.grad_src + (size_t)vb * 64 * HW;
           const int rr = wg * 64 + 16 * (warp & 3) + (lane >> 2);
@@ -398,7 +432,7 @@ cost_f_bwd_mma_kernel(const __grid_constant__ BwdParams p, const __grid_constant
       __syncthreads();
     }
     const float sc = hdr_src->inv_scale * inv_sg;
-    for (int idx = tid; idx < 64 * 64; idx += BNT) {
+    for (int idx = tid; idx < 64 * 64 && (!CW || p.grad_ref != nullptr); idx += BNT) {
       const int c = idx >> 6, q = idx & 63;
       const int x = tx0 + (q & 7), y = ty0 + (q >> 3);
       if (x < W && y < H) p.grad_ref[((size_t)b * 64 + c) * HW + (size_t)y * W + x] = st[c * 65 + q] * sc;
@@ -441,21 +475,24 @@ void f_bwd_mma_launch_info(int B, int H, int W, int* grid, int* block, int* smem
   *smem = B_SMEM_TOTAL;
 }
 
-// p.ref_feat / p.src_feat point to the SPLIT16 buffers of the forward (B and V*B images)
-cudaError_t launch_cost_f_bwd_mma(const BwdParams& p, cudaStream_t st, int* launches) {
+// work-counter tickets shared by every instantiation (they share the slots of g_fbwd_next / g_fbwd_done)
+static std::atomic<unsigned> ticket{0}, graph_ticket{0};
+
+// p.ref_feat / p.src_feat point to the SPLIT16 buffers of the forward (B and V*B images); p.g_score is written
+template <class P, int MODE, bool CW>
+static cudaError_t launch_bwd_mma(const P& p, cudaStream_t st) {
   static std::once_flag flags[64];
+  auto kern = cost_f_bwd_mma_kernel<P, MODE, CW>;
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
   cudaError_t res = cudaSuccess;
   std::call_once(flags[dev & 63], [&] {
-    res = cudaFuncSetAttribute(cost_f_bwd_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, B_SMEM_TOTAL);
+    res = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, B_SMEM_TOTAL);
     if (res == cudaSuccess)
-      res = cudaFuncSetAttribute(cost_f_bwd_mma_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                 cudaSharedmemCarveoutMaxShared);
+      res = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   });
   if (res != cudaSuccess) return res;
-  if ((e = launch_score_grad(p, st)) != cudaSuccess) return e;
   const unsigned char* refbuf = reinterpret_cast<const unsigned char*>(p.ref_feat);
   const unsigned char* srcbuf = reinterpret_cast<const unsigned char*>(p.src_feat);
   CUtensorMap tm_ref, tm_src;
@@ -464,7 +501,6 @@ cudaError_t launch_cost_f_bwd_mma(const BwdParams& p, cudaStream_t st, int* laun
   const int n_items = ((p.W + BTW - 1) / BTW) * ((p.H + BTH - 1) / BTH) * p.B;
   // work-counter slot: eager launches cycle through the lower half, captured launches own one of the upper half for
   // the life of their graph (cost_mma.cu)
-  static std::atomic<unsigned> ticket{0}, graph_ticket{0};
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   if (cudaStreamIsCapturing(st, &cap) != cudaSuccess) cap = cudaStreamCaptureStatusNone;
   const int slot = cap == cudaStreamCaptureStatusActive ? FB_SLOTS / 2 + (int)(graph_ticket.fetch_add(1) % (FB_SLOTS / 2))
@@ -473,10 +509,22 @@ cudaError_t launch_cost_f_bwd_mma(const BwdParams& p, cudaStream_t st, int* laun
 #ifdef MAGNET_MMA_DEBUG
   dbg = g_fbwd_dbg;
 #endif
-  cost_f_bwd_mma_kernel<<<std::min(n_items, 2 * sm_count(dev)), BNT, B_SMEM_TOTAL, st>>>(p, tm_ref, tm_src, n_items, slot,
-                                                                                         dbg);
-  *launches = 2;
+  kern<<<std::min(n_items, 2 * sm_count(dev)), BNT, B_SMEM_TOTAL, st>>>(p, tm_ref, tm_src, n_items, slot, dbg);
   return cudaGetLastError();
+}
+
+cudaError_t launch_cost_f_bwd_mma(const BwdParams& p, cudaStream_t st, int* launches) {
+  cudaError_t e = launch_score_grad(p, st);
+  if (e != cudaSuccess) return e;
+  *launches = 2;
+  return launch_bwd_mma<BwdParams, MAGNET_DEPTH_PLANES, false>(p, st);
+}
+
+// CW volume, feature gradients on the tensor cores: p.ref_feat / p.src_feat are the forward's split buffers, p.g_score
+// already holds grad_out / V (cost_cw_bwd.cu)
+cudaError_t launch_cost_cw_bwd_mma(const CwBwdParams& p, int mode, cudaStream_t st) {
+  if (mode == MAGNET_DEPTH_VOLUME) return launch_bwd_mma<CwBwdParams, MAGNET_DEPTH_VOLUME, true>(p, st);
+  return launch_bwd_mma<CwBwdParams, MAGNET_DEPTH_GAUSS, true>(p, st);
 }
 
 }  // namespace magnet

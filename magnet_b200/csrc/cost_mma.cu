@@ -47,6 +47,7 @@
 
 #include "common.cuh"
 #include "tma_common.cuh"
+#include "cw_mask.cuh"
 
 namespace magnet {
 
@@ -99,16 +100,6 @@ __device__ __forceinline__ float4 lds_f32x4(uint32_t a) {
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
   return v;
 }
-// bilinear interpolation of a (mu, sigma) pair; v01 - v00 as fma(v00, -1, v01) (exact product, one rounding = the
-// subtraction)
-__device__ __forceinline__ float2 lerp2d_x2(float4 top, float4 bot, float fx, float fy) {
-  const float2 v00 = make_float2(top.x, top.y), v01 = make_float2(top.z, top.w);
-  const float2 v10 = make_float2(bot.x, bot.y), v11 = make_float2(bot.z, bot.w);
-  const float2 m1 = make_float2(-1.0f, -1.0f), fx2 = make_float2(fx, fx), fy2 = make_float2(fy, fy);
-  const float2 t = ffma2_rn(fx2, ffma2_rn(v00, m1, v01), v00), u = ffma2_rn(fx2, ffma2_rn(v10, m1, v11), v10);
-  return ffma2_rn(fy2, ffma2_rn(t, m1, u), t);
-}
-
 template <int MODE, bool CW>
 __global__ void __launch_bounds__(MNT, 2)
 cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CUtensorMap tm_ref,
@@ -259,8 +250,8 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
     auto project_px = [&](const int i, float2& ix, float2& iy, float2& z) {
       const float4 t1 = pixt[2 * i], t2 = pixt[2 * i + 1];   // same address on every lane: broadcast
       project2(depth2(i, t2.y, t2.z), a0, a1, a2, t1.x, t1.y, t1.z, ix, iy, z);
-      ix.x = fminf(fmaxf(ix.x, -2.0f), xmax); ix.y = fminf(fmaxf(ix.y, -2.0f), xmax);
-      iy.x = fminf(fmaxf(iy.x, -2.0f), ymax); iy.y = fminf(fmaxf(iy.y, -2.0f), ymax);
+      ix.x = clamp_coord(ix.x, xmax); ix.y = clamp_coord(ix.y, xmax);
+      iy.x = clamp_coord(iy.x, ymax); iy.y = clamp_coord(iy.y, ymax);
     };
 
     // ---------------- projection of every hypothesis, bounding box of the tile's sample positions -------------
@@ -379,9 +370,10 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
             if (!((livemask >> i) & 1u)) continue;         // warp-uniform
             float2 x, y, z;
             project_px(i, x, y, z);
-            const float2 x0 = make_float2(floorf(x.x), floorf(x.y)), y0 = make_float2(floorf(y.x), floorf(y.y));
+            float2 x0, y0, fx, fy;                         // cell origins and fractions (cw_mask.cuh)
+            cell_split(x.x, x0.x, fx.x); cell_split(x.y, x0.y, fx.y);
+            cell_split(y.x, y0.x, fy.x); cell_split(y.y, y0.y, fy.y);
             const float2 m1 = make_float2(-1.0f, -1.0f);
-            const float2 fx = ffma2_rn(x0, m1, x), fy = ffma2_rn(y0, m1, y);       // x - floor(x), exact
             // byte offset of the cell in a G row = 4 * ((y0 - sy) * pitch + (x0 - sx)), in fp32 (small integers, exact)
             // on top of 1.5 * 2^23 so that the integer sits in the mantissa
             const float2 o = ffma2_rn(y0, make_float2(pitch4f, pitch4f), ffma2_rn(x0, make_float2(4.0f, 4.0f), make_float2(c0f, c0f)));
@@ -406,9 +398,8 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
               // table entry of a cell = (mu, sigma) of the cell and of its right neighbour: two 16-byte reads per hypothesis
               const float2 msa = lerp2d_x2(lds_f32x4(ma), lds_f32x4(ma + pitch4 * 4u), fx.x, fy.x);
               const float2 msb = lerp2d_x2(lds_f32x4(mb), lds_f32x4(mb + pitch4 * 4u), fx.y, fy.y);
-              // homography.py:157-158: |z - mu~| < sigma~ * kappa, strict
-              oka = fabsf(__fsub_rn(z.x, msa.x)) < __fmul_rn(msa.y, kappa);
-              okb = fabsf(__fsub_rn(z.y, msb.x)) < __fmul_rn(msb.y, kappa);
+              oka = cw_keep(z.x, msa, kappa);               // homography.py:157-158 (cw_mask.cuh)
+              okb = cw_keep(z.y, msb, kappa);
             } else {
               oka = fabsf(costa) < 3.0e38f;
               okb = fabsf(costb) < 3.0e38f;

@@ -14,8 +14,10 @@ per-(batch, view) Python loop):
   * ``nghbr_feat`` / ``nghbr_gmms`` / ``ref_feat`` arrive NCHW: split once per forward into the fp16 hi/lo planes the
     tensor-core kernel's TMA boxes fetch (C == 64; else the pixel-major PIXC layout of the TMA-staged CUDA-core kernel;
     cached the same way; bypassed under CUDA-graph capture).
-The CW volume is not differentiable (its inputs never require grad in the reference, SURVEY §3.2);
-the F volume is differentiable w.r.t. both feature maps (magnet_cost_volume_f_bwd_f32) for F-Net training.
+Both volumes are differentiable as in the reference: the CW volume w.r.t. both feature maps and the depth volume
+(magnet_cost_volume_bwd_f32; built only when grad mode is on and one of them requires grad, so that G-Net training,
+where none does, runs exactly the no-grad path), the F volume w.r.t. both feature maps (magnet_cost_volume_f_bwd_f32)
+for F-Net training.
 """
 from __future__ import annotations
 
@@ -168,6 +170,64 @@ def _packed_source(nghbr_feat, nghbr_gmms, V, variant, ref_feat=None, D=MMA_MIN_
     return hit, _lib.SRC_TILED32, None
 
 
+def check_geometry_grad(**named) -> None:
+    """The cost volume is differentiable in the feature maps and the depths only: raise instead of silently dropping
+    the gradient of a camera tensor."""
+    for name, x in named.items():
+        if isinstance(x, torch.Tensor) and x.requires_grad:
+            raise _lib.MagnetError(f"{name} requires grad, but the cost volume is differentiable only in the feature "
+                                   "maps and the depth hypotheses (detach the camera tensors)")
+
+
+def wants_cw_grad(*tensors) -> bool:
+    """The differentiable CW path is taken only when grad mode is on and one of the differentiable inputs requires
+    grad; otherwise the no-grad path runs (same kernels, nothing saved, no autograd node)."""
+    return torch.is_grad_enabled() and any(x is not None and x.requires_grad for x in tensors)
+
+
+class _CostVolumeCW(torch.autograd.Function):
+    """Cost volume with per-pixel depths (d_volume, or the Gaussian + k of the fused sampler), differentiable in the
+    depth source and both feature maps.  ``run()`` launches the forward kernel and returns (volume, layout, variant,
+    (ref split, source split) or None): the backward (magnet_cost_volume_bwd_f32) reproduces that kernel's consistency
+    mask.  After a SPLIT16 forward the feature gradients run on the tensor cores on the same split buffers (the rule of
+    _PlaneSweepF), otherwise on the CUDA cores; the depth gradient always on the CUDA cores.  The source Gaussians get
+    no gradient (the mask is piecewise constant)."""
+
+    @staticmethod
+    def forward(ctx, depth, ref_feat, nghbr_feat, nghbr_gmms, run, spec):
+        out, layout, variant, splits = run()
+        ctx.save_for_backward(depth.detach(), ref_feat.detach(), nghbr_feat.detach(), nghbr_gmms.detach())
+        ctx.spec, ctx.fwd, ctx.splits = spec, (layout, variant), splits or (None, None)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        depth, ref, src, gmm = ctx.saved_tensors
+        rays, cams, V, kappa, karr = ctx.spec
+        need_d, need_ref, need_src = ctx.needs_input_grad[:3]
+        g_ref, g_src, g_d = ops.cost_volume_bwd(
+            ref, src, gmm, rays, cams, grad_out.contiguous(), V=V, kappa=kappa,
+            d_volume=depth if karr is None else None, ref_gmm=depth if karr is not None else None, k=karr,
+            fwd_layout=ctx.fwd[0], fwd_variant=ctx.fwd[1], need_ref=need_ref, need_src=need_src, need_depth=need_d,
+            ref_split=ctx.splits[0], src_split=ctx.splits[1])
+        return g_d, g_ref, g_src, None, None, None
+
+
+def differentiable_layout(C: int, V: int, D: int, variant: int, split16_ok: bool = True) -> int:
+    """Source layout of a differentiable CW forward: SPLIT16 (tensor cores) where the no-grad path would use it, else
+    NCHW with the DIRECT kernel — the two forward kernels whose consistency mask the backward reproduces."""
+    if variant not in (_lib.VARIANT_AUTO, _lib.VARIANT_MMA, _lib.VARIANT_DIRECT):
+        raise _lib.MagnetError("a differentiable CW volume runs on the tensor-core or the DIRECT kernel (variant AUTO, MMA "
+                               f"or DIRECT), got variant {variant}")
+    if C > 64:
+        raise _lib.MagnetError(f"the CW backward supports C <= 64 channels, got C={C}")
+    if split16_ok and _wants_split16(C, V, variant, D):
+        return _lib.SRC_SPLIT16
+    if variant == _lib.VARIANT_MMA:
+        raise _lib.MagnetError(f"MAGNET_VARIANT_MMA needs C == 64 and V <= 16, got C={C}, V={V}")
+    return _lib.SRC_NCHW
+
+
 def est_costvolume_CW(d_volume, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms,
                       R, t, is_valid, cam_intrins, thres, variant=_lib.VARIANT_AUTO):
     """Consistency-weighted multi-view cost volume — drop-in for homography.est_costvolume_CW.
@@ -176,10 +236,32 @@ def est_costvolume_CW(d_volume, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms,
     the reference, SURVEY A.5 #7); nghbr_gmms (V*B,2,H,W) [mu, sigma]; R (B,V,3,3), t (B,V,3) device
     views; is_valid (B,V) int CPU or device; cam_intrins dict of 'intM' (B,3,3) and
     'unit_ray_array_2D' (B,3,H*W), CPU or device; thres int.  Returns (B,D,H,W) float32 on
-    ref_feat.device, freshly allocated, detached."""
+    ref_feat.device, freshly allocated.  Differentiable, as the reference, in d_volume, ref_feat and nghbr_feat when
+    grad mode is on and one of them requires grad (the camera tensors must not require grad); detached otherwise."""
     device = ref_feat.device
     B = d_volume.shape[0]
     V = int(nghbr_feat.shape[0] / B)
+    if torch.is_grad_enabled():
+        check_geometry_grad(R=R, t=t, intM=cam_intrins['intM'], unit_ray_array_2D=cam_intrins['unit_ray_array_2D'])
+    if wants_cw_grad(d_volume, ref_feat, nghbr_feat):
+        D, C = int(d_volume.shape[1]), int(ref_feat.shape[1])
+        layout = differentiable_layout(C, V, D, variant)
+        _, rays_d = _device_intrinsics(cam_intrins, device)
+        cams = _camera_table(cam_intrins, R, t, is_valid, device)
+
+        def run():
+            if layout == _lib.SRC_SPLIT16:
+                src, _, ref_split = _packed_source(nghbr_feat, nghbr_gmms, V, variant, ref_feat, D)
+                fv = variant
+            else:
+                src, ref_split, fv = nghbr_feat.detach().contiguous(), None, _lib.VARIANT_DIRECT
+            out = ops.cost_volume(ref_feat.detach(), src, rays_d, cams, V=V, src_layout=layout, consistency=True,
+                                  src_gmm=nghbr_gmms.detach(), kappa=float(thres), d_volume=d_volume.detach(),
+                                  variant=fv, ref_split=ref_split)
+            return out, layout, fv, (ref_split, src) if layout == _lib.SRC_SPLIT16 else None
+
+        return _CostVolumeCW.apply(d_volume, ref_feat, nghbr_feat, nghbr_gmms, run,
+                                   (rays_d, cams, V, float(thres), None))
     with torch.no_grad():
         _, rays_d = _device_intrinsics(cam_intrins, device)
         cams = _camera_table(cam_intrins, R, t, is_valid, device)

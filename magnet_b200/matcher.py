@@ -14,7 +14,8 @@ import torch
 import torch.nn as nn
 
 from . import _lib, ops
-from .homography import MMA_MIN_PLANES
+from .homography import (MMA_MIN_PLANES, _CostVolumeCW, check_geometry_grad, differentiable_layout,
+                         wants_cw_grad)
 from .sampling import depth_sampling
 
 
@@ -60,6 +61,9 @@ class MatchingPlan:
 
     def __init__(self, ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, *,
                  thres: int = 5, src_layout: int = _lib.SRC_SPLIT16):
+        if torch.is_grad_enabled():
+            check_geometry_grad(nghbr_poses=nghbr_poses, intM=cam_intrins['intM'],
+                                unit_ray_array_2D=cam_intrins['unit_ray_array_2D'])
         dev = ref_feat.device
         self.B, self.C, self.H, self.W = ref_feat.shape
         self.V = nghbr_feat.shape[0] // self.B
@@ -71,6 +75,7 @@ class MatchingPlan:
         R, t = nghbr_poses[:, :, :3, :3], nghbr_poses[:, :, :3, 3]
         self.cams = ops.pack_cameras(intM, R, t, is_valid.to(dev, torch.int32))
         self._nghbr_feat = nghbr_feat.detach()
+        self._ref_in, self._src_in = ref_feat, nghbr_feat   # the caller's tensors: cost() is differentiable in them
         self._packed = {}
         self._ref_split = None
         # Production: the tensor-core kernel on the fp16 hi/lo planes (C == 64 and at least half a chunk of hypotheses,
@@ -100,7 +105,11 @@ class MatchingPlan:
         return self._packed[layout]
 
     def cost(self, gmm: torch.Tensor, k, out: Optional[torch.Tensor] = None, variant=_lib.VARIANT_AUTO):
-        """Fused sampler + CW cost volume for the current Gaussian (B,2,H,W)."""
+        """Fused sampler + CW cost volume for the current Gaussian (B,2,H,W).  Differentiable in the plan's feature maps
+        and in ``gmm`` when grad mode is on and one of them requires grad (then ``out`` must be None); detached
+        otherwise."""
+        if wants_cw_grad(gmm, self._ref_in, self._src_in):
+            return self._cost_differentiable(gmm, k, out, variant)
         layout = self.layout
         n_planes = len(k)
         if layout == _lib.SRC_SPLIT16 and variant == _lib.VARIANT_AUTO and n_planes < MMA_MIN_PLANES:
@@ -118,23 +127,47 @@ class MatchingPlan:
                                ref_split=self._ref_split if layout == _lib.SRC_SPLIT16 else None)
 
 
+    def _cost_differentiable(self, gmm, k, out, variant):
+        if out is not None:
+            raise _lib.MagnetError("cost(out=...) writes into a caller buffer and cannot be differentiated")
+        karr = ops.k_array(k)
+        layout = differentiable_layout(self.C, self.V, len(karr), variant, split16_ok=self.layout == _lib.SRC_SPLIT16)
+
+        def run():
+            fv = variant if layout == _lib.SRC_SPLIT16 else _lib.VARIANT_DIRECT
+            src = self._source(layout)
+            vol = ops.cost_volume(self.ref_feat, src, self.rays, self.cams, V=self.V, src_layout=layout,
+                                  consistency=True, src_gmm=self.src_gmm, kappa=self.kappa, ref_gmm=gmm.detach(),
+                                  k=karr, variant=fv, ref_split=self._ref_split if layout == _lib.SRC_SPLIT16 else None)
+            return vol, layout, fv, (self._ref_split, src) if layout == _lib.SRC_SPLIT16 else None
+
+        return _CostVolumeCW.apply(gmm, self._ref_in, self._src_in, self.src_gmm, run,
+                                   (self.rays, self.cams, self.V, self.kappa, karr))
+
+
 def matching_loop(plan: MatchingPlan, ref_gmms: torch.Tensor, x_d3: torch.Tensor,
                   g_net_convs, n_iter: int, k: Sequence[float],
-                  variant=_lib.VARIANT_AUTO) -> List[torch.Tensor]:
+                  variant=_lib.VARIANT_AUTO, detach_cost: bool = True) -> List[torch.Tensor]:
     """pred_list of MAGNET.py:150-169: [ref_gmms, pred_1, ..., pred_n_iter] at quarter resolution.
 
     ``g_net_convs`` is either a callable mapping the (B, D+256, H, W) concatenation [cost volume, x_d3] to the
     raw (B,2,H,W) G-Net output (``GNET.gnet``, the reference's data flow), or a ``GNET`` module — then the
     iteration-invariant x_d3 half of the first convolution is computed once and the per-iteration ``cat`` is
     skipped (f-3).  Gradients flow exactly where the reference lets them: through the update into the conv
-    weights, never into the cost volume (MAGNET.py:167 detaches it)."""
+    weights, never into the cost volume (MAGNET.py:167 detaches it).  With ``detach_cost=False`` the cost volume stays
+    in the graph, so feature maps that require grad (a trainable F-Net upstream) receive gradients through it; the
+    Gaussian that places the hypotheses stays detached, as in the reference (MAGNET.py:153)."""
     karr = ops.k_array(k)
     preds = [ref_gmms]
     split = isinstance(g_net_convs, GNET)
     inv = g_net_convs.invariant_part(x_d3, len(karr)) if split else None
     for _ in range(n_iter):
         cur = preds[-1].detach()
-        cv = plan.cost(cur, karr, variant=variant)
+        if detach_cost:
+            with torch.no_grad():
+                cv = plan.cost(cur, karr, variant=variant)
+        else:
+            cv = plan.cost(cur, karr, variant=variant)
         raw = g_net_convs.raw_from_parts(cv, inv) if split else g_net_convs(torch.cat([cv, x_d3], dim=1))
         preds.append(ops.gaussian_update(raw, cur))
     return preds
@@ -146,9 +179,12 @@ class MagnetHead(nn.Module):
     checkpoints / torch.hub in the reference and are out of scope, SURVEY §2.1 #3-4)."""
 
     def __init__(self, n_samples: int = 5, sampling_range: float = 3, n_iter: int = 3, thres: int = 5,
-                 downsample_ratio: int = 4, dnet_fdim: int = 256):
+                 downsample_ratio: int = 4, dnet_fdim: int = 256, detach_cost: bool = True):
         super().__init__()
         self.n_iter, self.thres, self.downsample_ratio = n_iter, thres, downsample_ratio
+        # True: G-Net reads a detached cost volume (MAGNET.py:167).  False: the volume stays in the graph, so a trainable
+        # F-Net upstream receives gradients through the matching.
+        self.detach_cost = detach_cost
         self.k_list = depth_sampling(sampling_range, n_samples)
         self.g_net = GNET(ch_in=dnet_fdim + n_samples, ch_out=2)
         h_dim = 128
@@ -173,7 +209,7 @@ class MagnetHead(nn.Module):
         """The N_iter quarter-resolution predictions and the upsampling mask, NOT upsampled: what the fused
         upsample + NLL loss (``loss`` below) consumes during training."""
         plan = MatchingPlan(ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, thres=self.thres)
-        preds = matching_loop(plan, ref_gmms, x_d3, self.g_net, self.n_iter, self.k_list)
+        preds = matching_loop(plan, ref_gmms, x_d3, self.g_net, self.n_iter, self.k_list, detach_cost=self.detach_cost)
         return preds[1:], self.mask_head(x_d3)
 
     def loss(self, preds_quarter, mask, gt_depth, gt_depth_mask, gamma: float = 0.8):

@@ -285,6 +285,75 @@ def cost_volume_f_bwd(ref_feat, src_feat_nchw, rays, cams, planes, V, prob, grad
     return g_ref, g_src
 
 
+def cost_volume_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V: int, kappa: float, consistency=True,
+                    d_volume=None, ref_gmm=None, k=None, fwd_layout=_lib.SRC_NCHW, fwd_variant=_lib.VARIANT_DIRECT,
+                    need_ref=True, need_src=True, need_depth=True, ref_split=None, src_split=None):
+    """Gradients of the cost volume with per-pixel depths — one magnet_cost_volume_bwd_f32 call.
+    ref_feat (B,C,H,W), src_feat (V*B,C,H,W) view-major and src_gmm (V*B,2,H,W) are NCHW; the depth source is
+    ``d_volume`` (B,D,H,W) or ``ref_gmm`` (B,2,H,W) + ``k``, as in the forward.  ``fwd_layout`` / ``fwd_variant`` name
+    the forward kernel (SRC_SPLIT16 with AUTO / MMA: tensor cores; VARIANT_DIRECT): its consistency mask is applied.
+    After a SPLIT16 forward, ``ref_split`` / ``src_split`` are the repack_split16 buffers it read: both feature gradients
+    then come from the tensor-core kernel on them (the NCHW maps serve the depth gradient only); without them the
+    CUDA-core kernel computes every gradient with the tensor-core forward's mask (the cross-check).
+    Returns (grad_ref, grad_src, grad_depth), each None when not requested; grad_depth is (B,D,H,W) w.r.t. d_volume or
+    (B,2,H,W) w.r.t. ref_gmm."""
+    ref_feat = _need_cuda_f32("ref_feat", ref_feat)
+    src = _need_cuda_f32("src_feat", src_feat)
+    rays = _need_cuda_f32("rays", rays)
+    cams = _need_cuda_f32("cams", cams)
+    grad_out = _need_cuda_f32("grad_out", grad_out)
+    B, Cc, H, W = ref_feat.shape
+    _expect("src_feat", src, (V * B, Cc, H, W))
+    _expect("rays", rays, (B, 3, H * W))
+    if cams.numel() != B * V * 16:
+        raise _lib.MagnetError(f"cams must hold B*V = {B * V} camera records of 16 floats, got {tuple(cams.shape)}")
+    a = CostArgs()
+    a.B, a.V, a.C, a.H, a.W = B, V, Cc, H, W
+    a.src_layout, a.variant, a.consistency, a.softmax, a.kappa = fwd_layout, fwd_variant, 1 if consistency else 0, 0, float(kappa)
+    a.rays, a.cams = rays.data_ptr(), cams.data_ptr()
+    karr = None
+    if d_volume is not None:
+        d_volume = _need_cuda_f32("d_volume", d_volume)
+        if d_volume.dim() != 4 or d_volume.shape[0] != B or tuple(d_volume.shape[2:]) != (H, W):
+            raise _lib.MagnetError(f"d_volume must be (B,D,H,W) = ({B},D,{H},{W}), got {tuple(d_volume.shape)}")
+        a.depth_mode, a.D, a.d_volume = _lib.DEPTH_VOLUME, d_volume.shape[1], d_volume.data_ptr()
+        gd_shape = tuple(d_volume.shape)
+    else:
+        karr = k if isinstance(k, C.Array) else k_array(k)
+        ref_gmm = _need_cuda_f32("ref_gmm", ref_gmm)
+        _expect("ref_gmm", ref_gmm, (B, 2, H, W))
+        a.depth_mode, a.D, a.ref_gmm, a.k_host = _lib.DEPTH_GAUSS, len(karr), ref_gmm.data_ptr(), C.cast(karr, C.c_void_p)
+        gd_shape = (B, 2, H, W)
+    _expect("grad_out", grad_out, (B, a.D, H, W))
+    if fwd_layout == _lib.SRC_SPLIT16 and (ref_split is not None or src_split is not None):
+        for nm, buf, nimg in (("src_split", src_split, V * B), ("ref_split", ref_split, B)):
+            if not (isinstance(buf, torch.Tensor) and buf.is_cuda and buf.dtype == torch.uint8 and buf.is_contiguous()):
+                raise _lib.MagnetError(f"{nm} must be a contiguous uint8 CUDA buffer from repack_split16")
+            _expect(nm, buf, (int(lib().magnet_split16_bytes(nimg, H, W)),))
+        a.ref_feat, a.src_feat = ref_split.data_ptr(), src_split.data_ptr()
+    bw = _lib.CostBwdArgs()
+    bw.fwd = C.pointer(a)
+    bw.ref_feat, bw.src_feat = ref_feat.data_ptr(), src.data_ptr()
+    if consistency:
+        src_gmm = _need_cuda_f32("src_gmm", src_gmm)
+        _expect("src_gmm", src_gmm, (V * B, 2, H, W))
+        bw.src_gmm = src_gmm.data_ptr()
+    dev = _same_device(("ref_feat", ref_feat), ("src_feat", src), ("src_gmm", src_gmm if consistency else None),
+                       ("rays", rays), ("cams", cams), ("grad_out", grad_out), ("d_volume", d_volume),
+                       ("ref_gmm", ref_gmm), ("ref_split", ref_split), ("src_split", src_split))
+    work = torch.empty_like(grad_out)
+    g_ref = torch.empty_like(ref_feat) if need_ref else None
+    g_src = torch.zeros_like(src) if need_src else None
+    g_d = torch.empty(gd_shape, device=dev, dtype=torch.float32) if need_depth else None
+    bw.grad_out, bw.workspace = grad_out.data_ptr(), work.data_ptr()
+    bw.grad_ref = g_ref.data_ptr() if need_ref else None
+    bw.grad_src = g_src.data_ptr() if need_src else None
+    bw.grad_depth = g_d.data_ptr() if need_depth else None
+    with torch.cuda.device(dev):
+        check(lib().magnet_cost_volume_bwd_f32(C.byref(bw), _stream(dev)), "magnet_cost_volume_bwd_f32")
+    return g_ref, g_src, g_d
+
+
 def cost_launch_info(B, V, D, Cc, H, W, variant=_lib.VARIANT_AUTO):
     """(grid CTAs, threads per CTA, dynamic smem bytes) the cost kernel would use for these sizes."""
     a = CostArgs()
