@@ -21,7 +21,7 @@ void mma_launch_info(int B, int H, int W, int D, int* grid, int* block, int* sme
 size_t split16_buffer_bytes(int N, int H, int W);
 cudaError_t launch_repack_split16(const float* src, const float* gmm, void* dst, int N, int C, int H, int W,
                                   cudaStream_t st, int* launches);
-#ifdef MAGNET_MMA_DEBUG
+#if defined(MAGNET_MMA_DEBUG) || defined(MAGNET_MMA_PROFILE)
 void mma_set_debug_buffer(float* p);
 #endif
 cudaError_t launch_repack_pixc(const float* src, const float* gmm, float* dst, int N, int C, int H, int W,
@@ -352,8 +352,11 @@ int magnet_repack_split16_f32(const float* src_nchw, const float* src_gmm, void*
   return MAGNET_OK;
 }
 
-#ifdef MAGNET_MMA_DEBUG
+#if defined(MAGNET_MMA_DEBUG) || defined(MAGNET_MMA_PROFILE)
+// MAGNET_MMA_PROFILE builds: the buffer receives the per-stage clock64() totals of cost_mma_kernel (uint64[8])
 void magnet_mma_debug_buffer(float* p) { magnet::mma_set_debug_buffer(p); }
+#endif
+#ifdef MAGNET_MMA_DEBUG
 void magnet_f_bwd_mma_debug_buffer(float* p) { magnet::f_bwd_mma_set_debug_buffer(p); }
 #endif
 

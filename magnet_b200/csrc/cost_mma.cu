@@ -24,11 +24,12 @@
 //     64-hypothesis chunk, evaluated side by side as float2 pairs): the pixel's constants are warp-uniform (per-warp table
 //     in shared memory), the 32 lanes read a handful of neighbouring cells of ONE accumulator row (broadcast /
 //     conflict-free); lanes beyond the last hypothesis replicate it, so there are no activity predicates.
-//   * per view: project all hypotheses (exact bounding box) -> TMA window + paired (mu, sigma) table -> 12 x wgmma
-//     m64n128k16 per warpgroup (3 products x 4 K steps) -> the 64 accumulator rows into shared memory (over the window,
-//     which is dead by then) -> per-hypothesis phase, which projects again from the per-warp pixel table (the 32
-//     positions do not fit the registers next to the 64 accumulators).  The view
-//     accumulators live in shared memory (hypothesis-major: the layout the coalesced epilogue reads).
+//   * per view: TMA window + paired (mu, sigma) table -> 12 x wgmma m64n128k16 per warpgroup (3 products x 4 K steps)
+//     -> the 64 accumulator rows into shared memory (over the window, which is dead by then) -> the NEXT view's window
+//     box (projections of each pixel's smallest and largest depth, window_box) -> per-hypothesis phase, which projects
+//     from the per-warp pixel table.  The box is complete at the barrier that ends the phase, so the next view's copies
+//     are issued right after it.  The 16 view accumulators of a lane stay in registers; the epilogue transposes them
+//     through region R into the hypothesis-major layout of the coalesced stores.
 //   * a window that does not fit 256 cells is cut into sub-windows of <= 32 segments that overlap by one cell column /
 //     row; a hypothesis is evaluated in the sub-window that holds its cell origin.  Same code for any depth distribution.
 //   * persistent CTAs (two per SM): work items (batch element, tile, 64-hypothesis chunk) come from a global counter in a
@@ -69,11 +70,16 @@ constexpr int MOFF_CAM = MOFF_META + MSEG * META_SEG_BYTES; // magnet_camera[MMA
 constexpr int MOFF_KS = MOFF_CAM + MMAXV * 64;              // float[MCH]
 constexpr int MOFF_BBOX = MOFF_KS + MCH * 4;                // int[2 slots][4]
 constexpr int MOFF_BAR = MOFF_BBOX + 64;                    // 2 mbarriers, next work item
-constexpr int MOFF_ACC = MOFF_BAR + 64;                     // float[MCH][65]: view accumulators, hypothesis-major
-constexpr int MOFF_PIX = MOFF_ACC + MCH * 65 * 4;           // float4[8 warps][8 pixels][2]: (q0,q1,q2,-) (q2,mu,sigma,-)
+constexpr int MOFF_DV = MOFF_BAR + 64;                      // float[MPX][65]: depths of the item, pixel-major (VOLUME)
+constexpr int MOFF_DEND = MOFF_DV + MPX * 65 * 4;           // float2[MPX]: depth range of each pixel (VOLUME)
+constexpr int MOFF_PIXR = MOFF_DEND + MPX * 8;              // float4[MPX][2]: (ray, -) (mu, sigma, -, -) of each pixel
+constexpr int MOFF_PIX = MOFF_PIXR + MPX * 32;              // float4[8 warps][8 pixels][2]: (q0,q1,q2,a0) (a1,mu,sigma,a2)
 constexpr int M_SMEM_USED = MOFF_PIX + 8 * 8 * 32;
 constexpr int M_SMEM_TOTAL = M_SMEM_USED + 1024;            // slack for the 1024-byte alignment of the base
 static_assert(MR_BYTES >= MSEG * SEG_BYTES && MR_BYTES >= MPX * 264 * 4 && MR_BYTES >= MCH * 65 * 4, "region R");
+// MAGNET_MMA_DEBUG builds: the debug buffer holds a G dump (16 + 64 * 256 floats), then two uint32 counters: hypotheses
+// whose cell origin fell outside their window box (must stay 0) and tile rows whose box took the exact per-hypothesis pass
+constexpr int MMA_DBG_OUTSIDE = 16 + MPX * 256;
 static_assert(2 * (M_SMEM_TOTAL + 1024) <= 227 * 1024, "two CTAs per SM");
 
 // header | fp16 planes (N, 2, H, W, 64) | table (N, H, W + 1, 4): entry x + 1 of a row = (mu, sigma)[x], (mu, sigma)[x + 1]
@@ -100,6 +106,22 @@ __device__ __forceinline__ float4 lds_f32x4(uint32_t a) {
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
   return v;
 }
+// MAGNET_MMA_PROFILE builds: thread 0 reads clock64() at the CTA barriers that separate the stages of a work item and
+// adds each interval to its stage; at exit the CTA's totals go to the debug buffer (uint64[8], scripts/mma_profile.py)
+enum { PROF_SETUP, PROF_BOX, PROF_TMA, PROF_MMA, PROF_PHASEC, PROF_EPI, PROF_NSTAGES };
+#ifdef MAGNET_MMA_PROFILE
+#define MMA_STAGE(s)                                                                                                   \
+  do {                                                                                                                 \
+    if (tid == 0) {                                                                                                    \
+      const long long t_ = clock64();                                                                                  \
+      prof_s[s] += t_ - prof_s[7];                                                                                     \
+      prof_s[7] = t_;                                                                                                  \
+    }                                                                                                                  \
+  } while (0)
+#else
+#define MMA_STAGE(s) do { } while (0)
+#endif
+
 template <int MODE, bool CW>
 __global__ void __launch_bounds__(MNT, 2)
 cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CUtensorMap tm_ref,
@@ -115,10 +137,13 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
   int* bbox = reinterpret_cast<int*>(smem + MOFF_BBOX);
   float* regR = reinterpret_cast<float*>(smem + MOFF_R);
   const uint32_t bar_tma = sbase + MOFF_BAR, bar_cam = sbase + MOFF_BAR + 24;
-  float* acc_s = reinterpret_cast<float*>(smem + MOFF_ACC);
   const unsigned FULL = 0xffffffffu;
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+#ifdef MAGNET_MMA_PROFILE
+  __shared__ long long prof_s[8];
+  if (tid < 8) prof_s[tid] = tid == 7 ? clock64() : 0ll;
+#endif
   const int H = p.H, W = p.W, HW = p.HW, D = p.D, V = p.V;
   const int tiles_x = (W + MTW - 1) / MTW;
   const int items_per_b = tiles_x * ((H + MTH - 1) / MTH) * nchunks;
@@ -145,6 +170,9 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
   int cur_b = -1;
   const float xmax = (float)W + 1.0f, ymax = (float)H + 1.0f;
   const float kappa = p.kappa;
+  // window boxes from the depth-range endpoints: margin and the largest error amplification it covers (DESIGN.md §3.1)
+  constexpr float BOX_EPS = 0.015625f;
+  const float amp_max = 65536.0f / (float)(max(W, H) + 3) - 8.0f;
   const uint32_t g_row0 = sbase + MOFF_R, m_base = sbase + MOFF_META;
 
   // ---- persistent CTA: work items (batch element, tile, hypothesis chunk) are handed out dynamically -----------
@@ -171,16 +199,17 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
     *next_item = (int)gridDim.x + (int)atomicAdd(&g_mma_next[slot], 1u);   // read after the barrier that ends the item
   }
   // lanes beyond the last hypothesis of the chunk replicate it (same sample position: inside every window, no
-  // predicates); their accumulator rows are never stored
+  // predicates); their accumulators are never stored
   if (tid < MCH) ks[tid] = MODE != MAGNET_DEPTH_VOLUME ? p.k[min(jc + tid, D - 1)] : 0.0f;
-  for (int idx = tid; idx < MCH * 65; idx += MNT) acc_s[idx] = 0.0f;
   __syncthreads();
 
   // ---- per-warp constants: lane i (mod 8) holds the ray / Gaussian of pixel i of my tile row ----------------
+  // (kept in shared memory, pixr: registers are short next to the accumulators of the MMA)
   const int py = ty0 + warp;
-  float R0, R1, R2, MU = 0.f, SG = 0.f;
+  float4* pixr = reinterpret_cast<float4*>(smem + MOFF_PIXR) + warp * 16;
   unsigned livemask;
   {
+    float R0, R1, R2, MU = 0.f, SG = 0.f;
     const int px = tx0 + (lane & 7);
     const bool live = px < W && py < H;
     const int n = min(py, H - 1) * W + min(px, W - 1);     // dead pixels shadow the nearest pixel, never store
@@ -192,35 +221,115 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
       SG = ldg_f(p.ref_gmm + ((size_t)b * 2 + 1) * HW + n);
     }
     livemask = __ballot_sync(FULL, live) & 0xffu;
+    if (lane < 8) {
+      pixr[2 * lane] = make_float4(R0, R1, R2, 0.0f);
+      pixr[2 * lane + 1] = make_float4(MU, SG, 0.0f, 0.0f);
+    }
+    __syncwarp();
   }
   // my two hypotheses of every pixel of the row: (hypothesis jc + lane, hypothesis jc + 32 + lane).  Read from the
-  // depth volume they stay in registers; sampled (MAGNET.py:155: multiply, then add) or plane depths are recomputed
-  // from the pixel's Gaussian where needed (a few instructions instead of 16 registers).
-  float2 dvol[MODE == MAGNET_DEPTH_VOLUME ? MTW : 1];
-  float2 k2 = make_float2(0.f, 0.f);
-  if (MODE == MAGNET_DEPTH_VOLUME) {                       // coalesced read, transposed through shared memory
-    for (int idx = tid; idx < MCH * MPX; idx += MNT) {
-      const int j = idx >> 6, pp = idx & 63;
-      const int y = ty0 + (pp >> 3), x = tx0 + (pp & 7);
-      const size_t n = (size_t)min(y, H - 1) * W + min(x, W - 1);
-      regR[j * 65 + pp] = ldg_f(p.d_volume + ((size_t)b * D + jc + min(j, Dc - 1)) * HW + n);
+  // depth volume they stay in shared memory (pixel-major, conflict-free per pixel); sampled (MAGNET.py:155: multiply,
+  // then add) or plane depths are recomputed from the pixel's Gaussian where needed.
+  // (by 32-bit shared address: registers are short next to the accumulators of the MMA)
+  const uint32_t dvw = sbase + MOFF_DV + (uint32_t)(warp * 8 * 65 + lane) * 4u;
+  if (MODE == MAGNET_DEPTH_VOLUME) {
+    float* dv_s = reinterpret_cast<float*>(smem + MOFF_DV);                       // coalesced read, transposed through shared memory
+    // thread: pixel tid % 64, hypotheses tid / 64 + 4 r (loads in flight together, then the conflict-free stores)
+    const int pp = tid & 63, y = ty0 + (pp >> 3), x = tx0 + (pp & 7);
+    const float* dsrc = p.d_volume + ((size_t)b * D + jc) * HW + (size_t)min(y, H - 1) * W + min(x, W - 1);
+#pragma unroll 1
+    for (int j0 = tid >> 6; j0 < MCH; j0 += 32) {         // two batches of 8 loads (registers)
+      float dl[8];
+#pragma unroll
+      for (int r = 0; r < 8; ++r) dl[r] = ldg_f(dsrc + (size_t)min(j0 + 4 * r, Dc - 1) * HW);
+#pragma unroll
+      for (int r = 0; r < 8; ++r) dv_s[pp * 65 + j0 + 4 * r] = dl[r];
     }
     __syncthreads();
+    // depth range of every pixel of my row over the chunk (NaN when a depth is not finite): the window boxes
 #pragma unroll
-    for (int i = 0; i < MTW; ++i) dvol[i] = make_float2(regR[lane * 65 + warp * 8 + i], regR[(lane + 32) * 65 + warp * 8 + i]);
-    fence_proxy_async();
-    __syncthreads();
-  } else {
-    k2 = make_float2(ks[lane], ks[lane + 32]);
+    for (int i = 0; i < MTW; ++i) {
+      const float da = lds_f32(dvw + i * 260), db = lds_f32(dvw + i * 260 + 128);
+      float lo = fminf(da, db), hi = fmaxf(da, db);
+      const bool fin = __all_sync(FULL, isfinite(da) && isfinite(db));
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        lo = fminf(lo, __shfl_xor_sync(FULL, lo, o));
+        hi = fmaxf(hi, __shfl_xor_sync(FULL, hi, o));
+      }
+      if (lane == i) reinterpret_cast<float2*>(smem + MOFF_DEND)[warp * 8 + i] = fin ? make_float2(lo, hi) : make_float2(NAN, NAN);
+    }
+    __syncwarp();
   }
   // (mu, sigma) come from the warp's pixel table; the product is rounded by __fmul_rn so that it is never contracted
   // into an FMA with the add (the reference rounds twice)
   auto depth2 = [&](const int i, const float mu, const float sg) -> float2 {
-    if (MODE == MAGNET_DEPTH_VOLUME) return dvol[i];
+    if (MODE == MAGNET_DEPTH_VOLUME) return make_float2(lds_f32(dvw + i * 260), lds_f32(dvw + i * 260 + 128));
+    const float2 k2 = make_float2(ks[lane], ks[lane + 32]);
     if (MODE == MAGNET_DEPTH_PLANES) return k2;
     return fadd2_rn(make_float2(mu, mu), make_float2(__fmul_rn(sg, k2.x), __fmul_rn(sg, k2.y)));
   };
   float4* pixt = reinterpret_cast<float4*>(smem + MOFF_PIX) + warp * 16;
+
+  // ---- window box of view v: the bounding box of the cell origins of the tile's hypotheses, added into the bbox
+  // slot bb by shared atomics (complete after the next CTA barrier).  The sample position is a Moebius map of the depth,
+  // monotone on a depth interval where z keeps its sign, so the positions of a pixel's depths lie between those of its
+  // smallest and largest depth: 2 projections per pixel instead of 64, widened by BOX_EPS for the rounding of the
+  // evaluation (DESIGN.md §3.1).  A row with a pixel outside the conditions of that bound (non-finite depth range,
+  // unsorted k, z <= 0 or a large error amplification at an endpoint) projects every hypothesis instead, exactly as
+  // phase C does.
+  auto window_box = [&](const int v, int* bb) {
+    const magnet_camera* cam = cams_s + v;
+    const float a0 = cam->a[0], a1 = cam->a[1], a2 = cam->a[2];
+    const float4 ray = pixr[2 * (lane & 7)];
+    const float MU = pixr[2 * (lane & 7) + 1].x, SG = pixr[2 * (lane & 7) + 1].y;
+    const float Q0 = __fmaf_rn(cam->A[2], ray.z, __fmaf_rn(cam->A[1], ray.y, __fmul_rn(cam->A[0], ray.x)));
+    const float Q1 = __fmaf_rn(cam->A[5], ray.z, __fmaf_rn(cam->A[4], ray.y, __fmul_rn(cam->A[3], ray.x)));
+    const float Q2 = __fmaf_rn(cam->A[8], ray.z, __fmaf_rn(cam->A[7], ray.y, __fmul_rn(cam->A[6], ray.x)));
+    float2 dr;                                             // depth range of my pixel (lane & 7) over the chunk
+    if (MODE == MAGNET_DEPTH_VOLUME) {
+      const uint32_t a = sbase + MOFF_DEND + (uint32_t)(warp * 8 + (lane & 7)) * 8u;
+      dr = make_float2(lds_f32(a), lds_f32(a + 4));
+    }
+    else if (MODE == MAGNET_DEPTH_PLANES) dr = make_float2(ks[0], ks[MCH - 1]);
+    else dr = fadd2_rn(make_float2(MU, MU), make_float2(__fmul_rn(SG, ks[0]), __fmul_rn(SG, ks[MCH - 1])));
+    float2 ix, iy, z;
+    project2(dr, a0, a1, a2, Q0, Q1, Q2, ix, iy, z);
+    const float amp = fmaxf(fabsf(__fmul_rn(Q2, dr.x)) / z.x, fabsf(__fmul_rn(Q2, dr.y)) / z.y) + 2.0e-3f / fminf(z.x, z.y);
+    const bool ok = (MODE == MAGNET_DEPTH_VOLUME || p.k_sorted) && isfinite(dr.x) && isfinite(dr.y) && z.x > 0.0f &&
+                    z.y > 0.0f && amp <= amp_max && isfinite(ix.x) && isfinite(ix.y) && isfinite(iy.x) && isfinite(iy.y);
+    const bool live = (livemask >> (lane & 7)) & 1u;
+    float xl = 1e9f, xh = -1e9f, yl = 1e9f, yh = -1e9f;
+    if (__all_sync(FULL, ok || !live)) {                   // warp-uniform
+      if (live) {
+        xl = clamp_coord(__fsub_rn(fminf(ix.x, ix.y), BOX_EPS), xmax); xh = clamp_coord(__fadd_rn(fmaxf(ix.x, ix.y), BOX_EPS), xmax);
+        yl = clamp_coord(__fsub_rn(fminf(iy.x, iy.y), BOX_EPS), ymax); yh = clamp_coord(__fadd_rn(fmaxf(iy.x, iy.y), BOX_EPS), ymax);
+      }
+    } else {
+#ifdef MAGNET_MMA_DEBUG
+      if (dbg != nullptr && lane == 0) atomicAdd(reinterpret_cast<unsigned*>(dbg + MMA_DBG_OUTSIDE + 1), 1u);   // exact rows
+#endif
+#pragma unroll
+      for (int i = 0; i < MTW; ++i) {
+        const float q0 = __shfl_sync(FULL, Q0, i), q1 = __shfl_sync(FULL, Q1, i), q2 = __shfl_sync(FULL, Q2, i);
+        const float mu = __shfl_sync(FULL, MU, i), sg = __shfl_sync(FULL, SG, i);
+        project2(depth2(i, mu, sg), a0, a1, a2, q0, q1, q2, ix, iy, z);
+        ix.x = clamp_coord(ix.x, xmax); ix.y = clamp_coord(ix.y, xmax);
+        iy.x = clamp_coord(iy.x, ymax); iy.y = clamp_coord(iy.y, ymax);
+        if ((livemask >> i) & 1u) {                        // warp-uniform
+          xl = fminf(xl, fminf(ix.x, ix.y)); xh = fmaxf(xh, fmaxf(ix.x, ix.y));
+          yl = fminf(yl, fminf(iy.x, iy.y)); yh = fmaxf(yh, fmaxf(iy.x, iy.y));
+        }
+      }
+    }
+    const int r0 = __reduce_min_sync(FULL, (int)floorf(xl)), r1 = __reduce_max_sync(FULL, (int)floorf(xh));
+    const int r2 = __reduce_min_sync(FULL, (int)floorf(yl)), r3 = __reduce_max_sync(FULL, (int)floorf(yh));
+    if (lane == 0) { atomicMin(bb + 0, r0); atomicMax(bb + 1, r1); atomicMin(bb + 2, r2); atomicMax(bb + 3, r3); }
+  };
+  auto next_valid = [&](int v) {                           // CTA-uniform
+    while (v < V && cams_s[v].valid != 1.0f) ++v;          // V <= MMAXV is checked on the host
+    return v;
+  };
 
   if (b != cur_b) {                                        // CTA-uniform: camera table landed
     mbar_wait_or_trap(bar_cam, ph_cam);
@@ -228,19 +337,26 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
     cur_b = b;
   }
   bool first = true;                                       // the first window also waits for the reference tile
+  float2 accr[MTW];                                        // view accumulators of (hypotheses lane, lane + 32) x pixel
+#pragma unroll
+  for (int i = 0; i < MTW; ++i) accr[i] = make_float2(0.0f, 0.0f);
+  MMA_STAGE(PROF_SETUP);
+  int v = next_valid(0);
+  if (v < V) window_box(v, bbox + (it & 1) * 4);
+  __syncthreads();                                         // box of the first view complete
+  MMA_STAGE(PROF_BOX);
 
-  for (int v = 0; v < V; ++v) {
-    const magnet_camera* cam = cams_s + v;                 // V <= MMAXV is checked on the host
-    if (cam->valid != 1.0f) continue;                      // CTA-uniform
-    const float a0 = cam->a[0], a1 = cam->a[1], a2 = cam->a[2];
-    // (K R) ray of the pixel this lane holds (lane & 7); the pixel loop below broadcasts it
-    const float Q0 = __fmaf_rn(cam->A[2], R2, __fmaf_rn(cam->A[1], R1, __fmul_rn(cam->A[0], R0)));
-    const float Q1 = __fmaf_rn(cam->A[5], R2, __fmaf_rn(cam->A[4], R1, __fmul_rn(cam->A[3], R0)));
-    const float Q2 = __fmaf_rn(cam->A[8], R2, __fmaf_rn(cam->A[7], R1, __fmul_rn(cam->A[6], R0)));
+  while (v < V) {
+    const int vn = next_valid(v + 1);
     __syncwarp();                                          // the previous view's readers are done
-    if (lane < 8) {
-      pixt[2 * lane] = make_float4(Q0, Q1, Q2, 0.0f);
-      pixt[2 * lane + 1] = make_float4(Q2, MU, SG, 0.0f);
+    if (lane < 8) {                                        // (K R) ray of pixel `lane` of the row and the view's a
+      const magnet_camera* cam = cams_s + v;
+      const float4 ray = pixr[2 * lane], ms = pixr[2 * lane + 1];
+      const float Q0 = __fmaf_rn(cam->A[2], ray.z, __fmaf_rn(cam->A[1], ray.y, __fmul_rn(cam->A[0], ray.x)));
+      const float Q1 = __fmaf_rn(cam->A[5], ray.z, __fmaf_rn(cam->A[4], ray.y, __fmul_rn(cam->A[3], ray.x)));
+      const float Q2 = __fmaf_rn(cam->A[8], ray.z, __fmaf_rn(cam->A[7], ray.y, __fmul_rn(cam->A[6], ray.x)));
+      pixt[2 * lane] = make_float4(Q0, Q1, Q2, cam->a[0]);
+      pixt[2 * lane + 1] = make_float4(cam->a[1], ms.x, ms.y, cam->a[2]);
     }
     __syncwarp();
     const int vb = v * p.B + b;
@@ -249,31 +365,13 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
     // "out of bounds"; z = depth in the source camera
     auto project_px = [&](const int i, float2& ix, float2& iy, float2& z) {
       const float4 t1 = pixt[2 * i], t2 = pixt[2 * i + 1];   // same address on every lane: broadcast
-      project2(depth2(i, t2.y, t2.z), a0, a1, a2, t1.x, t1.y, t1.z, ix, iy, z);
+      project2(depth2(i, t2.y, t2.z), t1.w, t2.x, t2.w, t1.x, t1.y, t1.z, ix, iy, z);
       ix.x = clamp_coord(ix.x, xmax); ix.y = clamp_coord(ix.y, xmax);
       iy.x = clamp_coord(iy.x, ymax); iy.y = clamp_coord(iy.y, ymax);
     };
 
-    // ---------------- projection of every hypothesis, bounding box of the tile's sample positions -------------
-    // (phase C projects again from the pixel table: holding the 32 positions across the MMA would not fit the registers)
-    float xl = 1e9f, xh = -1e9f, yl = 1e9f, yh = -1e9f;
-#pragma unroll
-    for (int i = 0; i < MTW; ++i) {
-      float2 ix, iy, z;
-      project_px(i, ix, iy, z);
-      if ((livemask >> i) & 1u) {                          // warp-uniform
-        xl = fminf(xl, fminf(ix.x, ix.y)); xh = fmaxf(xh, fmaxf(ix.x, ix.y));
-        yl = fminf(yl, fminf(iy.x, iy.y)); yh = fmaxf(yh, fmaxf(iy.x, iy.y));
-      }
-    }
-    int* bb = bbox + (it & 1) * 4;
-    {
-      const int r0 = __reduce_min_sync(FULL, (int)floorf(xl)), r1 = __reduce_max_sync(FULL, (int)floorf(xh));
-      const int r2 = __reduce_min_sync(FULL, (int)floorf(yl)), r3 = __reduce_max_sync(FULL, (int)floorf(yh));
-      if (lane == 0) { atomicMin(bb + 0, r0); atomicMax(bb + 1, r1); atomicMin(bb + 2, r2); atomicMax(bb + 3, r3); }
-    }
-    fence_proxy_async();
-    __syncthreads();                                       // box complete; region R is free (phase C of the last pass)
+    // the box of this view was completed by the barrier that ended the previous pass (or the item set-up)
+    const int* bb = bbox + (it & 1) * 4;
     const int wx0 = bb[0], wx1 = bb[1], wy0 = bb[2], wy1 = bb[3];
     if (tid < 4) bbox[((it + 1) & 1) * 4 + tid] = (tid & 1) ? -(1 << 28) : (1 << 28);   // re-arm the other slot
     ++it;
@@ -306,6 +404,7 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
         const int gp = ((npad + 23) & ~31) + 8;            // row pitch of G in floats: >= npad, % 32 == 8
         mbar_wait_or_trap(bar_tma, ph_tma);                // every thread observes the copies (it reads the table)
         ph_tma ^= 1u;
+        MMA_STAGE(PROF_TMA);
         // ---------------- G = ref x window^T: warpgroup g computes columns [128 g, 128 g + 128) -----------------
         // (3 products x 4 K steps of m64n128k16; the whole fence .. wait sequence sits inside the warpgroup-uniform
         // branch, so ptxas keeps the wgmma pipelined)
@@ -342,6 +441,7 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
           }
           __syncthreads();
         }
+        MMA_STAGE(PROF_MMA);
 #ifdef MAGNET_MMA_DEBUG
         if (dbg != nullptr && item == 0 && v == 0 && sy == wy0 && sx == wx0) {
           if (tid == 0) {
@@ -351,6 +451,9 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
           for (int idx = tid; idx < MPX * npad; idx += MNT) dbg[16 + (idx / npad) * 256 + idx % npad] = regR[(idx / npad) * gp + idx % npad];
         }
 #endif
+        // the next view's box, ahead of this phase C: its copies are issued right after the barrier that ends it
+        if (sy == wy0 && sx == wx0 && vn < V) window_box(vn, bbox + (it & 1) * 4);
+        MMA_STAGE(PROF_BOX);
         // ---------------- per hypothesis: 4 G reads, 4 table reads, 3 bilinear interpolations -------------------
         // byte offset of cell (x0, y0) in a G row = 4 * ((y0 - sy) * pitch + (x0 - sx)), evaluated in fp32 (small
         // integers, exact) on top of 1.5 * 2^23 so that the integer sits in the mantissa
@@ -364,7 +467,7 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
           const float c0f = MAGIC - 4.0f * sxf - pitch4f * syf;   // exact: integers below 2^24
           const uint32_t pitch4 = (uint32_t)nseg * 32u;
           uint32_t rowaddr = g_row0 + (uint32_t)(warp * 8 * gp) * 4u;
-          float* accp = acc_s + lane * 65 + warp * 8;
+          const uint32_t cmax = pitch4 * (uint32_t)(rows - 1) - 8u;   // last cell origin of the window (bytes)
 #pragma unroll
           for (int i = 0; i < MTW; ++i, rowaddr += (uint32_t)gp * 4u) {
             if (!((livemask >> i) & 1u)) continue;         // warp-uniform
@@ -384,7 +487,18 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
               pb = x0.y >= sxf && x0.y < xend && y0.y >= syf && y0.y < yend;
               ca = pa ? ca : 0u;                           // the others read cell 0
               cb = pb ? cb : 0u;
+            } else {                                       // a wrong box can never address outside the window
+              ca = min(ca, cmax);
+              cb = min(cb, cmax);
             }
+#ifdef MAGNET_MMA_DEBUG
+            if (dbg != nullptr && sy == wy0 && sx == wx0) {  // hypotheses whose cell origin fell outside the box
+              const bool outa = lane < Dc && (x0.x < (float)wx0 || x0.x > (float)wx1 || y0.x < (float)wy0 || y0.x > (float)wy1);
+              const bool outb = lane + 32 < Dc && (x0.y < (float)wx0 || x0.y > (float)wx1 || y0.y < (float)wy0 || y0.y > (float)wy1);
+              const unsigned nout = __popc(__ballot_sync(FULL, outa)) + __popc(__ballot_sync(FULL, outb));
+              if (lane == 0 && nout != 0u) atomicAdd(reinterpret_cast<unsigned*>(dbg + MMA_DBG_OUTSIDE), nout);
+            }
+#endif
             const uint32_t ga = rowaddr + ca, gb = rowaddr + cb;
             const float2 g00 = make_float2(lds_f32(ga), lds_f32(gb)), g01 = make_float2(lds_f32(ga + 4), lds_f32(gb + 4));
             const float2 g10 = make_float2(lds_f32(ga + pitch4), lds_f32(gb + pitch4));
@@ -404,17 +518,18 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
               oka = fabsf(costa) < 3.0e38f;
               okb = fabsf(costb) < 3.0e38f;
             }
-            // the accumulator of (hypothesis, pixel) is touched by this lane only
-            if (pa && oka) accp[i] += costa;
-            if (pb && okb) accp[32 * 65 + i] += costb;
+            if (pa && oka) accr[i].x += costa;
+            if (pb && okb) accr[i].y += costb;
           }
         };
         if (single) phase_c(std::true_type{});
         else phase_c(std::false_type{});
         fence_proxy_async();
         __syncthreads();                                   // G / table dead: the next copies and MMAs may overwrite
+        MMA_STAGE(PROF_PHASEC);
       }
     }
+    v = vn;
   }
 
   if (first) {                                             // no valid view: the reference-tile copy is still in flight
@@ -425,6 +540,21 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
 
   // -------- epilogue: undo the split scales, 1/V mean over ALL views (homography.py:120), coalesced store --------
   {
+    // the accumulators go through region R (free: the last pass ended with a CTA barrier), hypothesis-major
+    float* acc_s = regR;
+    // the item's coordinates, decoded again: not kept in registers across the views
+    const int b = item / items_per_b;
+    const int rem = item - b * items_per_b;
+    const int tile = rem / nchunks;
+    const int jc = (rem - tile * nchunks) * MCH;
+    const int Dc = min(MCH, D - jc);
+    const int tx0 = (tile % tiles_x) * MTW, ty0 = (tile / tiles_x) * MTH;
+#pragma unroll
+    for (int i = 0; i < MTW; ++i) {
+      acc_s[lane * 65 + warp * 8 + i] = accr[i].x;
+      acc_s[(lane + 32) * 65 + warp * 8 + i] = accr[i].y;
+    }
+    __syncthreads();
     const float inv = hdr_ref->inv_scale * hdr_src->inv_scale;   // powers of two: exact
     const bool exact = p.inv_v_exact != 0.0f;              // V a power of two: the division is an exact scaling
     auto fin = [&](float a) { a *= inv; return exact ? a * p.inv_v_exact : __fdiv_rn(a, p.vf); };
@@ -447,10 +577,19 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
     }
   }
   const int nxt = *next_item;                              // written by thread 0 when this item began
+  fence_proxy_async();                                     // region R is overwritten by the next item's copies
   __syncthreads();                                         // accumulators and tables are free; next_item may be rewritten
+  MMA_STAGE(PROF_EPI);
   item = nxt;
   }  // work items
 
+#ifdef MAGNET_MMA_PROFILE
+  if (tid == 0 && dbg != nullptr) {
+    unsigned long long* tot = reinterpret_cast<unsigned long long*>(dbg);
+    for (int s = 0; s < PROF_NSTAGES; ++s) atomicAdd(tot + s, (unsigned long long)prof_s[s]);
+    atomicAdd(tot + 7, 1ull);                              // CTAs
+  }
+#endif
   if (tid == 0) {                                          // the last CTA to finish re-arms the work counter
     __threadfence();
     if (atomicAdd(&g_mma_done[slot], 1u) == gridDim.x - 1) {
@@ -641,7 +780,7 @@ static cudaError_t make_meta_map(CUtensorMap* tm, const void* meta, int N, int H
   return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
-#ifdef MAGNET_MMA_DEBUG
+#if defined(MAGNET_MMA_DEBUG) || defined(MAGNET_MMA_PROFILE)
 static float* g_mma_dbg = nullptr;
 void mma_set_debug_buffer(float* p) { g_mma_dbg = p; }
 #endif
@@ -680,7 +819,7 @@ static cudaError_t launch_mma_mw(const CostParams& p, cudaStream_t st) {
                                                         : (int)(ticket.fetch_add(1) % (MMA_SLOTS / 2));
   dim3 grid(std::min(n_items, 2 * sm_count(dev))), block(MNT);   // persistent: two CTAs per SM
   float* dbg = nullptr;
-#ifdef MAGNET_MMA_DEBUG
+#if defined(MAGNET_MMA_DEBUG) || defined(MAGNET_MMA_PROFILE)
   dbg = g_mma_dbg;
 #endif
   kern<<<grid, block, M_SMEM_TOTAL, st>>>(p, tm_ref, tm_src, tm_meta, nchunks, n_items, slot, dbg);
