@@ -120,10 +120,12 @@ cost_cw_bwd_kernel(const __grid_constant__ CwBwdParams p, const int C) {
       i10 = x0 >= 0 && x0 < W && y1 >= 0 && y1 < H; i11 = x1 >= 0 && x1 < W && y1 >= 0 && y1 < H;
       o00 = y0 * W + x0;
       const int o01 = o00 + 1, o10 = o00 + W, o11 = o10 + 1;
-      m00 = i00 ? ldg_f(gm + o00) : 0.f; s00 = i00 ? ldg_f(gm + HW + o00) : 0.f;
-      m01 = i01 ? ldg_f(gm + o01) : 0.f; s01 = i01 ? ldg_f(gm + HW + o01) : 0.f;
-      m10 = i10 ? ldg_f(gm + o10) : 0.f; s10 = i10 ? ldg_f(gm + HW + o10) : 0.f;
-      m11 = i11 ? ldg_f(gm + o11) : 0.f; s11 = i11 ? ldg_f(gm + HW + o11) : 0.f;
+      if (p.cw) {                                         // without consistency src_gmm may be NULL (the C ABI allows it)
+        m00 = i00 ? ldg_f(gm + o00) : 0.f; s00 = i00 ? ldg_f(gm + HW + o00) : 0.f;
+        m01 = i01 ? ldg_f(gm + o01) : 0.f; s01 = i01 ? ldg_f(gm + HW + o01) : 0.f;
+        m10 = i10 ? ldg_f(gm + o10) : 0.f; s10 = i10 ? ldg_f(gm + HW + o10) : 0.f;
+        m11 = i11 ? ldg_f(gm + o11) : 0.f; s11 = i11 ? ldg_f(gm + HW + o11) : 0.f;
+      }
       f00 = f01 = f10 = f11 = 0.f;
       if (need_d && (i00 | i01 | i10 | i11)) {
 #pragma unroll

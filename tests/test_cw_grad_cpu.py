@@ -71,6 +71,105 @@ def test_numpy_depth_gradient_matches_autograd_float64():
     assert err < 1e-9, err
 
 
+def _within(got, want, bound, rel, what):
+    err = np.abs(np.asarray(got, np.float64) - np.asarray(want, np.float64))
+    bad = err > rel * bound
+    assert not bad.any(), (what, int(bad.sum()), float(np.max(err / np.maximum(bound, 1e-300))))
+    assert np.abs(want).max() > 0, what
+
+
+def _f64_autograd(fn, leaves, gout):
+    default = torch.get_default_dtype()
+    torch.set_default_dtype(torch.float64)                  # the port's temporaries (grid, accumulators) in float64
+    try:
+        out = fn(*leaves)
+    finally:
+        torch.set_default_dtype(default)
+    (out * gout).sum().backward()
+    return out.detach().numpy(), [x.grad.numpy() for x in leaves]
+
+
+@pytest.mark.parametrize("C_", [1, 3, 8, 13])
+def test_float64_reference_matches_autograd(C_):
+    """tests/cw_grad_ref.Reference with float64 positions against float64 autograd of the ATen port: every output of
+    the CW volume (VOLUME and GAUSS depths, consistency on and off) and of the F volume (softmax on and off), within
+    1e-12 of each element's bound, after the upstream gradient was zeroed at the (rare) hypotheses that sit on a mask
+    flip, a cell edge or z ~ 0.  The inputs reach the +-10 clamp, taps outside the image, samples with every tap
+    outside, depths behind the source camera and an invalid view."""
+    from magnet_b200.synthetic import make_inputs
+    from tests.cw_grad_ref import Reference, cameras_f64, gauss_chain, softmax_score_grad
+    inp = make_inputs(B=2, V=3, D=6, H=10, W=14, C=C_, seed=17 + C_, depth="random", invalid=[(0, 1)])
+    B, V, H, W = 2, 3, 10, 14
+    f64 = {k: v.double() for k, v in inp.cam_intrins.items()}
+    R, t = inp.R.double(), inp.t.double()
+    cams = cameras_f64(f64['intM'].numpy(), R.numpy(), t.numpy(), inp.is_valid.numpy())
+    rays = f64['unit_ray_array_2D'].numpy()
+    ref, src, sgmm = inp.ref_feat.double(), inp.nghbr_feat.double(), inp.nghbr_gmms.double()
+    rng = np.random.default_rng(C_)
+    k = [-40.0, -9.0, -2.0, 0.0, 1.5, 4.0]                  # GAUSS: behind the camera, near z = 0, the clamp
+    dv = inp.depth_volume().double().numpy().copy()
+    dv[:, 0] = -dv[:, 0]
+    dv[:, 1] *= 0.02
+    assert int(inp.is_valid.min()) == 0
+    for mode in ("volume", "gauss"):
+        gmm = inp.ref_gmms.double().numpy()
+        depth = dv if mode == "volume" else gmm[:, 0:1] + gmm[:, 1:2] * np.asarray(k).reshape(1, -1, 1, 1)
+        for cw in (True, False):
+            thres = inp.thres if cw else 1e30
+            rf = Reference(depth, ref.numpy(), src.numpy(), sgmm.numpy(), cams, rays, float(thres), pos="f64",
+                           consistency=cw)
+            amb = rf.ambiguous(1e-9, 1e-9)
+            keep = ~amb
+            for name in ("clamped", "tap_outside", "all_outside", "behind"):
+                assert (rf.reached[name].reshape(amb.shape) & keep).any(), (mode, cw, name)
+            assert amb.mean() < 0.05, amb.mean()
+            gout = np.where(amb, 0.0, rng.standard_normal(amb.shape))
+            want_out, want_b, _, _ = rf.forward()
+            g = rf.backward(gout / V)
+            lf = [torch.from_numpy(depth).requires_grad_(True) if mode == "volume"
+                  else torch.from_numpy(gmm).requires_grad_(True),
+                  ref.clone().requires_grad_(True), src.clone().requires_grad_(True)]
+
+            def fn(d_or_gmm, r, s):
+                d = d_or_gmm if mode == "volume" else torch.cat([d_or_gmm[:, 0:1] + d_or_gmm[:, 1:2] * kj for kj in k], 1)
+                return torch_ref.cost_volume_cw(d, r, s, None, sgmm, R, t, inp.is_valid, f64, thres)
+            out, (gd, gr, gs) = _f64_autograd(fn, lf, torch.from_numpy(gout))
+            tag = f"{mode} cw={cw}"
+            flip = (rf.margin <= 1e-9).reshape(amb.shape)
+            _within(np.where(flip, 0, out), np.where(flip, 0, want_out), want_b, 1e-12, tag + " out")
+            _within(gr, g["ref"], g["ref_b"], 1e-12, tag + " ref")
+            _within(gs, g["src"], g["src_b"], 1e-12, tag + " src")
+            if mode == "volume":
+                _within(gd, g["d"], g["d_b"], 1e-12, tag + " depth")
+            else:
+                val, bnd = gauss_chain(g["d"], g["d_b"], k)
+                _within(gd, val, bnd, 1e-12, tag + " (mu, sigma)")
+    planes = np.array([0.002, 0.05, 0.5, 1.5, 3.0, 8.0])        # the smallest planes reach the clamp
+    depth = np.broadcast_to(planes.reshape(1, -1, 1, 1), (B, 6, H, W))
+    rf = Reference(depth, ref.numpy(), src.numpy(), None, cams, rays, 0.0, pos="f64", consistency=False)
+    for name in ("clamped", "tap_outside", "all_outside"):
+        assert rf.reached[name].any(), name
+    amb = rf.ambiguous(1e-9, 1e-9)
+    score, score_b, _, _ = rf.forward()
+    for softmax in (True, False):
+        gout = np.where(amb, 0.0, rng.standard_normal(amb.shape))
+        out, (gr, gs) = _f64_autograd(
+            lambda r, s: torch_ref.cost_volume_f(torch.from_numpy(planes).view(1, -1, 1, 1), r, s, R, t, inp.is_valid,
+                                                 f64, apply_softmax=softmax),
+            [ref.clone().requires_grad_(True), src.clone().requires_grad_(True)], torch.from_numpy(gout))
+        if softmax:
+            e = np.exp(score - score.max(1, keepdims=True))
+            prob = e / e.sum(1, keepdims=True)
+            _within(out, prob, prob * (1 + score_b), 1e-12, "F prob")
+            gsc, gsc_b = softmax_score_grad(prob, gout, V)
+        else:
+            _within(out, score, score_b, 1e-12, "F score")
+            gsc, gsc_b = gout / V, np.abs(gout) / V
+        g = rf.backward(gsc, gsc_b)
+        _within(gr, g["ref"], g["ref_b"], 1e-12, f"F softmax={softmax} ref")
+        _within(gs, g["src"], g["src_b"], 1e-12, f"F softmax={softmax} src")
+
+
 def _args(L, *, C_=64, V=2, D=8, layout=_lib.SRC_NCHW, variant=_lib.VARIANT_DIRECT, mode=_lib.DEPTH_VOLUME,
           null=(), softmax=0, consistency=1):
     buf = (C.c_float * 64)()
