@@ -24,12 +24,13 @@
 //     64-hypothesis chunk, evaluated side by side as float2 pairs): the pixel's constants are warp-uniform (per-warp table
 //     in shared memory), the 32 lanes read a handful of neighbouring cells of ONE accumulator row (broadcast /
 //     conflict-free); lanes beyond the last hypothesis replicate it, so there are no activity predicates.
-//   * per view: TMA window + paired (mu, sigma) table -> 12 x wgmma m64n128k16 per warpgroup (3 products x 4 K steps)
-//     -> the 64 accumulator rows into shared memory (over the window, which is dead by then) -> the NEXT view's window
-//     box (projections of each pixel's smallest and largest depth, window_box) -> per-hypothesis phase, which projects
-//     from the per-warp pixel table.  The box is complete at the barrier that ends the phase, so the next view's copies
-//     are issued right after it.  The 16 view accumulators of a lane stay in registers; the epilogue transposes them
-//     through region R into the hypothesis-major layout of the coalesced stores.
+//   * per view: TMA window + paired (mu, sigma) table, and while the copies land the NEXT view's window box
+//     (projections of each pixel's smallest and largest depth, window_box) -> 12 wgmma per warpgroup (3 products x 4 K
+//     steps; m64n128k16, or m64n64k16 for warpgroup 1 when the window ends below column 192) -> the 64 accumulator rows
+//     into shared memory (over the window, which is dead by then) -> per-hypothesis phase, which projects from the
+//     per-warp pixel table.  The box is complete at the barrier that ends the phase, so the next view's copies are issued
+//     right after it.  The 16 view accumulators of a lane stay in registers; the epilogue transposes them through
+//     region R into the hypothesis-major layout of the coalesced stores.
 //   * a window that does not fit 256 cells is cut into sub-windows of <= 32 segments that overlap by one cell column /
 //     row; a hypothesis is evaluated in the sub-window that holds its cell origin.  Same code for any depth distribution.
 //   * persistent CTAs (two per SM): work items (batch element, tile, 64-hypothesis chunk) come from a global counter in a
@@ -373,7 +374,6 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
     // the box of this view was completed by the barrier that ended the previous pass (or the item set-up)
     const int* bb = bbox + (it & 1) * 4;
     const int wx0 = bb[0], wx1 = bb[1], wy0 = bb[2], wy1 = bb[3];
-    if (tid < 4) bbox[((it + 1) & 1) * 4 + tid] = (tid & 1) ? -(1 << 28) : (1 << 28);   // re-arm the other slot
     ++it;
     // The cell origins span [wx0, wx1] x [wy0, wy1].  One pass when the window (origins + right / lower taps, cut into
     // 8-cell segments) fits MSEG segments, else sub-windows of <= MSEG segments that overlap by one cell column / row;
@@ -400,14 +400,19 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
           }
         }
         __syncwarp();
+        // the next view's box while the copies land: it reads only the camera and pixel tables, and it is complete at
+        // the barrier that ends this view's last phase C, right before the next view's copies are issued
+        const bool first_pass = sy == wy0 && sx == wx0;    // CTA-uniform
+        if (first_pass && vn < V) window_box(vn, bbox + (it & 1) * 4);
         const int npad = (nsegs * 8 + 15) & ~15;           // accumulator columns (N % 16 == 0)
         const int gp = ((npad + 23) & ~31) + 8;            // row pitch of G in floats: >= npad, % 32 == 8
         mbar_wait_or_trap(bar_tma, ph_tma);                // every thread observes the copies (it reads the table)
         ph_tma ^= 1u;
         MMA_STAGE(PROF_TMA);
         // ---------------- G = ref x window^T: warpgroup g computes columns [128 g, 128 g + 128) -----------------
-        // (3 products x 4 K steps of m64n128k16; the whole fence .. wait sequence sits inside the warpgroup-uniform
-        // branch, so ptxas keeps the wgmma pipelined)
+        // (3 products x 4 K steps; warpgroup 0 issues m64n128k16, warpgroup 1 the narrowest of n128 / n64 / nothing
+        // that covers npad - 128.  Each shape's whole fence .. wait sequence sits inside its own warpgroup-uniform
+        // branch, so ptxas keeps the wgmma pipelined.)
         {
           const int wg = warp >> 2;
           float acc[64];
@@ -417,7 +422,10 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
           const uint64_t a_hi = gmma_desc_sw128(sbase + MOFF_A, 1024), a_lo = gmma_desc_sw128(sbase + MOFF_A + 8192, 1024);
           const uint64_t b_hi = gmma_desc_sw128(bseg, SEG_BYTES), b_lo = gmma_desc_sw128(bseg + 1024, SEG_BYTES);
           __syncwarp();                                      // wgmma is warp-synchronous (.aligned)
-          if (wg == 0 || npad > 128) {                       // CTA-uniform: warpgroup 1 idles on a narrow window
+          // ptxas (CUDA 12.9) serialises the wgmma of <GAUSS, false> when it holds the second shape (C7511, out of
+          // registers), so that instantiation keeps n128 for warpgroup 1
+          constexpr bool WG1_N64 = CW || MODE != MAGNET_DEPTH_GAUSS;
+          if (wg == 0 || npad > (WG1_N64 ? 192 : 128)) {     // warpgroup-uniform: N = 128
             wgmma_fence();
 #pragma unroll
             for (int pr = 0; pr < 3; ++pr) {                // small cross terms first
@@ -427,8 +435,22 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
             }
             wgmma_commit();
             wgmma_wait_all();
-          }
-          __syncthreads();                                   // both warpgroups have read the window: G may overwrite it
+          } else if (WG1_N64 && npad > 128) {                // warpgroup 1, columns [128, 192): N = 64
+            float (&acc64)[32] = *reinterpret_cast<float (*)[32]>(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int pr = 0; pr < 3; ++pr) {
+              const uint64_t ad = pr == 0 ? a_lo : a_hi, bd = pr == 1 ? b_lo : b_hi;
+#pragma unroll
+              for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_f16(acc64, ad + 2u * kk, bd + 2u * kk, (pr | kk) != 0);
+            }
+            wgmma_commit();
+            wgmma_wait_all();
+          }                                                  // (else warpgroup 1 idles on a narrow window)
+          __syncthreads();                                   // both warpgroups have read the window: G may overwrite it;
+                                                             // every thread has read this view's box
+          // re-arm the box slot this view was read from: the view after next adds its box into it
+          if (tid == 0 && first_pass) *reinterpret_cast<int4*>(bbox + ((it + 1) & 1) * 4) = make_int4(1 << 28, -(1 << 28), 1 << 28, -(1 << 28));
           // accumulator fragment -> G rows (pixels) x columns (cells); gp % 32 == 8 keeps the 8-byte stores conflict-free
           const int r0 = ((warp & 3) << 4) + (lane >> 2);
           float* g0 = regR + (size_t)r0 * gp + wg * 128 + 2 * (lane & 3);
@@ -451,9 +473,6 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
           for (int idx = tid; idx < MPX * npad; idx += MNT) dbg[16 + (idx / npad) * 256 + idx % npad] = regR[(idx / npad) * gp + idx % npad];
         }
 #endif
-        // the next view's box, ahead of this phase C: its copies are issued right after the barrier that ends it
-        if (sy == wy0 && sx == wx0 && vn < V) window_box(vn, bbox + (it & 1) * 4);
-        MMA_STAGE(PROF_BOX);
         // ---------------- per hypothesis: 4 G reads, 4 table reads, 3 bilinear interpolations -------------------
         // byte offset of cell (x0, y0) in a G row = 4 * ((y0 - sy) * pitch + (x0 - sx)), evaluated in fp32 (small
         // integers, exact) on top of 1.5 * 2^23 so that the integer sits in the mantissa

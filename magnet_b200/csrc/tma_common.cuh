@@ -109,6 +109,16 @@ __device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t ad
       : "memory");
 }
 
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, both K-major: the narrow form of m64n128k16 (fragment as there, j < 8)
+__device__ __forceinline__ void wgmma_m64n64k16_f16(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
+      : "memory");
+}
+
 // D[64 x 64] += A[64 x 16] * B[16 x 64] with either operand K-major (TA / TB = 0) or MN-major (= 1, the transposed
 // form: rows of the 128-byte-swizzle atom are K indices holding 64 contiguous M / N elements; the descriptor's stride
 // byte offset is then the distance between consecutive 8-row K groups).  Accumulator fragment as m64n128k16, j < 8.

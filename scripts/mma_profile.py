@@ -28,7 +28,9 @@ from magnet_b200.synthetic import make_config              # noqa: E402
 L = _lib.lib()
 if not hasattr(L, "magnet_mma_debug_buffer"):
     sys.exit(f"{LIBFILE} is not a MAGNET_MMA_PROFILE build")
-STAGES = ["item setup", "box", "TMA wait", "MMA + G", "phase C", "epilogue + fetch"]
+# "box" is the first view's box of an item; the boxes of the other views are computed while a view's copies land, so
+# they count in "TMA wait + box"
+STAGES = ["item setup", "box", "TMA wait + box", "MMA + G", "phase C", "epilogue + fetch"]
 try:
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
                        capture_output=True, text=True).stdout.strip()
