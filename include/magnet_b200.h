@@ -293,6 +293,35 @@ int magnet_fnet_l1_bwd_f32(const float* scores, const float* planes_host, const 
                            float scale, const float* grad_scale, int32_t B, int32_t D, int32_t H, int32_t W,
                            float* grad_scores, void* stream);
 
+/*
+ * Depth evaluation — replaces the metric block of validate() (test_MaGNet.py:52-79, train_MaGNet.py:153-180) with
+ * utils.compute_depth_errors (utils/utils.py:106-144), for every image of the batch and up to MAGNET_METRICS_MAX_PRED
+ * predictions that share the GT (e.g. every prediction of pred_list).  Per image: gt > max_depth -> 0;
+ * valid = min_depth < gt < max_depth inside the evaluation box; mu clamped to [min_depth, max_depth], inf -> max,
+ * NaN -> min; var = max(sigma^2, 1e-6); per-pixel terms in float32, sums and the NLL in float64 (DESIGN §3.6).
+ * Two forms: k == 0, pred[p] is the full-resolution (B,2,H,W) [mu, sigma]; k >= 1, pred[p] is the quarter-resolution
+ * (B,2,H/k,W/k) [mu, sigma] and up_mask (B,9*k*k,H/k,W/k) the upsampling mask (upsample_depth_via_mask fused in, the
+ * full-resolution prediction is never written).
+ * out (P,B,13) float64: n, then a1 a2 a3 abs_diff abs_rel sq_rel rmse log_10 irmse rmse_log silog nll (NaN when n == 0).
+ * Two kernels, no atomics: results are bit-identical from run to run.
+ */
+#define MAGNET_METRICS_MAX_PRED 8
+#define MAGNET_METRICS_COLS 13
+typedef struct magnet_depth_metrics_args {
+  int32_t P, B, H, W;             /* predictions (1..MAGNET_METRICS_MAX_PRED), images, full-resolution GT size      */
+  int32_t k;                      /* 0: full-resolution predictions; >= 1: upsampling factor (H % k == W % k == 0)  */
+  int32_t row0, row1, col0, col1; /* evaluation box [row0,row1) x [col0,col1) (no crop: 0, H, 0, W)                 */
+  float min_depth, max_depth;     /* compared in float32                                                            */
+  const float* const* pred;       /* HOST array of P DEVICE pointers, each (B,2,H,W) or (B,2,H/k,W/k)               */
+  const float* up_mask;           /* (B,9*k*k,H/k,W/k) when k >= 1, else ignored                                    */
+  const float* gt;                /* (B,1,H,W) raw GT (values above max_depth are treated as 0)                     */
+  double* workspace;              /* magnet_depth_metrics_workspace(args) doubles of scratch                        */
+  double* out;                    /* (P,B,MAGNET_METRICS_COLS)                                                      */
+} magnet_depth_metrics_args;
+/* Doubles of workspace the call needs (shape fields and box of args only), or a negative magnet_status. */
+int64_t magnet_depth_metrics_workspace(const magnet_depth_metrics_args* args);
+int magnet_depth_metrics_f32(const magnet_depth_metrics_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -2,14 +2,18 @@
 
 Only the hot path of SURVEY §8: depth-candidate sampler, plane-sweep warp + bilinear feature
 sampling + depth-consistency weighting + view fusion (one fused sm_90a kernel), Gaussian update,
-and their reference-facing wrappers.  The CUDA library is mandatory; there is no CPU fallback.
+their reference-facing wrappers, and the depth evaluation of validate() (``DepthMetrics``).
+The CUDA library is mandatory; there is no CPU fallback.
 """
 from . import _lib
 from .sampling import depth_sampling, k_offsets_f32
 from .homography import est_costvolume_CW, est_costvolume_F, clear_cache, prep_cache
 from .matcher import GNET, MAGNET, MagnetF, MagnetHead, MatchingPlan, matching_loop, install, sid_planes
+from .metrics import DepthMetrics
+from .ops import depth_metrics
 
 __all__ = [
     "depth_sampling", "k_offsets_f32", "est_costvolume_CW", "est_costvolume_F", "clear_cache", "prep_cache",
     "GNET", "MAGNET", "MagnetF", "MagnetHead", "MatchingPlan", "matching_loop", "install", "sid_planes",
+    "DepthMetrics", "depth_metrics",
 ]

@@ -22,6 +22,8 @@ OK, ERR_NULL, ERR_SHAPE, ERR_UNSUPPORTED, ERR_CUDA, ERR_ALIGN = 0, -1, -2, -3, -
 DEPTH_VOLUME, DEPTH_GAUSS, DEPTH_PLANES = 0, 1, 2
 SRC_NCHW, SRC_TILED32, SRC_PIXC, SRC_SPLIT16 = 0, 1, 2, 3
 VARIANT_AUTO, VARIANT_DIRECT, VARIANT_CELLS, VARIANT_CELLS_NOREUSE, VARIANT_TMA, VARIANT_MMA = 0, 1, 2, 3, 4, 5
+MAGNET_METRICS_MAX_PRED = 8
+MAGNET_METRICS_COLS = 13
 
 # every symbol include/magnet_b200.h declares (tests check the library exports all of them)
 EXPORTS = (
@@ -33,6 +35,7 @@ EXPORTS = (
     "magnet_relative_poses_f32", "magnet_camera_rays_f32",
     "magnet_upsample_nll_partials", "magnet_upsample_nll_fwd_f32", "magnet_upsample_nll_bwd_f32",
     "magnet_fnet_l1_partials", "magnet_fnet_l1_fwd_f32", "magnet_fnet_l1_bwd_f32",
+    "magnet_depth_metrics_workspace", "magnet_depth_metrics_f32",
 )
 
 
@@ -59,6 +62,15 @@ class CostBwdArgs(C.Structure):
     _fields_ = [("fwd", C.POINTER(CostArgs)), ("ref_feat", C.c_void_p), ("src_feat", C.c_void_p), ("src_gmm", C.c_void_p),
                 ("grad_out", C.c_void_p), ("workspace", C.c_void_p), ("grad_ref", C.c_void_p), ("grad_src", C.c_void_p),
                 ("grad_depth", C.c_void_p)]
+
+
+class DepthMetricsArgs(C.Structure):
+    """Mirror of ``struct magnet_depth_metrics_args``."""
+    _fields_ = [("P", C.c_int32), ("B", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("k", C.c_int32),
+                ("row0", C.c_int32), ("row1", C.c_int32), ("col0", C.c_int32), ("col1", C.c_int32),
+                ("min_depth", C.c_float), ("max_depth", C.c_float),
+                ("pred", C.POINTER(C.c_void_p)), ("up_mask", C.c_void_p), ("gt", C.c_void_p), ("workspace", C.c_void_p),
+                ("out", C.c_void_p)]
 
 
 class MagnetError(RuntimeError):
@@ -140,6 +152,10 @@ def lib() -> C.CDLL:
     L.magnet_fnet_l1_bwd_f32.restype = C.c_int
     L.magnet_fnet_l1_bwd_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int32,
                                          C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+    L.magnet_depth_metrics_workspace.restype = C.c_int64
+    L.magnet_depth_metrics_workspace.argtypes = [C.POINTER(DepthMetricsArgs)]
+    L.magnet_depth_metrics_f32.restype = C.c_int
+    L.magnet_depth_metrics_f32.argtypes = [C.POINTER(DepthMetricsArgs), C.c_void_p]
     if L.magnet_abi_version() != MAGNET_ABI_VERSION:
         raise MagnetError(f"ABI version mismatch: library {L.magnet_abi_version()} != binding {MAGNET_ABI_VERSION}")
     _lib = L

@@ -62,6 +62,10 @@ cudaError_t launch_upsample_nll_fwd(const float* depth, const float* mask, const
                                     int H, int W, int k, float* partial, cudaStream_t st);
 cudaError_t launch_upsample_nll_bwd(const float* depth, const float* mask, const float* gt, const uint8_t* gtm, float scale,
                                     int B, int H, int W, int k, float* gdepth, float* gmask, cudaStream_t st);
+size_t depth_metrics_workspace(int P, int B, int rows, int cols);
+cudaError_t launch_depth_metrics(const float* const* preds, int P, const float* up_mask, const float* gt, int B, int H,
+                                 int W, int k, int r0, int r1, int c0, int c1, float min_d, float max_d,
+                                 double* partial, double* out, cudaStream_t st);
 }  // namespace magnet
 
 namespace {
@@ -499,6 +503,40 @@ int magnet_fnet_l1_bwd_f32(const float* scores, const float* planes_host, const 
                                              (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e);
   g_launches += 1;
+  return MAGNET_OK;
+}
+
+namespace {
+// Shape fields and box only (the sizing call needs no pointers).
+int validate_depth_metrics_shape(const magnet_depth_metrics_args* a) {
+  if (!a) return MAGNET_ERR_NULL;
+  if (a->P <= 0 || a->B <= 0 || a->H <= 0 || a->W <= 0 || a->k < 0) return MAGNET_ERR_SHAPE;
+  if (a->P > MAGNET_METRICS_MAX_PRED) return MAGNET_ERR_UNSUPPORTED;
+  if ((int64_t)a->P * a->B > 65535 || (int64_t)a->H * a->W > (1 << 28)) return MAGNET_ERR_SHAPE;
+  if (a->k > 0 && (a->H % a->k != 0 || a->W % a->k != 0)) return MAGNET_ERR_SHAPE;
+  if (a->row0 < 0 || a->row0 > a->row1 || a->row1 > a->H) return MAGNET_ERR_SHAPE;
+  if (a->col0 < 0 || a->col0 > a->col1 || a->col1 > a->W) return MAGNET_ERR_SHAPE;
+  return MAGNET_OK;
+}
+}  // namespace
+
+int64_t magnet_depth_metrics_workspace(const magnet_depth_metrics_args* a) {
+  const int st = validate_depth_metrics_shape(a);
+  if (st != MAGNET_OK) return st;
+  return (int64_t)magnet::depth_metrics_workspace(a->P, a->B, a->row1 - a->row0, a->col1 - a->col0);
+}
+
+int magnet_depth_metrics_f32(const magnet_depth_metrics_args* a, void* stream) {
+  const int st = validate_depth_metrics_shape(a);
+  if (st != MAGNET_OK) return st;
+  if (!a->pred || !a->gt || !a->workspace || !a->out || (a->k > 0 && !a->up_mask)) return MAGNET_ERR_NULL;
+  for (int p = 0; p < a->P; ++p)
+    if (!a->pred[p]) return MAGNET_ERR_NULL;
+  cudaError_t e = magnet::launch_depth_metrics(a->pred, a->P, a->k > 0 ? a->up_mask : nullptr, a->gt, a->B, a->H, a->W,
+                                               a->k, a->row0, a->row1, a->col0, a->col1, a->min_depth, a->max_depth,
+                                               a->workspace, a->out, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 2;
   return MAGNET_OK;
 }
 

@@ -1,5 +1,6 @@
 // Small kernels around the cost volume: camera constants, source repack, sampler, Gaussian update.
 #include "common.cuh"
+#include "upsample_common.cuh"
 
 namespace magnet {
 
@@ -252,30 +253,7 @@ __global__ void camera_rays_kernel(const double* __restrict__ raw, int H, int W,
 // upsample_depth_via_mask (MAGNET.py:15-27) and, where gt_mask is set, nll = (mu-gt)^2 / (2 var) + 0.5 log(var),
 // var = max(sigma^2, 1e-10).  The (B,2,kH,kW) prediction is never written: forward emits one partial sum per CTA
 // (summed by the caller: deterministic), backward scatters straight into grad_depth / grad_mask.
-__device__ __forceinline__ void upsampled_gaussian(const float* __restrict__ depth, const float* __restrict__ mask,
-                                                   size_t b, int H, int W, int k, int x, int y, int kx, int ky,
-                                                   float (&w)[9], float& mu, float& sg) {
-  const size_t HW = (size_t)H * W;
-  const float* mp = mask + (b * 9 * k * k + (size_t)ky * k + kx) * HW + (size_t)y * W + x;
-  float m = -INFINITY;
-#pragma unroll
-  for (int i = 0; i < 9; ++i) { w[i] = mp[(size_t)i * k * k * HW]; m = fmaxf(m, w[i]); }
-  float s = 0.0f;
-#pragma unroll
-  for (int i = 0; i < 9; ++i) { w[i] = expf(w[i] - m); s += w[i]; }
-  const float inv = 1.0f / s;
-  mu = sg = 0.0f;
-#pragma unroll
-  for (int i = 0; i < 9; ++i) {
-    w[i] *= inv;
-    const int yy = y + i / 3 - 1, xx = x + i % 3 - 1;
-    if (yy >= 0 && yy < H && xx >= 0 && xx < W) {
-      mu = __fmaf_rn(w[i], depth[(b * 2 + 0) * HW + (size_t)yy * W + xx], mu);
-      sg = __fmaf_rn(w[i], depth[(b * 2 + 1) * HW + (size_t)yy * W + xx], sg);
-    }
-  }
-}
-
+// The upsampled (mu, sigma) come from upsampled_gaussian (upsample_common.cuh), shared with the depth metrics.
 __global__ void __launch_bounds__(128) upsample_nll_fwd_kernel(const float* __restrict__ depth, const float* __restrict__ mask,
                                                                 const float* __restrict__ gt, const uint8_t* __restrict__ gtm,
                                                                 int H, int W, int k, float* __restrict__ partial) {

@@ -114,3 +114,17 @@ class FlatGradAllReduce:
                 p.grad = torch.empty_like(p)
             p.grad.copy_(self.bucket[off:off + p.numel()].view_as(p))
             off += p.numel()
+
+
+def sum_tensor_over_ranks_(t: torch.Tensor) -> torch.Tensor:
+    """In-place sum of ``t`` over ranks (a no-op in a single process).  NCCL reduces device tensors where they are;
+    other backends reduce a host copy, which is written back."""
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size() == 1:
+        return t
+    if dist.get_backend() == "nccl" or not t.is_cuda:
+        dist.all_reduce(t, op=dist.ReduceOp.SUM)
+    else:
+        h = t.cpu()
+        dist.all_reduce(h, op=dist.ReduceOp.SUM)
+        t.copy_(h)
+    return t

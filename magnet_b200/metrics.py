@@ -1,0 +1,67 @@
+"""Depth evaluation on the device: a replacement for the metric block of validate() (test_MaGNet.py:52-79,
+train_MaGNet.py:153-180) and its ``utils.RunningAverageDict`` (utils/utils.py:160-174)."""
+from __future__ import annotations
+
+from typing import Optional
+
+import torch
+
+from . import _lib, dist, ops
+from .ops import METRIC_KEYS
+
+
+class DepthMetrics:
+    """Running average over images of the per-image metrics of ``ops.depth_metrics``, kept on the device.
+
+    ``update`` adds every image of the batch (the reference scores only image 0 of each batch; its test loaders use
+    batch 1) without a host read, so it can be captured in a CUDA graph once the accumulator exists (after the first
+    update, or ``reset``).  ``value`` reads the accumulator once and returns the reference's dict.  Sums and the
+    average are float64; an image without a valid pixel contributes NaN, as it does to the reference's average."""
+
+    def __init__(self, min_depth: float, max_depth: float, crop: Optional[str] = None):
+        ops.crop_box(crop, 1, 1)                       # reject an unknown crop now, not at the first update
+        self.min_depth, self.max_depth, self.crop = float(min_depth), float(max_depth), crop
+        # (P, 14) float64: images seen, then the sums over images of the 13 columns of ops.depth_metrics
+        self._acc: Optional[torch.Tensor] = None
+
+    def reset(self) -> None:
+        """Zero the running sums in place (a captured update keeps accumulating into the same memory)."""
+        if self._acc is not None:
+            self._acc.zero_()
+
+    def update(self, pred_or_list, gt: torch.Tensor, up_mask: Optional[torch.Tensor] = None,
+               k: Optional[int] = None) -> torch.Tensor:
+        """Score one batch: ``pred_or_list`` is (a list of up to 8) full-resolution (B,2,H,W) [mu, sigma], or with
+        ``up_mask`` and ``k`` the quarter-resolution Gaussians of ``MagnetHead.forward_quarter``.  Returns the (P,B,13)
+        per-image rows of ``ops.depth_metrics``."""
+        rows = ops.depth_metrics(pred_or_list, gt, min_depth=self.min_depth, max_depth=self.max_depth, crop=self.crop,
+                                 up_mask=up_mask, k=k)
+        P, B = rows.shape[0], rows.shape[1]
+        if self._acc is None:
+            self._acc = torch.zeros(P, 1 + _lib.MAGNET_METRICS_COLS, device=rows.device, dtype=torch.float64)
+        elif self._acc.shape[0] != P or self._acc.device != rows.device:
+            raise _lib.MagnetError(f"this DepthMetrics accumulates {self._acc.shape[0]} predictions on "
+                                   f"{self._acc.device}, got {P} on {rows.device}")
+        self._acc[:, 0] += B
+        self._acc[:, 1:] += rows.sum(dim=1)
+        return rows
+
+    def all_reduce(self) -> None:
+        """Sum the running sums over the ranks of ``torch.distributed`` (sharded evaluation); afterwards ``value`` is the
+        average over every rank's images.  Call it once, after the last update."""
+        if self._acc is None:
+            raise _lib.MagnetError("DepthMetrics.all_reduce before any update")
+        dist.sum_tensor_over_ranks_(self._acc)
+
+    def images(self) -> int:
+        """Number of images accumulated (one host read)."""
+        return 0 if self._acc is None else int(self._acc[0, 0].item())
+
+    def value(self, all_predictions: bool = False):
+        """The reference's ``RunningAverageDict.get_value()`` (keys in METRIC_KEYS order) for the last prediction, or a
+        list with one such dict per prediction.  One host read."""
+        if self._acc is None:
+            raise _lib.MagnetError("DepthMetrics.value before any update")
+        acc = self._acc.cpu()
+        out = [{key: float(acc[p, 2 + i] / acc[p, 0]) for i, key in enumerate(METRIC_KEYS)} for p in range(acc.shape[0])]
+        return out if all_predictions else out[-1]

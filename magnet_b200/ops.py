@@ -587,3 +587,69 @@ def camera_rays(raw_intrinsics: torch.Tensor, H: int, W: int):
         check(lib().magnet_camera_rays_f32(raw_intrinsics.data_ptr(), B, H, W, intM.data_ptr(), rays.data_ptr(),
                                            _stream(raw_intrinsics.device)), "magnet_camera_rays_f32")
     return {"intM": intM, "unit_ray_array_2D": rays}
+
+
+# validate() (test_MaGNet.py:62-68): the KITTI evaluation crops as fractions of the GT size -> (row0, row1, col0, col1)
+_CROPS = {"garg": (0.40810811, 0.99189189, 0.03594771, 0.96405229),
+          "eigen": (0.3324324, 0.91351351, 0.0359477, 0.96405229)}
+METRIC_KEYS = ("a1", "a2", "a3", "abs_diff", "abs_rel", "sq_rel", "rmse", "log_10", "irmse", "rmse_log", "silog", "nll")
+
+
+def crop_box(crop, H: int, W: int):
+    """Evaluation box [row0, row1) x [col0, col1) of an H x W GT: the whole image for ``crop=None``, else the 'garg' /
+    'eigen' crop bounds, computed with Python floats and int() exactly as validate() slices its eval_mask."""
+    if crop is None:
+        return 0, H, 0, W
+    if crop not in _CROPS:
+        raise _lib.MagnetError(f"crop must be None, 'garg' or 'eigen', got {crop!r}")
+    r0, r1, c0, c1 = _CROPS[crop]
+    r0, r1, c0, c1 = int(r0 * H), int(r1 * H), int(c0 * W), int(c1 * W)
+    return r0, max(r0, r1), c0, max(c0, c1)
+
+
+def depth_metrics(pred_or_list, gt: torch.Tensor, *, min_depth: float, max_depth: float, crop=None,
+                  up_mask: Optional[torch.Tensor] = None, k: Optional[int] = None) -> torch.Tensor:
+    """Per-image depth metrics of validate() (test_MaGNet.py:52-79) + utils.compute_depth_errors, on the device.
+
+    pred_or_list: one prediction or a list of up to 8 sharing ``gt`` (B,1,H,W) (raw GT; values above max_depth count
+    as 0).  Each prediction is the full-resolution (B,2,H,W) [mu, sigma], or, with ``up_mask`` (B,9k^2,H/k,W/k) and
+    ``k``, the quarter-resolution (B,2,H/k,W/k) Gaussians, upsampled inside the kernel (upsample_depth_via_mask).
+    crop: None, 'garg' or 'eigen'.  Returns a (P,B,13) float64 device tensor: the number of valid pixels, then the
+    metrics in METRIC_KEYS order (NaN for an image without a valid pixel).  Two kernel launches, no host sync."""
+    preds = [pred_or_list] if isinstance(pred_or_list, torch.Tensor) else list(pred_or_list)
+    if not 1 <= len(preds) <= _lib.MAGNET_METRICS_MAX_PRED:
+        raise _lib.MagnetError(f"1 to {_lib.MAGNET_METRICS_MAX_PRED} predictions per call, got {len(preds)}")
+    gt = _need_cuda_f32("gt", gt)
+    if gt.dim() != 4 or gt.shape[1] != 1:
+        raise _lib.MagnetError(f"gt must be (B,1,H,W), got {tuple(gt.shape)}")
+    B, _, H, W = gt.shape
+    if (up_mask is None) != (k is None):
+        raise _lib.MagnetError("up_mask and k go together (the fused-upsampling form needs both)")
+    if up_mask is not None:
+        k = int(k)
+        if k < 1 or H % k or W % k:
+            raise _lib.MagnetError(f"k = {k} must be >= 1 and divide the GT size {H}x{W}")
+        up_mask = _need_cuda_f32("up_mask", up_mask)
+        _expect("up_mask", up_mask, (B, 9 * k * k, H // k, W // k))
+        pshape = (B, 2, H // k, W // k)
+    else:
+        pshape = (B, 2, H, W)
+    for i, p in enumerate(preds):
+        preds[i] = _need_cuda_f32(f"pred[{i}]", p)
+        _expect(f"pred[{i}]", preds[i], pshape)
+    dev = _same_device(("gt", gt), ("up_mask", up_mask), *((f"pred[{i}]", p) for i, p in enumerate(preds)))
+    r0, r1, c0, c1 = crop_box(crop, H, W)
+    ptrs = (C.c_void_p * len(preds))(*[p.data_ptr() for p in preds])
+    a = _lib.DepthMetricsArgs(P=len(preds), B=B, H=H, W=W, k=k or 0, row0=r0, row1=r1, col0=c0, col1=c1,
+                              min_depth=float(min_depth), max_depth=float(max_depth),
+                              pred=C.cast(ptrs, C.POINTER(C.c_void_p)), up_mask=up_mask.data_ptr() if k else None,
+                              gt=gt.data_ptr())
+    n = lib().magnet_depth_metrics_workspace(C.byref(a))
+    if n < 0:
+        check(int(n), "magnet_depth_metrics_workspace")
+    workspace = torch.empty(int(n), device=dev, dtype=torch.float64)
+    out = torch.empty(len(preds), B, _lib.MAGNET_METRICS_COLS, device=dev, dtype=torch.float64)
+    a.workspace, a.out = workspace.data_ptr(), out.data_ptr()
+    with torch.cuda.device(dev):
+        check(lib().magnet_depth_metrics_f32(C.byref(a), _stream(dev)), "magnet_depth_metrics_f32")
+    return out
