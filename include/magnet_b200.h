@@ -8,7 +8,8 @@
  *
  * Conventions
  *   - plain C, no torch types; every pointer is a DEVICE pointer unless the field says
- *     "host"; all tensors are fp32, dense, in the layout stated per field;
+ *     "host"; all tensors are fp32, dense, in the layout stated per field (the one exception:
+ *     the fp16 / bf16 input of magnet_repack_half16);
  *   - caller owns all memory; no entry point allocates, frees or synchronises; every
  *     launch goes to the cudaStream_t passed as `stream` (NULL = legacy default
  *     stream), so calls are CUDA-graph capturable;
@@ -54,17 +55,29 @@ typedef enum magnet_src_layout {
                             Gaussian (mu, sigma) and two zeros (see magnet_repack_pixc_f32): the layout the
                             TMA-staged CUDA-core kernel fetches its windows from.  With this layout
                             magnet_cost_args.src_gmm is ignored (the Gaussians travel inside src_feat). */
-  MAGNET_SRC_SPLIT16 = 3  /* tensor-core layout (C == 64): a 256-byte header (power-of-two scale s), two fp16 planes
+  MAGNET_SRC_SPLIT16 = 3, /* tensor-core layout (C == 64): a 256-byte header (power-of-two scale s), two fp16 planes
                             (V*B, 2, H, W, 64) with x*s = hi + lo, and a (V*B, H, W+1, 4) table whose entry x+1 holds (mu, sigma) of
                             pixel x and of pixel x+1 (zeros outside the row); see
                             magnet_repack_split16_f32 / magnet_split16_bytes.  With this layout ref_feat must ALSO
                             point to a split buffer (of the B reference feature maps, Gaussians NULL) and src_gmm is
                             ignored. */
+  MAGNET_SRC_HALF16 = 4   /* tensor-core layout for fp16 / bf16 feature maps (C == 64): SPLIT16's header and table around
+                            ONE fp16 plane (V*B, 1, H, W, 64) holding fp16(x*s), s from the same rule (x*s is then
+                            itself an fp16 number; DESIGN §3.7); see magnet_repack_half16 / magnet_half16_bytes.
+                            Accepted wherever SPLIT16 is, with the same rules: ref_feat must ALSO point to a HALF16
+                            buffer, src_gmm is ignored.  The ABI cannot tell the two kinds of buffer apart: the caller
+                            names the right one. */
 } magnet_src_layout;
+
+/* Element type of the input of magnet_repack_half16. */
+typedef enum magnet_dtype {
+  MAGNET_DTYPE_F16 = 0,   /* IEEE binary16 */
+  MAGNET_DTYPE_BF16 = 1   /* bfloat16 */
+} magnet_dtype;
 
 /* Kernel selection (for parity cross-checks and profiling). */
 typedef enum magnet_variant {
-  MAGNET_VARIANT_AUTO = 0,   /* production choice: MMA for MAGNET_SRC_SPLIT16, TMA for MAGNET_SRC_PIXC, CELLS for
+  MAGNET_VARIANT_AUTO = 0,   /* production choice: MMA for MAGNET_SRC_SPLIT16 / HALF16, TMA for MAGNET_SRC_PIXC, CELLS for
                                 MAGNET_SRC_TILED32, DIRECT otherwise                           */
   MAGNET_VARIANT_DIRECT = 1, /* one thread per output, 4 taps x C channels per hypothesis,
                                 reference operation order, fp64 view accumulation             */
@@ -74,7 +87,7 @@ typedef enum magnet_variant {
   MAGNET_VARIANT_TMA = 4,    /* CUDA-core tap-sharing kernel, 4 lanes per pixel, the CTA's source window
                                 staged in shared memory by TMA (MAGNET_SRC_PIXC only)          */
   MAGNET_VARIANT_MMA = 5     /* tensor-core kernel: all (reference pixel, window cell) channel dot products of an
-                                8x8 tile by wgmma tensor-core MMA (MAGNET_SRC_SPLIT16 only) */
+                                8x8 tile by wgmma tensor-core MMA (MAGNET_SRC_SPLIT16 / HALF16 only) */
 } magnet_variant;
 
 /* Per (batch element, view) camera constants, 16 floats, produced by magnet_pack_cameras_f32.
@@ -133,7 +146,8 @@ int magnet_cost_volume_f32(const magnet_cost_args* args, void* stream);
  * ignored.  Two forms:
  *   - src_layout MAGNET_SRC_NCHW, C in {8,16,32,64}: ref_feat / src_feat are the NCHW feature maps (CUDA-core kernel);
  *   - src_layout MAGNET_SRC_SPLIT16, variant AUTO or MMA, C == 64, V <= 16: ref_feat / src_feat are the split buffers
- *     the forward read (tensor-core kernel: both gradients as GEMMs on the fp16 hi/lo planes).
+ *     the forward read (tensor-core kernel: both gradients as GEMMs on the fp16 hi/lo planes).  MAGNET_SRC_HALF16 in
+ *     the same way, on HALF16 buffers.
  * grad_src is accumulated with atomics in either form, so results are not bit-deterministic from run to run.
  */
 typedef struct magnet_cost_f_bwd_args {
@@ -153,8 +167,8 @@ int magnet_cost_volume_f_bwd_f32(const magnet_cost_f_bwd_args* args, void* strea
  * grid_sample's bilinear gather, including its derivative in the sample position.
  * `fwd` is the forward call (depth_mode MAGNET_DEPTH_VOLUME or MAGNET_DEPTH_GAUSS); its src_layout and variant name the
  * forward kernel, whose consistency mask the backward reproduces bit for bit.  Two forms:
- *   - src_layout MAGNET_SRC_SPLIT16, variant AUTO or MMA (C == 64, V <= 16): fwd->ref_feat / fwd->src_feat are the split
- *     buffers the forward read; grad_ref and grad_src come from the tensor-core kernel (two GEMMs on the fp16 hi/lo
+ *   - src_layout MAGNET_SRC_SPLIT16 or MAGNET_SRC_HALF16, variant AUTO or MMA (C == 64, V <= 16): fwd->ref_feat /
+ *     fwd->src_feat are the SPLIT16 / HALF16 buffers the forward read; grad_ref and grad_src come from the tensor-core kernel (two GEMMs on the fp16 hi/lo
  *     planes).  The NCHW maps below are needed only for grad_depth.  With fwd->ref_feat and fwd->src_feat both NULL,
  *     every gradient comes from the CUDA-core kernel on the NCHW maps, still with the tensor-core forward's mask;
  *   - variant MAGNET_VARIANT_DIRECT (src_layout NCHW or TILED32): everything from the NCHW maps below, C <= 64.
@@ -199,6 +213,14 @@ int magnet_repack_pixc_f32(const float* src_nchw, const float* src_gmm, float* d
 size_t magnet_split16_bytes(int32_t N, int32_t H, int32_t W);
 int magnet_repack_split16_f32(const float* src_nchw, const float* src_gmm, void* dst, int32_t N, int32_t C, int32_t H,
                               int32_t W, void* stream);
+
+/* Half-precision feature maps (N, 64, H, W) of element type `dtype` (magnet_dtype) [+ fp32 (N, 2, H, W) Gaussians, may
+ * be NULL -> zeros] -> MAGNET_SRC_HALF16 buffer of magnet_half16_bytes(N, H, W) bytes; src and dst 16-byte aligned.
+ * The scale and the table are those magnet_repack_split16_f32 gives for the fp32 upcast of src, the plane is its hi
+ * plane.  C != 64 or an unknown dtype -> MAGNET_ERR_UNSUPPORTED.  Three stream operations, as the fp32 split. */
+size_t magnet_half16_bytes(int32_t N, int32_t H, int32_t W);
+int magnet_repack_half16(const void* src_nchw, int32_t dtype, const float* src_gmm, void* dst, int32_t N, int32_t C,
+                         int32_t H, int32_t W, void* stream);
 
 /* Source-feature repack (N, C, H, W) -> MAGNET_SRC_TILED32 (N, H, ceil(W/32), C/4, 32, 4);
  * C % 4 == 0, dst 16-byte aligned, padding pixels are written as zeros. */

@@ -20,7 +20,8 @@ MAGNET_MAX_PLANES = 256
 
 OK, ERR_NULL, ERR_SHAPE, ERR_UNSUPPORTED, ERR_CUDA, ERR_ALIGN = 0, -1, -2, -3, -4, -5
 DEPTH_VOLUME, DEPTH_GAUSS, DEPTH_PLANES = 0, 1, 2
-SRC_NCHW, SRC_TILED32, SRC_PIXC, SRC_SPLIT16 = 0, 1, 2, 3
+SRC_NCHW, SRC_TILED32, SRC_PIXC, SRC_SPLIT16, SRC_HALF16 = 0, 1, 2, 3, 4
+DTYPE_F16, DTYPE_BF16 = 0, 1
 VARIANT_AUTO, VARIANT_DIRECT, VARIANT_CELLS, VARIANT_CELLS_NOREUSE, VARIANT_TMA, VARIANT_MMA = 0, 1, 2, 3, 4, 5
 MAGNET_METRICS_MAX_PRED = 8
 MAGNET_METRICS_COLS = 13
@@ -30,7 +31,8 @@ EXPORTS = (
     "magnet_abi_version", "magnet_strerror", "magnet_last_cuda_error", "magnet_launch_count",
     "magnet_cost_launch_info", "magnet_cost_volume_f32", "magnet_cost_volume_f_bwd_f32", "magnet_cost_volume_bwd_f32",
     "magnet_pack_cameras_f32",
-    "magnet_repack_tiled32_f32", "magnet_repack_pixc_f32", "magnet_repack_split16_f32", "magnet_split16_bytes", "magnet_sample_depths_f32", "magnet_gaussian_update_fwd_f32",
+    "magnet_repack_tiled32_f32", "magnet_repack_pixc_f32", "magnet_repack_split16_f32", "magnet_split16_bytes",
+    "magnet_repack_half16", "magnet_half16_bytes", "magnet_sample_depths_f32", "magnet_gaussian_update_fwd_f32",
     "magnet_gaussian_update_bwd_f32", "magnet_convex_upsample_fwd_f32", "magnet_convex_upsample_bwd_f32",
     "magnet_relative_poses_f32", "magnet_camera_rays_f32",
     "magnet_upsample_nll_partials", "magnet_upsample_nll_fwd_f32", "magnet_upsample_nll_bwd_f32",
@@ -120,6 +122,11 @@ def lib() -> C.CDLL:
     L.magnet_repack_split16_f32.restype = C.c_int
     L.magnet_repack_split16_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                             C.c_void_p]
+    L.magnet_half16_bytes.restype = C.c_size_t
+    L.magnet_half16_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+    L.magnet_repack_half16.restype = C.c_int
+    L.magnet_repack_half16.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                       C.c_int32, C.c_void_p]
     L.magnet_sample_depths_f32.restype = C.c_int
     L.magnet_sample_depths_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     L.magnet_gaussian_update_fwd_f32.restype = C.c_int

@@ -15,12 +15,15 @@ bool cells_supports(int C, int D, int layout);
 cudaError_t launch_cost_tma(const CostParams& p, int mode, int C, bool cw, cudaStream_t st);
 bool tma_supports(int C, int D, int V, int layout);
 void tma_launch_info(int B, int H, int W, int D, int* grid, int* block, int* smem);
-cudaError_t launch_cost_mma(const CostParams& p, int mode, bool cw, cudaStream_t st);
+cudaError_t launch_cost_mma(const CostParams& p, int mode, bool cw, int layout, cudaStream_t st);
 bool mma_supports(int C, int D, int V, int layout);
 void mma_launch_info(int B, int H, int W, int D, int* grid, int* block, int* smem);
 size_t split16_buffer_bytes(int N, int H, int W);
+size_t half16_buffer_bytes(int N, int H, int W);
 cudaError_t launch_repack_split16(const float* src, const float* gmm, void* dst, int N, int C, int H, int W,
                                   cudaStream_t st, int* launches);
+cudaError_t launch_repack_half16(const void* src, int dtype, const float* gmm, void* dst, int N, int C, int H, int W,
+                                 cudaStream_t st, int* launches);
 #if defined(MAGNET_MMA_DEBUG) || defined(MAGNET_MMA_PROFILE)
 void mma_set_debug_buffer(float* p);
 #endif
@@ -44,10 +47,10 @@ cudaError_t launch_upsample_fwd(const float* depth, const float* mask, int B, in
 cudaError_t launch_upsample_bwd(const float* gout, const float* depth, const float* mask, int B, int CH, int H, int W,
                                 int k, float* gdepth, float* gmask, cudaStream_t st);
 cudaError_t launch_cost_f_bwd(const BwdParams& p, cudaStream_t st, int* launches);
-cudaError_t launch_cost_f_bwd_mma(const BwdParams& p, cudaStream_t st, int* launches);
+cudaError_t launch_cost_f_bwd_mma(const BwdParams& p, int layout, cudaStream_t st, int* launches);
 bool f_bwd_mma_supports(int C, int V);
-cudaError_t launch_cost_cw_bwd(const CwBwdParams& p, const CwBwdParams* split, int C, int mode, bool mask_mma,
-                               const float* grad_out, cudaStream_t st, int* launches);
+cudaError_t launch_cost_cw_bwd(const CwBwdParams& p, const CwBwdParams* split, int split_layout, int C, int mode,
+                               bool mask_mma, const float* grad_out, cudaStream_t st, int* launches);
 bool cw_bwd_supports(int C);
 #ifdef MAGNET_MMA_DEBUG
 void f_bwd_mma_set_debug_buffer(float* p);
@@ -72,6 +75,9 @@ namespace {
 std::atomic<uint64_t> g_launches{0};
 thread_local char g_cuda_err[256] = "";
 
+// the tensor-core layouts: a header + fp16 plane(s) + (mu, sigma) table per buffer, ref_feat included
+bool packed_layout(int layout) { return layout == MAGNET_SRC_SPLIT16 || layout == MAGNET_SRC_HALF16; }
+
 int cuda_fail(cudaError_t e) {
   snprintf(g_cuda_err, sizeof(g_cuda_err), "%s: %s", cudaGetErrorName(e), cudaGetErrorString(e));
   return MAGNET_ERR_CUDA;
@@ -83,7 +89,7 @@ int validate_cost(const magnet_cost_args* a) {
   if (a->D > MAGNET_MAX_PLANES) return MAGNET_ERR_UNSUPPORTED;
   if ((int64_t)a->H * a->W > (1 << 26)) return MAGNET_ERR_SHAPE;
   if (!a->ref_feat || !a->src_feat || !a->rays || !a->cams || !a->out) return MAGNET_ERR_NULL;
-  if (a->consistency && !a->src_gmm && a->src_layout != MAGNET_SRC_PIXC && a->src_layout != MAGNET_SRC_SPLIT16)
+  if (a->consistency && !a->src_gmm && a->src_layout != MAGNET_SRC_PIXC && !packed_layout(a->src_layout))
     return MAGNET_ERR_NULL;
   if (a->consistency && a->softmax) return MAGNET_ERR_UNSUPPORTED;
   switch (a->depth_mode) {
@@ -99,7 +105,7 @@ int validate_cost(const magnet_cost_args* a) {
     if (!magnet::tma_supports(a->C, a->D, a->V, a->src_layout)) return MAGNET_ERR_UNSUPPORTED;
     if (reinterpret_cast<uintptr_t>(a->src_feat) % 16 != 0) return MAGNET_ERR_ALIGN;
     if (a->variant != MAGNET_VARIANT_AUTO && a->variant != MAGNET_VARIANT_TMA) return MAGNET_ERR_UNSUPPORTED;
-  } else if (a->src_layout == MAGNET_SRC_SPLIT16) {
+  } else if (packed_layout(a->src_layout)) {
     if (!magnet::mma_supports(a->C, a->D, a->V, a->src_layout)) return MAGNET_ERR_UNSUPPORTED;
     if (reinterpret_cast<uintptr_t>(a->src_feat) % 16 != 0 || reinterpret_cast<uintptr_t>(a->ref_feat) % 16 != 0)
       return MAGNET_ERR_ALIGN;
@@ -129,8 +135,8 @@ bool use_tma(const magnet_cost_args* a) {                  // the PIXC layout is
   return a->src_layout == MAGNET_SRC_PIXC && magnet::tma_supports(a->C, a->D, a->V, a->src_layout);
 }
 
-bool use_mma(const magnet_cost_args* a) {                  // the SPLIT16 layout is served by the tensor-core kernel only
-  return a->src_layout == MAGNET_SRC_SPLIT16 && magnet::mma_supports(a->C, a->D, a->V, a->src_layout);
+bool use_mma(const magnet_cost_args* a) {                  // SPLIT16 / HALF16 are served by the tensor-core kernel only
+  return packed_layout(a->src_layout) && magnet::mma_supports(a->C, a->D, a->V, a->src_layout);
 }
 }  // namespace
 
@@ -191,7 +197,7 @@ int magnet_cost_volume_f32(const magnet_cost_args* a, void* stream) {
   cudaError_t e;
   if (use_mma(a) || use_tma(a) || use_cells(a)) {
     if (use_mma(a))
-      e = magnet::launch_cost_mma(p, a->depth_mode, a->consistency != 0, (cudaStream_t)stream);
+      e = magnet::launch_cost_mma(p, a->depth_mode, a->consistency != 0, a->src_layout, (cudaStream_t)stream);
     else if (use_tma(a))
       e = magnet::launch_cost_tma(p, a->depth_mode, a->C, a->consistency != 0, (cudaStream_t)stream);
     else
@@ -220,8 +226,8 @@ int magnet_cost_volume_f_bwd_f32(const magnet_cost_f_bwd_args* b, void* stream) 
   if (!b->grad_out || !b->workspace || !b->grad_ref || !b->grad_src) return MAGNET_ERR_NULL;
   if (a->softmax && !b->prob) return MAGNET_ERR_NULL;
   if (a->consistency || a->depth_mode != MAGNET_DEPTH_PLANES) return MAGNET_ERR_UNSUPPORTED;
-  const bool mma = a->src_layout == MAGNET_SRC_SPLIT16;
-  if (mma) {                                   // tensor-core backward on the forward's split buffers
+  const bool mma = packed_layout(a->src_layout);
+  if (mma) {                                   // tensor-core backward on the forward's SPLIT16 / HALF16 buffers
     if (a->variant != MAGNET_VARIANT_AUTO && a->variant != MAGNET_VARIANT_MMA) return MAGNET_ERR_UNSUPPORTED;
     if (!magnet::f_bwd_mma_supports(a->C, a->V)) return MAGNET_ERR_UNSUPPORTED;
     if (reinterpret_cast<uintptr_t>(a->src_feat) % 16 != 0 || reinterpret_cast<uintptr_t>(a->ref_feat) % 16 != 0)
@@ -238,7 +244,7 @@ int magnet_cost_volume_f_bwd_f32(const magnet_cost_f_bwd_args* b, void* stream) 
   p.prob = b->prob; p.grad_out = b->grad_out; p.g_score = b->workspace; p.grad_ref = b->grad_ref; p.grad_src = b->grad_src;
   for (int j = 0; j < MAGNET_MAX_PLANES; ++j) p.k[j] = j < a->D ? a->k_host[j] : 0.0f;
   int launches = 0;
-  cudaError_t e = mma ? magnet::launch_cost_f_bwd_mma(p, (cudaStream_t)stream, &launches)
+  cudaError_t e = mma ? magnet::launch_cost_f_bwd_mma(p, a->src_layout, (cudaStream_t)stream, &launches)
                       : magnet::launch_cost_f_bwd(p, (cudaStream_t)stream, &launches);
   if (e != cudaSuccess) return cuda_fail(e);
   g_launches += launches;
@@ -258,7 +264,7 @@ int magnet_cost_volume_bwd_f32(const magnet_cost_bwd_args* b, void* stream) {
     case MAGNET_DEPTH_GAUSS: if (!a->ref_gmm || !a->k_host) return MAGNET_ERR_NULL; break;
     default: return MAGNET_ERR_UNSUPPORTED;
   }
-  const bool mask_mma = a->src_layout == MAGNET_SRC_SPLIT16;   // the tensor-core forward's mask
+  const bool mask_mma = packed_layout(a->src_layout);   // the tensor-core forward's mask
   // its split buffers given: feature gradients on the tensor cores; both NULL: everything on the CUDA cores
   const bool split = mask_mma && (a->ref_feat || a->src_feat);
   if (mask_mma) {
@@ -294,8 +300,8 @@ int magnet_cost_volume_bwd_f32(const magnet_cost_bwd_args* b, void* stream) {
   magnet::CwBwdParams ps = p;
   ps.ref_feat = a->ref_feat; ps.src_feat = a->src_feat; ps.src_gmm = nullptr; ps.grad_depth = nullptr;
   int launches = 0;
-  cudaError_t e = magnet::launch_cost_cw_bwd(p, split ? &ps : nullptr, a->C, a->depth_mode, mask_mma, b->grad_out,
-                                             (cudaStream_t)stream, &launches);
+  cudaError_t e = magnet::launch_cost_cw_bwd(p, split ? &ps : nullptr, a->src_layout, a->C, a->depth_mode, mask_mma,
+                                             b->grad_out, (cudaStream_t)stream, &launches);
   if (e != cudaSuccess) return cuda_fail(e);
   g_launches += launches;
   return MAGNET_OK;
@@ -351,6 +357,24 @@ int magnet_repack_split16_f32(const float* src_nchw, const float* src_gmm, void*
   if (reinterpret_cast<uintptr_t>(dst) % 16 != 0 || reinterpret_cast<uintptr_t>(src_nchw) % 16 != 0) return MAGNET_ERR_ALIGN;
   int launches = 0;
   cudaError_t e = magnet::launch_repack_split16(src_nchw, src_gmm, dst, N, C, H, W, (cudaStream_t)stream, &launches);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += launches;
+  return MAGNET_OK;
+}
+
+size_t magnet_half16_bytes(int32_t N, int32_t H, int32_t W) {
+  if (N <= 0 || H <= 0 || W <= 0) return 0;
+  return magnet::half16_buffer_bytes(N, H, W);
+}
+
+int magnet_repack_half16(const void* src_nchw, int32_t dtype, const float* src_gmm, void* dst, int32_t N, int32_t C,
+                         int32_t H, int32_t W, void* stream) {
+  if (!src_nchw || !dst) return MAGNET_ERR_NULL;
+  if (N <= 0 || C <= 0 || H <= 0 || W <= 0 || N > 65535) return MAGNET_ERR_SHAPE;
+  if (C != 64 || (dtype != MAGNET_DTYPE_F16 && dtype != MAGNET_DTYPE_BF16)) return MAGNET_ERR_UNSUPPORTED;
+  if (reinterpret_cast<uintptr_t>(dst) % 16 != 0 || reinterpret_cast<uintptr_t>(src_nchw) % 16 != 0) return MAGNET_ERR_ALIGN;
+  int launches = 0;
+  cudaError_t e = magnet::launch_repack_half16(src_nchw, dtype, src_gmm, dst, N, C, H, W, (cudaStream_t)stream, &launches);
   if (e != cudaSuccess) return cuda_fail(e);
   g_launches += launches;
   return MAGNET_OK;

@@ -248,15 +248,15 @@ static void launch_cpl(const CwBwdParams& p, int C, int mode, int mask, dim3 gri
   }
 }
 
-cudaError_t launch_cost_cw_bwd_mma(const CwBwdParams& p, int mode, cudaStream_t st);   // cost_f_bwd_mma.cu
+cudaError_t launch_cost_cw_bwd_mma(const CwBwdParams& p, int mode, int layout, cudaStream_t st);   // cost_f_bwd_mma.cu
 
 // p: NCHW maps (CUDA-core kernel).  split: the same call with ref_feat / src_feat pointing to the forward's SPLIT16
-// buffers, or NULL.  With split, both feature gradients come from the tensor-core kernel and the CUDA-core kernel only
+// or HALF16 buffers (split_layout), or NULL.  With split, both feature gradients come from the tensor-core kernel and the CUDA-core kernel only
 // computes the depth gradient; otherwise the CUDA-core kernel computes everything that is requested.  mask_mma:
 // reproduce the mask of the tensor-core forward (else of the DIRECT forward).  First of all g_score = grad_out / V goes
 // to the workspace (score_grad_kernel with softmax = 0).
-cudaError_t launch_cost_cw_bwd(const CwBwdParams& p, const CwBwdParams* split, int C, int mode, bool mask_mma,
-                               const float* grad_out, cudaStream_t st, int* launches) {
+cudaError_t launch_cost_cw_bwd(const CwBwdParams& p, const CwBwdParams* split, int split_layout, int C, int mode,
+                               bool mask_mma, const float* grad_out, cudaStream_t st, int* launches) {
   BwdParams s;
   s.B = p.B; s.V = p.V; s.D = p.D; s.C = C; s.H = p.H; s.W = p.W; s.HW = p.HW;
   s.softmax = 0;
@@ -272,7 +272,7 @@ cudaError_t launch_cost_cw_bwd(const CwBwdParams& p, const CwBwdParams* split, i
   CwBwdParams cc = p;
   if (split != nullptr) {
     if (split->grad_ref != nullptr || split->grad_src != nullptr) {
-      if ((e = launch_cost_cw_bwd_mma(*split, mode, st)) != cudaSuccess) return e;
+      if ((e = launch_cost_cw_bwd_mma(*split, mode, split_layout, st)) != cudaSuccess) return e;
       ++*launches;
     }
     cc.grad_ref = cc.grad_src = nullptr;

@@ -35,6 +35,9 @@
 //     with red.global.add.f32 — results are NOT bit-deterministic from run to run (the order of the additions varies),
 //     exactly like cost_f_bwd.cu and torch's grid_sample backward.
 //
+//   * MAGNET_SRC_HALF16 operands (PLANES = 1, DESIGN §3.7): the boxes carry the one plane (the lo atom slots stay
+//     unwritten) and each GEMM issues Gc_lo*S + Gc_hi*S (Gc_lo*R + Gc_hi*R): the order above minus the *lo term.
+//
 // Shared memory: reference tile 16 KB + one 32 KB region that holds fp32 Gc, then (Gc dead) the source window, then the
 // g_ref partial sums + fp16 Gc 32 KB + tables: ~83 KB, two CTAs per SM (DESIGN §3.4).
 #include <cuda_fp16.h>
@@ -94,8 +97,8 @@ __device__ __noinline__ bool table_keep(const float4* __restrict__ meta, float i
 // P = BwdParams, MODE = PLANES, CW = false: the F volume.  P = CwBwdParams (MODE VOLUME or GAUSS, CW = true): the CW
 // volume, whose depths are per pixel and whose (pixel, hypothesis) pairs count only where the forward's consistency
 // mask kept them (p.cw == 1): the mask is evaluated with the helpers of cw_mask.cuh on the (mu, sigma) table of the
-// source SPLIT16 buffer, exactly as cost_mma.cu evaluates it.
-template <class P, int MODE, bool CW>
+// source SPLIT16 buffer, exactly as cost_mma.cu evaluates it.  PLANES = 2: SPLIT16 operands, 1: HALF16.
+template <class P, int MODE, bool CW, int PLANES>
 __global__ void __launch_bounds__(BNT, 2)
 cost_f_bwd_mma_kernel(const __grid_constant__ P p, const __grid_constant__ CUtensorMap tm_ref,
                       const __grid_constant__ CUtensorMap tm_src, const int n_items, const int slot,
@@ -117,6 +120,7 @@ cost_f_bwd_mma_kernel(const __grid_constant__ P p, const __grid_constant__ CUten
   const int tiles_x = (W + BTW - 1) / BTW, tiles = tiles_x * ((H + BTH - 1) / BTH);
   const Split16Header* hdr_ref = reinterpret_cast<const Split16Header*>(p.ref_feat);
   const Split16Header* hdr_src = reinterpret_cast<const Split16Header*>(p.src_feat);
+  static_assert(PLANES == 1 || PLANES == 2, "hi / lo planes, or hi only");
 
   if (tid == 0) {
     mbar_init(bar_ref, 1);
@@ -141,7 +145,7 @@ cost_f_bwd_mma_kernel(const __grid_constant__ P p, const __grid_constant__ CUten
   const int tx0 = (tile % tiles_x) * BTW, ty0 = (tile / tiles_x) * BTH;
   if (tid == 0) {
     // every reader of the tile region and of misc[8..9] passed the barrier that ended the previous item
-    mbar_arrive_expect_tx(bar_ref, 16384u);
+    mbar_arrive_expect_tx(bar_ref, 8192u * PLANES);
     tma_load_5d(sbase + BOFF_REF, &tm_ref, bar_ref, 0, tx0, ty0, 0, b);
     misc[8] = 0;
     misc[9] = (int)gridDim.x + (int)atomicAdd(&g_fbwd_next[slot], 1u);
@@ -189,7 +193,7 @@ cost_f_bwd_mma_kernel(const __grid_constant__ P p, const __grid_constant__ CUten
     const float4* meta = nullptr;                          // (mu, sigma) table of the source split buffer (CW)
     if constexpr (CW)
       meta = reinterpret_cast<const float4*>(reinterpret_cast<const unsigned char*>(p.src_feat) + SPLIT16_HEADER +
-                                             (size_t)p.B * V * HW * 256);
+                                             (size_t)p.B * V * HW * 128 * PLANES);
     // cell origin of plane j at my pixel, and whether it can contribute (a tap in the image, g != 0)
     auto cell = [&](const int j, float& g, float& ix, float& iy, int& x0, int& y0) -> bool {
       g = ldg_f(gs + (size_t)j * HW);
@@ -309,7 +313,7 @@ cost_f_bwd_mma_kernel(const __grid_constant__ P p, const __grid_constant__ CUten
       // ---------------- source window by TMA (an odd segment count is padded with a box wholly outside the image,
       // which the copy engine fills with zeros: the last K step of GEMM 1 spans two segments) -------------------------
       const int nload = nsegs + (nsegs & 1);
-      if (tid == 0) mbar_arrive_expect_tx(bar_win, (uint32_t)nload * BSEG_BYTES);
+      if (tid == 0) mbar_arrive_expect_tx(bar_win, (uint32_t)nload * 1024u * PLANES);
       if (lane == 0) {
         for (int s = warp; s < nload; s += BNT / 32) {
           const int r = s / nseg, xb = s - r * nseg;
@@ -344,7 +348,7 @@ cost_f_bwd_mma_kernel(const __grid_constant__ P p, const __grid_constant__ CUten
           const uint64_t ah = gmma_desc_sw128(g_hi + kk * 2048, 1024), al = gmma_desc_sw128(g_lo + kk * 2048, 1024);
           const uint64_t bh = gmma_desc_sw128(w_hi + kk * 4096, BSEG_BYTES), bl = gmma_desc_sw128(w_lo + kk * 4096, BSEG_BYTES);
           wgmma_m64n64k16_f16<1, 1>(acc1, al, bh);
-          wgmma_m64n64k16_f16<1, 1>(acc1, ah, bl);
+          if constexpr (PLANES == 2) wgmma_m64n64k16_f16<1, 1>(acc1, ah, bl);
           wgmma_m64n64k16_f16<1, 1>(acc1, ah, bh);
         }
         // g_src[cell][c] = sum_p Gc[p][cell] R[p][c]: A = Gc K-major (the K step of 16 pixels is +32 bytes inside the
@@ -355,7 +359,7 @@ cost_f_bwd_mma_kernel(const __grid_constant__ P p, const __grid_constant__ CUten
           for (int kk = 0; kk < 4; ++kk) {
             const uint64_t bh = gmma_desc_sw128(r_hi + kk * 2048, 1024), bl = gmma_desc_sw128(r_lo + kk * 2048, 1024);
             wgmma_m64n64k16_f16<0, 1>(acc2, al + 2u * kk, bh);
-            wgmma_m64n64k16_f16<0, 1>(acc2, ah + 2u * kk, bl);
+            if constexpr (PLANES == 2) wgmma_m64n64k16_f16<0, 1>(acc2, ah + 2u * kk, bl);
             wgmma_m64n64k16_f16<0, 1>(acc2, ah + 2u * kk, bh);
           }
         }
@@ -456,7 +460,8 @@ cost_f_bwd_mma_kernel(const __grid_constant__ P p, const __grid_constant__ CUten
 // ---------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------
-cudaError_t make_planes_map(CUtensorMap* tm, const void* planes, int N, int H, int W, int box_rows);   // cost_mma.cu
+cudaError_t make_planes_map(CUtensorMap* tm, const void* planes, int N, int H, int W, int box_rows,
+                            int nplanes);                                                              // cost_mma.cu
 int sm_count(int dev);                                                                                 // cost_mma.cu
 cudaError_t launch_score_grad(const BwdParams& p, cudaStream_t st);                                    // cost_f_bwd.cu
 
@@ -478,11 +483,12 @@ void f_bwd_mma_launch_info(int B, int H, int W, int* grid, int* block, int* smem
 // work-counter tickets shared by every instantiation (they share the slots of g_fbwd_next / g_fbwd_done)
 static std::atomic<unsigned> ticket{0}, graph_ticket{0};
 
-// p.ref_feat / p.src_feat point to the SPLIT16 buffers of the forward (B and V*B images); p.g_score is written
-template <class P, int MODE, bool CW>
+// p.ref_feat / p.src_feat point to the SPLIT16 (PLANES = 2) or HALF16 (PLANES = 1) buffers of the forward (B and V*B
+// images); p.g_score is written
+template <class P, int MODE, bool CW, int PLANES>
 static cudaError_t launch_bwd_mma(const P& p, cudaStream_t st) {
   static std::once_flag flags[64];
-  auto kern = cost_f_bwd_mma_kernel<P, MODE, CW>;
+  auto kern = cost_f_bwd_mma_kernel<P, MODE, CW, PLANES>;
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
@@ -496,8 +502,8 @@ static cudaError_t launch_bwd_mma(const P& p, cudaStream_t st) {
   const unsigned char* refbuf = reinterpret_cast<const unsigned char*>(p.ref_feat);
   const unsigned char* srcbuf = reinterpret_cast<const unsigned char*>(p.src_feat);
   CUtensorMap tm_ref, tm_src;
-  if ((e = make_planes_map(&tm_ref, refbuf + SPLIT16_HEADER, p.B, p.H, p.W, 8)) != cudaSuccess) return e;
-  if ((e = make_planes_map(&tm_src, srcbuf + SPLIT16_HEADER, p.B * p.V, p.H, p.W, 1)) != cudaSuccess) return e;
+  if ((e = make_planes_map(&tm_ref, refbuf + SPLIT16_HEADER, p.B, p.H, p.W, 8, PLANES)) != cudaSuccess) return e;
+  if ((e = make_planes_map(&tm_src, srcbuf + SPLIT16_HEADER, p.B * p.V, p.H, p.W, 1, PLANES)) != cudaSuccess) return e;
   const int n_items = ((p.W + BTW - 1) / BTW) * ((p.H + BTH - 1) / BTH) * p.B;
   // work-counter slot: eager launches cycle through the lower half, captured launches own one of the upper half for
   // the life of their graph (cost_mma.cu)
@@ -513,18 +519,24 @@ static cudaError_t launch_bwd_mma(const P& p, cudaStream_t st) {
   return cudaGetLastError();
 }
 
-cudaError_t launch_cost_f_bwd_mma(const BwdParams& p, cudaStream_t st, int* launches) {
+// layout: MAGNET_SRC_SPLIT16 or MAGNET_SRC_HALF16, the buffers' layout
+cudaError_t launch_cost_f_bwd_mma(const BwdParams& p, int layout, cudaStream_t st, int* launches) {
   cudaError_t e = launch_score_grad(p, st);
   if (e != cudaSuccess) return e;
   *launches = 2;
-  return launch_bwd_mma<BwdParams, MAGNET_DEPTH_PLANES, false>(p, st);
+  if (layout == MAGNET_SRC_HALF16) return launch_bwd_mma<BwdParams, MAGNET_DEPTH_PLANES, false, 1>(p, st);
+  return launch_bwd_mma<BwdParams, MAGNET_DEPTH_PLANES, false, 2>(p, st);
 }
 
-// CW volume, feature gradients on the tensor cores: p.ref_feat / p.src_feat are the forward's split buffers, p.g_score
-// already holds grad_out / V (cost_cw_bwd.cu)
-cudaError_t launch_cost_cw_bwd_mma(const CwBwdParams& p, int mode, cudaStream_t st) {
-  if (mode == MAGNET_DEPTH_VOLUME) return launch_bwd_mma<CwBwdParams, MAGNET_DEPTH_VOLUME, true>(p, st);
-  return launch_bwd_mma<CwBwdParams, MAGNET_DEPTH_GAUSS, true>(p, st);
+// CW volume, feature gradients on the tensor cores: p.ref_feat / p.src_feat are the forward's split buffers (layout
+// SPLIT16 or HALF16), p.g_score already holds grad_out / V (cost_cw_bwd.cu)
+cudaError_t launch_cost_cw_bwd_mma(const CwBwdParams& p, int mode, int layout, cudaStream_t st) {
+  if (layout == MAGNET_SRC_HALF16) {
+    if (mode == MAGNET_DEPTH_VOLUME) return launch_bwd_mma<CwBwdParams, MAGNET_DEPTH_VOLUME, true, 1>(p, st);
+    return launch_bwd_mma<CwBwdParams, MAGNET_DEPTH_GAUSS, true, 1>(p, st);
+  }
+  if (mode == MAGNET_DEPTH_VOLUME) return launch_bwd_mma<CwBwdParams, MAGNET_DEPTH_VOLUME, true, 2>(p, st);
+  return launch_bwd_mma<CwBwdParams, MAGNET_DEPTH_GAUSS, true, 2>(p, st);
 }
 
 }  // namespace magnet

@@ -14,7 +14,10 @@
 //   * fp32 accuracy on fp16 tensor cores: every feature map is split once per forward into x*s = hi + lo (two fp16
 //     planes, s a power of two that maps the largest finite |x| into [2^14, 2^15)); hi*hi + hi*lo + lo*hi carries 22
 //     significant bits per factor, products are exact in the fp32 accumulator (MAGNET_SRC_SPLIT16,
-//     magnet_repack_split16_f32).
+//     magnet_repack_split16_f32).  An fp16 / bf16 map needs no lo plane: x*s is itself an fp16 number (MAGNET_SRC_HALF16,
+//     magnet_repack_half16, DESIGN §3.7), so PLANES = 1 loads one plane per box and issues the hi*hi product only (4
+//     wgmma per warpgroup); shared-memory map, descriptors (the lo atom slot is left unwritten) and everything after
+//     the MMA are those of PLANES = 2.
 //   * the planes are (image, plane, y, x, 64 channels) fp16 = 128-byte rows: an 8-pixel x 2-plane TMA box with
 //     CU_TENSOR_MAP_SWIZZLE_128B lands as one canonical K-major wgmma atom per plane; the window of a (tile, view) is the
 //     bounding box of the tile's sample positions cut into such 8-cell segments (zero fill outside the image =
@@ -39,6 +42,7 @@
 // Numerics: the per-view channel sum is the tensor core's fp32 accumulation of exact products of the split factors
 // (relative error ~2^-21 of sum |ref||src|, the same order as an fp32 FMA chain); everything else — projection, weights,
 // consistency test, view accumulation, 1/V — is the fp32 arithmetic of the other kernels (common.cuh project2).
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
 #include <algorithm>
@@ -61,6 +65,8 @@ constexpr int MSEG = 32;               // 8-cell segments per window: N <= 256 a
 constexpr int MMAXV = 16;              // views whose camera constants are staged in shared memory
 constexpr int SEG_BYTES = 2048;        // hi atom (8 cells x 128 B) + lo atom
 constexpr int META_SEG_BYTES = 128;    // 8 cells x (mu, sigma of the cell and of its right neighbour)
+constexpr uint32_t SEG_TX = 1024;      // bytes per plane of a window segment's box (PLANES planes land, 1 or 2)
+constexpr uint32_t REF_TX = 8192;      // bytes per plane of the reference tile's box
 
 // shared-memory map (bytes from the 1024-aligned base)
 constexpr int MOFF_A = 0;                                   // reference tile: hi 8 KB | lo 8 KB
@@ -87,6 +93,10 @@ static_assert(2 * (M_SMEM_TOTAL + 1024) <= 227 * 1024, "two CTAs per SM");
 // with zeros outside the row — both horizontal taps of a bilinear cell in ONE 16-byte read
 __host__ __device__ inline size_t split16_bytes(size_t N, size_t H, size_t W) {
   return SPLIT16_HEADER + N * H * W * 256 + N * H * (W + 1) * 16;
+}
+// MAGNET_SRC_HALF16: the same header and table around ONE fp16 plane (N, 1, H, W, 64) = fp16(x*s)
+__host__ __device__ inline size_t half16_bytes(size_t N, size_t H, size_t W) {
+  return SPLIT16_HEADER + N * H * W * 128 + N * H * (W + 1) * 16;
 }
 
 // work counters of the persistent kernel: one slot per launch in flight (host ticket), re-armed by the last CTA of the
@@ -123,7 +133,8 @@ enum { PROF_SETUP, PROF_BOX, PROF_TMA, PROF_MMA, PROF_PHASEC, PROF_EPI, PROF_NST
 #define MMA_STAGE(s) do { } while (0)
 #endif
 
-template <int MODE, bool CW>
+// PLANES = 2: MAGNET_SRC_SPLIT16 (hi / lo), 1: MAGNET_SRC_HALF16 (one plane, the hi*hi product only)
+template <int MODE, bool CW, int PLANES>
 __global__ void __launch_bounds__(MNT, 2)
 cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CUtensorMap tm_ref,
                 const __grid_constant__ CUtensorMap tm_src, const __grid_constant__ CUtensorMap tm_meta, const int nchunks,
@@ -390,7 +401,7 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
         const int nsegs = nseg * rows;                     // <= MSEG
         // ---------------- window + (mu, sigma) table by TMA ---------------------------------------------------
         if (tid == 0)
-          mbar_arrive_expect_tx(bar_tma, (uint32_t)nsegs * (SEG_BYTES + (CW ? META_SEG_BYTES : 0)) + (first ? 16384u : 0u));
+          mbar_arrive_expect_tx(bar_tma, (uint32_t)nsegs * (SEG_TX * PLANES + (CW ? META_SEG_BYTES : 0)) + (first ? REF_TX * PLANES : 0u));
         first = false;
         if (lane == 0) {
           for (int s = warp; s < nsegs; s += MNT / 32) {
@@ -423,15 +434,17 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
           const uint64_t b_hi = gmma_desc_sw128(bseg, SEG_BYTES), b_lo = gmma_desc_sw128(bseg + 1024, SEG_BYTES);
           __syncwarp();                                      // wgmma is warp-synchronous (.aligned)
           // ptxas (CUDA 12.9) serialises the wgmma of <GAUSS, false> when it holds the second shape (C7511, out of
-          // registers), so that instantiation keeps n128 for warpgroup 1
-          constexpr bool WG1_N64 = CW || MODE != MAGNET_DEPTH_GAUSS;
+          // registers), so that instantiation keeps n128 for warpgroup 1; so does <VOLUME, false, 1> (HALF16), where the
+          // same happens with the second shape (DESIGN §3.7)
+          constexpr bool WG1_N64 = (CW || MODE != MAGNET_DEPTH_GAUSS) && (PLANES == 2 || CW || MODE != MAGNET_DEPTH_VOLUME);
+          // (PLANES = 1: the hi*hi product alone, scale-d 0 on its first K step)
           if (wg == 0 || npad > (WG1_N64 ? 192 : 128)) {     // warpgroup-uniform: N = 128
             wgmma_fence();
 #pragma unroll
-            for (int pr = 0; pr < 3; ++pr) {                // small cross terms first
+            for (int pr = PLANES == 2 ? 0 : 2; pr < 3; ++pr) {   // small cross terms first
               const uint64_t ad = pr == 0 ? a_lo : a_hi, bd = pr == 1 ? b_lo : b_hi;
 #pragma unroll
-              for (int kk = 0; kk < 4; ++kk) wgmma_m64n128k16_f16(acc, ad + 2u * kk, bd + 2u * kk, (pr | kk) != 0);
+              for (int kk = 0; kk < 4; ++kk) wgmma_m64n128k16_f16(acc, ad + 2u * kk, bd + 2u * kk, ((PLANES == 2 ? pr : 0) | kk) != 0);
             }
             wgmma_commit();
             wgmma_wait_all();
@@ -439,10 +452,10 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
             float (&acc64)[32] = *reinterpret_cast<float (*)[32]>(acc);
             wgmma_fence();
 #pragma unroll
-            for (int pr = 0; pr < 3; ++pr) {
+            for (int pr = PLANES == 2 ? 0 : 2; pr < 3; ++pr) {
               const uint64_t ad = pr == 0 ? a_lo : a_hi, bd = pr == 1 ? b_lo : b_hi;
 #pragma unroll
-              for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_f16(acc64, ad + 2u * kk, bd + 2u * kk, (pr | kk) != 0);
+              for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_f16(acc64, ad + 2u * kk, bd + 2u * kk, ((PLANES == 2 ? pr : 0) | kk) != 0);
             }
             wgmma_commit();
             wgmma_wait_all();
@@ -468,7 +481,7 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
         if (dbg != nullptr && item == 0 && v == 0 && sy == wy0 && sx == wx0) {
           if (tid == 0) {
             dbg[0] = (float)sx; dbg[1] = (float)sy; dbg[2] = (float)nseg; dbg[3] = (float)rows; dbg[4] = (float)npad;
-            dbg[5] = (float)gp; dbg[6] = (float)v; dbg[7] = 3.0f; dbg[8] = hdr_ref->scale; dbg[9] = hdr_src->scale;
+            dbg[5] = (float)gp; dbg[6] = (float)v; dbg[7] = 2.0f * PLANES - 1.0f; dbg[8] = hdr_ref->scale; dbg[9] = hdr_src->scale;
           }
           for (int idx = tid; idx < MPX * npad; idx += MNT) dbg[16 + (idx / npad) * 256 + idx % npad] = regR[(idx / npad) * gp + idx % npad];
         }
@@ -552,7 +565,7 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
   }
 
   if (first) {                                             // no valid view: the reference-tile copy is still in flight
-    if (tid == 0) mbar_arrive_expect_tx(bar_tma, 16384u);
+    if (tid == 0) mbar_arrive_expect_tx(bar_tma, REF_TX * PLANES);
     mbar_wait_or_trap(bar_tma, ph_tma);
     ph_tma ^= 1u;
   }
@@ -623,6 +636,9 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
 // MAGNET_SRC_SPLIT16 producer: (N, 64, H, W) fp32 [+ (N, 2, H, W) Gaussians] ->
 //   header | fp16 planes (N, 2, H, W, 64): hi = fp16(x*s), lo = fp16(x*s - hi) | table (N, H, W + 1, 4), entry x + 1 =
 //   (mu[x], sigma[x], mu[x+1], sigma[x+1]), zeros outside the row
+// MAGNET_SRC_HALF16 producer: (N, 64, H, W) fp16 / bf16 -> the same header and table around ONE plane fp16(x*s): the
+// same kernels with T = __half / __nv_bfloat16 and PLANES = 1 (exact for every element above the threshold of DESIGN
+// §3.7, so the plane equals the hi plane of the fp32 split of x.float(), whose lo plane is zero)
 // ---------------------------------------------------------------------------------------------------------------
 // bits of |x|, 0 for inf / NaN: the scale is chosen from the finite values, non-finite elements poison only their own
 // products
@@ -630,16 +646,28 @@ __device__ __forceinline__ unsigned finite_abs_bits(float x) {
   const unsigned u = __float_as_uint(x) & 0x7fffffffu;
   return u >= 0x7f800000u ? 0u : u;
 }
+__device__ __forceinline__ float to_f32(float x) { return x; }
+__device__ __forceinline__ float to_f32(__half x) { return __half2float(x); }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 x) { return __bfloat162float(x); }
 
-__global__ void __launch_bounds__(256) absmax_kernel(const float4* __restrict__ x, size_t n4, const float* __restrict__ tail,
+// x: n16 16-byte vectors of T, then ntail < 16 / sizeof(T) elements at `tail`
+template <class T>
+__global__ void __launch_bounds__(256) absmax_kernel(const T* __restrict__ x, size_t n16, const T* __restrict__ tail,
                                                      int ntail, unsigned* __restrict__ out) {
   unsigned m = 0u;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
-    const float4 v = __ldg(x + i);
-    m = max(max(m, finite_abs_bits(v.x)), finite_abs_bits(v.y));
-    m = max(max(m, finite_abs_bits(v.z)), finite_abs_bits(v.w));
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n16; i += (size_t)gridDim.x * blockDim.x) {
+    if constexpr (std::is_same<T, float>::value) {
+      const float4 v = __ldg(reinterpret_cast<const float4*>(x) + i);
+      m = max(max(m, finite_abs_bits(v.x)), finite_abs_bits(v.y));
+      m = max(max(m, finite_abs_bits(v.z)), finite_abs_bits(v.w));
+    } else {                                               // 8 half-precision elements, exact in fp32
+      const uint4 r = __ldg(reinterpret_cast<const uint4*>(x) + i);
+      const T* h = reinterpret_cast<const T*>(&r);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) m = max(m, finite_abs_bits(to_f32(h[e])));
+    }
   }
-  if (blockIdx.x == 0 && (int)threadIdx.x < ntail) m = max(m, finite_abs_bits(tail[threadIdx.x]));
+  if (blockIdx.x == 0 && (int)threadIdx.x < ntail) m = max(m, finite_abs_bits(to_f32(tail[threadIdx.x])));
   m = __reduce_max_sync(0xffffffffu, m);
   if ((threadIdx.x & 31) == 0 && m != 0u) atomicMax(out, m);
 }
@@ -651,11 +679,21 @@ __device__ __forceinline__ int split16_shift(unsigned absmax_bits) {
   return max(-100, min(100, 14 - (e - 127)));
 }
 
-// One CTA per SPX pixels of one image: channel planes are read coalesced along the pixels (16-byte loads when the image
-// size allows, all of a thread's loads in flight together), transposed through shared memory, and the two fp16 planes
-// are written as contiguous 128-byte pixel rows.
-template <int SPX, bool VEC>
-__global__ void __launch_bounds__(256) split16_repack_kernel(const float* __restrict__ src, const float* __restrict__ gmm,
+// One CTA per SPX pixels of one image: channel planes are read coalesced along the pixels (16-byte loads of fp32, 8-byte
+// loads of fp16 / bf16, when the image size allows; all of a thread's loads in flight together), transposed through
+// shared memory (as fp32: exact), and the PLANES fp16 planes are written as contiguous 128-byte pixel rows.
+template <class T> __device__ __forceinline__ float4 ldg_x4(const T* p) {   // 4 consecutive elements, 4 * sizeof(T) aligned
+  if constexpr (std::is_same<T, float>::value) {
+    return __ldg(reinterpret_cast<const float4*>(p));
+  } else {
+    const uint2 r = __ldg(reinterpret_cast<const uint2*>(p));
+    const T* h = reinterpret_cast<const T*>(&r);
+    return make_float4(to_f32(h[0]), to_f32(h[1]), to_f32(h[2]), to_f32(h[3]));
+  }
+}
+
+template <class T, int PLANES, int SPX, bool VEC>
+__global__ void __launch_bounds__(256) split16_repack_kernel(const T* __restrict__ src, const float* __restrict__ gmm,
                                                              unsigned char* __restrict__ dst, int N, int HW, int W) {
   constexpr int C = 64;
   __shared__ float t[SPX * (C + 1)];
@@ -678,7 +716,7 @@ __global__ void __launch_bounds__(256) split16_repack_kernel(const float* __rest
 #pragma unroll
     for (int e = 0; e < C / CPI; ++e) {
       const int c = c0 + e * CPI, pix = p0 + 4 * q4;
-      v[e] = pix < HW ? __ldg(reinterpret_cast<const float4*>(src + (img * C + c) * HW + pix)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      v[e] = pix < HW ? ldg_x4(src + (img * C + c) * HW + pix) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
 #pragma unroll
     for (int e = 0; e < C / CPI; ++e) {
@@ -690,11 +728,11 @@ __global__ void __launch_bounds__(256) split16_repack_kernel(const float* __rest
     }
   } else {
     const int xi = threadIdx.x % SPX, cy = threadIdx.x / SPX;
-    for (int c = cy; c < C; c += 256 / SPX) t[xi * (C + 1) + c] = p0 + xi < HW ? src[(img * C + c) * HW + p0 + xi] : 0.0f;
+    for (int c = cy; c < C; c += 256 / SPX) t[xi * (C + 1) + c] = p0 + xi < HW ? to_f32(src[(img * C + c) * HW + p0 + xi]) : 0.0f;
   }
   __syncthreads();
   __half* planes = reinterpret_cast<__half*>(dst + SPLIT16_HEADER);
-  float4* meta = reinterpret_cast<float4*>(dst + SPLIT16_HEADER + (size_t)N * HW * 256);
+  float4* meta = reinterpret_cast<float4*>(dst + SPLIT16_HEADER + (size_t)N * HW * 128 * PLANES);
 #pragma unroll
   for (int itw = 0; itw < SPX * 8 / 256; ++itw) {
     const int item = itw * 256 + threadIdx.x;
@@ -705,11 +743,12 @@ __global__ void __launch_bounds__(256) split16_repack_kernel(const float* __rest
       for (int e = 0; e < 8; ++e) {
         const float v = t[pl * (C + 1) + q * 8 + e] * s;
         hi[e] = __float2half_rn(v);
-        lo[e] = __float2half_rn(v - __half2float(hi[e]));
+        if constexpr (PLANES == 2) lo[e] = __float2half_rn(v - __half2float(hi[e]));
       }
       const size_t o = (size_t)(p0 + pl) * 64 + q * 8;
-      *reinterpret_cast<uint4*>(planes + (img * 2 + 0) * (size_t)HW * 64 + o) = *reinterpret_cast<const uint4*>(hi);
-      *reinterpret_cast<uint4*>(planes + (img * 2 + 1) * (size_t)HW * 64 + o) = *reinterpret_cast<const uint4*>(lo);
+      *reinterpret_cast<uint4*>(planes + (img * PLANES + 0) * (size_t)HW * 64 + o) = *reinterpret_cast<const uint4*>(hi);
+      if constexpr (PLANES == 2)
+        *reinterpret_cast<uint4*>(planes + (img * 2 + 1) * (size_t)HW * 64 + o) = *reinterpret_cast<const uint4*>(lo);
     }
   }
   if (threadIdx.x < SPX && p0 + threadIdx.x < HW) {       // my (mu, sigma): first half of entry x + 1, second half of entry x
@@ -736,29 +775,46 @@ int sm_count(int dev) {
   return c;
 }
 
-cudaError_t launch_repack_split16(const float* src, const float* gmm, void* dst, int N, int C, int H, int W,
-                                  cudaStream_t st, int* launches) {
+// T = float: MAGNET_SRC_SPLIT16 (two planes); T = __half / __nv_bfloat16: MAGNET_SRC_HALF16 (one plane)
+template <class T>
+static cudaError_t launch_repack_planes(const T* src, const float* gmm, void* dst, int N, int C, int H, int W,
+                                       cudaStream_t st, int* launches) {
+  constexpr int PLANES = std::is_same<T, float>::value ? 2 : 1;
+  constexpr size_t VEC = 16 / sizeof(T);                   // elements per 16-byte load of the reduction
   if (C != 64) return cudaErrorInvalidValue;
   const int HW = H * W;
   const size_t n = (size_t)N * C * HW;
   cudaError_t e = cudaMemsetAsync(dst, 0, SPLIT16_HEADER, st);
   if (e != cudaSuccess) return e;
-  const size_t n4 = n / 4;
+  const size_t n16 = n / VEC;
   int dev = 0;
   if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
-  const int blocks = (int)std::min<size_t>((size_t)sm_count(dev) * 8, (n4 + 255) / 256 + 1);
-  absmax_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const float4*>(src), n4, src + n4 * 4, (int)(n - n4 * 4),
-                                        reinterpret_cast<unsigned*>(static_cast<unsigned char*>(dst) + offsetof(Split16Header, absmax)));
+  const int blocks = (int)std::min<size_t>((size_t)sm_count(dev) * 8, (n16 + 255) / 256 + 1);
+  absmax_kernel<T><<<blocks, 256, 0, st>>>(src, n16, src + n16 * VEC, (int)(n - n16 * VEC),
+                                           reinterpret_cast<unsigned*>(static_cast<unsigned char*>(dst) + offsetof(Split16Header, absmax)));
   dim3 block(256);
   if (HW % 4 == 0 && reinterpret_cast<uintptr_t>(src) % 16 == 0) {
     dim3 grid((HW + 127) / 128, N);
-    split16_repack_kernel<128, true><<<grid, block, 0, st>>>(src, gmm, static_cast<unsigned char*>(dst), N, HW, W);
+    split16_repack_kernel<T, PLANES, 128, true><<<grid, block, 0, st>>>(src, gmm, static_cast<unsigned char*>(dst), N, HW, W);
   } else {
     dim3 grid((HW + 31) / 32, N);
-    split16_repack_kernel<32, false><<<grid, block, 0, st>>>(src, gmm, static_cast<unsigned char*>(dst), N, HW, W);
+    split16_repack_kernel<T, PLANES, 32, false><<<grid, block, 0, st>>>(src, gmm, static_cast<unsigned char*>(dst), N, HW, W);
   }
   *launches = 2;
   return cudaGetLastError();
+}
+
+cudaError_t launch_repack_split16(const float* src, const float* gmm, void* dst, int N, int C, int H, int W,
+                                  cudaStream_t st, int* launches) {
+  return launch_repack_planes(src, gmm, dst, N, C, H, W, st, launches);
+}
+
+// dtype: MAGNET_DTYPE_F16 or MAGNET_DTYPE_BF16 (checked by the caller)
+cudaError_t launch_repack_half16(const void* src, int dtype, const float* gmm, void* dst, int N, int C, int H, int W,
+                                 cudaStream_t st, int* launches) {
+  if (dtype == MAGNET_DTYPE_F16)
+    return launch_repack_planes(static_cast<const __half*>(src), gmm, dst, N, C, H, W, st, launches);
+  return launch_repack_planes(static_cast<const __nv_bfloat16*>(src), gmm, dst, N, C, H, W, st, launches);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -769,15 +825,15 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn encode_tiled_fn();   // cost_tma.cu
 
-// rank-5 map over the fp16 planes: (64 channels, W, H, 2 planes, N); box = 8 pixels of one row (window segment) or an
-// 8x8 tile (reference), both planes; 128-byte swizzle = the canonical K-major wgmma layout (cost_f_bwd_mma.cu reads
+// rank-5 map over the fp16 planes: (64 channels, W, H, planes, N); box = 8 pixels of one row (window segment) or an
+// 8x8 tile (reference), every plane (2: SPLIT16 hi / lo, 1: HALF16); 128-byte swizzle = the canonical K-major wgmma layout (cost_f_bwd_mma.cu reads
 // the same boxes as MN-major operands)
-cudaError_t make_planes_map(CUtensorMap* tm, const void* planes, int N, int H, int W, int box_rows) {
+cudaError_t make_planes_map(CUtensorMap* tm, const void* planes, int N, int H, int W, int box_rows, int nplanes) {
   EncodeTiledFn enc = encode_tiled_fn();
   if (!enc) return cudaErrorNotSupported;
-  const cuuint64_t dims[5] = {64, (cuuint64_t)W, (cuuint64_t)H, 2, (cuuint64_t)N};
-  const cuuint64_t strides[4] = {128, (cuuint64_t)W * 128, (cuuint64_t)H * W * 128, (cuuint64_t)H * W * 256};
-  const cuuint32_t box[5] = {64u, 8u, (cuuint32_t)box_rows, 2u, 1u};
+  const cuuint64_t dims[5] = {64, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)nplanes, (cuuint64_t)N};
+  const cuuint64_t strides[4] = {128, (cuuint64_t)W * 128, (cuuint64_t)H * W * 128, (cuuint64_t)H * W * 128 * nplanes};
+  const cuuint32_t box[5] = {64u, 8u, (cuuint32_t)box_rows, (cuuint32_t)nplanes, 1u};
   const cuuint32_t estr[5] = {1u, 1u, 1u, 1u, 1u};
   const CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(planes), dims, strides, box, estr,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -804,10 +860,10 @@ static float* g_mma_dbg = nullptr;
 void mma_set_debug_buffer(float* p) { g_mma_dbg = p; }
 #endif
 
-template <int MODE, bool CW>
+template <int MODE, bool CW, int PLANES>
 static cudaError_t launch_mma_mw(const CostParams& p, cudaStream_t st) {
   static std::once_flag flags[64];
-  auto kern = cost_mma_kernel<MODE, CW>;
+  auto kern = cost_mma_kernel<MODE, CW, PLANES>;
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
@@ -822,9 +878,10 @@ static cudaError_t launch_mma_mw(const CostParams& p, cudaStream_t st) {
   const unsigned char* refbuf = reinterpret_cast<const unsigned char*>(p.ref_feat);
   const unsigned char* srcbuf = reinterpret_cast<const unsigned char*>(p.src_feat);
   CUtensorMap tm_ref, tm_src, tm_meta;
-  if ((e = make_planes_map(&tm_ref, refbuf + SPLIT16_HEADER, p.B, p.H, p.W, 8)) != cudaSuccess) return e;
-  if ((e = make_planes_map(&tm_src, srcbuf + SPLIT16_HEADER, N, p.H, p.W, 1)) != cudaSuccess) return e;
-  if ((e = make_meta_map(&tm_meta, srcbuf + SPLIT16_HEADER + (size_t)N * p.HW * 256, N, p.H, p.W)) != cudaSuccess) return e;
+  if ((e = make_planes_map(&tm_ref, refbuf + SPLIT16_HEADER, p.B, p.H, p.W, 8, PLANES)) != cudaSuccess) return e;
+  if ((e = make_planes_map(&tm_src, srcbuf + SPLIT16_HEADER, N, p.H, p.W, 1, PLANES)) != cudaSuccess) return e;
+  if ((e = make_meta_map(&tm_meta, srcbuf + SPLIT16_HEADER + (size_t)N * p.HW * 128 * PLANES, N, p.H, p.W)) != cudaSuccess)
+    return e;
   const int nchunks = (p.D + MCH - 1) / MCH;
   const int tiles = ((p.W + MTW - 1) / MTW) * ((p.H + MTH - 1) / MTH);
   const int n_items = tiles * nchunks * p.B;
@@ -846,7 +903,7 @@ static cudaError_t launch_mma_mw(const CostParams& p, cudaStream_t st) {
 }
 
 bool mma_supports(int C, int D, int V, int layout) {
-  return C == 64 && layout == MAGNET_SRC_SPLIT16 && D >= 1 && V <= MMAXV;
+  return C == 64 && (layout == MAGNET_SRC_SPLIT16 || layout == MAGNET_SRC_HALF16) && D >= 1 && V <= MMAXV;
 }
 
 void mma_launch_info(int B, int H, int W, int D, int* grid, int* block, int* smem) {
@@ -858,16 +915,24 @@ void mma_launch_info(int B, int H, int W, int D, int* grid, int* block, int* sme
 }
 
 size_t split16_buffer_bytes(int N, int H, int W) { return split16_bytes((size_t)N, (size_t)H, (size_t)W); }
+size_t half16_buffer_bytes(int N, int H, int W) { return half16_bytes((size_t)N, (size_t)H, (size_t)W); }
 
-cudaError_t launch_cost_mma(const CostParams& p, int mode, bool cw, cudaStream_t st) {
+template <int PLANES>
+static cudaError_t launch_cost_mma_planes(const CostParams& p, int mode, bool cw, cudaStream_t st) {
   if (cw) {
-    if (mode == MAGNET_DEPTH_VOLUME) return launch_mma_mw<MAGNET_DEPTH_VOLUME, true>(p, st);
-    if (mode == MAGNET_DEPTH_GAUSS) return launch_mma_mw<MAGNET_DEPTH_GAUSS, true>(p, st);
-    return launch_mma_mw<MAGNET_DEPTH_PLANES, true>(p, st);
+    if (mode == MAGNET_DEPTH_VOLUME) return launch_mma_mw<MAGNET_DEPTH_VOLUME, true, PLANES>(p, st);
+    if (mode == MAGNET_DEPTH_GAUSS) return launch_mma_mw<MAGNET_DEPTH_GAUSS, true, PLANES>(p, st);
+    return launch_mma_mw<MAGNET_DEPTH_PLANES, true, PLANES>(p, st);
   }
-  if (mode == MAGNET_DEPTH_VOLUME) return launch_mma_mw<MAGNET_DEPTH_VOLUME, false>(p, st);
-  if (mode == MAGNET_DEPTH_GAUSS) return launch_mma_mw<MAGNET_DEPTH_GAUSS, false>(p, st);
-  return launch_mma_mw<MAGNET_DEPTH_PLANES, false>(p, st);
+  if (mode == MAGNET_DEPTH_VOLUME) return launch_mma_mw<MAGNET_DEPTH_VOLUME, false, PLANES>(p, st);
+  if (mode == MAGNET_DEPTH_GAUSS) return launch_mma_mw<MAGNET_DEPTH_GAUSS, false, PLANES>(p, st);
+  return launch_mma_mw<MAGNET_DEPTH_PLANES, false, PLANES>(p, st);
+}
+
+// layout: MAGNET_SRC_SPLIT16 (hi / lo planes) or MAGNET_SRC_HALF16 (one plane)
+cudaError_t launch_cost_mma(const CostParams& p, int mode, bool cw, int layout, cudaStream_t st) {
+  if (layout == MAGNET_SRC_HALF16) return launch_cost_mma_planes<1>(p, mode, cw, st);
+  return launch_cost_mma_planes<2>(p, mode, cw, st);
 }
 
 }  // namespace magnet

@@ -13,7 +13,9 @@ per-(batch, view) Python loop):
     ``magnet_pack_cameras_f32`` with their strides, no copy;
   * ``nghbr_feat`` / ``nghbr_gmms`` / ``ref_feat`` arrive NCHW: split once per forward into the fp16 hi/lo planes the
     tensor-core kernel's TMA boxes fetch (C == 64; else the pixel-major PIXC layout of the TMA-staged CUDA-core kernel;
-    cached the same way; bypassed under CUDA-graph capture).
+    cached the same way; bypassed under CUDA-graph capture).  fp16 / bf16 maps (torch.autocast) of one dtype go
+    to the single-plane HALF16 layout where SPLIT16 would be used; in every other case they are upcast to fp32
+    once (cached) and take the fp32 rules.  Volumes are fp32, gradients come back in each input's dtype.
 Both volumes are differentiable as in the reference: the CW volume w.r.t. both feature maps and the depth volume
 (magnet_cost_volume_bwd_f32; built only when grad mode is on and one of them requires grad, so that G-Net training,
 where none does, runs exactly the no-grad path), the F volume w.r.t. both feature maps (magnet_cost_volume_f_bwd_f32)
@@ -131,6 +133,23 @@ def _wants_split16(C: int, V: int, variant: int, D: int) -> bool:
     return variant == _lib.VARIANT_AUTO and C == 64 and V <= 16 and D >= MMA_MIN_PLANES
 
 
+def wants_half16(ref_dtype, src_dtype, C: int, V: int, variant: int, D: int) -> bool:
+    """The dispatch rule of half-precision feature maps: the single-plane HALF16 layout when both maps have the same
+    half dtype and the SPLIT16 conditions hold; otherwise (False) both maps are upcast and today's fp32 rules apply."""
+    return ref_dtype == src_dtype and ref_dtype in ops.HALF_DTYPES and _wants_split16(C, V, variant, D)
+
+
+def _f32(x):
+    """x as an fp32 tensor: x itself when it is fp32 (the same object, so that caches keyed on it still hit), else a
+    detached upcast cached on x (once per forward)."""
+    if x.dtype == torch.float32:
+        return x
+    hit = _cache.get("f32", (x,))
+    if hit is None:
+        hit = _cache.put("f32", (x,), x.detach().float())
+    return hit
+
+
 def _wants_pixc(C: int, V: int, variant: int) -> bool:
     return variant in (_lib.VARIANT_AUTO, _lib.VARIANT_TMA) and C in (16, 32, 64) and V <= 16
 
@@ -139,8 +158,22 @@ def _packed_source(nghbr_feat, nghbr_gmms, V, variant, ref_feat=None, D=MMA_MIN_
     """The source maps in the layout the selected kernel reads, repacked once per forward (cached on the caller's
     tensor objects): SPLIT16 (fp16 hi/lo planes + Gaussian table, also of the reference features) for the tensor-core
     production kernel (C == 64 and at least MMA_MIN_PLANES hypotheses), PIXC (features + Gaussians, pixel-major) for the TMA-staged CUDA-core kernel, TILED32 for the
-    global-gather kernels, NCHW when the channel count fits none.  Returns (source, layout, reference split or None)."""
+    global-gather kernels, NCHW when the channel count fits none.  Half-precision maps: HALF16 by ``wants_half16``,
+    else upcast.  Returns (source, layout, reference split or None)."""
     C = nghbr_feat.shape[1]
+    if ref_feat is not None and wants_half16(ref_feat.dtype, nghbr_feat.dtype, C, V, variant, D):
+        src = (nghbr_feat,) if nghbr_gmms is None else (nghbr_feat, nghbr_gmms)
+        hit = _cache.get("half16", src)
+        if hit is None:
+            hit = _cache.put("half16", src, ops.repack_half16(nghbr_feat.detach(),
+                                                              None if nghbr_gmms is None else _f32(nghbr_gmms)))
+        ref = _cache.get("half16ref", (ref_feat,))
+        if ref is None:
+            ref = _cache.put("half16ref", (ref_feat,), ops.repack_half16(ref_feat.detach()))
+        return hit, _lib.SRC_HALF16, ref
+    nghbr_feat = _f32(nghbr_feat)
+    nghbr_gmms = None if nghbr_gmms is None else _f32(nghbr_gmms)
+    ref_feat = None if ref_feat is None else _f32(ref_feat)
     if _wants_split16(C, V, variant, D) and ref_feat is not None:
         src = (nghbr_feat,) if nghbr_gmms is None else (nghbr_feat, nghbr_gmms)
         hit = _cache.get("split16", src)
@@ -202,27 +235,33 @@ class _CostVolumeCW(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out):
-        depth, ref, src, gmm = ctx.saved_tensors
+        depth, ref_in, src_in, gmm = ctx.saved_tensors
         rays, cams, V, kappa, karr = ctx.spec
         need_d, need_ref, need_src = ctx.needs_input_grad[:3]
+        # the CUDA-core kernel reads fp32 NCHW maps: always after a non-HALF16 forward, for the depth gradient after one
+        upcast = need_d or ctx.fwd[0] != _lib.SRC_HALF16
+        ref, src = (ref_in.float(), src_in.float()) if upcast else (ref_in, src_in)
         g_ref, g_src, g_d = ops.cost_volume_bwd(
-            ref, src, gmm, rays, cams, grad_out.contiguous(), V=V, kappa=kappa,
+            ref, src, gmm.float(), rays, cams, grad_out.contiguous(), V=V, kappa=kappa,
             d_volume=depth if karr is None else None, ref_gmm=depth if karr is not None else None, k=karr,
             fwd_layout=ctx.fwd[0], fwd_variant=ctx.fwd[1], need_ref=need_ref, need_src=need_src, need_depth=need_d,
             ref_split=ctx.splits[0], src_split=ctx.splits[1])
+        g_ref = None if g_ref is None else g_ref.to(ref_in.dtype)
+        g_src = None if g_src is None else g_src.to(src_in.dtype)
         return g_d, g_ref, g_src, None, None, None
 
 
-def differentiable_layout(C: int, V: int, D: int, variant: int, split16_ok: bool = True) -> int:
+def differentiable_layout(C: int, V: int, D: int, variant: int, split16_ok: bool = True, half=False) -> int:
     """Source layout of a differentiable CW forward: SPLIT16 (tensor cores) where the no-grad path would use it, else
-    NCHW with the DIRECT kernel — the two forward kernels whose consistency mask the backward reproduces."""
+    NCHW with the DIRECT kernel — the two forward kernels whose consistency mask the backward reproduces.  ``half``:
+    both feature maps have one half dtype, so HALF16 replaces SPLIT16 (wants_half16)."""
     if variant not in (_lib.VARIANT_AUTO, _lib.VARIANT_MMA, _lib.VARIANT_DIRECT):
         raise _lib.MagnetError("a differentiable CW volume runs on the tensor-core or the DIRECT kernel (variant AUTO, MMA "
                                f"or DIRECT), got variant {variant}")
     if C > 64:
         raise _lib.MagnetError(f"the CW backward supports C <= 64 channels, got C={C}")
     if split16_ok and _wants_split16(C, V, variant, D):
-        return _lib.SRC_SPLIT16
+        return _lib.SRC_HALF16 if half else _lib.SRC_SPLIT16
     if variant == _lib.VARIANT_MMA:
         raise _lib.MagnetError(f"MAGNET_VARIANT_MMA needs C == 64 and V <= 16, got C={C}, V={V}")
     return _lib.SRC_NCHW
@@ -237,28 +276,32 @@ def est_costvolume_CW(d_volume, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms,
     views; is_valid (B,V) int CPU or device; cam_intrins dict of 'intM' (B,3,3) and
     'unit_ray_array_2D' (B,3,H*W), CPU or device; thres int.  Returns (B,D,H,W) float32 on
     ref_feat.device, freshly allocated.  Differentiable, as the reference, in d_volume, ref_feat and nghbr_feat when
-    grad mode is on and one of them requires grad (the camera tensors must not require grad); detached otherwise."""
+    grad mode is on and one of them requires grad (the camera tensors must not require grad); detached otherwise.
+    Any of the tensors may be fp16 / bf16 (torch.autocast): the volume is fp32, each gradient has its input's dtype."""
     device = ref_feat.device
     B = d_volume.shape[0]
     V = int(nghbr_feat.shape[0] / B)
     if torch.is_grad_enabled():
         check_geometry_grad(R=R, t=t, intM=cam_intrins['intM'], unit_ray_array_2D=cam_intrins['unit_ray_array_2D'])
+    d_volume = d_volume.float()                            # differentiable upcast (a no-op for fp32)
     if wants_cw_grad(d_volume, ref_feat, nghbr_feat):
         D, C = int(d_volume.shape[1]), int(ref_feat.shape[1])
-        layout = differentiable_layout(C, V, D, variant)
+        half = wants_half16(ref_feat.dtype, nghbr_feat.dtype, C, V, variant, D)
+        layout = differentiable_layout(C, V, D, variant, half=half)
         _, rays_d = _device_intrinsics(cam_intrins, device)
         cams = _camera_table(cam_intrins, R, t, is_valid, device)
 
         def run():
-            if layout == _lib.SRC_SPLIT16:
+            if layout in ops.PACKED_LAYOUTS:
                 src, _, ref_split = _packed_source(nghbr_feat, nghbr_gmms, V, variant, ref_feat, D)
                 fv = variant
             else:
-                src, ref_split, fv = nghbr_feat.detach().contiguous(), None, _lib.VARIANT_DIRECT
-            out = ops.cost_volume(ref_feat.detach(), src, rays_d, cams, V=V, src_layout=layout, consistency=True,
-                                  src_gmm=nghbr_gmms.detach(), kappa=float(thres), d_volume=d_volume.detach(),
+                src, ref_split, fv = _f32(nghbr_feat).detach().contiguous(), None, _lib.VARIANT_DIRECT
+            ref = (ref_feat if layout == _lib.SRC_HALF16 else _f32(ref_feat)).detach()
+            out = ops.cost_volume(ref, src, rays_d, cams, V=V, src_layout=layout, consistency=True,
+                                  src_gmm=_f32(nghbr_gmms).detach(), kappa=float(thres), d_volume=d_volume.detach(),
                                   variant=fv, ref_split=ref_split)
-            return out, layout, fv, (ref_split, src) if layout == _lib.SRC_SPLIT16 else None
+            return out, layout, fv, (ref_split, src) if layout in ops.PACKED_LAYOUTS else None
 
         return _CostVolumeCW.apply(d_volume, ref_feat, nghbr_feat, nghbr_gmms, run,
                                    (rays_d, cams, V, float(thres), None))
@@ -266,8 +309,9 @@ def est_costvolume_CW(d_volume, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms,
         _, rays_d = _device_intrinsics(cam_intrins, device)
         cams = _camera_table(cam_intrins, R, t, is_valid, device)
         src, layout, ref_split = _packed_source(nghbr_feat, nghbr_gmms, V, variant, ref_feat, int(d_volume.shape[1]))
-        return ops.cost_volume(ref_feat.detach(), src, rays_d, cams, V=V, src_layout=layout, consistency=True,
-                               src_gmm=nghbr_gmms.detach(), kappa=float(thres), d_volume=d_volume.detach(),
+        ref = (ref_feat if layout == _lib.SRC_HALF16 else _f32(ref_feat)).detach()
+        return ops.cost_volume(ref, src, rays_d, cams, V=V, src_layout=layout, consistency=True,
+                               src_gmm=_f32(nghbr_gmms).detach(), kappa=float(thres), d_volume=d_volume.detach(),
                                variant=variant, ref_split=ref_split)
 
 
@@ -286,7 +330,8 @@ class _CostVolumeF(torch.autograd.Function):
     @staticmethod
     def forward(ctx, ref_feat, nghbr_feat, planes, rays_d, cams, V, variant):
         src, layout, ref_split = _packed_source(nghbr_feat, None, V, variant, ref_feat, len(planes))
-        out = ops.cost_volume(ref_feat.detach(), src, rays_d, cams, V=V, src_layout=layout, consistency=False,
+        ref = (ref_feat if layout == _lib.SRC_HALF16 else _f32(ref_feat)).detach()
+        out = ops.cost_volume(ref, src, rays_d, cams, V=V, src_layout=layout, consistency=False,
                               k=planes, planes=True, softmax=True, variant=variant, ref_split=ref_split)
         ctx.save_for_backward(ref_feat.detach(), nghbr_feat.detach(), out, rays_d, cams)
         ctx.planes, ctx.V = planes, V
@@ -295,9 +340,9 @@ class _CostVolumeF(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out):
         ref_feat, nghbr_feat, out, rays_d, cams = ctx.saved_tensors
-        g_ref, g_src = ops.cost_volume_f_bwd(ref_feat, nghbr_feat, rays_d, cams, ctx.planes, ctx.V, out,
+        g_ref, g_src = ops.cost_volume_f_bwd(ref_feat.float(), nghbr_feat.float(), rays_d, cams, ctx.planes, ctx.V, out,
                                              grad_out.contiguous(), softmax=True)
-        return g_ref, g_src, None, None, None, None, None
+        return g_ref.to(ref_feat.dtype), g_src.to(nghbr_feat.dtype), None, None, None, None, None
 
 
 class _PlaneSweepF(torch.autograd.Function):
@@ -309,10 +354,12 @@ class _PlaneSweepF(torch.autograd.Function):
     @staticmethod
     def forward(ctx, ref_feat, nghbr_feat, planes, rays_d, cams, V, softmax):
         src, layout, ref_split = _packed_source(nghbr_feat, None, V, _lib.VARIANT_AUTO, ref_feat, len(planes))
-        out = ops.cost_volume(ref_feat.detach(), src, rays_d, cams, V=V, src_layout=layout, consistency=False,
+        ref = (ref_feat if layout == _lib.SRC_HALF16 else _f32(ref_feat)).detach()
+        out = ops.cost_volume(ref, src, rays_d, cams, V=V, src_layout=layout, consistency=False,
                               k=planes, planes=True, softmax=softmax, ref_split=ref_split)
         ctx.save_for_backward(ref_feat.detach(), nghbr_feat.detach(), out if softmax else None, rays_d, cams)
-        ctx.splits = (ref_split, src) if layout == _lib.SRC_SPLIT16 else (None, None)
+        ctx.splits = (ref_split, src) if layout in ops.PACKED_LAYOUTS else (None, None)
+        ctx.layout = layout
         ctx.planes, ctx.V, ctx.softmax = planes, V, softmax
         return out
 
@@ -320,10 +367,14 @@ class _PlaneSweepF(torch.autograd.Function):
     def backward(ctx, grad_out):
         ref_feat, nghbr_feat, out, rays_d, cams = ctx.saved_tensors
         ref_split, src_split = ctx.splits
-        g_ref, g_src = ops.cost_volume_f_bwd(ref_feat, nghbr_feat, rays_d, cams, ctx.planes, ctx.V, out,
+        if ctx.layout == _lib.SRC_HALF16:                  # the NCHW maps only supply the shapes
+            ref, src = ref_feat, nghbr_feat
+        else:
+            ref, src = ref_feat.float(), nghbr_feat.float()
+        g_ref, g_src = ops.cost_volume_f_bwd(ref, src, rays_d, cams, ctx.planes, ctx.V, out,
                                              grad_out.contiguous(), softmax=ctx.softmax, ref_split=ref_split,
-                                             src_split=src_split)
-        return g_ref, g_src, None, None, None, None, None
+                                             src_split=src_split, split_layout=ctx.layout)
+        return g_ref.to(ref_feat.dtype), g_src.to(nghbr_feat.dtype), None, None, None, None, None
 
 
 def plane_sweep_f(d_center, ref_feat, nghbr_feat, R, t, is_valid, cam_intrins, softmax=True):

@@ -16,6 +16,7 @@ import torch.nn as nn
 from . import _lib, ops
 from .homography import (MMA_MIN_PLANES, _CostVolumeCW, check_geometry_grad, differentiable_layout,
                          wants_cw_grad)
+from .ops import HALF_DTYPES, PACKED_LAYOUTS
 from .sampling import depth_sampling
 
 
@@ -35,7 +36,8 @@ class GNET(nn.Module):
         )
 
     def forward(self, cost_volume: torch.Tensor, ref_gmm: torch.Tensor) -> torch.Tensor:
-        return ops.gaussian_update(self.gnet(cost_volume), ref_gmm)
+        # under torch.autocast the convolutions return half tensors: the update kernel reads fp32
+        return ops.gaussian_update(self.gnet(cost_volume).float(), ref_gmm.float())
 
     # --- SURVEY §8 f-3: G-Net input assembly without the per-iteration cat ------------------------------------
     # The reference concatenates [cost_volume (D ch), x_d3 (256 ch)] every iteration (MAGNET.py:167, a 197 MB copy at
@@ -57,7 +59,11 @@ class GNET(nn.Module):
 
 class MatchingPlan:
     """Everything about one batch that does not change across the N_iter iterations, prepared once:
-    device intrinsics / rays, camera-constant table, source features in the gather layout."""
+    device intrinsics / rays, camera-constant table, source features in the gather layout.
+
+    The feature maps may be fp16 / bf16 (torch.autocast).  Of one half dtype, they go to the single-plane HALF16
+    layout wherever the fp32 maps would go to SPLIT16; every other layout reads their fp32 upcast (made once).  The
+    Gaussians are upcast; volumes are fp32."""
 
     def __init__(self, ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, *,
                  thres: int = 5, src_layout: int = _lib.SRC_SPLIT16):
@@ -69,7 +75,10 @@ class MatchingPlan:
         self.V = nghbr_feat.shape[0] // self.B
         self.kappa = float(thres)
         self.ref_feat = ref_feat.detach().contiguous()
-        self.src_gmm = nghbr_gmms.detach().contiguous()
+        self.src_gmm = nghbr_gmms.detach().float().contiguous()
+        # the half dtype of both feature maps (tensor-core kernels on HALF16 buffers), or None (fp32 maps, or upcast)
+        self.half = ref_feat.dtype if ref_feat.dtype == nghbr_feat.dtype and ref_feat.dtype in HALF_DTYPES else None
+        self._f32 = {}
         self.rays = cam_intrins['unit_ray_array_2D'].to(dev, torch.float32).contiguous()
         intM = cam_intrins['intM'].to(dev, torch.float32).contiguous()
         R, t = nghbr_poses[:, :, :3, :3], nghbr_poses[:, :, :3, 3]
@@ -90,24 +99,45 @@ class MatchingPlan:
             src_layout = _lib.SRC_NCHW
         self.layout = src_layout
 
+    def _fp32(self, which: str) -> torch.Tensor:
+        """The reference ('ref') or source ('src') features in fp32: the plan's own when they are fp32, else their
+        upcast, made on first use."""
+        x = self.ref_feat if which == "ref" else self._nghbr_feat
+        if x.dtype == torch.float32:
+            return x
+        if which not in self._f32:
+            self._f32[which] = x.float()
+        return self._f32[which]
+
+    def _tc_layout(self, layout: int) -> int:
+        """The tensor-core layout the plan's maps take: HALF16 for half maps of one dtype, else SPLIT16."""
+        return _lib.SRC_HALF16 if layout == _lib.SRC_SPLIT16 and self.half is not None else layout
+
+    def _ref_operand(self, layout: int) -> torch.Tensor:
+        return self.ref_feat if layout == _lib.SRC_HALF16 else self._fp32("ref")
+
     def _source(self, layout: int):
         """Source maps in ``layout`` (built on first use; the cross-check variants read other layouts than production)."""
         if layout not in self._packed:
             if layout == _lib.SRC_PIXC:
-                self._packed[layout] = ops.repack_pixc(self._nghbr_feat, self.src_gmm)
+                self._packed[layout] = ops.repack_pixc(self._fp32("src"), self.src_gmm)
             elif layout == _lib.SRC_SPLIT16:
-                self._packed[layout] = ops.repack_split16(self._nghbr_feat, self.src_gmm)
-                self._ref_split = ops.repack_split16(self.ref_feat)
+                self._packed[layout] = ops.repack_split16(self._fp32("src"), self.src_gmm)
+                self._ref_split = ops.repack_split16(self._fp32("ref"))
+            elif layout == _lib.SRC_HALF16:
+                self._packed[layout] = ops.repack_half16(self._nghbr_feat, self.src_gmm)
+                self._ref_split = ops.repack_half16(self.ref_feat)
             elif layout == _lib.SRC_TILED32:
-                self._packed[layout] = ops.repack_tiled32(self._nghbr_feat)
+                self._packed[layout] = ops.repack_tiled32(self._fp32("src"))
             else:
-                self._packed[layout] = self._nghbr_feat.contiguous()
+                self._packed[layout] = self._fp32("src").contiguous()
         return self._packed[layout]
 
     def cost(self, gmm: torch.Tensor, k, out: Optional[torch.Tensor] = None, variant=_lib.VARIANT_AUTO):
         """Fused sampler + CW cost volume for the current Gaussian (B,2,H,W).  Differentiable in the plan's feature maps
         and in ``gmm`` when grad mode is on and one of them requires grad (then ``out`` must be None); detached
         otherwise."""
+        gmm = gmm.float()                                  # differentiable upcast (a no-op for fp32)
         if wants_cw_grad(gmm, self._ref_in, self._src_in):
             return self._cost_differentiable(gmm, k, out, variant)
         layout = self.layout
@@ -120,26 +150,29 @@ class MatchingPlan:
             layout = _lib.SRC_SPLIT16                      # the tensor-core kernel reads the fp16 hi/lo planes
         elif layout in (_lib.SRC_PIXC, _lib.SRC_SPLIT16) and variant in (_lib.VARIANT_DIRECT, _lib.VARIANT_CELLS, _lib.VARIANT_CELLS_NOREUSE):
             layout = _lib.SRC_TILED32                      # the global-gather kernels read TILED32
+        layout = self._tc_layout(layout)
         src = self._source(layout)
-        return ops.cost_volume(self.ref_feat, src, self.rays, self.cams, V=self.V, src_layout=layout,
+        return ops.cost_volume(self._ref_operand(layout), src, self.rays, self.cams, V=self.V, src_layout=layout,
                                consistency=True, src_gmm=self.src_gmm, kappa=self.kappa, ref_gmm=gmm.detach(),
                                k=k, out=out, variant=variant,
-                               ref_split=self._ref_split if layout == _lib.SRC_SPLIT16 else None)
+                               ref_split=self._ref_split if layout in PACKED_LAYOUTS else None)
 
 
     def _cost_differentiable(self, gmm, k, out, variant):
         if out is not None:
             raise _lib.MagnetError("cost(out=...) writes into a caller buffer and cannot be differentiated")
         karr = ops.k_array(k)
-        layout = differentiable_layout(self.C, self.V, len(karr), variant, split16_ok=self.layout == _lib.SRC_SPLIT16)
+        layout = differentiable_layout(self.C, self.V, len(karr), variant, split16_ok=self.layout == _lib.SRC_SPLIT16,
+                                       half=self.half is not None)
 
         def run():
-            fv = variant if layout == _lib.SRC_SPLIT16 else _lib.VARIANT_DIRECT
+            packed = layout in PACKED_LAYOUTS
+            fv = variant if packed else _lib.VARIANT_DIRECT
             src = self._source(layout)
-            vol = ops.cost_volume(self.ref_feat, src, self.rays, self.cams, V=self.V, src_layout=layout,
+            vol = ops.cost_volume(self._ref_operand(layout), src, self.rays, self.cams, V=self.V, src_layout=layout,
                                   consistency=True, src_gmm=self.src_gmm, kappa=self.kappa, ref_gmm=gmm.detach(),
-                                  k=karr, variant=fv, ref_split=self._ref_split if layout == _lib.SRC_SPLIT16 else None)
-            return vol, layout, fv, (self._ref_split, src) if layout == _lib.SRC_SPLIT16 else None
+                                  k=karr, variant=fv, ref_split=self._ref_split if packed else None)
+            return vol, layout, fv, (self._ref_split, src) if packed else None
 
         return _CostVolumeCW.apply(gmm, self._ref_in, self._src_in, self.src_gmm, run,
                                    (self.rays, self.cams, self.V, self.kappa, karr))
@@ -162,14 +195,14 @@ def matching_loop(plan: MatchingPlan, ref_gmms: torch.Tensor, x_d3: torch.Tensor
     split = isinstance(g_net_convs, GNET)
     inv = g_net_convs.invariant_part(x_d3, len(karr)) if split else None
     for _ in range(n_iter):
-        cur = preds[-1].detach()
+        cur = preds[-1].detach().float()                   # a half ref_gmms (autocast) enters the update as fp32
         if detach_cost:
             with torch.no_grad():
                 cv = plan.cost(cur, karr, variant=variant)
         else:
             cv = plan.cost(cur, karr, variant=variant)
         raw = g_net_convs.raw_from_parts(cv, inv) if split else g_net_convs(torch.cat([cv, x_d3], dim=1))
-        preds.append(ops.gaussian_update(raw, cur))
+        preds.append(ops.gaussian_update(raw.float(), cur))   # raw is half under autocast
     return preds
 
 
@@ -198,7 +231,7 @@ class MagnetHead(nn.Module):
     @staticmethod
     def upsample(depth, up_mask, k):
         """upsample_depth_via_mask (MAGNET.py:15-27) — fused kernels, no (B,2,9,k,k,H,W) temporaries (f-2)."""
-        return ops.convex_upsample(depth, up_mask, k)
+        return ops.convex_upsample(depth.float(), up_mask.float(), k)
 
     def forward(self, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins):
         preds, mask = self.forward_quarter(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid,
@@ -207,14 +240,16 @@ class MagnetHead(nn.Module):
 
     def forward_quarter(self, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins):
         """The N_iter quarter-resolution predictions and the upsampling mask, NOT upsampled: what the fused
-        upsample + NLL loss (``loss`` below) consumes during training."""
+        upsample + NLL loss (``loss`` below) consumes during training.  Under torch.autocast every input may be half;
+        the predictions and the mask are fp32."""
         plan = MatchingPlan(ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, thres=self.thres)
         preds = matching_loop(plan, ref_gmms, x_d3, self.g_net, self.n_iter, self.k_list, detach_cost=self.detach_cost)
-        return preds[1:], self.mask_head(x_d3)
+        return preds[1:], self.mask_head(x_d3).float()
 
     def loss(self, preds_quarter, mask, gt_depth, gt_depth_mask, gamma: float = 0.8):
         """MagnetLoss 'gaussian' (utils/losses.py:34-50) of the upsampled predictions without materialising them."""
-        return ops.magnet_loss(preds_quarter, mask, gt_depth, gt_depth_mask, self.downsample_ratio, gamma)
+        return ops.magnet_loss([p.float() for p in preds_quarter], mask.float(), gt_depth.float(), gt_depth_mask,
+                               self.downsample_ratio, gamma)
 
 
 class MAGNET(nn.Module):
@@ -300,6 +335,7 @@ class MagnetF(nn.Module):
         ref_feat, nghbr_feat = self._features(ref_img, nghbr_imgs)
         scores = plane_sweep_f(d_center, ref_feat, nghbr_feat, nghbr_poses[:, :, :3, :3], nghbr_poses[:, :, :3, 3],
                                is_valid, cam_intrins, softmax=False)
+        gt_dmap = gt_dmap.float()
         gt = torch.where(gt_dmap > max_depth, torch.zeros_like(gt_dmap), gt_dmap)
         gt = nn.functional.interpolate(gt, size=[scores.shape[2], scores.shape[3]], mode='nearest')
         return ops.fnet_l1_loss(scores, _plane_list(d_center), gt.contiguous(), gt > min_depth)

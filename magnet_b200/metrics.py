@@ -33,8 +33,11 @@ class DepthMetrics:
                k: Optional[int] = None) -> torch.Tensor:
         """Score one batch: ``pred_or_list`` is (a list of up to 8) full-resolution (B,2,H,W) [mu, sigma], or with
         ``up_mask`` and ``k`` the quarter-resolution Gaussians of ``MagnetHead.forward_quarter``.  Returns the (P,B,13)
-        per-image rows of ``ops.depth_metrics``."""
-        rows = ops.depth_metrics(pred_or_list, gt, min_depth=self.min_depth, max_depth=self.max_depth, crop=self.crop,
+        per-image rows of ``ops.depth_metrics``.  Half-precision predictions / masks (torch.autocast) are upcast."""
+        preds = [pred_or_list] if isinstance(pred_or_list, torch.Tensor) else list(pred_or_list)
+        pred_or_list = [p.float() for p in preds]
+        up_mask = None if up_mask is None else up_mask.float()
+        rows = ops.depth_metrics(pred_or_list, gt.float(), min_depth=self.min_depth, max_depth=self.max_depth, crop=self.crop,
                                  up_mask=up_mask, k=k)
         P, B = rows.shape[0], rows.shape[1]
         if self._acc is None:

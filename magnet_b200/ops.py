@@ -49,6 +49,38 @@ def _need_cuda_f32(name: str, x: torch.Tensor, contiguous: bool = True) -> torch
     return x
 
 
+def _need_cuda(name: str, x: torch.Tensor) -> torch.Tensor:
+    """An operand that only supplies a shape (any dtype, never read)."""
+    if not isinstance(x, torch.Tensor):
+        raise TypeError(f"{name} must be a torch.Tensor")
+    if not x.is_cuda:
+        raise _lib.MagnetError(f"{name} must be a CUDA tensor (magnet_b200 has no CPU path)")
+    return x
+
+
+# element types repack_half16 accepts
+HALF_DTYPES = {torch.float16: _lib.DTYPE_F16, torch.bfloat16: _lib.DTYPE_BF16}
+PACKED_LAYOUTS = (_lib.SRC_SPLIT16, _lib.SRC_HALF16)
+
+
+def packed_bytes(layout: int, N: int, H: int, W: int) -> int:
+    """Bytes of a SPLIT16 / HALF16 buffer of N images of H x W."""
+    fn = lib().magnet_split16_bytes if layout == _lib.SRC_SPLIT16 else lib().magnet_half16_bytes
+    return int(fn(N, H, W))
+
+
+def _check_packed(name: str, buf, layout: int, N: int, H: int, W: int) -> None:
+    """A SPLIT16 / HALF16 buffer of N images: uint8, contiguous, on the device, and exactly the layout's size (the
+    kernels cannot tell the two kinds apart, so a buffer of the other kind is refused here, before any launch)."""
+    what = "repack_split16" if layout == _lib.SRC_SPLIT16 else "repack_half16"
+    if not (isinstance(buf, torch.Tensor) and buf.is_cuda and buf.dtype == torch.uint8 and buf.is_contiguous()):
+        raise _lib.MagnetError(f"{name} must be a contiguous uint8 CUDA buffer from {what}")
+    nbytes = packed_bytes(layout, N, H, W)
+    if buf.numel() != nbytes:
+        raise _lib.MagnetError(f"{name} must be a {what} buffer of {N} images of {H}x{W} ({nbytes} bytes), got "
+                               f"{buf.numel()} bytes")
+
+
 def k_array(k: Sequence[float]):
     """Python / numpy / tensor sequence -> host float[D] (rounded to fp32 like torch does for
     tensor * python-scalar, MAGNET.py:155)."""
@@ -135,6 +167,38 @@ def repack_split16(x: torch.Tensor, gmm: Optional[torch.Tensor] = None, out: Opt
     return out
 
 
+def repack_half16(x: torch.Tensor, gmm: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """(N,64,H,W) fp16 / bf16 features [+ (N,2,H,W) fp32 Gaussians] -> HALF16 buffer (uint8): the header and table of
+    ``repack_split16(x.float(), gmm)`` around ONE fp16 plane (N,1,H,W,64) = its hi plane (its lo plane is zero for
+    every element above the threshold of DESIGN §3.7).  Read by the tensor-core kernels with ``src_layout=SRC_HALF16``."""
+    if not isinstance(x, torch.Tensor):
+        raise TypeError("x must be a torch.Tensor")
+    if not x.is_cuda:
+        raise _lib.MagnetError("x must be a CUDA tensor (magnet_b200 has no CPU path)")
+    if x.dtype not in HALF_DTYPES:
+        raise _lib.MagnetError(f"x must be float16 or bfloat16 (repack_split16 takes float32), got {x.dtype}")
+    if x.dim() != 4:
+        raise _lib.MagnetError(f"x must be (N,64,H,W), got {tuple(x.shape)}")
+    x = x.contiguous()
+    N, Cc, H, W = x.shape
+    gptr = None
+    if gmm is not None:
+        gmm = _need_cuda_f32("gmm", gmm)
+        if tuple(gmm.shape) != (N, 2, H, W):
+            raise _lib.MagnetError(f"gmm must be (N,2,H,W) = {(N, 2, H, W)}, got {tuple(gmm.shape)}")
+        gptr = gmm.data_ptr()
+    nbytes = int(lib().magnet_half16_bytes(N, H, W))
+    if out is None:
+        out = torch.empty(nbytes, device=x.device, dtype=torch.uint8)
+    elif out.numel() * out.element_size() < nbytes or out.device != x.device:
+        raise _lib.MagnetError(f"out must hold {nbytes} bytes on {x.device}")
+    _same_device(("x", x), ("gmm", gmm))
+    with torch.cuda.device(x.device):
+        check(lib().magnet_repack_half16(x.data_ptr(), HALF_DTYPES[x.dtype], gptr, out.data_ptr(), N, Cc, H, W,
+                                         _stream(x.device)), "magnet_repack_half16")
+    return out
+
+
 def sample_depths(gmm: torch.Tensor, k, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Sampler alone (MAGNET.py:154-156): gmm (B,2,H,W) -> d_volume (B,D,H,W)."""
     gmm = _need_cuda_f32("gmm", gmm)
@@ -157,13 +221,10 @@ def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tens
                 ref_split: Optional[torch.Tensor] = None) -> torch.Tensor:
     """One launch of magnet_cost_volume_f32.  Depth source: ``d_volume`` (drop-in), or ``ref_gmm`` + ``k``
     (fused sampler), or ``k`` with ``planes=True`` (fronto-parallel planes).  With ``src_layout=SRC_SPLIT16`` both
-    ``src_feat`` and ``ref_split`` are ``repack_split16`` buffers (``ref_feat`` then only supplies the shape)."""
-    ref_feat = _need_cuda_f32("ref_feat", ref_feat)
-    if src_layout == _lib.SRC_SPLIT16:
-        for nm, buf in (("src_feat", src_feat), ("ref_split", ref_split)):
-            if not (isinstance(buf, torch.Tensor) and buf.is_cuda and buf.dtype == torch.uint8 and buf.is_contiguous()):
-                raise _lib.MagnetError(f"{nm} must be a contiguous uint8 CUDA buffer from repack_split16")
-    else:
+    ``src_feat`` and ``ref_split`` are ``repack_split16`` buffers (``ref_feat`` then only supplies the shape); with
+    ``SRC_HALF16`` both are ``repack_half16`` buffers and ``ref_feat`` (any dtype) only supplies the shape."""
+    ref_feat = _need_cuda("ref_feat", ref_feat) if src_layout == _lib.SRC_HALF16 else _need_cuda_f32("ref_feat", ref_feat)
+    if src_layout not in PACKED_LAYOUTS:                   # the packed buffers are checked below, by their size
         src_feat = _need_cuda_f32("src_feat", src_feat)
     rays = _need_cuda_f32("rays", rays)
     cams = _need_cuda_f32("cams", cams)
@@ -174,13 +235,14 @@ def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tens
         raise _lib.MagnetError(f"V must be positive, got {V}")
     # every operand against (B, V, D, C, H, W): a mismatch would read out of bounds, the reference raises instead
     src_shape = {_lib.SRC_NCHW: (V * B, Cc, H, W), _lib.SRC_TILED32: (V * B, H, (W + 31) // 32, Cc // 4, 32, 4),
-                 _lib.SRC_PIXC: (V * B, H, W, Cc + 4),
-                 _lib.SRC_SPLIT16: (int(lib().magnet_split16_bytes(V * B, H, W)),)}.get(src_layout)
-    if src_shape is None:
+                 _lib.SRC_PIXC: (V * B, H, W, Cc + 4)}.get(src_layout)
+    if src_layout in PACKED_LAYOUTS:
+        _check_packed("src_feat", src_feat, src_layout, V * B, H, W)
+        _check_packed("ref_split", ref_split, src_layout, B, H, W)
+    elif src_shape is None:
         raise _lib.MagnetError(f"unknown src_layout {src_layout}")
-    _expect("src_feat", src_feat, src_shape)
-    if src_layout == _lib.SRC_SPLIT16:
-        _expect("ref_split", ref_split, (int(lib().magnet_split16_bytes(B, H, W)),))
+    else:
+        _expect("src_feat", src_feat, src_shape)
     _expect("rays", rays, (B, 3, H * W))
     if cams.numel() != B * V * 16:
         raise _lib.MagnetError(f"cams must hold B*V = {B * V} camera records of 16 floats, got {tuple(cams.shape)}")
@@ -196,10 +258,10 @@ def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tens
     a.kappa = float(kappa)
     a.ref_feat, a.src_feat, a.rays, a.cams = ref_feat.data_ptr(), src_feat.data_ptr(), rays.data_ptr(), cams.data_ptr()
     keep = [ref_feat, src_feat, rays, cams]
-    if src_layout == _lib.SRC_SPLIT16:
+    if src_layout in PACKED_LAYOUTS:
         a.ref_feat = ref_split.data_ptr()
         keep.append(ref_split)
-    if consistency and src_layout not in (_lib.SRC_PIXC, _lib.SRC_SPLIT16):   # those carry the source Gaussians inside src_feat
+    if consistency and src_layout not in (_lib.SRC_PIXC, *PACKED_LAYOUTS):   # those carry the source Gaussians inside src_feat
         src_gmm = _need_cuda_f32("src_gmm", src_gmm)
         _expect("src_gmm", src_gmm, (V * B, 2, H, W))
         a.src_gmm = src_gmm.data_ptr()
@@ -234,15 +296,20 @@ def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tens
 
 
 def cost_volume_f_bwd(ref_feat, src_feat_nchw, rays, cams, planes, V, prob, grad_out, softmax=True,
-                      ref_split=None, src_split=None):
+                      ref_split=None, src_split=None, split_layout=_lib.SRC_SPLIT16):
     """Gradients of the plane-sweep volume w.r.t. (ref_feat, src_feat) — one magnet_cost_volume_f_bwd_f32 call.
     src_feat_nchw (V*B,C,H,W) view-major; prob = forward output (read only when ``softmax``); grad_out = gradient w.r.t.
     the forward output (the probabilities, or the 1/V-averaged scores with ``softmax=False``).  Returns (grad_ref,
     grad_src) in NCHW.  With ``ref_split`` / ``src_split`` — the repack_split16 buffers the forward read (C == 64,
     V <= 16) — the tensor-core kernel computes both gradients and the NCHW maps only supply the shapes; without them
-    the CUDA-core kernel reads the NCHW maps (C in {8, 16, 32, 64})."""
-    ref_feat = _need_cuda_f32("ref_feat", ref_feat)
-    src = _need_cuda_f32("src_feat", src_feat_nchw)
+    the CUDA-core kernel reads the NCHW maps (C in {8, 16, 32, 64}).  ``split_layout=SRC_HALF16``: the buffers are
+    repack_half16 buffers, and the NCHW maps (any dtype) only supply the shapes.  The gradients are float32."""
+    split = ref_split is not None or src_split is not None
+    if split and split_layout not in PACKED_LAYOUTS:
+        raise _lib.MagnetError(f"split_layout must be SRC_SPLIT16 or SRC_HALF16, got {split_layout}")
+    shape_only = split and split_layout == _lib.SRC_HALF16
+    ref_feat = _need_cuda("ref_feat", ref_feat) if shape_only else _need_cuda_f32("ref_feat", ref_feat)
+    src = _need_cuda("src_feat", src_feat_nchw) if shape_only else _need_cuda_f32("src_feat", src_feat_nchw)
     rays = _need_cuda_f32("rays", rays)
     cams = _need_cuda_f32("cams", cams)
     grad_out = _need_cuda_f32("grad_out", grad_out)
@@ -256,25 +323,22 @@ def cost_volume_f_bwd(ref_feat, src_feat_nchw, rays, cams, planes, V, prob, grad
         _expect("prob", prob, (B, len(karr), H, W))
     if cams.numel() != B * V * 16:
         raise _lib.MagnetError(f"cams must hold B*V = {B * V} camera records of 16 floats, got {tuple(cams.shape)}")
-    split = ref_split is not None or src_split is not None
     if split:
         for nm, buf, n in (("src_split", src_split, V * B), ("ref_split", ref_split, B)):
-            if not (isinstance(buf, torch.Tensor) and buf.is_cuda and buf.dtype == torch.uint8 and buf.is_contiguous()):
-                raise _lib.MagnetError(f"{nm} must be a contiguous uint8 CUDA buffer from repack_split16")
-            _expect(nm, buf, (int(lib().magnet_split16_bytes(n, H, W)),))
+            _check_packed(nm, buf, split_layout, n, H, W)
     dev = _same_device(("ref_feat", ref_feat), ("src_feat", src), ("rays", rays), ("cams", cams),
                        ("prob", prob if softmax else None), ("grad_out", grad_out), ("ref_split", ref_split),
                        ("src_split", src_split))
     a = CostArgs()
     a.B, a.V, a.D, a.C, a.H, a.W = B, V, len(karr), Cc, H, W
     a.depth_mode, a.consistency, a.softmax = _lib.DEPTH_PLANES, 0, 1 if softmax else 0
-    a.src_layout = _lib.SRC_SPLIT16 if split else _lib.SRC_NCHW
+    a.src_layout = split_layout if split else _lib.SRC_NCHW
     a.ref_feat, a.src_feat = (ref_split.data_ptr(), src_split.data_ptr()) if split else (ref_feat.data_ptr(), src.data_ptr())
     a.rays, a.cams = rays.data_ptr(), cams.data_ptr()
     a.k_host = C.cast(karr, C.c_void_p)
     work = torch.empty_like(grad_out)
-    g_ref = torch.empty_like(ref_feat)
-    g_src = torch.zeros_like(src)
+    g_ref = torch.empty(ref_feat.shape, device=ref_feat.device, dtype=torch.float32)
+    g_src = torch.zeros(src.shape, device=src.device, dtype=torch.float32)
     bw = _lib.CostFBwdArgs()
     bw.fwd = C.pointer(a)
     bw.prob = prob.data_ptr() if softmax else None
@@ -294,11 +358,14 @@ def cost_volume_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V: int
     the forward kernel (SRC_SPLIT16 with AUTO / MMA: tensor cores; VARIANT_DIRECT): its consistency mask is applied.
     After a SPLIT16 forward, ``ref_split`` / ``src_split`` are the repack_split16 buffers it read: both feature gradients
     then come from the tensor-core kernel on them (the NCHW maps serve the depth gradient only); without them the
-    CUDA-core kernel computes every gradient with the tensor-core forward's mask (the cross-check).
+    CUDA-core kernel computes every gradient with the tensor-core forward's mask (the cross-check).  After a HALF16
+    forward (``fwd_layout=SRC_HALF16``) the buffers are repack_half16 buffers, and without ``need_depth`` the NCHW maps
+    (any dtype) only supply the shapes; the depth gradient reads them, so they must then be float32.
     Returns (grad_ref, grad_src, grad_depth), each None when not requested; grad_depth is (B,D,H,W) w.r.t. d_volume or
-    (B,2,H,W) w.r.t. ref_gmm."""
-    ref_feat = _need_cuda_f32("ref_feat", ref_feat)
-    src = _need_cuda_f32("src_feat", src_feat)
+    (B,2,H,W) w.r.t. ref_gmm.  The gradients are float32."""
+    shape_only = fwd_layout == _lib.SRC_HALF16 and not need_depth and (ref_split is not None or src_split is not None)
+    ref_feat = _need_cuda("ref_feat", ref_feat) if shape_only else _need_cuda_f32("ref_feat", ref_feat)
+    src = _need_cuda("src_feat", src_feat) if shape_only else _need_cuda_f32("src_feat", src_feat)
     rays = _need_cuda_f32("rays", rays)
     cams = _need_cuda_f32("cams", cams)
     grad_out = _need_cuda_f32("grad_out", grad_out)
@@ -325,15 +392,14 @@ def cost_volume_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V: int
         a.depth_mode, a.D, a.ref_gmm, a.k_host = _lib.DEPTH_GAUSS, len(karr), ref_gmm.data_ptr(), C.cast(karr, C.c_void_p)
         gd_shape = (B, 2, H, W)
     _expect("grad_out", grad_out, (B, a.D, H, W))
-    if fwd_layout == _lib.SRC_SPLIT16 and (ref_split is not None or src_split is not None):
+    if fwd_layout in PACKED_LAYOUTS and (ref_split is not None or src_split is not None):
         for nm, buf, nimg in (("src_split", src_split, V * B), ("ref_split", ref_split, B)):
-            if not (isinstance(buf, torch.Tensor) and buf.is_cuda and buf.dtype == torch.uint8 and buf.is_contiguous()):
-                raise _lib.MagnetError(f"{nm} must be a contiguous uint8 CUDA buffer from repack_split16")
-            _expect(nm, buf, (int(lib().magnet_split16_bytes(nimg, H, W)),))
+            _check_packed(nm, buf, fwd_layout, nimg, H, W)
         a.ref_feat, a.src_feat = ref_split.data_ptr(), src_split.data_ptr()
     bw = _lib.CostBwdArgs()
     bw.fwd = C.pointer(a)
-    bw.ref_feat, bw.src_feat = ref_feat.data_ptr(), src.data_ptr()
+    if not shape_only:                             # the NCHW maps are read (CUDA-core kernel)
+        bw.ref_feat, bw.src_feat = ref_feat.data_ptr(), src.data_ptr()
     if consistency:
         src_gmm = _need_cuda_f32("src_gmm", src_gmm)
         _expect("src_gmm", src_gmm, (V * B, 2, H, W))
@@ -342,8 +408,8 @@ def cost_volume_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V: int
                        ("rays", rays), ("cams", cams), ("grad_out", grad_out), ("d_volume", d_volume),
                        ("ref_gmm", ref_gmm), ("ref_split", ref_split), ("src_split", src_split))
     work = torch.empty_like(grad_out)
-    g_ref = torch.empty_like(ref_feat) if need_ref else None
-    g_src = torch.zeros_like(src) if need_src else None
+    g_ref = torch.empty(ref_feat.shape, device=dev, dtype=torch.float32) if need_ref else None
+    g_src = torch.zeros(src.shape, device=dev, dtype=torch.float32) if need_src else None
     g_d = torch.empty(gd_shape, device=dev, dtype=torch.float32) if need_depth else None
     bw.grad_out, bw.workspace = grad_out.data_ptr(), work.data_ptr()
     bw.grad_ref = g_ref.data_ptr() if need_ref else None
