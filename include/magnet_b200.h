@@ -248,6 +248,39 @@ int magnet_gaussian_update_bwd_f32(const float* grad_out, const float* d_output,
                                    int32_t B, int32_t HW, float* grad_d_output, void* stream);
 
 /*
+ * G-Net head of inference, fused — replaces one iteration's G-Net and update of models/MAGNET.py:167-168 when the
+ * x_d3 half of the first convolution is hoisted out of the loop (GNET.invariant_part):
+ *   h0 = ReLU(conv3x3(cost, W0[:, :D]) + invariant),  h1 = ReLU(W1 h0 + b1),  h2 = ReLU(W2 h1 + b2),
+ *   (mu1, sigma1) = W3 h2 + b3,  then the Gaussian update of magnet_gaussian_update_fwd_f32 on prev_gmm.
+ * One kernel on the fp16 tensor cores with fp32 accuracy (SPLIT16 products, DESIGN §3.8); no 128-channel map is
+ * written.  Forward only (inference); no atomics, so results are bit-identical from run to run.
+ *
+ * magnet_gnet_pack_weights_f32 writes the weights in the kernel's layout into `packed` (magnet_gnet_weights_bytes(D)
+ * bytes, 16-byte aligned): w0_cost (128, D, 3, 3) dense = the cost-volume slice of the first convolution's weight,
+ * w1 / w2 (128, 128), b1 / b2 (128), w3 (2, 128), b3 (2).  Two kernels; once per forward (the weights do not change
+ * across the iterations).  magnet_gnet_weights_bytes returns 0 for D outside 1..MAGNET_MAX_PLANES.
+ *
+ * magnet_gnet_update_f32: a memset of scratch, the cost volume's max |x| and the fused kernel.
+ * D > MAGNET_MAX_PLANES -> MAGNET_ERR_UNSUPPORTED; cost, invariant and packed_weights 16-byte aligned.
+ */
+#define MAGNET_HIDDEN_CHANNELS 128
+#define MAGNET_GNET_SCRATCH_BYTES 16
+typedef struct magnet_gnet_args {
+  int32_t B, D, H, W;
+  const float* cost;           /* (B, D, H, W) cost volume                                                      */
+  const float* invariant;      /* (B, 128, H, W) = conv3x3(x_d3, W0[:, D:]) + b0                                */
+  const void* packed_weights;  /* magnet_gnet_pack_weights_f32 output for this D                                */
+  const float* prev_gmm;       /* (B, 2, H, W) [mu0, sigma0]                                                    */
+  void* scratch;               /* MAGNET_GNET_SCRATCH_BYTES of device scratch (the cost volume's scale)         */
+  float* out;                  /* (B, 2, H, W) updated [mu, sigma]; must not overlap the inputs                 */
+} magnet_gnet_args;
+size_t magnet_gnet_weights_bytes(int32_t D);
+int magnet_gnet_pack_weights_f32(const float* w0_cost, const float* w1, const float* b1, const float* w2,
+                                 const float* b2, const float* w3, const float* b3, int32_t D, void* packed,
+                                 void* stream);
+int magnet_gnet_update_f32(const magnet_gnet_args* args, void* stream);
+
+/*
  * Caller-side camera preparation on the device (SURVEY §8 f-4).
  * magnet_relative_poses_f32 replaces utils/utils.py:72-98 (data_preprocess): poses_out[b,v] = ext_nghbr[v,b] *
  * inv(ext_ref[b]) (ref-camera -> source-camera), is_valid_out[b,v] = 0 when either extrinsic or the product holds a

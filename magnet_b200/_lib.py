@@ -38,7 +38,10 @@ EXPORTS = (
     "magnet_upsample_nll_partials", "magnet_upsample_nll_fwd_f32", "magnet_upsample_nll_bwd_f32",
     "magnet_fnet_l1_partials", "magnet_fnet_l1_fwd_f32", "magnet_fnet_l1_bwd_f32",
     "magnet_depth_metrics_workspace", "magnet_depth_metrics_f32",
+    "magnet_gnet_weights_bytes", "magnet_gnet_pack_weights_f32", "magnet_gnet_update_f32",
 )
+MAGNET_HIDDEN_CHANNELS = 128
+MAGNET_GNET_SCRATCH_BYTES = 16
 
 
 class CostArgs(C.Structure):
@@ -73,6 +76,13 @@ class DepthMetricsArgs(C.Structure):
                 ("min_depth", C.c_float), ("max_depth", C.c_float),
                 ("pred", C.POINTER(C.c_void_p)), ("up_mask", C.c_void_p), ("gt", C.c_void_p), ("workspace", C.c_void_p),
                 ("out", C.c_void_p)]
+
+
+class GnetArgs(C.Structure):
+    """Mirror of ``struct magnet_gnet_args``."""
+    _fields_ = [("B", C.c_int32), ("D", C.c_int32), ("H", C.c_int32), ("W", C.c_int32),
+                ("cost", C.c_void_p), ("invariant", C.c_void_p), ("packed_weights", C.c_void_p), ("prev_gmm", C.c_void_p),
+                ("scratch", C.c_void_p), ("out", C.c_void_p)]
 
 
 class MagnetError(RuntimeError):
@@ -163,6 +173,12 @@ def lib() -> C.CDLL:
     L.magnet_depth_metrics_workspace.argtypes = [C.POINTER(DepthMetricsArgs)]
     L.magnet_depth_metrics_f32.restype = C.c_int
     L.magnet_depth_metrics_f32.argtypes = [C.POINTER(DepthMetricsArgs), C.c_void_p]
+    L.magnet_gnet_weights_bytes.restype = C.c_size_t
+    L.magnet_gnet_weights_bytes.argtypes = [C.c_int32]
+    L.magnet_gnet_pack_weights_f32.restype = C.c_int
+    L.magnet_gnet_pack_weights_f32.argtypes = [C.c_void_p] * 7 + [C.c_int32, C.c_void_p, C.c_void_p]
+    L.magnet_gnet_update_f32.restype = C.c_int
+    L.magnet_gnet_update_f32.argtypes = [C.POINTER(GnetArgs), C.c_void_p]
     if L.magnet_abi_version() != MAGNET_ABI_VERSION:
         raise MagnetError(f"ABI version mismatch: library {L.magnet_abi_version()} != binding {MAGNET_ABI_VERSION}")
     _lib = L

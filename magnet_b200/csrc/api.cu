@@ -69,6 +69,11 @@ size_t depth_metrics_workspace(int P, int B, int rows, int cols);
 cudaError_t launch_depth_metrics(const float* const* preds, int P, const float* up_mask, const float* gt, int B, int H,
                                  int W, int k, int r0, int r1, int c0, int c1, float min_d, float max_d,
                                  double* partial, double* out, cudaStream_t st);
+size_t gnet_weights_bytes(int D);
+cudaError_t launch_gnet_pack(const float* w0, const float* w1, const float* b1, const float* w2, const float* b2,
+                             const float* w3, const float* b3, int D, void* dst, cudaStream_t st);
+cudaError_t launch_gnet_update(int B, int D, int H, int W, const float* cost, const float* inv, const void* weights,
+                               const float* prev, unsigned* scratch, float* out, cudaStream_t st);
 }  // namespace magnet
 
 namespace {
@@ -543,6 +548,42 @@ int validate_depth_metrics_shape(const magnet_depth_metrics_args* a) {
   return MAGNET_OK;
 }
 }  // namespace
+
+size_t magnet_gnet_weights_bytes(int32_t D) {
+  if (D <= 0 || D > MAGNET_MAX_PLANES) return 0;
+  return magnet::gnet_weights_bytes(D);
+}
+
+int magnet_gnet_pack_weights_f32(const float* w0_cost, const float* w1, const float* b1, const float* w2,
+                                 const float* b2, const float* w3, const float* b3, int32_t D, void* packed,
+                                 void* stream) {
+  if (!w0_cost || !w1 || !b1 || !w2 || !b2 || !w3 || !b3 || !packed) return MAGNET_ERR_NULL;
+  if (D <= 0) return MAGNET_ERR_SHAPE;
+  if (D > MAGNET_MAX_PLANES) return MAGNET_ERR_UNSUPPORTED;
+  if (reinterpret_cast<uintptr_t>(packed) % 16 != 0) return MAGNET_ERR_ALIGN;
+  cudaError_t e = magnet::launch_gnet_pack(w0_cost, w1, b1, w2, b2, w3, b3, D, packed, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 2;
+  return MAGNET_OK;
+}
+
+int magnet_gnet_update_f32(const magnet_gnet_args* a, void* stream) {
+  if (!a) return MAGNET_ERR_NULL;
+  if (a->B <= 0 || a->D <= 0 || a->H <= 0 || a->W <= 0) return MAGNET_ERR_SHAPE;
+  if ((int64_t)a->H * a->W > (1 << 26) || (int64_t)a->B * ((a->H + 7) / 8) * ((a->W + 15) / 16) > (1 << 30))
+    return MAGNET_ERR_SHAPE;
+  if (a->D > MAGNET_MAX_PLANES) return MAGNET_ERR_UNSUPPORTED;
+  if (!a->cost || !a->invariant || !a->packed_weights || !a->prev_gmm || !a->scratch || !a->out) return MAGNET_ERR_NULL;
+  if (reinterpret_cast<uintptr_t>(a->cost) % 16 != 0 || reinterpret_cast<uintptr_t>(a->invariant) % 16 != 0 ||
+      reinterpret_cast<uintptr_t>(a->packed_weights) % 16 != 0 || reinterpret_cast<uintptr_t>(a->scratch) % 4 != 0)
+    return MAGNET_ERR_ALIGN;
+  cudaError_t e = magnet::launch_gnet_update(a->B, a->D, a->H, a->W, a->cost, a->invariant, a->packed_weights,
+                                             a->prev_gmm, static_cast<unsigned*>(a->scratch), a->out,
+                                             (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 2;
+  return MAGNET_OK;
+}
 
 int64_t magnet_depth_metrics_workspace(const magnet_depth_metrics_args* a) {
   const int st = validate_depth_metrics_shape(a);

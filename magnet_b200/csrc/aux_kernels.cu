@@ -1,5 +1,6 @@
 // Small kernels around the cost volume: camera constants, source repack, sampler, Gaussian update.
 #include "common.cuh"
+#include "gaussian_common.cuh"
 #include "upsample_common.cuh"
 
 namespace magnet {
@@ -69,7 +70,7 @@ __global__ void sample_depths_kernel(const float* __restrict__ gmm, const __grid
   for (int j = 0; j < D; ++j) o[(size_t)j * HW] = __fadd_rn(mu, __fmul_rn(sg, kp.k[j]));
 }
 
-// MAGNET.py:60,65-69.  torch's ELU evaluates exp(x) - 1 on the negative side (not expm1).
+// MAGNET.py:60,65-69 (gaussian_update, gaussian_common.cuh)
 __global__ void gaussian_update_fwd_kernel(const float* __restrict__ dout, const float* __restrict__ gmm0,
                                            int HW, float* __restrict__ out) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
@@ -77,9 +78,10 @@ __global__ void gaussian_update_fwd_kernel(const float* __restrict__ dout, const
   const size_t b = blockIdx.y;
   const float mu1 = dout[(b * 2 + 0) * HW + n], s1 = dout[(b * 2 + 1) * HW + n];
   const float mu0 = gmm0[(b * 2 + 0) * HW + n], s0 = gmm0[(b * 2 + 1) * HW + n];
-  const float elu = s1 > 0.0f ? s1 : __fsub_rn(expf(s1), 1.0f);
-  out[(b * 2 + 0) * HW + n] = __fadd_rn(mu0, __fmul_rn(mu1, s0));
-  out[(b * 2 + 1) * HW + n] = __fmul_rn(__fadd_rn(__fadd_rn(elu, 1.0f), 1e-10f), s0);
+  float mu, sg;
+  gaussian_update(mu1, s1, mu0, s0, mu, sg);
+  out[(b * 2 + 0) * HW + n] = mu;
+  out[(b * 2 + 1) * HW + n] = sg;
 }
 
 __global__ void gaussian_update_bwd_kernel(const float* __restrict__ gout, const float* __restrict__ dout,

@@ -71,6 +71,14 @@ __device__ __forceinline__ float rcp_nr(float x) {
 
 __device__ __forceinline__ float ldg_f(const float* p) { return __ldg(p); }
 
+// SPLIT16 scale rule: the power-of-two shift that maps absmax into [2^14, 2^15); 0 (scale 1) for an all-zero or
+// non-finite tensor
+__device__ __forceinline__ int split16_shift(unsigned absmax_bits) {
+  const int e = (int)(absmax_bits >> 23) & 0xff;
+  if (e == 0 || e == 255) return 0;
+  return max(-100, min(100, 14 - (e - 127)));
+}
+
 // Element-wise float2 arithmetic, each element one IEEE round-to-nearest operation (sm_90 has no packed f32x2 FMA):
 // the kernels evaluate two hypotheses / two channel partial sums side by side with these.
 __device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) {

@@ -672,13 +672,6 @@ __global__ void __launch_bounds__(256) absmax_kernel(const T* __restrict__ x, si
   if ((threadIdx.x & 31) == 0 && m != 0u) atomicMax(out, m);
 }
 
-// power-of-two scale that maps absmax into [2^14, 2^15); 1 for an all-zero or non-finite tensor
-__device__ __forceinline__ int split16_shift(unsigned absmax_bits) {
-  const int e = (int)(absmax_bits >> 23) & 0xff;
-  if (e == 0 || e == 255) return 0;
-  return max(-100, min(100, 14 - (e - 127)));
-}
-
 // One CTA per SPX pixels of one image: channel planes are read coalesced along the pixels (16-byte loads of fp32, 8-byte
 // loads of fp16 / bf16, when the image size allows; all of a thread's loads in flight together), transposed through
 // shared memory (as fp32: exact), and the PLANES fp16 planes are written as contiguous 128-byte pixel rows.
@@ -801,6 +794,18 @@ static cudaError_t launch_repack_planes(const T* src, const float* gmm, void* ds
     split16_repack_kernel<T, PLANES, 32, false><<<grid, block, 0, st>>>(src, gmm, static_cast<unsigned char*>(dst), N, HW, W);
   }
   *launches = 2;
+  return cudaGetLastError();
+}
+
+// *out = bits of the largest finite |x[i]|, i < n (x 16-byte aligned): a memset and one reduction kernel
+cudaError_t launch_absmax_f32(const float* x, size_t n, unsigned* out, cudaStream_t st) {
+  cudaError_t e = cudaMemsetAsync(out, 0, sizeof(unsigned), st);
+  if (e != cudaSuccess) return e;
+  int dev = 0;
+  if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
+  const size_t n16 = n / 4;
+  const int blocks = (int)std::min<size_t>((size_t)sm_count(dev) * 8, (n16 + 255) / 256 + 1);
+  absmax_kernel<float><<<blocks, 256, 0, st>>>(x, n16, x + n16 * 4, (int)(n - n16 * 4), out);
   return cudaGetLastError();
 }
 

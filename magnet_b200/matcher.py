@@ -4,7 +4,8 @@ the cost kernel and the Gaussian update as one kernel, prepared once per forward
 The reference inlines the sampler (MAGNET.py:154-156) and the update (inside GNET.forward, :60-69),
 so they are only reachable through this alternative loop (or the ``GNET`` mirror below); the
 cost-volume function itself is also available as a pure drop-in (``magnet_b200.homography``).
-The G-Net / mask-head convolutions stay ordinary ``nn.Module``s (cuDNN), as north_star states.
+In inference the per-iteration G-Net head and update run as one fused kernel (``fused_gnet_applies``); training,
+autocast, the hoisted x_d3 convolution and the mask head stay ordinary ``nn.Module``s (cuDNN).
 """
 from __future__ import annotations
 
@@ -189,11 +190,14 @@ def matching_loop(plan: MatchingPlan, ref_gmms: torch.Tensor, x_d3: torch.Tensor
     skipped (f-3).  Gradients flow exactly where the reference lets them: through the update into the conv
     weights, never into the cost volume (MAGNET.py:167 detaches it).  With ``detach_cost=False`` the cost volume stays
     in the graph, so feature maps that require grad (a trainable F-Net upstream) receive gradients through it; the
-    Gaussian that places the hypotheses stays detached, as in the reference (MAGNET.py:153)."""
+    Gaussian that places the hypotheses stays detached, as in the reference (MAGNET.py:153).  When nothing needs a
+    gradient (see ``fused_gnet_applies``), a ``GNET``'s head and the update of each iteration are one fused kernel, with
+    the weights packed once per call."""
     karr = ops.k_array(k)
     preds = [ref_gmms]
     split = isinstance(g_net_convs, GNET)
     inv = g_net_convs.invariant_part(x_d3, len(karr)) if split else None
+    packed = None
     for _ in range(n_iter):
         cur = preds[-1].detach().float()                   # a half ref_gmms (autocast) enters the update as fp32
         if detach_cost:
@@ -201,9 +205,31 @@ def matching_loop(plan: MatchingPlan, ref_gmms: torch.Tensor, x_d3: torch.Tensor
                 cv = plan.cost(cur, karr, variant=variant)
         else:
             cv = plan.cost(cur, karr, variant=variant)
+        if fused_gnet_applies(g_net_convs, cv, inv):
+            if packed is None:                             # the weights are read once per call
+                packed = ops.pack_gnet_weights(g_net_convs, cv.shape[1])
+            preds.append(ops.gnet_update(cv, inv, packed, cur))
+            continue
         raw = g_net_convs.raw_from_parts(cv, inv) if split else g_net_convs(torch.cat([cv, x_d3], dim=1))
         preds.append(ops.gaussian_update(raw.float(), cur))   # raw is half under autocast
     return preds
+
+
+def fused_gnet_applies(g_net_convs, cv: torch.Tensor, inv: Optional[torch.Tensor]) -> bool:
+    """Whether an iteration of ``matching_loop`` runs the fused G-Net head (``ops.gnet_update``) instead of the module
+    path (``raw_from_parts`` + ``gaussian_update``): the split data flow of a ``GNET``, nothing to differentiate (grad
+    mode off, or no requires_grad among the head's parameters, the cost volume and the invariant), no CUDA autocast,
+    fp32 weights and 1 <= D <= MAGNET_MAX_PLANES cost channels.  The fused head has no backward."""
+    if not isinstance(g_net_convs, GNET) or inv is None:
+        return False
+    params = list(g_net_convs.parameters())
+    if torch.is_grad_enabled() and (cv.requires_grad or inv.requires_grad or any(p.requires_grad for p in params)):
+        return False
+    if torch.is_autocast_enabled("cuda"):
+        return False
+    if any(p.dtype != torch.float32 for p in params) or cv.dtype != torch.float32 or inv.dtype != torch.float32:
+        return False
+    return 1 <= cv.shape[1] <= _lib.MAGNET_MAX_PLANES
 
 
 class MagnetHead(nn.Module):

@@ -468,6 +468,71 @@ def gaussian_update(d_output: torch.Tensor, ref_gmm: torch.Tensor) -> torch.Tens
     return GaussianUpdate.apply(d_output, ref_gmm)
 
 
+def gnet_weights_bytes(D: int) -> int:
+    """Bytes of the packed G-Net weights for D cost channels (0 outside 1..MAGNET_MAX_PLANES)."""
+    return int(lib().magnet_gnet_weights_bytes(int(D)))
+
+
+def pack_gnet_weights(gnet, D: int) -> torch.Tensor:
+    """The weights of a ``GNET`` (or its ``gnet`` Sequential) in the fused head's layout, for D cost channels: the
+    cost slice W0[:, :D] of the first convolution, the two 128x128 layers and the 128->2 layer, split into fp16 hi/lo
+    with one power-of-two scale per layer.  Read from the module at each call (nothing is cached).  Two launches."""
+    seq = gnet.gnet if hasattr(gnet, "gnet") else gnet
+    c0, c1, c2, c3 = seq[0], seq[2], seq[4], seq[6]
+    hid = _lib.MAGNET_HIDDEN_CHANNELS
+    if not (c0.weight.shape[0] == hid and c0.weight.shape[1] >= D and tuple(c0.weight.shape[2:]) == (3, 3)
+            and tuple(c1.weight.shape) == (hid, hid, 1, 1) and tuple(c2.weight.shape) == (hid, hid, 1, 1)
+            and tuple(c3.weight.shape) == (2, hid, 1, 1)):
+        raise _lib.MagnetError(f"not a G-Net head with {hid} hidden channels and at least {D} cost channels")
+    nbytes = gnet_weights_bytes(D)
+    if nbytes == 0:
+        raise _lib.MagnetError(f"the fused G-Net head takes 1 to {_lib.MAGNET_MAX_PLANES} cost channels, got {D}")
+    with torch.no_grad():
+        w0 = _need_cuda_f32("W0", c0.weight[:, :D])
+        ts = [w0] + [_need_cuda_f32(nm, t) for nm, t in (("W1", c1.weight), ("b1", c1.bias), ("W2", c2.weight),
+                                                         ("b2", c2.bias), ("W3", c3.weight), ("b3", c3.bias))]
+    dev = _same_device(*((f"weight {i}", t) for i, t in enumerate(ts)))
+    out = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+    with torch.cuda.device(dev):
+        check(lib().magnet_gnet_pack_weights_f32(*(t.data_ptr() for t in ts), int(D), out.data_ptr(), _stream(dev)),
+              "magnet_gnet_pack_weights_f32")
+    return out
+
+
+def gnet_update(cost: torch.Tensor, invariant: torch.Tensor, packed: torch.Tensor, prev_gmm: torch.Tensor,
+                out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """One inference iteration of the G-Net head and the Gaussian update in one fused kernel: cost (B,D,H,W),
+    invariant (B,128,H,W) = ``GNET.invariant_part(x_d3, D)``, packed = ``pack_gnet_weights(g_net, D)``, prev_gmm
+    (B,2,H,W) -> the updated (B,2,H,W) Gaussian.  Not differentiable (forward only)."""
+    cost = _need_cuda_f32("cost", cost)
+    if cost.dim() != 4:
+        raise _lib.MagnetError(f"cost must be (B,D,H,W), got {tuple(cost.shape)}")
+    B, D, H, W = cost.shape
+    invariant = _need_cuda_f32("invariant", invariant)
+    _expect("invariant", invariant, (B, _lib.MAGNET_HIDDEN_CHANNELS, H, W))
+    prev_gmm = _need_cuda_f32("prev_gmm", prev_gmm)
+    _expect("prev_gmm", prev_gmm, (B, 2, H, W))
+    nbytes = gnet_weights_bytes(D)
+    if nbytes == 0:
+        raise _lib.MagnetError(f"the fused G-Net head takes 1 to {_lib.MAGNET_MAX_PLANES} cost channels, got {D}")
+    if not (isinstance(packed, torch.Tensor) and packed.is_cuda and packed.dtype == torch.uint8
+            and packed.is_contiguous() and packed.numel() == nbytes):
+        raise _lib.MagnetError(f"packed must be a pack_gnet_weights buffer for D = {D} ({nbytes} bytes)")
+    if out is None:
+        out = torch.empty(B, 2, H, W, device=cost.device, dtype=torch.float32)
+    else:
+        out = _need_cuda_f32("out", out)
+        _expect("out", out, (B, 2, H, W))
+    dev = _same_device(("cost", cost), ("invariant", invariant), ("packed", packed), ("prev_gmm", prev_gmm), ("out", out))
+    scratch = torch.empty(_lib.MAGNET_GNET_SCRATCH_BYTES // 4, device=dev, dtype=torch.int32)
+    a = _lib.GnetArgs(B=B, D=D, H=H, W=W, cost=cost.data_ptr(), invariant=invariant.data_ptr(),
+                      packed_weights=packed.data_ptr(), prev_gmm=prev_gmm.data_ptr(), scratch=scratch.data_ptr(),
+                      out=out.data_ptr())
+    with torch.cuda.device(dev):
+        check(lib().magnet_gnet_update_f32(C.byref(a), _stream(dev)), "magnet_gnet_update_f32")
+    return out
+
+
 class ConvexUpsample(torch.autograd.Function):
     """upsample_depth_via_mask (MAGNET.py:15-27) as one kernel each way; differentiable in depth and mask."""
 
