@@ -650,36 +650,92 @@ __device__ __forceinline__ float to_f32(float x) { return x; }
 __device__ __forceinline__ float to_f32(__half x) { return __half2float(x); }
 __device__ __forceinline__ float to_f32(__nv_bfloat16 x) { return __bfloat162float(x); }
 
-// x: n16 16-byte vectors of T, then ntail < 16 / sizeof(T) elements at `tail`
-template <class T>
-__global__ void __launch_bounds__(256) absmax_kernel(const T* __restrict__ x, size_t n16, const T* __restrict__ tail,
-                                                     int ntail, unsigned* __restrict__ out) {
+template <class T> __device__ __forceinline__ unsigned finite_abs_bits16(uint4 r) {   // one 16-byte vector of T
+  const T* h = reinterpret_cast<const T*>(&r);
   unsigned m = 0u;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n16; i += (size_t)gridDim.x * blockDim.x) {
-    if constexpr (std::is_same<T, float>::value) {
-      const float4 v = __ldg(reinterpret_cast<const float4*>(x) + i);
-      m = max(max(m, finite_abs_bits(v.x)), finite_abs_bits(v.y));
-      m = max(max(m, finite_abs_bits(v.z)), finite_abs_bits(v.w));
-    } else {                                               // 8 half-precision elements, exact in fp32
-      const uint4 r = __ldg(reinterpret_cast<const uint4*>(x) + i);
-      const T* h = reinterpret_cast<const T*>(&r);
 #pragma unroll
-      for (int e = 0; e < 8; ++e) m = max(m, finite_abs_bits(to_f32(h[e])));
-    }
+  for (int e = 0; e < (int)(16 / sizeof(T)); ++e) m = max(m, finite_abs_bits(to_f32(h[e])));   // half types: exact in fp32
+  return m;
+}
+
+// Reduction slots of absmax_kernel: the running maximum and the count of finished blocks of one launch in flight (host
+// ticket, as g_mma_next / g_mma_done), re-armed by the launch's last block, so the kernel needs no memset before it and
+// a captured launch can be replayed.
+constexpr int ABSMAX_SLOTS = 1024;
+__device__ unsigned g_absmax_max[ABSMAX_SLOTS];
+__device__ unsigned g_absmax_done[ABSMAX_SLOTS];
+
+static int absmax_slot(cudaStream_t st) {                  // eager launches: lower half, captured ones: upper half
+  static std::atomic<unsigned> ticket{0}, graph_ticket{0};
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(st, &cap) != cudaSuccess) cap = cudaStreamCaptureStatusNone;
+  return cap == cudaStreamCaptureStatusActive ? ABSMAX_SLOTS / 2 + (int)(graph_ticket.fetch_add(1) % (ABSMAX_SLOTS / 2))
+                                              : (int)(ticket.fetch_add(1) % (ABSMAX_SLOTS / 2));
+}
+
+// Largest finite |x| of x: n16 16-byte vectors of T, then ntail < 16 / sizeof(T) elements at `tail`.  Grid-stride over
+// the vectors, four loads in flight per thread; one atomicMax per block into the slot, and the last block to finish
+// writes the result: HEADER = the whole 256-byte Split16Header (absmax bits, scale and 1 / scale of the SPLIT16 rule,
+// zeros) at `out`, otherwise the absmax bits alone.
+template <class T, bool HEADER>
+__global__ void __launch_bounds__(256) absmax_kernel(const T* __restrict__ x, size_t n16, const T* __restrict__ tail,
+                                                     int ntail, unsigned* __restrict__ out, int slot) {
+  constexpr int U = 4;
+  __shared__ unsigned red[8];
+  __shared__ bool last;
+  const uint4* v = reinterpret_cast<const uint4*>(x);
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned m = 0u;
+  for (; i + (U - 1) * stride < n16; i += U * stride) {
+    uint4 r[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) r[u] = __ldg(v + i + u * stride);
+#pragma unroll
+    for (int u = 0; u < U; ++u) m = max(m, finite_abs_bits16<T>(r[u]));
   }
+  for (; i < n16; i += stride) m = max(m, finite_abs_bits16<T>(__ldg(v + i)));
   if (blockIdx.x == 0 && (int)threadIdx.x < ntail) m = max(m, finite_abs_bits(to_f32(tail[threadIdx.x])));
   m = __reduce_max_sync(0xffffffffu, m);
-  if ((threadIdx.x & 31) == 0 && m != 0u) atomicMax(out, m);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < 8; ++w) m = max(m, red[w]);
+    if (m != 0u) atomicMax(&g_absmax_max[slot], m);
+    __threadfence();                                       // the maximum is visible before the block counts as done
+    last = atomicAdd(&g_absmax_done[slot], 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!last) return;
+  if (threadIdx.x == 0) {                                  // every other block's maximum is in the slot: read and re-arm
+    __threadfence();
+    red[0] = atomicExch(&g_absmax_max[slot], 0u);
+    g_absmax_done[slot] = 0u;
+  }
+  __syncthreads();
+  m = red[0];
+  if constexpr (HEADER) {
+    static_assert(sizeof(Split16Header) == 12 && SPLIT16_HEADER == 256, "header words below");
+    const int sh = split16_shift(m);
+    const unsigned word = threadIdx.x == 0 ? (unsigned)(127 + sh) << 23     // scale
+                        : threadIdx.x == 1 ? (unsigned)(127 - sh) << 23     // 1 / scale
+                        : threadIdx.x == 2 ? m : 0u;                        // absmax bits, then zeros
+    if (threadIdx.x < SPLIT16_HEADER / 4) out[threadIdx.x] = word;
+  } else if (threadIdx.x == 0) {
+    *out = m;
+  }
 }
 
 // One CTA per SPX pixels of one image: channel planes are read coalesced along the pixels (16-byte loads of fp32, 8-byte
 // loads of fp16 / bf16, when the image size allows; all of a thread's loads in flight together), transposed through
 // shared memory (as fp32: exact), and the PLANES fp16 planes are written as contiguous 128-byte pixel rows.
+// The vector loads of the map and the plane stores are evict-first in L2 (ld / st .cs): lines the kernel has re-read or
+// written do not push out the ones absmax_kernel left in L2 that it has still to re-read.
 template <class T> __device__ __forceinline__ float4 ldg_x4(const T* p) {   // 4 consecutive elements, 4 * sizeof(T) aligned
   if constexpr (std::is_same<T, float>::value) {
-    return __ldg(reinterpret_cast<const float4*>(p));
+    return __ldcs(reinterpret_cast<const float4*>(p));
   } else {
-    const uint2 r = __ldg(reinterpret_cast<const uint2*>(p));
+    const uint2 r = __ldcs(reinterpret_cast<const uint2*>(p));
     const T* h = reinterpret_cast<const T*>(&r);
     return make_float4(to_f32(h[0]), to_f32(h[1]), to_f32(h[2]), to_f32(h[3]));
   }
@@ -690,15 +746,14 @@ __global__ void __launch_bounds__(256) split16_repack_kernel(const T* __restrict
                                                              unsigned char* __restrict__ dst, int N, int HW, int W) {
   constexpr int C = 64;
   __shared__ float t[SPX * (C + 1)];
-  Split16Header* hdr = reinterpret_cast<Split16Header*>(dst);
-  const int sh = split16_shift(hdr->absmax);
-  const float s = __uint_as_float((unsigned)(127 + sh) << 23);
-  if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {
-    hdr->scale = s;
-    hdr->inv_scale = __uint_as_float((unsigned)(127 - sh) << 23);
-  }
-  const size_t img = blockIdx.y;
-  const int p0 = blockIdx.x * SPX;
+  const float s = reinterpret_cast<const Split16Header*>(dst)->scale;   // written by absmax_kernel<T, true>
+  // blocks are dispatched in blockIdx order: walk the images and pixel blocks from the end of the map back to its
+  // start, the reverse of absmax_kernel's grid stride, so the first re-reads find the lines it touched last in L2 (and
+  // image 0, which the first work items of the cost kernel read, is written last).  The kernel does not know the batch
+  // size, so the other images of the first items (v * B) get no place of their own; in a step the reference repack
+  // follows the source repack and replaces most of what the latter left in L2 anyway.
+  const size_t img = gridDim.y - 1 - blockIdx.y;
+  const int p0 = (gridDim.x - 1 - blockIdx.x) * SPX;
   if constexpr (VEC) {                                     // HW % 4 == 0, src 16-byte aligned
     static_assert(SPX == 128, "thread mapping below");
     constexpr int CPI = 8;                                 // channels per iteration
@@ -739,9 +794,9 @@ __global__ void __launch_bounds__(256) split16_repack_kernel(const T* __restrict
         if constexpr (PLANES == 2) lo[e] = __float2half_rn(v - __half2float(hi[e]));
       }
       const size_t o = (size_t)(p0 + pl) * 64 + q * 8;
-      *reinterpret_cast<uint4*>(planes + (img * PLANES + 0) * (size_t)HW * 64 + o) = *reinterpret_cast<const uint4*>(hi);
+      __stcs(reinterpret_cast<uint4*>(planes + (img * PLANES + 0) * (size_t)HW * 64 + o), *reinterpret_cast<const uint4*>(hi));
       if constexpr (PLANES == 2)
-        *reinterpret_cast<uint4*>(planes + (img * 2 + 1) * (size_t)HW * 64 + o) = *reinterpret_cast<const uint4*>(lo);
+        __stcs(reinterpret_cast<uint4*>(planes + (img * 2 + 1) * (size_t)HW * 64 + o), *reinterpret_cast<const uint4*>(lo));
     }
   }
   if (threadIdx.x < SPX && p0 + threadIdx.x < HW) {       // my (mu, sigma): first half of entry x + 1, second half of entry x
@@ -777,14 +832,13 @@ static cudaError_t launch_repack_planes(const T* src, const float* gmm, void* ds
   if (C != 64) return cudaErrorInvalidValue;
   const int HW = H * W;
   const size_t n = (size_t)N * C * HW;
-  cudaError_t e = cudaMemsetAsync(dst, 0, SPLIT16_HEADER, st);
-  if (e != cudaSuccess) return e;
   const size_t n16 = n / VEC;
   int dev = 0;
-  if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
   const int blocks = (int)std::min<size_t>((size_t)sm_count(dev) * 8, (n16 + 255) / 256 + 1);
-  absmax_kernel<T><<<blocks, 256, 0, st>>>(src, n16, src + n16 * VEC, (int)(n - n16 * VEC),
-                                           reinterpret_cast<unsigned*>(static_cast<unsigned char*>(dst) + offsetof(Split16Header, absmax)));
+  absmax_kernel<T, true><<<blocks, 256, 0, st>>>(src, n16, src + n16 * VEC, (int)(n - n16 * VEC),
+                                                 static_cast<unsigned*>(dst), absmax_slot(st));
   dim3 block(256);
   if (HW % 4 == 0 && reinterpret_cast<uintptr_t>(src) % 16 == 0) {
     dim3 grid((HW + 127) / 128, N);
@@ -797,15 +851,14 @@ static cudaError_t launch_repack_planes(const T* src, const float* gmm, void* ds
   return cudaGetLastError();
 }
 
-// *out = bits of the largest finite |x[i]|, i < n (x 16-byte aligned): a memset and one reduction kernel
+// *out = bits of the largest finite |x[i]|, i < n (x 16-byte aligned): one reduction kernel
 cudaError_t launch_absmax_f32(const float* x, size_t n, unsigned* out, cudaStream_t st) {
-  cudaError_t e = cudaMemsetAsync(out, 0, sizeof(unsigned), st);
-  if (e != cudaSuccess) return e;
   int dev = 0;
-  if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
   const size_t n16 = n / 4;
   const int blocks = (int)std::min<size_t>((size_t)sm_count(dev) * 8, (n16 + 255) / 256 + 1);
-  absmax_kernel<float><<<blocks, 256, 0, st>>>(x, n16, x + n16 * 4, (int)(n - n16 * 4), out);
+  absmax_kernel<float, false><<<blocks, 256, 0, st>>>(x, n16, x + n16 * 4, (int)(n - n16 * 4), out, absmax_slot(st));
   return cudaGetLastError();
 }
 
