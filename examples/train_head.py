@@ -41,6 +41,9 @@ def main():
     ap.add_argument("--unfused-loss", action="store_true",
                     help="materialise the N_iter upsampled (B,2,4H,4W) predictions and evaluate the NLL in torch (the "
                          "reference's data flow) instead of the fused upsample+NLL kernels (SURVEY §8 f-2)")
+    ap.add_argument("--fused-head", action="store_true",
+                    help="train the G-Net head through the fused tensor-core forward and backward (DESIGN §3.10) "
+                         "instead of the cuDNN module chain")
     args = ap.parse_args()
     rank, local_rank, world = md.env_world()
     torch.cuda.set_device(local_rank)
@@ -58,7 +61,7 @@ def main():
     mask = gt > 1e-3
 
     torch.manual_seed(0)                                                   # same init on every rank
-    head = magnet_b200.MagnetHead(n_samples=D, sampling_range=3, n_iter=3, thres=5).to(dev)
+    head = magnet_b200.MagnetHead(n_samples=D, sampling_range=3, n_iter=3, thres=5, fused_train=args.fused_head).to(dev)
     reducer = md.FlatGradAllReduce(head.parameters())
     reducer.broadcast_parameters(0)
     opt = torch.optim.AdamW(head.parameters(), lr=3.57e-4, weight_decay=1e-2)
@@ -90,6 +93,7 @@ def main():
     per_step = sorted(marks[i].elapsed_time(marks[i + 1]) for i in range(len(marks) - 1))   # device time between step starts
     if rank == 0:
         print(json.dumps({"config": "train head, ScanNet shape", "n_gpus": world, "global_batch": gb, "steps": args.steps,
+                          "head_path": "fused G-Net kernels" if args.fused_head else "cuDNN module chain",
                           "loss_path": "unfused (torch NLL on upsampled predictions)" if args.unfused_loss else "fused upsample+NLL kernels",
                           "ms_per_step": 1e3 * dt / args.steps, "frames_per_s": gb * args.steps / dt,
                           "rank0_step_ms_median": per_step[len(per_step) // 2], "rank0_step_ms_max": per_step[-1],

@@ -281,6 +281,57 @@ int magnet_gnet_pack_weights_f32(const float* w0_cost, const float* w1, const fl
 int magnet_gnet_update_f32(const magnet_gnet_args* args, void* stream);
 
 /*
+ * G-Net head of training, fused — replaces one iteration's G-Net and update of models/MAGNET.py:47-70,167-168 (split
+ * data flow, detached cost volume) and their autograd backward into the head's weights (DESIGN §3.10).
+ *
+ * magnet_gnet_pack_train_weights_f32: the inference pack of magnet_gnet_pack_weights_f32 followed by W1^T and W2^T for
+ * the backward, magnet_gnet_train_weights_bytes(D) bytes (0 for D outside 1..MAGNET_MAX_PLANES).  Three kernels.
+ *
+ * magnet_gnet_train_fwd_f32: the inference kernel's arithmetic (out is bit-identical to magnet_gnet_update_f32 on the
+ * same inputs) plus stores of h0, h1, h2 (B,128,H,W each) and the raw (mu1, sigma1) (B,2,H,W) into `saved`
+ * (magnet_gnet_saved_bytes(B,H,W) bytes).  Reads cost, invariant, packed_weights, prev_gmm; writes scratch, out, saved.
+ *
+ * magnet_gnet_bwd_f32: given grad_out = dL/d out, writes
+ *   grad_invariant (B,128,H,W) = dL/d(pre-activation of h0), which is also the gradient of conv3x3(x_d3, W0[:, D:]) + b0;
+ *   grad_w0_cost (128,D,3,3), grad_w1 / grad_w2 (128,128), grad_b1 / grad_b2 (128), grad_w3 (2,128), grad_b3 (2);
+ *   grad_prev (B,2,H,W) when not NULL.
+ * Weight / bias gradient pointers may be NULL (not computed).  No gradient into the cost volume.  Reads cost, prev_gmm,
+ * packed_weights, saved (the forward's); uses `workspace` (magnet_gnet_bwd_workspace_bytes(B,D,H,W) bytes).  Weight
+ * gradients are sums over pixels of per-CTA partials in a fixed order: bit-identical from run to run.
+ * Both calls: D > MAGNET_MAX_PLANES -> MAGNET_ERR_UNSUPPORTED; B*H*W < 2^31; cost, invariant, packed_weights, saved and
+ * workspace 16-byte aligned.
+ */
+typedef struct magnet_gnet_train_args {
+  int32_t B, D, H, W;
+  const float* cost;           /* (B, D, H, W) cost volume                                                      */
+  const float* invariant;      /* (B, 128, H, W), forward only                                                  */
+  const void* packed_weights;  /* magnet_gnet_pack_train_weights_f32 output for this D                          */
+  const float* prev_gmm;       /* (B, 2, H, W) [mu0, sigma0]                                                    */
+  void* scratch;               /* MAGNET_GNET_SCRATCH_BYTES, forward only                                       */
+  float* out;                  /* (B, 2, H, W) updated [mu, sigma], forward only                                */
+  float* saved;                /* magnet_gnet_saved_bytes(B, H, W): written by the forward, read by the backward  */
+  const float* grad_out;       /* (B, 2, H, W), backward only                                                   */
+  void* workspace;             /* magnet_gnet_bwd_workspace_bytes(B, D, H, W), backward only                    */
+  float* grad_invariant;       /* (B, 128, H, W), backward only                                                 */
+  float* grad_w0_cost;         /* (128, D, 3, 3) or NULL                                                        */
+  float* grad_w1;              /* (128, 128) or NULL                                                            */
+  float* grad_b1;              /* (128) or NULL                                                                 */
+  float* grad_w2;              /* (128, 128) or NULL                                                            */
+  float* grad_b2;              /* (128) or NULL                                                                 */
+  float* grad_w3;              /* (2, 128) or NULL                                                              */
+  float* grad_b3;              /* (2) or NULL                                                                   */
+  float* grad_prev;            /* (B, 2, H, W) or NULL                                                          */
+} magnet_gnet_train_args;
+size_t magnet_gnet_train_weights_bytes(int32_t D);
+size_t magnet_gnet_saved_bytes(int32_t B, int32_t H, int32_t W);
+size_t magnet_gnet_bwd_workspace_bytes(int32_t B, int32_t D, int32_t H, int32_t W);
+int magnet_gnet_pack_train_weights_f32(const float* w0_cost, const float* w1, const float* b1, const float* w2,
+                                       const float* b2, const float* w3, const float* b3, int32_t D, void* packed,
+                                       void* stream);
+int magnet_gnet_train_fwd_f32(const magnet_gnet_train_args* args, void* stream);
+int magnet_gnet_bwd_f32(const magnet_gnet_train_args* args, void* stream);
+
+/*
  * Caller-side camera preparation on the device (SURVEY §8 f-4).
  * magnet_relative_poses_f32 replaces utils/utils.py:72-98 (data_preprocess): poses_out[b,v] = ext_nghbr[v,b] *
  * inv(ext_ref[b]) (ref-camera -> source-camera), is_valid_out[b,v] = 0 when either extrinsic or the product holds a

@@ -39,6 +39,8 @@ EXPORTS = (
     "magnet_fnet_l1_partials", "magnet_fnet_l1_fwd_f32", "magnet_fnet_l1_bwd_f32",
     "magnet_depth_metrics_workspace", "magnet_depth_metrics_f32",
     "magnet_gnet_weights_bytes", "magnet_gnet_pack_weights_f32", "magnet_gnet_update_f32",
+    "magnet_gnet_train_weights_bytes", "magnet_gnet_saved_bytes", "magnet_gnet_bwd_workspace_bytes",
+    "magnet_gnet_pack_train_weights_f32", "magnet_gnet_train_fwd_f32", "magnet_gnet_bwd_f32",
 )
 MAGNET_HIDDEN_CHANNELS = 128
 MAGNET_GNET_SCRATCH_BYTES = 16
@@ -83,6 +85,14 @@ class GnetArgs(C.Structure):
     _fields_ = [("B", C.c_int32), ("D", C.c_int32), ("H", C.c_int32), ("W", C.c_int32),
                 ("cost", C.c_void_p), ("invariant", C.c_void_p), ("packed_weights", C.c_void_p), ("prev_gmm", C.c_void_p),
                 ("scratch", C.c_void_p), ("out", C.c_void_p)]
+
+
+class GnetTrainArgs(C.Structure):
+    """Mirror of ``struct magnet_gnet_train_args``."""
+    _fields_ = [("B", C.c_int32), ("D", C.c_int32), ("H", C.c_int32), ("W", C.c_int32)] + [
+        (n, C.c_void_p) for n in ("cost", "invariant", "packed_weights", "prev_gmm", "scratch", "out", "saved", "grad_out",
+                                  "workspace", "grad_invariant", "grad_w0_cost", "grad_w1", "grad_b1", "grad_w2", "grad_b2",
+                                  "grad_w3", "grad_b3", "grad_prev")]
 
 
 class MagnetError(RuntimeError):
@@ -179,6 +189,18 @@ def lib() -> C.CDLL:
     L.magnet_gnet_pack_weights_f32.argtypes = [C.c_void_p] * 7 + [C.c_int32, C.c_void_p, C.c_void_p]
     L.magnet_gnet_update_f32.restype = C.c_int
     L.magnet_gnet_update_f32.argtypes = [C.POINTER(GnetArgs), C.c_void_p]
+    L.magnet_gnet_train_weights_bytes.restype = C.c_size_t
+    L.magnet_gnet_train_weights_bytes.argtypes = [C.c_int32]
+    L.magnet_gnet_saved_bytes.restype = C.c_size_t
+    L.magnet_gnet_saved_bytes.argtypes = [C.c_int32] * 3
+    L.magnet_gnet_bwd_workspace_bytes.restype = C.c_size_t
+    L.magnet_gnet_bwd_workspace_bytes.argtypes = [C.c_int32] * 4
+    L.magnet_gnet_pack_train_weights_f32.restype = C.c_int
+    L.magnet_gnet_pack_train_weights_f32.argtypes = [C.c_void_p] * 7 + [C.c_int32, C.c_void_p, C.c_void_p]
+    L.magnet_gnet_train_fwd_f32.restype = C.c_int
+    L.magnet_gnet_train_fwd_f32.argtypes = [C.POINTER(GnetTrainArgs), C.c_void_p]
+    L.magnet_gnet_bwd_f32.restype = C.c_int
+    L.magnet_gnet_bwd_f32.argtypes = [C.POINTER(GnetTrainArgs), C.c_void_p]
     if L.magnet_abi_version() != MAGNET_ABI_VERSION:
         raise MagnetError(f"ABI version mismatch: library {L.magnet_abi_version()} != binding {MAGNET_ABI_VERSION}")
     _lib = L

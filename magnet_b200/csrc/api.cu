@@ -74,6 +74,17 @@ cudaError_t launch_gnet_pack(const float* w0, const float* w1, const float* b1, 
                              const float* w3, const float* b3, int D, void* dst, cudaStream_t st);
 cudaError_t launch_gnet_update(int B, int D, int H, int W, const float* cost, const float* inv, const void* weights,
                                const float* prev, unsigned* scratch, float* out, cudaStream_t st);
+size_t gnet_train_weights_bytes(int D);
+size_t gnet_saved_bytes(int B, int H, int W);
+size_t gnet_bwd_workspace_bytes(int B, int D, int H, int W);
+cudaError_t launch_gnet_pack_train(const float* w0, const float* w1, const float* b1, const float* w2, const float* b2,
+                                   const float* w3, const float* b3, int D, void* dst, cudaStream_t st);
+cudaError_t launch_gnet_train_fwd(int B, int D, int H, int W, const float* cost, const float* inv, const void* weights,
+                                  const float* prev, unsigned* scratch, float* out, float* saved, cudaStream_t st);
+cudaError_t launch_gnet_bwd(int B, int D, int H, int W, const float* cost, const float* prev, const void* weights,
+                            const float* saved, const float* grad, void* workspace, float* grad_inv, float* gw0,
+                            float* gw1, float* gb1, float* gw2, float* gb2, float* gw3, float* gb3, float* grad_prev,
+                            cudaStream_t st, int* launches);
 }  // namespace magnet
 
 namespace {
@@ -582,6 +593,77 @@ int magnet_gnet_update_f32(const magnet_gnet_args* a, void* stream) {
                                              (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e);
   g_launches += 2;
+  return MAGNET_OK;
+}
+
+namespace {
+bool misaligned16(const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 != 0; }
+
+// shape and the pointers both training calls read
+int validate_gnet_train(const magnet_gnet_train_args* a) {
+  if (!a) return MAGNET_ERR_NULL;
+  if (a->B <= 0 || a->D <= 0 || a->H <= 0 || a->W <= 0) return MAGNET_ERR_SHAPE;
+  if ((int64_t)a->H * a->W > (1 << 26) || (int64_t)a->B * a->H * a->W >= ((int64_t)1 << 31)) return MAGNET_ERR_SHAPE;
+  if (a->D > MAGNET_MAX_PLANES) return MAGNET_ERR_UNSUPPORTED;
+  if (!a->cost || !a->packed_weights || !a->prev_gmm || !a->saved) return MAGNET_ERR_NULL;
+  if (misaligned16(a->cost) || misaligned16(a->packed_weights) || misaligned16(a->saved)) return MAGNET_ERR_ALIGN;
+  return MAGNET_OK;
+}
+}  // namespace
+
+size_t magnet_gnet_train_weights_bytes(int32_t D) {
+  if (D <= 0 || D > MAGNET_MAX_PLANES) return 0;
+  return magnet::gnet_train_weights_bytes(D);
+}
+
+size_t magnet_gnet_saved_bytes(int32_t B, int32_t H, int32_t W) {
+  if (B <= 0 || H <= 0 || W <= 0) return 0;
+  return magnet::gnet_saved_bytes(B, H, W);
+}
+
+size_t magnet_gnet_bwd_workspace_bytes(int32_t B, int32_t D, int32_t H, int32_t W) {
+  if (B <= 0 || H <= 0 || W <= 0 || D <= 0 || D > MAGNET_MAX_PLANES) return 0;
+  return magnet::gnet_bwd_workspace_bytes(B, D, H, W);
+}
+
+int magnet_gnet_pack_train_weights_f32(const float* w0_cost, const float* w1, const float* b1, const float* w2,
+                                       const float* b2, const float* w3, const float* b3, int32_t D, void* packed,
+                                       void* stream) {
+  if (!w0_cost || !w1 || !b1 || !w2 || !b2 || !w3 || !b3 || !packed) return MAGNET_ERR_NULL;
+  if (D <= 0) return MAGNET_ERR_SHAPE;
+  if (D > MAGNET_MAX_PLANES) return MAGNET_ERR_UNSUPPORTED;
+  if (misaligned16(packed)) return MAGNET_ERR_ALIGN;
+  cudaError_t e = magnet::launch_gnet_pack_train(w0_cost, w1, b1, w2, b2, w3, b3, D, packed, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 3;
+  return MAGNET_OK;
+}
+
+int magnet_gnet_train_fwd_f32(const magnet_gnet_train_args* a, void* stream) {
+  const int st = validate_gnet_train(a);
+  if (st != MAGNET_OK) return st;
+  if (!a->invariant || !a->scratch || !a->out) return MAGNET_ERR_NULL;
+  if (misaligned16(a->invariant) || reinterpret_cast<uintptr_t>(a->scratch) % 4 != 0) return MAGNET_ERR_ALIGN;
+  cudaError_t e = magnet::launch_gnet_train_fwd(a->B, a->D, a->H, a->W, a->cost, a->invariant, a->packed_weights,
+                                                a->prev_gmm, static_cast<unsigned*>(a->scratch), a->out, a->saved,
+                                                (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 2;
+  return MAGNET_OK;
+}
+
+int magnet_gnet_bwd_f32(const magnet_gnet_train_args* a, void* stream) {
+  const int st = validate_gnet_train(a);
+  if (st != MAGNET_OK) return st;
+  if (!a->grad_out || !a->workspace || !a->grad_invariant) return MAGNET_ERR_NULL;
+  if (misaligned16(a->workspace)) return MAGNET_ERR_ALIGN;
+  int launches = 0;
+  cudaError_t e = magnet::launch_gnet_bwd(a->B, a->D, a->H, a->W, a->cost, a->prev_gmm, a->packed_weights, a->saved,
+                                          a->grad_out, a->workspace, a->grad_invariant, a->grad_w0_cost, a->grad_w1,
+                                          a->grad_b1, a->grad_w2, a->grad_b2, a->grad_w3, a->grad_b3, a->grad_prev,
+                                          (cudaStream_t)stream, &launches);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += launches;
   return MAGNET_OK;
 }
 

@@ -92,9 +92,10 @@ __global__ void gaussian_update_bwd_kernel(const float* __restrict__ gout, const
   const float s1 = dout[(b * 2 + 1) * HW + n];
   const float s0 = gmm0[(b * 2 + 1) * HW + n];
   const float g_mu = gout[(b * 2 + 0) * HW + n], g_sg = gout[(b * 2 + 1) * HW + n];
-  gin[(b * 2 + 0) * HW + n] = __fmul_rn(g_mu, s0);
-  const float delu = s1 > 0.0f ? 1.0f : expf(s1);
-  gin[(b * 2 + 1) * HW + n] = __fmul_rn(__fmul_rn(g_sg, delu), s0);
+  float d_mu1, d_s1;
+  gaussian_update_bwd(g_mu, g_sg, s1, s0, d_mu1, d_s1);
+  gin[(b * 2 + 0) * HW + n] = d_mu1;
+  gin[(b * 2 + 1) * HW + n] = d_s1;
 }
 
 // Learned convex upsampling (upsample_depth_via_mask, MAGNET.py:15-27) without the (B,C,9,k,k,H,W) temporaries.

@@ -58,6 +58,7 @@ struct GnetParams {
   const float* __restrict__ prev;
   const unsigned* __restrict__ absmax;
   float* __restrict__ out;
+  float* __restrict__ save;   // SAVE: h0, h1, h2 as (B,128,H,W) each, then raw (mu1, sigma1) as (B,2,H,W)
 };
 
 __device__ __forceinline__ float pow2(int e) { return __uint_as_float((unsigned)(127 + e) << 23); }   // |e| <= 126
@@ -136,6 +137,31 @@ __device__ __forceinline__ void hidden_layer(float (&acc)[NTILE][4], const uint4
   }
 }
 
+// The accumulator fragment of rows g, g+8 (pixels x, x+8 of one image row) into a (128, H, W) map: p points at channel
+// 2q of pixel x.  Pixel x+8 is only valid when x is.
+// The channel stride goes through an opaque copy: otherwise the compiler keeps the 32 channel addresses of one call
+// live for the next call, across a layer's MMAs, and spills.
+__device__ __forceinline__ int opaque(int v) {
+  int r;
+  asm volatile("mov.b32 %0, %1;" : "=r"(r) : "r"(v));
+  return r;
+}
+__device__ __forceinline__ void store_rows(float* __restrict__ p, const float (&acc)[NTILE][4], int HW, bool va, bool vb) {
+  HW = opaque(HW);
+#pragma unroll
+  for (int nt = 0; nt < NTILE; ++nt) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      float* c = p + (size_t)(nt * 8 + e) * HW;
+      if (va) c[0] = acc[nt][e];
+      if (vb) c[8] = acc[nt][2 + e];
+    }
+  }
+}
+
+// SAVE (training forward, DESIGN §3.10): the same arithmetic, plus stores of the three ReLU'd hidden maps and the raw
+// output for the backward.
+template <bool SAVE>
 __global__ void __launch_bounds__(NT, 1) gnet_head_kernel(const GnetParams p) {
   extern __shared__ __align__(16) unsigned char smem[];
   uint4* w12 = reinterpret_cast<uint4*>(smem);                          // W1 then W2, resident
@@ -238,8 +264,17 @@ __global__ void __launch_bounds__(NT, 1) gnet_head_kernel(const GnetParams p) {
       }
     }
 
+    // SAVE: layer l's activations of the warp's valid pixels into plane l of the saved maps
+    auto save_hidden = [&](int l) {
+      float* hp = p.save + ((size_t)l * p.B + b) * HID * HW + (size_t)(va ? y * p.W + xa : 0) + (size_t)(2 * q) * HW;
+      store_rows(hp, acc, HW, va, vb);
+      __syncwarp();   // keeps ptxas from sinking the stores into the next layer's MMAs (which spills)
+    };
+    if constexpr (SAVE) save_hidden(0);
     hidden_layer(acc, w12, vec, sh_w1, lane);
+    if constexpr (SAVE) save_hidden(1);
     hidden_layer(acc, w12 + G_LAYER / 16, vec + HID, sh_w2, lane);
+    if constexpr (SAVE) save_hidden(2);
 
     // ---- 128 -> 2 on the CUDA cores, quad reduction, Gaussian update ----
     const float* w3 = vec + 2 * HID;
@@ -269,6 +304,11 @@ __global__ void __launch_bounds__(NT, 1) gnet_head_kernel(const GnetParams p) {
       gaussian_update(mu1, s1, __ldg(p.prev + o), __ldg(p.prev + o + HW), mu, sg);
       p.out[o] = mu;
       p.out[o + HW] = sg;
+      if constexpr (SAVE) {
+        float* rp = p.save + (size_t)3 * p.B * HID * HW;
+        rp[o] = mu1;
+        rp[o + HW] = s1;
+      }
     }
   }
 }
@@ -345,15 +385,17 @@ cudaError_t launch_gnet_pack(const float* w0, const float* w1, const float* b1, 
   return cudaGetLastError();
 }
 
-cudaError_t launch_gnet_update(int B, int D, int H, int W, const float* cost, const float* inv, const void* weights,
-                               const float* prev, unsigned* scratch, float* out, cudaStream_t st) {
+namespace {
+template <bool SAVE>
+cudaError_t launch_gnet_head(int B, int D, int H, int W, const float* cost, const float* inv, const void* weights,
+                             const float* prev, unsigned* scratch, float* out, float* save, cudaStream_t st) {
   static std::once_flag flags[64];
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
   cudaError_t res = cudaSuccess;
   std::call_once(flags[dev & 63], [&] {
-    res = cudaFuncSetAttribute(gnet_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S_TOTAL);
+    res = cudaFuncSetAttribute(gnet_head_kernel<SAVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S_TOTAL);
   });
   if (res != cudaSuccess) return res;
   if ((e = launch_absmax_f32(cost, (size_t)B * D * H * W, scratch, st)) != cudaSuccess) return e;
@@ -364,9 +406,458 @@ cudaError_t launch_gnet_update(int B, int D, int H, int W, const float* cost, co
   p.tiles_y = (H + TY - 1) / TY;
   p.ntiles = B * p.tiles_x * p.tiles_y;
   p.cost = cost; p.inv = inv; p.weights = static_cast<const unsigned char*>(weights); p.prev = prev;
-  p.absmax = scratch; p.out = out;
-  gnet_head_kernel<<<std::min(p.ntiles, sm_count(dev)), NT, S_TOTAL, st>>>(p);   // persistent: one CTA per SM
+  p.absmax = scratch; p.out = out; p.save = save;
+  gnet_head_kernel<SAVE><<<std::min(p.ntiles, sm_count(dev)), NT, S_TOTAL, st>>>(p);   // persistent: one CTA per SM
   return cudaGetLastError();
+}
+}  // namespace
+
+cudaError_t launch_gnet_update(int B, int D, int H, int W, const float* cost, const float* inv, const void* weights,
+                               const float* prev, unsigned* scratch, float* out, cudaStream_t st) {
+  return launch_gnet_head<false>(B, D, H, W, cost, inv, weights, prev, scratch, out, nullptr, st);
+}
+
+// ================================================ training (DESIGN §3.10) ==========================================
+// Training pack: the inference pack, then W1^T and W2^T as B fragments of the same form (layer shifts of the header).
+size_t gnet_train_weights_bytes(int D) { return gnet_weights_bytes(D) + 2 * G_LAYER; }
+size_t gnet_saved_bytes(int B, int H, int W) { return (size_t)(3 * HID + 2) * B * H * W * 4; }
+
+namespace {
+constexpr int WG_KS = 32;            // pixels per shared-memory slab of the weight-gradient GEMMs
+constexpr int WG_KC = 1024;          // pixels per CTA (one partial per CTA and output element)
+constexpr int WG_M = 128, WG_N = 64; // CTA output tile
+constexpr int WG_SA = WG_M + 8, WG_SB = WG_N + 8;   // row strides = 8 mod 32 banks: conflict-free fragment loads
+constexpr size_t WG_SMEM = (size_t)2 * WG_KS * (WG_SA + WG_SB) * 4;
+
+int wgrad_chunks(int P) { return (P + WG_KC - 1) / WG_KC; }
+size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
+}  // namespace
+
+// backward scratch: d_h2, d_h1 (B,128,H,W), d_raw (B,2,H,W), the GEMM partials (one set, reused by the four GEMMs)
+size_t gnet_bwd_workspace_bytes(int B, int D, int H, int W) {
+  const size_t map = (size_t)B * H * W * 4;
+  const size_t ncols = (size_t)std::max(HID, 9 * D);
+  return align256(2 * HID * map) + align256(2 * map) + align256((size_t)wgrad_chunks(B * H * W) * HID * (ncols + 1) * 4);
+}
+
+namespace {
+// W1^T (layer 0 of the tail) and W2^T: Bmat[k][n] = W[k][n], fragment order as gnet_pack_kernel
+__global__ void __launch_bounds__(256) gnet_pack_t_kernel(const float* __restrict__ w1, const float* __restrict__ w2,
+                                                          unsigned char* __restrict__ dst, size_t tail) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int per_layer = (int)(G_LAYER / 16);
+  if (i >= 2 * per_layer) return;
+  const int layer = i / per_layer, f = i - layer * per_layer;
+  const int lane = f & 31, nt = (f >> 5) % NTILE, step = (f >> 5) / NTILE;
+  const int n = nt * 8 + (lane >> 2);
+  const float* w = layer == 0 ? w1 : w2;
+  const float s = pow2(reinterpret_cast<const int*>(dst + G_HDR)[1 + layer]);
+  float v[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) v[e] = w[(step * 16 + 2 * (lane & 3) + (e & 1) + (e >> 1) * 8) * HID + n];
+  uint32_t h0, l0, h1, l1;
+  split2(__fmul_rn(v[0], s), __fmul_rn(v[1], s), h0, l0);
+  split2(__fmul_rn(v[2], s), __fmul_rn(v[3], s), h1, l1);
+  reinterpret_cast<uint4*>(dst + tail)[i] = make_uint4(h0, h1, l0, l1);
+}
+
+// One 128 -> 128 layer of the backward chain on the gradient fragment (any sign): per-row scale from max |x|, split,
+// three products against the resident transposed weights, descale.  The caller applies the ReLU mask.
+__device__ __forceinline__ void grad_layer(float (&acc)[NTILE][4], const uint4* __restrict__ wsm, int shw, int lane) {
+  float m0 = 0.0f, m1 = 0.0f;
+#pragma unroll
+  for (int nt = 0; nt < NTILE; ++nt) {
+    m0 = fmaxf(m0, fmaxf(fabsf(acc[nt][0]), fabsf(acc[nt][1])));
+    m1 = fmaxf(m1, fmaxf(fabsf(acc[nt][2]), fabsf(acc[nt][3])));
+  }
+#pragma unroll
+  for (int o = 1; o <= 2; o <<= 1) {
+    m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, o));
+    m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, o));
+  }
+  const int sh0 = split16_shift(__float_as_uint(m0)), sh1 = split16_shift(__float_as_uint(m1));
+  const float s0 = pow2(sh0), s1 = pow2(sh1);
+  uint32_t ah[HID / 16][4], al[HID / 16][4];
+#pragma unroll
+  for (int kk = 0; kk < HID / 16; ++kk) {
+    split2(__fmul_rn(acc[2 * kk][0], s0), __fmul_rn(acc[2 * kk][1], s0), ah[kk][0], al[kk][0]);
+    split2(__fmul_rn(acc[2 * kk][2], s1), __fmul_rn(acc[2 * kk][3], s1), ah[kk][1], al[kk][1]);
+    split2(__fmul_rn(acc[2 * kk + 1][0], s0), __fmul_rn(acc[2 * kk + 1][1], s0), ah[kk][2], al[kk][2]);
+    split2(__fmul_rn(acc[2 * kk + 1][2], s1), __fmul_rn(acc[2 * kk + 1][3], s1), ah[kk][3], al[kk][3]);
+  }
+#pragma unroll
+  for (int nt = 0; nt < NTILE; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.0f;
+#pragma unroll
+  for (int kk = 0; kk < HID / 16; ++kk) {
+#pragma unroll
+    for (int nt = 0; nt < NTILE; ++nt) mma3(acc[nt], ah[kk], al[kk], wsm[(kk * NTILE + nt) * 32 + lane]);
+  }
+  const float dw = pow2(-shw), d0 = pow2(-sh0), d1 = pow2(-sh1);
+#pragma unroll
+  for (int nt = 0; nt < NTILE; ++nt) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      acc[nt][e] = __fmul_rn(__fmul_rn(acc[nt][e], d0), dw);
+      acc[nt][2 + e] = __fmul_rn(__fmul_rn(acc[nt][2 + e], d1), dw);
+    }
+  }
+}
+
+// ReLU backward on the fragment, as torch's threshold_backward: zero where the saved activation is <= 0 (a NaN
+// activation passes the gradient); h as store_rows addresses it
+__device__ __forceinline__ void relu_mask(float (&acc)[NTILE][4], const float* __restrict__ h, int HW, bool va, bool vb) {
+  HW = opaque(HW);
+#pragma unroll
+  for (int nt = 0; nt < NTILE; ++nt) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const float* c = h + (size_t)(nt * 8 + e) * HW;
+      acc[nt][e] = va && !(__ldg(c) <= 0.0f) ? acc[nt][e] : 0.0f;
+      acc[nt][2 + e] = vb && !(__ldg(c + 8) <= 0.0f) ? acc[nt][2 + e] : 0.0f;
+    }
+  }
+}
+
+struct GnetBwdParams {
+  int B, HW, gpi, ngroups;                   // gpi: 16-pixel groups per image
+  const float* __restrict__ grad;            // (B,2,H,W) gradient of the updated Gaussian
+  const float* __restrict__ prev;            // (B,2,H,W)
+  const float* __restrict__ save;            // the training forward's h0, h1, h2, raw
+  const unsigned char* __restrict__ weights; // training pack: header and fp32 vectors of its inference part ...
+  const unsigned char* __restrict__ wt;      // ... and its tail, W1^T then W2^T
+  float* __restrict__ grad_inv;              // (B,128,H,W) = d_h0
+  float* __restrict__ dh;                    // d_h2, d_h1 (B,128,H,W), d_raw (B,2,H,W)
+  float* __restrict__ grad_prev;             // (B,2,H,W) or NULL
+};
+
+// Per warp 16 consecutive pixels of one image (rows g and g+8 of the MMA): d_raw from the update's derivative,
+// d_h2 = (W3^T d_raw) [h2 > 0] on the CUDA cores, d_h1 = (W2^T d_h2) [h1 > 0] and d_h0 = (W1^T d_h1) [h0 > 0] on the
+// tensor cores.  Pixels past the image carry zeros.
+__global__ void __launch_bounds__(NT, 1) gnet_bwd_chain_kernel(const GnetBwdParams p) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  uint4* wt = reinterpret_cast<uint4*>(smem);                       // W1^T then W2^T, resident
+  float* w3 = reinterpret_cast<float*>(smem + S_W12);               // W3 [2][128]
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, q = lane & 3;
+  {
+    const uint4* src = reinterpret_cast<const uint4*>(p.wt);
+    for (int i = tid; i < (int)(S_W12 / 16); i += NT) wt[i] = __ldg(src + i);
+    const float* vs = reinterpret_cast<const float*>(p.weights + G_VEC) + 2 * HID;
+    for (int i = tid; i < 2 * HID; i += NT) w3[i] = __ldg(vs + i);
+  }
+  __syncthreads();
+  const int* shw = reinterpret_cast<const int*>(p.weights + G_HDR);
+  const int sh_w1 = __ldg(shw + 1), sh_w2 = __ldg(shw + 2);
+  const int HW = p.HW;
+  const size_t plane = (size_t)p.B * HID * HW;
+  const float* h0s = p.save;
+  const float* h1s = p.save + plane;
+  const float* h2s = p.save + 2 * plane;
+  const float* raws = p.save + 3 * plane;
+  float* dh2 = p.dh;
+  float* dh1 = p.dh + plane;
+  float* draw = p.dh + 2 * plane;
+
+  for (int base = blockIdx.x * (NT / 32); base < p.ngroups; base += gridDim.x * (NT / 32)) {
+    const int gi = base + warp;
+    if (gi >= p.ngroups) break;
+    const int b = gi / p.gpi, hw0 = (gi - b * p.gpi) * 16;
+    const int pa = hw0 + g, pb = hw0 + g + 8;
+    const bool va = pa < HW, vb = pb < HW;
+    // ---- d_raw from the update's derivative ----
+    float d[4] = {0.0f, 0.0f, 0.0f, 0.0f};     // (d_mu1, d_sigma1) of pixels pa, pb
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int px = r == 0 ? pa : pb;
+      if (!(r == 0 ? va : vb)) continue;
+      const size_t o = (size_t)b * 2 * HW + px;
+      const float g_mu = __ldg(p.grad + o), g_sg = __ldg(p.grad + o + HW);
+      const float mu1 = __ldg(raws + o), s1 = __ldg(raws + o + HW);
+      gaussian_update_bwd(g_mu, g_sg, s1, __ldg(p.prev + o + HW), d[2 * r], d[2 * r + 1]);
+      if (q == r) {
+        draw[o] = d[2 * r];
+        draw[o + HW] = d[2 * r + 1];
+        if (p.grad_prev) {
+          float d_mu0, d_s0;
+          gaussian_update_bwd_prev(g_mu, g_sg, mu1, s1, d_mu0, d_s0);
+          p.grad_prev[o] = d_mu0;
+          p.grad_prev[o + HW] = d_s0;
+        }
+      }
+    }
+    // offset of channel 2q of pixel pa in a (B,128,H,W) map
+    const size_t off = ((size_t)b * HID + 2 * q) * HW + (va ? pa : 0);
+    // ---- d_h2 on the CUDA cores ----
+    float acc[NTILE][4];
+#pragma unroll
+    for (int nt = 0; nt < NTILE; ++nt) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int c = nt * 8 + 2 * q + e;
+        const float wm = w3[c], ws = w3[HID + c];
+        acc[nt][e] = __fmaf_rn(ws, d[1], __fmul_rn(wm, d[0]));
+        acc[nt][2 + e] = __fmaf_rn(ws, d[3], __fmul_rn(wm, d[2]));
+      }
+    }
+    relu_mask(acc, h2s + off, HW, va, vb);
+    store_rows(dh2 + off, acc, HW, va, vb);
+    // ---- d_h1, d_h0 on the tensor cores ----
+#pragma unroll 1
+    for (int l = 0; l < 2; ++l) {
+      grad_layer(acc, wt + (l == 0 ? G_LAYER / 16 : 0), l == 0 ? sh_w2 : sh_w1, lane);
+      relu_mask(acc, (l == 0 ? h1s : h0s) + off, HW, va, vb);
+      store_rows((l == 0 ? dh1 : p.grad_inv) + off, acc, HW, va, vb);
+    }
+  }
+}
+
+// ---- weight gradients: out[m][n] = sum over pixels of A_m(p) B_n(p), 3xTF32 on the tensor cores ----
+struct WgradParams {
+  int HW, H, W, P, Ma, Nw, D, im2col;
+  const float* __restrict__ a;      // (B, Ma, HW)
+  const float* __restrict__ bsrc;   // dense: (B, Nw, HW); im2col: the cost volume (B, D, H, W), n = 9c + tap
+  float* __restrict__ part_w;       // [chunk][Ma][Nw]
+  float* __restrict__ part_b;       // [chunk][Ma] (sum of A over the pixels: the bias gradient) or NULL
+};
+
+__device__ __forceinline__ uint32_t tf32(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return r;
+}
+__device__ __forceinline__ void mma1688(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
+                                        uint32_t b1) {
+  asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
+// CTA (chunk, n block): its WG_KC pixels in slabs of WG_KS; each operand element is split x = hi + lo (tf32) once on
+// its way into shared memory; per k8 step three products lo*hi + hi*lo + hi*hi into the fp32 accumulators.
+__global__ void __launch_bounds__(256, 2) gnet_wgrad_kernel(const WgradParams p) {
+  extern __shared__ __align__(16) float wsm[];
+  uint32_t* ah = reinterpret_cast<uint32_t*>(wsm);
+  uint32_t* al = ah + WG_KS * WG_SA;
+  uint32_t* bh = al + WG_KS * WG_SA;
+  uint32_t* bl = bh + WG_KS * WG_SB;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, q = lane & 3;
+  const int wm = warp & 3, wn = warp >> 2;
+  const int chunk = blockIdx.x, n0 = blockIdx.y * WG_N;
+  const int k_begin = chunk * WG_KC, k_end = min(p.P, k_begin + WG_KC);
+  const bool bias = p.part_b != nullptr && blockIdx.y == 0;
+  float tot[2][4][4];        // the CTA's sums; each slab's MMAs accumulate from zero and are added here (IEEE adds)
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt) tot[mt][nt][0] = tot[mt][nt][1] = tot[mt][nt][2] = tot[mt][nt][3] = 0.0f;
+  float bsum[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+  const int lk = tid & 7, lr = tid >> 3;     // loader: pixel k = lk + 8*kk of the slab, row / column lr + 32*j
+  const bool warp_live = wm * 32 < p.Ma;
+
+  for (int k0 = k_begin; k0 < k_end; k0 += WG_KS) {
+    int pb_[4], phw[4], py[4], px[4];
+    bool pv[4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      const int pix = k0 + lk + 8 * kk;
+      pv[kk] = pix < k_end;
+      pb_[kk] = pv[kk] ? pix / p.HW : 0;
+      phw[kk] = pv[kk] ? pix - pb_[kk] * p.HW : 0;
+      py[kk] = phw[kk] / p.W;
+      px[kk] = phw[kk] - py[kk] * p.W;
+    }
+    __syncthreads();                                   // the previous slab is consumed
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int m = lr + 32 * j;
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        const float v = pv[kk] && m < p.Ma ? __ldg(p.a + ((size_t)pb_[kk] * p.Ma + m) * p.HW + phw[kk]) : 0.0f;
+        bsum[j] = __fadd_rn(bsum[j], v);
+        const uint32_t h = tf32(v);
+        const int k = lk + 8 * kk;
+        ah[k * WG_SA + m] = h;
+        al[k * WG_SA + m] = tf32(__fsub_rn(v, __uint_as_float(h)));
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int n = n0 + lr + 32 * j;
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        float v = 0.0f;
+        if (pv[kk] && n < p.Nw) {
+          if (p.im2col) {
+            const int c = n / 9, tap = n - 9 * c;
+            const int yy = py[kk] + tap / 3 - 1, xx = px[kk] + tap % 3 - 1;
+            if (yy >= 0 && yy < p.H && xx >= 0 && xx < p.W)
+              v = __ldg(p.bsrc + ((size_t)pb_[kk] * p.D + c) * p.HW + (size_t)yy * p.W + xx);
+          } else {
+            v = __ldg(p.bsrc + ((size_t)pb_[kk] * p.Nw + n) * p.HW + phw[kk]);
+          }
+        }
+        const uint32_t h = tf32(v);
+        const int k = lk + 8 * kk;
+        bh[k * WG_SB + n - n0] = h;
+        bl[k * WG_SB + n - n0] = tf32(__fsub_rn(v, __uint_as_float(h)));
+      }
+    }
+    __syncthreads();
+    if (warp_live) {
+      float acc[2][4][4];
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) acc[mt][nt][0] = acc[mt][nt][1] = acc[mt][nt][2] = acc[mt][nt][3] = 0.0f;
+#pragma unroll
+      for (int ks = 0; ks < WG_KS / 8; ++ks) {
+        const int r0 = (ks * 8 + q) * WG_SA, r1 = r0 + 4 * WG_SA;
+        uint32_t fh[2][4], fl[2][4];
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) {
+          const int m = wm * 32 + mt * 16 + g;
+          fh[mt][0] = ah[r0 + m]; fh[mt][1] = ah[r0 + m + 8]; fh[mt][2] = ah[r1 + m]; fh[mt][3] = ah[r1 + m + 8];
+          fl[mt][0] = al[r0 + m]; fl[mt][1] = al[r0 + m + 8]; fl[mt][2] = al[r1 + m]; fl[mt][3] = al[r1 + m + 8];
+        }
+        const int s0 = (ks * 8 + q) * WG_SB, s1 = s0 + 4 * WG_SB;
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+          const int n = wn * 32 + nt * 8 + g;
+          const uint32_t b0h = bh[s0 + n], b1h = bh[s1 + n], b0l = bl[s0 + n], b1l = bl[s1 + n];
+#pragma unroll
+          for (int mt = 0; mt < 2; ++mt) {
+            mma1688(acc[mt][nt], fl[mt][0], fl[mt][1], fl[mt][2], fl[mt][3], b0h, b1h);
+            mma1688(acc[mt][nt], fh[mt][0], fh[mt][1], fh[mt][2], fh[mt][3], b0l, b1l);
+            mma1688(acc[mt][nt], fh[mt][0], fh[mt][1], fh[mt][2], fh[mt][3], b0h, b1h);
+          }
+        }
+      }
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) tot[mt][nt][e] = __fadd_rn(tot[mt][nt][e], acc[mt][nt][e]);
+    }
+  }
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt) {
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int m = wm * 32 + mt * 16 + g + (e >> 1) * 8, n = n0 + wn * 32 + nt * 8 + 2 * q + (e & 1);
+        if (m < p.Ma && n < p.Nw) p.part_w[((size_t)chunk * p.Ma + m) * p.Nw + n] = tot[mt][nt][e];
+      }
+    }
+  }
+  if (bias) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float s = bsum[j];
+      s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, 1));
+      s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, 2));
+      s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, 4));
+      const int m = lr + 32 * j;
+      if (lk == 0 && m < p.Ma) p.part_b[(size_t)chunk * p.Ma + m] = s;
+    }
+  }
+}
+
+// fixed-order sum of the per-CTA partials
+__global__ void __launch_bounds__(256) gnet_wgrad_reduce_kernel(const float* __restrict__ part, int nchunk, int count,
+                                                                float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  float s = 0.0f;
+  for (int c = 0; c < nchunk; ++c) s = __fadd_rn(s, __ldg(part + (size_t)c * count + i));
+  out[i] = s;
+}
+
+cudaError_t launch_wgrad(int B, int H, int W, int Ma, const float* a, int Nw, int D, bool im2col, const float* bsrc,
+                         float* part, float* out_w, float* out_b, cudaStream_t st) {
+  WgradParams p;
+  p.HW = H * W; p.H = H; p.W = W; p.P = B * H * W; p.Ma = Ma; p.Nw = Nw; p.D = D; p.im2col = im2col ? 1 : 0;
+  p.a = a; p.bsrc = bsrc;
+  const int nchunk = wgrad_chunks(p.P);
+  p.part_w = part;
+  p.part_b = out_b ? part + (size_t)nchunk * Ma * Nw : nullptr;
+  gnet_wgrad_kernel<<<dim3(nchunk, (Nw + WG_N - 1) / WG_N), 256, WG_SMEM, st>>>(p);
+  if (out_w) {
+    const int count = Ma * Nw;
+    gnet_wgrad_reduce_kernel<<<(count + 255) / 256, 256, 0, st>>>(part, nchunk, count, out_w);
+  }
+  if (out_b) gnet_wgrad_reduce_kernel<<<(Ma + 255) / 256, 256, 0, st>>>(p.part_b, nchunk, Ma, out_b);
+  return cudaGetLastError();
+}
+}  // namespace
+
+cudaError_t launch_gnet_pack_train(const float* w0, const float* w1, const float* b1, const float* w2, const float* b2,
+                                   const float* w3, const float* b3, int D, void* dst, cudaStream_t st) {
+  cudaError_t e = launch_gnet_pack(w0, w1, b1, w2, b2, w3, b3, D, dst, st);
+  if (e != cudaSuccess) return e;
+  const int n = (int)(2 * G_LAYER / 16);
+  gnet_pack_t_kernel<<<(n + 255) / 256, 256, 0, st>>>(w1, w2, static_cast<unsigned char*>(dst), gnet_weights_bytes(D));
+  return cudaGetLastError();
+}
+
+cudaError_t launch_gnet_train_fwd(int B, int D, int H, int W, const float* cost, const float* inv, const void* weights,
+                                  const float* prev, unsigned* scratch, float* out, float* saved, cudaStream_t st) {
+  return launch_gnet_head<true>(B, D, H, W, cost, inv, weights, prev, scratch, out, saved, st);
+}
+
+// Launches: the chain kernel, then per requested (weight, bias) pair one GEMM and one or two reductions.
+cudaError_t launch_gnet_bwd(int B, int D, int H, int W, const float* cost, const float* prev, const void* weights,
+                            const float* saved, const float* grad, void* workspace, float* grad_inv, float* gw0,
+                            float* gw1, float* gb1, float* gw2, float* gb2, float* gw3, float* gb3, float* grad_prev,
+                            cudaStream_t st, int* launches) {
+  static std::once_flag flags[64];
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  cudaError_t res = cudaSuccess;
+  std::call_once(flags[dev & 63], [&] {
+    res = cudaFuncSetAttribute(gnet_bwd_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S_W12 + 2 * HID * 4));
+    if (res == cudaSuccess)
+      res = cudaFuncSetAttribute(gnet_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM);
+  });
+  if (res != cudaSuccess) return res;
+  const int HW = H * W;
+  const size_t map = (size_t)B * HW;
+  float* dh = static_cast<float*>(workspace);
+  float* part = reinterpret_cast<float*>(static_cast<unsigned char*>(workspace) + align256(2 * HID * map * 4) +
+                                         align256(2 * map * 4));
+  const unsigned char* wb = static_cast<const unsigned char*>(weights);
+  GnetBwdParams p;
+  p.B = B; p.HW = HW; p.gpi = (HW + 15) / 16; p.ngroups = B * p.gpi;
+  p.grad = grad; p.prev = prev; p.save = saved; p.weights = wb; p.wt = wb + gnet_weights_bytes(D);
+  p.grad_inv = grad_inv; p.dh = dh; p.grad_prev = grad_prev;
+  const int ctas = std::min((p.ngroups + NT / 32 - 1) / (NT / 32), sm_count(dev));
+  gnet_bwd_chain_kernel<<<ctas, NT, S_W12 + 2 * HID * 4, st>>>(p);
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  int n = 1;
+  const size_t plane = (size_t)HID * map;
+  const float* h0 = saved;
+  const float* h1 = saved + plane;
+  const float* h2 = saved + 2 * plane;
+  auto pair = [&](float* w, float* bias) { return (w ? 1 : 0) + (bias ? 1 : 0) + 1; };
+  if (gw1 || gb1) {          // dW1 = sum d_h1 h0^T, db1 = sum d_h1
+    if ((e = launch_wgrad(B, H, W, HID, dh + plane, HID, D, false, h0, part, gw1, gb1, st)) != cudaSuccess) return e;
+    n += pair(gw1, gb1);
+  }
+  if (gw2 || gb2) {          // dW2 = sum d_h2 h1^T, db2 = sum d_h2
+    if ((e = launch_wgrad(B, H, W, HID, dh, HID, D, false, h1, part, gw2, gb2, st)) != cudaSuccess) return e;
+    n += pair(gw2, gb2);
+  }
+  if (gw3 || gb3) {          // dW3 = sum d_raw h2^T, db3 = sum d_raw
+    if ((e = launch_wgrad(B, H, W, 2, dh + 2 * plane, HID, D, false, h2, part, gw3, gb3, st)) != cudaSuccess) return e;
+    n += pair(gw3, gb3);
+  }
+  if (gw0) {                 // dW0[o][c][tap] = sum d_h0[o] cost[c](p + tap)
+    if ((e = launch_wgrad(B, H, W, HID, grad_inv, 9 * D, D, true, cost, part, gw0, nullptr, st)) != cudaSuccess) return e;
+    n += 2;
+  }
+  *launches = n;
+  return cudaSuccess;
 }
 
 }  // namespace magnet

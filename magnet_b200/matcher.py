@@ -4,8 +4,9 @@ the cost kernel and the Gaussian update as one kernel, prepared once per forward
 The reference inlines the sampler (MAGNET.py:154-156) and the update (inside GNET.forward, :60-69),
 so they are only reachable through this alternative loop (or the ``GNET`` mirror below); the
 cost-volume function itself is also available as a pure drop-in (``magnet_b200.homography``).
-In inference the per-iteration G-Net head and update run as one fused kernel (``fused_gnet_applies``); training,
-autocast, the hoisted x_d3 convolution and the mask head stay ordinary ``nn.Module``s (cuDNN).
+In inference the per-iteration G-Net head and update run as one fused kernel (``fused_gnet_applies``); with
+``fused_train=True`` so do training iterations of the head (``fused_gnet_trains``, with a fused backward).  Autocast,
+the hoisted x_d3 convolution and the mask head stay ordinary ``nn.Module``s (cuDNN).
 """
 from __future__ import annotations
 
@@ -181,7 +182,7 @@ class MatchingPlan:
 
 def matching_loop(plan: MatchingPlan, ref_gmms: torch.Tensor, x_d3: torch.Tensor,
                   g_net_convs, n_iter: int, k: Sequence[float],
-                  variant=_lib.VARIANT_AUTO, detach_cost: bool = True) -> List[torch.Tensor]:
+                  variant=_lib.VARIANT_AUTO, detach_cost: bool = True, fused_train: bool = False) -> List[torch.Tensor]:
     """pred_list of MAGNET.py:150-169: [ref_gmms, pred_1, ..., pred_n_iter] at quarter resolution.
 
     ``g_net_convs`` is either a callable mapping the (B, D+256, H, W) concatenation [cost volume, x_d3] to the
@@ -192,7 +193,8 @@ def matching_loop(plan: MatchingPlan, ref_gmms: torch.Tensor, x_d3: torch.Tensor
     in the graph, so feature maps that require grad (a trainable F-Net upstream) receive gradients through it; the
     Gaussian that places the hypotheses stays detached, as in the reference (MAGNET.py:153).  When nothing needs a
     gradient (see ``fused_gnet_applies``), a ``GNET``'s head and the update of each iteration are one fused kernel, with
-    the weights packed once per call."""
+    the weights packed once per call.  With ``fused_train`` and a head to train (see ``fused_gnet_trains``), each
+    iteration is one differentiable fused op (``ops.gnet_head_train``) instead of the module chain."""
     karr = ops.k_array(k)
     preds = [ref_gmms]
     split = isinstance(g_net_convs, GNET)
@@ -209,6 +211,9 @@ def matching_loop(plan: MatchingPlan, ref_gmms: torch.Tensor, x_d3: torch.Tensor
             if packed is None:                             # the weights are read once per call
                 packed = ops.pack_gnet_weights(g_net_convs, cv.shape[1])
             preds.append(ops.gnet_update(cv, inv, packed, cur))
+            continue
+        if fused_train and fused_gnet_trains(g_net_convs, cv, inv):
+            preds.append(ops.gnet_head_train(cv, inv, g_net_convs, cur))
             continue
         raw = g_net_convs.raw_from_parts(cv, inv) if split else g_net_convs(torch.cat([cv, x_d3], dim=1))
         preds.append(ops.gaussian_update(raw.float(), cur))   # raw is half under autocast
@@ -232,15 +237,34 @@ def fused_gnet_applies(g_net_convs, cv: torch.Tensor, inv: Optional[torch.Tensor
     return 1 <= cv.shape[1] <= _lib.MAGNET_MAX_PLANES
 
 
+def fused_gnet_trains(g_net_convs, cv: torch.Tensor, inv: Optional[torch.Tensor]) -> bool:
+    """Whether a training iteration of ``matching_loop(..., fused_train=True)`` runs the differentiable fused head
+    (``ops.gnet_head_train``): the split data flow of a ``GNET``, grad mode on and a head parameter or the invariant
+    requiring grad, a cost volume that does not (the fused backward has no gradient into it), no CUDA autocast, fp32
+    weights and volume and 1 <= D <= MAGNET_MAX_PLANES cost channels."""
+    if not isinstance(g_net_convs, GNET) or inv is None:
+        return False
+    params = list(g_net_convs.parameters())
+    if not torch.is_grad_enabled() or not (inv.requires_grad or any(p.requires_grad for p in params)):
+        return False
+    if cv.requires_grad or torch.is_autocast_enabled("cuda"):
+        return False
+    if any(p.dtype != torch.float32 for p in params) or cv.dtype != torch.float32 or inv.dtype != torch.float32:
+        return False
+    return 1 <= cv.shape[1] <= _lib.MAGNET_MAX_PLANES
+
+
 class MagnetHead(nn.Module):
     """G-Net + mask head + convex upsampling of the reference's ``MAGNET`` (models/MAGNET.py:100-118,
     150-175) operating on backbone outputs; D-Net / F-Net are supplied by the caller (they need
     checkpoints / torch.hub in the reference and are out of scope, SURVEY §2.1 #3-4)."""
 
     def __init__(self, n_samples: int = 5, sampling_range: float = 3, n_iter: int = 3, thres: int = 5,
-                 downsample_ratio: int = 4, dnet_fdim: int = 256, detach_cost: bool = True):
+                 downsample_ratio: int = 4, dnet_fdim: int = 256, detach_cost: bool = True, fused_train: bool = False):
         super().__init__()
         self.n_iter, self.thres, self.downsample_ratio = n_iter, thres, downsample_ratio
+        # True: training iterations of the G-Net head run the differentiable fused kernels where fused_gnet_trains holds
+        self.fused_train = fused_train
         # True: G-Net reads a detached cost volume (MAGNET.py:167).  False: the volume stays in the graph, so a trainable
         # F-Net upstream receives gradients through the matching.
         self.detach_cost = detach_cost
@@ -269,7 +293,8 @@ class MagnetHead(nn.Module):
         upsample + NLL loss (``loss`` below) consumes during training.  Under torch.autocast every input may be half;
         the predictions and the mask are fp32."""
         plan = MatchingPlan(ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, thres=self.thres)
-        preds = matching_loop(plan, ref_gmms, x_d3, self.g_net, self.n_iter, self.k_list, detach_cost=self.detach_cost)
+        preds = matching_loop(plan, ref_gmms, x_d3, self.g_net, self.n_iter, self.k_list, detach_cost=self.detach_cost,
+                              fused_train=self.fused_train)
         return preds[1:], self.mask_head(x_d3).float()
 
     def loss(self, preds_quarter, mask, gt_depth, gt_depth_mask, gamma: float = 0.8):
@@ -290,7 +315,7 @@ class MAGNET(nn.Module):
 
     def __init__(self, d_net: nn.Module, f_net: nn.Module, n_samples: int = 5, sampling_range: float = 3,
                  weighting: str = "CW5", train_iter: int = 3, test_iter: int = 3, downsample_ratio: int = 4,
-                 dnet_fdim: int = 256):
+                 dnet_fdim: int = 256, fused_train: bool = False):
         super().__init__()
         self.d_net, self.f_net = d_net, f_net
         for net in (self.d_net, self.f_net):
@@ -300,7 +325,7 @@ class MAGNET(nn.Module):
         self.train_iter, self.test_iter = train_iter, test_iter
         thres = int(weighting.split('CW')[1])                   # "CW5" -> kappa = 5 (MAGNET.py:159)
         self.head = MagnetHead(n_samples=n_samples, sampling_range=sampling_range, n_iter=train_iter, thres=thres,
-                               downsample_ratio=downsample_ratio, dnet_fdim=dnet_fdim)
+                               downsample_ratio=downsample_ratio, dnet_fdim=dnet_fdim, fused_train=fused_train)
         self.g_net, self.mask_head = self.head.g_net, self.head.mask_head   # reference attribute names
 
     def train(self, mode: bool = True):

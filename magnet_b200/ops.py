@@ -533,6 +533,88 @@ def gnet_update(cost: torch.Tensor, invariant: torch.Tensor, packed: torch.Tenso
     return out
 
 
+class GnetHeadTrain(torch.autograd.Function):
+    """One iteration of the G-Net head and the Gaussian update, differentiable in the head's weights, the invariant and
+    prev_gmm (DESIGN §3.10): the inference kernel's arithmetic plus stores of the hidden maps, and a backward of one
+    tensor-core chain kernel and fixed-order weight-gradient GEMMs.  No gradient into the cost volume.  The weights are
+    packed at every call (nothing is cached: they change at every optimizer step)."""
+
+    @staticmethod
+    def forward(ctx, cost, invariant, w0, w1, b1, w2, b2, w3, b3, prev_gmm):
+        hid = _lib.MAGNET_HIDDEN_CHANNELS
+        cost = _need_cuda_f32("cost", cost.detach())
+        if cost.dim() != 4:
+            raise _lib.MagnetError(f"cost must be (B,D,H,W), got {tuple(cost.shape)}")
+        B, D, H, W = cost.shape
+        invariant = _need_cuda_f32("invariant", invariant.detach())
+        _expect("invariant", invariant, (B, hid, H, W))
+        prev_gmm = _need_cuda_f32("prev_gmm", prev_gmm.detach())
+        _expect("prev_gmm", prev_gmm, (B, 2, H, W))
+        nbytes = int(lib().magnet_gnet_train_weights_bytes(D))
+        if nbytes == 0:
+            raise _lib.MagnetError(f"the fused G-Net head takes 1 to {_lib.MAGNET_MAX_PLANES} cost channels, got {D}")
+        shapes = (("W0", w0, (hid, D, 3, 3)), ("W1", w1, (hid, hid, 1, 1)), ("b1", b1, (hid,)),
+                  ("W2", w2, (hid, hid, 1, 1)), ("b2", b2, (hid,)), ("W3", w3, (2, hid, 1, 1)), ("b3", b3, (2,)))
+        ws = []
+        for nm, t, shp in shapes:
+            t = _need_cuda_f32(nm, t.detach())
+            _expect(nm, t, shp)
+            ws.append(t)
+        dev = _same_device(("cost", cost), ("invariant", invariant), ("prev_gmm", prev_gmm),
+                           *((nm, t) for (nm, _, _), t in zip(shapes, ws)))
+        packed = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        saved = torch.empty(int(lib().magnet_gnet_saved_bytes(B, H, W)) // 4, device=dev, dtype=torch.float32)
+        out = torch.empty(B, 2, H, W, device=dev, dtype=torch.float32)
+        scratch = torch.empty(_lib.MAGNET_GNET_SCRATCH_BYTES // 4, device=dev, dtype=torch.int32)
+        a = _lib.GnetTrainArgs(B=B, D=D, H=H, W=W, cost=cost.data_ptr(), invariant=invariant.data_ptr(),
+                               packed_weights=packed.data_ptr(), prev_gmm=prev_gmm.data_ptr(), scratch=scratch.data_ptr(),
+                               out=out.data_ptr(), saved=saved.data_ptr())
+        with torch.cuda.device(dev):
+            check(lib().magnet_gnet_pack_train_weights_f32(*(t.data_ptr() for t in ws), D, packed.data_ptr(), _stream(dev)),
+                  "magnet_gnet_pack_train_weights_f32")
+            check(lib().magnet_gnet_train_fwd_f32(C.byref(a), _stream(dev)), "magnet_gnet_train_fwd_f32")
+        ctx.save_for_backward(cost, prev_gmm, packed, saved)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        cost, prev_gmm, packed, saved = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        B, D, H, W = cost.shape
+        hid = _lib.MAGNET_HIDDEN_CHANNELS
+        dev = cost.device
+        grad_out = _need_cuda_f32("grad_out", grad_out)
+        new = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.float32)
+        g_inv = new(B, hid, H, W)
+        g = [new(hid, D, 3, 3) if need[2] else None, new(hid, hid, 1, 1) if need[3] else None,
+             new(hid) if need[4] else None, new(hid, hid, 1, 1) if need[5] else None, new(hid) if need[6] else None,
+             new(2, hid, 1, 1) if need[7] else None, new(2) if need[8] else None]
+        g_prev = new(B, 2, H, W) if need[9] else None
+        ws = torch.empty(int(lib().magnet_gnet_bwd_workspace_bytes(B, D, H, W)), device=dev, dtype=torch.uint8)
+        ptr = lambda t: None if t is None else t.data_ptr()
+        a = _lib.GnetTrainArgs(B=B, D=D, H=H, W=W, cost=cost.data_ptr(), packed_weights=packed.data_ptr(),
+                               prev_gmm=prev_gmm.data_ptr(), saved=saved.data_ptr(), grad_out=grad_out.data_ptr(),
+                               workspace=ws.data_ptr(), grad_invariant=g_inv.data_ptr(), grad_w0_cost=ptr(g[0]),
+                               grad_w1=ptr(g[1]), grad_b1=ptr(g[2]), grad_w2=ptr(g[3]), grad_b2=ptr(g[4]),
+                               grad_w3=ptr(g[5]), grad_b3=ptr(g[6]), grad_prev=ptr(g_prev))
+        with torch.cuda.device(dev):
+            check(lib().magnet_gnet_bwd_f32(C.byref(a), _stream(dev)), "magnet_gnet_bwd_f32")
+        return (None, g_inv if need[1] else None, *g, g_prev)
+
+
+def gnet_head_train(cost, invariant, gnet, prev_gmm):
+    """``GnetHeadTrain`` on the weights of a ``GNET`` (or its ``gnet`` Sequential): the cost slice W0[:, :D] of the first
+    convolution (autograd scatters its gradient into the full weight), the two 128x128 layers and the 128->2 layer.
+    Validates like ``gnet_update``."""
+    seq = gnet.gnet if hasattr(gnet, "gnet") else gnet
+    c0, c1, c2, c3 = seq[0], seq[2], seq[4], seq[6]
+    if cost.dim() != 4 or c0.weight.dim() != 4 or c0.weight.shape[1] < cost.shape[1]:
+        raise _lib.MagnetError(f"not a G-Net head with at least {cost.shape[1] if cost.dim() == 4 else '?'} cost channels")
+    D = cost.shape[1]
+    return GnetHeadTrain.apply(cost, invariant, c0.weight[:, :D], c1.weight, c1.bias, c2.weight, c2.bias, c3.weight,
+                               c3.bias, prev_gmm)
+
+
 class ConvexUpsample(torch.autograd.Function):
     """upsample_depth_via_mask (MAGNET.py:15-27) as one kernel each way; differentiable in depth and mask."""
 
