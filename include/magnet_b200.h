@@ -190,6 +190,36 @@ typedef struct magnet_cost_bwd_args {
 int magnet_cost_volume_bwd_f32(const magnet_cost_bwd_args* args, void* stream);
 
 /*
+ * Gradients of either cost volume w.r.t. the cameras (DESIGN §3.11) — what autograd derives for the reference's
+ * term1_pix = K t and term2_pix = (K R) Ray through grid_sample's position derivative; the consistency mask passes none.
+ * `fwd` is the forward call:
+ *   - depth_mode MAGNET_DEPTH_VOLUME or MAGNET_DEPTH_GAUSS, consistency 0 or 1, softmax 0: src_layout and variant name the
+ *     forward kernel whose mask is reproduced, as for magnet_cost_volume_bwd_f32 (SPLIT16 / HALF16 with AUTO or MMA, or
+ *     DIRECT with NCHW / TILED32; CELLS and TMA forwards are rejected);
+ *   - depth_mode MAGNET_DEPTH_PLANES, consistency 0, softmax 0 or 1 (the F volume): any forward kernel; the positions
+ *     are those of the tensor-core forward.
+ * fwd->ref_feat / src_feat / out are ignored: the kernel reads the NCHW fp32 maps below.  Feature gradients are not
+ * computed here (magnet_cost_volume_bwd_f32 / magnet_cost_volume_f_bwd_f32).  Requires C <= 64.  No atomics: the
+ * results are bit-identical from run to run.  Three launches, no allocation, no synchronisation.
+ */
+typedef struct magnet_cost_geom_bwd_args {
+  const magnet_cost_args* fwd;
+  const float* ref_feat;  /* (B,C,H,W) NCHW                                                                       */
+  const float* src_feat;  /* (V*B,C,H,W) NCHW, view-major                                                         */
+  const float* src_gmm;   /* (V*B,2,H,W) [mu, sigma]; required when fwd->consistency == 1                         */
+  const float* grad_out;  /* (B,D,H,W) gradient w.r.t. the forward output                                         */
+  const float* prob;      /* (B,D,H,W) forward output; required when fwd->softmax == 1                            */
+  float* score;           /* (B,D,H,W) scratch                                                                    */
+  void* workspace;        /* magnet_cost_geom_workspace_bytes(B, V, H, W) bytes, 16-byte aligned, scratch         */
+  float* grad_cams;       /* (B*V, 12) written: d/dA (K R, row-major), then d/da (K t); zero for an invalid view   */
+  float* grad_rays;       /* (B,3,H*W) written, or NULL                                                           */
+  float* grad_depth;      /* VOLUME (B,D,H,W) / GAUSS (B,2,H,W) written, or NULL; must be NULL for PLANES         */
+} magnet_cost_geom_bwd_args;
+/* Bytes of the workspace of magnet_cost_volume_geom_bwd_f32 (0 for a non-positive dimension). */
+size_t magnet_cost_geom_workspace_bytes(int32_t B, int32_t V, int32_t H, int32_t W);
+int magnet_cost_volume_geom_bwd_f32(const magnet_cost_geom_bwd_args* args, void* stream);
+
+/*
  * Camera constants.  Replaces homography.py:89,98-102 (IntM/R/t products, done there per pair per
  * iteration).  intM (B,3,3) dense; R and t are addressed with element strides so that the
  * non-contiguous views nghbr_poses[:,:,:3,:3] / [:,:,:3,3] of MAGNET.py:147-148 can be passed as is:

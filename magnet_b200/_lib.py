@@ -41,6 +41,7 @@ EXPORTS = (
     "magnet_gnet_weights_bytes", "magnet_gnet_pack_weights_f32", "magnet_gnet_update_f32",
     "magnet_gnet_train_weights_bytes", "magnet_gnet_saved_bytes", "magnet_gnet_bwd_workspace_bytes",
     "magnet_gnet_pack_train_weights_f32", "magnet_gnet_train_fwd_f32", "magnet_gnet_bwd_f32",
+    "magnet_cost_geom_workspace_bytes", "magnet_cost_volume_geom_bwd_f32",
 )
 MAGNET_HIDDEN_CHANNELS = 128
 MAGNET_GNET_SCRATCH_BYTES = 16
@@ -69,6 +70,13 @@ class CostBwdArgs(C.Structure):
     _fields_ = [("fwd", C.POINTER(CostArgs)), ("ref_feat", C.c_void_p), ("src_feat", C.c_void_p), ("src_gmm", C.c_void_p),
                 ("grad_out", C.c_void_p), ("workspace", C.c_void_p), ("grad_ref", C.c_void_p), ("grad_src", C.c_void_p),
                 ("grad_depth", C.c_void_p)]
+
+
+class CostGeomBwdArgs(C.Structure):
+    """Mirror of ``struct magnet_cost_geom_bwd_args``."""
+    _fields_ = [("fwd", C.POINTER(CostArgs))] + [
+        (n, C.c_void_p) for n in ("ref_feat", "src_feat", "src_gmm", "grad_out", "prob", "score", "workspace",
+                                  "grad_cams", "grad_rays", "grad_depth")]
 
 
 class DepthMetricsArgs(C.Structure):
@@ -201,6 +209,10 @@ def lib() -> C.CDLL:
     L.magnet_gnet_train_fwd_f32.argtypes = [C.POINTER(GnetTrainArgs), C.c_void_p]
     L.magnet_gnet_bwd_f32.restype = C.c_int
     L.magnet_gnet_bwd_f32.argtypes = [C.POINTER(GnetTrainArgs), C.c_void_p]
+    L.magnet_cost_geom_workspace_bytes.restype = C.c_size_t
+    L.magnet_cost_geom_workspace_bytes.argtypes = [C.c_int32] * 4
+    L.magnet_cost_volume_geom_bwd_f32.restype = C.c_int
+    L.magnet_cost_volume_geom_bwd_f32.argtypes = [C.POINTER(CostGeomBwdArgs), C.c_void_p]
     if L.magnet_abi_version() != MAGNET_ABI_VERSION:
         raise MagnetError(f"ABI version mismatch: library {L.magnet_abi_version()} != binding {MAGNET_ABI_VERSION}")
     _lib = L

@@ -52,6 +52,10 @@ bool f_bwd_mma_supports(int C, int V);
 cudaError_t launch_cost_cw_bwd(const CwBwdParams& p, const CwBwdParams* split, int split_layout, int C, int mode,
                                bool mask_mma, const float* grad_out, cudaStream_t st, int* launches);
 bool cw_bwd_supports(int C);
+size_t geom_workspace_bytes(int B, int V, int H, int W);
+cudaError_t launch_cost_geom_bwd(const CwBwdParams& p, int C, int mode, bool mask_mma, int softmax, const float* prob,
+                                 const float* grad_out, float* partials, float* grad_rays, float* grad_cams,
+                                 cudaStream_t st, int* launches);
 #ifdef MAGNET_MMA_DEBUG
 void f_bwd_mma_set_debug_buffer(float* p);
 #endif
@@ -318,6 +322,63 @@ int magnet_cost_volume_bwd_f32(const magnet_cost_bwd_args* b, void* stream) {
   int launches = 0;
   cudaError_t e = magnet::launch_cost_cw_bwd(p, split ? &ps : nullptr, a->src_layout, a->C, a->depth_mode, mask_mma,
                                              b->grad_out, (cudaStream_t)stream, &launches);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += launches;
+  return MAGNET_OK;
+}
+
+size_t magnet_cost_geom_workspace_bytes(int32_t B, int32_t V, int32_t H, int32_t W) {
+  if (B <= 0 || V <= 0 || H <= 0 || W <= 0) return 0;
+  return magnet::geom_workspace_bytes(B, V, H, W);
+}
+
+int magnet_cost_volume_geom_bwd_f32(const magnet_cost_geom_bwd_args* b, void* stream) {
+  if (!b || !b->fwd) return MAGNET_ERR_NULL;
+  const magnet_cost_args* a = b->fwd;
+  if (a->B <= 0 || a->V <= 0 || a->D <= 0 || a->C <= 0 || a->H <= 0 || a->W <= 0) return MAGNET_ERR_SHAPE;
+  if ((int64_t)a->H * a->W > (1 << 26) || a->B > 65535 || (int64_t)a->B * a->V > (1 << 30)) return MAGNET_ERR_SHAPE;
+  if (a->D > MAGNET_MAX_PLANES || !magnet::cw_bwd_supports(a->C)) return MAGNET_ERR_UNSUPPORTED;
+  if (!a->rays || !a->cams || !b->ref_feat || !b->src_feat || !b->grad_out || !b->score || !b->workspace ||
+      !b->grad_cams)
+    return MAGNET_ERR_NULL;
+  bool mask_mma = false;
+  switch (a->depth_mode) {
+    case MAGNET_DEPTH_VOLUME: if (!a->d_volume) return MAGNET_ERR_NULL; break;
+    case MAGNET_DEPTH_GAUSS: if (!a->ref_gmm || !a->k_host) return MAGNET_ERR_NULL; break;
+    case MAGNET_DEPTH_PLANES: if (!a->k_host) return MAGNET_ERR_NULL; break;
+    default: return MAGNET_ERR_UNSUPPORTED;
+  }
+  if (a->depth_mode == MAGNET_DEPTH_PLANES) {      // the F volume: no mask, the tensor-core forward's positions
+    if (a->consistency || b->grad_depth) return MAGNET_ERR_UNSUPPORTED;
+    if (a->softmax && !b->prob) return MAGNET_ERR_NULL;
+  } else {
+    if (a->softmax) return MAGNET_ERR_UNSUPPORTED;
+    mask_mma = packed_layout(a->src_layout);     // the tensor-core forward's mask, else the DIRECT forward's
+    if (mask_mma) {
+      if (a->variant != MAGNET_VARIANT_AUTO && a->variant != MAGNET_VARIANT_MMA) return MAGNET_ERR_UNSUPPORTED;
+      if (!magnet::mma_supports(a->C, a->D, a->V, a->src_layout)) return MAGNET_ERR_UNSUPPORTED;
+    } else if (a->variant != MAGNET_VARIANT_DIRECT ||
+               (a->src_layout != MAGNET_SRC_NCHW && a->src_layout != MAGNET_SRC_TILED32)) {
+      return MAGNET_ERR_UNSUPPORTED;
+    }
+    if (a->consistency && !b->src_gmm) return MAGNET_ERR_NULL;
+  }
+  if (reinterpret_cast<uintptr_t>(b->workspace) % 16 != 0) return MAGNET_ERR_ALIGN;
+  magnet::CwBwdParams p;
+  p.B = a->B; p.V = a->V; p.D = a->D; p.H = a->H; p.W = a->W; p.HW = a->H * a->W;
+  p.cw = a->consistency != 0;
+  p.kappa = a->kappa;
+  p.ref_feat = b->ref_feat; p.src_feat = b->src_feat; p.src_gmm = b->src_gmm; p.rays = a->rays; p.cams = a->cams;
+  p.d_volume = a->d_volume; p.ref_gmm = a->ref_gmm;
+  p.g_score = b->score;
+  p.grad_ref = p.grad_src = nullptr;
+  p.grad_depth = b->grad_depth;
+  for (int j = 0; j < MAGNET_MAX_PLANES; ++j)
+    p.k[j] = (a->depth_mode != MAGNET_DEPTH_VOLUME && j < a->D) ? a->k_host[j] : 0.0f;
+  int launches = 0;
+  cudaError_t e = magnet::launch_cost_geom_bwd(p, a->C, a->depth_mode, mask_mma, a->softmax != 0, b->prob, b->grad_out,
+                                               static_cast<float*>(b->workspace), b->grad_rays, b->grad_cams,
+                                               (cudaStream_t)stream, &launches);
   if (e != cudaSuccess) return cuda_fail(e);
   g_launches += launches;
   return MAGNET_OK;

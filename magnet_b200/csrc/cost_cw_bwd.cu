@@ -23,6 +23,15 @@
 // to 4 corner coefficients G_t before the C channels are touched.  Four lanes per (b, pixel); any hypothesis order.
 // After a tensor-core forward the feature gradients come from the tensor-core kernel on the forward's split buffers
 // (cost_f_bwd_mma.cu, same mask helpers) and this kernel computes the depth gradient only.
+//
+// Camera gradients (GEOM, DESIGN §3.11): the same walk takes the position derivative one step further.  With
+// gx = g m dcost/dix, gy = g m dcost/diy, P = a + q d (q = A r), Zp = P2 + 1e-10, u = P0/Zp, w = P1/Zp:
+//   g_P = (gx, gy, -(gx u + gy w)) / Zp;   grad_a[b,v] = sum_{p,j} g_P;   grad_A[b,v] = sum_p (sum_j g_P d_j) r_p^T;
+//   grad_ray[b,:,p] = sum_v A_v^T sum_j g_P d_j.
+// Per (pixel, view) 6 accumulators, per pixel 3 ray accumulators; per view each block reduces its pixels' 12-vectors
+// in a fixed order into a caller-owned workspace, and geom_reduce_kernel adds the blocks in a fixed order: no atomics,
+// bit-identical from run to run.  MAGNET_DEPTH_PLANES (the F volume, no mask) uses the position arithmetic of project().
+// The GEOM flag sits on the shared body so that the existing kernels keep their parameter block and their code.
 #include "cells_common.cuh"
 #include "cw_mask.cuh"
 
@@ -35,15 +44,25 @@ constexpr int MASK_MMA = 0, MASK_DIRECT = 1;
 // Four lanes per (b, pixel): lane q of the quad holds channels [q*CPL, q*CPL + CPL) of ref and grad_ref (channels >= C
 // are idle), so at C = 64 a thread keeps 2 x 16 channel values instead of 2 x 64.  The four lanes walk the same
 // hypotheses with the same data, hence in lockstep; the per-cell dot products are reduced across the quad by shuffles.
-template <int CPL, int MODE, int MASK>
-__global__ void __launch_bounds__(128)
-cost_cw_bwd_kernel(const __grid_constant__ CwBwdParams p, const int C) {
+// Outputs of a GEOM launch: per-block partials [(b*V + v)*12 + k][block] and the ray gradient (B,3,HW) or NULL.
+struct GeomOut {
+  float* __restrict__ partials;
+  float* __restrict__ grad_rays;
+};
+
+template <int CPL, int MODE, int MASK, bool GEOM>
+__device__ __forceinline__ void cw_bwd_body(const CwBwdParams& p, const int C, const GeomOut* go) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  const int n = t >> 2, q = t & 3;
-  if (n >= p.HW) return;                                  // whole quads leave together (HW quads per row of blocks)
+  const int n0 = t >> 2, q = t & 3;
+  // whole quads leave together (HW quads per row of blocks); a GEOM block keeps them for its per-view reductions,
+  // walking the last pixel again without writing anything
+  if (!GEOM && n0 >= p.HW) return;
+  const bool active = n0 < p.HW;
+  const int n = GEOM && !active ? p.HW - 1 : n0;
   const unsigned qmask = 0xfu << (threadIdx.x & 28);
   const int b = blockIdx.y, H = p.H, W = p.W, HW = p.HW, D = p.D;
-  const bool need_ref = p.grad_ref != nullptr, need_src = p.grad_src != nullptr, need_d = p.grad_depth != nullptr;
+  const bool need_ref = !GEOM && p.grad_ref != nullptr, need_src = !GEOM && p.grad_src != nullptr;
+  const bool need_d = p.grad_depth != nullptr;
   const int c0 = q * CPL;
   float ref[CPL], gref[CPL];
 #pragma unroll
@@ -61,11 +80,12 @@ cost_cw_bwd_kernel(const __grid_constant__ CwBwdParams p, const int C) {
     sg_p = ldg_f(p.ref_gmm + ((size_t)b * 2 + 1) * HW + n);
   }
   float* gd = p.grad_depth + (size_t)b * D * HW + n;       // VOLUME: this pixel's column, accumulated over the views
-  const bool writer = q == 0;                             // lane 0 of the quad owns the depth gradient
+  const bool writer = GEOM ? q == 0 && active : q == 0;   // lane 0 of the quad owns the depth gradient
   if (MODE == MAGNET_DEPTH_VOLUME && need_d && writer)
     for (int j = 0; j < D; ++j) gd[(size_t)j * HW] = 0.0f;
   const float xmax = (float)W + 1.0f, ymax = (float)H + 1.0f;
   const float uc = (float)W / 2.0f, vc = (float)H / 2.0f;
+  float gr0 = 0.f, gr1 = 0.f, gr2 = 0.f;                  // GEOM: the ray gradient, summed over the views
 
   for (int v = 0; v < p.V; ++v) {
     const magnet_camera* cam = p.cams + (b * p.V + v);
@@ -78,6 +98,7 @@ cost_cw_bwd_kernel(const __grid_constant__ CwBwdParams p, const int C) {
     const float* src = p.src_feat + ((size_t)vb * C + c0) * HW;
     const float* gm = p.src_gmm + (size_t)vb * 2 * HW;
     float* gsrc = need_src ? p.grad_src + ((size_t)vb * C + c0) * HW : nullptr;
+    float sa0 = 0.f, sa1 = 0.f, sa2 = 0.f, sd0 = 0.f, sd1 = 0.f, sd2 = 0.f;   // GEOM: sum_j g_P, sum_j g_P d_j
 
     // the current cell: origin, which taps are inside, their (mu, sigma), their dot products, the coefficients G_t
     float cx = -1e30f, cy = -1e30f;
@@ -127,7 +148,7 @@ cost_cw_bwd_kernel(const __grid_constant__ CwBwdParams p, const int C) {
         m11 = i11 ? ldg_f(gm + o11) : 0.f; s11 = i11 ? ldg_f(gm + HW + o11) : 0.f;
       }
       f00 = f01 = f10 = f11 = 0.f;
-      if (need_d && (i00 | i01 | i10 | i11)) {
+      if ((need_d || GEOM) && (i00 | i01 | i10 | i11)) {
 #pragma unroll
         for (int i = 0; i < CPL; ++i) {
           if (c0 + i >= C) break;
@@ -151,9 +172,12 @@ cost_cw_bwd_kernel(const __grid_constant__ CwBwdParams p, const int C) {
     for (int j = 0; j < D; ++j) {
       float d;
       if (MODE == MAGNET_DEPTH_VOLUME) d = ldg_f(p.d_volume + ((size_t)b * D + j) * HW + n);
+      else if (MODE == MAGNET_DEPTH_PLANES) d = p.k[j];
       else d = __fadd_rn(mu_p, __fmul_rn(sg_p, p.k[j]));  // MAGNET.py:155: mul, then add
       // sample position, source depth z, du/dd, dv/dd in the forward kernel's arithmetic
       float ix, iy, z, dudd, dvdd;
+      float u_g = 0.f, w_g = 0.f, rz_g = 0.f;             // GEOM: u, w, 1/Zp
+      bool clx = false, cly = false;                      // GEOM, DIRECT: the axis hit the +-10 clamp
       if (MASK == MASK_MMA) {
         project(d, a0, a1, a2, q0, q1, q2, ix, iy, z);    // element by element == project2 of cost_mma.cu
         ix = clamp_coord(ix, xmax);
@@ -161,6 +185,11 @@ cost_cw_bwd_kernel(const __grid_constant__ CwBwdParams p, const int C) {
         const float r = rcp_nr(__fadd_rn(z, 1e-10f));
         dudd = (q0 - __fmaf_rn(q0, d, a0) * r * q2) * r;
         dvdd = (q1 - __fmaf_rn(q1, d, a1) * r * q2) * r;
+        if (GEOM) {
+          u_g = __fmaf_rn(q0, d, a0) * r;
+          w_g = __fmaf_rn(q1, d, a1) * r;
+          rz_g = r;
+        }
       } else {                                            // cost_direct.cu, homography.py:132-148
         const float P0 = __fadd_rn(a0, __fmul_rn(q0, d));
         const float P1 = __fadd_rn(a1, __fmul_rn(q1, d));
@@ -171,6 +200,13 @@ cost_cw_bwd_kernel(const __grid_constant__ CwBwdParams p, const int C) {
         float gy = __fdiv_rn(__fsub_rn(w, vc), vc);
         dudd = (q0 - u * q2) / Zp;
         dvdd = (q1 - w * q2) / Zp;
+        if (GEOM) {
+          u_g = u;
+          w_g = w;
+          rz_g = __fdiv_rn(1.0f, Zp);
+          clx = !(fabsf(gx) <= 10.0f);
+          cly = !(fabsf(gy) <= 10.0f);
+        }
         if (gx > 10.0f) { gx = 10.0f; dudd = 0.0f; }      // the masked assignment passes no gradient
         if (gx < -10.0f) { gx = -10.0f; dudd = 0.0f; }
         if (gy > 10.0f) { gy = 10.0f; dvdd = 0.0f; }
@@ -221,8 +257,49 @@ cost_cw_bwd_kernel(const __grid_constant__ CwBwdParams p, const int C) {
           g_sg = __fmaf_rn(p.k[j], gdv, g_sg);
         }
       }
+      if (GEOM) {                                         // kept apart so that the block above compiles as before
+        const float dcdx = (f01 - f00) * wy0 + (f11 - f10) * wy1;     // the same values as above
+        const float dcdy = (f10 - f00) * wx0 + (f11 - f01) * wx1;
+        const float gx = clx ? 0.f : __fmul_rn(g, dcdx), gy = cly ? 0.f : __fmul_rn(g, dcdy);
+        const float gp0 = __fmul_rn(gx, rz_g), gp1 = __fmul_rn(gy, rz_g);
+        const float gp2 = -__fmul_rn(__fmaf_rn(gy, w_g, __fmul_rn(gx, u_g)), rz_g);
+        sa0 = __fadd_rn(sa0, gp0); sa1 = __fadd_rn(sa1, gp1); sa2 = __fadd_rn(sa2, gp2);
+        sd0 = __fmaf_rn(gp0, d, sd0); sd1 = __fmaf_rn(gp1, d, sd1); sd2 = __fmaf_rn(gp2, d, sd2);
+      }
     }
     flush();
+    if (GEOM) {
+      // ray gradient A^T h, h = sum_j g_P d_j
+      gr0 = __fmaf_rn(cam->A[6], sd2, __fmaf_rn(cam->A[3], sd1, __fmaf_rn(cam->A[0], sd0, gr0)));
+      gr1 = __fmaf_rn(cam->A[7], sd2, __fmaf_rn(cam->A[4], sd1, __fmaf_rn(cam->A[1], sd0, gr1)));
+      gr2 = __fmaf_rn(cam->A[8], sd2, __fmaf_rn(cam->A[5], sd1, __fmaf_rn(cam->A[2], sd0, gr2)));
+      // this pixel's 12-vector (A row-major: h_i r_k, then a: sum_j g_P), owner lanes only, reduced over the block
+      __shared__ float red[4][12];
+      float c[12] = {sd0 * r0, sd0 * r1, sd0 * r2, sd1 * r0, sd1 * r1, sd1 * r2, sd2 * r0, sd2 * r1, sd2 * r2,
+                     sa0, sa1, sa2};
+#pragma unroll
+      for (int k = 0; k < 12; ++k) {
+        c[k] = writer ? c[k] : 0.0f;                      // lanes 0, 4, .., 28 hold the warp's pixels
+#pragma unroll
+        for (int m = 16; m >= 4; m >>= 1) c[k] = __fadd_rn(c[k], __shfl_xor_sync(0xffffffffu, c[k], m));
+      }
+      if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+        for (int k = 0; k < 12; ++k) red[threadIdx.x >> 5][k] = c[k];
+      }
+      __syncthreads();
+      if (threadIdx.x < 12) {
+        const float s = __fadd_rn(__fadd_rn(red[0][threadIdx.x], red[1][threadIdx.x]),
+                                  __fadd_rn(red[2][threadIdx.x], red[3][threadIdx.x]));
+        go->partials[((size_t)(b * p.V + v) * 12 + threadIdx.x) * gridDim.x + blockIdx.x] = s;
+      }
+      __syncthreads();
+    }
+  }
+  if (GEOM && writer && go->grad_rays != nullptr) {
+    go->grad_rays[((size_t)b * 3 + 0) * HW + n] = gr0;
+    go->grad_rays[((size_t)b * 3 + 1) * HW + n] = gr1;
+    go->grad_rays[((size_t)b * 3 + 2) * HW + n] = gr2;
   }
   if (need_ref) {
 #pragma unroll
@@ -235,7 +312,40 @@ cost_cw_bwd_kernel(const __grid_constant__ CwBwdParams p, const int C) {
   }
 }
 
+template <int CPL, int MODE, int MASK>
+__global__ void __launch_bounds__(128)
+cost_cw_bwd_kernel(const __grid_constant__ CwBwdParams p, const int C) {
+  cw_bwd_body<CPL, MODE, MASK, false>(p, C, nullptr);
+}
+
+template <int CPL, int MODE, int MASK>
+__global__ void __launch_bounds__(128)
+cost_geom_bwd_kernel(const __grid_constant__ CwBwdParams p, const int C, const __grid_constant__ GeomOut go) {
+  cw_bwd_body<CPL, MODE, MASK, true>(p, C, &go);
+}
+
+// grad_cams[bv, k] = sum over the blocks of the partials, in a fixed order: warp k, lane l adds blocks l, l + 32, ...,
+// then a butterfly over the lanes.  Zero for an invalid view (its partials were never written).
+__global__ void __launch_bounds__(384)
+geom_reduce_kernel(const float* __restrict__ partials, const magnet_camera* __restrict__ cams, int nblk,
+                   float* __restrict__ grad_cams) {
+  const int bv = blockIdx.x, k = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float s = 0.0f;
+  if (cams[bv].valid == 1.0f) {
+    const float* src = partials + ((size_t)bv * 12 + k) * nblk;
+    for (int i = lane; i < nblk; i += 32) s = __fadd_rn(s, src[i]);
+#pragma unroll
+    for (int m = 16; m >= 1; m >>= 1) s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, m));
+  }
+  if (lane == 0) grad_cams[(size_t)bv * 12 + k] = s;
+}
+
 bool cw_bwd_supports(int C) { return C >= 1 && C <= 64; }
+
+size_t geom_workspace_bytes(int B, int V, int H, int W) {
+  const size_t nblk = ((size_t)H * W + 31) / 32;               // 32 pixels (128 threads, 4 lanes each) per block
+  return (size_t)B * V * 12 * nblk * sizeof(float);
+}
 
 template <int CPL>
 static void launch_cpl(const CwBwdParams& p, int C, int mode, int mask, dim3 grid, cudaStream_t st) {
@@ -249,6 +359,54 @@ static void launch_cpl(const CwBwdParams& p, int C, int mode, int mask, dim3 gri
 }
 
 cudaError_t launch_cost_cw_bwd_mma(const CwBwdParams& p, int mode, int layout, cudaStream_t st);   // cost_f_bwd_mma.cu
+
+template <int CPL>
+static void launch_geom_cpl(const CwBwdParams& p, const GeomOut& go, int C, int mode, int mask, dim3 grid,
+                            cudaStream_t st) {
+  if (mode == MAGNET_DEPTH_PLANES) {
+    cost_geom_bwd_kernel<CPL, MAGNET_DEPTH_PLANES, MASK_MMA><<<grid, 128, 0, st>>>(p, C, go);
+  } else if (mode == MAGNET_DEPTH_VOLUME) {
+    if (mask == MASK_MMA) cost_geom_bwd_kernel<CPL, MAGNET_DEPTH_VOLUME, MASK_MMA><<<grid, 128, 0, st>>>(p, C, go);
+    else cost_geom_bwd_kernel<CPL, MAGNET_DEPTH_VOLUME, MASK_DIRECT><<<grid, 128, 0, st>>>(p, C, go);
+  } else {
+    if (mask == MASK_MMA) cost_geom_bwd_kernel<CPL, MAGNET_DEPTH_GAUSS, MASK_MMA><<<grid, 128, 0, st>>>(p, C, go);
+    else cost_geom_bwd_kernel<CPL, MAGNET_DEPTH_GAUSS, MASK_DIRECT><<<grid, 128, 0, st>>>(p, C, go);
+  }
+}
+
+// Camera (and optionally ray and depth) gradients: g_score (softmax or not) into p.g_score, the GEOM walk with
+// per-block partials into `partials`, then the fixed-order reduction into grad_cams (B*V, 12).  Three launches.
+cudaError_t launch_cost_geom_bwd(const CwBwdParams& p, int C, int mode, bool mask_mma, int softmax, const float* prob,
+                                 const float* grad_out, float* partials, float* grad_rays, float* grad_cams,
+                                 cudaStream_t st, int* launches) {
+  BwdParams s;
+  s.B = p.B; s.V = p.V; s.D = p.D; s.C = C; s.H = p.H; s.W = p.W; s.HW = p.HW;
+  s.softmax = softmax;
+  s.vf = (float)p.V;
+  s.ref_feat = s.src_feat = s.rays = nullptr;
+  s.cams = nullptr;
+  s.prob = prob;
+  s.grad_out = grad_out;
+  s.g_score = const_cast<float*>(p.g_score);
+  s.grad_ref = s.grad_src = nullptr;
+  cudaError_t e = launch_score_grad(s, st);
+  if (e != cudaSuccess) return e;
+  GeomOut go;
+  go.partials = partials;
+  go.grad_rays = grad_rays;
+  const dim3 grid((4 * p.HW + 127) / 128, p.B);
+  const int mask = mask_mma || mode == MAGNET_DEPTH_PLANES ? MASK_MMA : MASK_DIRECT;
+  if (C <= 4) launch_geom_cpl<1>(p, go, C, mode, mask, grid, st);
+  else if (C <= 8) launch_geom_cpl<2>(p, go, C, mode, mask, grid, st);
+  else if (C <= 16) launch_geom_cpl<4>(p, go, C, mode, mask, grid, st);
+  else if (C <= 32) launch_geom_cpl<8>(p, go, C, mode, mask, grid, st);
+  else if (C <= 64) launch_geom_cpl<16>(p, go, C, mode, mask, grid, st);
+  else return cudaErrorInvalidValue;
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  geom_reduce_kernel<<<p.B * p.V, 384, 0, st>>>(partials, p.cams, (int)grid.x, grad_cams);
+  *launches = 3;
+  return cudaGetLastError();
+}
 
 // p: NCHW maps (CUDA-core kernel).  split: the same call with ref_feat / src_feat pointing to the forward's SPLIT16
 // or HALF16 buffers (split_layout), or NULL.  With split, both feature gradients come from the tensor-core kernel and the CUDA-core kernel only

@@ -19,10 +19,12 @@ per-(batch, view) Python loop):
 Both volumes are differentiable as in the reference: the CW volume w.r.t. both feature maps and the depth volume
 (magnet_cost_volume_bwd_f32; built only when grad mode is on and one of them requires grad, so that G-Net training,
 where none does, runs exactly the no-grad path), the F volume w.r.t. both feature maps (magnet_cost_volume_f_bwd_f32)
-for F-Net training.
+for F-Net training.  Inside ``geometry_grad()`` both are differentiable in the cameras too (R, t, intM and the rays;
+magnet_cost_volume_geom_bwd_f32).
 """
 from __future__ import annotations
 
+import contextlib
 import weakref
 from typing import Dict, Tuple
 
@@ -104,8 +106,8 @@ def _device_intrinsics(cam_intrins, device):
     hit = _cache.get("intr", (intM, rays), (str(device),))
     if hit is not None:
         return hit
-    value = (intM.to(device=device, dtype=torch.float32).contiguous(),
-             rays.to(device=device, dtype=torch.float32).contiguous())
+    value = (intM.detach().to(device=device, dtype=torch.float32).contiguous(),
+             rays.detach().to(device=device, dtype=torch.float32).contiguous())
     return _cache.put("intr", (intM, rays), value, (str(device),))
 
 
@@ -203,9 +205,59 @@ def _packed_source(nghbr_feat, nghbr_gmms, V, variant, ref_feat=None, D=MMA_MIN_
     return hit, _lib.SRC_TILED32, None
 
 
+_geometry_grad = [False]
+
+
+@contextlib.contextmanager
+def geometry_grad(enabled: bool = True):
+    """Inside the block, camera tensors that require grad (R / t, i.e. ``nghbr_poses``, ``intM``,
+    ``unit_ray_array_2D``) get gradients from ``est_costvolume_CW``, ``est_costvolume_F``, ``plane_sweep_f`` (``MagnetF``)
+    and ``MatchingPlan.cost``, as the reference's operators give them (DESIGN §3.11).  Off by default: outside the
+    block the CW volume and ``MatchingPlan`` refuse such tensors.  A context manager, so that callers that cannot pass
+    a keyword (``MAGNET.forward``, ``train_FNet.py``) run unchanged inside it."""
+    prev = _geometry_grad[0]
+    _geometry_grad[0] = bool(enabled)
+    try:
+        yield
+    finally:
+        _geometry_grad[0] = prev
+
+
+def geometry_grad_enabled() -> bool:
+    return _geometry_grad[0]
+
+
+def camera_inputs(R, t, cam_intrins):
+    """The caller's camera tensors, in the order the autograd Functions take them: R, t, intM, rays."""
+    return R, t, cam_intrins['intM'], cam_intrins['unit_ray_array_2D']
+
+
+def wants_camera_grad(cam_inputs) -> bool:
+    """Camera gradients are computed only under geometry_grad() and when one of the camera tensors requires grad."""
+    return geometry_grad_enabled() and wants_cw_grad(*cam_inputs)
+
+
+def _detached(*xs):
+    """The camera tensors as saved for backward: detached views, which share the version counter, so an in-place update
+    of a pose between forward and backward raises as it does in autograd."""
+    return tuple(None if x is None else x.detach() for x in xs)
+
+
+def camera_grads(ctx, g_cams, g_rays, cam_inputs):
+    """(grad_R, grad_t, grad_intM, grad_rays) from the kernel's (B*V,12) table and ray gradient, each in its input's
+    dtype and on its input's device, None where not wanted (ctx.needs_input_grad of the last four inputs).
+    cam_inputs: the saved (R, t, intM, rays)."""
+    R, t, intM, rays = cam_inputs
+    need = ctx.needs_input_grad[-4:]
+    gR, gt, gK = ops.camera_chain(g_cams, intM.detach().to(g_cams.device), R.detach(), t.detach())
+    out = [gR, gt, gK, None if g_rays is None else g_rays.reshape(rays.shape)]
+    return tuple(None if not n or g is None else g.to(device=x.device, dtype=x.dtype)
+                 for n, g, x in zip(need, out, cam_inputs))
+
+
 def check_geometry_grad(**named) -> None:
-    """The cost volume is differentiable in the feature maps and the depths only: raise instead of silently dropping
-    the gradient of a camera tensor."""
+    """Outside geometry_grad() the cost volume is differentiable in the feature maps and the depths only: raise instead
+    of silently dropping the gradient of a camera tensor."""
     for name, x in named.items():
         if isinstance(x, torch.Tensor) and x.requires_grad:
             raise _lib.MagnetError(f"{name} requires grad, but the cost volume is differentiable only in the feature "
@@ -227,28 +279,41 @@ class _CostVolumeCW(torch.autograd.Function):
     no gradient (the mask is piecewise constant)."""
 
     @staticmethod
-    def forward(ctx, depth, ref_feat, nghbr_feat, nghbr_gmms, run, spec):
+    def forward(ctx, depth, ref_feat, nghbr_feat, nghbr_gmms, run, spec, R=None, t=None, intM=None, rays=None):
         out, layout, variant, splits = run()
-        ctx.save_for_backward(depth.detach(), ref_feat.detach(), nghbr_feat.detach(), nghbr_gmms.detach())
+        ctx.save_for_backward(depth.detach(), ref_feat.detach(), nghbr_feat.detach(), nghbr_gmms.detach(),
+                              *_detached(R, t, intM, rays))
         ctx.spec, ctx.fwd, ctx.splits = spec, (layout, variant), splits or (None, None)
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
-        depth, ref_in, src_in, gmm = ctx.saved_tensors
+        depth, ref_in, src_in, gmm, *cam_saved = ctx.saved_tensors
         rays, cams, V, kappa, karr = ctx.spec
         need_d, need_ref, need_src = ctx.needs_input_grad[:3]
-        # the CUDA-core kernel reads fp32 NCHW maps: always after a non-HALF16 forward, for the depth gradient after one
-        upcast = need_d or ctx.fwd[0] != _lib.SRC_HALF16
-        ref, src = (ref_in.float(), src_in.float()) if upcast else (ref_in, src_in)
-        g_ref, g_src, g_d = ops.cost_volume_bwd(
-            ref, src, gmm.float(), rays, cams, grad_out.contiguous(), V=V, kappa=kappa,
-            d_volume=depth if karr is None else None, ref_gmm=depth if karr is not None else None, k=karr,
-            fwd_layout=ctx.fwd[0], fwd_variant=ctx.fwd[1], need_ref=need_ref, need_src=need_src, need_depth=need_d,
-            ref_split=ctx.splits[0], src_split=ctx.splits[1])
-        g_ref = None if g_ref is None else g_ref.to(ref_in.dtype)
-        g_src = None if g_src is None else g_src.to(src_in.dtype)
-        return g_d, g_ref, g_src, None, None, None
+        need_cam = any(ctx.needs_input_grad[6:])
+        depth_src = dict(d_volume=depth if karr is None else None, ref_gmm=depth if karr is not None else None, k=karr)
+        # the existing entry point computes the feature and depth gradients exactly as without camera gradients (the
+        # camera kernel's own depth gradient can differ from it in the last bit, DESIGN §3.11); the camera entry point
+        # adds the camera and ray gradients
+        g_ref = g_src = g_d = None
+        if need_ref or need_src or need_d:
+            # the CUDA-core kernel reads fp32 NCHW maps: always after a non-HALF16 forward, for the depth gradient after one
+            upcast = need_d or ctx.fwd[0] != _lib.SRC_HALF16
+            ref, src = (ref_in.float(), src_in.float()) if upcast else (ref_in, src_in)
+            g_ref, g_src, g_d = ops.cost_volume_bwd(
+                ref, src, gmm.float(), rays, cams, grad_out.contiguous(), V=V, kappa=kappa, **depth_src,
+                fwd_layout=ctx.fwd[0], fwd_variant=ctx.fwd[1], need_ref=need_ref, need_src=need_src,
+                need_depth=need_d, ref_split=ctx.splits[0], src_split=ctx.splits[1])
+            g_ref = None if g_ref is None else g_ref.to(ref_in.dtype)
+            g_src = None if g_src is None else g_src.to(src_in.dtype)
+        g_cam = (None,) * 4
+        if need_cam:
+            g_cams, g_rays, _ = ops.cost_volume_geom_bwd(
+                ref_in.float(), src_in.float(), gmm.float(), rays, cams, grad_out.contiguous(), V=V, kappa=kappa,
+                **depth_src, fwd_layout=ctx.fwd[0], fwd_variant=ctx.fwd[1], need_rays=ctx.needs_input_grad[9])
+            g_cam = camera_grads(ctx, g_cams, g_rays, cam_saved)
+        return (g_d, g_ref, g_src, None, None, None) + g_cam
 
 
 def differentiable_layout(C: int, V: int, D: int, variant: int, split16_ok: bool = True, half=False) -> int:
@@ -276,15 +341,17 @@ def est_costvolume_CW(d_volume, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms,
     views; is_valid (B,V) int CPU or device; cam_intrins dict of 'intM' (B,3,3) and
     'unit_ray_array_2D' (B,3,H*W), CPU or device; thres int.  Returns (B,D,H,W) float32 on
     ref_feat.device, freshly allocated.  Differentiable, as the reference, in d_volume, ref_feat and nghbr_feat when
-    grad mode is on and one of them requires grad (the camera tensors must not require grad); detached otherwise.
+    grad mode is on and one of them requires grad; in R, t, intM and the rays too inside geometry_grad() (outside it the
+    camera tensors must not require grad); detached otherwise.
     Any of the tensors may be fp16 / bf16 (torch.autocast): the volume is fp32, each gradient has its input's dtype."""
     device = ref_feat.device
     B = d_volume.shape[0]
     V = int(nghbr_feat.shape[0] / B)
-    if torch.is_grad_enabled():
+    cam_in = camera_inputs(R, t, cam_intrins)
+    if torch.is_grad_enabled() and not geometry_grad_enabled():
         check_geometry_grad(R=R, t=t, intM=cam_intrins['intM'], unit_ray_array_2D=cam_intrins['unit_ray_array_2D'])
     d_volume = d_volume.float()                            # differentiable upcast (a no-op for fp32)
-    if wants_cw_grad(d_volume, ref_feat, nghbr_feat):
+    if wants_cw_grad(d_volume, ref_feat, nghbr_feat) or wants_camera_grad(cam_in):
         D, C = int(d_volume.shape[1]), int(ref_feat.shape[1])
         half = wants_half16(ref_feat.dtype, nghbr_feat.dtype, C, V, variant, D)
         layout = differentiable_layout(C, V, D, variant, half=half)
@@ -304,7 +371,7 @@ def est_costvolume_CW(d_volume, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms,
             return out, layout, fv, (ref_split, src) if layout in ops.PACKED_LAYOUTS else None
 
         return _CostVolumeCW.apply(d_volume, ref_feat, nghbr_feat, nghbr_gmms, run,
-                                   (rays_d, cams, V, float(thres), None))
+                                   (rays_d, cams, V, float(thres), None), *cam_in)
     with torch.no_grad():
         _, rays_d = _device_intrinsics(cam_intrins, device)
         cams = _camera_table(cam_intrins, R, t, is_valid, device)
@@ -328,21 +395,31 @@ class _CostVolumeF(torch.autograd.Function):
     """Plane-sweep probability volume for F-Net training (homography.py:10-75), forward + backward kernels."""
 
     @staticmethod
-    def forward(ctx, ref_feat, nghbr_feat, planes, rays_d, cams, V, variant):
+    def forward(ctx, ref_feat, nghbr_feat, planes, rays_d, cams, V, variant, R=None, t=None, intM=None, rays=None):
         src, layout, ref_split = _packed_source(nghbr_feat, None, V, variant, ref_feat, len(planes))
         ref = (ref_feat if layout == _lib.SRC_HALF16 else _f32(ref_feat)).detach()
         out = ops.cost_volume(ref, src, rays_d, cams, V=V, src_layout=layout, consistency=False,
                               k=planes, planes=True, softmax=True, variant=variant, ref_split=ref_split)
-        ctx.save_for_backward(ref_feat.detach(), nghbr_feat.detach(), out, rays_d, cams)
+        ctx.save_for_backward(ref_feat.detach(), nghbr_feat.detach(), out, rays_d, cams, *_detached(R, t, intM, rays))
         ctx.planes, ctx.V = planes, V
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
-        ref_feat, nghbr_feat, out, rays_d, cams = ctx.saved_tensors
-        g_ref, g_src = ops.cost_volume_f_bwd(ref_feat.float(), nghbr_feat.float(), rays_d, cams, ctx.planes, ctx.V, out,
-                                             grad_out.contiguous(), softmax=True)
-        return g_ref.to(ref_feat.dtype), g_src.to(nghbr_feat.dtype), None, None, None, None, None
+        ref_feat, nghbr_feat, out, rays_d, cams, *cam_saved = ctx.saved_tensors
+        if not any(ctx.needs_input_grad[7:]):
+            g_ref, g_src = ops.cost_volume_f_bwd(ref_feat.float(), nghbr_feat.float(), rays_d, cams, ctx.planes, ctx.V,
+                                                 out, grad_out.contiguous(), softmax=True)
+            return g_ref.to(ref_feat.dtype), g_src.to(nghbr_feat.dtype), None, None, None, None, None, None, None, None, None
+        g_ref = g_src = None
+        if any(ctx.needs_input_grad[:2]):
+            g_ref, g_src = ops.cost_volume_f_bwd(ref_feat.float(), nghbr_feat.float(), rays_d, cams, ctx.planes, ctx.V,
+                                                 out, grad_out.contiguous(), softmax=True)
+            g_ref, g_src = g_ref.to(ref_feat.dtype), g_src.to(nghbr_feat.dtype)
+        g_cams, g_rays, _ = ops.cost_volume_geom_bwd(ref_feat.float(), nghbr_feat.float(), None, rays_d, cams,
+                                                     grad_out.contiguous(), V=ctx.V, k=ctx.planes, planes=True,
+                                                     softmax=True, prob=out, need_rays=ctx.needs_input_grad[10])
+        return (g_ref, g_src, None, None, None, None, None) + camera_grads(ctx, g_cams, g_rays, cam_saved)
 
 
 class _PlaneSweepF(torch.autograd.Function):
@@ -352,12 +429,13 @@ class _PlaneSweepF(torch.autograd.Function):
     the CUDA-core kernel reads the NCHW maps."""
 
     @staticmethod
-    def forward(ctx, ref_feat, nghbr_feat, planes, rays_d, cams, V, softmax):
+    def forward(ctx, ref_feat, nghbr_feat, planes, rays_d, cams, V, softmax, R=None, t=None, intM=None, rays=None):
         src, layout, ref_split = _packed_source(nghbr_feat, None, V, _lib.VARIANT_AUTO, ref_feat, len(planes))
         ref = (ref_feat if layout == _lib.SRC_HALF16 else _f32(ref_feat)).detach()
         out = ops.cost_volume(ref, src, rays_d, cams, V=V, src_layout=layout, consistency=False,
                               k=planes, planes=True, softmax=softmax, ref_split=ref_split)
-        ctx.save_for_backward(ref_feat.detach(), nghbr_feat.detach(), out if softmax else None, rays_d, cams)
+        ctx.save_for_backward(ref_feat.detach(), nghbr_feat.detach(), out if softmax else None, rays_d, cams,
+                              *_detached(R, t, intM, rays))
         ctx.splits = (ref_split, src) if layout in ops.PACKED_LAYOUTS else (None, None)
         ctx.layout = layout
         ctx.planes, ctx.V, ctx.softmax = planes, V, softmax
@@ -365,37 +443,58 @@ class _PlaneSweepF(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out):
-        ref_feat, nghbr_feat, out, rays_d, cams = ctx.saved_tensors
+        ref_feat, nghbr_feat, out, rays_d, cams, *cam_saved = ctx.saved_tensors
         ref_split, src_split = ctx.splits
-        if ctx.layout == _lib.SRC_HALF16:                  # the NCHW maps only supply the shapes
-            ref, src = ref_feat, nghbr_feat
-        else:
-            ref, src = ref_feat.float(), nghbr_feat.float()
-        g_ref, g_src = ops.cost_volume_f_bwd(ref, src, rays_d, cams, ctx.planes, ctx.V, out,
-                                             grad_out.contiguous(), softmax=ctx.softmax, ref_split=ref_split,
-                                             src_split=src_split, split_layout=ctx.layout)
-        return g_ref.to(ref_feat.dtype), g_src.to(nghbr_feat.dtype), None, None, None, None, None
+        need_cam = any(ctx.needs_input_grad[7:])
+        g_ref = g_src = None
+        if not need_cam or any(ctx.needs_input_grad[:2]):
+            if ctx.layout == _lib.SRC_HALF16:              # the NCHW maps only supply the shapes
+                ref, src = ref_feat, nghbr_feat
+            else:
+                ref, src = ref_feat.float(), nghbr_feat.float()
+            g_ref, g_src = ops.cost_volume_f_bwd(ref, src, rays_d, cams, ctx.planes, ctx.V, out,
+                                                 grad_out.contiguous(), softmax=ctx.softmax, ref_split=ref_split,
+                                                 src_split=src_split, split_layout=ctx.layout)
+            g_ref, g_src = g_ref.to(ref_feat.dtype), g_src.to(nghbr_feat.dtype)
+        if not need_cam:
+            return g_ref, g_src, None, None, None, None, None, None, None, None, None
+        g_cams, g_rays, _ = ops.cost_volume_geom_bwd(ref_feat.float(), nghbr_feat.float(), None, rays_d, cams,
+                                                     grad_out.contiguous(), V=ctx.V, k=ctx.planes, planes=True,
+                                                     softmax=ctx.softmax, prob=out, need_rays=ctx.needs_input_grad[10])
+        return (g_ref, g_src, None, None, None, None, None) + camera_grads(ctx, g_cams, g_rays, cam_saved)
+
+
+def _f_camera_inputs(d_center, R, t, cam_intrins):
+    """The camera inputs of the F volume's autograd Functions: the caller's tensors under geometry_grad() (a d_center
+    that requires grad is refused there: the planes are host constants), else none, as before."""
+    if not geometry_grad_enabled():
+        return ()
+    if torch.is_grad_enabled() and isinstance(d_center, torch.Tensor) and d_center.requires_grad:
+        raise _lib.MagnetError("d_center requires grad, but the plane depths are constants of the F volume (detach it)")
+    return camera_inputs(R, t, cam_intrins)
 
 
 def plane_sweep_f(d_center, ref_feat, nghbr_feat, R, t, is_valid, cam_intrins, softmax=True):
     """The F volume of est_costvolume_F (softmax=True) or its 1/V-averaged scores (softmax=False), with the
     tensor-core backward where the forward ran on the tensor cores (MagnetF's path; est_costvolume_F keeps the
     CUDA-core backward)."""
+    cam_in = _f_camera_inputs(d_center, R, t, cam_intrins)
     device = ref_feat.device
     V = int(nghbr_feat.shape[0] / ref_feat.shape[0])
     planes = _plane_list(d_center)
     _, rays_d = _device_intrinsics(cam_intrins, device)
     cams = _camera_table(cam_intrins, R, t, is_valid, device)
-    return _PlaneSweepF.apply(ref_feat, nghbr_feat, planes, rays_d, cams, V, softmax)
+    return _PlaneSweepF.apply(ref_feat, nghbr_feat, planes, rays_d, cams, V, softmax, *cam_in)
 
 
 def est_costvolume_F(d_center, ref_feat, nghbr_feat, R, t, is_valid, cam_intrins, variant=_lib.VARIANT_AUTO):
     """Fronto-parallel plane-sweep volume with softmax over planes — drop-in (forward) for
     homography.est_costvolume_F.  d_center (1,D,1,1); the rest as in est_costvolume_CW."""
+    cam_in = _f_camera_inputs(d_center, R, t, cam_intrins)
     device = ref_feat.device
     B = ref_feat.shape[0]
     V = int(nghbr_feat.shape[0] / B)
     planes = _plane_list(d_center)
     _, rays_d = _device_intrinsics(cam_intrins, device)
     cams = _camera_table(cam_intrins, R, t, is_valid, device)
-    return _CostVolumeF.apply(ref_feat, nghbr_feat, planes, rays_d, cams, V, variant)
+    return _CostVolumeF.apply(ref_feat, nghbr_feat, planes, rays_d, cams, V, variant, *cam_in)

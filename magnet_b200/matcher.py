@@ -16,8 +16,8 @@ import torch
 import torch.nn as nn
 
 from . import _lib, ops
-from .homography import (MMA_MIN_PLANES, _CostVolumeCW, check_geometry_grad, differentiable_layout,
-                         wants_cw_grad)
+from .homography import (MMA_MIN_PLANES, _CostVolumeCW, camera_inputs, check_geometry_grad, differentiable_layout,
+                         geometry_grad_enabled, wants_cw_grad)
 from .ops import HALF_DTYPES, PACKED_LAYOUTS
 from .sampling import depth_sampling
 
@@ -69,9 +69,13 @@ class MatchingPlan:
 
     def __init__(self, ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, *,
                  thres: int = 5, src_layout: int = _lib.SRC_SPLIT16):
-        if torch.is_grad_enabled():
+        if torch.is_grad_enabled() and not geometry_grad_enabled():
             check_geometry_grad(nghbr_poses=nghbr_poses, intM=cam_intrins['intM'],
                                 unit_ray_array_2D=cam_intrins['unit_ray_array_2D'])
+        # the caller's camera tensors: a plan built under geometry_grad() is differentiable in them on every cost()
+        # call, wherever that call runs (the switch is latched here); a plan built outside never is
+        self._cam_in = camera_inputs(nghbr_poses[:, :, :3, :3], nghbr_poses[:, :, :3, 3], cam_intrins) \
+            if geometry_grad_enabled() else (None,) * 4
         dev = ref_feat.device
         self.B, self.C, self.H, self.W = ref_feat.shape
         self.V = nghbr_feat.shape[0] // self.B
@@ -81,9 +85,9 @@ class MatchingPlan:
         # the half dtype of both feature maps (tensor-core kernels on HALF16 buffers), or None (fp32 maps, or upcast)
         self.half = ref_feat.dtype if ref_feat.dtype == nghbr_feat.dtype and ref_feat.dtype in HALF_DTYPES else None
         self._f32 = {}
-        self.rays = cam_intrins['unit_ray_array_2D'].to(dev, torch.float32).contiguous()
-        intM = cam_intrins['intM'].to(dev, torch.float32).contiguous()
-        R, t = nghbr_poses[:, :, :3, :3], nghbr_poses[:, :, :3, 3]
+        self.rays = cam_intrins['unit_ray_array_2D'].detach().to(dev, torch.float32).contiguous()
+        intM = cam_intrins['intM'].detach().to(dev, torch.float32).contiguous()
+        R, t = nghbr_poses.detach()[:, :, :3, :3], nghbr_poses.detach()[:, :, :3, 3]
         self.cams = ops.pack_cameras(intM, R, t, is_valid.to(dev, torch.int32))
         self._nghbr_feat = nghbr_feat.detach()
         self._ref_in, self._src_in = ref_feat, nghbr_feat   # the caller's tensors: cost() is differentiable in them
@@ -140,7 +144,7 @@ class MatchingPlan:
         and in ``gmm`` when grad mode is on and one of them requires grad (then ``out`` must be None); detached
         otherwise."""
         gmm = gmm.float()                                  # differentiable upcast (a no-op for fp32)
-        if wants_cw_grad(gmm, self._ref_in, self._src_in):
+        if wants_cw_grad(gmm, self._ref_in, self._src_in, *self._cam_in):
             return self._cost_differentiable(gmm, k, out, variant)
         layout = self.layout
         n_planes = len(k)
@@ -177,7 +181,7 @@ class MatchingPlan:
             return vol, layout, fv, (self._ref_split, src) if packed else None
 
         return _CostVolumeCW.apply(gmm, self._ref_in, self._src_in, self.src_gmm, run,
-                                   (self.rays, self.cams, self.V, self.kappa, karr))
+                                   (self.rays, self.cams, self.V, self.kappa, karr), *self._cam_in)
 
 
 def matching_loop(plan: MatchingPlan, ref_gmms: torch.Tensor, x_d3: torch.Tensor,

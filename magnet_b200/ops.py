@@ -420,6 +420,97 @@ def cost_volume_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V: int
     return g_ref, g_src, g_d
 
 
+def geom_workspace_bytes(B: int, V: int, H: int, W: int) -> int:
+    """Bytes of the workspace of cost_volume_geom_bwd (per-block partials of the camera gradients)."""
+    return int(lib().magnet_cost_geom_workspace_bytes(B, V, H, W))
+
+
+def cost_volume_geom_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V: int, kappa: float = 0.0,
+                         consistency=True, d_volume=None, ref_gmm=None, k=None, planes=False, softmax=False, prob=None,
+                         fwd_layout=_lib.SRC_NCHW, fwd_variant=_lib.VARIANT_DIRECT, need_rays=True, need_depth=False):
+    """Camera gradients of either cost volume — one magnet_cost_volume_geom_bwd_f32 call.  ref_feat (B,C,H,W) and
+    src_feat (V*B,C,H,W) are the NCHW fp32 maps; the depth source is ``d_volume``, ``ref_gmm`` + ``k``, or ``k`` with
+    ``planes=True`` (the F volume: no consistency, ``softmax`` with the forward output ``prob``).  ``fwd_layout`` /
+    ``fwd_variant`` name the CW forward kernel, whose mask is applied.  Returns (grad_cams (B*V,12): d/d(K R) row-major
+    then d/d(K t); grad_rays (B,3,H*W) or None; grad_depth or None), float32."""
+    ref_feat = _need_cuda_f32("ref_feat", ref_feat)
+    src = _need_cuda_f32("src_feat", src_feat)
+    rays = _need_cuda_f32("rays", rays)
+    cams = _need_cuda_f32("cams", cams)
+    grad_out = _need_cuda_f32("grad_out", grad_out)
+    B, Cc, H, W = ref_feat.shape
+    _expect("src_feat", src, (V * B, Cc, H, W))
+    _expect("rays", rays, (B, 3, H * W))
+    if cams.numel() != B * V * 16:
+        raise _lib.MagnetError(f"cams must hold B*V = {B * V} camera records of 16 floats, got {tuple(cams.shape)}")
+    a = CostArgs()
+    a.B, a.V, a.C, a.H, a.W = B, V, Cc, H, W
+    a.src_layout, a.variant, a.kappa = fwd_layout, fwd_variant, float(kappa)
+    a.consistency, a.softmax = 1 if consistency and not planes else 0, 1 if softmax else 0
+    a.rays, a.cams = rays.data_ptr(), cams.data_ptr()
+    karr = None
+    if d_volume is not None:
+        d_volume = _need_cuda_f32("d_volume", d_volume)
+        if d_volume.dim() != 4 or d_volume.shape[0] != B or tuple(d_volume.shape[2:]) != (H, W):
+            raise _lib.MagnetError(f"d_volume must be (B,D,H,W) = ({B},D,{H},{W}), got {tuple(d_volume.shape)}")
+        a.depth_mode, a.D, a.d_volume = _lib.DEPTH_VOLUME, d_volume.shape[1], d_volume.data_ptr()
+        gd_shape = tuple(d_volume.shape)
+    else:
+        karr = k if isinstance(k, C.Array) else k_array(k)
+        a.D, a.k_host = len(karr), C.cast(karr, C.c_void_p)
+        if planes:
+            a.depth_mode = _lib.DEPTH_PLANES
+            gd_shape = None
+        else:
+            ref_gmm = _need_cuda_f32("ref_gmm", ref_gmm)
+            _expect("ref_gmm", ref_gmm, (B, 2, H, W))
+            a.depth_mode, a.ref_gmm = _lib.DEPTH_GAUSS, ref_gmm.data_ptr()
+            gd_shape = (B, 2, H, W)
+    if need_depth and gd_shape is None:
+        raise _lib.MagnetError("the plane depths of the F volume are constants: no depth gradient")
+    _expect("grad_out", grad_out, (B, a.D, H, W))
+    bw = _lib.CostGeomBwdArgs()
+    bw.fwd = C.pointer(a)
+    bw.ref_feat, bw.src_feat = ref_feat.data_ptr(), src.data_ptr()
+    if a.consistency:
+        src_gmm = _need_cuda_f32("src_gmm", src_gmm)
+        _expect("src_gmm", src_gmm, (V * B, 2, H, W))
+        bw.src_gmm = src_gmm.data_ptr()
+    if softmax:
+        prob = _need_cuda_f32("prob", prob)
+        _expect("prob", prob, (B, a.D, H, W))
+        bw.prob = prob.data_ptr()
+    dev = _same_device(("ref_feat", ref_feat), ("src_feat", src), ("src_gmm", src_gmm if a.consistency else None),
+                       ("rays", rays), ("cams", cams), ("grad_out", grad_out), ("d_volume", d_volume),
+                       ("ref_gmm", ref_gmm), ("prob", prob if softmax else None))
+    score = torch.empty_like(grad_out)
+    work = torch.empty(geom_workspace_bytes(B, V, H, W), device=dev, dtype=torch.uint8)
+    g_cams = torch.empty(B * V, 12, device=dev, dtype=torch.float32)
+    g_rays = torch.empty(B, 3, H * W, device=dev, dtype=torch.float32) if need_rays else None
+    g_d = torch.empty(gd_shape, device=dev, dtype=torch.float32) if need_depth else None
+    bw.score, bw.workspace, bw.grad_out, bw.grad_cams = score.data_ptr(), work.data_ptr(), grad_out.data_ptr(), g_cams.data_ptr()
+    bw.grad_rays = g_rays.data_ptr() if need_rays else None
+    bw.grad_depth = g_d.data_ptr() if need_depth else None
+    with torch.cuda.device(dev):
+        check(lib().magnet_cost_volume_geom_bwd_f32(C.byref(bw), _stream(dev)), "magnet_cost_volume_geom_bwd_f32")
+    return g_cams, g_rays, g_d
+
+
+def camera_chain(grad_cams, intM, R, t):
+    """d/dA and d/da of the camera table (grad_cams (B*V,12), A = K R, a = K t) -> (grad_R (B,V,3,3), grad_t (B,V,3),
+    grad_K (B,3,3)) by the chain rule of the reference's grouping (K R) Ray and K t: grad_R = K^T grad_A, grad_t =
+    K^T grad_a, grad_K = sum_v (grad_A R^T + grad_a t^T).  Small batched matmuls in the dtype of grad_cams."""
+    B, V = R.shape[:2]
+    g = grad_cams.reshape(B, V, 12)
+    gA, ga = g[..., :9].reshape(B, V, 3, 3), g[..., 9:]
+    K = intM.to(g).unsqueeze(1)
+    R, t = R.to(g), t.to(g)
+    grad_R = K.transpose(-1, -2) @ gA
+    grad_t = (K.transpose(-1, -2) @ ga.unsqueeze(-1)).squeeze(-1)
+    grad_K = (gA @ R.transpose(-1, -2) + ga.unsqueeze(-1) * t.unsqueeze(-2)).sum(1)
+    return grad_R, grad_t, grad_K
+
+
 def cost_launch_info(B, V, D, Cc, H, W, variant=_lib.VARIANT_AUTO):
     """(grid CTAs, threads per CTA, dynamic smem bytes) the cost kernel would use for these sizes."""
     a = CostArgs()
