@@ -246,8 +246,10 @@ __global__ void camera_rays_kernel(const double* __restrict__ raw, int H, int W,
   if (n >= H * W) return;
   const int x = n % W, y = n / W;
   const size_t HW = (size_t)H * W;
-  rays[(b * 3 + 0) * HW + n] = (float)((((((double)x + 0.5) * (iw / (double)W)) - cx) + left) / fx);
-  rays[(b * 3 + 1) * HW + n] = (float)((((((double)y + 0.5) * (ih / (double)H)) - cy) + top) / fy);
+  // the product is rounded before cx is subtracted, as numpy does: a contracted fma would differ from the reference
+  // wherever the pixel-centre position is not exact in fp64 (by far more than an ulp where it cancels against cx)
+  rays[(b * 3 + 0) * HW + n] = (float)((__dadd_rn(__dmul_rn((double)x + 0.5, iw / (double)W), -cx) + left) / fx);
+  rays[(b * 3 + 1) * HW + n] = (float)((__dadd_rn(__dmul_rn((double)y + 0.5, ih / (double)H), -cy) + top) / fy);
   rays[(b * 3 + 2) * HW + n] = 1.0f;
 }
 
