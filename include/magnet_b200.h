@@ -362,6 +362,37 @@ int magnet_gnet_train_fwd_f32(const magnet_gnet_train_args* args, void* stream);
 int magnet_gnet_bwd_f32(const magnet_gnet_train_args* args, void* stream);
 
 /*
+ * Mask head and learned upsampling of inference, fused (DESIGN §3.12) — replaces, after the reference's first mask-head
+ * convolution, the rest of mask_head (models/MAGNET.py:111-118) and upsample_depth_via_mask (MAGNET.py:15-27,172-173)
+ * of every prediction:
+ *   h0 = ReLU(pre0),  h1 = ReLU(W1 h0 + b1),  h2 = ReLU(W2 h1 + b2),  mask = W3 h2 + b3 (144 = 9 x k x k channels),
+ *   out[p] = the convex upsampling of pred[p] by the mask, for p < P.
+ * One kernel on the fp16 tensor cores with fp32 accuracy (SPLIT16 products, as the G-Net head); neither the hidden
+ * maps nor the mask are written.  For equal mask logits the upsampling is bit-identical to
+ * magnet_convex_upsample_fwd_f32.  Forward only; no atomics, so results are bit-identical from run to run.
+ *
+ * magnet_mask_pack_weights_f32 writes the weights in the kernel's layout into `packed` (magnet_mask_weights_bytes(4)
+ * bytes, 16-byte aligned): w1 / w2 (128, 128), b1 / b2 (128), w3 (144, 128), b3 (144).  Two kernels.
+ * magnet_mask_weights_bytes returns 0 for any k other than 4 (the only factor the kernel takes).
+ *
+ * magnet_mask_upsample_f32: one kernel.  P outside 1..MAGNET_MASK_MAX_PRED or k != 4 -> MAGNET_ERR_UNSUPPORTED;
+ * B*H*W < 2^31; pre0, packed_weights and every pred / out pointer 16-byte aligned.
+ */
+#define MAGNET_MASK_MAX_PRED 8
+typedef struct magnet_mask_upsample_args {
+  int32_t P, B, H, W;        /* predictions, images, quarter-resolution size                                        */
+  int32_t k;                 /* upsampling factor: 4                                                                */
+  const float* pre0;         /* (B, 128, H, W) the first mask-head convolution's output, before its ReLU             */
+  const void* packed_weights;/* magnet_mask_pack_weights_f32 output                                                 */
+  const float* const* pred;  /* HOST array of P DEVICE pointers, each (B, 2, H, W) [mu, sigma]                      */
+  float* const* out;         /* HOST array of P DEVICE pointers, each (B, 2, k*H, k*W); must not overlap the inputs  */
+} magnet_mask_upsample_args;
+size_t magnet_mask_weights_bytes(int32_t k);
+int magnet_mask_pack_weights_f32(const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
+                                 const float* b3, void* packed, void* stream);
+int magnet_mask_upsample_f32(const magnet_mask_upsample_args* args, void* stream);
+
+/*
  * Caller-side camera preparation on the device (SURVEY §8 f-4).
  * magnet_relative_poses_f32 replaces utils/utils.py:72-98 (data_preprocess): poses_out[b,v] = ext_nghbr[v,b] *
  * inv(ext_ref[b]) (ref-camera -> source-camera), is_valid_out[b,v] = 0 when either extrinsic or the product holds a

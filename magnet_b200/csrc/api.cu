@@ -79,6 +79,11 @@ cudaError_t launch_gnet_pack(const float* w0, const float* w1, const float* b1, 
 cudaError_t launch_gnet_update(int B, int D, int H, int W, const float* cost, const float* inv, const void* weights,
                                const float* prev, unsigned* scratch, float* out, cudaStream_t st);
 size_t gnet_train_weights_bytes(int D);
+size_t mask_weights_bytes();
+cudaError_t launch_mask_pack(const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
+                             const float* b3, void* dst, cudaStream_t st);
+cudaError_t launch_mask_upsample(int P, int B, int H, int W, const float* pre0, const void* weights,
+                                 const float* const* pred, float* const* out, cudaStream_t st);
 size_t gnet_saved_bytes(int B, int H, int W);
 size_t gnet_bwd_workspace_bytes(int B, int D, int H, int W);
 cudaError_t launch_gnet_pack_train(const float* w0, const float* w1, const float* b1, const float* w2, const float* b2,
@@ -725,6 +730,36 @@ int magnet_gnet_bwd_f32(const magnet_gnet_train_args* a, void* stream) {
                                           (cudaStream_t)stream, &launches);
   if (e != cudaSuccess) return cuda_fail(e);
   g_launches += launches;
+  return MAGNET_OK;
+}
+
+size_t magnet_mask_weights_bytes(int32_t k) { return k == 4 ? magnet::mask_weights_bytes() : 0; }
+
+int magnet_mask_pack_weights_f32(const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
+                                 const float* b3, void* packed, void* stream) {
+  if (!w1 || !b1 || !w2 || !b2 || !w3 || !b3 || !packed) return MAGNET_ERR_NULL;
+  if (misaligned16(packed)) return MAGNET_ERR_ALIGN;
+  cudaError_t e = magnet::launch_mask_pack(w1, b1, w2, b2, w3, b3, packed, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 2;
+  return MAGNET_OK;
+}
+
+int magnet_mask_upsample_f32(const magnet_mask_upsample_args* a, void* stream) {
+  if (!a) return MAGNET_ERR_NULL;
+  if (a->B <= 0 || a->H <= 0 || a->W <= 0) return MAGNET_ERR_SHAPE;
+  if ((int64_t)a->B * a->H * a->W >= ((int64_t)1 << 31)) return MAGNET_ERR_SHAPE;
+  if (a->P < 1 || a->P > MAGNET_MASK_MAX_PRED || a->k != 4) return MAGNET_ERR_UNSUPPORTED;
+  if (!a->pre0 || !a->packed_weights || !a->pred || !a->out) return MAGNET_ERR_NULL;
+  for (int p = 0; p < a->P; ++p)
+    if (!a->pred[p] || !a->out[p]) return MAGNET_ERR_NULL;
+  if (misaligned16(a->pre0) || misaligned16(a->packed_weights)) return MAGNET_ERR_ALIGN;
+  for (int p = 0; p < a->P; ++p)
+    if (misaligned16(a->pred[p]) || misaligned16(a->out[p])) return MAGNET_ERR_ALIGN;
+  cudaError_t e = magnet::launch_mask_upsample(a->P, a->B, a->H, a->W, a->pre0, a->packed_weights, a->pred, a->out,
+                                               (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 1;
   return MAGNET_OK;
 }
 

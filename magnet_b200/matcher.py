@@ -5,8 +5,10 @@ The reference inlines the sampler (MAGNET.py:154-156) and the update (inside GNE
 so they are only reachable through this alternative loop (or the ``GNET`` mirror below); the
 cost-volume function itself is also available as a pure drop-in (``magnet_b200.homography``).
 In inference the per-iteration G-Net head and update run as one fused kernel (``fused_gnet_applies``); with
-``fused_train=True`` so do training iterations of the head (``fused_gnet_trains``, with a fused backward).  Autocast,
-the hoisted x_d3 convolution and the mask head stay ordinary ``nn.Module``s (cuDNN).
+``fused_train=True`` so do training iterations of the head (``fused_gnet_trains``, with a fused backward).  With
+``fused_upsample=True``, inference runs the mask head after its first convolution and the upsampling of every
+prediction as one fused kernel too (``fused_mask_applies``).  Autocast, the hoisted x_d3 convolutions (G-Net's and the
+mask head's first layer) and the mask head of training stay ordinary ``nn.Module``s (cuDNN).
 """
 from __future__ import annotations
 
@@ -258,15 +260,37 @@ def fused_gnet_trains(g_net_convs, cv: torch.Tensor, inv: Optional[torch.Tensor]
     return 1 <= cv.shape[1] <= _lib.MAGNET_MAX_PLANES
 
 
+def fused_mask_applies(mask_head, pre0: Optional[torch.Tensor], preds, k: int) -> bool:
+    """Whether ``MagnetHead(fused_upsample=True).forward`` runs the fused mask head and upsampling
+    (``ops.mask_upsample``) instead of ``mask_head(x_d3)`` + ``convex_upsample`` per prediction: a mask head with the
+    reference's structure and k == 4, nothing to differentiate (grad mode off, or no requires_grad among the mask
+    head's parameters, pre0 and the predictions), no CUDA autocast, fp32 weights, pre0 and predictions.  pre0 may be
+    None when it is not computed yet.  The fused kernel has no backward."""
+    if int(k) != 4 or ops.mask_head_layers(mask_head) is None:
+        return False
+    params = list(mask_head.parameters())
+    preds = [preds] if isinstance(preds, torch.Tensor) else list(preds)
+    tensors = preds + ([pre0] if pre0 is not None else [])
+    if torch.is_grad_enabled() and (any(p.requires_grad for p in params) or any(t.requires_grad for t in tensors)):
+        return False
+    if torch.is_autocast_enabled("cuda"):
+        return False
+    return all(p.dtype == torch.float32 for p in params) and all(t.dtype == torch.float32 for t in tensors)
+
+
 class MagnetHead(nn.Module):
     """G-Net + mask head + convex upsampling of the reference's ``MAGNET`` (models/MAGNET.py:100-118,
     150-175) operating on backbone outputs; D-Net / F-Net are supplied by the caller (they need
     checkpoints / torch.hub in the reference and are out of scope, SURVEY §2.1 #3-4)."""
 
     def __init__(self, n_samples: int = 5, sampling_range: float = 3, n_iter: int = 3, thres: int = 5,
-                 downsample_ratio: int = 4, dnet_fdim: int = 256, detach_cost: bool = True, fused_train: bool = False):
+                 downsample_ratio: int = 4, dnet_fdim: int = 256, detach_cost: bool = True, fused_train: bool = False,
+                 fused_upsample: bool = False):
         super().__init__()
         self.n_iter, self.thres, self.downsample_ratio = n_iter, thres, downsample_ratio
+        # True: forward runs the mask head after its first convolution and the upsampling of every prediction as one
+        # fused kernel where fused_mask_applies holds (inference); the full mask is then never computed
+        self.fused_upsample = fused_upsample
         # True: training iterations of the G-Net head run the differentiable fused kernels where fused_gnet_trains holds
         self.fused_train = fused_train
         # True: G-Net reads a detached cost volume (MAGNET.py:167).  False: the volume stays in the graph, so a trainable
@@ -287,19 +311,39 @@ class MagnetHead(nn.Module):
         """upsample_depth_via_mask (MAGNET.py:15-27) — fused kernels, no (B,2,9,k,k,H,W) temporaries (f-2)."""
         return ops.convex_upsample(depth.float(), up_mask.float(), k)
 
+    def mask_pre(self, x_d3: torch.Tensor) -> torch.Tensor:
+        """The mask head's first layer before its ReLU, conv3x3(x_d3, W0) + b0: the part of the mask head that stays on
+        cuDNN when the rest runs fused (``ops.mask_upsample``).  The same convolution ``mask_head[0]`` computes."""
+        c0 = self.mask_head[0]
+        return nn.functional.conv2d(x_d3, c0.weight, c0.bias, c0.stride, c0.padding, c0.dilation, c0.groups)
+
     def forward(self, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins):
-        preds, mask = self.forward_quarter(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid,
-                                           cam_intrins)
-        return [self.upsample(pr, mask, self.downsample_ratio) for pr in preds]
+        k = self.downsample_ratio
+        if self.fused_upsample:
+            preds = self._predictions(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid,
+                                      cam_intrins)
+            if fused_mask_applies(self.mask_head, None, preds, k):
+                pre0 = self.mask_pre(x_d3)
+                if fused_mask_applies(self.mask_head, pre0, preds, k):
+                    return ops.mask_upsample(pre0, ops.pack_mask_weights(self.mask_head), preds, k)
+            mask = self.mask_head(x_d3).float()
+        else:
+            preds, mask = self.forward_quarter(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid,
+                                               cam_intrins)
+        return [self.upsample(pr, mask, k) for pr in preds]
+
+    def _predictions(self, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins):
+        plan = MatchingPlan(ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, thres=self.thres)
+        preds = matching_loop(plan, ref_gmms, x_d3, self.g_net, self.n_iter, self.k_list, detach_cost=self.detach_cost,
+                              fused_train=self.fused_train)
+        return preds[1:]
 
     def forward_quarter(self, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins):
         """The N_iter quarter-resolution predictions and the upsampling mask, NOT upsampled: what the fused
         upsample + NLL loss (``loss`` below) consumes during training.  Under torch.autocast every input may be half;
         the predictions and the mask are fp32."""
-        plan = MatchingPlan(ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, thres=self.thres)
-        preds = matching_loop(plan, ref_gmms, x_d3, self.g_net, self.n_iter, self.k_list, detach_cost=self.detach_cost,
-                              fused_train=self.fused_train)
-        return preds[1:], self.mask_head(x_d3).float()
+        preds = self._predictions(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins)
+        return preds, self.mask_head(x_d3).float()
 
     def loss(self, preds_quarter, mask, gt_depth, gt_depth_mask, gamma: float = 0.8):
         """MagnetLoss 'gaussian' (utils/losses.py:34-50) of the upsampled predictions without materialising them."""
@@ -319,7 +363,7 @@ class MAGNET(nn.Module):
 
     def __init__(self, d_net: nn.Module, f_net: nn.Module, n_samples: int = 5, sampling_range: float = 3,
                  weighting: str = "CW5", train_iter: int = 3, test_iter: int = 3, downsample_ratio: int = 4,
-                 dnet_fdim: int = 256, fused_train: bool = False):
+                 dnet_fdim: int = 256, fused_train: bool = False, fused_upsample: bool = False):
         super().__init__()
         self.d_net, self.f_net = d_net, f_net
         for net in (self.d_net, self.f_net):
@@ -329,7 +373,8 @@ class MAGNET(nn.Module):
         self.train_iter, self.test_iter = train_iter, test_iter
         thres = int(weighting.split('CW')[1])                   # "CW5" -> kappa = 5 (MAGNET.py:159)
         self.head = MagnetHead(n_samples=n_samples, sampling_range=sampling_range, n_iter=train_iter, thres=thres,
-                               downsample_ratio=downsample_ratio, dnet_fdim=dnet_fdim, fused_train=fused_train)
+                               downsample_ratio=downsample_ratio, dnet_fdim=dnet_fdim, fused_train=fused_train,
+                               fused_upsample=fused_upsample)
         self.g_net, self.mask_head = self.head.g_net, self.head.mask_head   # reference attribute names
 
     def train(self, mode: bool = True):

@@ -743,6 +743,90 @@ def convex_upsample(depth: torch.Tensor, up_mask: torch.Tensor, k: int) -> torch
     return ConvexUpsample.apply(depth, up_mask, k)
 
 
+def mask_weights_bytes(k: int = 4) -> int:
+    """Bytes of the packed mask-head weights for upsampling factor k (0 for any k but 4)."""
+    return int(lib().magnet_mask_weights_bytes(int(k)))
+
+
+def mask_head_layers(mask_head):
+    """The four convolutions of a mask head with the reference's structure (MAGNET.py:111-118): Conv(*,128,3), ReLU,
+    Conv(128,128,1), ReLU, Conv(128,128,1), ReLU, Conv(128,144,1), every convolution with a bias.  None otherwise."""
+    hid = _lib.MAGNET_HIDDEN_CHANNELS
+    if not isinstance(mask_head, torch.nn.Sequential) or len(mask_head) != 7:
+        return None
+    convs, relus = [mask_head[i] for i in (0, 2, 4, 6)], [mask_head[i] for i in (1, 3, 5)]
+    if not all(isinstance(c, torch.nn.Conv2d) and c.bias is not None for c in convs):
+        return None
+    if not all(isinstance(r, torch.nn.ReLU) for r in relus):
+        return None
+    c0, c1, c2, c3 = convs
+    if not (c0.out_channels == hid and c0.kernel_size == (3, 3) and c0.padding == (1, 1) and c0.stride == (1, 1)
+            and c0.dilation == (1, 1) and c0.groups == 1 and c0.padding_mode == "zeros"):
+        return None
+    for c, cout in ((c1, hid), (c2, hid), (c3, 9 * 4 * 4)):
+        if not (c.in_channels == hid and c.out_channels == cout and c.kernel_size == (1, 1) and c.padding == (0, 0)
+                and c.stride == (1, 1) and c.groups == 1):
+            return None
+    return convs
+
+
+def pack_mask_weights(mask_head) -> torch.Tensor:
+    """The weights of the mask head's last three layers in the fused kernel's layout (``mask_upsample``): the two
+    128x128 layers and the 128->144 layer, split into fp16 hi/lo with one power-of-two scale per layer, and the fp32
+    biases.  The first (3x3) layer stays outside (``MagnetHead.mask_pre``).  Read from the module at each call (nothing
+    is cached).  Two launches."""
+    convs = mask_head_layers(mask_head)
+    if convs is None:
+        raise _lib.MagnetError("not a mask head with the reference's structure (Conv(*,128,3), ReLU, Conv(128,128,1), "
+                               "ReLU, Conv(128,128,1), ReLU, Conv(128,144,1))")
+    _, c1, c2, c3 = convs
+    with torch.no_grad():
+        ts = [_need_cuda_f32(nm, t) for nm, t in (("W1", c1.weight), ("b1", c1.bias), ("W2", c2.weight),
+                                                  ("b2", c2.bias), ("W3", c3.weight), ("b3", c3.bias))]
+    dev = _same_device(*((f"weight {i}", t) for i, t in enumerate(ts)))
+    out = torch.empty(mask_weights_bytes(4), device=dev, dtype=torch.uint8)
+    with torch.cuda.device(dev):
+        check(lib().magnet_mask_pack_weights_f32(*(t.data_ptr() for t in ts), out.data_ptr(), _stream(dev)),
+              "magnet_mask_pack_weights_f32")
+    return out
+
+
+def mask_upsample(pre0: torch.Tensor, packed: torch.Tensor, preds, k: int = 4) -> list:
+    """The mask head after its first convolution and the learned upsampling of every prediction, in one kernel per 8
+    predictions: pre0 (B,128,H,W) = the first convolution's output before its ReLU (``MagnetHead.mask_pre``), packed =
+    ``pack_mask_weights(mask_head)``, preds = quarter-resolution (B,2,H,W) [mu, sigma] tensors -> a list of
+    (B,2,k*H,k*W) tensors, as ``convex_upsample(pred, mask_head(x_d3), k)`` gives them.  The 144-channel mask is never
+    written.  k = 4 only.  Not differentiable (forward only)."""
+    preds = [preds] if isinstance(preds, torch.Tensor) else list(preds)
+    if not preds:
+        raise _lib.MagnetError("mask_upsample needs at least one prediction")
+    if int(k) != 4:
+        raise _lib.MagnetError(f"the fused mask head takes k = 4 only (144 mask channels), got {k}")
+    pre0 = _need_cuda_f32("pre0", pre0)
+    if pre0.dim() != 4 or pre0.shape[1] != _lib.MAGNET_HIDDEN_CHANNELS:
+        raise _lib.MagnetError(f"pre0 must be (B,{_lib.MAGNET_HIDDEN_CHANNELS},H,W), got {tuple(pre0.shape)}")
+    B, _, H, W = pre0.shape
+    nbytes = mask_weights_bytes(4)
+    if not (isinstance(packed, torch.Tensor) and packed.is_cuda and packed.dtype == torch.uint8
+            and packed.is_contiguous() and packed.numel() == nbytes):
+        raise _lib.MagnetError(f"packed must be a pack_mask_weights buffer ({nbytes} bytes)")
+    for i, p in enumerate(preds):
+        preds[i] = _need_cuda_f32(f"preds[{i}]", p)
+        _expect(f"preds[{i}]", preds[i], (B, 2, H, W))
+    dev = _same_device(("pre0", pre0), ("packed", packed), *((f"preds[{i}]", p) for i, p in enumerate(preds)))
+    outs = [torch.empty(B, 2, 4 * H, 4 * W, device=dev, dtype=torch.float32) for _ in preds]
+    n = _lib.MAGNET_MASK_MAX_PRED
+    with torch.cuda.device(dev):
+        for c in range(0, len(preds), n):
+            ps, os_ = preds[c:c + n], outs[c:c + n]
+            pp = (C.c_void_p * len(ps))(*[p.data_ptr() for p in ps])
+            op = (C.c_void_p * len(os_))(*[o.data_ptr() for o in os_])
+            a = _lib.MaskUpsampleArgs(P=len(ps), B=B, H=H, W=W, k=4, pre0=pre0.data_ptr(), packed_weights=packed.data_ptr(),
+                                      pred=C.cast(pp, C.POINTER(C.c_void_p)), out=C.cast(op, C.POINTER(C.c_void_p)))
+            check(lib().magnet_mask_upsample_f32(C.byref(a), _stream(dev)), "magnet_mask_upsample_f32")
+    return outs
+
+
 class UpsampleNLL(torch.autograd.Function):
     """mean over the supervised pixels of the Gaussian NLL of ONE convex-upsampled prediction — upsample_depth_via_mask
     (MAGNET.py:15-27) + the per-prediction term of MagnetLoss (utils/losses.py:39-49) in one kernel each way; the
