@@ -9,6 +9,7 @@ import torch
 
 from magnet_b200 import _lib
 from magnet_b200.matcher import GNET, fused_gnet_trains
+from tests.head_ref import wgrad3
 
 
 def _args(p):
@@ -117,38 +118,7 @@ def test_train_dispatch_rule_truth_table():
     assert fused_gnet_trains(g, cv, inv.clone().requires_grad_(True))   # the invariant still wants a gradient
 
 
-# ---- numpy restatement of the weight-gradient GEMM ----------------------------------------------------------------
-def tf32(x):
-    """cvt.rna.tf32.f32: round to nearest, ties away from zero, to 10 explicit mantissa bits."""
-    u = np.asarray(x, np.float32).view(np.uint32).astype(np.uint64)
-    r = ((u + 0x1000) & 0xFFFFE000).astype(np.uint32)
-    return r.view(np.float32)
-
-
-def wgrad3(a, b, kc=1024, slab=32, ks=8):
-    """out[m][n] = sum_p a[p][m] b[p][n] as the kernel evaluates it: x = hi + lo (tf32 each); per slab of 32 pixels a
-    fresh fp32 accumulator takes, per k8 step, the three products lo*hi, hi*lo, hi*hi (each MMA's sum of exact products
-    rounded once to fp32) and is added to the CTA's running fp32 sum; the per-chunk (kc pixels) sums are then added
-    in order in fp32."""
-    ah = tf32(a); al = tf32(a - ah)
-    bh = tf32(b); bl = tf32(b - bh)
-    f = lambda u: u.astype(np.float64)
-    P = a.shape[0]
-    r32 = lambda x: x.astype(np.float32)
-    total = np.zeros((a.shape[1], b.shape[1]), np.float32)
-    for c0 in range(0, P, kc):
-        tot = np.zeros_like(total)
-        for s0 in range(c0, min(P, c0 + kc), slab):
-            acc = np.zeros_like(total)
-            for k0 in range(s0, min(P, c0 + kc, s0 + slab), ks):
-                s = slice(k0, min(P, c0 + kc, k0 + ks))
-                for x, y in ((al, bh), (ah, bl), (ah, bh)):
-                    acc = r32(f(acc) + f(x[s]).T @ f(y[s]))
-            tot = r32(f(tot) + f(acc))
-        total = r32(f(total) + f(tot))
-    return total
-
-
+# ---- numpy restatement of the weight-gradient GEMM (tests/head_ref.wgrad3) ----------------------------------------
 @pytest.mark.parametrize("scale", [1e-3, 1.0, 1e3])
 @pytest.mark.parametrize("P", [37, 1024, 3000])
 def test_three_product_tf32_wgrad_error(scale, P):

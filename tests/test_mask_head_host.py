@@ -10,6 +10,7 @@ import torch.nn as nn
 
 from magnet_b200 import _lib, ops
 from magnet_b200.matcher import MagnetHead, fused_mask_applies
+from tests.head_ref import shift, split
 
 
 def _args(P=1, B=1, H=4, W=4, k=4, ptr=None, preds=None, outs=None):
@@ -131,21 +132,7 @@ def test_tile_mapping_matches_the_reference_view():
     assert cols == list(range(64))
 
 
-# ---- numpy restatement of the 144-column layer's SPLIT16 numerics --------------------------------------------------
-def shift(m):
-    m = np.float32(m)
-    if m == 0 or not np.isfinite(m) or m < np.finfo(np.float32).tiny:
-        return 0
-    return int(np.clip(14 - int(np.floor(np.log2(m))), -100, 100))
-
-
-def split(x, sh):
-    xs = (x.astype(np.float32) * np.float32(2.0 ** sh)).astype(np.float32)
-    hi = xs.astype(np.float16)
-    lo = (xs - hi.astype(np.float32)).astype(np.float16)
-    return hi, lo
-
-
+# ---- numpy restatement of the 144-column layer's SPLIT16 numerics (tests/head_ref.shift, split) --------------------
 @pytest.mark.parametrize("scale", [1e-3, 1.0, 1e3])
 def test_three_product_error_of_the_mask_layer(scale):
     """h2 (M,128) post-ReLU rows with one shift each, W3 (144,128) with one shift: hi*hi + hi*lo + lo*hi in float64
