@@ -22,8 +22,12 @@ Sample positions (``pos``):
   "mma"    — the sequence of ``project()`` (cells_common.cuh), whose reciprocal (rcp + one Newton step) is not
              reproducible here: the bounds then carry a position-error term |g| |d cost / d ix| delta with
              delta = (A + 8) u |ix + 0.5| (DESIGN §3.1).  The F volume and every tap-sharing kernel use these positions.
-Everything downstream of the positions (dot products, products with g, sums over j, t, v) is float64."""
+Everything downstream of the positions (dot products, products with g, sums over j, t, v) is float64.  The geometry is
+numpy; the contractions gather each tap's source vector and scatter into its cell (never the all-pairs matrix
+<ref_p, src_s>) in torch float64 on the device the caller names (the GPU tests pass theirs), one hypothesis chunk of one
+view at a time, so the reference runs at the production shapes."""
 import numpy as np
+import torch
 
 from oracle import magnet_oracle as mo
 
@@ -174,6 +178,7 @@ def _view(cam, rays, d, H, W, pos, src_gmm, kappa, consistency):
     if pos == "mma":                              # clamp_coord: only moves positions whose taps are all outside
         ixs, iys = np.clip(ixs, -2.0, W + 1.0), np.clip(iys, -2.0, H + 1.0)
     x0, y0 = np.floor(ixs), np.floor(iys)
+    g.x0, g.y0 = x0, y0
     fx, fy = ixs - x0, iys - y0
     g.wx, g.wy = (1.0 - fx, fx), (1.0 - fy, fy)
     g.idx, g.inb, g.w = {}, {}, {}
@@ -225,51 +230,94 @@ def _view(cam, rays, d, H, W, pos, src_gmm, kappa, consistency):
 
 
 class Reference:
-    """The reference for one call: ``Reference(...)`` computes the geometry of every valid (b, v) pair; ``forward()``
-    the volume and its bound; ``backward(gs, gs_abs)`` the gradients for a score gradient gs (= gout / V for the CW
-    volume) and its bound.
+    """The reference for one call: ``Reference(...)`` walks the geometry of every valid (b, v) pair once and keeps
+    only the ambiguity and ``reached`` maps; ``forward()`` the volume and its bound; ``backward(gs, gs_abs)`` the
+    gradients for a score gradient gs (= gout / V for the CW volume) and its bound.  Each call recomputes the geometry
+    (numpy, O(D HW) per view) in hypothesis chunks, so no more than one chunk of one view is alive at a time.
+
+    The contractions are gathers and scatters in torch float64 on ``device``: f_t = <ref_p, src[idx_t]> from the
+    gathered tap vectors, grad_ref the weighted sum of gathered source vectors, grad_src an ``index_add_`` into the
+    tap's cell; each bound is the same expression over absolute values.  They equal the all-pairs contraction
+    <ref_p, src_s> up to the float64 summation order (tests/test_cw_grad_cpu.py holds them to it).
 
     depth (B,D,H,W) hypothesis depths (fp32 for "direct" / "mma"); ref (B,C,H,W); src (V*B,C,H,W) view-major;
     src_gmm (V*B,2,H,W) or None; cams (B*V,16) the kernel's camera table (b-major); rays (B,3,HW)."""
 
-    def __init__(self, depth, ref, src, src_gmm, cams, rays, kappa, *, pos="direct", consistency=True):
-        depth = np.asarray(depth)
-        self.B, self.D, self.H, self.W = depth.shape
+    CHUNK = 1 << 25                            # elements of one gathered (C, chunk, HW) block: 256 MB in float64
+
+    def __init__(self, depth, ref, src, src_gmm, cams, rays, kappa, *, pos="direct", consistency=True, device="cpu"):
+        self.depth = np.asarray(depth)
+        self.B, self.D, self.H, self.W = self.depth.shape
         self.HW = self.H * self.W
         self.C = ref.shape[1]
         self.V = src.shape[0] // self.B
-        self.ref = np.asarray(ref, np.float64).reshape(self.B, self.C, self.HW)
-        self.src = np.asarray(src, np.float64).reshape(self.V * self.B, self.C, self.HW)
+        self.dev = torch.device(device)
+        self.ref = self._t(np.asarray(ref, np.float64).reshape(self.B, self.C, self.HW))
+        self.src = self._t(np.asarray(src, np.float64).reshape(self.V * self.B, self.C, self.HW))
+        self.cams, self.rays = np.asarray(cams), np.asarray(rays)
+        self.src_gmm, self.kappa, self.consistency = src_gmm, kappa, consistency
         self.pos = pos
         self.pos_err = pos == "mma"            # bounds carry the position-error term by default on mma positions
-        self.views = {}
+        self.valid = [(b, v) for b in range(self.B) for v in range(self.V) if self.cams[b * self.V + v][0] == 1.0]
+        self.nj = max(1, min(self.D, self.CHUNK // (self.C * self.HW), (1 << 20) // self.HW))
         self._memo = {}
         shp = (self.B, self.D, self.HW)
         self.margin, self.edge, self.delta = np.full(shp, np.inf), np.full(shp, np.inf), np.zeros(shp)
         self.amp_bad = np.zeros(shp, bool)
         self.reached = {k: np.zeros(shp, bool) for k in ("clamped", "tap_outside", "all_outside", "behind")}
-        for b in range(self.B):
-            for v in range(self.V):
-                cam = np.asarray(cams[b * self.V + v])
-                if cam[0] != 1.0:
-                    continue
-                gm = None if src_gmm is None else src_gmm[v * self.B + b]
-                g = _view(cam, rays[b], depth[b].reshape(self.D, self.HW), self.H, self.W, pos, gm, kappa, consistency)
-                self.views[b, v] = g
-                self.margin[b] = np.minimum(self.margin[b], g.margin)
-                self.edge[b] = np.minimum(self.edge[b], g.edge)
-                self.delta[b] = np.maximum(self.delta[b], U * np.maximum(g.ex, g.ey))
-                self.amp_bad[b] |= g.amp_bad & g.any_in
-                for k in self.reached:
-                    self.reached[k][b] |= getattr(g, k)
-        self._dots = {}
+        # box of the cell origins of every (valid view, 64-hypothesis chunk, pixel): the tensor-core window
+        nk = -(-self.D // 64)
+        self.origins = np.stack([np.full((self.B, self.V, nk, self.HW), s * np.inf) for s in (1, -1, 1, -1)])
+        for b, v, j0, j1, g in self._chunks():
+            sl = (b, slice(j0, j1))
+            self.margin[sl] = np.minimum(self.margin[sl], g.margin)
+            self.edge[sl] = np.minimum(self.edge[sl], g.edge)
+            self.delta[sl] = np.maximum(self.delta[sl], U * np.maximum(g.ex, g.ey))
+            self.amp_bad[sl] |= g.amp_bad & g.any_in
+            for k in self.reached:
+                self.reached[k][sl] |= getattr(g, k)
+            for k in range(j0 // 64, (j1 - 1) // 64 + 1):
+                s = slice(max(j0, 64 * k) - j0, min(j1, 64 * k + 64) - j0)
+                o = self.origins[:, b, v, k]
+                o[0], o[1] = np.minimum(o[0], g.x0[s].min(0)), np.maximum(o[1], g.x0[s].max(0))
+                o[2], o[3] = np.minimum(o[2], g.y0[s].min(0)), np.maximum(o[3], g.y0[s].max(0))
 
-    def _dot(self, b, v):
-        """<ref_p, src_s> for every (reference pixel, source pixel) pair and its absolute companion."""
-        if (b, v) not in self._dots:
-            r, s = self.ref[b], self.src[v * self.B + b]
-            self._dots[b, v] = (r.T @ s, np.abs(r).T @ np.abs(s))
-        return self._dots[b, v]
+    def _t(self, x):
+        return torch.tensor(np.asarray(x), device=self.dev)
+
+    def _chunks(self):
+        """(b, v, j0, j1, View of hypotheses j0..j1-1) for every valid (b, v) pair."""
+        for b, v in self.valid:
+            gm = None if self.src_gmm is None else self.src_gmm[v * self.B + b]
+            d = self.depth[b].reshape(self.D, self.HW)
+            for j0 in range(0, self.D, self.nj):
+                j1 = min(self.D, j0 + self.nj)
+                yield b, v, j0, j1, _view(self.cams[b * self.V + v], self.rays[b], d[j0:j1], self.H, self.W, self.pos,
+                                          gm, self.kappa, self.consistency)
+
+    def _taps(self, b, v, g):
+        """Per tap t: f_t = <ref_p, src[idx_t]> and <|ref_p|, |src[idx_t]|> (chunk, HW), zero outside the image."""
+        r, s = self.ref[b], self.src[v * self.B + b]
+        f, fa = {}, {}
+        for t in g.idx:
+            S = s[:, self._t(g.idx[t])]                              # (C, chunk, HW) gathered tap vectors
+            inb = self._t(g.inb[t])
+            f[t] = torch.where(inb, (S * r[:, None]).sum(0), 0.0)
+            fa[t] = torch.where(inb, (S.abs() * r.abs()[:, None]).sum(0), 0.0)
+        return f, fa
+
+    def _feature_grads(self, b, v, g, coef, coef_abs, out):
+        """grad_ref[b] += sum_{j,t} coef_t src[idx_t], grad_src[v B + b][idx_t] += ref coef_t, and their bounds from
+        coef_abs.  coef / coef_abs: per tap (chunk, HW), zero outside the image; out: (gref, grefb, gsrc, gsrcb)."""
+        gref, grefb, gsrc, gsrcb = out
+        r, s, i = self.ref[b], self.src[v * self.B + b], v * self.B + b
+        for t in g.idx:
+            idx = self._t(g.idx[t])
+            S = s[:, idx]
+            gref[b] += (S * coef[t][None]).sum(1)
+            grefb[b] += (S.abs() * coef_abs[t][None]).sum(1)
+            gsrc[i].index_add_(1, idx.reshape(-1), (r[:, None] * coef[t][None]).reshape(self.C, -1))
+            gsrcb[i].index_add_(1, idx.reshape(-1), (r.abs()[:, None] * coef_abs[t][None]).reshape(self.C, -1))
 
     def ambiguous(self, margin_tol=1e-3, edge_tol=1e-3):
         """(B,D,H,W): hypotheses near a mask flip, near a cell edge (or within 4 position errors of one, on mma
@@ -296,64 +344,55 @@ class Reference:
         return self._memo["fwd", pos_err]
 
     def _forward(self, pos_err):
-        B, D, HW, V = self.B, self.D, self.HW, self.V
-        out, bound = np.zeros((B, D, HW)), np.zeros((B, D, HW))
-        terms, vmargin = np.zeros((V, B, D, HW)), np.full((V, B, D, HW), np.inf)
-        for (b, v), g in self.views.items():
-            dot, dabs = self._dot(b, v)
-            p = np.arange(HW)[None, :]
-            cost = sum(g.w[t] * np.where(g.inb[t], dot[p, g.idx[t]], 0.0) for t in g.w)
-            cabs = sum(self._wabs(g, t, pos_err) * np.where(g.inb[t], dabs[p, g.idx[t]], 0.0) for t in g.w)
-            out[b] += np.where(g.m, cost, 0.0) / V
-            bound[b] += np.where(g.m | (g.margin <= 1e-3), cabs, 0.0) / V
-            terms[v, b] = cost / V
-            vmargin[v, b] = g.margin
+        B, D, HW, V, T = self.B, self.D, self.HW, self.V, self._t
+        z = lambda *s: torch.zeros(s, dtype=torch.float64, device=self.dev)
+        out, bound, terms = z(B, D, HW), z(B, D, HW), z(V, B, D, HW)
+        vmargin = torch.full((V, B, D, HW), np.inf, dtype=torch.float64, device=self.dev)
+        for b, v, j0, j1, g in self._chunks():
+            f, fa = self._taps(b, v, g)
+            cost = sum(T(g.w[t]) * f[t] for t in f)
+            cabs = sum(T(self._wabs(g, t, pos_err)) * fa[t] for t in f)
+            m, margin = T(g.m), T(g.margin)
+            out[b, j0:j1] += torch.where(m, cost, 0.0) / V
+            bound[b, j0:j1] += torch.where(m | (margin <= 1e-3), cabs, 0.0) / V
+            terms[v, b, j0:j1] = cost / V
+            vmargin[v, b, j0:j1] = margin
         sh = (B, D, self.H, self.W)
-        return out.reshape(sh), bound.reshape(sh), terms.reshape((V,) + sh), vmargin.reshape((V,) + sh)
+        return tuple(x.reshape(s).cpu().numpy() for x, s in ((out, sh), (bound, sh), (terms, (V,) + sh),
+                                                               (vmargin, (V,) + sh)))
 
     def backward(self, gs, gs_abs=None, pos_err=None):
         """gs (B,D,H,W): the score gradient (gout / V for the CW volume).  Returns a dict of float64 arrays: ref,
         src (V*B,C,H,W), d (B,D,H,W) and their bounds ref_b, src_b, d_b (in units of u: tolerance c u bound)."""
-        B, D, HW, V, C = self.B, self.D, self.HW, self.V, self.C
+        B, D, HW, V, C, T = self.B, self.D, self.HW, self.V, self.C, self._t
         pos_err = self.pos_err if pos_err is None else pos_err
         gs = np.asarray(gs, np.float64).reshape(B, D, HW)
-        gs_abs = np.abs(gs) if gs_abs is None else np.asarray(gs_abs, np.float64).reshape(B, D, HW)
-        gref, grefb = np.zeros((B, C, HW)), np.zeros((B, C, HW))
-        gsrc, gsrcb = np.zeros((V * B, C, HW)), np.zeros((V * B, C, HW))
-        gd, gdb = np.zeros((B, D, HW)), np.zeros((B, D, HW))
-        p = np.broadcast_to(np.arange(HW)[None, :], (D, HW))
-        for (b, v), g in self.views.items():
-            dot, dabs = self._dot(b, v)
-            gm, gma = np.where(g.m, gs[b], 0.0), np.where(g.m, gs_abs[b], 0.0)
-            M, Ma = np.zeros(HW * HW), np.zeros(HW * HW)
-            f, fa = {}, {}
-            for t in g.w:
-                sel = g.inb[t] & (gma != 0)
-                key = (g.idx[t] * HW + p)[sel]
-                M += np.bincount(key, weights=(gm * g.w[t])[sel], minlength=HW * HW)
-                Ma += np.bincount(key, weights=(gma * self._wabs(g, t, pos_err))[sel], minlength=HW * HW)
-                f[t] = np.where(g.inb[t], dot[p, g.idx[t]], 0.0)
-                fa[t] = np.where(g.inb[t], dabs[p, g.idx[t]], 0.0)
-            M, Ma = M.reshape(HW, HW), Ma.reshape(HW, HW)     # [source pixel, reference pixel]
-            s = self.src[v * B + b]
-            gref[b] += s @ M
-            grefb[b] += np.abs(s) @ Ma
-            gsrc[v * B + b] += self.ref[b] @ M.T
-            gsrcb[v * B + b] += np.abs(self.ref[b]) @ Ma.T
-            (wy0, wy1), (wx0, wx1) = g.wy, g.wx
+        gs_abs = T(np.abs(gs) if gs_abs is None else np.asarray(gs_abs, np.float64).reshape(B, D, HW))
+        gs = T(gs)
+        z = lambda *s: torch.zeros(s, dtype=torch.float64, device=self.dev)
+        feat = (z(B, C, HW), z(B, C, HW), z(V * B, C, HW), z(V * B, C, HW))
+        gd, gdb = z(B, D, HW), z(B, D, HW)
+        for b, v, j0, j1, g in self._chunks():
+            m = T(g.m)
+            gm, gma = torch.where(m, gs[b, j0:j1], 0.0), torch.where(m, gs_abs[b, j0:j1], 0.0)
+            self._feature_grads(b, v, g, {t: gm * T(g.w[t]) for t in g.idx},
+                                {t: gma * T(self._wabs(g, t, pos_err)) for t in g.idx}, feat)
+            f, fa = self._taps(b, v, g)
+            (wy0, wy1), (wx0, wx1) = map(T, g.wy), map(T, g.wx)
             dcdx = (f[0, 1] - f[0, 0]) * wy0 + (f[1, 1] - f[1, 0]) * wy1
             dcdy = (f[1, 0] - f[0, 0]) * wx0 + (f[1, 1] - f[0, 1]) * wx1
             DX = (fa[0, 1] + fa[0, 0]) * wy0 + (fa[1, 1] + fa[1, 0]) * wy1
             DY = (fa[1, 0] + fa[0, 0]) * wx0 + (fa[1, 1] + fa[0, 1]) * wx1
             FA = fa[0, 0] + fa[0, 1] + fa[1, 0] + fa[1, 1]
-            with np.errstate(invalid="ignore", over="ignore"):
-                gd[b] += np.where(gm != 0, gm * (dcdx * g.dudd + dcdy * g.dvdd), 0.0)
-                pe = FA * (g.ey * g.Du + g.ex * g.Dv) if pos_err else 0.0
-                gdb[b] += np.where(gma != 0, gma * (DX * g.Du + DY * g.Dv + pe), 0.0)
+            Du, Dv = T(g.Du), T(g.Dv)
+            gd[b, j0:j1] += torch.where(gm != 0, gm * (dcdx * T(g.dudd) + dcdy * T(g.dvdd)), 0.0)
+            pe = FA * (T(g.ey) * Du + T(g.ex) * Dv) if pos_err else 0.0
+            gdb[b, j0:j1] += torch.where(gma != 0, gma * (DX * Du + DY * Dv + pe), 0.0)
         sh = (self.H, self.W)
-        return dict(ref=gref.reshape((B, C) + sh), ref_b=grefb.reshape((B, C) + sh),
-                    src=gsrc.reshape((V * B, C) + sh), src_b=gsrcb.reshape((V * B, C) + sh),
-                    d=gd.reshape((B, D) + sh), d_b=gdb.reshape((B, D) + sh))
+        n = lambda x, s: x.reshape(s + sh).cpu().numpy()
+        gref, grefb, gsrc, gsrcb = feat
+        return dict(ref=n(gref, (B, C)), ref_b=n(grefb, (B, C)), src=n(gsrc, (V * B, C)), src_b=n(gsrcb, (V * B, C)),
+                    d=n(gd, (B, D)), d_b=n(gdb, (B, D)))
 
 
 def gauss_chain(gd, gd_b, k):

@@ -1,6 +1,7 @@
 """Autograd of the CW volume without a GPU: the ATen port against the reference's frozen backward, a float64 numpy
-restatement of the depth gradient against autograd of the port, the new C export's argument checks and the Python
-wrapper's refusal to drop a camera gradient."""
+restatement of the depth gradient against autograd of the port, the gather / scatter contractions of
+tests/cw_grad_ref.py (on the CPU here) against a dense all-pairs restatement, the new C export's argument checks and the
+Python wrapper's refusal to drop a camera gradient."""
 import ctypes as C
 
 import numpy as np
@@ -168,6 +169,82 @@ def test_float64_reference_matches_autograd(C_):
         g = rf.backward(gsc, gsc_b)
         _within(gr, g["ref"], g["ref_b"], 1e-12, f"F softmax={softmax} ref")
         _within(gs, g["src"], g["src_b"], 1e-12, f"F softmax={softmax} src")
+
+
+def _dense_reference():
+    """tests/cw_grad_ref.Reference with its two contractions restated over all (reference pixel p, source pixel s)
+    pairs: the dense matrix <ref_p, src_s> read through each tap's one-hot (chunk, p, s) selector, and the coefficient
+    matrix sum_{j,t} coef_t [idx_t = s] applied to the whole maps."""
+    from tests.cw_grad_ref import Reference
+
+    def onehot(rf, g, t):
+        idx, inb = rf._t(g.idx[t]), rf._t(g.inb[t])
+        return torch.zeros(idx.shape + (rf.HW,), dtype=torch.float64).scatter_(2, idx[..., None], inb[..., None].double())
+
+    class Dense(Reference):
+        def _taps(self, b, v, g):
+            r, s = self.ref[b], self.src[v * self.B + b]
+            dot, dabs = torch.einsum("cp,cs->ps", r, s), torch.einsum("cp,cs->ps", r.abs(), s.abs())
+            O = {t: onehot(self, g, t) for t in g.idx}
+            return ({t: torch.einsum("jps,ps->jp", O[t], dot) for t in O},
+                    {t: torch.einsum("jps,ps->jp", O[t], dabs) for t in O})
+
+        def _feature_grads(self, b, v, g, coef, coef_abs, out):
+            r, s, i = self.ref[b], self.src[v * self.B + b], v * self.B + b
+            M = sum(torch.einsum("jps,jp->ps", onehot(self, g, t), coef[t]) for t in g.idx)
+            Ma = sum(torch.einsum("jps,jp->ps", onehot(self, g, t), coef_abs[t]) for t in g.idx)
+            out[0][b] += s @ M.T
+            out[1][b] += s.abs() @ Ma.T
+            out[2][i] += r @ M
+            out[3][i] += r.abs() @ Ma
+    return Dense
+
+
+@pytest.mark.parametrize("case", ["c1_cw_direct", "c64_volume_mma_invalid", "planes_softmax_f64"])
+def test_gather_contractions_equal_all_pairs(case):
+    """The reference's gathers and scatters against the dense all-pairs restatement: forward, backward and camera
+    gradients to 1e-12 of each bound, on positions "direct", "mma" and "f64", with consistency on and off."""
+    from magnet_b200.synthetic import make_inputs
+    from tests.cw_grad_ref import Reference, cameras_f64, softmax_score_grad
+    from tests.geom_grad_ref import camera_grads
+    C_, pos, kind, invalid = {"c1_cw_direct": (1, "direct", "cw", []),
+                              "c64_volume_mma_invalid": (64, "mma", "volume", [(1, 2)]),
+                              "planes_softmax_f64": (5, "f64", "planes", [])}[case]
+    B, V, D, H, W = 2, 3, 6, 7, 11
+    inp = make_inputs(B=B, V=V, D=D, H=H, W=W, C=C_, seed=C_, depth="random", invalid=invalid)
+    cams = cameras_f64(inp.cam_intrins['intM'].double().numpy(), inp.R.double().numpy(), inp.t.double().numpy(),
+                       inp.is_valid.numpy())
+    rays = inp.cam_intrins['unit_ray_array_2D'].numpy()
+    if pos != "f64":                                       # the kernels' fp32 camera table and depths
+        cams, depth = cams.astype(np.float32), inp.depth_volume().numpy().copy()
+        depth[:, 1] *= np.float32(0.02)
+    else:
+        depth = np.broadcast_to(np.array([0.002, 0.05, 0.5, 1.5, 3.0, 8.0]).reshape(1, -1, 1, 1), (B, D, H, W))
+    cw = kind == "cw"
+    args = (depth, inp.ref_feat.numpy(), inp.nghbr_feat.numpy(), inp.nghbr_gmms.numpy() if cw else None, cams, rays,
+            float(inp.thres))
+    chunked = type("Chunked", (Reference,), {"CHUNK": 4 * C_ * H * W})     # hypothesis chunks of 4 and 2
+    rfs = [cls(*args, pos=pos, consistency=cw) for cls in (chunked, _dense_reference())]
+    assert rfs[0].nj == 4 and rfs[1].nj == D and rfs[0].reached["tap_outside"].any()
+    rng = np.random.default_rng(C_)
+    gout = rng.standard_normal((B, D, H, W))
+    if kind == "planes":
+        score = rfs[0].forward()[0]
+        e = np.exp(score - score.max(1, keepdims=True))
+        gs, gs_abs = softmax_score_grad(e / e.sum(1, keepdims=True), gout, V)
+    else:
+        gs, gs_abs = gout / V, None
+    got, want = [(rf.forward(), rf.backward(gs, gs_abs), camera_grads(rf, depth, cams, rays, gs, gs_abs))
+                 for rf in rfs]
+    for k, (a, b) in enumerate(zip(got[0][:3], want[0][:3])):
+        _within(a, b, want[0][1], 1e-12, f"forward {k}")
+    np.testing.assert_array_equal(got[0][3], want[0][3])
+    for out in ("ref", "src", "d"):
+        _within(got[1][out], want[1][out], want[1][out + "_b"], 1e-12, out)
+        _within(got[1][out + "_b"], want[1][out + "_b"], want[1][out + "_b"], 1e-12, out + " bound")
+    for out in ("cams", "rays"):
+        _within(got[2][out], want[2][out], want[2][out + "_b"], 1e-12, out)
+        _within(got[2][out + "_b"], want[2][out + "_b"], want[2][out + "_b"], 1e-12, out + " bound")
 
 
 def _args(L, *, C_=64, V=2, D=8, layout=_lib.SRC_NCHW, variant=_lib.VARIANT_DIRECT, mode=_lib.DEPTH_VOLUME,

@@ -1,5 +1,6 @@
 """Camera gradients on the GPU (magnet_cost_volume_geom_bwd_f32), element by element against the float64 restatement of
-tests/geom_grad_ref.py, and through the public entry points under geometry_grad().
+tests/geom_grad_ref.py (contracted from gathered tap dot products in torch float64 on the test's GPU, up to the cfg2,
+cfg3 and F-Net shapes), and through the public entry points under geometry_grad().
 
 Tolerance: |got - ref| <= c u bound with u = 2^-24, bound the float64 sum of absolute contributions (geom_grad_ref) and
 c = D + C + V + nblk / 32 + 64 (DESIGN §3.11: the longest fp32 chain any term passes through: the channel dot product,
@@ -37,7 +38,7 @@ def _close(got, want, bound, c, what):
     assert ratio <= 1.0, (what, ratio)
 
 
-# (C, D, V, H, W, depth mode, forward kernel, consistency, softmax, family)
+# (C, D, V, H, W, depth mode, forward kernel, consistency, softmax, family[, B = 2])
 CASES = {
     "c1_direct": (1, 5, 2, 9, 13, "volume", "direct", True, False, "scannet"),
     "c8_gauss_direct": (8, 32, 4, 10, 14, "gauss", "direct", True, False, "scannet"),
@@ -49,17 +50,28 @@ CASES = {
     "planes_c8_softmax": (8, 32, 2, 11, 15, "planes", None, False, True, "scannet"),
     "planes_c64_scores_v4": (64, 64, 4, 12, 20, "planes", None, False, False, "kitti"),
     "planes_c33_sid_softmax": (33, 5, 8, 6, 33, "planes", None, False, True, "scannet"),
+    # production shapes: the cfg2 / cfg3 matching step, where each lane of the fixed-order reduction adds nblk / 32 > 1
+    # blocks.  On the DIRECT kernel's positions, which the reference reproduces: on project() positions the bound of
+    # every term carries the position error (A + 8) u |ix + 0.5| of some 100 px, and the sum of 10^6 terms of random
+    # sign per (b, v) then lies far inside c u bound, so a wrong reduction would pass
+    "cfg2_gauss_direct": (64, 64, 4, 120, 160, "gauss", "direct", True, False, "scannet", 8),
+    "cfg3_volume_direct": (64, 64, 4, 88, 304, "volume", "direct", True, False, "kitti", 4),
 }
 
 
 class Case:
     def __init__(self, name, cuda):
-        Cc, D, V, H, W, mode, fwd, cw, softmax, family = CASES[name]
-        self.__dict__.update(C=Cc, D=D, V=V, H=H, W=W, mode=mode, fwd=fwd, cw=cw, softmax=softmax)
+        Cc, D, V, H, W, mode, fwd, cw, softmax, family, *batch = CASES[name]
+        B = batch[0] if batch else 2
+        self.__dict__.update(B=B, C=Cc, D=D, V=V, H=H, W=W, mode=mode, fwd=fwd, cw=cw, softmax=softmax,
+                             production=bool(batch))
         seed = sum(map(ord, name))
-        B = 2
+        # the production cases also have a batch element without a valid view
+        self.invalid = ([(1, V - 1)] if V > 1 else []) + ([(2, v) for v in range(V)] if B > 2 else [])
         inp = make_inputs(B=B, V=V, D=D, H=H, W=W, C=Cc, seed=seed, family=family, depth="smooth",
-                          invalid=[(1, V - 1)] if V > 1 else [])
+                          invalid=self.invalid)
+        if self.production:                                # view 0 of batch element 0 moves sideways: the +-10 clamp
+            inp.nghbr_poses[0, 0, :3, 3] = torch.tensor([0.3, 0.05, 0.01])
         rng = np.random.default_rng(seed)
         self.inp, self.dev = inp, cuda
         g = inp.to(cuda)
@@ -71,6 +83,8 @@ class Case:
         self.k = None
         if mode == "gauss":
             self.k = np.linspace(-2.5, 2.5, D).astype(np.float32).tolist()
+            if self.production:                            # behind the source cameras, and beyond the +-10 clamp
+                self.k = [-40.0, -9.98] + self.k[2:]
             depth = gauss_depths(gmm, self.k, "direct")
         elif mode == "planes":
             if name.endswith("sid_softmax"):               # SID planes reaching behind a source camera
@@ -89,7 +103,8 @@ class Case:
         pos = "direct" if fwd == "direct" else "mma"
         self.rf = Reference(depth, inp.ref_feat.numpy(), inp.nghbr_feat.numpy(),
                             inp.nghbr_gmms.numpy() if cw else None, self.cams.cpu().numpy(),
-                            inp.cam_intrins['unit_ray_array_2D'].numpy(), float(inp.thres), pos=pos, consistency=cw)
+                            inp.cam_intrins['unit_ray_array_2D'].numpy(), float(inp.thres), pos=pos, consistency=cw,
+                            device=cuda)
         amb = self.rf.ambiguous()
         gout = rng.standard_normal(amb.shape).astype(np.float32)
         if softmax:
@@ -126,15 +141,28 @@ class Case:
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_camera_gradients_elementwise(name, cuda):
     cs = Case(name, cuda)
-    print(f"{name}: zeroed {cs.rf.ambiguous().mean():.4f}")
+    amb = cs.rf.ambiguous()
+    print(f"{name}: zeroed {amb.mean():.4f}")
+    c = _c(cs.D, cs.C, cs.V, cs.H * cs.W)
+    if cs.production:
+        # each lane of geom_reduce_kernel adds several blocks; the planted edges are compared; the gate is sharp: most
+        # valid camera-table entries and ray elements exceed their tolerance, so a zeroed output or a missing block
+        # partial of that size is rejected
+        assert (cs.H * cs.W + 31) // 32 > 32 and amb.mean() <= 0.025, amb.mean()
+        for k in ("behind", "clamped", "tap_outside"):
+            assert (cs.rf.reached[k].reshape(amb.shape) & ~amb).any(), k
+        valid = cs.inp.is_valid.numpy().reshape(-1) == 1
+        for out, sel in (("cams", valid), ("rays", cs.want["rays_b"] > 0)):
+            sharp = (np.abs(cs.want[out]) > c * U * cs.want[out + "_b"])[sel]
+            print(f"{name} {out}: {sharp.mean():.3f} of the elements exceed c u bound")
+            assert sharp.mean() > 0.75, (out, sharp.mean())
     g_cams, g_rays, _ = cs.call()
     torch.cuda.synchronize()
-    c = _c(cs.D, cs.C, cs.V, cs.H * cs.W)
     _close(g_cams, cs.want["cams"], cs.want["cams_b"], c, f"{name} cams")
     _close(g_rays, cs.want["rays"], cs.want["rays_b"], c, f"{name} rays")
     assert np.abs(cs.want["cams"]).max() > 0
-    if cs.V > 1:                                           # the invalid view (1, V-1) gets exactly zero
-        assert not g_cams[1 * cs.V + cs.V - 1].any()
+    for b, v in cs.invalid:                                # invalid views get exactly zero
+        assert not g_cams[b * cs.V + v].any()
     # determinism: no atomics
     g2, r2, _ = cs.call()
     assert torch.equal(g_cams, g2) and torch.equal(g_rays, r2)

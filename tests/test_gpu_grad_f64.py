@@ -1,5 +1,6 @@
 """Both cost volumes and every gradient their backward kernels write, element by element, against the float64
-reference of tests/cw_grad_ref.py.
+reference of tests/cw_grad_ref.py (gathers and scatters in torch float64 on the test's GPU), from toy sizes up to the
+production shapes of synthetic.CONFIGS, BASELINE.json's stress points and the F-Net training shapes.
 
 Tolerance: |got - ref| <= c u bound (+ floor on tensor-core outputs), u = 2^-24, c = C_TOL = 32, where bound is the
 same sum as the output with the absolute value of every factor (plus, on positions from project(), the position-error
@@ -24,7 +25,7 @@ import torch
 import magnet_b200
 from magnet_b200 import _lib, ops
 from magnet_b200.homography import plane_sweep_f
-from magnet_b200.synthetic import make_inputs
+from magnet_b200.synthetic import CONFIGS, make_inputs
 from tests.cw_grad_ref import U, Reference, gauss_chain, gauss_depths, softmax_score_grad
 
 pytestmark = pytest.mark.gpu
@@ -39,13 +40,18 @@ def _np(x):
     return x.detach().double().cpu().numpy()
 
 
+def _beyond(got, want, bound, floor=0.0):
+    """Mask of the elements beyond c u bound + floor."""
+    return np.abs(got - want) > C_TOL * U * bound + floor
+
+
 def _close(got, want, bound, what, floor=0.0):
     got = _np(got) if isinstance(got, torch.Tensor) else np.asarray(got, np.float64)
     assert got.shape == want.shape, (what, got.shape, want.shape)
     assert np.isfinite(got).all(), f"{what}: non-finite output"
     tol = C_TOL * U * bound + floor
     err = np.abs(got - want)
-    bad = err > tol
+    bad = _beyond(got, want, bound, floor)
     ratio = float(np.max(np.where(tol > 0, err / np.where(tol > 0, tol, 1.0), 0.0))) * C_TOL
     print(f"{what}: max |err| / (u bound + floor) = {ratio:.3g}")
     if bad.any():
@@ -54,21 +60,30 @@ def _close(got, want, bound, what, floor=0.0):
                              f"{got[i]!r}, want {want[i]!r}, tol {tol[i]!r}")
 
 
-def _close_fwd(got, rf, what, pos_err=None, floor=0.0):
-    """The volume, element by element; an element beyond the tolerance must be a clean flip of one view whose float64
-    margin is <= 1e-3."""
+def _fwd_bad(got, rf, pos_err=None, floor=0.0):
+    """(beyond, rejected): the volume's elements beyond the tolerance, and those of them that are not a clean flip of
+    one view whose float64 margin is <= 1e-3."""
     want, bound, terms, vmargin = rf.forward(pos_err)
-    got = _np(got)
-    assert np.isfinite(got).all(), f"{what}: non-finite output"
     tol = C_TOL * U * bound + floor
-    bad = np.abs(got - want) > tol
+    bad = _beyond(got, want, bound, floor)
     clean = np.zeros_like(bad)
     for v in range(terms.shape[0]):
         for sign in (1.0, -1.0):
             clean |= (vmargin[v] <= 1e-3) & (np.abs(got - want - sign * terms[v]) <= tol)
+    return bad, bad & ~clean
+
+
+def _close_fwd(got, rf, what, pos_err=None, floor=0.0):
+    """The volume, element by element; an element beyond the tolerance must be a clean flip of one view whose float64
+    margin is <= 1e-3."""
+    got = _np(got)
+    assert np.isfinite(got).all(), f"{what}: non-finite output"
+    bad, rejected = _fwd_bad(got, rf, pos_err, floor)
     print(f"{what}: {int(bad.sum())} clean flips of {bad.size}")
-    assert not (bad & ~clean).any(), (what, int((bad & ~clean).sum()),
-                                      float(np.max(np.abs(got - want)[bad & ~clean] / tol[bad & ~clean])))
+    if rejected.any():
+        want, bound = rf.forward(pos_err)[:2]
+        tol = C_TOL * U * bound + floor
+        raise AssertionError((what, int(rejected.sum()), float(np.max(np.abs(got - want)[rejected] / tol[rejected]))))
 
 
 def _tile_gbound(gs):
@@ -133,6 +148,20 @@ CASES = {
     # consistency off
     "nocw_c8": dict(C=8, B=2, V=3, H=10, W=14, D=9, path="nocw"),
     "nocw_c64_mma_mask": dict(C=64, B=1, V=3, H=12, W=16, D=32, path="nocw", mask="mma"),
+    # production shapes (synthetic.CONFIGS): each persistent CTA of the tensor-core kernels takes at least `per_cta` work
+    # items, the geometry reduction runs its block loop, the windows span every width of DESIGN §3.1
+    "cfg2_gauss": dict(cfg="cfg2", path="tc", mode="gauss", invalid=[(2, 1), (1, 0), (1, 1), (1, 2), (1, 3)],
+                       per_cta=4, max_zeroed=0.02),
+    "cfg3_volume": dict(cfg="cfg3", path="tc", per_cta=4, max_zeroed=0.02),
+    # BASELINE.json's stress points: V = 8, and D = 256 (4 hypothesis chunks per tile); B = 2 gives 600 tiles, two or
+    # more per CTA
+    "stress_v8_d256": dict(cfg="cfg2", B=2, V=8, D=256, path="tc", depth="random", per_cta=2, max_zeroed=0.05),
+    "stress_v2_d32": dict(cfg="cfg2", B=2, V=2, D=32, path="tc", per_cta=2, max_zeroed=0.015),
+    # one partial 32-hypothesis chunk, ragged tiles on both axes, feature scales far apart, pixels at the split16 floor
+    "ragged_many_items": dict(C=64, B=6, V=5, H=117, W=157, D=96, path="tc", depth="random", sr=1e-3, ss=1e3,
+                              tiny=True, per_cta=4, max_zeroed=0.035),
+    # the shipped N_s = 5 point: DIRECT forward, CUDA-core backward
+    "cfg2_ship_d5": dict(cfg="ship", B=8, path="auto", max_zeroed=0.025),
 }
 
 
@@ -154,10 +183,22 @@ def _wide_baseline(inp):
     inp.nghbr_poses[0, 0, :3, 3] = torch.tensor([0.3, 0.05, 0.01])
 
 
+def _check_persistent(B, V, D, H, W, per_cta, dev):
+    """The persistent tensor-core kernels hand each CTA at least ``per_cta`` work items: the forward's (batch element,
+    8x8 tile, 64-hypothesis chunk) items against the grid it launches, the backward's (batch element, tile) items
+    against its two CTAs per SM.  So the state carried from one item to the next is compared too."""
+    tiles = B * -(-H // 8) * -(-W // 8)
+    grid = ops.cost_launch_info(B, V, D, 64, H, W, variant=_lib.VARIANT_MMA)[0]
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    print(f"work items per CTA: forward {tiles * -(-D // 64) / grid:.1f}, backward {tiles / (2 * sms):.1f}")
+    assert tiles * -(-D // 64) >= per_cta * grid and tiles >= per_cta * 2 * sms, (tiles, D, grid, sms)
+
+
 class Case:
     def __init__(self, name, cuda):
         spec = dict(depth="smooth", invalid=[], sr=1.0, ss=1.0, tiny=False, gout="span", mode="volume", trans=None,
-                    mask=None, max_zeroed=0.06)
+                    mask=None, max_zeroed=0.06, family="scannet", per_cta=None)
+        spec.update(CONFIGS.get(CASES[name].get("cfg"), {}))
         spec.update(CASES[name])
         self.__dict__.update(spec)
         self.name = name
@@ -165,7 +206,7 @@ class Case:
         seed = sum(map(ord, name))
         depth_kind = "smooth" if self.mode == "gauss" else self.depth
         inp = make_inputs(B=B, V=V, D=D, H=H, W=W, C=C, seed=seed, depth=depth_kind, invalid=self.invalid,
-                          trans=self.trans)
+                          trans=self.trans, family=self.family)
         _wide_baseline(inp)
         rng = np.random.default_rng(seed)
         ref = inp.ref_feat.numpy() * np.float32(self.sr)
@@ -200,7 +241,7 @@ class Case:
         self.pos = "mma" if tc else "direct"
         self.rf = Reference(self.depth_vol, ref, src, inp.nghbr_gmms.numpy(), self.cams.cpu().numpy(),
                             inp.cam_intrins['unit_ray_array_2D'].numpy(), float(inp.thres), pos=self.pos,
-                            consistency=self.path != "nocw")
+                            consistency=self.path != "nocw", device=cuda)
         amb = self.rf.ambiguous()
         self.amb = amb
         if self.gout == "zero":
@@ -221,15 +262,19 @@ class Case:
         reach = ["tap_outside", "behind"] + (["clamped"] if self.D > 1 else [])
         for k in reach:
             assert (self.rf.reached[k].reshape(keep.shape) & keep).any(), (self.name, k)
+        if self.per_cta:
+            _check_persistent(self.B, self.V, self.D, self.H, self.W, self.per_cta, self.dev)
 
-    def leaves(self, need=("d", "ref", "src")):
+    def leaves(self, need=("d", "ref", "src"), ref=None):
         d = torch.from_numpy(self.depth_vol if self.mode == "volume" else self.inp.ref_gmms.numpy()).to(self.dev)
-        return (d.clone().requires_grad_("d" in need), torch.from_numpy(self.ref).to(self.dev).requires_grad_("ref" in need),
+        ref = self.ref if ref is None else ref
+        return (d.clone().requires_grad_("d" in need), torch.from_numpy(ref).to(self.dev).requires_grad_("ref" in need),
                 torch.from_numpy(self.src).to(self.dev).requires_grad_("src" in need))
 
-    def run(self, need=("d", "ref", "src"), variant=None):
-        """Forward + backward through the public entry point; returns (out, grad_d, grad_ref, grad_src)."""
-        d, ref, src = self.leaves(need)
+    def run(self, need=("d", "ref", "src"), variant=None, ref=None):
+        """Forward + backward through the public entry point, optionally on other reference features; returns (out,
+        grad_d, grad_ref, grad_src)."""
+        d, ref, src = self.leaves(need, ref)
         g, inp = self.g, self.inp
         if variant is None:
             variant = _lib.VARIANT_DIRECT if self.path == "direct" else _lib.VARIANT_AUTO
@@ -244,10 +289,12 @@ class Case:
         torch.cuda.synchronize()
         return out.detach(), d.grad, ref.grad, src.grad
 
-    def forward_variant(self, name):
-        """No-grad forward on one kernel variant, or None when the variant does not take this call."""
+    def forward_variant(self, name, src=None):
+        """No-grad forward on one kernel variant (optionally on other source features), or None when the variant does
+        not take this call."""
         g, inp = self.g, self.inp
-        ref, src = torch.from_numpy(self.ref).to(self.dev), torch.from_numpy(self.src).to(self.dev)
+        src = self.src if src is None else src
+        ref, src = torch.from_numpy(self.ref).to(self.dev), torch.from_numpy(src).to(self.dev)
         try:
             with torch.no_grad():
                 if self.mode == "gauss":
@@ -361,7 +408,8 @@ def test_cw_without_consistency(cuda, name):
 SUBSETS = [("d",), ("ref",), ("src",), ("d", "ref"), ("d", "src"), ("ref", "src")]
 
 
-@pytest.mark.parametrize("name", ["c3_w1", "c8_scales", "c16_scales", "c24", "c64_d5", "tc_d32", "gauss_c13"])
+@pytest.mark.parametrize("name", ["c3_w1", "c8_scales", "c16_scales", "c24", "c64_d5", "tc_d32", "gauss_c13",
+                                  "cfg2_gauss"])
 def test_gradient_subsets(cuda, name):
     """Asking for fewer gradients changes none of the others.  The CUDA-core kernel's grad_ref and grad_d have one owner
     each and a fixed summation order: bit-identical to the run with all three.  grad_src (global atomics) and the
@@ -385,6 +433,86 @@ def test_gradient_subsets(cuda, name):
             assert gs is None
 
 
+def _window_cells(rf):
+    """Cells of the tensor-core window of every (batch element, 8x8 tile, 64-hypothesis chunk, valid view): the box of
+    the float64 reference's cell origins plus the right / lower taps, cut into 8-cell segments (cost_mma.cu)."""
+    x0, x1, y0, y1 = rf.origins                                   # (B, V, chunks, HW)
+    B, V, nk = x0.shape[:3]
+    H, W = rf.H, rf.W
+    Hp, Wp = -(-H // 8) * 8, -(-W // 8) * 8
+
+    def tile(a, red, fill):
+        pad = np.full((B, V, nk, Hp, Wp), fill)
+        pad[..., :H, :W] = a.reshape(B, V, nk, H, W)
+        return red(pad.reshape(B, V, nk, Hp // 8, 8, Wp // 8, 8), axis=(4, 6))
+    lx, hx, ly, hy = tile(x0, np.min, np.inf), tile(x1, np.max, -np.inf), tile(y0, np.min, np.inf), tile(y1, np.max, -np.inf)
+    live = np.isfinite(lx)                                        # the valid views
+    return (((hx - lx + 2 + 7) // 8) * (hy - ly + 2) * 8)[live]
+
+
+def test_tensor_core_cases_reach_every_window_width(cuda):
+    """Across the tensor-core CW cases the windows take all four shapes of DESIGN §3.1: warpgroup 1 idle (<= 128
+    cells), n64 (129-192), n128 (193-256) and sub-windows (> 256)."""
+    cells = np.concatenate([_window_cells(_case(n, cuda).rf) for n in sorted(CASES) if CASES[n]["path"] == "tc"])
+    widths = {"<= 128": cells <= 128, "129-192": (cells > 128) & (cells <= 192),
+              "193-256": (cells > 192) & (cells <= 256), "> 256": cells > 256}
+    print({k: int(m.sum()) for k, m in widths.items()})
+    assert all(m.any() for m in widths.values())
+
+
+def test_gate_rejects_subtle_errors_at_production_scale(cuda):
+    """At cfg2 the bounds sum over many more terms than at the small cases; they must still reject a forward on source
+    maps rounded to fp16 (relative error 2^-11), a grad_src on a reference map rounded to bf16 (2^-8), and one view's
+    term cost_v / V subtracted over the last work item handed out (the last 8x8 tile of the last batch element): where
+    the view is in the mask that removes its term, elsewhere it adds a spurious one.  The gate must flag that tile and
+    nothing else.
+
+    The rounded inputs go through the kernels whose positions the reference reproduces exactly (the DIRECT forward,
+    the CUDA-core backward with its mask): on project() positions the bound carries the position error
+    (A + 8) u |ix + 0.5| |d cost / d ix|, at |ix| ~ 100 px some 2^-9 of the value, which a 2^-11 feature error hides in."""
+    cs = _case("cfg2_gauss", cuda)
+    V = cs.V
+    rf = Reference(cs.depth_vol, cs.ref, cs.src, cs.inp.nghbr_gmms.numpy(), cs.cams.cpu().numpy(),
+                   cs.inp.cam_intrins['unit_ray_array_2D'].numpy(), float(cs.inp.thres), pos="direct", device=cuda)
+    amb = rf.ambiguous()
+    assert not _fwd_bad(_np(cs.forward_variant("direct")), rf, pos_err=False)[1].any()
+    src16 = cs.src.astype(np.float16).astype(np.float32)
+    _, rejected = _fwd_bad(_np(cs.forward_variant("direct", src=src16)), rf, pos_err=False)
+    live = ~amb & (rf.forward(False)[1] > 0)
+    print(f"fp16 source maps: forward rejected at {rejected[live].mean():.3f} of the unambiguous elements")
+    assert rejected[live].mean() > 0.5
+    gout = np.where(amb, np.float32(0), cs.gout).astype(np.float32)
+    want = rf.backward(gout.astype(np.float64) / V)
+    ref16 = torch.from_numpy(cs.ref).bfloat16().float().numpy()
+    for ref, rounded in ((cs.ref, False), (ref16, True)):
+        _, gsrc, _ = ops.cost_volume_bwd(torch.from_numpy(ref).to(cuda), torch.from_numpy(cs.src).to(cuda),
+                                         cs.g.nghbr_gmms, cs.rays, cs.cams, torch.from_numpy(gout).to(cuda), V=V,
+                                         kappa=float(cs.inp.thres), fwd_layout=_lib.SRC_NCHW,
+                                         fwd_variant=_lib.VARIANT_DIRECT, need_ref=False, need_depth=False,
+                                         ref_gmm=cs.g.ref_gmms, k=cs.k)
+        bad = _beyond(_np(gsrc), want["src"], want["src_b"])
+        live = want["src_b"] > 0
+        print(f"reference map rounded={rounded}: grad_src rejected at {bad[live].mean():.3f} of its elements")
+        assert bad[live].mean() > 0.5 if rounded else not bad.any()
+    # one view's term subtracted over one tile, on the tensor-core forward and its own reference
+    floor = _mma_fwd_floor(cs)
+    want, bound, terms, vmargin = cs.rf.forward()
+    got = _np(cs.forward_variant("mma"))
+    assert not _fwd_bad(got, cs.rf, floor=floor)[1].any()
+    tile = np.zeros(got.shape, bool)
+    tile[-1, :, -8:, -8:] = True
+    tol = C_TOL * U * bound + floor
+    # the view whose samples of the corner tile fall inside the image most often; an element must be rejected when
+    # the subtracted term exceeds the tolerance and the view is not within 1e-3 of a mask flip
+    musts = {v: tile & (np.abs(terms[v]) > tol) & (vmargin[v] > 1e-3) for v in range(cs.V) if (cs.B - 1, v) in cs.rf.valid}
+    v = max(musts, key=lambda v: musts[v].sum())
+    got[tile] -= terms[v][tile]
+    _, rejected = _fwd_bad(got, cs.rf, floor=floor)
+    print(f"view {v}'s term subtracted: {int(rejected.sum())} rejected, {int(musts[v].sum())} of the tile's "
+          f"{int(tile.sum())} elements must be")
+    assert musts[v].any() and rejected[musts[v]].all() and not (rejected & ~tile).any()
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # F volume
 
@@ -394,20 +522,27 @@ F_CASES = {
     "f32": dict(C=32, B=2, V=2, H=10, W=14, D=20),
     "f64": dict(C=64, B=1, V=3, H=12, W=16, D=9),
     "f64_tc_sid": dict(C=64, B=2, V=3, H=12, W=20, D=48, tc=True),
+    # the F-Net training shapes (test_gpu_fnet.py): 80 SID planes from 1e-3 to the family's maximum depth
+    "fnet_scannet": dict(C=64, B=2, V=4, H=120, W=160, D=80, tc=True, per_cta=2),
+    "fnet_kitti": dict(C=64, B=4, V=2, H=88, W=304, D=80, tc=True, family="kitti", far=80.0, per_cta=4),
 }
 
 
 class FCase:
     def __init__(self, name, cuda):
-        spec = dict(F_CASES[name])
-        self.name, self.tc = name, spec.pop("tc", False)
+        spec = dict(tc=False, family="scannet", far=10.0, per_cta=None)
+        spec.update(F_CASES[name])
         self.__dict__.update(spec)
+        self.name = name
         seed = sum(map(ord, name))
-        inp = make_inputs(**spec, seed=seed, depth="smooth", invalid=[(0, 1)])
+        inp = make_inputs(B=self.B, V=self.V, D=self.D, H=self.H, W=self.W, C=self.C, seed=seed, depth="smooth",
+                          invalid=[(0, 1)], family=self.family)
         _wide_baseline(inp)
         self.inp, self.dev = inp, cuda
+        if self.per_cta:
+            _check_persistent(self.B, self.V, self.D, self.H, self.W, self.per_cta, cuda)
         if self.tc:                            # SID planes from 1e-3: a tile spreads along an epipolar line
-            self.planes = magnet_b200.sid_planes(1e-3, 10.0, self.D, device=cuda).reshape(1, -1, 1, 1)
+            self.planes = magnet_b200.sid_planes(1e-3, self.far, self.D, device=cuda).reshape(1, -1, 1, 1)
         else:                                  # the first plane is close enough to reach the clamp
             self.planes = torch.tensor([0.002] + np.linspace(0.3, 8.0, self.D - 1).tolist(),
                                        device=cuda).reshape(1, -1, 1, 1)
@@ -418,7 +553,7 @@ class FCase:
         pl = np.float32(self.planes.reshape(-1).cpu().numpy())
         depth = np.broadcast_to(pl.reshape(1, -1, 1, 1), (self.B, self.D, self.H, self.W))
         self.rf = Reference(depth, inp.ref_feat.numpy(), inp.nghbr_feat.numpy(), None, cams.cpu().numpy(),
-                            inp.cam_intrins['unit_ray_array_2D'].numpy(), 0.0, pos="mma", consistency=False)
+                            inp.cam_intrins['unit_ray_array_2D'].numpy(), 0.0, pos="mma", consistency=False, device=cuda)
         rng = np.random.default_rng(seed)
         self.gout = _spanning_gout(rng, (self.B, self.D, self.H, self.W))
 

@@ -183,8 +183,8 @@ def test_volume_mode_without_consistency_at_ops_level(cuda, dt):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# gradients: the float64 reference of tests/cw_grad_ref.py on the upcast maps (cases of test_gpu_grad_f64 with unit
-# feature scales, so that the half maps are the rounded fp32 ones)
+# gradients: the float64 reference of tests/cw_grad_ref.py on the upcast maps, contracted on the GPU (cases of
+# test_gpu_grad_f64 with unit feature scales, so that the half maps are the rounded fp32 ones, up to cfg2)
 def _half_case(name, cuda, dt):
     orig = gf.make_inputs
 
@@ -211,7 +211,7 @@ def _ulp(x, dt):
 
 
 @pytest.mark.parametrize("dt", DTYPES, ids=DT_IDS)
-@pytest.mark.parametrize("name", ["tc_d32", "gauss_c64_tc"])
+@pytest.mark.parametrize("name", ["tc_d32", "gauss_c64_tc", "cfg2_gauss"])
 def test_cw_gradients_half16(cuda, dt, name):
     cs = _half_case(name, cuda, dt)
     g, inp = cs.g, cs.inp
