@@ -44,7 +44,13 @@ def main():
     ap.add_argument("--fused-head", action="store_true",
                     help="train the G-Net head through the fused tensor-core forward and backward (DESIGN §3.10) "
                          "instead of the cuDNN module chain")
+    ap.add_argument("--fused-mask", action="store_true",
+                    help="run the mask head after its first convolution, the upsampling and the loss as one fused "
+                         "tensor-core op with its backward (MagnetHead.train_loss with fused_upsample, DESIGN §3.13) "
+                         "instead of the cuDNN mask head and the fused upsample+NLL kernels")
     args = ap.parse_args()
+    if args.fused_mask and args.unfused_loss:
+        raise SystemExit("--fused-mask and --unfused-loss exclude each other")
     rank, local_rank, world = md.env_world()
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
@@ -61,7 +67,8 @@ def main():
     mask = gt > 1e-3
 
     torch.manual_seed(0)                                                   # same init on every rank
-    head = magnet_b200.MagnetHead(n_samples=D, sampling_range=3, n_iter=3, thres=5, fused_train=args.fused_head).to(dev)
+    head = magnet_b200.MagnetHead(n_samples=D, sampling_range=3, n_iter=3, thres=5, fused_train=args.fused_head,
+                                   fused_upsample=args.fused_mask).to(dev)
     reducer = md.FlatGradAllReduce(head.parameters())
     reducer.broadcast_parameters(0)
     opt = torch.optim.AdamW(head.parameters(), lr=3.57e-4, weight_decay=1e-2)
@@ -77,6 +84,9 @@ def main():
             preds = head(inp.ref_feat, inp.nghbr_feat, inp.ref_gmms, inp.nghbr_gmms, x_d3, inp.nghbr_poses,
                          inp.is_valid, inp.cam_intrins)
             loss = gaussian_nll(preds, gt, mask)
+        elif args.fused_mask:
+            loss = head.train_loss(inp.ref_feat, inp.nghbr_feat, inp.ref_gmms, inp.nghbr_gmms, x_d3, inp.nghbr_poses,
+                                   inp.is_valid, inp.cam_intrins, gt, mask)
         else:                                                              # f-2: no (B,2,4H,4W) tensors, fwd or bwd
             preds_q, up_mask = head.forward_quarter(inp.ref_feat, inp.nghbr_feat, inp.ref_gmms, inp.nghbr_gmms, x_d3,
                                                     inp.nghbr_poses, inp.is_valid, inp.cam_intrins)
@@ -94,7 +104,8 @@ def main():
     if rank == 0:
         print(json.dumps({"config": "train head, ScanNet shape", "n_gpus": world, "global_batch": gb, "steps": args.steps,
                           "head_path": "fused G-Net kernels" if args.fused_head else "cuDNN module chain",
-                          "loss_path": "unfused (torch NLL on upsampled predictions)" if args.unfused_loss else "fused upsample+NLL kernels",
+                          "loss_path": "unfused (torch NLL on upsampled predictions)" if args.unfused_loss else
+                                       "fused mask head + upsample + NLL kernel" if args.fused_mask else "fused upsample+NLL kernels",
                           "ms_per_step": 1e3 * dt / args.steps, "frames_per_s": gb * args.steps / dt,
                           "rank0_step_ms_median": per_step[len(per_step) // 2], "rank0_step_ms_max": per_step[-1],
                           "loss_first": losses[0], "loss_last": losses[-1], "trainable_params": reducer.bucket.numel()}))

@@ -393,6 +393,70 @@ int magnet_mask_pack_weights_f32(const float* w1, const float* b1, const float* 
 int magnet_mask_upsample_f32(const magnet_mask_upsample_args* args, void* stream);
 
 /*
+ * Mask head, learned upsampling and Gaussian NLL of training, fused (DESIGN §3.13) — replaces, after the first mask-head
+ * convolution, mask_head (models/MAGNET.py:111-118), upsample_depth_via_mask (MAGNET.py:15-27,172-173) and MagnetLoss
+ * (utils/losses.py:34-50) of every prediction, and their autograd backward:
+ *   loss = sum_p gamma_p mean_{gt_mask} nll(upsample(pred[p], mask)),  nll = (mu-gt)^2 / (2 var) + 0.5 log(var),
+ *   var = max(sigma^2, 1e-10), mask as magnet_mask_upsample_f32 computes it (the logits are that kernel's bits).
+ *
+ * magnet_mask_pack_train_weights_f32: the inference pack of magnet_mask_pack_weights_f32 followed by W3^T, W2^T and W1^T
+ * for the backward, magnet_mask_train_weights_bytes(4) bytes (0 for any other k).  Three kernels.
+ *
+ * magnet_mask_train_fwd_f32: partial[magnet_mask_train_partials(B,H,W) x P] receives, per 8x16 tile and prediction,
+ * the tile's sum of nll over its supervised full-resolution pixels (row-major [tile][p]; the caller adds them in a
+ * fixed order, divides by the number of supervised pixels and weights them).  pred_scale[p] (HOST) = gamma_p / count,
+ * the scale of prediction p's gradient at unit upstream gradient.  With save_maps the forward stores h0, h1, h2 and the
+ * logits' gradient into `saved` (needed by any weight or pre0 gradient); with pred_grad it accumulates the prediction
+ * gradients there (needed by grad_pred).  `saved` holds magnet_mask_saved_bytes(P,B,H,W) bytes: the P prediction
+ * gradients (B,2,H,W) first, then h0, h1, h2 (B,128,H,W) and the logits' gradient (B,128,H,W) + (B,16,H,W); a forward
+ * without save_maps uses only the first 2*P*B*H*W floats, so the caller may pass a buffer of that size.  No upsampled
+ * prediction and no mask is written.  Loss partials and saved maps are bit-identical from run to run; the prediction
+ * gradients are sums of atomic adds.  One memset (pred_grad) and one kernel.
+ *
+ * magnet_mask_bwd_f32: given grad_scale = dL/d loss (a DEVICE float), writes grad_pre0 (B,128,H,W) = dL/d pre0,
+ * grad_w1 / grad_w2 (128,128), grad_b1 / grad_b2 (128), grad_w3 (144,128), grad_b3 (144) and grad_pred[p] (B,2,H,W);
+ * each may be NULL (not computed), as may grad_pred itself.  Each output is its unit-gradient value times grad_scale
+ * (one rounding; exact for 1.0).  Weight gradients are fixed-order sums: bit-identical from run to run.  Uses
+ * `workspace` (magnet_mask_bwd_workspace_bytes(B,H,W) bytes).  Asking for a weight or pre0 gradient after a forward
+ * without save_maps, or for a prediction gradient after one without pred_grad, reads unwritten memory.
+ *
+ * Both calls: P outside 1..MAGNET_MASK_MAX_PRED or k != 4 -> MAGNET_ERR_UNSUPPORTED; B*H*W < 2^31; pre0,
+ * packed_weights, saved, workspace and every pred pointer 16-byte aligned.
+ */
+typedef struct magnet_mask_train_args {
+  int32_t P, B, H, W;        /* predictions, images, quarter-resolution size                                        */
+  int32_t k;                 /* upsampling factor: 4                                                                */
+  const float* pre0;         /* (B, 128, H, W) the first mask-head convolution's output, before its ReLU; forward    */
+  const void* packed_weights;/* magnet_mask_pack_train_weights_f32 output                                           */
+  const float* const* pred;  /* HOST array of P DEVICE pointers, each (B, 2, H, W) [mu, sigma]; forward             */
+  const float* gt;           /* (B, 1, k*H, k*W) ground-truth depth; forward                                         */
+  const uint8_t* gt_mask;    /* (B, 1, k*H, k*W) nonzero = supervised; forward                                       */
+  const float* pred_scale;   /* HOST array of P floats: gamma_p / number of supervised pixels; forward              */
+  int32_t save_maps;         /* forward: nonzero = store what the weight and pre0 gradients need                     */
+  int32_t pred_grad;         /* forward: nonzero = accumulate the prediction gradients                               */
+  float* partial;            /* forward: magnet_mask_train_partials(B, H, W) x P floats                              */
+  float* saved;              /* magnet_mask_saved_bytes(P, B, H, W): written by the forward, read by the backward    */
+  const float* grad_scale;   /* DEVICE float, the loss's upstream gradient; backward                                */
+  void* workspace;           /* magnet_mask_bwd_workspace_bytes(B, H, W); backward                                  */
+  float* grad_pre0;          /* (B, 128, H, W) or NULL                                                              */
+  float* grad_w1;            /* (128, 128) or NULL                                                                  */
+  float* grad_b1;            /* (128) or NULL                                                                       */
+  float* grad_w2;            /* (128, 128) or NULL                                                                  */
+  float* grad_b2;            /* (128) or NULL                                                                       */
+  float* grad_w3;            /* (144, 128) or NULL                                                                  */
+  float* grad_b3;            /* (144) or NULL                                                                       */
+  float* const* grad_pred;   /* HOST array of P DEVICE pointers (entries may be NULL), or NULL; backward            */
+} magnet_mask_train_args;
+size_t magnet_mask_train_weights_bytes(int32_t k);
+size_t magnet_mask_saved_bytes(int32_t P, int32_t B, int32_t H, int32_t W);
+size_t magnet_mask_bwd_workspace_bytes(int32_t B, int32_t H, int32_t W);
+int magnet_mask_train_partials(int32_t B, int32_t H, int32_t W);
+int magnet_mask_pack_train_weights_f32(const float* w1, const float* b1, const float* w2, const float* b2,
+                                       const float* w3, const float* b3, void* packed, void* stream);
+int magnet_mask_train_fwd_f32(const magnet_mask_train_args* args, void* stream);
+int magnet_mask_bwd_f32(const magnet_mask_train_args* args, void* stream);
+
+/*
  * Caller-side camera preparation on the device (SURVEY §8 f-4).
  * magnet_relative_poses_f32 replaces utils/utils.py:72-98 (data_preprocess): poses_out[b,v] = ext_nghbr[v,b] *
  * inv(ext_ref[b]) (ref-camera -> source-camera), is_valid_out[b,v] = 0 when either extrinsic or the product holds a

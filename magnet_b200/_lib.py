@@ -43,6 +43,9 @@ EXPORTS = (
     "magnet_gnet_pack_train_weights_f32", "magnet_gnet_train_fwd_f32", "magnet_gnet_bwd_f32",
     "magnet_cost_geom_workspace_bytes", "magnet_cost_volume_geom_bwd_f32",
     "magnet_mask_weights_bytes", "magnet_mask_pack_weights_f32", "magnet_mask_upsample_f32",
+    "magnet_mask_train_weights_bytes", "magnet_mask_saved_bytes", "magnet_mask_bwd_workspace_bytes",
+    "magnet_mask_train_partials", "magnet_mask_pack_train_weights_f32", "magnet_mask_train_fwd_f32",
+    "magnet_mask_bwd_f32",
 )
 MAGNET_HIDDEN_CHANNELS = 128
 MAGNET_GNET_SCRATCH_BYTES = 16
@@ -110,6 +113,17 @@ class MaskUpsampleArgs(C.Structure):
     _fields_ = [("P", C.c_int32), ("B", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("k", C.c_int32),
                 ("pre0", C.c_void_p), ("packed_weights", C.c_void_p), ("pred", C.POINTER(C.c_void_p)),
                 ("out", C.POINTER(C.c_void_p))]
+
+
+class MaskTrainArgs(C.Structure):
+    """Mirror of ``struct magnet_mask_train_args``."""
+    _fields_ = [("P", C.c_int32), ("B", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("k", C.c_int32),
+                ("pre0", C.c_void_p), ("packed_weights", C.c_void_p), ("pred", C.POINTER(C.c_void_p)),
+                ("gt", C.c_void_p), ("gt_mask", C.c_void_p), ("pred_scale", C.POINTER(C.c_float)),
+                ("save_maps", C.c_int32), ("pred_grad", C.c_int32), ("partial", C.c_void_p), ("saved", C.c_void_p),
+                ("grad_scale", C.c_void_p), ("workspace", C.c_void_p)] + [
+        (n, C.c_void_p) for n in ("grad_pre0", "grad_w1", "grad_b1", "grad_w2", "grad_b2", "grad_w3", "grad_b3")] + [
+        ("grad_pred", C.POINTER(C.c_void_p))]
 
 
 class MagnetError(RuntimeError):
@@ -228,6 +242,20 @@ def lib() -> C.CDLL:
     L.magnet_mask_pack_weights_f32.argtypes = [C.c_void_p] * 8
     L.magnet_mask_upsample_f32.restype = C.c_int
     L.magnet_mask_upsample_f32.argtypes = [C.POINTER(MaskUpsampleArgs), C.c_void_p]
+    L.magnet_mask_train_weights_bytes.restype = C.c_size_t
+    L.magnet_mask_train_weights_bytes.argtypes = [C.c_int32]
+    L.magnet_mask_saved_bytes.restype = C.c_size_t
+    L.magnet_mask_saved_bytes.argtypes = [C.c_int32] * 4
+    L.magnet_mask_bwd_workspace_bytes.restype = C.c_size_t
+    L.magnet_mask_bwd_workspace_bytes.argtypes = [C.c_int32] * 3
+    L.magnet_mask_train_partials.restype = C.c_int
+    L.magnet_mask_train_partials.argtypes = [C.c_int32] * 3
+    L.magnet_mask_pack_train_weights_f32.restype = C.c_int
+    L.magnet_mask_pack_train_weights_f32.argtypes = [C.c_void_p] * 8
+    L.magnet_mask_train_fwd_f32.restype = C.c_int
+    L.magnet_mask_train_fwd_f32.argtypes = [C.POINTER(MaskTrainArgs), C.c_void_p]
+    L.magnet_mask_bwd_f32.restype = C.c_int
+    L.magnet_mask_bwd_f32.argtypes = [C.POINTER(MaskTrainArgs), C.c_void_p]
     if L.magnet_abi_version() != MAGNET_ABI_VERSION:
         raise MagnetError(f"ABI version mismatch: library {L.magnet_abi_version()} != binding {MAGNET_ABI_VERSION}")
     _lib = L

@@ -84,6 +84,19 @@ cudaError_t launch_mask_pack(const float* w1, const float* b1, const float* w2, 
                              const float* b3, void* dst, cudaStream_t st);
 cudaError_t launch_mask_upsample(int P, int B, int H, int W, const float* pre0, const void* weights,
                                  const float* const* pred, float* const* out, cudaStream_t st);
+size_t mask_train_weights_bytes();
+int mask_train_partials(int B, int H, int W);
+size_t mask_saved_bytes(int P, int B, int H, int W);
+size_t mask_bwd_workspace_bytes(int B, int H, int W);
+cudaError_t launch_mask_pack_train(const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
+                                   const float* b3, void* dst, cudaStream_t st);
+cudaError_t launch_mask_train_fwd(int P, int B, int H, int W, const float* pre0, const void* weights,
+                                  const float* const* pred, const float* gt, const unsigned char* gtm,
+                                  const float* scale, bool save_maps, bool pred_grad, float* partial, float* saved,
+                                  cudaStream_t st, int* launches);
+cudaError_t launch_mask_bwd(int P, int B, int H, int W, const void* weights, const float* saved, const float* gscale,
+                            void* workspace, float* grad_pre0, float* gw1, float* gb1, float* gw2, float* gb2,
+                            float* gw3, float* gb3, float* const* grad_pred, cudaStream_t st, int* launches);
 size_t gnet_saved_bytes(int B, int H, int W);
 size_t gnet_bwd_workspace_bytes(int B, int D, int H, int W);
 cudaError_t launch_gnet_pack_train(const float* w0, const float* w1, const float* b1, const float* w2, const float* b2,
@@ -760,6 +773,81 @@ int magnet_mask_upsample_f32(const magnet_mask_upsample_args* a, void* stream) {
                                                (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e);
   g_launches += 1;
+  return MAGNET_OK;
+}
+
+namespace {
+bool mask_train_shape_ok(int32_t B, int32_t H, int32_t W) {
+  return B > 0 && H > 0 && W > 0 && (int64_t)B * H * W < ((int64_t)1 << 31);
+}
+
+// shape, factor, prediction count and the pointers both training calls read
+int validate_mask_train(const magnet_mask_train_args* a) {
+  if (!a) return MAGNET_ERR_NULL;
+  if (!mask_train_shape_ok(a->B, a->H, a->W)) return MAGNET_ERR_SHAPE;
+  if (a->P < 1 || a->P > MAGNET_MASK_MAX_PRED || a->k != 4) return MAGNET_ERR_UNSUPPORTED;
+  if (!a->packed_weights || !a->saved) return MAGNET_ERR_NULL;
+  if (misaligned16(a->packed_weights) || misaligned16(a->saved)) return MAGNET_ERR_ALIGN;
+  return MAGNET_OK;
+}
+}  // namespace
+
+size_t magnet_mask_train_weights_bytes(int32_t k) { return k == 4 ? magnet::mask_train_weights_bytes() : 0; }
+
+size_t magnet_mask_saved_bytes(int32_t P, int32_t B, int32_t H, int32_t W) {
+  if (P < 1 || P > MAGNET_MASK_MAX_PRED || !mask_train_shape_ok(B, H, W)) return 0;
+  return magnet::mask_saved_bytes(P, B, H, W);
+}
+
+size_t magnet_mask_bwd_workspace_bytes(int32_t B, int32_t H, int32_t W) {
+  if (!mask_train_shape_ok(B, H, W)) return 0;
+  return magnet::mask_bwd_workspace_bytes(B, H, W);
+}
+
+int magnet_mask_train_partials(int32_t B, int32_t H, int32_t W) {
+  if (!mask_train_shape_ok(B, H, W)) return MAGNET_ERR_SHAPE;
+  return magnet::mask_train_partials(B, H, W);
+}
+
+int magnet_mask_pack_train_weights_f32(const float* w1, const float* b1, const float* w2, const float* b2,
+                                       const float* w3, const float* b3, void* packed, void* stream) {
+  if (!w1 || !b1 || !w2 || !b2 || !w3 || !b3 || !packed) return MAGNET_ERR_NULL;
+  if (misaligned16(packed)) return MAGNET_ERR_ALIGN;
+  cudaError_t e = magnet::launch_mask_pack_train(w1, b1, w2, b2, w3, b3, packed, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 3;
+  return MAGNET_OK;
+}
+
+int magnet_mask_train_fwd_f32(const magnet_mask_train_args* a, void* stream) {
+  const int st = validate_mask_train(a);
+  if (st != MAGNET_OK) return st;
+  if (!a->pre0 || !a->pred || !a->gt || !a->gt_mask || !a->pred_scale || !a->partial) return MAGNET_ERR_NULL;
+  for (int p = 0; p < a->P; ++p)
+    if (!a->pred[p]) return MAGNET_ERR_NULL;
+  if (misaligned16(a->pre0)) return MAGNET_ERR_ALIGN;
+  for (int p = 0; p < a->P; ++p)
+    if (misaligned16(a->pred[p])) return MAGNET_ERR_ALIGN;
+  int launches = 0;
+  cudaError_t e = magnet::launch_mask_train_fwd(a->P, a->B, a->H, a->W, a->pre0, a->packed_weights, a->pred, a->gt,
+                                                a->gt_mask, a->pred_scale, a->save_maps != 0, a->pred_grad != 0,
+                                                a->partial, a->saved, (cudaStream_t)stream, &launches);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += launches;
+  return MAGNET_OK;
+}
+
+int magnet_mask_bwd_f32(const magnet_mask_train_args* a, void* stream) {
+  const int st = validate_mask_train(a);
+  if (st != MAGNET_OK) return st;
+  if (!a->grad_scale || !a->workspace) return MAGNET_ERR_NULL;
+  if (misaligned16(a->workspace)) return MAGNET_ERR_ALIGN;
+  int launches = 0;
+  cudaError_t e = magnet::launch_mask_bwd(a->P, a->B, a->H, a->W, a->packed_weights, a->saved, a->grad_scale,
+                                          a->workspace, a->grad_pre0, a->grad_w1, a->grad_b1, a->grad_w2, a->grad_b2,
+                                          a->grad_w3, a->grad_b3, a->grad_pred, (cudaStream_t)stream, &launches);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += launches;
   return MAGNET_OK;
 }
 

@@ -59,28 +59,6 @@ struct GnetParams {
   float* __restrict__ save;   // SAVE: h0, h1, h2 as (B,128,H,W) each, then raw (mu1, sigma1) as (B,2,H,W)
 };
 
-// The accumulator fragment of rows g, g+8 (pixels x, x+8 of one image row) into a (128, H, W) map: p points at channel
-// 2q of pixel x.  Pixel x+8 is only valid when x is.
-// The channel stride goes through an opaque copy: otherwise the compiler keeps the 32 channel addresses of one call
-// live for the next call, across a layer's MMAs, and spills.
-__device__ __forceinline__ int opaque(int v) {
-  int r;
-  asm volatile("mov.b32 %0, %1;" : "=r"(r) : "r"(v));
-  return r;
-}
-__device__ __forceinline__ void store_rows(float* __restrict__ p, const float (&acc)[NTILE][4], int HW, bool va, bool vb) {
-  HW = opaque(HW);
-#pragma unroll
-  for (int nt = 0; nt < NTILE; ++nt) {
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      float* c = p + (size_t)(nt * 8 + e) * HW;
-      if (va) c[0] = acc[nt][e];
-      if (vb) c[8] = acc[nt][2 + e];
-    }
-  }
-}
-
 // SAVE (training forward, DESIGN §3.10): the same arithmetic, plus stores of the three ReLU'd hidden maps and the raw
 // output for the backward.
 template <bool SAVE>
@@ -383,63 +361,6 @@ __global__ void __launch_bounds__(256) gnet_pack_t_kernel(const float* __restric
   reinterpret_cast<uint4*>(dst + tail)[i] = make_uint4(h0, h1, l0, l1);
 }
 
-// One 128 -> 128 layer of the backward chain on the gradient fragment (any sign): per-row scale from max |x|, split,
-// three products against the resident transposed weights, descale.  The caller applies the ReLU mask.
-__device__ __forceinline__ void grad_layer(float (&acc)[NTILE][4], const uint4* __restrict__ wsm, int shw, int lane) {
-  float m0 = 0.0f, m1 = 0.0f;
-#pragma unroll
-  for (int nt = 0; nt < NTILE; ++nt) {
-    m0 = fmaxf(m0, fmaxf(fabsf(acc[nt][0]), fabsf(acc[nt][1])));
-    m1 = fmaxf(m1, fmaxf(fabsf(acc[nt][2]), fabsf(acc[nt][3])));
-  }
-#pragma unroll
-  for (int o = 1; o <= 2; o <<= 1) {
-    m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, o));
-    m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, o));
-  }
-  const int sh0 = split16_shift(__float_as_uint(m0)), sh1 = split16_shift(__float_as_uint(m1));
-  const float s0 = pow2(sh0), s1 = pow2(sh1);
-  uint32_t ah[HID / 16][4], al[HID / 16][4];
-#pragma unroll
-  for (int kk = 0; kk < HID / 16; ++kk) {
-    split2(__fmul_rn(acc[2 * kk][0], s0), __fmul_rn(acc[2 * kk][1], s0), ah[kk][0], al[kk][0]);
-    split2(__fmul_rn(acc[2 * kk][2], s1), __fmul_rn(acc[2 * kk][3], s1), ah[kk][1], al[kk][1]);
-    split2(__fmul_rn(acc[2 * kk + 1][0], s0), __fmul_rn(acc[2 * kk + 1][1], s0), ah[kk][2], al[kk][2]);
-    split2(__fmul_rn(acc[2 * kk + 1][2], s1), __fmul_rn(acc[2 * kk + 1][3], s1), ah[kk][3], al[kk][3]);
-  }
-#pragma unroll
-  for (int nt = 0; nt < NTILE; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.0f;
-#pragma unroll
-  for (int kk = 0; kk < HID / 16; ++kk) {
-#pragma unroll
-    for (int nt = 0; nt < NTILE; ++nt) mma3(acc[nt], ah[kk], al[kk], wsm[(kk * NTILE + nt) * 32 + lane]);
-  }
-  const float dw = pow2(-shw), d0 = pow2(-sh0), d1 = pow2(-sh1);
-#pragma unroll
-  for (int nt = 0; nt < NTILE; ++nt) {
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      acc[nt][e] = __fmul_rn(__fmul_rn(acc[nt][e], d0), dw);
-      acc[nt][2 + e] = __fmul_rn(__fmul_rn(acc[nt][2 + e], d1), dw);
-    }
-  }
-}
-
-// ReLU backward on the fragment, as torch's threshold_backward: zero where the saved activation is <= 0 (a NaN
-// activation passes the gradient); h as store_rows addresses it
-__device__ __forceinline__ void relu_mask(float (&acc)[NTILE][4], const float* __restrict__ h, int HW, bool va, bool vb) {
-  HW = opaque(HW);
-#pragma unroll
-  for (int nt = 0; nt < NTILE; ++nt) {
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      const float* c = h + (size_t)(nt * 8 + e) * HW;
-      acc[nt][e] = va && !(__ldg(c) <= 0.0f) ? acc[nt][e] : 0.0f;
-      acc[nt][2 + e] = vb && !(__ldg(c + 8) <= 0.0f) ? acc[nt][2 + e] : 0.0f;
-    }
-  }
-}
-
 struct GnetBwdParams {
   int B, HW, gpi, ngroups;                   // gpi: 16-pixel groups per image
   const float* __restrict__ grad;            // (B,2,H,W) gradient of the updated Gaussian
@@ -525,7 +446,7 @@ __global__ void __launch_bounds__(NT, 1) gnet_bwd_chain_kernel(const GnetBwdPara
     // ---- d_h1, d_h0 on the tensor cores ----
 #pragma unroll 1
     for (int l = 0; l < 2; ++l) {
-      grad_layer(acc, wt + (l == 0 ? G_LAYER / 16 : 0), l == 0 ? sh_w2 : sh_w1, lane);
+      grad_layer(acc, acc, wt + (l == 0 ? G_LAYER / 16 : 0), l == 0 ? sh_w2 : sh_w1, lane);
       relu_mask(acc, (l == 0 ? h1s : h0s) + off, HW, va, vb);
       store_rows((l == 0 ? dh1 : p.grad_inv) + off, acc, HW, va, vb);
     }
@@ -712,6 +633,27 @@ cudaError_t launch_wgrad(int B, int H, int W, int Ma, const float* a, int Nw, in
   return cudaGetLastError();
 }
 }  // namespace
+
+// The same weight-gradient GEMMs for the mask head's training (mask_head.cu): out_w[m][n] = sum over the B*H*W pixels
+// of a[m] b[n] on dense (B, Ma, H, W) / (B, Nw, H, W) maps, Ma <= 128, out_b[m] = sum of a[m].  `part` holds
+// head_wgrad_partial_floats(B, H, W, Ma, Nw) floats.
+size_t head_wgrad_partial_floats(int B, int H, int W, int Ma, int Nw) {
+  return (size_t)wgrad_chunks(B * H * W) * Ma * (Nw + 1);
+}
+
+cudaError_t launch_head_wgrad(int B, int H, int W, int Ma, const float* a, int Nw, const float* b, float* part,
+                              float* out_w, float* out_b, cudaStream_t st) {
+  static std::once_flag flags[64];
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  cudaError_t res = cudaSuccess;
+  std::call_once(flags[dev & 63], [&] {
+    res = cudaFuncSetAttribute(gnet_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM);
+  });
+  if (res != cudaSuccess) return res;
+  return launch_wgrad(B, H, W, Ma, a, Nw, 0, false, b, part, out_w, out_b, st);
+}
 
 cudaError_t launch_gnet_pack_train(const float* w0, const float* w1, const float* b1, const float* w2, const float* b2,
                                    const float* w3, const float* b3, int D, void* dst, cudaStream_t st) {

@@ -96,4 +96,87 @@ __device__ __forceinline__ void hidden_layer(float (&acc)[NTILE][4], const uint4
   }
 }
 
+// ---- training (DESIGN §3.10, §3.13) --------------------------------------------------------------------------------
+// The accumulator fragment of rows g, g+8 (pixels x, x+8 of one image row) into a (128, H, W) map: p points at channel
+// 2q of pixel x.  Pixel x+8 is only valid when x is.
+// The channel stride goes through an opaque copy: otherwise the compiler keeps the 32 channel addresses of one call
+// live for the next call, across a layer's MMAs, and spills.
+__device__ __forceinline__ int opaque(int v) {
+  int r;
+  asm volatile("mov.b32 %0, %1;" : "=r"(r) : "r"(v));
+  return r;
+}
+__device__ __forceinline__ void store_rows(float* __restrict__ p, const float (&acc)[NTILE][4], int HW, bool va, bool vb) {
+  HW = opaque(HW);
+#pragma unroll
+  for (int nt = 0; nt < NTILE; ++nt) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      float* c = p + (size_t)(nt * 8 + e) * HW;
+      if (va) c[0] = acc[nt][e];
+      if (vb) c[8] = acc[nt][2 + e];
+    }
+  }
+}
+
+// One layer of the backward chain on a gradient fragment of KT n8 tiles (any sign; KT even) into 128 channels: per-row
+// scale from max |x|, split, three products against resident transposed weights of KT/2 K steps, descale.  `in` is
+// read completely before `out` is written, so both may name one array.  The caller applies the ReLU mask.
+template <int KT>
+__device__ __forceinline__ void grad_layer(const float (&in)[KT][4], float (&out)[NTILE][4], const uint4* __restrict__ wsm,
+                                           int shw, int lane) {
+  float m0 = 0.0f, m1 = 0.0f;
+#pragma unroll
+  for (int nt = 0; nt < KT; ++nt) {
+    m0 = fmaxf(m0, fmaxf(fabsf(in[nt][0]), fabsf(in[nt][1])));
+    m1 = fmaxf(m1, fmaxf(fabsf(in[nt][2]), fabsf(in[nt][3])));
+  }
+#pragma unroll
+  for (int o = 1; o <= 2; o <<= 1) {
+    m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, o));
+    m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, o));
+  }
+  const int sh0 = split16_shift(__float_as_uint(m0)), sh1 = split16_shift(__float_as_uint(m1));
+  const float s0 = pow2(sh0), s1 = pow2(sh1);
+  uint32_t ah[KT / 2][4], al[KT / 2][4];
+#pragma unroll
+  for (int kk = 0; kk < KT / 2; ++kk) {
+    split2(__fmul_rn(in[2 * kk][0], s0), __fmul_rn(in[2 * kk][1], s0), ah[kk][0], al[kk][0]);
+    split2(__fmul_rn(in[2 * kk][2], s1), __fmul_rn(in[2 * kk][3], s1), ah[kk][1], al[kk][1]);
+    split2(__fmul_rn(in[2 * kk + 1][0], s0), __fmul_rn(in[2 * kk + 1][1], s0), ah[kk][2], al[kk][2]);
+    split2(__fmul_rn(in[2 * kk + 1][2], s1), __fmul_rn(in[2 * kk + 1][3], s1), ah[kk][3], al[kk][3]);
+  }
+#pragma unroll
+  for (int nt = 0; nt < NTILE; ++nt) out[nt][0] = out[nt][1] = out[nt][2] = out[nt][3] = 0.0f;
+#pragma unroll
+  for (int kk = 0; kk < KT / 2; ++kk) {
+#pragma unroll
+    for (int nt = 0; nt < NTILE; ++nt) mma3(out[nt], ah[kk], al[kk], wsm[(kk * NTILE + nt) * 32 + lane]);
+  }
+  const float dw = pow2(-shw), d0 = pow2(-sh0), d1 = pow2(-sh1);
+#pragma unroll
+  for (int nt = 0; nt < NTILE; ++nt) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      out[nt][e] = __fmul_rn(__fmul_rn(out[nt][e], d0), dw);
+      out[nt][2 + e] = __fmul_rn(__fmul_rn(out[nt][2 + e], d1), dw);
+    }
+  }
+}
+
+// ReLU backward on the fragment, as torch's threshold_backward: zero where the saved activation is <= 0 (a NaN
+// activation passes the gradient); h as store_rows addresses it
+__device__ __forceinline__ void relu_mask(float (&acc)[NTILE][4], const float* __restrict__ h, int HW, bool va, bool vb) {
+  HW = opaque(HW);
+#pragma unroll
+  for (int nt = 0; nt < NTILE; ++nt) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const float* c = h + (size_t)(nt * 8 + e) * HW;
+      acc[nt][e] = va && !(__ldg(c) <= 0.0f) ? acc[nt][e] : 0.0f;
+      acc[nt][2 + e] = vb && !(__ldg(c + 8) <= 0.0f) ? acc[nt][2 + e] : 0.0f;
+    }
+  }
+}
+
 }  // namespace magnet

@@ -7,8 +7,9 @@ cost-volume function itself is also available as a pure drop-in (``magnet_b200.h
 In inference the per-iteration G-Net head and update run as one fused kernel (``fused_gnet_applies``); with
 ``fused_train=True`` so do training iterations of the head (``fused_gnet_trains``, with a fused backward).  With
 ``fused_upsample=True``, inference runs the mask head after its first convolution and the upsampling of every
-prediction as one fused kernel too (``fused_mask_applies``).  Autocast, the hoisted x_d3 convolutions (G-Net's and the
-mask head's first layer) and the mask head of training stay ordinary ``nn.Module``s (cuDNN).
+prediction as one fused kernel too (``fused_mask_applies``), and ``MagnetHead.train_loss`` runs the same part of the
+mask head, the upsampling and the training loss as one differentiable fused op (``fused_mask_trains``).  Autocast and
+the hoisted x_d3 convolutions (G-Net's and the mask head's first layer) stay ordinary ``nn.Module``s (cuDNN).
 """
 from __future__ import annotations
 
@@ -265,7 +266,8 @@ def fused_mask_applies(mask_head, pre0: Optional[torch.Tensor], preds, k: int) -
     (``ops.mask_upsample``) instead of ``mask_head(x_d3)`` + ``convex_upsample`` per prediction: a mask head with the
     reference's structure and k == 4, nothing to differentiate (grad mode off, or no requires_grad among the mask
     head's parameters, pre0 and the predictions), no CUDA autocast, fp32 weights, pre0 and predictions.  pre0 may be
-    None when it is not computed yet.  The fused kernel has no backward."""
+    None when it is not computed yet.  The inference kernel has no backward; training takes the fused path of
+    ``fused_mask_trains``."""
     if int(k) != 4 or ops.mask_head_layers(mask_head) is None:
         return False
     params = list(mask_head.parameters())
@@ -275,6 +277,27 @@ def fused_mask_applies(mask_head, pre0: Optional[torch.Tensor], preds, k: int) -
         return False
     if torch.is_autocast_enabled("cuda"):
         return False
+    return all(p.dtype == torch.float32 for p in params) and all(t.dtype == torch.float32 for t in tensors)
+
+
+def fused_mask_trains(mask_head, pre0: Optional[torch.Tensor], preds, k: int, gt: Optional[torch.Tensor] = None) -> bool:
+    """Whether ``MagnetHead(fused_upsample=True).train_loss`` runs the differentiable fused mask head, upsampling and
+    loss (``ops.mask_head_loss``) instead of ``mask_head(x_d3)`` + ``magnet_loss``: a mask head with the reference's
+    structure and k == 4, grad mode on with something to differentiate (a mask-head parameter, pre0 or a prediction
+    requiring grad), 1 <= P <= MAGNET_MASK_MAX_PRED predictions, no CUDA autocast, fp32 weights, pre0, predictions and
+    gt.  pre0 and gt may be None when they are not known yet."""
+    if int(k) != 4 or ops.mask_head_layers(mask_head) is None:
+        return False
+    params = list(mask_head.parameters())
+    preds = [preds] if isinstance(preds, torch.Tensor) else list(preds)
+    if not 1 <= len(preds) <= _lib.MAGNET_MASK_MAX_PRED:
+        return False
+    tensors = preds + ([pre0] if pre0 is not None else [])
+    if not torch.is_grad_enabled() or not (any(p.requires_grad for p in params) or any(t.requires_grad for t in tensors)):
+        return False
+    if torch.is_autocast_enabled("cuda"):
+        return False
+    tensors += [gt] if gt is not None else []
     return all(p.dtype == torch.float32 for p in params) and all(t.dtype == torch.float32 for t in tensors)
 
 
@@ -289,7 +312,8 @@ class MagnetHead(nn.Module):
         super().__init__()
         self.n_iter, self.thres, self.downsample_ratio = n_iter, thres, downsample_ratio
         # True: forward runs the mask head after its first convolution and the upsampling of every prediction as one
-        # fused kernel where fused_mask_applies holds (inference); the full mask is then never computed
+        # fused kernel where fused_mask_applies holds (inference), and train_loss runs that part and the loss as one
+        # differentiable fused op where fused_mask_trains holds; the full mask is then never computed
         self.fused_upsample = fused_upsample
         # True: training iterations of the G-Net head run the differentiable fused kernels where fused_gnet_trains holds
         self.fused_train = fused_train
@@ -349,6 +373,25 @@ class MagnetHead(nn.Module):
         """MagnetLoss 'gaussian' (utils/losses.py:34-50) of the upsampled predictions without materialising them."""
         return ops.magnet_loss([p.float() for p in preds_quarter], mask.float(), gt_depth.float(), gt_depth_mask,
                                self.downsample_ratio, gamma)
+
+    def train_loss(self, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins, gt_depth,
+                   gt_depth_mask, gamma: float = 0.8):
+        """The scalar loss of one training step: ``loss(*forward_quarter(...), gt_depth, gt_depth_mask, gamma)``.  With
+        ``fused_upsample`` and ``fused_mask_trains`` holding, the mask head after ``mask_pre`` runs with the upsampling
+        and the loss as one differentiable fused op (``ops.mask_head_loss``): the 144-channel mask is never computed."""
+        k = self.downsample_ratio
+        if self.fused_upsample:
+            preds = self._predictions(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid,
+                                      cam_intrins)
+            if fused_mask_trains(self.mask_head, None, preds, k, gt_depth):
+                pre0 = self.mask_pre(x_d3)
+                if fused_mask_trains(self.mask_head, pre0, preds, k, gt_depth):
+                    return ops.mask_head_loss(pre0, self.mask_head, preds, gt_depth, gt_depth_mask, k, gamma)
+            mask = self.mask_head(x_d3).float()
+        else:
+            preds, mask = self.forward_quarter(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid,
+                                               cam_intrins)
+        return self.loss(preds, mask, gt_depth, gt_depth_mask, gamma)
 
 
 class MAGNET(nn.Module):

@@ -796,7 +796,8 @@ def mask_upsample(pre0: torch.Tensor, packed: torch.Tensor, preds, k: int = 4) -
     predictions: pre0 (B,128,H,W) = the first convolution's output before its ReLU (``MagnetHead.mask_pre``), packed =
     ``pack_mask_weights(mask_head)``, preds = quarter-resolution (B,2,H,W) [mu, sigma] tensors -> a list of
     (B,2,k*H,k*W) tensors, as ``convex_upsample(pred, mask_head(x_d3), k)`` gives them.  The 144-channel mask is never
-    written.  k = 4 only.  Not differentiable (forward only)."""
+    written.  k = 4 only.  Not differentiable (forward only): training runs the mask head, the upsampling and the
+    loss through ``mask_head_loss``, which has a backward."""
     preds = [preds] if isinstance(preds, torch.Tensor) else list(preds)
     if not preds:
         raise _lib.MagnetError("mask_upsample needs at least one prediction")
@@ -825,6 +826,129 @@ def mask_upsample(pre0: torch.Tensor, packed: torch.Tensor, preds, k: int = 4) -
                                       pred=C.cast(pp, C.POINTER(C.c_void_p)), out=C.cast(op, C.POINTER(C.c_void_p)))
             check(lib().magnet_mask_upsample_f32(C.byref(a), _stream(dev)), "magnet_mask_upsample_f32")
     return outs
+
+
+class MaskLossTrain(torch.autograd.Function):
+    """The mask head after its first convolution, the learned upsampling and MagnetLoss 'gaussian' (utils/losses.py:
+    34-50) of training in one forward kernel, differentiable in pre0, W1, b1, W2, b2, W3, b3 and every prediction
+    (DESIGN §3.13): the forward also forms the loss's gradient with respect to the 144 logits and the predictions while
+    they are on chip, so the mask is never written and is never read back per prediction (the logits' gradient is
+    written once, for the backward); the backward is one tensor-core chain
+    kernel and fixed-order weight-gradient GEMMs.  Inputs after b3: gt (B,1,4H,4W), the uint8 gt mask, k (4), gamma,
+    the number of supervised pixels, then the P predictions (B,2,H,W).  The weights are packed at every call.
+
+    Memory: the forward keeps h0, h1, h2 and the 144-channel gradient of the logits for the backward (528 channels per
+    pixel when a layer or pre0 needs a gradient; none otherwise) and the unit-scale prediction gradients (2 per
+    prediction); the backward adds d_h2 and d_h1 (256 channels).  The module path keeps about the same 528 channels
+    (the three hidden maps and the mask), so this is no memory saving."""
+
+    @staticmethod
+    def forward(ctx, pre0, w1, b1, w2, b2, w3, b3, gt, gt_mask_u8, k, gamma, count, *preds):
+        hid, nout = _lib.MAGNET_HIDDEN_CHANNELS, 9 * 4 * 4
+        P = len(preds)
+        if not 1 <= P <= _lib.MAGNET_MASK_MAX_PRED:
+            raise _lib.MagnetError(f"the fused mask-head loss takes 1 to {_lib.MAGNET_MASK_MAX_PRED} predictions, got {P}")
+        if int(k) != 4:
+            raise _lib.MagnetError(f"the fused mask head takes k = 4 only (144 mask channels), got {k}")
+        pre0 = _need_cuda_f32("pre0", pre0.detach())
+        if pre0.dim() != 4 or pre0.shape[1] != hid:
+            raise _lib.MagnetError(f"pre0 must be (B,{hid},H,W), got {tuple(pre0.shape)}")
+        B, _, H, W = pre0.shape
+        shapes = (("W1", w1, (hid, hid, 1, 1)), ("b1", b1, (hid,)), ("W2", w2, (hid, hid, 1, 1)), ("b2", b2, (hid,)),
+                  ("W3", w3, (nout, hid, 1, 1)), ("b3", b3, (nout,)))
+        ws = []
+        for nm, t, shp in shapes:
+            t = _need_cuda_f32(nm, t.detach())
+            _expect(nm, t, shp)
+            ws.append(t)
+        ps = []
+        for i, p in enumerate(preds):
+            p = _need_cuda_f32(f"preds[{i}]", p.detach())
+            _expect(f"preds[{i}]", p, (B, 2, H, W))
+            ps.append(p)
+        gt = _need_cuda_f32("gt", gt.detach())
+        _expect("gt", gt, (B, 1, 4 * H, 4 * W))
+        if gt_mask_u8.dtype != torch.uint8 or not gt_mask_u8.is_cuda or tuple(gt_mask_u8.shape) != (B, 1, 4 * H, 4 * W):
+            raise _lib.MagnetError("gt_mask must be a CUDA uint8 tensor of shape (B,1,4H,4W)")
+        gt_mask_u8 = gt_mask_u8.contiguous()
+        dev = _same_device(("pre0", pre0), ("gt", gt), ("gt_mask", gt_mask_u8),
+                           *((nm, t) for (nm, _, _), t in zip(shapes, ws)), *((f"preds[{i}]", p) for i, p in enumerate(ps)))
+        need = ctx.needs_input_grad
+        save_maps, pred_grad = any(need[:7]), any(need[12:])
+        gammas = [gamma ** (P - i - 1) for i in range(P)]
+        scale = (C.c_float * P)(*[g / float(count) for g in gammas])
+        pp = (C.c_void_p * P)(*[p.data_ptr() for p in ps])
+        packed = torch.empty(int(lib().magnet_mask_train_weights_bytes(4)), device=dev, dtype=torch.uint8)
+        partial = torch.empty(int(lib().magnet_mask_train_partials(B, H, W)) * P, device=dev, dtype=torch.float32)
+        # the prediction gradients come first in `saved`; the maps after them only when a layer gradient needs them
+        nsaved = int(lib().magnet_mask_saved_bytes(P, B, H, W)) // 4 if save_maps else 2 * P * B * H * W
+        saved = torch.empty(nsaved, device=dev, dtype=torch.float32)
+        a = _lib.MaskTrainArgs(P=P, B=B, H=H, W=W, k=4, pre0=pre0.data_ptr(), packed_weights=packed.data_ptr(),
+                               pred=C.cast(pp, C.POINTER(C.c_void_p)), gt=gt.data_ptr(), gt_mask=gt_mask_u8.data_ptr(),
+                               pred_scale=C.cast(scale, C.POINTER(C.c_float)), save_maps=int(save_maps),
+                               pred_grad=int(pred_grad), partial=partial.data_ptr(), saved=saved.data_ptr())
+        with torch.cuda.device(dev):
+            check(lib().magnet_mask_pack_train_weights_f32(*(t.data_ptr() for t in ws), packed.data_ptr(), _stream(dev)),
+                  "magnet_mask_pack_train_weights_f32")
+            check(lib().magnet_mask_train_fwd_f32(C.byref(a), _stream(dev)), "magnet_mask_train_fwd_f32")
+        ctx.save_for_backward(packed, saved)
+        ctx.shape = (P, B, H, W)
+        # as magnet_loss sums its terms: per prediction the float64 sum of the partials, in fp32 over count, weighted
+        terms = partial.view(-1, P).sum(0, dtype=torch.float64).to(torch.float32) / float(count)
+        loss = 0.0
+        for i in range(P):
+            loss = loss + gammas[i] * terms[i]
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad_loss):
+        packed, saved = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        P, B, H, W = ctx.shape
+        hid, nout = _lib.MAGNET_HIDDEN_CHANNELS, 9 * 4 * 4
+        dev = saved.device
+        new = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.float32)
+        g_pre0 = new(B, hid, H, W) if need[0] else None
+        g = [new(hid, hid, 1, 1) if need[1] else None, new(hid) if need[2] else None,
+             new(hid, hid, 1, 1) if need[3] else None, new(hid) if need[4] else None,
+             new(nout, hid, 1, 1) if need[5] else None, new(nout) if need[6] else None]
+        g_preds = [new(B, 2, H, W) if need[12 + i] else None for i in range(P)]
+        grad_scale = grad_loss.detach().to(device=dev, dtype=torch.float32).reshape(1).contiguous()
+        nws = int(lib().magnet_mask_bwd_workspace_bytes(B, H, W)) if any(need[:7]) else 256
+        ws = torch.empty(nws, device=dev, dtype=torch.uint8)
+        ptr = lambda t: None if t is None else t.data_ptr()
+        gp = (C.c_void_p * P)(*[ptr(t) for t in g_preds])
+        a = _lib.MaskTrainArgs(P=P, B=B, H=H, W=W, k=4, packed_weights=packed.data_ptr(), saved=saved.data_ptr(),
+                               grad_scale=grad_scale.data_ptr(), workspace=ws.data_ptr(), grad_pre0=ptr(g_pre0),
+                               grad_w1=ptr(g[0]), grad_b1=ptr(g[1]), grad_w2=ptr(g[2]), grad_b2=ptr(g[3]),
+                               grad_w3=ptr(g[4]), grad_b3=ptr(g[5]), grad_pred=C.cast(gp, C.POINTER(C.c_void_p)))
+        with torch.cuda.device(dev):
+            check(lib().magnet_mask_bwd_f32(C.byref(a), _stream(dev)), "magnet_mask_bwd_f32")
+        return (g_pre0, *g, None, None, None, None, None, *g_preds)
+
+
+def mask_head_loss(pre0, mask_head, preds, gt, gt_mask, k: int = 4, gamma: float = 0.8):
+    """MagnetLoss 'gaussian' of the predictions upsampled by the mask of ``mask_head``, from pre0 = the mask head's first
+    convolution before its ReLU (``MagnetHead.mask_pre``): ``magnet_loss(preds, mask_head(x_d3), gt, gt_mask, k, gamma)``
+    through ``MaskLossTrain``, differentiable in pre0, the last three layers' weights and biases and every prediction.
+    k = 4 and 1 to MAGNET_MASK_MAX_PRED predictions; gt_mask bool / uint8.  Validates like ``mask_upsample`` and
+    ``UpsampleNLL``; reads the number of supervised pixels with one host read, as ``magnet_loss``."""
+    convs = mask_head_layers(mask_head)
+    if convs is None:
+        raise _lib.MagnetError("not a mask head with the reference's structure (Conv(*,128,3), ReLU, Conv(128,128,1), "
+                               "ReLU, Conv(128,128,1), ReLU, Conv(128,144,1))")
+    preds = [preds] if isinstance(preds, torch.Tensor) else list(preds)
+    if not preds:
+        raise _lib.MagnetError("mask_head_loss needs at least one prediction")
+    if int(k) != 4:
+        raise _lib.MagnetError(f"the fused mask head takes k = 4 only (144 mask channels), got {k}")
+    gtm = gt_mask.to(torch.uint8)
+    count = int(gtm.sum().item())          # one host read per step, as magnet_loss
+    if count == 0:
+        raise _lib.MagnetError("gt_mask selects no pixel")
+    _, c1, c2, c3 = convs
+    return MaskLossTrain.apply(pre0, c1.weight, c1.bias, c2.weight, c2.bias, c3.weight, c3.bias, gt, gtm, 4, gamma,
+                               count, *preds)
 
 
 class UpsampleNLL(torch.autograd.Function):
