@@ -11,11 +11,12 @@ per-(batch, view) Python loop):
     cached across the N_iter calls of one forward (keyed by object identity + version counter);
   * ``R`` / ``t`` arrive as non-contiguous views of ``nghbr_poses`` (MAGNET.py:147-148): passed to
     ``magnet_pack_cameras_f32`` with their strides, no copy;
-  * ``nghbr_feat`` / ``nghbr_gmms`` / ``ref_feat`` arrive NCHW: split once per forward into the fp16 hi/lo planes the
-    tensor-core kernel's TMA boxes fetch (C == 64; else the pixel-major PIXC layout of the TMA-staged CUDA-core kernel;
-    cached the same way; bypassed under CUDA-graph capture).  fp16 / bf16 maps (torch.autocast) of one dtype go
-    to the single-plane HALF16 layout where SPLIT16 would be used; in every other case they are upcast to fp32
-    once (cached) and take the fp32 rules.  Volumes are fp32, gradients come back in each input's dtype.
+  * ``nghbr_feat`` / ``nghbr_gmms`` / ``ref_feat`` arrive NCHW: repacked once per forward (cached the same way;
+    bypassed under CUDA-graph capture) into the source layout ``route()`` picks for the call — the one rule shared
+    with ``MatchingPlan``: the fp16 hi/lo planes the tensor-core kernel's TMA boxes fetch (C == 64 and at least
+    MMA_MIN_PLANES hypotheses), or for fp16 / bf16 maps of one dtype (torch.autocast) their single-plane HALF16
+    form; else the pixel-major PIXC layout of the TMA-staged CUDA-core kernel, TILED32 or NCHW, read from fp32 maps
+    (half maps upcast once, cached).  Volumes are fp32, gradients come back in each input's dtype.
 Both volumes are differentiable as in the reference: the CW volume w.r.t. both feature maps and the depth volume
 (magnet_cost_volume_bwd_f32; built only when grad mode is on and one of them requires grad, so that G-Net training,
 where none does, runs exactly the no-grad path), the F volume w.r.t. both feature maps (magnet_cost_volume_f_bwd_f32)
@@ -129,80 +130,98 @@ def _camera_table(cam_intrins, R, t, is_valid, device):
 MMA_MIN_PLANES = 32   # below half a 64-hypothesis chunk the all-pairs GEMM is wasted: the gather kernel does only the needed taps
 
 
-def _wants_split16(C: int, V: int, variant: int, D: int) -> bool:
-    if variant == _lib.VARIANT_MMA:
-        return C == 64 and V <= 16
-    return variant == _lib.VARIANT_AUTO and C == 64 and V <= 16 and D >= MMA_MIN_PLANES
+def _tensor_cores(C: int, V: int, variant: int, D: int) -> bool:
+    return C == 64 and V <= 16 and (variant == _lib.VARIANT_MMA or (variant == _lib.VARIANT_AUTO and D >= MMA_MIN_PLANES))
 
 
 def wants_half16(ref_dtype, src_dtype, C: int, V: int, variant: int, D: int) -> bool:
-    """The dispatch rule of half-precision feature maps: the single-plane HALF16 layout when both maps have the same
-    half dtype and the SPLIT16 conditions hold; otherwise (False) both maps are upcast and today's fp32 rules apply."""
-    return ref_dtype == src_dtype and ref_dtype in ops.HALF_DTYPES and _wants_split16(C, V, variant, D)
+    """The half-precision part of ``route``: the single-plane HALF16 layout when the tensor-core kernel runs and both
+    feature maps have the same half dtype; otherwise (False) both maps are upcast and the fp32 layouts apply."""
+    return _tensor_cores(C, V, variant, D) and ref_dtype == src_dtype and ref_dtype in ops.HALF_DTYPES
+
+
+def route(C: int, V: int, D: int, variant: int, depth_mode: int, ref_dtype, src_dtype,
+          differentiable: bool = False) -> Tuple[int, int]:
+    """(source layout, kernel variant) of one cost-volume forward of C channels, V views and D hypotheses: the one rule
+    of ``est_costvolume_CW``, ``est_costvolume_F``, ``plane_sweep_f`` and ``MatchingPlan.cost``.
+
+    The tensor-core kernel (C == 64, V <= 16, and variant MMA, or AUTO with at least MMA_MIN_PLANES hypotheses) reads
+    HALF16 when both feature maps have the same half dtype, else SPLIT16; MMA is refused anywhere else.  Otherwise a
+    differentiable CW forward takes NCHW with the DIRECT kernel (the backward reproduces the consistency masks of these
+    two forwards only); a plain forward takes PIXC for the TMA-staged CUDA-core kernel (variant TMA, which is refused
+    where PIXC does not fit, or AUTO outside the fused sampler), else TILED32 for the global-gather kernels, or NCHW
+    when C is not a multiple of 4.  Every layout but HALF16 reads fp32 maps (half maps upcast once)."""
+    if differentiable:
+        if variant not in (_lib.VARIANT_AUTO, _lib.VARIANT_MMA, _lib.VARIANT_DIRECT):
+            raise _lib.MagnetError("a differentiable CW volume runs on the tensor-core or the DIRECT kernel (variant AUTO, "
+                                   f"MMA or DIRECT), got variant {variant}")
+        if C > 64:
+            raise _lib.MagnetError(f"the CW backward supports C <= 64 channels, got C={C}")
+    if _tensor_cores(C, V, variant, D):
+        return (_lib.SRC_HALF16 if wants_half16(ref_dtype, src_dtype, C, V, variant, D) else _lib.SRC_SPLIT16), variant
+    if variant == _lib.VARIANT_MMA:
+        raise _lib.MagnetError(f"MAGNET_VARIANT_MMA needs C == 64 and V <= 16, got C={C}, V={V}")
+    if differentiable:
+        return _lib.SRC_NCHW, _lib.VARIANT_DIRECT
+    pixc = C in (16, 32, 64) and V <= 16
+    if variant == _lib.VARIANT_TMA and not pixc:
+        raise _lib.MagnetError(f"MAGNET_VARIANT_TMA needs C in (16, 32, 64) and V <= 16, got C={C}, V={V}")
+    # AUTO: the fused sampler (DEPTH_GAUSS) stays on the global-gather kernel, which is faster than the TMA-staged one there
+    if pixc and (variant == _lib.VARIANT_TMA or (variant == _lib.VARIANT_AUTO and depth_mode != _lib.DEPTH_GAUSS)):
+        return _lib.SRC_PIXC, variant
+    return (_lib.SRC_TILED32 if C % 4 == 0 else _lib.SRC_NCHW), variant
+
+
+def differentiable_layout(C: int, V: int, D: int, variant: int, half: bool = False) -> int:
+    """The source layout ``route`` gives a differentiable CW forward, for feature maps of one half dtype (``half``) or
+    fp32: HALF16 / SPLIT16 on the tensor cores, else NCHW (read by the DIRECT kernel)."""
+    dtype = torch.float16 if half else torch.float32
+    return route(C, V, D, variant, _lib.DEPTH_VOLUME, dtype, dtype, differentiable=True)[0]
+
+
+def repack_source(layout: int, nghbr_feat, nghbr_gmms=None, ref_feat=None):
+    """(source maps in ``layout``, reference split or None): SPLIT16 / HALF16 (feature planes + Gaussian table, and with
+    ``ref_feat`` the reference features' planes, which the tensor-core kernels read in place of ``ref_feat``), PIXC
+    (features + Gaussians, pixel-major), TILED32 (features only) or the NCHW maps.  The maps are read as given: fp16 /
+    bf16 for HALF16, fp32 for every other layout."""
+    feat = nghbr_feat.detach()
+    if layout == _lib.SRC_NCHW:
+        return feat.contiguous(), None
+    if layout == _lib.SRC_TILED32:
+        return ops.repack_tiled32(feat), None
+    fn = {_lib.SRC_PIXC: ops.repack_pixc, _lib.SRC_SPLIT16: ops.repack_split16, _lib.SRC_HALF16: ops.repack_half16}[layout]
+    src = fn(feat, None if nghbr_gmms is None else nghbr_gmms.detach())
+    return src, (fn(ref_feat.detach()) if ref_feat is not None and layout in ops.PACKED_LAYOUTS else None)
+
+
+def _cached(kind, tensors, make):
+    hit = _cache.get(kind, tensors)
+    return hit if hit is not None else _cache.put(kind, tensors, make())
 
 
 def _f32(x):
     """x as an fp32 tensor: x itself when it is fp32 (the same object, so that caches keyed on it still hit), else a
     detached upcast cached on x (once per forward)."""
-    if x.dtype == torch.float32:
-        return x
-    hit = _cache.get("f32", (x,))
-    if hit is None:
-        hit = _cache.put("f32", (x,), x.detach().float())
-    return hit
+    return x if x.dtype == torch.float32 else _cached("f32", (x,), lambda: x.detach().float())
 
 
-def _wants_pixc(C: int, V: int, variant: int) -> bool:
-    return variant in (_lib.VARIANT_AUTO, _lib.VARIANT_TMA) and C in (16, 32, 64) and V <= 16
+_CACHE_KIND = {_lib.SRC_HALF16: "half16", _lib.SRC_SPLIT16: "split16", _lib.SRC_PIXC: "pixc", _lib.SRC_TILED32: "tiled32"}
 
 
-def _packed_source(nghbr_feat, nghbr_gmms, V, variant, ref_feat=None, D=MMA_MIN_PLANES):
-    """The source maps in the layout the selected kernel reads, repacked once per forward (cached on the caller's
-    tensor objects): SPLIT16 (fp16 hi/lo planes + Gaussian table, also of the reference features) for the tensor-core
-    production kernel (C == 64 and at least MMA_MIN_PLANES hypotheses), PIXC (features + Gaussians, pixel-major) for the TMA-staged CUDA-core kernel, TILED32 for the
-    global-gather kernels, NCHW when the channel count fits none.  Half-precision maps: HALF16 by ``wants_half16``,
-    else upcast.  Returns (source, layout, reference split or None)."""
-    C = nghbr_feat.shape[1]
-    if ref_feat is not None and wants_half16(ref_feat.dtype, nghbr_feat.dtype, C, V, variant, D):
-        src = (nghbr_feat,) if nghbr_gmms is None else (nghbr_feat, nghbr_gmms)
-        hit = _cache.get("half16", src)
-        if hit is None:
-            hit = _cache.put("half16", src, ops.repack_half16(nghbr_feat.detach(),
-                                                              None if nghbr_gmms is None else _f32(nghbr_gmms)))
-        ref = _cache.get("half16ref", (ref_feat,))
-        if ref is None:
-            ref = _cache.put("half16ref", (ref_feat,), ops.repack_half16(ref_feat.detach()))
-        return hit, _lib.SRC_HALF16, ref
-    nghbr_feat = _f32(nghbr_feat)
-    nghbr_gmms = None if nghbr_gmms is None else _f32(nghbr_gmms)
-    ref_feat = None if ref_feat is None else _f32(ref_feat)
-    if _wants_split16(C, V, variant, D) and ref_feat is not None:
-        src = (nghbr_feat,) if nghbr_gmms is None else (nghbr_feat, nghbr_gmms)
-        hit = _cache.get("split16", src)
-        if hit is None:
-            hit = _cache.put("split16", src, ops.repack_split16(nghbr_feat.detach(),
-                                                                None if nghbr_gmms is None else nghbr_gmms.detach()))
-        ref = _cache.get("split16ref", (ref_feat,))
-        if ref is None:
-            ref = _cache.put("split16ref", (ref_feat,), ops.repack_split16(ref_feat.detach()))
-        return hit, _lib.SRC_SPLIT16, ref
-    if variant == _lib.VARIANT_MMA:
-        raise _lib.MagnetError(f"MAGNET_VARIANT_MMA needs C == 64 and V <= 16, got C={C}, V={V}")
-    if _wants_pixc(C, V, variant):
-        src = (nghbr_feat,) if nghbr_gmms is None else (nghbr_feat, nghbr_gmms)
-        hit = _cache.get("pixc", src)
-        if hit is None:
-            hit = _cache.put("pixc", src, ops.repack_pixc(nghbr_feat.detach(),
-                                                          None if nghbr_gmms is None else nghbr_gmms.detach()))
-        return hit, _lib.SRC_PIXC, None
-    if variant == _lib.VARIANT_TMA:
-        raise _lib.MagnetError(f"MAGNET_VARIANT_TMA needs C in (16, 32, 64) and V <= 16, got C={C}, V={V}")
-    if C % 4 != 0:
-        return nghbr_feat.detach().contiguous(), _lib.SRC_NCHW, None
-    hit = _cache.get("tiled32", (nghbr_feat,))
-    if hit is None:
-        hit = _cache.put("tiled32", (nghbr_feat,), ops.repack_tiled32(nghbr_feat.detach()))
-    return hit, _lib.SRC_TILED32, None
+def _packed_source(layout, nghbr_feat, nghbr_gmms, ref_feat):
+    """``repack_source`` once per forward: the source maps and the reference split are each cached on the maps they are
+    made from, so a change of the reference features alone repacks only them.  Returns (source, reference split)."""
+    if layout != _lib.SRC_HALF16:
+        nghbr_feat, ref_feat = _f32(nghbr_feat), _f32(ref_feat)
+    if layout == _lib.SRC_NCHW:
+        return repack_source(layout, nghbr_feat)
+    gmms = None if nghbr_gmms is None or layout == _lib.SRC_TILED32 else _f32(nghbr_gmms)
+    kind = _CACHE_KIND[layout]
+    src = _cached(kind, (nghbr_feat,) if gmms is None else (nghbr_feat, gmms),
+                  lambda: repack_source(layout, nghbr_feat, gmms)[0])
+    if layout not in ops.PACKED_LAYOUTS:
+        return src, None
+    return src, _cached(kind + "ref", (ref_feat,), lambda: repack_source(layout, ref_feat)[0])
 
 
 _geometry_grad = [False]
@@ -274,9 +293,9 @@ class _CostVolumeCW(torch.autograd.Function):
     """Cost volume with per-pixel depths (d_volume, or the Gaussian + k of the fused sampler), differentiable in the
     depth source and both feature maps.  ``run()`` launches the forward kernel and returns (volume, layout, variant,
     (ref split, source split) or None): the backward (magnet_cost_volume_bwd_f32) reproduces that kernel's consistency
-    mask.  After a SPLIT16 forward the feature gradients run on the tensor cores on the same split buffers (the rule of
-    _PlaneSweepF), otherwise on the CUDA cores; the depth gradient always on the CUDA cores.  The source Gaussians get
-    no gradient (the mask is piecewise constant)."""
+    mask.  After a SPLIT16 / HALF16 forward the feature gradients run on the tensor cores on the same split buffers,
+    otherwise on the CUDA cores; the depth gradient always on the CUDA cores.  The source Gaussians get no gradient (the
+    mask is piecewise constant)."""
 
     @staticmethod
     def forward(ctx, depth, ref_feat, nghbr_feat, nghbr_gmms, run, spec, R=None, t=None, intM=None, rays=None):
@@ -316,22 +335,6 @@ class _CostVolumeCW(torch.autograd.Function):
         return (g_d, g_ref, g_src, None, None, None) + g_cam
 
 
-def differentiable_layout(C: int, V: int, D: int, variant: int, split16_ok: bool = True, half=False) -> int:
-    """Source layout of a differentiable CW forward: SPLIT16 (tensor cores) where the no-grad path would use it, else
-    NCHW with the DIRECT kernel — the two forward kernels whose consistency mask the backward reproduces.  ``half``:
-    both feature maps have one half dtype, so HALF16 replaces SPLIT16 (wants_half16)."""
-    if variant not in (_lib.VARIANT_AUTO, _lib.VARIANT_MMA, _lib.VARIANT_DIRECT):
-        raise _lib.MagnetError("a differentiable CW volume runs on the tensor-core or the DIRECT kernel (variant AUTO, MMA "
-                               f"or DIRECT), got variant {variant}")
-    if C > 64:
-        raise _lib.MagnetError(f"the CW backward supports C <= 64 channels, got C={C}")
-    if split16_ok and _wants_split16(C, V, variant, D):
-        return _lib.SRC_HALF16 if half else _lib.SRC_SPLIT16
-    if variant == _lib.VARIANT_MMA:
-        raise _lib.MagnetError(f"MAGNET_VARIANT_MMA needs C == 64 and V <= 16, got C={C}, V={V}")
-    return _lib.SRC_NCHW
-
-
 def est_costvolume_CW(d_volume, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms,
                       R, t, is_valid, cam_intrins, thres, variant=_lib.VARIANT_AUTO):
     """Consistency-weighted multi-view cost volume — drop-in for homography.est_costvolume_CW.
@@ -351,101 +354,59 @@ def est_costvolume_CW(d_volume, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms,
     if torch.is_grad_enabled() and not geometry_grad_enabled():
         check_geometry_grad(R=R, t=t, intM=cam_intrins['intM'], unit_ray_array_2D=cam_intrins['unit_ray_array_2D'])
     d_volume = d_volume.float()                            # differentiable upcast (a no-op for fp32)
-    if wants_cw_grad(d_volume, ref_feat, nghbr_feat) or wants_camera_grad(cam_in):
-        D, C = int(d_volume.shape[1]), int(ref_feat.shape[1])
-        half = wants_half16(ref_feat.dtype, nghbr_feat.dtype, C, V, variant, D)
-        layout = differentiable_layout(C, V, D, variant, half=half)
-        _, rays_d = _device_intrinsics(cam_intrins, device)
-        cams = _camera_table(cam_intrins, R, t, is_valid, device)
+    grad = wants_cw_grad(d_volume, ref_feat, nghbr_feat) or wants_camera_grad(cam_in)
+    layout, fv = route(int(ref_feat.shape[1]), V, int(d_volume.shape[1]), variant, _lib.DEPTH_VOLUME, ref_feat.dtype,
+                       nghbr_feat.dtype, differentiable=grad)
+    _, rays_d = _device_intrinsics(cam_intrins, device)
+    cams = _camera_table(cam_intrins, R, t, is_valid, device)
 
-        def run():
-            if layout in ops.PACKED_LAYOUTS:
-                src, _, ref_split = _packed_source(nghbr_feat, nghbr_gmms, V, variant, ref_feat, D)
-                fv = variant
-            else:
-                src, ref_split, fv = _f32(nghbr_feat).detach().contiguous(), None, _lib.VARIANT_DIRECT
-            ref = (ref_feat if layout == _lib.SRC_HALF16 else _f32(ref_feat)).detach()
-            out = ops.cost_volume(ref, src, rays_d, cams, V=V, src_layout=layout, consistency=True,
-                                  src_gmm=_f32(nghbr_gmms).detach(), kappa=float(thres), d_volume=d_volume.detach(),
-                                  variant=fv, ref_split=ref_split)
-            return out, layout, fv, (ref_split, src) if layout in ops.PACKED_LAYOUTS else None
+    def run():
+        src, ref_split = _packed_source(layout, nghbr_feat, nghbr_gmms, ref_feat)
+        ref = (ref_feat if layout == _lib.SRC_HALF16 else _f32(ref_feat)).detach()
+        out = ops.cost_volume(ref, src, rays_d, cams, V=V, src_layout=layout, consistency=True,
+                              src_gmm=_f32(nghbr_gmms).detach(), kappa=float(thres), d_volume=d_volume.detach(),
+                              variant=fv, ref_split=ref_split)
+        return out, layout, fv, (ref_split, src) if layout in ops.PACKED_LAYOUTS else None
 
+    if grad:
         return _CostVolumeCW.apply(d_volume, ref_feat, nghbr_feat, nghbr_gmms, run,
                                    (rays_d, cams, V, float(thres), None), *cam_in)
     with torch.no_grad():
-        _, rays_d = _device_intrinsics(cam_intrins, device)
-        cams = _camera_table(cam_intrins, R, t, is_valid, device)
-        src, layout, ref_split = _packed_source(nghbr_feat, nghbr_gmms, V, variant, ref_feat, int(d_volume.shape[1]))
-        ref = (ref_feat if layout == _lib.SRC_HALF16 else _f32(ref_feat)).detach()
-        return ops.cost_volume(ref, src, rays_d, cams, V=V, src_layout=layout, consistency=True,
-                               src_gmm=_f32(nghbr_gmms).detach(), kappa=float(thres), d_volume=d_volume.detach(),
-                               variant=variant, ref_split=ref_split)
+        return run()[0]
 
 
 def _plane_list(d_center):
     """The D plane depths as host floats.  ``d_center`` is a constant of the training run (train_FNet.py:56-66): the
     device -> host read happens once per tensor, not once per step."""
-    hit = _cache.get("planes", (d_center,))
-    if hit is None:
-        hit = _cache.put("planes", (d_center,), d_center.detach().reshape(-1).cpu().tolist())
-    return hit
+    return _cached("planes", (d_center,), lambda: d_center.detach().reshape(-1).cpu().tolist())
 
 
 class _CostVolumeF(torch.autograd.Function):
-    """Plane-sweep probability volume for F-Net training (homography.py:10-75), forward + backward kernels."""
+    """Plane-sweep volume (homography.py:10-75) — the probabilities (``softmax``) or the 1/V-averaged scores the fused
+    F-Net loss reads — differentiable in both feature maps.  With ``tc_bwd`` the backward runs on the tensor cores
+    after a SPLIT16 / HALF16 forward, on the forward's buffers; otherwise the CUDA-core kernel reads the fp32 NCHW
+    maps."""
 
     @staticmethod
-    def forward(ctx, ref_feat, nghbr_feat, planes, rays_d, cams, V, variant, R=None, t=None, intM=None, rays=None):
-        src, layout, ref_split = _packed_source(nghbr_feat, None, V, variant, ref_feat, len(planes))
+    def forward(ctx, ref_feat, nghbr_feat, planes, rays_d, cams, V, variant, softmax, tc_bwd,
+                R=None, t=None, intM=None, rays=None):
+        layout, fv = route(int(ref_feat.shape[1]), V, len(planes), variant, _lib.DEPTH_PLANES, ref_feat.dtype,
+                           nghbr_feat.dtype)
+        src, ref_split = _packed_source(layout, nghbr_feat, None, ref_feat)
         ref = (ref_feat if layout == _lib.SRC_HALF16 else _f32(ref_feat)).detach()
         out = ops.cost_volume(ref, src, rays_d, cams, V=V, src_layout=layout, consistency=False,
-                              k=planes, planes=True, softmax=True, variant=variant, ref_split=ref_split)
-        ctx.save_for_backward(ref_feat.detach(), nghbr_feat.detach(), out, rays_d, cams, *_detached(R, t, intM, rays))
-        ctx.planes, ctx.V = planes, V
-        return out
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        ref_feat, nghbr_feat, out, rays_d, cams, *cam_saved = ctx.saved_tensors
-        if not any(ctx.needs_input_grad[7:]):
-            g_ref, g_src = ops.cost_volume_f_bwd(ref_feat.float(), nghbr_feat.float(), rays_d, cams, ctx.planes, ctx.V,
-                                                 out, grad_out.contiguous(), softmax=True)
-            return g_ref.to(ref_feat.dtype), g_src.to(nghbr_feat.dtype), None, None, None, None, None, None, None, None, None
-        g_ref = g_src = None
-        if any(ctx.needs_input_grad[:2]):
-            g_ref, g_src = ops.cost_volume_f_bwd(ref_feat.float(), nghbr_feat.float(), rays_d, cams, ctx.planes, ctx.V,
-                                                 out, grad_out.contiguous(), softmax=True)
-            g_ref, g_src = g_ref.to(ref_feat.dtype), g_src.to(nghbr_feat.dtype)
-        g_cams, g_rays, _ = ops.cost_volume_geom_bwd(ref_feat.float(), nghbr_feat.float(), None, rays_d, cams,
-                                                     grad_out.contiguous(), V=ctx.V, k=ctx.planes, planes=True,
-                                                     softmax=True, prob=out, need_rays=ctx.needs_input_grad[10])
-        return (g_ref, g_src, None, None, None, None, None) + camera_grads(ctx, g_cams, g_rays, cam_saved)
-
-
-class _PlaneSweepF(torch.autograd.Function):
-    """Plane-sweep volume of ``MagnetF`` — the 1/V-averaged scores (``softmax=False``, what the fused F-Net loss reads)
-    or the probabilities — differentiable in both feature maps.  The backward runs on the tensor cores whenever the
-    forward read SPLIT16 buffers (C == 64, V <= 16, at least MMA_MIN_PLANES planes), on the same buffers; otherwise
-    the CUDA-core kernel reads the NCHW maps."""
-
-    @staticmethod
-    def forward(ctx, ref_feat, nghbr_feat, planes, rays_d, cams, V, softmax, R=None, t=None, intM=None, rays=None):
-        src, layout, ref_split = _packed_source(nghbr_feat, None, V, _lib.VARIANT_AUTO, ref_feat, len(planes))
-        ref = (ref_feat if layout == _lib.SRC_HALF16 else _f32(ref_feat)).detach()
-        out = ops.cost_volume(ref, src, rays_d, cams, V=V, src_layout=layout, consistency=False,
-                              k=planes, planes=True, softmax=softmax, ref_split=ref_split)
+                              k=planes, planes=True, softmax=softmax, variant=fv, ref_split=ref_split)
         ctx.save_for_backward(ref_feat.detach(), nghbr_feat.detach(), out if softmax else None, rays_d, cams,
                               *_detached(R, t, intM, rays))
-        ctx.splits = (ref_split, src) if layout in ops.PACKED_LAYOUTS else (None, None)
-        ctx.layout = layout
+        ctx.layout = layout if tc_bwd else _lib.SRC_NCHW   # what the feature gradients read
+        ctx.splits = (ref_split, src) if ctx.layout in ops.PACKED_LAYOUTS else (None, None)
         ctx.planes, ctx.V, ctx.softmax = planes, V, softmax
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
         ref_feat, nghbr_feat, out, rays_d, cams, *cam_saved = ctx.saved_tensors
-        ref_split, src_split = ctx.splits
-        need_cam = any(ctx.needs_input_grad[7:])
+        need_cam = any(ctx.needs_input_grad[9:])
         g_ref = g_src = None
         if not need_cam or any(ctx.needs_input_grad[:2]):
             if ctx.layout == _lib.SRC_HALF16:              # the NCHW maps only supply the shapes
@@ -453,48 +414,43 @@ class _PlaneSweepF(torch.autograd.Function):
             else:
                 ref, src = ref_feat.float(), nghbr_feat.float()
             g_ref, g_src = ops.cost_volume_f_bwd(ref, src, rays_d, cams, ctx.planes, ctx.V, out,
-                                                 grad_out.contiguous(), softmax=ctx.softmax, ref_split=ref_split,
-                                                 src_split=src_split, split_layout=ctx.layout)
+                                                 grad_out.contiguous(), softmax=ctx.softmax, ref_split=ctx.splits[0],
+                                                 src_split=ctx.splits[1], split_layout=ctx.layout)
             g_ref, g_src = g_ref.to(ref_feat.dtype), g_src.to(nghbr_feat.dtype)
-        if not need_cam:
-            return g_ref, g_src, None, None, None, None, None, None, None, None, None
-        g_cams, g_rays, _ = ops.cost_volume_geom_bwd(ref_feat.float(), nghbr_feat.float(), None, rays_d, cams,
-                                                     grad_out.contiguous(), V=ctx.V, k=ctx.planes, planes=True,
-                                                     softmax=ctx.softmax, prob=out, need_rays=ctx.needs_input_grad[10])
-        return (g_ref, g_src, None, None, None, None, None) + camera_grads(ctx, g_cams, g_rays, cam_saved)
+        g_cam = (None,) * 4
+        if need_cam:
+            g_cams, g_rays, _ = ops.cost_volume_geom_bwd(ref_feat.float(), nghbr_feat.float(), None, rays_d, cams,
+                                                         grad_out.contiguous(), V=ctx.V, k=ctx.planes, planes=True,
+                                                         softmax=ctx.softmax, prob=out,
+                                                         need_rays=ctx.needs_input_grad[12])
+            g_cam = camera_grads(ctx, g_cams, g_rays, cam_saved)
+        return (g_ref, g_src) + (None,) * 7 + g_cam
 
 
-def _f_camera_inputs(d_center, R, t, cam_intrins):
-    """The camera inputs of the F volume's autograd Functions: the caller's tensors under geometry_grad() (a d_center
-    that requires grad is refused there: the planes are host constants), else none, as before."""
-    if not geometry_grad_enabled():
-        return ()
-    if torch.is_grad_enabled() and isinstance(d_center, torch.Tensor) and d_center.requires_grad:
-        raise _lib.MagnetError("d_center requires grad, but the plane depths are constants of the F volume (detach it)")
-    return camera_inputs(R, t, cam_intrins)
+def _f_volume(d_center, ref_feat, nghbr_feat, R, t, is_valid, cam_intrins, variant, softmax, tc_bwd):
+    # the camera tensors take part only under geometry_grad(), where a d_center that requires grad is refused: the
+    # planes are host constants
+    cam_in = ()
+    if geometry_grad_enabled():
+        if torch.is_grad_enabled() and isinstance(d_center, torch.Tensor) and d_center.requires_grad:
+            raise _lib.MagnetError("d_center requires grad, but the plane depths are constants of the F volume (detach it)")
+        cam_in = camera_inputs(R, t, cam_intrins)
+    device = ref_feat.device
+    V = int(nghbr_feat.shape[0] / ref_feat.shape[0])
+    planes = _plane_list(d_center)
+    _, rays_d = _device_intrinsics(cam_intrins, device)
+    cams = _camera_table(cam_intrins, R, t, is_valid, device)
+    return _CostVolumeF.apply(ref_feat, nghbr_feat, planes, rays_d, cams, V, variant, softmax, tc_bwd, *cam_in)
 
 
 def plane_sweep_f(d_center, ref_feat, nghbr_feat, R, t, is_valid, cam_intrins, softmax=True):
     """The F volume of est_costvolume_F (softmax=True) or its 1/V-averaged scores (softmax=False), with the
     tensor-core backward where the forward ran on the tensor cores (MagnetF's path; est_costvolume_F keeps the
     CUDA-core backward)."""
-    cam_in = _f_camera_inputs(d_center, R, t, cam_intrins)
-    device = ref_feat.device
-    V = int(nghbr_feat.shape[0] / ref_feat.shape[0])
-    planes = _plane_list(d_center)
-    _, rays_d = _device_intrinsics(cam_intrins, device)
-    cams = _camera_table(cam_intrins, R, t, is_valid, device)
-    return _PlaneSweepF.apply(ref_feat, nghbr_feat, planes, rays_d, cams, V, softmax, *cam_in)
+    return _f_volume(d_center, ref_feat, nghbr_feat, R, t, is_valid, cam_intrins, _lib.VARIANT_AUTO, softmax, True)
 
 
 def est_costvolume_F(d_center, ref_feat, nghbr_feat, R, t, is_valid, cam_intrins, variant=_lib.VARIANT_AUTO):
     """Fronto-parallel plane-sweep volume with softmax over planes — drop-in (forward) for
     homography.est_costvolume_F.  d_center (1,D,1,1); the rest as in est_costvolume_CW."""
-    cam_in = _f_camera_inputs(d_center, R, t, cam_intrins)
-    device = ref_feat.device
-    B = ref_feat.shape[0]
-    V = int(nghbr_feat.shape[0] / B)
-    planes = _plane_list(d_center)
-    _, rays_d = _device_intrinsics(cam_intrins, device)
-    cams = _camera_table(cam_intrins, R, t, is_valid, device)
-    return _CostVolumeF.apply(ref_feat, nghbr_feat, planes, rays_d, cams, V, variant, *cam_in)
+    return _f_volume(d_center, ref_feat, nghbr_feat, R, t, is_valid, cam_intrins, variant, True, False)

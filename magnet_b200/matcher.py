@@ -3,7 +3,9 @@ the cost kernel and the Gaussian update as one kernel, prepared once per forward
 
 The reference inlines the sampler (MAGNET.py:154-156) and the update (inside GNET.forward, :60-69),
 so they are only reachable through this alternative loop (or the ``GNET`` mirror below); the
-cost-volume function itself is also available as a pure drop-in (``magnet_b200.homography``).
+cost-volume function itself is also available as a pure drop-in (``magnet_b200.homography``).  Both take the source
+layout and kernel of each call from ``homography.route``; under the default variant the fused sampler keeps the
+global-gather kernel where the drop-in takes the TMA-staged one.
 In inference the per-iteration G-Net head and update run as one fused kernel (``fused_gnet_applies``); with
 ``fused_train=True`` so do training iterations of the head (``fused_gnet_trains``, with a fused backward).  With
 ``fused_upsample=True``, inference runs the mask head after its first convolution and the upsampling of every
@@ -19,9 +21,9 @@ import torch
 import torch.nn as nn
 
 from . import _lib, ops
-from .homography import (MMA_MIN_PLANES, _CostVolumeCW, camera_inputs, check_geometry_grad, differentiable_layout,
-                         geometry_grad_enabled, wants_cw_grad)
-from .ops import HALF_DTYPES, PACKED_LAYOUTS
+from .homography import (_CostVolumeCW, camera_inputs, check_geometry_grad, geometry_grad_enabled, repack_source, route,
+                         wants_cw_grad)
+from .ops import PACKED_LAYOUTS
 from .sampling import depth_sampling
 
 
@@ -64,14 +66,15 @@ class GNET(nn.Module):
 
 class MatchingPlan:
     """Everything about one batch that does not change across the N_iter iterations, prepared once:
-    device intrinsics / rays, camera-constant table, source features in the gather layout.
+    device intrinsics / rays, camera-constant table, source features in the layouts ``cost()`` reads.
 
-    The feature maps may be fp16 / bf16 (torch.autocast).  Of one half dtype, they go to the single-plane HALF16
+    Each ``cost()`` call takes its source layout and kernel from ``homography.route`` (the drop-in's rule, except that
+    AUTO keeps the global-gather kernel where the drop-in would take the TMA-staged one); a layout is packed on first
+    use.  The feature maps may be fp16 / bf16 (torch.autocast): of one half dtype, they go to the single-plane HALF16
     layout wherever the fp32 maps would go to SPLIT16; every other layout reads their fp32 upcast (made once).  The
     Gaussians are upcast; volumes are fp32."""
 
-    def __init__(self, ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, *,
-                 thres: int = 5, src_layout: int = _lib.SRC_SPLIT16):
+    def __init__(self, ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, *, thres: int = 5):
         if torch.is_grad_enabled() and not geometry_grad_enabled():
             check_geometry_grad(nghbr_poses=nghbr_poses, intM=cam_intrins['intM'],
                                 unit_ray_array_2D=cam_intrins['unit_ray_array_2D'])
@@ -85,8 +88,6 @@ class MatchingPlan:
         self.kappa = float(thres)
         self.ref_feat = ref_feat.detach().contiguous()
         self.src_gmm = nghbr_gmms.detach().float().contiguous()
-        # the half dtype of both feature maps (tensor-core kernels on HALF16 buffers), or None (fp32 maps, or upcast)
-        self.half = ref_feat.dtype if ref_feat.dtype == nghbr_feat.dtype and ref_feat.dtype in HALF_DTYPES else None
         self._f32 = {}
         self.rays = cam_intrins['unit_ray_array_2D'].detach().to(dev, torch.float32).contiguous()
         intM = cam_intrins['intM'].detach().to(dev, torch.float32).contiguous()
@@ -96,17 +97,6 @@ class MatchingPlan:
         self._ref_in, self._src_in = ref_feat, nghbr_feat   # the caller's tensors: cost() is differentiable in them
         self._packed = {}
         self._ref_split = None
-        # Production: the tensor-core kernel on the fp16 hi/lo planes (C == 64 and at least half a chunk of hypotheses,
-        # decided per cost() call); otherwise the global-gather kernel (TILED32), which needs no staging window and
-        # no per-thread scratch.  Pass src_layout=SRC_PIXC / variant=VARIANT_TMA for the TMA-staged
-        # CUDA-core kernel.  Layouts are packed on first use.
-        if src_layout == _lib.SRC_SPLIT16 and not (self.C == 64 and self.V <= 16):
-            src_layout = _lib.SRC_TILED32
-        if src_layout == _lib.SRC_PIXC and not (self.C in (16, 32, 64) and self.V <= 16):
-            src_layout = _lib.SRC_TILED32
-        if src_layout == _lib.SRC_TILED32 and self.C % 4 != 0:
-            src_layout = _lib.SRC_NCHW
-        self.layout = src_layout
 
     def _fp32(self, which: str) -> torch.Tensor:
         """The reference ('ref') or source ('src') features in fp32: the plan's own when they are fp32, else their
@@ -118,28 +108,16 @@ class MatchingPlan:
             self._f32[which] = x.float()
         return self._f32[which]
 
-    def _tc_layout(self, layout: int) -> int:
-        """The tensor-core layout the plan's maps take: HALF16 for half maps of one dtype, else SPLIT16."""
-        return _lib.SRC_HALF16 if layout == _lib.SRC_SPLIT16 and self.half is not None else layout
-
     def _ref_operand(self, layout: int) -> torch.Tensor:
         return self.ref_feat if layout == _lib.SRC_HALF16 else self._fp32("ref")
 
     def _source(self, layout: int):
         """Source maps in ``layout`` (built on first use; the cross-check variants read other layouts than production)."""
         if layout not in self._packed:
-            if layout == _lib.SRC_PIXC:
-                self._packed[layout] = ops.repack_pixc(self._fp32("src"), self.src_gmm)
-            elif layout == _lib.SRC_SPLIT16:
-                self._packed[layout] = ops.repack_split16(self._fp32("src"), self.src_gmm)
-                self._ref_split = ops.repack_split16(self._fp32("ref"))
-            elif layout == _lib.SRC_HALF16:
-                self._packed[layout] = ops.repack_half16(self._nghbr_feat, self.src_gmm)
-                self._ref_split = ops.repack_half16(self.ref_feat)
-            elif layout == _lib.SRC_TILED32:
-                self._packed[layout] = ops.repack_tiled32(self._fp32("src"))
-            else:
-                self._packed[layout] = self._fp32("src").contiguous()
+            feat = self._nghbr_feat if layout == _lib.SRC_HALF16 else self._fp32("src")
+            self._packed[layout], ref_split = repack_source(layout, feat, self.src_gmm, self._ref_operand(layout))
+            if ref_split is not None:
+                self._ref_split = ref_split
         return self._packed[layout]
 
     def cost(self, gmm: torch.Tensor, k, out: Optional[torch.Tensor] = None, variant=_lib.VARIANT_AUTO):
@@ -147,44 +125,26 @@ class MatchingPlan:
         and in ``gmm`` when grad mode is on and one of them requires grad (then ``out`` must be None); detached
         otherwise."""
         gmm = gmm.float()                                  # differentiable upcast (a no-op for fp32)
-        if wants_cw_grad(gmm, self._ref_in, self._src_in, *self._cam_in):
-            return self._cost_differentiable(gmm, k, out, variant)
-        layout = self.layout
-        n_planes = len(k)
-        if layout == _lib.SRC_SPLIT16 and variant == _lib.VARIANT_AUTO and n_planes < MMA_MIN_PLANES:
-            layout = _lib.SRC_TILED32 if self.C % 4 == 0 else _lib.SRC_NCHW   # few hypotheses: the gather kernel is faster
-        if variant == _lib.VARIANT_TMA:
-            layout = _lib.SRC_PIXC                         # the TMA-staged kernel fetches its windows from PIXC
-        elif variant == _lib.VARIANT_MMA:
-            layout = _lib.SRC_SPLIT16                      # the tensor-core kernel reads the fp16 hi/lo planes
-        elif layout in (_lib.SRC_PIXC, _lib.SRC_SPLIT16) and variant in (_lib.VARIANT_DIRECT, _lib.VARIANT_CELLS, _lib.VARIANT_CELLS_NOREUSE):
-            layout = _lib.SRC_TILED32                      # the global-gather kernels read TILED32
-        layout = self._tc_layout(layout)
-        src = self._source(layout)
-        return ops.cost_volume(self._ref_operand(layout), src, self.rays, self.cams, V=self.V, src_layout=layout,
-                               consistency=True, src_gmm=self.src_gmm, kappa=self.kappa, ref_gmm=gmm.detach(),
-                               k=k, out=out, variant=variant,
-                               ref_split=self._ref_split if layout in PACKED_LAYOUTS else None)
-
-
-    def _cost_differentiable(self, gmm, k, out, variant):
-        if out is not None:
-            raise _lib.MagnetError("cost(out=...) writes into a caller buffer and cannot be differentiated")
-        karr = ops.k_array(k)
-        layout = differentiable_layout(self.C, self.V, len(karr), variant, split16_ok=self.layout == _lib.SRC_SPLIT16,
-                                       half=self.half is not None)
+        grad = wants_cw_grad(gmm, self._ref_in, self._src_in, *self._cam_in)
+        if grad:
+            if out is not None:
+                raise _lib.MagnetError("cost(out=...) writes into a caller buffer and cannot be differentiated")
+            k = ops.k_array(k)
+        layout, fv = route(self.C, self.V, len(k), variant, _lib.DEPTH_GAUSS, self.ref_feat.dtype,
+                           self._nghbr_feat.dtype, differentiable=grad)
 
         def run():
-            packed = layout in PACKED_LAYOUTS
-            fv = variant if packed else _lib.VARIANT_DIRECT
             src = self._source(layout)
+            packed = layout in PACKED_LAYOUTS
             vol = ops.cost_volume(self._ref_operand(layout), src, self.rays, self.cams, V=self.V, src_layout=layout,
                                   consistency=True, src_gmm=self.src_gmm, kappa=self.kappa, ref_gmm=gmm.detach(),
-                                  k=karr, variant=fv, ref_split=self._ref_split if packed else None)
+                                  k=k, out=out, variant=fv, ref_split=self._ref_split if packed else None)
             return vol, layout, fv, (self._ref_split, src) if packed else None
 
-        return _CostVolumeCW.apply(gmm, self._ref_in, self._src_in, self.src_gmm, run,
-                                   (self.rays, self.cams, self.V, self.kappa, karr), *self._cam_in)
+        if grad:
+            return _CostVolumeCW.apply(gmm, self._ref_in, self._src_in, self.src_gmm, run,
+                                       (self.rays, self.cams, self.V, self.kappa, k), *self._cam_in)
+        return run()[0]
 
 
 def matching_loop(plan: MatchingPlan, ref_gmms: torch.Tensor, x_d3: torch.Tensor,

@@ -6,6 +6,7 @@ Everything here requires CUDA tensors and the built library; nothing falls back 
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Optional, Sequence
 
 import torch
@@ -112,6 +113,27 @@ def pack_cameras(intM: torch.Tensor, R: torch.Tensor, t: torch.Tensor, is_valid:
     return cams
 
 
+def _repack_operands(x: torch.Tensor, gmm: Optional[torch.Tensor], out: Optional[torch.Tensor], shape,
+                     dtype=torch.uint8):
+    """The operands of a repack of x (N,C,H,W) besides x: the optional Gaussians (N,2,H,W), checked, and the output,
+    ``out`` if it holds a buffer of ``shape`` / ``dtype`` on x's device, else a new one.  Returns (gmm, out)."""
+    N, _, H, W = x.shape
+    if gmm is not None:
+        gmm = _need_cuda_f32("gmm", gmm)
+        if tuple(gmm.shape) != (N, 2, H, W):
+            raise _lib.MagnetError(f"gmm must be (N,2,H,W) = {(N, 2, H, W)}, got {tuple(gmm.shape)}")
+    if out is None:
+        return gmm, torch.empty(shape, device=x.device, dtype=dtype)
+    nbytes = math.prod(shape) * dtype.itemsize
+    if out.numel() * out.element_size() < nbytes or out.device != x.device:
+        raise _lib.MagnetError(f"out must hold {nbytes} bytes on {x.device}")
+    return gmm, out
+
+
+def _ptr(x: Optional[torch.Tensor]):
+    return None if x is None else x.data_ptr()
+
+
 def repack_tiled32(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """(N,C,H,W) -> TILED32 (N, H, ceil(W/32), C/4, 32, 4): the source-feature layout the tap-sharing
     kernel gathers from (channel quads of a pixel 512 B apart, 32 neighbouring pixels contiguous)."""
@@ -130,16 +152,9 @@ def repack_pixc(x: torch.Tensor, gmm: Optional[torch.Tensor] = None, out: Option
     (mu, sigma, 0, 0) — the layout the TMA-staged CUDA-core kernel fetches its windows from.  C in {16, 32, 64}."""
     x = _need_cuda_f32("x", x)
     N, Cc, H, W = x.shape
-    gptr = None
-    if gmm is not None:
-        gmm = _need_cuda_f32("gmm", gmm)
-        if tuple(gmm.shape) != (N, 2, H, W):
-            raise _lib.MagnetError(f"gmm must be (N,2,H,W) = {(N, 2, H, W)}, got {tuple(gmm.shape)}")
-        gptr = gmm.data_ptr()
-    if out is None:
-        out = torch.empty(N, H, W, Cc + 4, device=x.device, dtype=torch.float32)
+    gmm, out = _repack_operands(x, gmm, out, (N, H, W, Cc + 4), torch.float32)
     with torch.cuda.device(x.device):
-        check(lib().magnet_repack_pixc_f32(x.data_ptr(), gptr, out.data_ptr(), N, Cc, H, W, _stream(x.device)),
+        check(lib().magnet_repack_pixc_f32(x.data_ptr(), _ptr(gmm), out.data_ptr(), N, Cc, H, W, _stream(x.device)),
               "magnet_repack_pixc_f32")
     return out
 
@@ -150,19 +165,9 @@ def repack_split16(x: torch.Tensor, gmm: Optional[torch.Tensor] = None, out: Opt
     fetch (reference features: gmm=None)."""
     x = _need_cuda_f32("x", x)
     N, Cc, H, W = x.shape
-    gptr = None
-    if gmm is not None:
-        gmm = _need_cuda_f32("gmm", gmm)
-        if tuple(gmm.shape) != (N, 2, H, W):
-            raise _lib.MagnetError(f"gmm must be (N,2,H,W) = {(N, 2, H, W)}, got {tuple(gmm.shape)}")
-        gptr = gmm.data_ptr()
-    nbytes = int(lib().magnet_split16_bytes(N, H, W))
-    if out is None:
-        out = torch.empty(nbytes, device=x.device, dtype=torch.uint8)
-    elif out.numel() * out.element_size() < nbytes or out.device != x.device:
-        raise _lib.MagnetError(f"out must hold {nbytes} bytes on {x.device}")
+    gmm, out = _repack_operands(x, gmm, out, (int(lib().magnet_split16_bytes(N, H, W)),))
     with torch.cuda.device(x.device):
-        check(lib().magnet_repack_split16_f32(x.data_ptr(), gptr, out.data_ptr(), N, Cc, H, W, _stream(x.device)),
+        check(lib().magnet_repack_split16_f32(x.data_ptr(), _ptr(gmm), out.data_ptr(), N, Cc, H, W, _stream(x.device)),
               "magnet_repack_split16_f32")
     return out
 
@@ -181,20 +186,10 @@ def repack_half16(x: torch.Tensor, gmm: Optional[torch.Tensor] = None, out: Opti
         raise _lib.MagnetError(f"x must be (N,64,H,W), got {tuple(x.shape)}")
     x = x.contiguous()
     N, Cc, H, W = x.shape
-    gptr = None
-    if gmm is not None:
-        gmm = _need_cuda_f32("gmm", gmm)
-        if tuple(gmm.shape) != (N, 2, H, W):
-            raise _lib.MagnetError(f"gmm must be (N,2,H,W) = {(N, 2, H, W)}, got {tuple(gmm.shape)}")
-        gptr = gmm.data_ptr()
-    nbytes = int(lib().magnet_half16_bytes(N, H, W))
-    if out is None:
-        out = torch.empty(nbytes, device=x.device, dtype=torch.uint8)
-    elif out.numel() * out.element_size() < nbytes or out.device != x.device:
-        raise _lib.MagnetError(f"out must hold {nbytes} bytes on {x.device}")
+    gmm, out = _repack_operands(x, gmm, out, (int(lib().magnet_half16_bytes(N, H, W)),))
     _same_device(("x", x), ("gmm", gmm))
     with torch.cuda.device(x.device):
-        check(lib().magnet_repack_half16(x.data_ptr(), HALF_DTYPES[x.dtype], gptr, out.data_ptr(), N, Cc, H, W,
+        check(lib().magnet_repack_half16(x.data_ptr(), HALF_DTYPES[x.dtype], _ptr(gmm), out.data_ptr(), N, Cc, H, W,
                                          _stream(x.device)), "magnet_repack_half16")
     return out
 
@@ -213,6 +208,42 @@ def sample_depths(gmm: torch.Tensor, k, out: Optional[torch.Tensor] = None) -> t
     return out
 
 
+def _cost_args(ref_feat: torch.Tensor, V: int, rays, cams, *, d_volume=None, ref_gmm=None, k=None, planes=False):
+    """The CostArgs every cost-volume entry point shares, for ref_feat (B,C,H,W) and V views: ``rays`` and ``cams``
+    checked against (B, V, H, W), the shape fields filled, and the depth source — ``d_volume`` (B,D,H,W), or
+    ``ref_gmm`` (B,2,H,W) + ``k``, or ``k`` with ``planes=True``.  Returns (args, shape of the depth gradient or None
+    for the constant planes, the checked operands by name for the device check).  The args keep the buffers they
+    point into alive."""
+    rays = _need_cuda_f32("rays", rays)
+    cams = _need_cuda_f32("cams", cams)
+    B, Cc, H, W = ref_feat.shape
+    _expect("rays", rays, (B, 3, H * W))
+    if cams.numel() != B * V * 16:
+        raise _lib.MagnetError(f"cams must hold B*V = {B * V} camera records of 16 floats, got {tuple(cams.shape)}")
+    a = CostArgs()
+    a.B, a.V, a.C, a.H, a.W = B, V, Cc, H, W
+    a.rays, a.cams = rays.data_ptr(), cams.data_ptr()
+    karr = gd_shape = None
+    if d_volume is not None:
+        d_volume = _need_cuda_f32("d_volume", d_volume)
+        if d_volume.dim() != 4 or d_volume.shape[0] != B or tuple(d_volume.shape[2:]) != (H, W):
+            raise _lib.MagnetError(f"d_volume must be (B,D,H,W) = ({B},D,{H},{W}), got {tuple(d_volume.shape)}")
+        a.depth_mode, a.D, a.d_volume = _lib.DEPTH_VOLUME, d_volume.shape[1], d_volume.data_ptr()
+        gd_shape = tuple(d_volume.shape)
+    else:
+        karr = k if isinstance(k, C.Array) else k_array(k)
+        a.D, a.k_host = len(karr), C.cast(karr, C.c_void_p)
+        if planes:
+            a.depth_mode = _lib.DEPTH_PLANES
+        else:
+            ref_gmm = _need_cuda_f32("ref_gmm", ref_gmm)
+            _expect("ref_gmm", ref_gmm, (B, 2, H, W))
+            a.depth_mode, a.ref_gmm = _lib.DEPTH_GAUSS, ref_gmm.data_ptr()
+            gd_shape = (B, 2, H, W)
+    a._keep = (rays, cams, d_volume, ref_gmm, karr)
+    return a, gd_shape, (("rays", rays), ("cams", cams), ("d_volume", d_volume), ("ref_gmm", ref_gmm))
+
+
 def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tensor, cams: torch.Tensor, *,
                 V: int, src_layout: int, consistency: bool, src_gmm: Optional[torch.Tensor] = None,
                 kappa: float = 5.0, d_volume: Optional[torch.Tensor] = None,
@@ -226,8 +257,6 @@ def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tens
     ref_feat = _need_cuda("ref_feat", ref_feat) if src_layout == _lib.SRC_HALF16 else _need_cuda_f32("ref_feat", ref_feat)
     if src_layout not in PACKED_LAYOUTS:                   # the packed buffers are checked below, by their size
         src_feat = _need_cuda_f32("src_feat", src_feat)
-    rays = _need_cuda_f32("rays", rays)
-    cams = _need_cuda_f32("cams", cams)
     if ref_feat.dim() != 4:
         raise _lib.MagnetError(f"ref_feat must be (B,C,H,W), got {tuple(ref_feat.shape)}")
     B, Cc, H, W = ref_feat.shape
@@ -243,47 +272,20 @@ def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tens
         raise _lib.MagnetError(f"unknown src_layout {src_layout}")
     else:
         _expect("src_feat", src_feat, src_shape)
-    _expect("rays", rays, (B, 3, H * W))
-    if cams.numel() != B * V * 16:
-        raise _lib.MagnetError(f"cams must hold B*V = {B * V} camera records of 16 floats, got {tuple(cams.shape)}")
-    dev = _same_device(("ref_feat", ref_feat), ("src_feat", src_feat), ("rays", rays), ("cams", cams),
-                       ("src_gmm", src_gmm), ("d_volume", d_volume), ("ref_gmm", ref_gmm), ("out", out),
+    a, _, named = _cost_args(ref_feat, V, rays, cams, d_volume=d_volume, ref_gmm=ref_gmm, k=k, planes=planes)
+    dev = _same_device(("ref_feat", ref_feat), ("src_feat", src_feat), ("src_gmm", src_gmm), *named, ("out", out),
                        ("ref_split", ref_split))
-    a = CostArgs()
-    a.B, a.V, a.C, a.H, a.W = B, V, Cc, H, W
     a.src_layout = src_layout
     a.consistency = 1 if consistency else 0
     a.softmax = 1 if softmax else 0
     a.variant = variant
     a.kappa = float(kappa)
-    a.ref_feat, a.src_feat, a.rays, a.cams = ref_feat.data_ptr(), src_feat.data_ptr(), rays.data_ptr(), cams.data_ptr()
-    keep = [ref_feat, src_feat, rays, cams]
-    if src_layout in PACKED_LAYOUTS:
-        a.ref_feat = ref_split.data_ptr()
-        keep.append(ref_split)
+    a.ref_feat = ref_split.data_ptr() if src_layout in PACKED_LAYOUTS else ref_feat.data_ptr()
+    a.src_feat = src_feat.data_ptr()
     if consistency and src_layout not in (_lib.SRC_PIXC, *PACKED_LAYOUTS):   # those carry the source Gaussians inside src_feat
         src_gmm = _need_cuda_f32("src_gmm", src_gmm)
         _expect("src_gmm", src_gmm, (V * B, 2, H, W))
         a.src_gmm = src_gmm.data_ptr()
-        keep.append(src_gmm)
-    karr = None
-    if d_volume is not None:
-        d_volume = _need_cuda_f32("d_volume", d_volume)
-        if d_volume.dim() != 4 or d_volume.shape[0] != B or tuple(d_volume.shape[2:]) != (H, W):
-            raise _lib.MagnetError(f"d_volume must be (B,D,H,W) = ({B},D,{H},{W}), got {tuple(d_volume.shape)}")
-        a.depth_mode, a.D, a.d_volume = _lib.DEPTH_VOLUME, d_volume.shape[1], d_volume.data_ptr()
-        keep.append(d_volume)
-    else:
-        karr = k if isinstance(k, C.Array) else k_array(k)
-        a.D = len(karr)
-        a.k_host = C.cast(karr, C.c_void_p)
-        if planes:
-            a.depth_mode = _lib.DEPTH_PLANES
-        else:
-            ref_gmm = _need_cuda_f32("ref_gmm", ref_gmm)
-            _expect("ref_gmm", ref_gmm, (B, 2, H, W))
-            a.depth_mode, a.ref_gmm = _lib.DEPTH_GAUSS, ref_gmm.data_ptr()
-            keep.append(ref_gmm)
     if out is None:
         out = torch.empty(B, a.D, H, W, device=ref_feat.device, dtype=torch.float32)
     else:
@@ -310,32 +312,22 @@ def cost_volume_f_bwd(ref_feat, src_feat_nchw, rays, cams, planes, V, prob, grad
     shape_only = split and split_layout == _lib.SRC_HALF16
     ref_feat = _need_cuda("ref_feat", ref_feat) if shape_only else _need_cuda_f32("ref_feat", ref_feat)
     src = _need_cuda("src_feat", src_feat_nchw) if shape_only else _need_cuda_f32("src_feat", src_feat_nchw)
-    rays = _need_cuda_f32("rays", rays)
-    cams = _need_cuda_f32("cams", cams)
     grad_out = _need_cuda_f32("grad_out", grad_out)
     B, Cc, H, W = ref_feat.shape
-    karr = planes if isinstance(planes, C.Array) else k_array(planes)
     _expect("src_feat", src, (V * B, Cc, H, W))
-    _expect("rays", rays, (B, 3, H * W))
-    _expect("grad_out", grad_out, (B, len(karr), H, W))
+    a, _, named = _cost_args(ref_feat, V, rays, cams, k=planes, planes=True)
+    _expect("grad_out", grad_out, (B, a.D, H, W))
     if softmax:
         prob = _need_cuda_f32("prob", prob)
-        _expect("prob", prob, (B, len(karr), H, W))
-    if cams.numel() != B * V * 16:
-        raise _lib.MagnetError(f"cams must hold B*V = {B * V} camera records of 16 floats, got {tuple(cams.shape)}")
+        _expect("prob", prob, (B, a.D, H, W))
     if split:
         for nm, buf, n in (("src_split", src_split, V * B), ("ref_split", ref_split, B)):
             _check_packed(nm, buf, split_layout, n, H, W)
-    dev = _same_device(("ref_feat", ref_feat), ("src_feat", src), ("rays", rays), ("cams", cams),
-                       ("prob", prob if softmax else None), ("grad_out", grad_out), ("ref_split", ref_split),
-                       ("src_split", src_split))
-    a = CostArgs()
-    a.B, a.V, a.D, a.C, a.H, a.W = B, V, len(karr), Cc, H, W
-    a.depth_mode, a.consistency, a.softmax = _lib.DEPTH_PLANES, 0, 1 if softmax else 0
+    dev = _same_device(("ref_feat", ref_feat), ("src_feat", src), *named, ("prob", prob if softmax else None),
+                       ("grad_out", grad_out), ("ref_split", ref_split), ("src_split", src_split))
+    a.consistency, a.softmax = 0, 1 if softmax else 0
     a.src_layout = split_layout if split else _lib.SRC_NCHW
     a.ref_feat, a.src_feat = (ref_split.data_ptr(), src_split.data_ptr()) if split else (ref_feat.data_ptr(), src.data_ptr())
-    a.rays, a.cams = rays.data_ptr(), cams.data_ptr()
-    a.k_host = C.cast(karr, C.c_void_p)
     work = torch.empty_like(grad_out)
     g_ref = torch.empty(ref_feat.shape, device=ref_feat.device, dtype=torch.float32)
     g_src = torch.zeros(src.shape, device=src.device, dtype=torch.float32)
@@ -366,31 +358,11 @@ def cost_volume_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V: int
     shape_only = fwd_layout == _lib.SRC_HALF16 and not need_depth and (ref_split is not None or src_split is not None)
     ref_feat = _need_cuda("ref_feat", ref_feat) if shape_only else _need_cuda_f32("ref_feat", ref_feat)
     src = _need_cuda("src_feat", src_feat) if shape_only else _need_cuda_f32("src_feat", src_feat)
-    rays = _need_cuda_f32("rays", rays)
-    cams = _need_cuda_f32("cams", cams)
     grad_out = _need_cuda_f32("grad_out", grad_out)
     B, Cc, H, W = ref_feat.shape
     _expect("src_feat", src, (V * B, Cc, H, W))
-    _expect("rays", rays, (B, 3, H * W))
-    if cams.numel() != B * V * 16:
-        raise _lib.MagnetError(f"cams must hold B*V = {B * V} camera records of 16 floats, got {tuple(cams.shape)}")
-    a = CostArgs()
-    a.B, a.V, a.C, a.H, a.W = B, V, Cc, H, W
+    a, gd_shape, named = _cost_args(ref_feat, V, rays, cams, d_volume=d_volume, ref_gmm=ref_gmm, k=k)
     a.src_layout, a.variant, a.consistency, a.softmax, a.kappa = fwd_layout, fwd_variant, 1 if consistency else 0, 0, float(kappa)
-    a.rays, a.cams = rays.data_ptr(), cams.data_ptr()
-    karr = None
-    if d_volume is not None:
-        d_volume = _need_cuda_f32("d_volume", d_volume)
-        if d_volume.dim() != 4 or d_volume.shape[0] != B or tuple(d_volume.shape[2:]) != (H, W):
-            raise _lib.MagnetError(f"d_volume must be (B,D,H,W) = ({B},D,{H},{W}), got {tuple(d_volume.shape)}")
-        a.depth_mode, a.D, a.d_volume = _lib.DEPTH_VOLUME, d_volume.shape[1], d_volume.data_ptr()
-        gd_shape = tuple(d_volume.shape)
-    else:
-        karr = k if isinstance(k, C.Array) else k_array(k)
-        ref_gmm = _need_cuda_f32("ref_gmm", ref_gmm)
-        _expect("ref_gmm", ref_gmm, (B, 2, H, W))
-        a.depth_mode, a.D, a.ref_gmm, a.k_host = _lib.DEPTH_GAUSS, len(karr), ref_gmm.data_ptr(), C.cast(karr, C.c_void_p)
-        gd_shape = (B, 2, H, W)
     _expect("grad_out", grad_out, (B, a.D, H, W))
     if fwd_layout in PACKED_LAYOUTS and (ref_split is not None or src_split is not None):
         for nm, buf, nimg in (("src_split", src_split, V * B), ("ref_split", ref_split, B)):
@@ -405,16 +377,13 @@ def cost_volume_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V: int
         _expect("src_gmm", src_gmm, (V * B, 2, H, W))
         bw.src_gmm = src_gmm.data_ptr()
     dev = _same_device(("ref_feat", ref_feat), ("src_feat", src), ("src_gmm", src_gmm if consistency else None),
-                       ("rays", rays), ("cams", cams), ("grad_out", grad_out), ("d_volume", d_volume),
-                       ("ref_gmm", ref_gmm), ("ref_split", ref_split), ("src_split", src_split))
+                       *named, ("grad_out", grad_out), ("ref_split", ref_split), ("src_split", src_split))
     work = torch.empty_like(grad_out)
     g_ref = torch.empty(ref_feat.shape, device=dev, dtype=torch.float32) if need_ref else None
     g_src = torch.zeros(src.shape, device=dev, dtype=torch.float32) if need_src else None
     g_d = torch.empty(gd_shape, device=dev, dtype=torch.float32) if need_depth else None
     bw.grad_out, bw.workspace = grad_out.data_ptr(), work.data_ptr()
-    bw.grad_ref = g_ref.data_ptr() if need_ref else None
-    bw.grad_src = g_src.data_ptr() if need_src else None
-    bw.grad_depth = g_d.data_ptr() if need_depth else None
+    bw.grad_ref, bw.grad_src, bw.grad_depth = _ptr(g_ref), _ptr(g_src), _ptr(g_d)
     with torch.cuda.device(dev):
         check(lib().magnet_cost_volume_bwd_f32(C.byref(bw), _stream(dev)), "magnet_cost_volume_bwd_f32")
     return g_ref, g_src, g_d
@@ -435,37 +404,12 @@ def cost_volume_geom_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V
     then d/d(K t); grad_rays (B,3,H*W) or None; grad_depth or None), float32."""
     ref_feat = _need_cuda_f32("ref_feat", ref_feat)
     src = _need_cuda_f32("src_feat", src_feat)
-    rays = _need_cuda_f32("rays", rays)
-    cams = _need_cuda_f32("cams", cams)
     grad_out = _need_cuda_f32("grad_out", grad_out)
     B, Cc, H, W = ref_feat.shape
     _expect("src_feat", src, (V * B, Cc, H, W))
-    _expect("rays", rays, (B, 3, H * W))
-    if cams.numel() != B * V * 16:
-        raise _lib.MagnetError(f"cams must hold B*V = {B * V} camera records of 16 floats, got {tuple(cams.shape)}")
-    a = CostArgs()
-    a.B, a.V, a.C, a.H, a.W = B, V, Cc, H, W
+    a, gd_shape, named = _cost_args(ref_feat, V, rays, cams, d_volume=d_volume, ref_gmm=ref_gmm, k=k, planes=planes)
     a.src_layout, a.variant, a.kappa = fwd_layout, fwd_variant, float(kappa)
     a.consistency, a.softmax = 1 if consistency and not planes else 0, 1 if softmax else 0
-    a.rays, a.cams = rays.data_ptr(), cams.data_ptr()
-    karr = None
-    if d_volume is not None:
-        d_volume = _need_cuda_f32("d_volume", d_volume)
-        if d_volume.dim() != 4 or d_volume.shape[0] != B or tuple(d_volume.shape[2:]) != (H, W):
-            raise _lib.MagnetError(f"d_volume must be (B,D,H,W) = ({B},D,{H},{W}), got {tuple(d_volume.shape)}")
-        a.depth_mode, a.D, a.d_volume = _lib.DEPTH_VOLUME, d_volume.shape[1], d_volume.data_ptr()
-        gd_shape = tuple(d_volume.shape)
-    else:
-        karr = k if isinstance(k, C.Array) else k_array(k)
-        a.D, a.k_host = len(karr), C.cast(karr, C.c_void_p)
-        if planes:
-            a.depth_mode = _lib.DEPTH_PLANES
-            gd_shape = None
-        else:
-            ref_gmm = _need_cuda_f32("ref_gmm", ref_gmm)
-            _expect("ref_gmm", ref_gmm, (B, 2, H, W))
-            a.depth_mode, a.ref_gmm = _lib.DEPTH_GAUSS, ref_gmm.data_ptr()
-            gd_shape = (B, 2, H, W)
     if need_depth and gd_shape is None:
         raise _lib.MagnetError("the plane depths of the F volume are constants: no depth gradient")
     _expect("grad_out", grad_out, (B, a.D, H, W))
@@ -481,16 +425,14 @@ def cost_volume_geom_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V
         _expect("prob", prob, (B, a.D, H, W))
         bw.prob = prob.data_ptr()
     dev = _same_device(("ref_feat", ref_feat), ("src_feat", src), ("src_gmm", src_gmm if a.consistency else None),
-                       ("rays", rays), ("cams", cams), ("grad_out", grad_out), ("d_volume", d_volume),
-                       ("ref_gmm", ref_gmm), ("prob", prob if softmax else None))
+                       *named, ("grad_out", grad_out), ("prob", prob if softmax else None))
     score = torch.empty_like(grad_out)
     work = torch.empty(geom_workspace_bytes(B, V, H, W), device=dev, dtype=torch.uint8)
     g_cams = torch.empty(B * V, 12, device=dev, dtype=torch.float32)
     g_rays = torch.empty(B, 3, H * W, device=dev, dtype=torch.float32) if need_rays else None
     g_d = torch.empty(gd_shape, device=dev, dtype=torch.float32) if need_depth else None
     bw.score, bw.workspace, bw.grad_out, bw.grad_cams = score.data_ptr(), work.data_ptr(), grad_out.data_ptr(), g_cams.data_ptr()
-    bw.grad_rays = g_rays.data_ptr() if need_rays else None
-    bw.grad_depth = g_d.data_ptr() if need_depth else None
+    bw.grad_rays, bw.grad_depth = _ptr(g_rays), _ptr(g_d)
     with torch.cuda.device(dev):
         check(lib().magnet_cost_volume_geom_bwd_f32(C.byref(bw), _stream(dev)), "magnet_cost_volume_geom_bwd_f32")
     return g_cams, g_rays, g_d

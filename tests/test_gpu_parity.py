@@ -9,6 +9,7 @@ import torch
 
 import magnet_b200
 from magnet_b200 import _lib, ops
+from magnet_b200.homography import route
 from magnet_b200.synthetic import make_config, make_inputs
 from oracle import magnet_oracle as mo
 from tests import kat
@@ -121,7 +122,7 @@ def test_tma_kernel_fuzz_against_direct_kernel(cuda):
     print("fuzz: worst fraction of threshold-adjacent elements", worst)
 
 
-def test_mma_kernel_fuzz_against_direct_kernel(cuda):
+def test_mma_kernel_fuzz_against_direct_kernel_on_routed_layout(cuda):
     """Randomised shapes / poses for the tensor-core kernel against the reference-order direct kernel (both depth modes):
     ragged tiles, 1..6 views with invalid ones, 1..150 planes (partial and multiple 64-hypothesis chunks), large baselines
     and random depths (windows beyond 256 cells -> sub-windows), both camera families, feature scales from 1e-3 to 1e3
@@ -143,8 +144,9 @@ def test_mma_kernel_fuzz_against_direct_kernel(cuda):
         g = inp.to(cuda)
         plan = magnet_b200.MatchingPlan(g.ref_feat, g.nghbr_feat, g.nghbr_gmms, g.nghbr_poses, inp.is_valid,
                                         inp.cam_intrins, thres=inp.thres)
-        assert plan.layout == _lib.SRC_SPLIT16
         k = inp.k.tolist()
+        assert route(plan.C, plan.V, len(k), _lib.VARIANT_MMA, _lib.DEPTH_GAUSS, g.ref_feat.dtype,
+                     g.nghbr_feat.dtype)[0] == _lib.SRC_SPLIT16
         want = plan.cost(g.ref_gmms, k, variant=_lib.VARIANT_DIRECT)
         dvol = ops.sample_depths(g.ref_gmms, k)
         for mode, got in (("fused", plan.cost(g.ref_gmms, k, variant=_lib.VARIANT_MMA)),

@@ -6,7 +6,7 @@ import pytest
 import torch
 
 from magnet_b200 import _lib
-from magnet_b200.homography import MMA_MIN_PLANES, differentiable_layout, wants_half16
+from magnet_b200.homography import MMA_MIN_PLANES, differentiable_layout, route, wants_half16
 
 F16, BF16, F32 = torch.float16, torch.bfloat16, torch.float32
 
@@ -28,13 +28,19 @@ F16, BF16, F32 = torch.float16, torch.bfloat16, torch.float32
 ])
 def test_dispatch_rule(ref, src, C_, V, D, variant, want):
     assert wants_half16(ref, src, C_, V, variant, D) is want
+    layout, kernel = route(C_, V, D, variant, _lib.DEPTH_VOLUME, ref, src)
+    assert (layout == _lib.SRC_HALF16) is want and kernel == variant
 
 
-def test_differentiable_layout_with_half_maps():
+def test_route_differentiable_layout_with_half_maps():
+    def layout(D, dtype):
+        return route(64, 2, D, _lib.VARIANT_AUTO, _lib.DEPTH_VOLUME, dtype, dtype, differentiable=True)
+    assert layout(64, F16) == (_lib.SRC_HALF16, _lib.VARIANT_AUTO)
+    assert layout(64, F32) == (_lib.SRC_SPLIT16, _lib.VARIANT_AUTO)
+    assert layout(5, F16) == (_lib.SRC_NCHW, _lib.VARIANT_DIRECT)
     assert differentiable_layout(64, 2, 64, _lib.VARIANT_AUTO, half=True) == _lib.SRC_HALF16
     assert differentiable_layout(64, 2, 64, _lib.VARIANT_AUTO, half=False) == _lib.SRC_SPLIT16
     assert differentiable_layout(64, 2, 5, _lib.VARIANT_AUTO, half=True) == _lib.SRC_NCHW
-    assert differentiable_layout(64, 2, 64, _lib.VARIANT_AUTO, split16_ok=False, half=True) == _lib.SRC_NCHW
 
 
 def test_constants_and_bytes_formula():

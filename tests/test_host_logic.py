@@ -182,7 +182,7 @@ def test_product_never_imports_the_oracle():
             assert not re.search(r"^\s*(from|import)\s+oracle\b", open(os.path.join(ROOT, f)).read(), re.M), f
 
 
-def test_packed_source_cache_hits_on_the_callers_tensor(monkeypatch):
+def test_drop_in_repack_cache_hits_on_the_callers_tensor(monkeypatch):
     """ADVICE r1 (medium): the repack must be keyed on the tensor object the caller passes — a `.detach()` temporary dies
     before the next call and made every est_costvolume_CW call repack (157 MB at config 2).  Counted with mocked ops."""
     from magnet_b200 import homography as hg, ops
@@ -204,34 +204,37 @@ def test_packed_source_cache_hits_on_the_callers_tensor(monkeypatch):
     monkeypatch.setattr(ops, "repack_tiled32", fake_tiled)
     monkeypatch.setattr(ops, "repack_split16", fake_split)
     hg.clear_cache()
-    feat, gmm = torch.zeros(4, 16, 3, 5), torch.zeros(4, 2, 3, 5)
+
+    def packed(feat, gmm, variant, ref, D=5):
+        layout, _ = hg.route(feat.shape[1], 2, D, variant, _lib.DEPTH_VOLUME, ref.dtype, feat.dtype)
+        return (layout,) + hg._packed_source(layout, feat, gmm, ref)
+
+    feat, gmm, ref = torch.zeros(4, 16, 3, 5), torch.zeros(4, 2, 3, 5), torch.zeros(2, 16, 3, 5)
     for _ in range(3):                                       # the N_iter calls of one forward
-        _, layout, _ = hg._packed_source(feat, gmm, 2, _lib.VARIANT_AUTO)
-        assert layout == _lib.SRC_PIXC
+        assert packed(feat, gmm, _lib.VARIANT_AUTO, ref)[0] == _lib.SRC_PIXC
     assert calls["pixc"] == 1
     feat.add_(1.0)                                           # next forward writes new features in place
-    hg._packed_source(feat, gmm, 2, _lib.VARIANT_AUTO)
+    packed(feat, gmm, _lib.VARIANT_AUTO, ref)
     assert calls["pixc"] == 2
     for _ in range(2):                                       # cross-check variants read TILED32, cached separately
-        _, layout, _ = hg._packed_source(feat, gmm, 2, _lib.VARIANT_CELLS)
-        assert layout == _lib.SRC_TILED32
+        assert packed(feat, gmm, _lib.VARIANT_CELLS, ref)[0] == _lib.SRC_TILED32
     assert calls["tiled"] == 1
     # C == 64: the tensor-core kernel's fp16 hi/lo planes, source views and reference features split once per forward
     feat64, ref64 = torch.zeros(4, 64, 3, 5), torch.zeros(2, 64, 3, 5)
     for _ in range(3):
-        _, layout, ref_split = hg._packed_source(feat64, gmm, 2, _lib.VARIANT_AUTO, ref64, 64)
+        layout, _, ref_split = packed(feat64, gmm, _lib.VARIANT_AUTO, ref64, 64)
         assert layout == _lib.SRC_SPLIT16 and ref_split is not None
     assert calls["split"] == 2
-    assert hg._packed_source(feat64, gmm, 2, _lib.VARIANT_AUTO, ref64, 5)[1] == _lib.SRC_PIXC   # N_s = 5: CUDA-core kernel
+    assert packed(feat64, gmm, _lib.VARIANT_AUTO, ref64, 5)[0] == _lib.SRC_PIXC   # N_s = 5: CUDA-core kernel
     ref64.add_(1.0)
-    hg._packed_source(feat64, gmm, 2, _lib.VARIANT_AUTO, ref64, 64)
+    packed(feat64, gmm, _lib.VARIANT_AUTO, ref64, 64)
     assert calls["split"] == 3                               # only the reference features changed
     hg.prep_cache(False)
-    hg._packed_source(feat, gmm, 2, _lib.VARIANT_AUTO)
-    hg._packed_source(feat, gmm, 2, _lib.VARIANT_AUTO)
+    packed(feat, gmm, _lib.VARIANT_AUTO, ref)
+    packed(feat, gmm, _lib.VARIANT_AUTO, ref)
     assert calls["pixc"] == 5                                # disabled: every call repacks
     hg.prep_cache(True)
-    _, layout, _ = hg._packed_source(torch.zeros(4, 20, 3, 5), None, 2, _lib.VARIANT_AUTO)
+    layout = packed(torch.zeros(4, 20, 3, 5), None, _lib.VARIANT_AUTO, torch.zeros(2, 20, 3, 5))[0]
     assert layout == _lib.SRC_TILED32                        # C = 20: not a PIXC channel count
     hg.clear_cache()
 
