@@ -553,6 +553,41 @@ typedef struct magnet_depth_metrics_args {
 int64_t magnet_depth_metrics_workspace(const magnet_depth_metrics_args* args);
 int magnet_depth_metrics_f32(const magnet_depth_metrics_args* args, void* stream);
 
+/*
+ * F-Net depth map — the soft-argmin prediction of train_FNet.py:96 / :180, sum_j prob_j * planes_host[j], without the
+ * probability volume.  volume (B,D,H,W); planes_host: HOST pointer, D floats; out (B,1,H,W).
+ *   scores != 0: volume holds the 1/V-averaged scores of magnet_cost_volume_f32 with softmax == 0 (depth_mode
+ *     MAGNET_DEPTH_PLANES); the softmax over the planes is fused in, with the same code as magnet_fnet_l1_fwd_f32, so
+ *     the prediction is bit for bit the one the training loss supervises.
+ *   scores == 0: volume holds the probabilities (the output of est_costvolume_F / MAGNET_F.forward).
+ * A row with a NaN or an infinite maximum gives NaN, as torch.softmax does.  One kernel.
+ * D outside 1..MAGNET_MAX_PLANES: D <= 0 -> MAGNET_ERR_SHAPE, D > MAGNET_MAX_PLANES -> MAGNET_ERR_UNSUPPORTED.
+ */
+int magnet_plane_depth_f32(const float* volume, const float* planes_host, int32_t B, int32_t D, int32_t H, int32_t W,
+                           int32_t scores, float* out, void* stream);
+
+/*
+ * Depth evaluation of F-Net — replaces the metric block of train_FNet.py validate() (:165-193): the (B,1,h,w)
+ * predictions are upsampled to the GT size with F.interpolate(..., size=(H, W), mode='nearest') inside the kernel,
+ * source row min(floor(Y * (float)h / H), h - 1) in float32 (likewise for columns), any h <= H and w <= W.  Masking,
+ * per-pixel terms and sums as magnet_depth_metrics_f32.  There is no variance: the nll column is 0.0 for every image,
+ * also one without a valid pixel (compute_depth_errors(..., var=None)), while the other columns are NaN there.
+ * out (P,B,MAGNET_METRICS_COLS) float64 as magnet_depth_metrics_f32.  Two kernels, no atomics.
+ */
+typedef struct magnet_depth_metrics_nearest_args {
+  int32_t P, B, H, W;             /* predictions (1..MAGNET_METRICS_MAX_PRED), images, full-resolution GT size      */
+  int32_t h, w;                   /* prediction grid, 1 <= h <= H, 1 <= w <= W                                      */
+  int32_t row0, row1, col0, col1; /* evaluation box [row0,row1) x [col0,col1) of the GT (no crop: 0, H, 0, W)      */
+  float min_depth, max_depth;     /* compared in float32                                                            */
+  const float* const* pred;       /* HOST array of P DEVICE pointers, each (B,1,h,w)                                */
+  const float* gt;                /* (B,1,H,W) raw GT (values above max_depth are treated as 0)                     */
+  double* workspace;              /* magnet_depth_metrics_nearest_workspace(args) doubles of scratch                */
+  double* out;                    /* (P,B,MAGNET_METRICS_COLS)                                                      */
+} magnet_depth_metrics_nearest_args;
+/* Doubles of workspace the call needs (shape fields and box of args only), or a negative magnet_status. */
+int64_t magnet_depth_metrics_nearest_workspace(const magnet_depth_metrics_nearest_args* args);
+int magnet_depth_metrics_nearest_f32(const magnet_depth_metrics_nearest_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

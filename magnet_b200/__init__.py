@@ -10,11 +10,11 @@ from .sampling import depth_sampling, k_offsets_f32
 from .homography import est_costvolume_CW, est_costvolume_F, clear_cache, geometry_grad, prep_cache
 from .matcher import GNET, MAGNET, MagnetF, MagnetHead, MatchingPlan, matching_loop, install, sid_planes
 from .metrics import DepthMetrics
-from .ops import depth_metrics
+from .ops import depth_metrics, plane_depth
 
 __all__ = [
     "depth_sampling", "k_offsets_f32", "est_costvolume_CW", "est_costvolume_F", "clear_cache", "prep_cache",
     "geometry_grad",
     "GNET", "MAGNET", "MagnetF", "MagnetHead", "MatchingPlan", "matching_loop", "install", "sid_planes",
-    "DepthMetrics", "depth_metrics",
+    "DepthMetrics", "depth_metrics", "plane_depth",
 ]

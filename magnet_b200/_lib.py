@@ -38,6 +38,7 @@ EXPORTS = (
     "magnet_upsample_nll_partials", "magnet_upsample_nll_fwd_f32", "magnet_upsample_nll_bwd_f32",
     "magnet_fnet_l1_partials", "magnet_fnet_l1_fwd_f32", "magnet_fnet_l1_bwd_f32",
     "magnet_depth_metrics_workspace", "magnet_depth_metrics_f32",
+    "magnet_plane_depth_f32", "magnet_depth_metrics_nearest_workspace", "magnet_depth_metrics_nearest_f32",
     "magnet_gnet_weights_bytes", "magnet_gnet_pack_weights_f32", "magnet_gnet_update_f32",
     "magnet_gnet_train_weights_bytes", "magnet_gnet_saved_bytes", "magnet_gnet_bwd_workspace_bytes",
     "magnet_gnet_pack_train_weights_f32", "magnet_gnet_train_fwd_f32", "magnet_gnet_bwd_f32",
@@ -91,6 +92,14 @@ class DepthMetricsArgs(C.Structure):
                 ("min_depth", C.c_float), ("max_depth", C.c_float),
                 ("pred", C.POINTER(C.c_void_p)), ("up_mask", C.c_void_p), ("gt", C.c_void_p), ("workspace", C.c_void_p),
                 ("out", C.c_void_p)]
+
+
+class DepthMetricsNearestArgs(C.Structure):
+    """Mirror of ``struct magnet_depth_metrics_nearest_args``."""
+    _fields_ = [("P", C.c_int32), ("B", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("h", C.c_int32),
+                ("w", C.c_int32), ("row0", C.c_int32), ("row1", C.c_int32), ("col0", C.c_int32), ("col1", C.c_int32),
+                ("min_depth", C.c_float), ("max_depth", C.c_float),
+                ("pred", C.POINTER(C.c_void_p)), ("gt", C.c_void_p), ("workspace", C.c_void_p), ("out", C.c_void_p)]
 
 
 class GnetArgs(C.Structure):
@@ -214,6 +223,12 @@ def lib() -> C.CDLL:
     L.magnet_depth_metrics_workspace.argtypes = [C.POINTER(DepthMetricsArgs)]
     L.magnet_depth_metrics_f32.restype = C.c_int
     L.magnet_depth_metrics_f32.argtypes = [C.POINTER(DepthMetricsArgs), C.c_void_p]
+    L.magnet_plane_depth_f32.restype = C.c_int
+    L.magnet_plane_depth_f32.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p, C.c_void_p]
+    L.magnet_depth_metrics_nearest_workspace.restype = C.c_int64
+    L.magnet_depth_metrics_nearest_workspace.argtypes = [C.POINTER(DepthMetricsNearestArgs)]
+    L.magnet_depth_metrics_nearest_f32.restype = C.c_int
+    L.magnet_depth_metrics_nearest_f32.argtypes = [C.POINTER(DepthMetricsNearestArgs), C.c_void_p]
     L.magnet_gnet_weights_bytes.restype = C.c_size_t
     L.magnet_gnet_weights_bytes.argtypes = [C.c_int32]
     L.magnet_gnet_pack_weights_f32.restype = C.c_int

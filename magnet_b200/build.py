@@ -18,9 +18,9 @@ CSRC = PKG / "csrc"
 BUILD = PKG / "_build"
 LIB = PKG / "libmagnet_b200.so"
 SOURCES = ["api.cu", "cost_mma.cu", "cost_tma.cu", "cost_cells.cu", "cost_direct.cu", "cost_f_bwd.cu", "cost_f_bwd_mma.cu", "cost_cw_bwd.cu", "fnet_l1.cu",
-           "aux_kernels.cu", "depth_metrics.cu", "gnet_head.cu", "mask_head.cu"]
+           "plane_depth.cu", "aux_kernels.cu", "depth_metrics.cu", "gnet_head.cu", "mask_head.cu"]
 HEADERS = [CSRC / "common.cuh", CSRC / "cells_common.cuh", CSRC / "tma_common.cuh", CSRC / "cw_mask.cuh",
-           CSRC / "upsample_common.cuh", CSRC / "gaussian_common.cuh", CSRC / "head_common.cuh", PKG.parent / "include" / "magnet_b200.h"]
+           CSRC / "upsample_common.cuh", CSRC / "gaussian_common.cuh", CSRC / "head_common.cuh", CSRC / "soft_argmin.cuh", PKG.parent / "include" / "magnet_b200.h"]
 ARCH = "arch=compute_90a,code=sm_90a"
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", ARCH, "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"]

@@ -69,9 +69,11 @@ cudaError_t launch_upsample_nll_fwd(const float* depth, const float* mask, const
                                     int H, int W, int k, float* partial, cudaStream_t st);
 cudaError_t launch_upsample_nll_bwd(const float* depth, const float* mask, const float* gt, const uint8_t* gtm, float scale,
                                     int B, int H, int W, int k, float* gdepth, float* gmask, cudaStream_t st);
+cudaError_t launch_plane_depth(const float* vol, const float* planes, int B, int D, int HW, bool scores, float* out,
+                               cudaStream_t st);
 size_t depth_metrics_workspace(int P, int B, int rows, int cols);
 cudaError_t launch_depth_metrics(const float* const* preds, int P, const float* up_mask, const float* gt, int B, int H,
-                                 int W, int k, int r0, int r1, int c0, int c1, float min_d, float max_d,
+                                 int W, int k, int h, int w, int r0, int r1, int c0, int c1, float min_d, float max_d,
                                  double* partial, double* out, cudaStream_t st);
 size_t gnet_weights_bytes(int D);
 cudaError_t launch_gnet_pack(const float* w0, const float* w1, const float* b1, const float* w2, const float* b2,
@@ -864,8 +866,54 @@ int magnet_depth_metrics_f32(const magnet_depth_metrics_args* a, void* stream) {
   for (int p = 0; p < a->P; ++p)
     if (!a->pred[p]) return MAGNET_ERR_NULL;
   cudaError_t e = magnet::launch_depth_metrics(a->pred, a->P, a->k > 0 ? a->up_mask : nullptr, a->gt, a->B, a->H, a->W,
-                                               a->k, a->row0, a->row1, a->col0, a->col1, a->min_depth, a->max_depth,
-                                               a->workspace, a->out, (cudaStream_t)stream);
+                                               a->k, 0, 0, a->row0, a->row1, a->col0, a->col1, a->min_depth,
+                                               a->max_depth, a->workspace, a->out, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 2;
+  return MAGNET_OK;
+}
+
+int magnet_plane_depth_f32(const float* volume, const float* planes_host, int32_t B, int32_t D, int32_t H, int32_t W,
+                           int32_t scores, float* out, void* stream) {
+  if (!volume || !planes_host || !out) return MAGNET_ERR_NULL;
+  if (B <= 0 || D <= 0 || H <= 0 || W <= 0 || B > 65535) return MAGNET_ERR_SHAPE;
+  if ((int64_t)H * W > (1 << 26)) return MAGNET_ERR_SHAPE;
+  if (D > MAGNET_MAX_PLANES) return MAGNET_ERR_UNSUPPORTED;
+  cudaError_t e = magnet::launch_plane_depth(volume, planes_host, B, D, H * W, scores != 0, out, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 1;
+  return MAGNET_OK;
+}
+
+namespace {
+// Shape fields and box only (the sizing call needs no pointers).
+int validate_depth_metrics_nearest_shape(const magnet_depth_metrics_nearest_args* a) {
+  if (!a) return MAGNET_ERR_NULL;
+  if (a->P <= 0 || a->B <= 0 || a->H <= 0 || a->W <= 0 || a->h <= 0 || a->w <= 0) return MAGNET_ERR_SHAPE;
+  if (a->P > MAGNET_METRICS_MAX_PRED) return MAGNET_ERR_UNSUPPORTED;
+  if ((int64_t)a->P * a->B > 65535 || (int64_t)a->H * a->W > (1 << 28)) return MAGNET_ERR_SHAPE;
+  if (a->h > a->H || a->w > a->W) return MAGNET_ERR_SHAPE;
+  if (a->row0 < 0 || a->row0 > a->row1 || a->row1 > a->H) return MAGNET_ERR_SHAPE;
+  if (a->col0 < 0 || a->col0 > a->col1 || a->col1 > a->W) return MAGNET_ERR_SHAPE;
+  return MAGNET_OK;
+}
+}  // namespace
+
+int64_t magnet_depth_metrics_nearest_workspace(const magnet_depth_metrics_nearest_args* a) {
+  const int st = validate_depth_metrics_nearest_shape(a);
+  if (st != MAGNET_OK) return st;
+  return (int64_t)magnet::depth_metrics_workspace(a->P, a->B, a->row1 - a->row0, a->col1 - a->col0);
+}
+
+int magnet_depth_metrics_nearest_f32(const magnet_depth_metrics_nearest_args* a, void* stream) {
+  const int st = validate_depth_metrics_nearest_shape(a);
+  if (st != MAGNET_OK) return st;
+  if (!a->pred || !a->gt || !a->workspace || !a->out) return MAGNET_ERR_NULL;
+  for (int p = 0; p < a->P; ++p)
+    if (!a->pred[p]) return MAGNET_ERR_NULL;
+  cudaError_t e = magnet::launch_depth_metrics(a->pred, a->P, nullptr, a->gt, a->B, a->H, a->W, 0, a->h, a->w, a->row0,
+                                               a->row1, a->col0, a->col1, a->min_depth, a->max_depth, a->workspace,
+                                               a->out, (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e);
   g_launches += 2;
   return MAGNET_OK;

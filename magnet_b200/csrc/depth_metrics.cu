@@ -1,5 +1,6 @@
 // Depth evaluation on the device: the per-image metrics of validate() (test_MaGNet.py:27-81, train_MaGNet.py:132-182)
-// and utils.compute_depth_errors (utils/utils.py:106-144), for up to MAGNET_METRICS_MAX_PRED predictions sharing one GT.
+// and utils.compute_depth_errors (utils/utils.py:106-144), for up to MAGNET_METRICS_MAX_PRED predictions sharing one GT;
+// also the F-Net form of train_FNet.py:165-193 (a depth map on a coarser grid, nearest-upsampled, no variance).
 //
 // Stage 1 (depth_metrics_partial_kernel): one CTA per (128-column x DM_ROWS-row tile of the evaluation box, image,
 // prediction).  Every pixel forms the float32 terms of compute_depth_errors in numpy's operation order and adds them to
@@ -30,10 +31,29 @@ struct DmBox {
   int r0, c0, rows, cols;
 };
 
-template <bool FUSED>
+// Where a pixel's prediction comes from.
+//   DM_FULL: full-resolution (B,2,H,W) [mu, sigma].
+//   DM_FUSED: quarter-resolution (B,2,H/k,W/k) [mu, sigma] and the upsampling mask (upsample_depth_via_mask fused in).
+//   DM_NEAREST: a (B,1,h,w) depth map, F.interpolate(..., size=(H, W), mode='nearest') fused in (train_FNet.py:181).
+//     No variance: the NLL slot stays 0 and the final kernel writes nll = 0.0, as compute_depth_errors(var=None).
+enum : int { DM_FULL = 0, DM_FUSED = 1, DM_NEAREST = 2 };
+
+// The prediction grid of DM_NEAREST and ATen's source-index scales (float)h / H, (float)w / W.
+struct DmNearest {
+  int h, w;
+  float sh, sw;
+};
+
+// ATen's nearest source index (UpSample.h nearest_idx with size=..., CPU and CUDA alike): min(floor(dst * scale),
+// in - 1) with the product in float32.  Its shortcuts for equal and doubled sizes give the same index.
+__device__ __forceinline__ int nearest_src(int dst, float scale, int in) {
+  return min((int)floorf(__fmul_rn((float)dst, scale)), in - 1);
+}
+
+template <int FORM>
 __global__ void __launch_bounds__(DM_THREADS) depth_metrics_partial_kernel(
     const __grid_constant__ DmPreds preds, const float* __restrict__ up_mask, const float* __restrict__ gt, int B,
-    int H, int W, int k, DmBox box, float min_d, float max_d, double* __restrict__ partial) {
+    int H, int W, int k, DmNearest nn, DmBox box, float min_d, float max_d, double* __restrict__ partial) {
   const int tile = blockIdx.y * gridDim.x + blockIdx.x, tiles = gridDim.x * gridDim.y;
   const int img = blockIdx.z;                       // p * B + b
   const int p = img / B;
@@ -47,6 +67,7 @@ __global__ void __launch_bounds__(DM_THREADS) depth_metrics_partial_kernel(
   if (c < box.cols) {
     const int X = box.c0 + c;
     const size_t HW = (size_t)H * W;
+    const int xs = FORM == DM_NEAREST ? nearest_src(X, nn.sw, nn.w) : 0;
     for (int j = 0; j < DM_ROWS; ++j) {
       const int r = blockIdx.y * DM_ROWS + j;
       if (r >= box.rows) break;
@@ -54,13 +75,15 @@ __global__ void __launch_bounds__(DM_THREADS) depth_metrics_partial_kernel(
       float g = gt[b * HW + (size_t)Y * W + X];
       if (g > max_d) g = 0.0f;                            // gt_dmap[gt_dmap > max_depth] = 0
       if (!(g > min_d && g < max_d)) continue;            // valid_mask
-      float mu, sg;
-      if (FUSED) {
+      float mu, sg = 0.0f;
+      if (FORM == DM_FUSED) {
         float w[9];
         upsampled_gaussian(pred, up_mask, b, H / k, W / k, k, X / k, Y / k, X % k, Y % k, w, mu, sg);
-      } else {
+      } else if (FORM == DM_FULL) {
         mu = pred[(b * 2 + 0) * HW + (size_t)Y * W + X];
         sg = pred[(b * 2 + 1) * HW + (size_t)Y * W + X];
+      } else {
+        mu = pred[(b * nn.h + nearest_src(Y, nn.sh, nn.h)) * (size_t)nn.w + xs];
       }
       // masking, in the reference's order
       if (mu < min_d) mu = min_d;
@@ -89,7 +112,8 @@ __global__ void __launch_bounds__(DM_THREADS) depth_metrics_partial_kernel(
       s[S_LOG10] += (double)l10;
       s[S_INV] += (double)__fmul_rn(iv, iv);
       // 0.5 * (log(var) + log(2 pi) + square(gt - pred) / var): float32 terms, float64 sum (numpy 2 promotion)
-      s[S_NLL] += 0.5 * __dadd_rn(__dadd_rn((double)logf(var), log_2pi), (double)__fdiv_rn(d2, var));
+      if (FORM != DM_NEAREST)
+        s[S_NLL] += 0.5 * __dadd_rn(__dadd_rn((double)logf(var), log_2pi), (double)__fdiv_rn(d2, var));
     }
   }
   // fixed-order CTA reduction: butterfly inside each warp, then the four warps in index order
@@ -113,10 +137,12 @@ __global__ void __launch_bounds__(DM_THREADS) depth_metrics_partial_kernel(
 }
 
 // One CTA per (prediction, image): thread t adds rows t, t + 256, ... in order, then a fixed tree over the threads.
+// has_var == 0 (DM_NEAREST): nll = 0.0 whatever n, as compute_depth_errors(..., var=None) returns it.
 constexpr int DM_FINAL_THREADS = 256;
 
 __global__ void __launch_bounds__(DM_FINAL_THREADS) depth_metrics_final_kernel(const double* __restrict__ partial,
-                                                                              int tiles, double* __restrict__ out) {
+                                                                              int tiles, int has_var,
+                                                                              double* __restrict__ out) {
   const int img = blockIdx.x;
   const double* rows = partial + (size_t)img * tiles * DM_SUMS;
   double s[DM_SUMS];
@@ -154,7 +180,7 @@ __global__ void __launch_bounds__(DM_FINAL_THREADS) depth_metrics_final_kernel(c
     o[9] = sqrt(S[S_INV] / n);                                    // irmse
     o[10] = sqrt(S[S_LOGSQ] / n);                                 // rmse_log
     o[11] = sqrt(__dsub_rn(S[S_LOGSQ] / n, __dmul_rn(mean_err, mean_err))) * 100.0;   // silog (no FMA contraction)
-    o[12] = S[S_NLL] / n;                                         // nll
+    o[12] = has_var ? S[S_NLL] / n : 0.0;                         // nll
   }
 }
 
@@ -169,24 +195,30 @@ size_t depth_metrics_workspace(int P, int B, int rows, int cols) {
   return (size_t)P * B * g.x * g.y * DM_SUMS;
 }
 
+// k > 0: the fused-upsampling form; else h > 0: the nearest form with a (B,1,h,w) prediction; else full resolution.
 cudaError_t launch_depth_metrics(const float* const* preds, int P, const float* up_mask, const float* gt, int B, int H,
-                                 int W, int k, int r0, int r1, int c0, int c1, float min_d, float max_d,
+                                 int W, int k, int h, int w, int r0, int r1, int c0, int c1, float min_d, float max_d,
                                  double* partial, double* out, cudaStream_t st) {
   DmPreds pp;
   for (int i = 0; i < MAGNET_METRICS_MAX_PRED; ++i) pp.p[i] = i < P ? preds[i] : nullptr;
   const DmBox box{r0, c0, r1 - r0, c1 - c0};
+  // ATen's compute_scales_value without a scale factor: (float)input_size / output_size, rounded to float32
+  const DmNearest nn{h, w, h > 0 ? (float)h / (float)H : 0.0f, w > 0 ? (float)w / (float)W : 0.0f};
   dim3 grid = dm_grid(box.rows, box.cols);
   const int gx = grid.x, gy = grid.y;
   grid.z = P * B;
   if (k > 0)
-    depth_metrics_partial_kernel<true><<<grid, DM_THREADS, 0, st>>>(pp, up_mask, gt, B, H, W, k, box, min_d, max_d,
-                                                                    partial);
+    depth_metrics_partial_kernel<DM_FUSED><<<grid, DM_THREADS, 0, st>>>(pp, up_mask, gt, B, H, W, k, nn, box, min_d,
+                                                                        max_d, partial);
+  else if (h > 0)
+    depth_metrics_partial_kernel<DM_NEAREST><<<grid, DM_THREADS, 0, st>>>(pp, up_mask, gt, B, H, W, k, nn, box, min_d,
+                                                                          max_d, partial);
   else
-    depth_metrics_partial_kernel<false><<<grid, DM_THREADS, 0, st>>>(pp, up_mask, gt, B, H, W, k, box, min_d, max_d,
-                                                                     partial);
+    depth_metrics_partial_kernel<DM_FULL><<<grid, DM_THREADS, 0, st>>>(pp, up_mask, gt, B, H, W, k, nn, box, min_d,
+                                                                       max_d, partial);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  depth_metrics_final_kernel<<<P * B, DM_FINAL_THREADS, 0, st>>>(partial, gx * gy, out);
+  depth_metrics_final_kernel<<<P * B, DM_FINAL_THREADS, 0, st>>>(partial, gx * gy, k > 0 || h <= 0, out);
   return cudaGetLastError();
 }
 

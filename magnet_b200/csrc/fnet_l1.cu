@@ -5,6 +5,7 @@
 //   forward: one partial sum of |pred - gt| per CTA of 128 pixels (the caller adds them and divides by the count)
 //   backward: dL/dscore_j = prob_j (d_j - pred) sign(pred - gt) mask scale, sign(0) = 0 (torch's abs backward)
 #include "common.cuh"
+#include "soft_argmin.cuh"
 
 namespace magnet {
 
@@ -21,27 +22,13 @@ struct FnetL1Params {
   float d[MAGNET_MAX_PLANES];           // plane depths
 };
 
-// softmax statistics of one pixel: max, 1 / sum exp(s - max) and the soft-argmin prediction
-__device__ __forceinline__ void soft_argmin(const FnetL1Params& p, const float* s, float& m, float& inv_z, float& pred) {
-  m = -INFINITY;
-  for (int j = 0; j < p.D; ++j) m = fmaxf(m, s[(size_t)j * p.HW]);
-  float z = 0.0f, num = 0.0f;
-  for (int j = 0; j < p.D; ++j) {
-    const float e = expf(s[(size_t)j * p.HW] - m);
-    z += e;
-    num = __fmaf_rn(e, p.d[j], num);
-  }
-  inv_z = 1.0f / z;
-  pred = num * inv_z;
-}
-
 __global__ void __launch_bounds__(L1_THREADS) fnet_l1_fwd_kernel(const __grid_constant__ FnetL1Params p) {
   const int n = blockIdx.x * L1_THREADS + threadIdx.x;
   const size_t b = blockIdx.y;
   float l1 = 0.0f;
   if (n < p.HW && p.mask[b * p.HW + n]) {
     float m, inv_z, pred;
-    soft_argmin(p, p.scores + b * p.D * p.HW + n, m, inv_z, pred);
+    soft_argmin(p.scores + b * p.D * p.HW + n, p.HW, p.D, p.d, m, inv_z, pred);
     l1 = fabsf(pred - p.gt[b * p.HW + n]);
   }
   __shared__ float red[L1_THREADS / 32];
@@ -60,7 +47,7 @@ __global__ void __launch_bounds__(L1_THREADS) fnet_l1_bwd_kernel(const __grid_co
   float* g = p.out + b * p.D * p.HW + n;
   float coef = 0.0f, m = 0.0f, inv_z = 0.0f, pred = 0.0f;
   if (p.mask[b * p.HW + n]) {
-    soft_argmin(p, s, m, inv_z, pred);
+    soft_argmin(s, p.HW, p.D, p.d, m, inv_z, pred);
     const float d = pred - p.gt[b * p.HW + n];
     const float sgn = d > 0.0f ? 1.0f : (d < 0.0f ? -1.0f : 0.0f);
     coef = sgn * p.scale * (p.grad_scale != nullptr ? *p.grad_scale : 1.0f);

@@ -443,6 +443,19 @@ class MagnetF(nn.Module):
         gt = nn.functional.interpolate(gt, size=[scores.shape[2], scores.shape[3]], mode='nearest')
         return ops.fnet_l1_loss(scores, _plane_list(d_center), gt.contiguous(), gt > min_depth)
 
+    def predict(self, ref_img, nghbr_imgs, nghbr_poses, is_valid, cam_intrins, d_center):
+        """F-Net's soft-argmin depth map (train_FNet.py:96 / :180) on the volume's grid, (B, 1, h, w) float32: the
+        plane-sweep scores followed by ``ops.plane_depth`` with the softmax fused in, so the probability volume is never
+        written.  The prediction is bit for bit the one ``loss`` supervises.  Inference
+        only: it runs under ``torch.no_grad()`` and the result carries no graph.  Score it against the full-resolution
+        GT with ``DepthMetrics.update(pred, gt, nearest=True)``."""
+        from .homography import _plane_list, plane_sweep_f
+        with torch.no_grad():
+            ref_feat, nghbr_feat = self._features(ref_img, nghbr_imgs)
+            scores = plane_sweep_f(d_center, ref_feat, nghbr_feat, nghbr_poses[:, :, :3, :3], nghbr_poses[:, :, :3, 3],
+                                   is_valid, cam_intrins, softmax=False)
+            return ops.plane_depth(scores, _plane_list(d_center), scores=True)
+
 
 def install(homography_module=None) -> None:
     """Rebind the reference's operators to the H100 kernels so that ``MAGNET.forward`` /

@@ -16,13 +16,18 @@ class DepthMetrics:
     ``update`` adds every image of the batch (the reference scores only image 0 of each batch; its test loaders use
     batch 1) without a host read, so it can be captured in a CUDA graph once the accumulator exists (after the first
     update, or ``reset``).  ``value`` reads the accumulator once and returns the reference's dict.  Sums and the
-    average are float64; an image without a valid pixel contributes NaN, as it does to the reference's average."""
+    average are float64; an image without a valid pixel contributes NaN, as it does to the reference's average.
+
+    An instance scores either Gaussian predictions (full resolution or fused upsampling; nll is the Gaussian NLL) or,
+    with ``nearest=True``, F-Net depth maps (train_FNet.py's validate(); nll is 0.0).  The form is fixed at the first
+    update and the other one is refused, because the nll column means something different in each."""
 
     def __init__(self, min_depth: float, max_depth: float, crop: Optional[str] = None):
         ops.crop_box(crop, 1, 1)                       # reject an unknown crop now, not at the first update
         self.min_depth, self.max_depth, self.crop = float(min_depth), float(max_depth), crop
         # (P, 14) float64: images seen, then the sums over images of the 13 columns of ops.depth_metrics
         self._acc: Optional[torch.Tensor] = None
+        self._nearest: Optional[bool] = None           # the form of the first update
 
     def reset(self) -> None:
         """Zero the running sums in place (a captured update keeps accumulating into the same memory)."""
@@ -30,15 +35,23 @@ class DepthMetrics:
             self._acc.zero_()
 
     def update(self, pred_or_list, gt: torch.Tensor, up_mask: Optional[torch.Tensor] = None,
-               k: Optional[int] = None) -> torch.Tensor:
+               k: Optional[int] = None, nearest: bool = False) -> torch.Tensor:
         """Score one batch: ``pred_or_list`` is (a list of up to 8) full-resolution (B,2,H,W) [mu, sigma], or with
-        ``up_mask`` and ``k`` the quarter-resolution Gaussians of ``MagnetHead.forward_quarter``.  Returns the (P,B,13)
-        per-image rows of ``ops.depth_metrics``.  Half-precision predictions / masks (torch.autocast) are upcast."""
+        ``up_mask`` and ``k`` the quarter-resolution Gaussians of ``MagnetHead.forward_quarter``, or with
+        ``nearest=True`` the (B,1,h,w) depth maps of ``MagnetF.predict`` / ``ops.plane_depth``, nearest-upsampled to
+        the GT size.  Returns the (P,B,13) per-image rows of ``ops.depth_metrics``.  Half-precision predictions / masks
+        (torch.autocast) are upcast."""
+        nearest = bool(nearest)
+        if self._nearest is not None and nearest != self._nearest:
+            raise _lib.MagnetError("this DepthMetrics scores " + ("F-Net depth maps (nearest=True)" if self._nearest
+                                                                  else "Gaussian predictions (nearest=False)")
+                                   + "; use another instance for the other form (its nll column differs)")
         preds = [pred_or_list] if isinstance(pred_or_list, torch.Tensor) else list(pred_or_list)
         pred_or_list = [p.float() for p in preds]
         up_mask = None if up_mask is None else up_mask.float()
         rows = ops.depth_metrics(pred_or_list, gt.float(), min_depth=self.min_depth, max_depth=self.max_depth, crop=self.crop,
-                                 up_mask=up_mask, k=k)
+                                 up_mask=up_mask, k=k, nearest=nearest)
+        self._nearest = nearest
         P, B = rows.shape[0], rows.shape[1]
         if self._acc is None:
             self._acc = torch.zeros(P, 1 + _lib.MAGNET_METRICS_COLS, device=rows.device, dtype=torch.float64)

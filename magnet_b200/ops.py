@@ -1008,6 +1008,32 @@ def fnet_l1_loss(scores, planes, gt_q, mask_q, count=None):
     return FnetL1Loss.apply(scores, planes, gt_q, mask_u8, count)
 
 
+def plane_depth(volume: torch.Tensor, planes, *, scores: bool) -> torch.Tensor:
+    """F-Net's soft-argmin depth map sum_j prob_j d_j (train_FNet.py:96 / :180) of a (B,D,h,w) plane volume ->
+    (B,1,h,w) float32, one kernel.  ``scores=True``: ``volume`` is the 1/V-averaged scores of
+    ``plane_sweep_f(softmax=False)``; the softmax over the planes is fused in and the prediction is bit for bit the one
+    ``fnet_l1_loss`` supervises.  ``scores=False``: ``volume`` is the probability volume of ``est_costvolume_F`` /
+    ``MAGNET_F.forward``.  ``planes``: the D plane depths, a sequence of floats or the (1,D,1,1) ``d_center`` tensor
+    (read to the host once per tensor).  Half-precision volumes (torch.autocast) are upcast."""
+    if isinstance(volume, torch.Tensor) and volume.dtype in (torch.float16, torch.bfloat16):
+        volume = volume.float()
+    volume = _need_cuda_f32("volume", volume)
+    if volume.dim() != 4:
+        raise _lib.MagnetError(f"volume must be (B,D,H,W), got {tuple(volume.shape)}")
+    B, D, H, W = volume.shape
+    if isinstance(planes, torch.Tensor):
+        from .homography import _plane_list
+        planes = _plane_list(planes)
+    karr = planes if isinstance(planes, C.Array) else k_array(planes)
+    if len(karr) != D:
+        raise _lib.MagnetError(f"{len(karr)} plane depths for {D} planes of the volume")
+    out = torch.empty(B, 1, H, W, device=volume.device, dtype=torch.float32)
+    with torch.cuda.device(volume.device):
+        check(lib().magnet_plane_depth_f32(volume.data_ptr(), C.cast(karr, C.c_void_p), B, D, H, W, int(bool(scores)),
+                                           out.data_ptr(), _stream(volume.device)), "magnet_plane_depth_f32")
+    return out
+
+
 def relative_poses(ext_ref: torch.Tensor, ext_nghbr: torch.Tensor):
     """data_preprocess (utils/utils.py:72-98) on the device: ext_ref (B,4,4), ext_nghbr (V,B,4,4) ->
     (nghbr_poses (B,V,4,4), is_valid (B,V) int32)."""
@@ -1062,21 +1088,29 @@ def crop_box(crop, H: int, W: int):
 
 
 def depth_metrics(pred_or_list, gt: torch.Tensor, *, min_depth: float, max_depth: float, crop=None,
-                  up_mask: Optional[torch.Tensor] = None, k: Optional[int] = None) -> torch.Tensor:
+                  up_mask: Optional[torch.Tensor] = None, k: Optional[int] = None, nearest: bool = False) -> torch.Tensor:
     """Per-image depth metrics of validate() (test_MaGNet.py:52-79) + utils.compute_depth_errors, on the device.
 
     pred_or_list: one prediction or a list of up to 8 sharing ``gt`` (B,1,H,W) (raw GT; values above max_depth count
     as 0).  Each prediction is the full-resolution (B,2,H,W) [mu, sigma], or, with ``up_mask`` (B,9k^2,H/k,W/k) and
     ``k``, the quarter-resolution (B,2,H/k,W/k) Gaussians, upsampled inside the kernel (upsample_depth_via_mask).
+    With ``nearest=True`` (F-Net's validate(), train_FNet.py:165-193) each prediction is a (B,1,h,w) depth map with
+    h <= H, w <= W, upsampled inside the kernel as F.interpolate(..., size=(H, W), mode='nearest'); there is no
+    variance and the nll column is 0.0, as compute_depth_errors(..., var=None) gives it.
     crop: None, 'garg' or 'eigen'.  Returns a (P,B,13) float64 device tensor: the number of valid pixels, then the
-    metrics in METRIC_KEYS order (NaN for an image without a valid pixel).  Two kernel launches, no host sync."""
+    metrics in METRIC_KEYS order (NaN for an image without a valid pixel; nll 0.0 there in the nearest form).  Two
+    kernel launches, no host sync."""
     preds = [pred_or_list] if isinstance(pred_or_list, torch.Tensor) else list(pred_or_list)
     if not 1 <= len(preds) <= _lib.MAGNET_METRICS_MAX_PRED:
         raise _lib.MagnetError(f"1 to {_lib.MAGNET_METRICS_MAX_PRED} predictions per call, got {len(preds)}")
+    if nearest and (up_mask is not None or k is not None):
+        raise _lib.MagnetError("nearest=True takes (B,1,h,w) depth maps: it does not combine with up_mask / k")
     gt = _need_cuda_f32("gt", gt)
     if gt.dim() != 4 or gt.shape[1] != 1:
         raise _lib.MagnetError(f"gt must be (B,1,H,W), got {tuple(gt.shape)}")
     B, _, H, W = gt.shape
+    if nearest:
+        return _depth_metrics_nearest(preds, gt, min_depth, max_depth, crop)
     if (up_mask is None) != (k is None):
         raise _lib.MagnetError("up_mask and k go together (the fused-upsampling form needs both)")
     if up_mask is not None:
@@ -1106,4 +1140,31 @@ def depth_metrics(pred_or_list, gt: torch.Tensor, *, min_depth: float, max_depth
     a.workspace, a.out = workspace.data_ptr(), out.data_ptr()
     with torch.cuda.device(dev):
         check(lib().magnet_depth_metrics_f32(C.byref(a), _stream(dev)), "magnet_depth_metrics_f32")
+    return out
+
+
+def _depth_metrics_nearest(preds, gt, min_depth, max_depth, crop):
+    """The nearest form of ``depth_metrics``: ``preds`` (B,1,h,w) each, ``gt`` the checked (B,1,H,W) GT."""
+    B, _, H, W = gt.shape
+    for i, p in enumerate(preds):
+        preds[i] = _need_cuda_f32(f"pred[{i}]", p)
+    pshape = tuple(preds[0].shape)
+    if len(pshape) != 4 or pshape[:2] != (B, 1) or not (1 <= pshape[2] <= H and 1 <= pshape[3] <= W):
+        raise _lib.MagnetError(f"pred[0] must be (B,1,h,w) with B = {B}, h <= {H}, w <= {W}, got {pshape}")
+    for i, p in enumerate(preds):
+        _expect(f"pred[{i}]", p, pshape)
+    dev = _same_device(("gt", gt), *((f"pred[{i}]", p) for i, p in enumerate(preds)))
+    r0, r1, c0, c1 = crop_box(crop, H, W)
+    ptrs = (C.c_void_p * len(preds))(*[p.data_ptr() for p in preds])
+    a = _lib.DepthMetricsNearestArgs(P=len(preds), B=B, H=H, W=W, h=pshape[2], w=pshape[3], row0=r0, row1=r1, col0=c0,
+                                     col1=c1, min_depth=float(min_depth), max_depth=float(max_depth),
+                                     pred=C.cast(ptrs, C.POINTER(C.c_void_p)), gt=gt.data_ptr())
+    n = lib().magnet_depth_metrics_nearest_workspace(C.byref(a))
+    if n < 0:
+        check(int(n), "magnet_depth_metrics_nearest_workspace")
+    workspace = torch.empty(int(n), device=dev, dtype=torch.float64)
+    out = torch.empty(len(preds), B, _lib.MAGNET_METRICS_COLS, device=dev, dtype=torch.float64)
+    a.workspace, a.out = workspace.data_ptr(), out.data_ptr()
+    with torch.cuda.device(dev):
+        check(lib().magnet_depth_metrics_nearest_f32(C.byref(a), _stream(dev)), "magnet_depth_metrics_nearest_f32")
     return out
