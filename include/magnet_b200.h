@@ -457,6 +457,41 @@ int magnet_mask_train_fwd_f32(const magnet_mask_train_args* args, void* stream);
 int magnet_mask_bwd_f32(const magnet_mask_train_args* args, void* stream);
 
 /*
+ * D-Net heads of inference, fused (DESIGN §3.15) — replace, after the reference's first depth-head and mask-head
+ * convolutions, the rest of Decoder.depth_head / mask_head (models/submodules/D_dense_depth.py:148-160,187-192),
+ * upsample_depth_via_mask (D_dense_depth.py:86-100) and DNET's activations (models/DNET.py:56-67):
+ *   depth:    h0 = ReLU(pre_d),  h1 = ReLU(W1 h0 + b1),  [mu, v] = W2 h1 + b2 (2 channels);
+ *   upsample: g0 = ReLU(pre_m),  g1 = ReLU(M1 g0 + c1),  mask = M3 g1 + c3 (144 = 9 x k x k channels),
+ *             [mu, v'] = convex upsampling of the raw [mu, v] by the mask,  var = (elu(v') + 1) + 1e-10.
+ * The 128 -> 128 layers and the 128 -> 144 layer run on the fp16 tensor cores with fp32 accuracy (SPLIT16, as the G-Net
+ * and mask heads), the 128 -> 2 layer on the CUDA cores; no hidden map and no mask is written.  elu is x <= 0 ?
+ * expm1f(x) : x and every add is one fp32 rounding, in torch's order.  Forward only; no atomics, so results are
+ * bit-identical from run to run.
+ *
+ * magnet_dnet_pack_weights_f32 writes both heads in the kernels' layout into `packed` (magnet_dnet_weights_bytes(k)
+ * bytes, 16-byte aligned): depth head d_w1 (128, 128), d_b1 (128), d_w2 (2, 128), d_b2 (2); with k == 4 also the mask
+ * head m_w1 (128, 128), m_b1 (128), m_w3 (144, 128), m_b3 (144); with k == 0 the m_* pointers are not read (may be
+ * NULL).  Two kernels, four with the mask head.  magnet_dnet_weights_bytes: k == 0 the depth head alone, k == 4 both
+ * heads, 0 for any other k.
+ *
+ * magnet_dnet_depth_f32: pre_d (B, 128, H, W) the first depth-head convolution's output before its ReLU -> out
+ * (B, 2, H, W): with sigma == 0 the raw [mu, v] (what magnet_dnet_upsample_f32 reads), else [mu, sqrt(var)]
+ * (activation_G_magnet: D-Net's mono_gmms inside MaGNet).  One kernel.
+ * magnet_dnet_upsample_f32: pre_m (B, 128, H, W) the first mask-head convolution's output before its ReLU, raw (B, 2, H,
+ * W) from magnet_dnet_depth_f32 with sigma == 0, a k == 4 pack -> out (B, 2, k*H, k*W) [mu, var] (activation_G: what
+ * DNET(args) returns).  One kernel.  k != 4 -> MAGNET_ERR_UNSUPPORTED.
+ * Both: B*H*W < 2^31; every pointer 16-byte aligned; out must not overlap the inputs.
+ */
+size_t magnet_dnet_weights_bytes(int32_t k);
+int magnet_dnet_pack_weights_f32(const float* d_w1, const float* d_b1, const float* d_w2, const float* d_b2,
+                                 const float* m_w1, const float* m_b1, const float* m_w3, const float* m_b3, int32_t k,
+                                 void* packed, void* stream);
+int magnet_dnet_depth_f32(const float* pre_d, const void* packed, int32_t B, int32_t H, int32_t W, int32_t sigma,
+                          float* out, void* stream);
+int magnet_dnet_upsample_f32(const float* pre_m, const void* packed, const float* raw, int32_t B, int32_t H, int32_t W,
+                             int32_t k, float* out, void* stream);
+
+/*
  * Caller-side camera preparation on the device (SURVEY §8 f-4).
  * magnet_relative_poses_f32 replaces utils/utils.py:72-98 (data_preprocess): poses_out[b,v] = ext_nghbr[v,b] *
  * inv(ext_ref[b]) (ref-camera -> source-camera), is_valid_out[b,v] = 0 when either extrinsic or the product holds a
@@ -587,6 +622,15 @@ typedef struct magnet_depth_metrics_nearest_args {
 /* Doubles of workspace the call needs (shape fields and box of args only), or a negative magnet_status. */
 int64_t magnet_depth_metrics_nearest_workspace(const magnet_depth_metrics_nearest_args* args);
 int magnet_depth_metrics_nearest_f32(const magnet_depth_metrics_nearest_args* args, void* stream);
+
+/*
+ * Depth evaluation of D-Net — replaces the metric block of test_DNet.py validate() (:40-71): the full-resolution
+ * prediction's channel 1 is the variance D-Net returns (activation_G), passed to compute_depth_errors as var, so
+ * var = max(channel 1, 1e-6) on the float32 value instead of max(sigma^2, 1e-6).  Everything else as
+ * magnet_depth_metrics_f32 with k == 0: the same args (k must be 0, up_mask is ignored), the same workspace
+ * (magnet_depth_metrics_workspace), out (P,B,MAGNET_METRICS_COLS).  k != 0 -> MAGNET_ERR_UNSUPPORTED.  Two kernels.
+ */
+int magnet_depth_metrics_var_f32(const magnet_depth_metrics_args* args, void* stream);
 
 #ifdef __cplusplus
 }

@@ -47,6 +47,8 @@ EXPORTS = (
     "magnet_mask_train_weights_bytes", "magnet_mask_saved_bytes", "magnet_mask_bwd_workspace_bytes",
     "magnet_mask_train_partials", "magnet_mask_pack_train_weights_f32", "magnet_mask_train_fwd_f32",
     "magnet_mask_bwd_f32",
+    "magnet_dnet_weights_bytes", "magnet_dnet_pack_weights_f32", "magnet_dnet_depth_f32", "magnet_dnet_upsample_f32",
+    "magnet_depth_metrics_var_f32",
 )
 MAGNET_HIDDEN_CHANNELS = 128
 MAGNET_GNET_SCRATCH_BYTES = 16
@@ -271,6 +273,16 @@ def lib() -> C.CDLL:
     L.magnet_mask_train_fwd_f32.argtypes = [C.POINTER(MaskTrainArgs), C.c_void_p]
     L.magnet_mask_bwd_f32.restype = C.c_int
     L.magnet_mask_bwd_f32.argtypes = [C.POINTER(MaskTrainArgs), C.c_void_p]
+    L.magnet_dnet_weights_bytes.restype = C.c_size_t
+    L.magnet_dnet_weights_bytes.argtypes = [C.c_int32]
+    L.magnet_dnet_pack_weights_f32.restype = C.c_int
+    L.magnet_dnet_pack_weights_f32.argtypes = [C.c_void_p] * 8 + [C.c_int32, C.c_void_p, C.c_void_p]
+    L.magnet_dnet_depth_f32.restype = C.c_int
+    L.magnet_dnet_depth_f32.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p, C.c_void_p]
+    L.magnet_dnet_upsample_f32.restype = C.c_int
+    L.magnet_dnet_upsample_f32.argtypes = [C.c_void_p] * 3 + [C.c_int32] * 4 + [C.c_void_p, C.c_void_p]
+    L.magnet_depth_metrics_var_f32.restype = C.c_int
+    L.magnet_depth_metrics_var_f32.argtypes = [C.POINTER(DepthMetricsArgs), C.c_void_p]
     if L.magnet_abi_version() != MAGNET_ABI_VERSION:
         raise MagnetError(f"ABI version mismatch: library {L.magnet_abi_version()} != binding {MAGNET_ABI_VERSION}")
     _lib = L

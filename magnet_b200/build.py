@@ -18,7 +18,7 @@ CSRC = PKG / "csrc"
 BUILD = PKG / "_build"
 LIB = PKG / "libmagnet_b200.so"
 SOURCES = ["api.cu", "cost_mma.cu", "cost_tma.cu", "cost_cells.cu", "cost_direct.cu", "cost_f_bwd.cu", "cost_f_bwd_mma.cu", "cost_cw_bwd.cu", "fnet_l1.cu",
-           "plane_depth.cu", "aux_kernels.cu", "depth_metrics.cu", "gnet_head.cu", "mask_head.cu"]
+           "plane_depth.cu", "aux_kernels.cu", "depth_metrics.cu", "gnet_head.cu", "mask_head.cu", "dnet_head.cu"]
 HEADERS = [CSRC / "common.cuh", CSRC / "cells_common.cuh", CSRC / "tma_common.cuh", CSRC / "cw_mask.cuh",
            CSRC / "upsample_common.cuh", CSRC / "gaussian_common.cuh", CSRC / "head_common.cuh", CSRC / "soft_argmin.cuh", PKG.parent / "include" / "magnet_b200.h"]
 ARCH = "arch=compute_90a,code=sm_90a"

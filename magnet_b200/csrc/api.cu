@@ -73,8 +73,16 @@ cudaError_t launch_plane_depth(const float* vol, const float* planes, int B, int
                                cudaStream_t st);
 size_t depth_metrics_workspace(int P, int B, int rows, int cols);
 cudaError_t launch_depth_metrics(const float* const* preds, int P, const float* up_mask, const float* gt, int B, int H,
-                                 int W, int k, int h, int w, int r0, int r1, int c0, int c1, float min_d, float max_d,
-                                 double* partial, double* out, cudaStream_t st);
+                                 int W, int k, int h, int w, bool variance, int r0, int r1, int c0, int c1, float min_d,
+                                 float max_d, double* partial, double* out, cudaStream_t st);
+size_t dnet_weights_bytes(bool with_mask);
+cudaError_t launch_dnet_pack(const float* dw1, const float* db1, const float* dw2, const float* db2, const float* mw1,
+                             const float* mb1, const float* mw3, const float* mb3, bool with_mask, void* dst,
+                             cudaStream_t st, int* launches);
+cudaError_t launch_dnet_depth(int B, int H, int W, const float* pre_d, const void* weights, bool sigma, float* out,
+                              cudaStream_t st);
+cudaError_t launch_dnet_upsample_packed(int B, int H, int W, const float* pre_m, const void* weights, const float* raw,
+                                        float* out, cudaStream_t st);
 size_t gnet_weights_bytes(int D);
 cudaError_t launch_gnet_pack(const float* w0, const float* w1, const float* b1, const float* w2, const float* b2,
                              const float* w3, const float* b3, int D, void* dst, cudaStream_t st);
@@ -866,10 +874,73 @@ int magnet_depth_metrics_f32(const magnet_depth_metrics_args* a, void* stream) {
   for (int p = 0; p < a->P; ++p)
     if (!a->pred[p]) return MAGNET_ERR_NULL;
   cudaError_t e = magnet::launch_depth_metrics(a->pred, a->P, a->k > 0 ? a->up_mask : nullptr, a->gt, a->B, a->H, a->W,
-                                               a->k, 0, 0, a->row0, a->row1, a->col0, a->col1, a->min_depth,
+                                               a->k, 0, 0, false, a->row0, a->row1, a->col0, a->col1, a->min_depth,
                                                a->max_depth, a->workspace, a->out, (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e);
   g_launches += 2;
+  return MAGNET_OK;
+}
+
+int magnet_depth_metrics_var_f32(const magnet_depth_metrics_args* a, void* stream) {
+  const int st = validate_depth_metrics_shape(a);
+  if (st != MAGNET_OK) return st;
+  if (a->k != 0) return MAGNET_ERR_UNSUPPORTED;
+  if (!a->pred || !a->gt || !a->workspace || !a->out) return MAGNET_ERR_NULL;
+  for (int p = 0; p < a->P; ++p)
+    if (!a->pred[p]) return MAGNET_ERR_NULL;
+  cudaError_t e = magnet::launch_depth_metrics(a->pred, a->P, nullptr, a->gt, a->B, a->H, a->W, 0, 0, 0, true, a->row0,
+                                               a->row1, a->col0, a->col1, a->min_depth, a->max_depth, a->workspace,
+                                               a->out, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 2;
+  return MAGNET_OK;
+}
+
+size_t magnet_dnet_weights_bytes(int32_t k) {
+  return k == 0 || k == 4 ? magnet::dnet_weights_bytes(k == 4) : 0;
+}
+
+int magnet_dnet_pack_weights_f32(const float* d_w1, const float* d_b1, const float* d_w2, const float* d_b2,
+                                 const float* m_w1, const float* m_b1, const float* m_w3, const float* m_b3, int32_t k,
+                                 void* packed, void* stream) {
+  if (k != 0 && k != 4) return MAGNET_ERR_UNSUPPORTED;
+  if (!d_w1 || !d_b1 || !d_w2 || !d_b2 || !packed) return MAGNET_ERR_NULL;
+  if (k == 4 && (!m_w1 || !m_b1 || !m_w3 || !m_b3)) return MAGNET_ERR_NULL;
+  if (misaligned16(packed)) return MAGNET_ERR_ALIGN;
+  int launches = 0;
+  cudaError_t e = magnet::launch_dnet_pack(d_w1, d_b1, d_w2, d_b2, m_w1, m_b1, m_w3, m_b3, k == 4, packed,
+                                           (cudaStream_t)stream, &launches);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += launches;
+  return MAGNET_OK;
+}
+
+namespace {
+bool dnet_shape_ok(int32_t B, int32_t H, int32_t W) {
+  return B > 0 && H > 0 && W > 0 && (int64_t)B * H * W < ((int64_t)1 << 31);
+}
+}  // namespace
+
+int magnet_dnet_depth_f32(const float* pre_d, const void* packed, int32_t B, int32_t H, int32_t W, int32_t sigma,
+                          float* out, void* stream) {
+  if (!dnet_shape_ok(B, H, W)) return MAGNET_ERR_SHAPE;
+  if (!pre_d || !packed || !out) return MAGNET_ERR_NULL;
+  if (misaligned16(pre_d) || misaligned16(packed) || misaligned16(out)) return MAGNET_ERR_ALIGN;
+  cudaError_t e = magnet::launch_dnet_depth(B, H, W, pre_d, packed, sigma != 0, out, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 1;
+  return MAGNET_OK;
+}
+
+int magnet_dnet_upsample_f32(const float* pre_m, const void* packed, const float* raw, int32_t B, int32_t H, int32_t W,
+                             int32_t k, float* out, void* stream) {
+  if (!dnet_shape_ok(B, H, W)) return MAGNET_ERR_SHAPE;
+  if (k != 4) return MAGNET_ERR_UNSUPPORTED;
+  if (!pre_m || !packed || !raw || !out) return MAGNET_ERR_NULL;
+  if (misaligned16(pre_m) || misaligned16(packed) || misaligned16(raw) || misaligned16(out)) return MAGNET_ERR_ALIGN;
+  cudaError_t e = magnet::launch_dnet_upsample_packed(B, H, W, pre_m, packed, raw, out, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += 1;
   return MAGNET_OK;
 }
 
@@ -911,7 +982,7 @@ int magnet_depth_metrics_nearest_f32(const magnet_depth_metrics_nearest_args* a,
   if (!a->pred || !a->gt || !a->workspace || !a->out) return MAGNET_ERR_NULL;
   for (int p = 0; p < a->P; ++p)
     if (!a->pred[p]) return MAGNET_ERR_NULL;
-  cudaError_t e = magnet::launch_depth_metrics(a->pred, a->P, nullptr, a->gt, a->B, a->H, a->W, 0, a->h, a->w, a->row0,
+  cudaError_t e = magnet::launch_depth_metrics(a->pred, a->P, nullptr, a->gt, a->B, a->H, a->W, 0, a->h, a->w, false, a->row0,
                                                a->row1, a->col0, a->col1, a->min_depth, a->max_depth, a->workspace,
                                                a->out, (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e);

@@ -36,7 +36,8 @@ struct DmBox {
 //   DM_FUSED: quarter-resolution (B,2,H/k,W/k) [mu, sigma] and the upsampling mask (upsample_depth_via_mask fused in).
 //   DM_NEAREST: a (B,1,h,w) depth map, F.interpolate(..., size=(H, W), mode='nearest') fused in (train_FNet.py:181).
 //     No variance: the NLL slot stays 0 and the final kernel writes nll = 0.0, as compute_depth_errors(var=None).
-enum : int { DM_FULL = 0, DM_FUSED = 1, DM_NEAREST = 2 };
+//   DM_VAR: full-resolution (B,2,H,W) [mu, var], D-Net's output (test_DNet.py:40-71): channel 1 is the variance itself.
+enum : int { DM_FULL = 0, DM_FUSED = 1, DM_NEAREST = 2, DM_VAR = 3 };
 
 // The prediction grid of DM_NEAREST and ATen's source-index scales (float)h / H, (float)w / W.
 struct DmNearest {
@@ -79,7 +80,7 @@ __global__ void __launch_bounds__(DM_THREADS) depth_metrics_partial_kernel(
       if (FORM == DM_FUSED) {
         float w[9];
         upsampled_gaussian(pred, up_mask, b, H / k, W / k, k, X / k, Y / k, X % k, Y % k, w, mu, sg);
-      } else if (FORM == DM_FULL) {
+      } else if (FORM == DM_FULL || FORM == DM_VAR) {
         mu = pred[(b * 2 + 0) * HW + (size_t)Y * W + X];
         sg = pred[(b * 2 + 1) * HW + (size_t)Y * W + X];
       } else {
@@ -90,7 +91,7 @@ __global__ void __launch_bounds__(DM_THREADS) depth_metrics_partial_kernel(
       if (mu > max_d) mu = max_d;
       if (isinf(mu)) mu = max_d;
       if (isnan(mu)) mu = min_d;
-      float var = __fmul_rn(sg, sg);                      // np.square of the unclamped sigma
+      float var = FORM == DM_VAR ? sg : __fmul_rn(sg, sg);   // the variance, or np.square of the unclamped sigma
       if (var < 1e-6f) var = 1e-6f;
       const float r1 = __fdiv_rn(g, mu), r2 = __fdiv_rn(mu, g);
       const float th = (isnan(r1) || isnan(r2)) ? r1 + r2 : fmaxf(r1, r2);   // np.maximum propagates NaN
@@ -195,10 +196,11 @@ size_t depth_metrics_workspace(int P, int B, int rows, int cols) {
   return (size_t)P * B * g.x * g.y * DM_SUMS;
 }
 
-// k > 0: the fused-upsampling form; else h > 0: the nearest form with a (B,1,h,w) prediction; else full resolution.
+// k > 0: the fused-upsampling form; else h > 0: the nearest form with a (B,1,h,w) prediction; else full resolution,
+// [mu, var] with `variance`, else [mu, sigma].
 cudaError_t launch_depth_metrics(const float* const* preds, int P, const float* up_mask, const float* gt, int B, int H,
-                                 int W, int k, int h, int w, int r0, int r1, int c0, int c1, float min_d, float max_d,
-                                 double* partial, double* out, cudaStream_t st) {
+                                 int W, int k, int h, int w, bool variance, int r0, int r1, int c0, int c1, float min_d,
+                                 float max_d, double* partial, double* out, cudaStream_t st) {
   DmPreds pp;
   for (int i = 0; i < MAGNET_METRICS_MAX_PRED; ++i) pp.p[i] = i < P ? preds[i] : nullptr;
   const DmBox box{r0, c0, r1 - r0, c1 - c0};
@@ -213,6 +215,9 @@ cudaError_t launch_depth_metrics(const float* const* preds, int P, const float* 
   else if (h > 0)
     depth_metrics_partial_kernel<DM_NEAREST><<<grid, DM_THREADS, 0, st>>>(pp, up_mask, gt, B, H, W, k, nn, box, min_d,
                                                                           max_d, partial);
+  else if (variance)
+    depth_metrics_partial_kernel<DM_VAR><<<grid, DM_THREADS, 0, st>>>(pp, up_mask, gt, B, H, W, k, nn, box, min_d,
+                                                                      max_d, partial);
   else
     depth_metrics_partial_kernel<DM_FULL><<<grid, DM_THREADS, 0, st>>>(pp, up_mask, gt, B, H, W, k, nn, box, min_d,
                                                                        max_d, partial);

@@ -177,25 +177,8 @@ __global__ void __launch_bounds__(NT, 1) gnet_head_kernel(const GnetParams p) {
     if constexpr (SAVE) save_hidden(2);
 
     // ---- 128 -> 2 on the CUDA cores, quad reduction, Gaussian update ----
-    const float* w3 = vec + 2 * HID;
-    float r[4] = {0.0f, 0.0f, 0.0f, 0.0f};               // (mu1, sigma1) of rows g and g+8
-#pragma unroll
-    for (int nt = 0; nt < NTILE; ++nt) {
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int n = nt * 8 + 2 * q + e;
-        const float wm = w3[n], ws = w3[HID + n];
-        r[0] = __fmaf_rn(acc[nt][e], wm, r[0]);
-        r[1] = __fmaf_rn(acc[nt][e], ws, r[1]);
-        r[2] = __fmaf_rn(acc[nt][2 + e], wm, r[2]);
-        r[3] = __fmaf_rn(acc[nt][2 + e], ws, r[3]);
-      }
-    }
-#pragma unroll
-    for (int o = 1; o <= 2; o <<= 1) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) r[i] = __fadd_rn(r[i], __shfl_xor_sync(0xffffffffu, r[i], o));
-    }
+    float r[4];                                          // (mu1, sigma1) of rows g and g+8
+    out2_layer(acc, vec + 2 * HID, q, r);
     if (q < 2 && (q == 0 ? va : vb)) {                  // lane 0 of the quad writes pixel g, lane 1 pixel g+8
       const size_t o = (size_t)b * 2 * HW + (size_t)y * p.W + (q == 0 ? xa : xb);
       const float mu1 = __fadd_rn(q == 0 ? r[0] : r[2], vec[4 * HID]);

@@ -96,6 +96,38 @@ __device__ __forceinline__ void hidden_layer(float (&acc)[NTILE][4], const uint4
   }
 }
 
+// The 128 -> 2 layer on the CUDA cores (G-Net's output layer, D-Net's depth head): w = [W(0, :), W(1, :)] fp32, 32
+// sequential FMAs per lane, then the quad's two-step butterfly.  r = (out0, out1) of row g, then of row g+8, bias not
+// yet added; every lane of the quad holds the sums.
+__device__ __forceinline__ void out2_layer(const float (&acc)[NTILE][4], const float* __restrict__ w, int q,
+                                           float (&r)[4]) {
+  r[0] = r[1] = r[2] = r[3] = 0.0f;
+#pragma unroll
+  for (int nt = 0; nt < NTILE; ++nt) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int n = nt * 8 + 2 * q + e;
+      const float wm = w[n], ws = w[HID + n];
+      r[0] = __fmaf_rn(acc[nt][e], wm, r[0]);
+      r[1] = __fmaf_rn(acc[nt][e], ws, r[1]);
+      r[2] = __fmaf_rn(acc[nt][2 + e], wm, r[2]);
+      r[3] = __fmaf_rn(acc[nt][2 + e], ws, r[3]);
+    }
+  }
+#pragma unroll
+  for (int o = 1; o <= 2; o <<= 1) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) r[i] = __fadd_rn(r[i], __shfl_xor_sync(0xffffffffu, r[i], o));
+  }
+}
+
+// D-Net's activation_G (models/DNET.py:56-60) on the raw variance channel, in torch's order: F.elu as ATen's CUDA kernel
+// evaluates it (x <= 0 ? expm1(x) : x), then + 1.0 and + 1e-10 as two fp32 additions.  NaN stays NaN.
+__device__ __forceinline__ float activation_g(float v) {
+  const float e = v <= 0.0f ? expm1f(v) : v;
+  return __fadd_rn(__fadd_rn(e, 1.0f), 1e-10f);
+}
+
 // ---- training (DESIGN §3.10, §3.13) --------------------------------------------------------------------------------
 // The accumulator fragment of rows g, g+8 (pixels x, x+8 of one image row) into a (128, H, W) map: p points at channel
 // 2q of pixel x.  Pixel x+8 is only valid when x is.

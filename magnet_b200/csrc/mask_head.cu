@@ -1,7 +1,8 @@
 // Mask head and learned upsampling of inference in one kernel (DESIGN §3.12): per 8x16 pixel tile, the ReLU of the
 // hoisted first layer, the two 128 -> 128 layers, the 128 -> 144 layer, the softmax over the 9 taps and the convex
 // combination of every prediction (upsample_depth_via_mask, MAGNET.py:15-27,111-118,172-173).  Neither a 128-channel
-// map nor the 144-channel mask leaves the SM; the full-resolution Gaussians are written once.
+// map nor the 144-channel mask leaves the SM; the full-resolution Gaussians are written once.  With one hidden layer
+// and activation_G on the upsampled second channel the same kernel is D-Net's mask head (DESIGN §3.15).
 //
 // GEMMs run on the fp16 tensor cores in the SPLIT16 scheme of the G-Net head (head_common.cuh): one shift per layer
 // for the weights (chosen by the pack), one per pixel for the activations, three products, exact descale.
@@ -42,7 +43,17 @@ constexpr size_t S_NB = (size_t)2 * HP * 4;                          // per pred
 static_assert(M_VEC + M_NVEC * 4 <= M_W1, "vectors fit before W1");
 static_assert(S_W + S_VEC + MAX_PRED * S_NB <= 227 * 1024, "one CTA per SM");
 
-size_t smem_bytes(int P) { return S_W + S_VEC + (size_t)P * S_NB; }
+// The inference pack of a mask head with NHID 128 -> 128 layers: 2 for MaGNet's (MAGNET.py:111-118, the layout above),
+// 1 for D-Net's (D_dense_depth.py:156-160).  Header shifts of W1, [W2,] W3; vectors b1, [b2,] b3; then the fragments.
+template <int NHID>
+struct MaskLayout {
+  static constexpr int NVEC = NHID * HID + NOUT;
+  static constexpr size_t W = NHID * M_LAYER + M_LAYER3;              // resident weights
+  static constexpr size_t VEC = ((NVEC * 4 + 15) / 16) * 16;
+  static constexpr size_t BYTES = M_W1 + W;
+};
+static_assert(MaskLayout<2>::W == S_W && MaskLayout<2>::VEC == S_VEC && MaskLayout<2>::BYTES == M_BYTES, "");
+static_assert(MaskLayout<1>::W + MaskLayout<1>::VEC + S_NB <= 227 * 1024, "D-Net: one prediction");
 
 struct MaskParams {
   int B, H, W, P, tiles_x, tiles_y, ntiles;
@@ -52,23 +63,26 @@ struct MaskParams {
   float* out[MAX_PRED];
 };
 
+// ACT_G: the upsampled second channel goes through D-Net's activation_G (activation_g), so out = [mu, var].
+template <int NHID, bool ACT_G>
 __global__ void __launch_bounds__(NT, 1) mask_upsample_kernel(const MaskParams p) {
+  using L = MaskLayout<NHID>;
   extern __shared__ __align__(16) unsigned char smem[];
-  uint4* wsm = reinterpret_cast<uint4*>(smem);                          // W1, W2, W3
-  float* vec = reinterpret_cast<float*>(smem + S_W);                    // b1, b2, b3
-  float* nb = reinterpret_cast<float*>(smem + S_W + S_VEC);            // [P][mu, sigma][HP]
+  uint4* wsm = reinterpret_cast<uint4*>(smem);                          // W1, [W2,] W3
+  float* vec = reinterpret_cast<float*>(smem + L::W);                   // b1, [b2,] b3
+  float* nb = reinterpret_cast<float*>(smem + L::W + L::VEC);           // [P][mu, sigma][HP]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, q = lane & 3;
   const int H = p.H, W = p.W, HW = H * W;
   {
     const uint4* src = reinterpret_cast<const uint4*>(p.weights + M_W1);
-    for (int i = tid; i < (int)(S_W / 16); i += NT) wsm[i] = __ldg(src + i);
+    for (int i = tid; i < (int)(L::W / 16); i += NT) wsm[i] = __ldg(src + i);
     const float* vs = reinterpret_cast<const float*>(p.weights + M_VEC);
-    for (int i = tid; i < M_NVEC; i += NT) vec[i] = __ldg(vs + i);
+    for (int i = tid; i < L::NVEC; i += NT) vec[i] = __ldg(vs + i);
   }
   const int* shw = reinterpret_cast<const int*>(p.weights + M_HDR);
-  const int sh_w1 = __ldg(shw + 0), sh_w2 = __ldg(shw + 1), sh_w3 = __ldg(shw + 2);
-  const uint4* w3 = wsm + 2 * M_LAYER / 16;
-  const float* b3 = vec + 2 * HID;
+  const int sh_w1 = __ldg(shw + 0), sh_w2 = NHID == 2 ? __ldg(shw + 1) : 0, sh_w3 = __ldg(shw + NHID);
+  const uint4* w3 = wsm + NHID * M_LAYER / 16;
+  const float* b3 = vec + NHID * HID;
   const float dw3 = pow2(-sh_w3);
   const int per_img = p.tiles_x * p.tiles_y;
 
@@ -104,7 +118,7 @@ __global__ void __launch_bounds__(NT, 1) mask_upsample_kernel(const MaskParams p
       }
     }
     hidden_layer(acc, wsm, vec, sh_w1, lane);
-    hidden_layer(acc, wsm + M_LAYER / 16, vec + HID, sh_w2, lane);
+    if constexpr (NHID == 2) hidden_layer(acc, wsm + M_LAYER / 16, vec + HID, sh_w2, lane);
     uint32_t ah[HID / 16][4], al[HID / 16][4];
     int sh0, sh1;
     split_rows(acc, ah, al, sh0, sh1);
@@ -161,6 +175,7 @@ __global__ void __launch_bounds__(NT, 1) mask_upsample_kernel(const MaskParams p
           for (int e = 0; e < 2; ++e) {
             if (pp == 0) convex_gaussian(w[e], tap, mu[e], sg[e]);
             else convex_combine(w[e], tap, mu[e], sg[e]);
+            if constexpr (ACT_G) sg[e] = activation_g(sg[e]);
           }
           float* op = p.out[pp] + o;
           *reinterpret_cast<float2*>(op) = make_float2(mu[0], mu[1]);
@@ -172,12 +187,13 @@ __global__ void __launch_bounds__(NT, 1) mask_upsample_kernel(const MaskParams p
 }
 
 // ---- weight pack --------------------------------------------------------------------------------------------------
-// CTA l of 3 writes the shift of layer l + 1 (W1, W2, W3): largest finite |w| mapped into [2^14, 2^15).
+// CTA l of NHID + 1 writes the shift of layer l + 1 (W1, [W2,] W3): largest finite |w| mapped into [2^14, 2^15).
+template <int NHID>
 __global__ void __launch_bounds__(1024) mask_weight_scale_kernel(const float* __restrict__ w1,
                                                                  const float* __restrict__ w2,
                                                                  const float* __restrict__ w3, int* __restrict__ shifts) {
-  const float* w = blockIdx.x == 0 ? w1 : blockIdx.x == 1 ? w2 : w3;
-  const int n = blockIdx.x == 2 ? NOUT * HID : HID * HID;
+  const float* w = blockIdx.x == 0 ? w1 : (NHID == 2 && blockIdx.x == 1) ? w2 : w3;
+  const int n = blockIdx.x == NHID ? NOUT * HID : HID * HID;
   unsigned m = 0u;
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     const unsigned u = __float_as_uint(w[i]) & 0x7fffffffu;
@@ -194,25 +210,29 @@ __global__ void __launch_bounds__(1024) mask_weight_scale_kernel(const float* __
   }
 }
 
-// One thread per 16-byte fragment of W1, W2 and W3, then the fp32 vectors.  Fragment (k step, n tile, lane):
+// One thread per 16-byte fragment of W1, [W2,] W3, then the fp32 vectors.  Fragment (k step, n tile, lane):
 // n = 8*tile + lane/4, k = 16*step + 2*(lane%4) + {0, 1, 8, 9}.
+template <int NHID>
 __global__ void __launch_bounds__(256) mask_pack_kernel(const float* __restrict__ w1, const float* __restrict__ b1,
                                                         const float* __restrict__ w2, const float* __restrict__ b2,
                                                         const float* __restrict__ w3, const float* __restrict__ b3,
                                                         unsigned char* __restrict__ dst) {
+  using L = MaskLayout<NHID>;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < M_NVEC) {
+  if (i < L::NVEC) {
     float* vec = reinterpret_cast<float*>(dst + M_VEC);
-    vec[i] = i < HID ? b1[i] : i < 2 * HID ? b2[i - HID] : b3[i - 2 * HID];
+    if constexpr (NHID == 2) vec[i] = i < HID ? b1[i] : i < 2 * HID ? b2[i - HID] : b3[i - 2 * HID];
+    else vec[i] = i < HID ? b1[i] : b3[i - HID];
   }
   const int per_layer = (int)(M_LAYER / 16);
-  if (i >= (int)(S_W / 16)) return;
-  const int layer = i < per_layer ? 0 : i < 2 * per_layer ? 1 : 2;
+  if (i >= (int)(L::W / 16)) return;
+  // the two-layer expressions as they were before the template, so that pack compiles to the same instructions
+  const int layer = NHID == 2 ? (i < per_layer ? 0 : i < 2 * per_layer ? 1 : 2) : (i < per_layer ? 0 : 1);
   const int f = i - layer * per_layer;
-  const int ntile = layer == 2 ? NTILE3 : NTILE;
+  const int ntile = layer == NHID ? NTILE3 : NTILE;
   const int lane = f & 31, nt = (f >> 5) % ntile, step = (f >> 5) / ntile;
   const int n = nt * 8 + (lane >> 2);
-  const float* w = layer == 0 ? w1 : layer == 1 ? w2 : w3;
+  const float* w = NHID == 2 ? (layer == 0 ? w1 : layer == 1 ? w2 : w3) : (layer == 0 ? w1 : w3);
   const float s = pow2(reinterpret_cast<const int*>(dst + M_HDR)[layer]);
   float v[4];
 #pragma unroll
@@ -226,25 +246,29 @@ __global__ void __launch_bounds__(256) mask_pack_kernel(const float* __restrict_
 
 size_t mask_weights_bytes() { return M_BYTES; }
 
-cudaError_t launch_mask_pack(const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
-                             const float* b3, void* dst, cudaStream_t st) {
+namespace {
+template <int NHID>
+cudaError_t launch_pack(const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
+                        const float* b3, void* dst, cudaStream_t st) {
   unsigned char* d = static_cast<unsigned char*>(dst);
-  mask_weight_scale_kernel<<<3, 1024, 0, st>>>(w1, w2, w3, reinterpret_cast<int*>(d + M_HDR));
-  const int n = (int)(S_W / 16);
-  mask_pack_kernel<<<(n + 255) / 256, 256, 0, st>>>(w1, b1, w2, b2, w3, b3, d);
+  mask_weight_scale_kernel<NHID><<<NHID + 1, 1024, 0, st>>>(w1, w2, w3, reinterpret_cast<int*>(d + M_HDR));
+  const int n = (int)(MaskLayout<NHID>::W / 16);
+  mask_pack_kernel<NHID><<<(n + 255) / 256, 256, 0, st>>>(w1, b1, w2, b2, w3, b3, d);
   return cudaGetLastError();
 }
 
-cudaError_t launch_mask_upsample(int P, int B, int H, int W, const float* pre0, const void* weights,
-                                 const float* const* pred, float* const* out, cudaStream_t st) {
+template <int NHID, bool ACT_G>
+cudaError_t launch_upsample(int P, int B, int H, int W, const float* pre0, const void* weights,
+                            const float* const* pred, float* const* out, cudaStream_t st) {
+  using L = MaskLayout<NHID>;
   static std::once_flag flags[64];
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
   cudaError_t res = cudaSuccess;
   std::call_once(flags[dev & 63], [&] {
-    res = cudaFuncSetAttribute(mask_upsample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)smem_bytes(MAX_PRED));
+    res = cudaFuncSetAttribute(mask_upsample_kernel<NHID, ACT_G>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)(L::W + L::VEC + MAX_PRED * S_NB));
   });
   if (res != cudaSuccess) return res;
   MaskParams p;
@@ -258,8 +282,33 @@ cudaError_t launch_mask_upsample(int P, int B, int H, int W, const float* pre0, 
     p.pred[i] = i < P ? pred[i] : nullptr;
     p.out[i] = i < P ? out[i] : nullptr;
   }
-  mask_upsample_kernel<<<std::min(p.ntiles, sm_count(dev)), NT, smem_bytes(P), st>>>(p);   // persistent
+  mask_upsample_kernel<NHID, ACT_G><<<std::min(p.ntiles, sm_count(dev)), NT, L::W + L::VEC + P * S_NB, st>>>(p);   // persistent
   return cudaGetLastError();
+}
+}  // namespace
+
+cudaError_t launch_mask_pack(const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
+                             const float* b3, void* dst, cudaStream_t st) {
+  return launch_pack<2>(w1, b1, w2, b2, w3, b3, dst, st);
+}
+
+cudaError_t launch_mask_upsample(int P, int B, int H, int W, const float* pre0, const void* weights,
+                                 const float* const* pred, float* const* out, cudaStream_t st) {
+  return launch_upsample<2, false>(P, B, H, W, pre0, weights, pred, out, st);
+}
+
+// D-Net's mask head (one hidden layer), its learned upsampling of the raw (mu, v) and activation_G (DESIGN §3.15):
+// `weights` is the mask-head part of the D-Net pack.
+size_t dnet_mask_weights_bytes() { return MaskLayout<1>::BYTES; }
+
+cudaError_t launch_dnet_mask_pack(const float* w1, const float* b1, const float* w3, const float* b3, void* dst,
+                                  cudaStream_t st) {
+  return launch_pack<1>(w1, b1, nullptr, nullptr, w3, b3, dst, st);
+}
+
+cudaError_t launch_dnet_upsample(int B, int H, int W, const float* pre_m, const void* weights, const float* raw,
+                                 float* out, cudaStream_t st) {
+  return launch_upsample<1, true>(1, B, H, W, pre_m, weights, &raw, &out, st);
 }
 
 // ================================================ training (DESIGN §3.13) ==========================================

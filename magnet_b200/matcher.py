@@ -261,6 +261,77 @@ def fused_mask_trains(mask_head, pre0: Optional[torch.Tensor], preds, k: int, gt
     return all(p.dtype == torch.float32 for p in params) and all(t.dtype == torch.float32 for t in tensors)
 
 
+def fused_dnet_applies(depth_head, mask_head, x_feat: torch.Tensor, k: int) -> bool:
+    """Whether ``DnetHead.forward`` runs the fused D-Net heads (``ops.dnet_depth`` / ``ops.dnet_upsample``) instead of
+    the module chain: heads with the reference's structure (``mask_head`` None when it is not run) and k == 4 when the
+    mask head is run, nothing to differentiate (grad mode off, or no requires_grad among the heads' parameters and
+    x_feat), no CUDA autocast, fp32 weights and x_feat.  The fused kernels have no backward."""
+    if ops.dnet_head_layers(depth_head, mask_head) is None:
+        return False
+    if mask_head is not None and int(k) != 4:
+        return False
+    params = list(depth_head.parameters()) + (list(mask_head.parameters()) if mask_head is not None else [])
+    if torch.is_grad_enabled() and (x_feat.requires_grad or any(p.requires_grad for p in params)):
+        return False
+    if torch.is_autocast_enabled("cuda"):
+        return False
+    return all(p.dtype == torch.float32 for p in params) and x_feat.dtype == torch.float32
+
+
+class DnetHead(nn.Module):
+    """D-Net after its trunk: the depth head and the mask head of the reference's ``Decoder``
+    (models/submodules/D_dense_depth.py:147-161,187-195) and DNET's activations (models/DNET.py:56-67), on the fused
+    kernels where ``fused_dnet_applies`` holds (DESIGN §3.15).
+
+    ``depth_head`` and ``mask_head`` have the reference's structure and names, so a reference checkpoint's
+    ``d_net.decoder.depth_head.*`` / ``d_net.decoder.mask_head.*`` entries load with that prefix stripped.
+    ``forward(x_feat)`` with x_feat (B, in_dim, h, w), the decoder's output:
+      dnet=True:  (B,2,kh,kw) [mu, var], what ``DNET(args)(img)`` returns for that trunk output;
+      dnet=False: ((B,2,h,w) [mu, sigma], x_feat), the ``DNET(args, dnet=False)`` contract, so
+                  ``nn.Sequential(trunk, DnetHead(dnet=False))`` is a ``d_net`` for ``MAGNET``.  The mask head is built
+                  (a checkpoint loads strictly) but not run.
+    Where the rule does not hold (training, autocast, other dtypes, other structures or k) the module chain runs, with
+    ``ops.convex_upsample`` and torch's elu / sqrt, and stays differentiable."""
+
+    def __init__(self, in_dim: int = 256, downsample_ratio: int = 4, dnet: bool = True):
+        super().__init__()
+        h_dim = 128
+        self.downsample_ratio, self.dnet = downsample_ratio, dnet
+        self.depth_head = nn.Sequential(
+            nn.Conv2d(in_dim, h_dim, 3, padding=1), nn.ReLU(inplace=True),
+            nn.Conv2d(h_dim, h_dim, 1), nn.ReLU(inplace=True),
+            nn.Conv2d(h_dim, 2, 1),
+        )
+        self.mask_head = nn.Sequential(
+            nn.Conv2d(in_dim, h_dim, 3, padding=1), nn.ReLU(inplace=True),
+            nn.Conv2d(h_dim, h_dim, 1), nn.ReLU(inplace=True),
+            nn.Conv2d(h_dim, 9 * downsample_ratio * downsample_ratio, 1),
+        )
+
+    @staticmethod
+    def _pre(head: nn.Sequential, x: torch.Tensor) -> torch.Tensor:
+        """The head's 3x3 convolution before its ReLU (cuDNN), the part that stays outside the fused kernels."""
+        c0 = head[0]
+        return nn.functional.conv2d(x, c0.weight, c0.bias, c0.stride, c0.padding, c0.dilation, c0.groups)
+
+    def forward(self, x_feat: torch.Tensor):
+        k = self.downsample_ratio
+        mask_head = self.mask_head if self.dnet else None
+        if fused_dnet_applies(self.depth_head, mask_head, x_feat, k):
+            packed = ops.pack_dnet_weights(self.depth_head, mask_head)
+            raw = ops.dnet_depth(self._pre(self.depth_head, x_feat), packed, sigma=not self.dnet)
+            if not self.dnet:
+                return raw, x_feat
+            return ops.dnet_upsample(self._pre(self.mask_head, x_feat), packed, raw, k)
+        depth = self.depth_head(x_feat)
+        if not self.dnet:                                   # activation_G_magnet (DNET.py:62-67)
+            mu, v = torch.split(depth, 1, dim=1)
+            return torch.cat([mu, torch.sqrt(nn.functional.elu(v) + 1.0 + 1e-10)], dim=1), x_feat
+        up = ops.convex_upsample(depth.float(), self.mask_head(x_feat).float(), k)
+        mu, v = torch.split(up, 1, dim=1)                   # activation_G (DNET.py:56-60)
+        return torch.cat([mu, nn.functional.elu(v) + 1.0 + 1e-10], dim=1)
+
+
 class MagnetHead(nn.Module):
     """G-Net + mask head + convex upsampling of the reference's ``MAGNET`` (models/MAGNET.py:100-118,
     150-175) operating on backbone outputs; D-Net / F-Net are supplied by the caller (they need

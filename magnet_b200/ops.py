@@ -770,6 +770,122 @@ def mask_upsample(pre0: torch.Tensor, packed: torch.Tensor, preds, k: int = 4) -
     return outs
 
 
+def _is_conv(c, cin, cout, ksize: int) -> bool:
+    """A biased Conv2d cout <- cin (cin None: any) with a ksize x ksize kernel, stride 1, 'same' zero padding."""
+    pad = ksize // 2
+    return (isinstance(c, torch.nn.Conv2d) and c.bias is not None and (cin is None or c.in_channels == cin)
+            and c.out_channels == cout and c.kernel_size == (ksize, ksize) and c.padding == (pad, pad)
+            and c.stride == (1, 1) and c.dilation == (1, 1) and c.groups == 1 and c.padding_mode == "zeros")
+
+
+def _dnet_chain(seq, cout):
+    """The three convolutions of Conv(*,128,3), ReLU, Conv(128,128,1), ReLU, Conv(128,cout,1), or None."""
+    hid = _lib.MAGNET_HIDDEN_CHANNELS
+    if not isinstance(seq, torch.nn.Sequential) or len(seq) != 5:
+        return None
+    if not (isinstance(seq[1], torch.nn.ReLU) and isinstance(seq[3], torch.nn.ReLU)):
+        return None
+    c0, c1, c2 = seq[0], seq[2], seq[4]
+    if not (_is_conv(c0, None, hid, 3) and _is_conv(c1, hid, hid, 1) and _is_conv(c2, hid, cout, 1)):
+        return None
+    return [c0, c1, c2]
+
+
+def dnet_head_layers(depth_head, mask_head=None):
+    """The convolutions of D-Net's heads with the reference's structure (D_dense_depth.py:148-160): depth_head =
+    Conv(*,128,3), ReLU, Conv(128,128,1), ReLU, Conv(128,2,1), and, when given, mask_head = the same with a last
+    Conv(128,144,1) (k = 4), every convolution with a bias.  -> (depth convs, mask convs or None), or None."""
+    d = _dnet_chain(depth_head, 2)
+    if d is None:
+        return None
+    if mask_head is None:
+        return d, None
+    m = _dnet_chain(mask_head, 9 * 4 * 4)
+    return None if m is None else (d, m)
+
+
+def dnet_weights_bytes(k: int = 4) -> int:
+    """Bytes of the packed D-Net weights: k = 0 the depth head alone, k = 4 both heads (0 for any other k)."""
+    return int(lib().magnet_dnet_weights_bytes(int(k)))
+
+
+def pack_dnet_weights(depth_head, mask_head=None) -> torch.Tensor:
+    """The 1x1 layers of D-Net's depth head (and, when given, its mask head) in the fused kernels' layout
+    (``dnet_depth``, ``dnet_upsample``): the 128x128 layers and the 128->144 layer split into fp16 hi/lo with one
+    power-of-two scale per layer, the 128->2 layer and every bias in fp32.  The 3x3 layers stay outside (cuDNN).  Read
+    from the modules at each call (nothing is cached).  Two launches, four with the mask head."""
+    layers = dnet_head_layers(depth_head, mask_head)
+    if layers is None:
+        raise _lib.MagnetError("not D-Net heads with the reference's structure (Conv(*,128,3), ReLU, Conv(128,128,1), "
+                               "ReLU, Conv(128,2,1); mask head: the same ending in Conv(128,144,1))")
+    (_, d1, d2), m = layers
+    k = 0 if m is None else 4
+    named = [("depth W1", d1.weight), ("depth b1", d1.bias), ("depth W2", d2.weight), ("depth b2", d2.bias)]
+    if m is not None:
+        named += [("mask W1", m[1].weight), ("mask b1", m[1].bias), ("mask W3", m[2].weight), ("mask b3", m[2].bias)]
+    with torch.no_grad():
+        ts = [_need_cuda_f32(nm, t) for nm, t in named]
+    dev = _same_device(*zip([nm for nm, _ in named], ts))
+    out = torch.empty(dnet_weights_bytes(k), device=dev, dtype=torch.uint8)
+    ptrs = [t.data_ptr() for t in ts] + [None] * (8 - len(ts))
+    with torch.cuda.device(dev):
+        check(lib().magnet_dnet_pack_weights_f32(*ptrs, k, out.data_ptr(), _stream(dev)), "magnet_dnet_pack_weights_f32")
+    return out
+
+
+def _check_dnet_packed(packed, k: int) -> None:
+    nbytes = dnet_weights_bytes(k)
+    ok = (isinstance(packed, torch.Tensor) and packed.is_cuda and packed.dtype == torch.uint8 and packed.is_contiguous()
+          and (packed.numel() == nbytes if k == 4 else packed.numel() in (nbytes, dnet_weights_bytes(4))))
+    if not ok:
+        what = "with the mask head " if k == 4 else ""
+        raise _lib.MagnetError(f"packed must be a pack_dnet_weights buffer {what}({nbytes} bytes"
+                               + (")" if k == 4 else f" or {dnet_weights_bytes(4)})"))
+
+
+def _dnet_pre(name: str, pre: torch.Tensor) -> torch.Tensor:
+    pre = _need_cuda_f32(name, pre)
+    if pre.dim() != 4 or pre.shape[1] != _lib.MAGNET_HIDDEN_CHANNELS:
+        raise _lib.MagnetError(f"{name} must be (B,{_lib.MAGNET_HIDDEN_CHANNELS},H,W), got {tuple(pre.shape)}")
+    return pre
+
+
+def dnet_depth(pre_d: torch.Tensor, packed: torch.Tensor, sigma: bool) -> torch.Tensor:
+    """D-Net's depth head after its first convolution in one kernel: pre_d (B,128,H,W) = that convolution's output
+    before its ReLU, packed = ``pack_dnet_weights(depth_head[, mask_head])`` -> (B,2,H,W): with ``sigma`` [mu, sigma] as
+    activation_G_magnet gives it (DNET.py:62-67, MaGNet's mono_gmms), else the raw [mu, v] that ``dnet_upsample``
+    reads.  Forward only."""
+    pre_d = _dnet_pre("pre_d", pre_d)
+    _check_dnet_packed(packed, 0)
+    B, _, H, W = pre_d.shape
+    dev = _same_device(("pre_d", pre_d), ("packed", packed))
+    out = torch.empty(B, 2, H, W, device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        check(lib().magnet_dnet_depth_f32(pre_d.data_ptr(), packed.data_ptr(), B, H, W, int(bool(sigma)), out.data_ptr(),
+                                          _stream(dev)), "magnet_dnet_depth_f32")
+    return out
+
+
+def dnet_upsample(pre_m: torch.Tensor, packed: torch.Tensor, raw: torch.Tensor, k: int = 4) -> torch.Tensor:
+    """D-Net's mask head after its first convolution, the learned upsampling of the raw prediction and activation_G in
+    one kernel: pre_m (B,128,H,W) = the mask head's first convolution before its ReLU, packed = ``pack_dnet_weights(
+    depth_head, mask_head)``, raw = ``dnet_depth(..., sigma=False)`` -> (B,2,4H,4W) [mu, var], what DNET(args)
+    returns (DNET.py:56-60).  The 144-channel mask is never written.  k = 4 only.  Forward only."""
+    if int(k) != 4:
+        raise _lib.MagnetError(f"the fused D-Net mask head takes k = 4 only (144 mask channels), got {k}")
+    pre_m = _dnet_pre("pre_m", pre_m)
+    _check_dnet_packed(packed, 4)
+    B, _, H, W = pre_m.shape
+    raw = _need_cuda_f32("raw", raw)
+    _expect("raw", raw, (B, 2, H, W))
+    dev = _same_device(("pre_m", pre_m), ("packed", packed), ("raw", raw))
+    out = torch.empty(B, 2, 4 * H, 4 * W, device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        check(lib().magnet_dnet_upsample_f32(pre_m.data_ptr(), packed.data_ptr(), raw.data_ptr(), B, H, W, 4,
+                                             out.data_ptr(), _stream(dev)), "magnet_dnet_upsample_f32")
+    return out
+
+
 class MaskLossTrain(torch.autograd.Function):
     """The mask head after its first convolution, the learned upsampling and MagnetLoss 'gaussian' (utils/losses.py:
     34-50) of training in one forward kernel, differentiable in pre0, W1, b1, W2, b2, W3, b3 and every prediction
@@ -1088,7 +1204,8 @@ def crop_box(crop, H: int, W: int):
 
 
 def depth_metrics(pred_or_list, gt: torch.Tensor, *, min_depth: float, max_depth: float, crop=None,
-                  up_mask: Optional[torch.Tensor] = None, k: Optional[int] = None, nearest: bool = False) -> torch.Tensor:
+                  up_mask: Optional[torch.Tensor] = None, k: Optional[int] = None, nearest: bool = False,
+                  variance: bool = False) -> torch.Tensor:
     """Per-image depth metrics of validate() (test_MaGNet.py:52-79) + utils.compute_depth_errors, on the device.
 
     pred_or_list: one prediction or a list of up to 8 sharing ``gt`` (B,1,H,W) (raw GT; values above max_depth count
@@ -1097,6 +1214,9 @@ def depth_metrics(pred_or_list, gt: torch.Tensor, *, min_depth: float, max_depth
     With ``nearest=True`` (F-Net's validate(), train_FNet.py:165-193) each prediction is a (B,1,h,w) depth map with
     h <= H, w <= W, upsampled inside the kernel as F.interpolate(..., size=(H, W), mode='nearest'); there is no
     variance and the nll column is 0.0, as compute_depth_errors(..., var=None) gives it.
+    With ``variance=True`` (D-Net's validate(), test_DNet.py:22-73) each prediction is the full-resolution (B,2,H,W)
+    [mu, var] that D-Net returns: channel 1 is the variance itself, clamped at 1e-6, not squared.  It does not combine
+    with ``nearest`` or ``up_mask`` / ``k``.
     crop: None, 'garg' or 'eigen'.  Returns a (P,B,13) float64 device tensor: the number of valid pixels, then the
     metrics in METRIC_KEYS order (NaN for an image without a valid pixel; nll 0.0 there in the nearest form).  Two
     kernel launches, no host sync."""
@@ -1105,6 +1225,9 @@ def depth_metrics(pred_or_list, gt: torch.Tensor, *, min_depth: float, max_depth
         raise _lib.MagnetError(f"1 to {_lib.MAGNET_METRICS_MAX_PRED} predictions per call, got {len(preds)}")
     if nearest and (up_mask is not None or k is not None):
         raise _lib.MagnetError("nearest=True takes (B,1,h,w) depth maps: it does not combine with up_mask / k")
+    if variance and (nearest or up_mask is not None or k is not None):
+        raise _lib.MagnetError("variance=True takes full-resolution (B,2,H,W) [mu, var]: it does not combine with "
+                               "nearest or up_mask / k")
     gt = _need_cuda_f32("gt", gt)
     if gt.dim() != 4 or gt.shape[1] != 1:
         raise _lib.MagnetError(f"gt must be (B,1,H,W), got {tuple(gt.shape)}")
@@ -1138,8 +1261,9 @@ def depth_metrics(pred_or_list, gt: torch.Tensor, *, min_depth: float, max_depth
     workspace = torch.empty(int(n), device=dev, dtype=torch.float64)
     out = torch.empty(len(preds), B, _lib.MAGNET_METRICS_COLS, device=dev, dtype=torch.float64)
     a.workspace, a.out = workspace.data_ptr(), out.data_ptr()
+    fn = "magnet_depth_metrics_var_f32" if variance else "magnet_depth_metrics_f32"
     with torch.cuda.device(dev):
-        check(lib().magnet_depth_metrics_f32(C.byref(a), _stream(dev)), "magnet_depth_metrics_f32")
+        check(getattr(lib(), fn)(C.byref(a), _stream(dev)), fn)
     return out
 
 
