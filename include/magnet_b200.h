@@ -315,7 +315,7 @@ int magnet_gnet_update_f32(const magnet_gnet_args* args, void* stream);
  * data flow, detached cost volume) and their autograd backward into the head's weights (DESIGN §3.10).
  *
  * magnet_gnet_pack_train_weights_f32: the inference pack of magnet_gnet_pack_weights_f32 followed by W1^T and W2^T for
- * the backward, magnet_gnet_train_weights_bytes(D) bytes (0 for D outside 1..MAGNET_MAX_PLANES).  Three kernels.
+ * the backward, magnet_gnet_train_weights_bytes(D) bytes (0 for D outside 1..MAGNET_MAX_PLANES).  Two kernels.
  *
  * magnet_gnet_train_fwd_f32: the inference kernel's arithmetic (out is bit-identical to magnet_gnet_update_f32 on the
  * same inputs) plus stores of h0, h1, h2 (B,128,H,W each) and the raw (mu1, sigma1) (B,2,H,W) into `saved`
@@ -400,7 +400,7 @@ int magnet_mask_upsample_f32(const magnet_mask_upsample_args* args, void* stream
  *   var = max(sigma^2, 1e-10), mask as magnet_mask_upsample_f32 computes it (the logits are that kernel's bits).
  *
  * magnet_mask_pack_train_weights_f32: the inference pack of magnet_mask_pack_weights_f32 followed by W3^T, W2^T and W1^T
- * for the backward, magnet_mask_train_weights_bytes(4) bytes (0 for any other k).  Three kernels.
+ * for the backward, magnet_mask_train_weights_bytes(4) bytes (0 for any other k).  Two kernels.
  *
  * magnet_mask_train_fwd_f32: partial[magnet_mask_train_partials(B,H,W) x P] receives, per 8x16 tile and prediction,
  * the tile's sum of nll over its supervised full-resolution pixels (row-major [tile][p]; the caller adds them in a
@@ -471,7 +471,7 @@ int magnet_mask_bwd_f32(const magnet_mask_train_args* args, void* stream);
  * magnet_dnet_pack_weights_f32 writes both heads in the kernels' layout into `packed` (magnet_dnet_weights_bytes(k)
  * bytes, 16-byte aligned): depth head d_w1 (128, 128), d_b1 (128), d_w2 (2, 128), d_b2 (2); with k == 4 also the mask
  * head m_w1 (128, 128), m_b1 (128), m_w3 (144, 128), m_b3 (144); with k == 0 the m_* pointers are not read (may be
- * NULL).  Two kernels, four with the mask head.  magnet_dnet_weights_bytes: k == 0 the depth head alone, k == 4 both
+ * NULL).  Two kernels.  magnet_dnet_weights_bytes: k == 0 the depth head alone, k == 4 both
  * heads, 0 for any other k.
  *
  * magnet_dnet_depth_f32: pre_d (B, 128, H, W) the first depth-head convolution's output before its ReLU -> out

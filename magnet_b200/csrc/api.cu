@@ -78,7 +78,7 @@ cudaError_t launch_depth_metrics(const float* const* preds, int P, const float* 
 size_t dnet_weights_bytes(bool with_mask);
 cudaError_t launch_dnet_pack(const float* dw1, const float* db1, const float* dw2, const float* db2, const float* mw1,
                              const float* mb1, const float* mw3, const float* mb3, bool with_mask, void* dst,
-                             cudaStream_t st, int* launches);
+                             cudaStream_t st);
 cudaError_t launch_dnet_depth(int B, int H, int W, const float* pre_d, const void* weights, bool sigma, float* out,
                               cudaStream_t st);
 cudaError_t launch_dnet_upsample_packed(int B, int H, int W, const float* pre_m, const void* weights, const float* raw,
@@ -724,7 +724,7 @@ int magnet_gnet_pack_train_weights_f32(const float* w0_cost, const float* w1, co
   if (misaligned16(packed)) return MAGNET_ERR_ALIGN;
   cudaError_t e = magnet::launch_gnet_pack_train(w0_cost, w1, b1, w2, b2, w3, b3, D, packed, (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e);
-  g_launches += 3;
+  g_launches += 2;
   return MAGNET_OK;
 }
 
@@ -825,7 +825,7 @@ int magnet_mask_pack_train_weights_f32(const float* w1, const float* b1, const f
   if (misaligned16(packed)) return MAGNET_ERR_ALIGN;
   cudaError_t e = magnet::launch_mask_pack_train(w1, b1, w2, b2, w3, b3, packed, (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e);
-  g_launches += 3;
+  g_launches += 2;
   return MAGNET_OK;
 }
 
@@ -907,11 +907,10 @@ int magnet_dnet_pack_weights_f32(const float* d_w1, const float* d_b1, const flo
   if (!d_w1 || !d_b1 || !d_w2 || !d_b2 || !packed) return MAGNET_ERR_NULL;
   if (k == 4 && (!m_w1 || !m_b1 || !m_w3 || !m_b3)) return MAGNET_ERR_NULL;
   if (misaligned16(packed)) return MAGNET_ERR_ALIGN;
-  int launches = 0;
   cudaError_t e = magnet::launch_dnet_pack(d_w1, d_b1, d_w2, d_b2, m_w1, m_b1, m_w3, m_b3, k == 4, packed,
-                                           (cudaStream_t)stream, &launches);
+                                           (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(e);
-  g_launches += launches;
+  g_launches += 2;
   return MAGNET_OK;
 }
 

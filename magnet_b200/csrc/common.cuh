@@ -2,9 +2,31 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <mutex>
+
 #include "../../include/magnet_b200.h"
 
 namespace magnet {
+
+int sm_count(int dev);                                                  // cost_mma.cu
+inline size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
+
+// Opt-in shared memory (and, with max_carveout, the largest carveout): set once per (kernel, device), not on every
+// launch.  `flags` belongs to the kernel; dev, when given, receives the current device.
+template <typename K>
+cudaError_t set_smem_once(K kern, std::once_flag (&flags)[64], int bytes, bool max_carveout, int* dev = nullptr) {
+  int d = 0;
+  cudaError_t e = cudaGetDevice(&d);
+  if (e != cudaSuccess) return e;
+  if (dev) *dev = d;
+  std::call_once(flags[d & 63], [&] {
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess && max_carveout)
+      e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  });
+  return e;
+}
 
 // Kernel-side view of magnet_cost_args; k values travel in the launch parameters
 // (constant bank, uniform loads) so that no __constant__ symbol / extra copy is needed.

@@ -264,24 +264,11 @@ cost_cells_kernel(const __grid_constant__ CostParams p, const int chunk, const i
 
 static int cells_grid_x(int H, int W) { return ((W + TILE_W - 1) / TILE_W) * ((H + TILE_H - 1) / TILE_H); }
 
-// Opt-in shared memory size: set once per (kernel instantiation, device), not on every launch.
-template <typename K>
-static cudaError_t cells_attr_once(K kern, std::once_flag (&flags)[64]) {
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  cudaError_t res = cudaSuccess;
-  std::call_once(flags[dev & 63], [&] {
-    res = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cells_smem_bytes(MAGNET_MAX_PLANES));
-  });
-  return res;
-}
-
 template <int C, int MODE, bool CW, bool REUSE>
 static cudaError_t launch_cmw(const CostParams& p, cudaStream_t st) {
   static std::once_flag flags[64];
   auto kern = cost_cells_kernel<C, MODE, CW, REUSE>;
-  cudaError_t e = cells_attr_once(kern, flags);
+  cudaError_t e = set_smem_once(kern, flags, (int)cells_smem_bytes(MAGNET_MAX_PLANES), false);
   if (e != cudaSuccess) return e;
   const size_t smem = cells_smem_bytes(p.D);
   const int chunk = cells_chunk(p.D), nchunks = (p.D + chunk - 1) / chunk;

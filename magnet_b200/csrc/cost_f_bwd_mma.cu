@@ -462,7 +462,6 @@ cost_f_bwd_mma_kernel(const __grid_constant__ P p, const __grid_constant__ CUten
 // ---------------------------------------------------------------------------------------------------------------
 cudaError_t make_planes_map(CUtensorMap* tm, const void* planes, int N, int H, int W, int box_rows,
                             int nplanes);                                                              // cost_mma.cu
-int sm_count(int dev);                                                                                 // cost_mma.cu
 cudaError_t launch_score_grad(const BwdParams& p, cudaStream_t st);                                    // cost_f_bwd.cu
 
 #ifdef MAGNET_MMA_DEBUG
@@ -490,15 +489,8 @@ static cudaError_t launch_bwd_mma(const P& p, cudaStream_t st) {
   static std::once_flag flags[64];
   auto kern = cost_f_bwd_mma_kernel<P, MODE, CW, PLANES>;
   int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = set_smem_once(kern, flags, B_SMEM_TOTAL, true, &dev);
   if (e != cudaSuccess) return e;
-  cudaError_t res = cudaSuccess;
-  std::call_once(flags[dev & 63], [&] {
-    res = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, B_SMEM_TOTAL);
-    if (res == cudaSuccess)
-      res = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  });
-  if (res != cudaSuccess) return res;
   const unsigned char* refbuf = reinterpret_cast<const unsigned char*>(p.ref_feat);
   const unsigned char* srcbuf = reinterpret_cast<const unsigned char*>(p.src_feat);
   CUtensorMap tm_ref, tm_src;

@@ -923,15 +923,8 @@ static cudaError_t launch_mma_mw(const CostParams& p, cudaStream_t st) {
   static std::once_flag flags[64];
   auto kern = cost_mma_kernel<MODE, CW, PLANES>;
   int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = set_smem_once(kern, flags, M_SMEM_TOTAL, true, &dev);
   if (e != cudaSuccess) return e;
-  cudaError_t res = cudaSuccess;
-  std::call_once(flags[dev & 63], [&] {
-    res = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, M_SMEM_TOTAL);
-    if (res == cudaSuccess)
-      res = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  });
-  if (res != cudaSuccess) return res;
   const int N = p.B * p.V;
   const unsigned char* refbuf = reinterpret_cast<const unsigned char*>(p.ref_feat);
   const unsigned char* srcbuf = reinterpret_cast<const unsigned char*>(p.src_feat);

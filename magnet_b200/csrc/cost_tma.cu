@@ -643,26 +643,11 @@ static cudaError_t make_pixc_map(CUtensorMap* tm, const float* src, int N, int C
   return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
-// opt-in shared memory: once per (kernel instantiation, device), not per launch
-template <typename K>
-static cudaError_t ensure_smem_attr(K kern, std::once_flag (&flags)[64]) {
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  cudaError_t res = cudaSuccess;
-  std::call_once(flags[dev & 63], [&] {
-    res = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TMA_SMEM_TOTAL);
-    if (res == cudaSuccess)
-      res = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  });
-  return res;
-}
-
 template <int C, int MODE, bool CW>
 static cudaError_t launch_tma_cmw(const CostParams& p, cudaStream_t st) {
   static std::once_flag flags[64];
   auto kern = cost_tma_kernel<C, MODE, CW>;
-  cudaError_t e = ensure_smem_attr(kern, flags);
+  cudaError_t e = set_smem_once(kern, flags, TMA_SMEM_TOTAL, true);
   if (e != cudaSuccess) return e;
   CUtensorMap tm;
   e = make_pixc_map(&tm, p.src_feat, p.B * p.V, C, p.H, p.W);

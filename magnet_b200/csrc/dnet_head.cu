@@ -2,7 +2,7 @@
 // layer, the 128 -> 128 layer on the fp16 tensor cores (SPLIT16, as the G-Net and mask heads, head_common.cuh), ReLU,
 // and the 128 -> 2 layer on the CUDA cores (G-Net's output layer); optionally activation_G_magnet (DNET.py:62-67).
 // The 128-channel hidden map never leaves the SM.  D-Net's mask head and upsampling run in mask_head.cu's kernel with
-// one hidden layer; this file also writes the pack both kernels read.
+// one hidden layer; this file also describes the pack both kernels read.
 #include <algorithm>
 #include <mutex>
 
@@ -10,10 +10,8 @@
 
 namespace magnet {
 
-int sm_count(int dev);                                                                              // cost_mma.cu
 size_t dnet_mask_weights_bytes();                                                                   // mask_head.cu
-cudaError_t launch_dnet_mask_pack(const float* w1, const float* b1, const float* w3, const float* b3, void* dst,
-                                  cudaStream_t st);
+void add_dnet_mask_pack(HeadPack& p, const float* w1, const float* b1, const float* w3, const float* b3, size_t base);
 cudaError_t launch_dnet_upsample(int B, int H, int W, const float* pre_m, const void* weights, const float* raw,
                                  float* out, cudaStream_t st);
 
@@ -92,57 +90,12 @@ __global__ void __launch_bounds__(NT, CTAS_PER_SM) dnet_depth_kernel(const DnetP
   }
 }
 
-// CTA 0 writes the shift of the depth head's W1: largest finite |w| mapped into [2^14, 2^15) (as the mask pack).
-__global__ void __launch_bounds__(1024) dnet_weight_scale_kernel(const float* __restrict__ w1, int* __restrict__ shift) {
-  unsigned m = 0u;
-  for (int i = threadIdx.x; i < HID * HID; i += blockDim.x) {
-    const unsigned u = __float_as_uint(w1[i]) & 0x7fffffffu;
-    m = max(m, u >= 0x7f800000u ? 0u : u);
-  }
-  m = __reduce_max_sync(0xffffffffu, m);
-  __shared__ unsigned red[32];
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int i = 1; i < (int)(blockDim.x >> 5); ++i) m = max(m, red[i]);
-    m = max(m, red[0]);
-    *shift = split16_shift(m);
-  }
-}
-
-// One thread per 16-byte fragment of W1 (the mask pack's fragment order), then the fp32 vectors.
-__global__ void __launch_bounds__(256) dnet_pack_kernel(const float* __restrict__ w1, const float* __restrict__ b1,
-                                                        const float* __restrict__ w2, const float* __restrict__ b2,
-                                                        unsigned char* __restrict__ dst) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < D_NVEC) {
-    float* vec = reinterpret_cast<float*>(dst + D_VEC);
-    vec[i] = i < HID ? b1[i] : i < 3 * HID ? w2[i - HID] : b2[i - 3 * HID];
-  }
-  if (i >= (int)(D_LAYER / 16)) return;
-  const int lane = i & 31, nt = (i >> 5) % NTILE, step = (i >> 5) / NTILE;
-  const int n = nt * 8 + (lane >> 2);
-  const float s = pow2(*reinterpret_cast<const int*>(dst + D_HDR));
-  float v[4];
-#pragma unroll
-  for (int e = 0; e < 4; ++e) v[e] = w1[n * HID + step * 16 + 2 * (lane & 3) + (e & 1) + (e >> 1) * 8];
-  uint32_t h0, l0, h1, l1;
-  split2(__fmul_rn(v[0], s), __fmul_rn(v[1], s), h0, l0);
-  split2(__fmul_rn(v[2], s), __fmul_rn(v[3], s), h1, l1);
-  reinterpret_cast<uint4*>(dst + D_W1)[i] = make_uint4(h0, h1, l0, l1);
-}
-
 template <bool SIGMA>
 cudaError_t launch_depth(int B, int H, int W, const float* pre, const void* weights, float* out, cudaStream_t st) {
   static std::once_flag flags[64];
   int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = set_smem_once(dnet_depth_kernel<SIGMA>, flags, (int)S_TOTAL, false, &dev);
   if (e != cudaSuccess) return e;
-  cudaError_t res = cudaSuccess;
-  std::call_once(flags[dev & 63], [&] {
-    res = cudaFuncSetAttribute(dnet_depth_kernel<SIGMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S_TOTAL);
-  });
-  if (res != cudaSuccess) return res;
   DnetParams p;
   p.B = B; p.HW = H * W; p.gpi = (p.HW + 15) / 16; p.ngroups = B * p.gpi;
   p.pre = pre; p.weights = static_cast<const unsigned char*>(weights); p.out = out;
@@ -155,18 +108,18 @@ cudaError_t launch_depth(int B, int H, int W, const float* pre, const void* weig
 // k = 0: the depth head only; k = 4: both heads.
 size_t dnet_weights_bytes(bool with_mask) { return D_BYTES + (with_mask ? dnet_mask_weights_bytes() : 0); }
 
+// DESIGN §3.16: the depth head's W1 shift, fragments and vectors b1, W2, b2; then the mask head's pack at D_BYTES.
 cudaError_t launch_dnet_pack(const float* dw1, const float* db1, const float* dw2, const float* db2, const float* mw1,
                              const float* mb1, const float* mw3, const float* mb3, bool with_mask, void* dst,
-                             cudaStream_t st, int* launches) {
-  unsigned char* d = static_cast<unsigned char*>(dst);
-  dnet_weight_scale_kernel<<<1, 1024, 0, st>>>(dw1, reinterpret_cast<int*>(d + D_HDR));
-  const int n = (int)(D_LAYER / 16);
-  dnet_pack_kernel<<<(n + 255) / 256, 256, 0, st>>>(dw1, db1, dw2, db2, d);
-  cudaError_t e = cudaGetLastError();
-  *launches = 2;
-  if (e != cudaSuccess || !with_mask) return e;
-  *launches = 4;
-  return launch_dnet_mask_pack(mw1, mb1, mw3, mb3, d + D_BYTES, st);
+                             cudaStream_t st) {
+  HeadPack p;
+  p.add_scale(dw1, HID * HID, D_HDR);
+  p.add_frags(dw1, PACK_ROWS, HID / 16, NTILE, 0, D_HDR, D_W1);
+  p.add_vec(db1, HID, D_VEC);
+  p.add_vec(dw2, 2 * HID, D_VEC + HID * 4);
+  p.add_vec(db2, 2, D_VEC + 3 * HID * 4);
+  if (with_mask) add_dnet_mask_pack(p, mw1, mb1, mw3, mb3, D_BYTES);
+  return launch_head_pack(p, dst, st);
 }
 
 cudaError_t launch_dnet_depth(int B, int H, int W, const float* pre_d, const void* weights, bool sigma, float* out,

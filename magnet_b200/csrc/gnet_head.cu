@@ -15,7 +15,6 @@
 
 namespace magnet {
 
-int sm_count(int dev);                                                                   // cost_mma.cu
 cudaError_t launch_absmax_f32(const float* x, size_t n, unsigned* out, cudaStream_t st);  // cost_mma.cu
 
 namespace {
@@ -24,9 +23,8 @@ constexpr int HX = TX + 2, HP = (TY + 2) * HX; // the tile's 3x3 halo, 180 pixel
 constexpr int NT = 32 * TY;
 constexpr int CCH = 16;                        // cost channels staged per chunk (one K step)
 
-// Packed weight buffer (magnet_gnet_pack_weights_f32).  B fragments are stored in the order the MMA consumes them:
-// per (K step, n8 tile) 32 lanes x 16 bytes {hi(b0), hi(b1), lo(b0), lo(b1)}, so each lane loads its fragment with
-// one 16-byte load.
+// Packed weight buffer (magnet_gnet_pack_weights_f32) in the SPLIT16 pack format of head_common.cuh: each lane loads
+// its B fragment with one 16-byte load.
 constexpr size_t G_HDR = 0;                    // int32 shift of W0, W1, W2
 constexpr size_t G_VEC = 256;                  // fp32 b1[128], b2[128], W3[2][128], b3[2]
 constexpr int G_NVEC = 4 * HID + 2;
@@ -196,76 +194,27 @@ __global__ void __launch_bounds__(NT, 1) gnet_head_kernel(const GnetParams p) {
   }
 }
 
-// ---- weight pack --------------------------------------------------------------------------------------------------
-// CTA l of 3 writes the shift of layer l (W0 cost slice, W1, W2): largest finite |w| mapped into [2^14, 2^15).
-__global__ void __launch_bounds__(1024) gnet_weight_scale_kernel(const float* __restrict__ w0, int n0,
-                                                                 const float* __restrict__ w1,
-                                                                 const float* __restrict__ w2,
-                                                                 int* __restrict__ shifts) {
-  const float* w = blockIdx.x == 0 ? w0 : blockIdx.x == 1 ? w1 : w2;
-  const int n = blockIdx.x == 0 ? n0 : HID * HID;
-  unsigned m = 0u;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    const unsigned u = __float_as_uint(w[i]) & 0x7fffffffu;
-    m = max(m, u >= 0x7f800000u ? 0u : u);
-  }
-  m = __reduce_max_sync(0xffffffffu, m);
-  __shared__ unsigned red[32];
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int i = 1; i < (int)(blockDim.x >> 5); ++i) m = max(m, red[i]);
-    m = max(m, red[0]);
-    shifts[blockIdx.x] = split16_shift(m);
-  }
-}
-
-// One thread per 16-byte fragment of W1, W2 and W0 (in that order), then the fp32 vectors.  Fragment (k step, n tile,
-// lane): n = 8*tile + lane/4, k = 16*step + 2*(lane%4) + {0, 1, 8, 9}.  W0's k step is (16-channel chunk, tap).
-__global__ void __launch_bounds__(256) gnet_pack_kernel(const float* __restrict__ w0, const float* __restrict__ w1,
-                                                        const float* __restrict__ b1, const float* __restrict__ w2,
-                                                        const float* __restrict__ b2, const float* __restrict__ w3,
-                                                        const float* __restrict__ b3, int D, int n_frag,
-                                                        unsigned char* __restrict__ dst) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int* shifts = reinterpret_cast<const int*>(dst + G_HDR);
-  if (i < G_NVEC) {
-    float* vec = reinterpret_cast<float*>(dst + G_VEC);
-    vec[i] = i < HID ? b1[i] : i < 2 * HID ? b2[i - HID] : i < 4 * HID ? w3[i - 2 * HID] : b3[i - 4 * HID];
-  }
-  if (i >= n_frag) return;
-  const int per_layer = (int)(G_LAYER / 16);
-  const int layer = i < per_layer ? 1 : i < 2 * per_layer ? 2 : 0;
-  const int f = layer == 1 ? i : layer == 2 ? i - per_layer : i - 2 * per_layer;
-  const int lane = f & 31, nt = (f >> 5) % NTILE, step = (f >> 5) / NTILE;
-  const int n = nt * 8 + (lane >> 2);
-  const float s = pow2(shifts[layer]);
-  float v[4];
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    const int kk = 2 * (lane & 3) + (e & 1) + (e >> 1) * 8;            // 0,1 -> b0 ; 8,9 -> b1
-    if (layer == 0) {
-      const int cs = step / 9, tap = step - cs * 9, c = cs * CCH + kk;
-      v[e] = c < D ? w0[((size_t)n * D + c) * 9 + tap] : 0.0f;
-    } else {
-      v[e] = (layer == 1 ? w1 : w2)[n * HID + step * 16 + kk];
-    }
-  }
-  uint32_t h0, l0, h1, l1;
-  split2(__fmul_rn(v[0], s), __fmul_rn(v[1], s), h0, l0);
-  split2(__fmul_rn(v[2], s), __fmul_rn(v[3], s), h1, l1);
-  const size_t base = layer == 1 ? G_W1 : layer == 2 ? G_W2 : G_W0;
-  reinterpret_cast<uint4*>(dst + base)[f] = make_uint4(h0, h1, l0, l1);
+// ---- weight pack (DESIGN §3.16): header shifts of W0's cost slice, W1, W2; fragments of W1, W2, then W0 ----
+HeadPack gnet_pack(const float* w0, const float* w1, const float* b1, const float* w2, const float* b2,
+                   const float* w3, const float* b3, int D) {
+  HeadPack p;
+  p.add_scale(w0, HID * D * 9, G_HDR);
+  p.add_scale(w1, HID * HID, G_HDR + 4);
+  p.add_scale(w2, HID * HID, G_HDR + 8);
+  p.add_frags(w1, PACK_ROWS, HID / 16, NTILE, 0, G_HDR + 4, G_W1);
+  p.add_frags(w2, PACK_ROWS, HID / 16, NTILE, 0, G_HDR + 8, G_W2);
+  p.add_frags(w0, PACK_CONV3X3, (D + CCH - 1) / CCH * 9, NTILE, D, G_HDR, G_W0);
+  p.add_vec(b1, HID, G_VEC);
+  p.add_vec(b2, HID, G_VEC + HID * 4);
+  p.add_vec(w3, 2 * HID, G_VEC + 2 * HID * 4);
+  p.add_vec(b3, 2, G_VEC + 4 * HID * 4);
+  return p;
 }
 }  // namespace
 
 cudaError_t launch_gnet_pack(const float* w0, const float* w1, const float* b1, const float* w2, const float* b2,
                              const float* w3, const float* b3, int D, void* dst, cudaStream_t st) {
-  unsigned char* d = static_cast<unsigned char*>(dst);
-  gnet_weight_scale_kernel<<<3, 1024, 0, st>>>(w0, HID * D * 9, w1, w2, reinterpret_cast<int*>(d + G_HDR));
-  const int n_frag = (int)((gnet_weights_bytes(D) - G_W1) / 16);
-  gnet_pack_kernel<<<(n_frag + 255) / 256, 256, 0, st>>>(w0, w1, b1, w2, b2, w3, b3, D, n_frag, d);
-  return cudaGetLastError();
+  return launch_head_pack(gnet_pack(w0, w1, b1, w2, b2, w3, b3, D), dst, st);
 }
 
 namespace {
@@ -274,13 +223,8 @@ cudaError_t launch_gnet_head(int B, int D, int H, int W, const float* cost, cons
                              const float* prev, unsigned* scratch, float* out, float* save, cudaStream_t st) {
   static std::once_flag flags[64];
   int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = set_smem_once(gnet_head_kernel<SAVE>, flags, (int)S_TOTAL, false, &dev);
   if (e != cudaSuccess) return e;
-  cudaError_t res = cudaSuccess;
-  std::call_once(flags[dev & 63], [&] {
-    res = cudaFuncSetAttribute(gnet_head_kernel<SAVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S_TOTAL);
-  });
-  if (res != cudaSuccess) return res;
   if ((e = launch_absmax_f32(cost, (size_t)B * D * H * W, scratch, st)) != cudaSuccess) return e;
   GnetParams p;
   p.B = B; p.D = D; p.H = H; p.W = W;
@@ -313,7 +257,6 @@ constexpr int WG_SA = WG_M + 8, WG_SB = WG_N + 8;   // row strides = 8 mod 32 ba
 constexpr size_t WG_SMEM = (size_t)2 * WG_KS * (WG_SA + WG_SB) * 4;
 
 int wgrad_chunks(int P) { return (P + WG_KC - 1) / WG_KC; }
-size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
 }  // namespace
 
 // backward scratch: d_h2, d_h1 (B,128,H,W), d_raw (B,2,H,W), the GEMM partials (one set, reused by the four GEMMs)
@@ -324,26 +267,6 @@ size_t gnet_bwd_workspace_bytes(int B, int D, int H, int W) {
 }
 
 namespace {
-// W1^T (layer 0 of the tail) and W2^T: Bmat[k][n] = W[k][n], fragment order as gnet_pack_kernel
-__global__ void __launch_bounds__(256) gnet_pack_t_kernel(const float* __restrict__ w1, const float* __restrict__ w2,
-                                                          unsigned char* __restrict__ dst, size_t tail) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int per_layer = (int)(G_LAYER / 16);
-  if (i >= 2 * per_layer) return;
-  const int layer = i / per_layer, f = i - layer * per_layer;
-  const int lane = f & 31, nt = (f >> 5) % NTILE, step = (f >> 5) / NTILE;
-  const int n = nt * 8 + (lane >> 2);
-  const float* w = layer == 0 ? w1 : w2;
-  const float s = pow2(reinterpret_cast<const int*>(dst + G_HDR)[1 + layer]);
-  float v[4];
-#pragma unroll
-  for (int e = 0; e < 4; ++e) v[e] = w[(step * 16 + 2 * (lane & 3) + (e & 1) + (e >> 1) * 8) * HID + n];
-  uint32_t h0, l0, h1, l1;
-  split2(__fmul_rn(v[0], s), __fmul_rn(v[1], s), h0, l0);
-  split2(__fmul_rn(v[2], s), __fmul_rn(v[3], s), h1, l1);
-  reinterpret_cast<uint4*>(dst + tail)[i] = make_uint4(h0, h1, l0, l1);
-}
-
 struct GnetBwdParams {
   int B, HW, gpi, ngroups;                   // gpi: 16-pixel groups per image
   const float* __restrict__ grad;            // (B,2,H,W) gradient of the updated Gaussian
@@ -599,8 +522,12 @@ __global__ void __launch_bounds__(256) gnet_wgrad_reduce_kernel(const float* __r
   out[i] = s;
 }
 
+// opts gnet_wgrad_kernel into its shared memory first
 cudaError_t launch_wgrad(int B, int H, int W, int Ma, const float* a, int Nw, int D, bool im2col, const float* bsrc,
                          float* part, float* out_w, float* out_b, cudaStream_t st) {
+  static std::once_flag flags[64];
+  cudaError_t e = set_smem_once(gnet_wgrad_kernel, flags, (int)WG_SMEM, false);
+  if (e != cudaSuccess) return e;
   WgradParams p;
   p.HW = H * W; p.H = H; p.W = W; p.P = B * H * W; p.Ma = Ma; p.Nw = Nw; p.D = D; p.im2col = im2col ? 1 : 0;
   p.a = a; p.bsrc = bsrc;
@@ -626,25 +553,16 @@ size_t head_wgrad_partial_floats(int B, int H, int W, int Ma, int Nw) {
 
 cudaError_t launch_head_wgrad(int B, int H, int W, int Ma, const float* a, int Nw, const float* b, float* part,
                               float* out_w, float* out_b, cudaStream_t st) {
-  static std::once_flag flags[64];
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  cudaError_t res = cudaSuccess;
-  std::call_once(flags[dev & 63], [&] {
-    res = cudaFuncSetAttribute(gnet_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM);
-  });
-  if (res != cudaSuccess) return res;
   return launch_wgrad(B, H, W, Ma, a, Nw, 0, false, b, part, out_w, out_b, st);
 }
 
+// the inference pack, then W1^T and W2^T under the same shifts
 cudaError_t launch_gnet_pack_train(const float* w0, const float* w1, const float* b1, const float* w2, const float* b2,
                                    const float* w3, const float* b3, int D, void* dst, cudaStream_t st) {
-  cudaError_t e = launch_gnet_pack(w0, w1, b1, w2, b2, w3, b3, D, dst, st);
-  if (e != cudaSuccess) return e;
-  const int n = (int)(2 * G_LAYER / 16);
-  gnet_pack_t_kernel<<<(n + 255) / 256, 256, 0, st>>>(w1, w2, static_cast<unsigned char*>(dst), gnet_weights_bytes(D));
-  return cudaGetLastError();
+  HeadPack p = gnet_pack(w0, w1, b1, w2, b2, w3, b3, D);
+  p.add_frags(w1, PACK_COLS, HID / 16, NTILE, 0, G_HDR + 4, gnet_weights_bytes(D));
+  p.add_frags(w2, PACK_COLS, HID / 16, NTILE, 0, G_HDR + 8, gnet_weights_bytes(D) + G_LAYER);
+  return launch_head_pack(p, dst, st);
 }
 
 cudaError_t launch_gnet_train_fwd(int B, int D, int H, int W, const float* cost, const float* inv, const void* weights,
@@ -659,15 +577,8 @@ cudaError_t launch_gnet_bwd(int B, int D, int H, int W, const float* cost, const
                             cudaStream_t st, int* launches) {
   static std::once_flag flags[64];
   int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = set_smem_once(gnet_bwd_chain_kernel, flags, (int)(S_W12 + 2 * HID * 4), false, &dev);
   if (e != cudaSuccess) return e;
-  cudaError_t res = cudaSuccess;
-  std::call_once(flags[dev & 63], [&] {
-    res = cudaFuncSetAttribute(gnet_bwd_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S_W12 + 2 * HID * 4));
-    if (res == cudaSuccess)
-      res = cudaFuncSetAttribute(gnet_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM);
-  });
-  if (res != cudaSuccess) return res;
   const int HW = H * W;
   const size_t map = (size_t)B * HW;
   float* dh = static_cast<float*>(workspace);

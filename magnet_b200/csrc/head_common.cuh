@@ -211,4 +211,36 @@ __device__ __forceinline__ void relu_mask(float (&acc)[NTILE][4], const float* _
   }
 }
 
+// ---- the weight pack (DESIGN §3.16) --------------------------------------------------------------------------------
+// A pack is described by where each piece goes, and launch_head_pack (head_pack.cu) writes it in two launches: one CTA
+// per scale entry writes split16_shift(largest finite |w|) as an int32 at dst + shift_off; then one thread per 16-byte
+// B fragment {hi b0, hi b1, lo b0, lo b1} (K step, n8 tile, lane: n = 8 tile + lane/4, k = 16 step + 2 (lane%4) +
+// {0, 1, 8, 9}) of the fragment segments, scaled by the shift at dst + shift_off, and the fp32 vectors copied as they are.
+enum PackKind {
+  PACK_ROWS,      // W[n K + k]: a 1x1 layer (N, K)
+  PACK_COLS,      // W[k N + n]: its transpose, for the backward chains
+  PACK_CONV3X3,   // W0[(n D + c) 9 + tap], K step = 9 chunk + tap, c = 16 chunk + k % 16, zero for c >= D
+};
+struct PackScale { const float* w; int n; size_t shift_off; };
+struct PackFrags { const float* w; PackKind kind; int k_steps, n_tiles, D; size_t shift_off, dst_off; int first; };
+struct PackVec { const float* src; int n; size_t dst_off; int first; };
+
+struct HeadPack {
+  PackScale scale[3];
+  PackFrags frag[6];
+  PackVec vec[5];
+  int nscale = 0, nfrag = 0, nvec = 0, frag_total = 0, vec_total = 0;   // first: index of the segment's first thread
+
+  void add_scale(const float* w, int n, size_t shift_off) { scale[nscale++] = {w, n, shift_off}; }
+  void add_frags(const float* w, PackKind kind, int k_steps, int n_tiles, int D, size_t shift_off, size_t dst_off) {
+    frag[nfrag++] = {w, kind, k_steps, n_tiles, D, shift_off, dst_off, frag_total};
+    frag_total += k_steps * n_tiles * 32;
+  }
+  void add_vec(const float* src, int n, size_t dst_off) {
+    vec[nvec++] = {src, n, dst_off, vec_total};
+    vec_total += n;
+  }
+};
+cudaError_t launch_head_pack(const HeadPack& p, void* dst, cudaStream_t st);
+
 }  // namespace magnet

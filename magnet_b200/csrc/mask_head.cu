@@ -14,8 +14,6 @@
 
 namespace magnet {
 
-int sm_count(int dev);   // cost_mma.cu
-
 namespace {
 constexpr int K_UP = 4;                        // upsampling factor: 9 taps x 4 x 4 sub-pixels = 144 mask channels
 constexpr int NOUT = 9 * K_UP * K_UP;
@@ -25,8 +23,7 @@ constexpr int HX = TX + 2, HP = (TY + 2) * HX; // the tile's 3x3 neighbourhood, 
 constexpr int NT = 32 * TY;
 constexpr int MAX_PRED = MAGNET_MASK_MAX_PRED;
 
-// Packed weight buffer (magnet_mask_pack_weights_f32): B fragments in the order the MMA consumes them, per (K step,
-// n8 tile) 32 lanes x 16 bytes {hi(b0), hi(b1), lo(b0), lo(b1)}, as the G-Net pack.
+// Packed weight buffer (magnet_mask_pack_weights_f32) in the SPLIT16 pack format of head_common.cuh.
 constexpr size_t M_HDR = 0;                    // int32 shift of W1, W2, W3
 constexpr size_t M_VEC = 256;                  // fp32 b1[128], b2[128], b3[144]
 constexpr int M_NVEC = 2 * HID + NOUT;
@@ -186,91 +183,36 @@ __global__ void __launch_bounds__(NT, 1) mask_upsample_kernel(const MaskParams p
   }
 }
 
-// ---- weight pack --------------------------------------------------------------------------------------------------
-// CTA l of NHID + 1 writes the shift of layer l + 1 (W1, [W2,] W3): largest finite |w| mapped into [2^14, 2^15).
+// ---- weight pack (DESIGN §3.16) ----
+// The inference pack at `base` of p: header shifts of W1, [W2,] W3; fragments of W1, [W2,] W3; vectors b1, [b2,] b3.
 template <int NHID>
-__global__ void __launch_bounds__(1024) mask_weight_scale_kernel(const float* __restrict__ w1,
-                                                                 const float* __restrict__ w2,
-                                                                 const float* __restrict__ w3, int* __restrict__ shifts) {
-  const float* w = blockIdx.x == 0 ? w1 : (NHID == 2 && blockIdx.x == 1) ? w2 : w3;
-  const int n = blockIdx.x == NHID ? NOUT * HID : HID * HID;
-  unsigned m = 0u;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    const unsigned u = __float_as_uint(w[i]) & 0x7fffffffu;
-    m = max(m, u >= 0x7f800000u ? 0u : u);
+void add_pack(HeadPack& p, const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
+              const float* b3, size_t base) {
+  const float* w[2] = {w1, w2};
+  const float* b[2] = {b1, b2};
+  for (int l = 0; l < NHID; ++l) {
+    p.add_scale(w[l], HID * HID, base + M_HDR + 4 * l);
+    p.add_frags(w[l], PACK_ROWS, HID / 16, NTILE, 0, base + M_HDR + 4 * l, base + M_W1 + l * M_LAYER);
+    p.add_vec(b[l], HID, base + M_VEC + l * HID * 4);
   }
-  m = __reduce_max_sync(0xffffffffu, m);
-  __shared__ unsigned red[32];
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int i = 1; i < (int)(blockDim.x >> 5); ++i) m = max(m, red[i]);
-    m = max(m, red[0]);
-    shifts[blockIdx.x] = split16_shift(m);
-  }
-}
-
-// One thread per 16-byte fragment of W1, [W2,] W3, then the fp32 vectors.  Fragment (k step, n tile, lane):
-// n = 8*tile + lane/4, k = 16*step + 2*(lane%4) + {0, 1, 8, 9}.
-template <int NHID>
-__global__ void __launch_bounds__(256) mask_pack_kernel(const float* __restrict__ w1, const float* __restrict__ b1,
-                                                        const float* __restrict__ w2, const float* __restrict__ b2,
-                                                        const float* __restrict__ w3, const float* __restrict__ b3,
-                                                        unsigned char* __restrict__ dst) {
-  using L = MaskLayout<NHID>;
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < L::NVEC) {
-    float* vec = reinterpret_cast<float*>(dst + M_VEC);
-    if constexpr (NHID == 2) vec[i] = i < HID ? b1[i] : i < 2 * HID ? b2[i - HID] : b3[i - 2 * HID];
-    else vec[i] = i < HID ? b1[i] : b3[i - HID];
-  }
-  const int per_layer = (int)(M_LAYER / 16);
-  if (i >= (int)(L::W / 16)) return;
-  // the two-layer expressions as they were before the template, so that pack compiles to the same instructions
-  const int layer = NHID == 2 ? (i < per_layer ? 0 : i < 2 * per_layer ? 1 : 2) : (i < per_layer ? 0 : 1);
-  const int f = i - layer * per_layer;
-  const int ntile = layer == NHID ? NTILE3 : NTILE;
-  const int lane = f & 31, nt = (f >> 5) % ntile, step = (f >> 5) / ntile;
-  const int n = nt * 8 + (lane >> 2);
-  const float* w = NHID == 2 ? (layer == 0 ? w1 : layer == 1 ? w2 : w3) : (layer == 0 ? w1 : w3);
-  const float s = pow2(reinterpret_cast<const int*>(dst + M_HDR)[layer]);
-  float v[4];
-#pragma unroll
-  for (int e = 0; e < 4; ++e) v[e] = w[n * HID + step * 16 + 2 * (lane & 3) + (e & 1) + (e >> 1) * 8];
-  uint32_t h0, l0, h1, l1;
-  split2(__fmul_rn(v[0], s), __fmul_rn(v[1], s), h0, l0);
-  split2(__fmul_rn(v[2], s), __fmul_rn(v[3], s), h1, l1);
-  reinterpret_cast<uint4*>(dst + M_W1)[i] = make_uint4(h0, h1, l0, l1);
+  p.add_scale(w3, NOUT * HID, base + M_HDR + 4 * NHID);
+  p.add_frags(w3, PACK_ROWS, HID / 16, NTILE3, 0, base + M_HDR + 4 * NHID, base + M_W1 + NHID * M_LAYER);
+  p.add_vec(b3, NOUT, base + M_VEC + NHID * HID * 4);
 }
 }  // namespace
 
 size_t mask_weights_bytes() { return M_BYTES; }
 
 namespace {
-template <int NHID>
-cudaError_t launch_pack(const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
-                        const float* b3, void* dst, cudaStream_t st) {
-  unsigned char* d = static_cast<unsigned char*>(dst);
-  mask_weight_scale_kernel<NHID><<<NHID + 1, 1024, 0, st>>>(w1, w2, w3, reinterpret_cast<int*>(d + M_HDR));
-  const int n = (int)(MaskLayout<NHID>::W / 16);
-  mask_pack_kernel<NHID><<<(n + 255) / 256, 256, 0, st>>>(w1, b1, w2, b2, w3, b3, d);
-  return cudaGetLastError();
-}
-
 template <int NHID, bool ACT_G>
 cudaError_t launch_upsample(int P, int B, int H, int W, const float* pre0, const void* weights,
                             const float* const* pred, float* const* out, cudaStream_t st) {
   using L = MaskLayout<NHID>;
   static std::once_flag flags[64];
   int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = set_smem_once(mask_upsample_kernel<NHID, ACT_G>, flags, (int)(L::W + L::VEC + MAX_PRED * S_NB),
+                                false, &dev);
   if (e != cudaSuccess) return e;
-  cudaError_t res = cudaSuccess;
-  std::call_once(flags[dev & 63], [&] {
-    res = cudaFuncSetAttribute(mask_upsample_kernel<NHID, ACT_G>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)(L::W + L::VEC + MAX_PRED * S_NB));
-  });
-  if (res != cudaSuccess) return res;
   MaskParams p;
   p.B = B; p.H = H; p.W = W; p.P = P;
   p.tiles_x = (W + TX - 1) / TX;
@@ -289,7 +231,9 @@ cudaError_t launch_upsample(int P, int B, int H, int W, const float* pre0, const
 
 cudaError_t launch_mask_pack(const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
                              const float* b3, void* dst, cudaStream_t st) {
-  return launch_pack<2>(w1, b1, w2, b2, w3, b3, dst, st);
+  HeadPack p;
+  add_pack<2>(p, w1, b1, w2, b2, w3, b3, 0);
+  return launch_head_pack(p, dst, st);
 }
 
 cudaError_t launch_mask_upsample(int P, int B, int H, int W, const float* pre0, const void* weights,
@@ -301,9 +245,8 @@ cudaError_t launch_mask_upsample(int P, int B, int H, int W, const float* pre0, 
 // `weights` is the mask-head part of the D-Net pack.
 size_t dnet_mask_weights_bytes() { return MaskLayout<1>::BYTES; }
 
-cudaError_t launch_dnet_mask_pack(const float* w1, const float* b1, const float* w3, const float* b3, void* dst,
-                                  cudaStream_t st) {
-  return launch_pack<1>(w1, b1, nullptr, nullptr, w3, b3, dst, st);
+void add_dnet_mask_pack(HeadPack& p, const float* w1, const float* b1, const float* w3, const float* b3, size_t base) {
+  add_pack<1>(p, w1, b1, nullptr, nullptr, w3, b3, base);
 }
 
 cudaError_t launch_dnet_upsample(int B, int H, int W, const float* pre_m, const void* weights, const float* raw,
@@ -332,7 +275,6 @@ static_assert(S_W + S_VEC + MAX_PRED * (S_NB + S_GP) + 32 * MAX_PRED * 4 <= 227 
 static_assert(S_WT <= 227 * 1024, "W3^T, W2^T, W1^T resident");
 
 size_t smem_train(int P) { return S_W + S_VEC + (size_t)P * (S_NB + S_GP); }
-size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
 
 struct MaskTrainParams {
   int B, H, W, P, tiles_x, tiles_y, ntiles;
@@ -624,27 +566,6 @@ __global__ void __launch_bounds__(NT, 1) mask_bwd_chain_kernel(const MaskBwdPara
   }
 }
 
-// W3^T, W2^T, W1^T after the inference pack: Bmat[k][n] = W[k][n], fragment order as mask_pack_kernel
-__global__ void __launch_bounds__(256) mask_pack_t_kernel(const float* __restrict__ w1, const float* __restrict__ w2,
-                                                          const float* __restrict__ w3, unsigned char* __restrict__ dst) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int per3 = (int)(M_LAYER3T / 16), per = (int)(M_LAYER / 16);
-  if (i >= per3 + 2 * per) return;
-  const int layer = i < per3 ? 0 : i < per3 + per ? 1 : 2;            // W3^T, W2^T, W1^T
-  const int f = layer == 0 ? i : i - per3 - (layer - 1) * per;
-  const int lane = f & 31, nt = (f >> 5) % NTILE, step = (f >> 5) / NTILE;
-  const int n = nt * 8 + (lane >> 2);
-  const float* w = layer == 0 ? w3 : layer == 1 ? w2 : w1;
-  const float s = pow2(reinterpret_cast<const int*>(dst + M_HDR)[2 - layer]);
-  float v[4];
-#pragma unroll
-  for (int e = 0; e < 4; ++e) v[e] = w[(step * 16 + 2 * (lane & 3) + (e & 1) + (e >> 1) * 8) * HID + n];
-  uint32_t h0, l0, h1, l1;
-  split2(__fmul_rn(v[0], s), __fmul_rn(v[1], s), h0, l0);
-  split2(__fmul_rn(v[2], s), __fmul_rn(v[3], s), h1, l1);
-  reinterpret_cast<uint4*>(dst + M_BYTES)[i] = make_uint4(h0, h1, l0, l1);
-}
-
 // out[i] = in[i] * upstream gradient for up to 16 (in, out, n) triples, one per blockIdx.y
 struct ScaleList {
   const float* in[16];
@@ -666,13 +587,15 @@ size_t mask_bwd_workspace_bytes(int B, int H, int W) {
   return align256((size_t)2 * HID * B * H * W * 4) + head_wgrad_partial_floats(B, H, W, HID, HID) * 4;
 }
 
+// the inference pack, then W3^T (9 K steps), W2^T and W1^T under the same shifts
 cudaError_t launch_mask_pack_train(const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
                                    const float* b3, void* dst, cudaStream_t st) {
-  cudaError_t e = launch_mask_pack(w1, b1, w2, b2, w3, b3, dst, st);
-  if (e != cudaSuccess) return e;
-  const int n = (int)(S_WT / 16);
-  mask_pack_t_kernel<<<(n + 255) / 256, 256, 0, st>>>(w1, w2, w3, static_cast<unsigned char*>(dst));
-  return cudaGetLastError();
+  HeadPack p;
+  add_pack<2>(p, w1, b1, w2, b2, w3, b3, 0);
+  p.add_frags(w3, PACK_COLS, NOUT / 16, NTILE, 0, M_HDR + 8, M_BYTES);
+  p.add_frags(w2, PACK_COLS, HID / 16, NTILE, 0, M_HDR + 4, M_BYTES + M_LAYER3T);
+  p.add_frags(w1, PACK_COLS, HID / 16, NTILE, 0, M_HDR, M_BYTES + M_LAYER3T + M_LAYER);
+  return launch_head_pack(p, dst, st);
 }
 
 cudaError_t launch_mask_train_fwd(int P, int B, int H, int W, const float* pre0, const void* weights,
@@ -681,14 +604,8 @@ cudaError_t launch_mask_train_fwd(int P, int B, int H, int W, const float* pre0,
                                   cudaStream_t st, int* launches) {
   static std::once_flag flags[64];
   int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = set_smem_once(mask_train_fwd_kernel, flags, (int)smem_train(MAX_PRED), false, &dev);
   if (e != cudaSuccess) return e;
-  cudaError_t res = cudaSuccess;
-  std::call_once(flags[dev & 63], [&] {
-    res = cudaFuncSetAttribute(mask_train_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)smem_train(MAX_PRED));
-  });
-  if (res != cudaSuccess) return res;
   const size_t map = (size_t)B * H * W;
   MaskTrainParams p;
   p.B = B; p.H = H; p.W = W; p.P = P;
@@ -725,13 +642,8 @@ cudaError_t launch_mask_bwd(int P, int B, int H, int W, const void* weights, con
                             float* gw3, float* gb3, float* const* grad_pred, cudaStream_t st, int* launches) {
   static std::once_flag flags[64];
   int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = set_smem_once(mask_bwd_chain_kernel, flags, (int)S_WT, false, &dev);
   if (e != cudaSuccess) return e;
-  cudaError_t res = cudaSuccess;
-  std::call_once(flags[dev & 63], [&] {
-    res = cudaFuncSetAttribute(mask_bwd_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S_WT);
-  });
-  if (res != cudaSuccess) return res;
   const int HW = H * W;
   const size_t map = (size_t)B * HW, plane = (size_t)HID * map;
   float* dh = static_cast<float*>(workspace);

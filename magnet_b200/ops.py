@@ -813,7 +813,7 @@ def pack_dnet_weights(depth_head, mask_head=None) -> torch.Tensor:
     """The 1x1 layers of D-Net's depth head (and, when given, its mask head) in the fused kernels' layout
     (``dnet_depth``, ``dnet_upsample``): the 128x128 layers and the 128->144 layer split into fp16 hi/lo with one
     power-of-two scale per layer, the 128->2 layer and every bias in fp32.  The 3x3 layers stay outside (cuDNN).  Read
-    from the modules at each call (nothing is cached).  Two launches, four with the mask head."""
+    from the modules at each call (nothing is cached).  Two launches."""
     layers = dnet_head_layers(depth_head, mask_head)
     if layers is None:
         raise _lib.MagnetError("not D-Net heads with the reference's structure (Conv(*,128,3), ReLU, Conv(128,128,1), "

@@ -92,7 +92,7 @@ def main():
                               TF32_FLOPS),
     }
     for ev in prof.key_averages():
-        name = next((k for k in list(model) + ["gnet_wgrad_reduce_kernel", "scale_grads_kernel", "mask_pack"]
+        name = next((k for k in list(model) + ["gnet_wgrad_reduce_kernel", "scale_grads_kernel", "head_scale", "head_pack"]
                      if k in ev.key), None)
         if name is None:
             continue
