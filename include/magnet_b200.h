@@ -139,6 +139,24 @@ int magnet_cost_launch_info(const magnet_cost_args* args, int* grid_ctas, int* b
 int magnet_cost_volume_f32(const magnet_cost_args* args, void* stream);
 
 /*
+ * Cost volume, forward, with the source views read through a frame table (sequence evaluation, where consecutive
+ * references share most of their neighbours: each distinct frame is repacked once).  Everything is as in
+ * magnet_cost_volume_f32, except that args->src_feat (and args->src_gmm, and the Gaussians inside PIXC / SPLIT16 /
+ * HALF16 buffers) hold n_src source images in any order, and view (b, v) reads image src_index[b*V + v] instead of
+ * v*B + b.  The cameras stay per (b, v) and the reference operands per b.
+ *   src_index: DEVICE int32 array (B, V), b*V + v order.  Every entry, also those of views with is_valid == 0, must lie
+ *              in [0, n_src): the kernels do not check them (the Python layer does, on the host, before any launch).
+ *   n_src:     images in src_feat, >= 1; a SPLIT16 / HALF16 buffer is magnet_split16_bytes(n_src, H, W) /
+ *              magnet_half16_bytes(n_src, H, W) bytes.
+ * MAGNET_ERR_NULL for a NULL src_index, MAGNET_ERR_SHAPE for n_src < 1, MAGNET_ERR_ALIGN for a misaligned src_index.
+ * Forward only: the backward entry points read view-major buffers.
+ */
+int magnet_cost_volume_indexed_f32(const magnet_cost_args* args, const int32_t* src_index, int32_t n_src, void* stream);
+/* magnet_cost_launch_info for magnet_cost_volume_indexed_f32 (the same kernels and grid; the arguments checked alike). */
+int magnet_cost_indexed_launch_info(const magnet_cost_args* args, const int32_t* src_index, int32_t n_src,
+                                    int* grid_ctas, int* block_threads, int* smem_bytes);
+
+/*
  * Backward of the plane-sweep volume (est_costvolume_F) w.r.t. both feature maps — what autograd derives for
  * homography.py:10-75 during F-Net training (train_FNet.py:95-114): through the softmax, the 1/V mean, the channel
  * dot product and grid_sample's bilinear gather (scatter-add into the source features).

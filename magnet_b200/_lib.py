@@ -49,6 +49,7 @@ EXPORTS = (
     "magnet_mask_bwd_f32",
     "magnet_dnet_weights_bytes", "magnet_dnet_pack_weights_f32", "magnet_dnet_depth_f32", "magnet_dnet_upsample_f32",
     "magnet_depth_metrics_var_f32",
+    "magnet_cost_volume_indexed_f32", "magnet_cost_indexed_launch_info",
 )
 MAGNET_HIDDEN_CHANNELS = 128
 MAGNET_GNET_SCRATCH_BYTES = 16
@@ -166,6 +167,11 @@ def lib() -> C.CDLL:
     L.magnet_cost_launch_info.argtypes = [C.POINTER(CostArgs), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.magnet_cost_volume_f32.restype = C.c_int
     L.magnet_cost_volume_f32.argtypes = [C.POINTER(CostArgs), C.c_void_p]
+    L.magnet_cost_volume_indexed_f32.restype = C.c_int
+    L.magnet_cost_volume_indexed_f32.argtypes = [C.POINTER(CostArgs), C.c_void_p, C.c_int32, C.c_void_p]
+    L.magnet_cost_indexed_launch_info.restype = C.c_int
+    L.magnet_cost_indexed_launch_info.argtypes = [C.POINTER(CostArgs), C.c_void_p, C.c_int32, C.POINTER(C.c_int),
+                                                  C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.magnet_cost_volume_f_bwd_f32.restype = C.c_int
     L.magnet_cost_volume_f_bwd_f32.argtypes = [C.POINTER(CostFBwdArgs), C.c_void_p]
     L.magnet_cost_volume_bwd_f32.restype = C.c_int

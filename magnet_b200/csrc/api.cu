@@ -8,14 +8,17 @@
 
 namespace magnet {
 cudaError_t launch_cost_direct(const CostParams& p, int depth_mode, int src_layout, int C, bool cw,
-                               bool softmax, cudaStream_t st, int* launches);
-cudaError_t launch_cost_cells(const CostParams& p, int mode, int C, bool cw, bool reuse, cudaStream_t st);
+                               bool softmax, const int32_t* src_index, cudaStream_t st, int* launches);
+cudaError_t launch_cost_cells(const CostParams& p, int mode, int C, bool cw, bool reuse, const int32_t* src_index,
+                              cudaStream_t st);
 cudaError_t launch_softmax_planes(float* vol, int B, int D, int HW, cudaStream_t st);
 bool cells_supports(int C, int D, int layout);
-cudaError_t launch_cost_tma(const CostParams& p, int mode, int C, bool cw, cudaStream_t st);
+cudaError_t launch_cost_tma(const CostParams& p, int mode, int C, bool cw, const int32_t* src_index, int n_src,
+                            cudaStream_t st);
 bool tma_supports(int C, int D, int V, int layout);
 void tma_launch_info(int B, int H, int W, int D, int* grid, int* block, int* smem);
-cudaError_t launch_cost_mma(const CostParams& p, int mode, bool cw, int layout, cudaStream_t st);
+cudaError_t launch_cost_mma(const CostParams& p, int mode, bool cw, int layout, const int32_t* src_index, int n_src,
+                            cudaStream_t st);
 bool mma_supports(int C, int D, int V, int layout);
 void mma_launch_info(int B, int H, int W, int D, int* grid, int* block, int* smem);
 size_t split16_buffer_bytes(int N, int H, int W);
@@ -186,6 +189,71 @@ bool use_tma(const magnet_cost_args* a) {                  // the PIXC layout is
 bool use_mma(const magnet_cost_args* a) {                  // SPLIT16 / HALF16 are served by the tensor-core kernel only
   return packed_layout(a->src_layout) && magnet::mma_supports(a->C, a->D, a->V, a->src_layout);
 }
+
+// The frame table of an indexed forward: a (B, V) device array over n_src >= 1 source images.  Its entries are read
+// by the kernels only; the caller guarantees that each lies in [0, n_src).
+int validate_index(const int32_t* src_index, int32_t n_src) {
+  if (!src_index) return MAGNET_ERR_NULL;
+  if (n_src < 1) return MAGNET_ERR_SHAPE;
+  if (reinterpret_cast<uintptr_t>(src_index) % 4 != 0) return MAGNET_ERR_ALIGN;
+  return MAGNET_OK;
+}
+
+int launch_info(const magnet_cost_args* a, int* grid_ctas, int* block_threads, int* smem_bytes) {
+  if (!grid_ctas || !block_threads || !smem_bytes) return MAGNET_ERR_NULL;
+  if (use_mma(a)) {
+    magnet::mma_launch_info(a->B, a->H, a->W, a->D, grid_ctas, block_threads, smem_bytes);
+  } else if (use_tma(a)) {
+    magnet::tma_launch_info(a->B, a->H, a->W, a->D, grid_ctas, block_threads, smem_bytes);
+  } else if (use_cells(a)) {
+    magnet::cells_launch_info(a->B, a->H, a->W, a->D, grid_ctas, block_threads, smem_bytes);
+  } else {
+    *grid_ctas = ((a->H * a->W + 127) / 128) * a->D * a->B;
+    *block_threads = 128;
+    *smem_bytes = 0;
+  }
+  return MAGNET_OK;
+}
+
+// One cost-volume forward of validated arguments: view (b, v) reads source image v*B + b (src_index NULL) or
+// src_index[b*V + v] of n_src images.
+int run_cost(const magnet_cost_args* a, const int32_t* src_index, int n_src, void* stream) {
+  magnet::CostParams p;
+  p.B = a->B; p.V = a->V; p.D = a->D; p.H = a->H; p.W = a->W; p.HW = a->H * a->W;
+  p.kappa = a->kappa;
+  p.vf = (float)a->V;
+  p.inv_v_exact = ((a->V & (a->V - 1)) == 0) ? 1.0f / (float)a->V : 0.0f;
+  p.ref_feat = a->ref_feat; p.src_feat = a->src_feat; p.src_gmm = a->src_gmm; p.rays = a->rays;
+  p.cams = a->cams; p.d_volume = a->d_volume; p.ref_gmm = a->ref_gmm; p.out = a->out;
+  for (int j = 0; j < MAGNET_MAX_PLANES; ++j)
+    p.k[j] = (a->depth_mode != MAGNET_DEPTH_VOLUME && j < a->D) ? a->k_host[j] : 0.0f;
+  p.k_sorted = 1;
+  for (int j = 1; j < a->D; ++j)
+    if (!(p.k[j] >= p.k[j - 1])) p.k_sorted = 0;
+  int launches = 0;
+  cudaError_t e;
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (use_mma(a) || use_tma(a) || use_cells(a)) {
+    if (use_mma(a))
+      e = magnet::launch_cost_mma(p, a->depth_mode, a->consistency != 0, a->src_layout, src_index, n_src, st);
+    else if (use_tma(a))
+      e = magnet::launch_cost_tma(p, a->depth_mode, a->C, a->consistency != 0, src_index, n_src, st);
+    else
+      e = magnet::launch_cost_cells(p, a->depth_mode, a->C, a->consistency != 0,
+                                    a->variant != MAGNET_VARIANT_CELLS_NOREUSE, src_index, st);
+    launches = 1;
+    if (e == cudaSuccess && a->softmax) {          // homography.py:46, in place on the 1/V-averaged scores
+      e = magnet::launch_softmax_planes(a->out, a->B, a->D, a->H * a->W, st);
+      launches = 2;
+    }
+  } else {
+    e = magnet::launch_cost_direct(p, a->depth_mode, a->src_layout, a->C, a->consistency != 0, a->softmax != 0,
+                                   src_index, st, &launches);
+  }
+  if (e != cudaSuccess) return cuda_fail(e);
+  g_launches += launches;
+  return MAGNET_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -211,58 +279,28 @@ uint64_t magnet_launch_count(void) { return g_launches.load(); }
 int magnet_cost_launch_info(const magnet_cost_args* a, int* grid_ctas, int* block_threads, int* smem_bytes) {
   const int st = validate_cost(a);
   if (st != MAGNET_OK) return st;
-  if (!grid_ctas || !block_threads || !smem_bytes) return MAGNET_ERR_NULL;
-  if (use_mma(a)) {
-    magnet::mma_launch_info(a->B, a->H, a->W, a->D, grid_ctas, block_threads, smem_bytes);
-  } else if (use_tma(a)) {
-    magnet::tma_launch_info(a->B, a->H, a->W, a->D, grid_ctas, block_threads, smem_bytes);
-  } else if (use_cells(a)) {
-    magnet::cells_launch_info(a->B, a->H, a->W, a->D, grid_ctas, block_threads, smem_bytes);
-  } else {
-    *grid_ctas = ((a->H * a->W + 127) / 128) * a->D * a->B;
-    *block_threads = 128;
-    *smem_bytes = 0;
-  }
-  return MAGNET_OK;
+  return launch_info(a, grid_ctas, block_threads, smem_bytes);
 }
 
 int magnet_cost_volume_f32(const magnet_cost_args* a, void* stream) {
   const int st = validate_cost(a);
   if (st != MAGNET_OK) return st;
-  magnet::CostParams p;
-  p.B = a->B; p.V = a->V; p.D = a->D; p.H = a->H; p.W = a->W; p.HW = a->H * a->W;
-  p.kappa = a->kappa;
-  p.vf = (float)a->V;
-  p.inv_v_exact = ((a->V & (a->V - 1)) == 0) ? 1.0f / (float)a->V : 0.0f;
-  p.ref_feat = a->ref_feat; p.src_feat = a->src_feat; p.src_gmm = a->src_gmm; p.rays = a->rays;
-  p.cams = a->cams; p.d_volume = a->d_volume; p.ref_gmm = a->ref_gmm; p.out = a->out;
-  for (int j = 0; j < MAGNET_MAX_PLANES; ++j)
-    p.k[j] = (a->depth_mode != MAGNET_DEPTH_VOLUME && j < a->D) ? a->k_host[j] : 0.0f;
-  p.k_sorted = 1;
-  for (int j = 1; j < a->D; ++j)
-    if (!(p.k[j] >= p.k[j - 1])) p.k_sorted = 0;
-  int launches = 0;
-  cudaError_t e;
-  if (use_mma(a) || use_tma(a) || use_cells(a)) {
-    if (use_mma(a))
-      e = magnet::launch_cost_mma(p, a->depth_mode, a->consistency != 0, a->src_layout, (cudaStream_t)stream);
-    else if (use_tma(a))
-      e = magnet::launch_cost_tma(p, a->depth_mode, a->C, a->consistency != 0, (cudaStream_t)stream);
-    else
-      e = magnet::launch_cost_cells(p, a->depth_mode, a->C, a->consistency != 0,
-                                    a->variant != MAGNET_VARIANT_CELLS_NOREUSE, (cudaStream_t)stream);
-    launches = 1;
-    if (e == cudaSuccess && a->softmax) {          // homography.py:46, in place on the 1/V-averaged scores
-      e = magnet::launch_softmax_planes(a->out, a->B, a->D, a->H * a->W, (cudaStream_t)stream);
-      launches = 2;
-    }
-  } else {
-    e = magnet::launch_cost_direct(p, a->depth_mode, a->src_layout, a->C, a->consistency != 0, a->softmax != 0,
-                                   (cudaStream_t)stream, &launches);
-  }
-  if (e != cudaSuccess) return cuda_fail(e);
-  g_launches += launches;
-  return MAGNET_OK;
+  return run_cost(a, nullptr, 0, stream);
+}
+
+int magnet_cost_indexed_launch_info(const magnet_cost_args* a, const int32_t* src_index, int32_t n_src, int* grid_ctas,
+                                    int* block_threads, int* smem_bytes) {
+  int st = validate_cost(a);
+  if (st == MAGNET_OK) st = validate_index(src_index, n_src);
+  if (st != MAGNET_OK) return st;
+  return launch_info(a, grid_ctas, block_threads, smem_bytes);
+}
+
+int magnet_cost_volume_indexed_f32(const magnet_cost_args* a, const int32_t* src_index, int32_t n_src, void* stream) {
+  int st = validate_cost(a);
+  if (st == MAGNET_OK) st = validate_index(src_index, n_src);
+  if (st != MAGNET_OK) return st;
+  return run_cost(a, src_index, n_src, stream);
 }
 
 int magnet_cost_volume_f_bwd_f32(const magnet_cost_f_bwd_args* b, void* stream) {

@@ -47,6 +47,15 @@ struct CostParams {
   float k[MAGNET_MAX_PLANES];
 };
 
+// Source image of view (b, v) of a cost-volume forward: the view-major slot v*B + b (homography.py:105), or with IDX
+// the entry b*V + v of the caller's frame table (magnet_cost_volume_indexed_f32).  IDX is a template flag, so the
+// view-major instantiations compile to the code they had before the table existed.
+template <bool IDX>
+__device__ __forceinline__ int src_image(const int32_t* __restrict__ src_index, int b, int v, int B, int V) {
+  if constexpr (IDX) return __ldg(src_index + b * V + v);
+  else return v * B + b;
+}
+
 // Kernel-side arguments of the F-volume backward (magnet_cost_f_bwd_args + the geometry of its forward call).
 struct BwdParams {
   int B, V, D, C, H, W, HW;

@@ -71,9 +71,10 @@ static_assert(JCHUNK <= 32, "the cell start mask of a chunk is one 32-bit word")
 #ifndef MAGNET_MIN_CTAS
 #define MAGNET_MIN_CTAS 3   // 168 registers: more tap loads in flight per thread beats a 4th resident CTA
 #endif
-template <int C, int MODE, bool CW, bool REUSE>
+template <int C, int MODE, bool CW, bool REUSE, bool IDX>
 __global__ void __launch_bounds__(NT, MAGNET_MIN_CTAS)
-cost_cells_kernel(const __grid_constant__ CostParams p, const int chunk, const int grid_chunks) {
+cost_cells_kernel(const __grid_constant__ CostParams p, const int chunk, const int grid_chunks,
+                  const int32_t* __restrict__ src_index) {
   extern __shared__ float4 smem4[];
   float4* rec = smem4;                                                   // [NCELL][3][NT]
   float2* hdr = reinterpret_cast<float2*>(smem4 + NCELL * 3 * NT);       // [NCELL][NT]
@@ -134,7 +135,7 @@ cost_cells_kernel(const __grid_constant__ CostParams p, const int chunk, const i
     const float q0 = __fmaf_rn(cam->A[2], r2, __fmaf_rn(cam->A[1], r1, __fmul_rn(cam->A[0], r0)));
     const float q1 = __fmaf_rn(cam->A[5], r2, __fmaf_rn(cam->A[4], r1, __fmul_rn(cam->A[3], r0)));
     const float q2 = __fmaf_rn(cam->A[8], r2, __fmaf_rn(cam->A[7], r1, __fmul_rn(cam->A[6], r0)));
-    const int vb = v * p.B + b;
+    const int vb = src_image<IDX>(src_index, b, v, p.B, p.V);
     const float4* src_img = reinterpret_cast<const float4*>(p.src_feat) + (size_t)vb * img_stride4;
     const float* gm = CW ? p.src_gmm + (size_t)vb * 2 * HW : nullptr;
 
@@ -264,33 +265,39 @@ cost_cells_kernel(const __grid_constant__ CostParams p, const int chunk, const i
 
 static int cells_grid_x(int H, int W) { return ((W + TILE_W - 1) / TILE_W) * ((H + TILE_H - 1) / TILE_H); }
 
-template <int C, int MODE, bool CW, bool REUSE>
-static cudaError_t launch_cmw(const CostParams& p, cudaStream_t st) {
+template <int C, int MODE, bool CW, bool REUSE, bool IDX>
+static cudaError_t launch_cmwi(const CostParams& p, const int32_t* src_index, cudaStream_t st) {
   static std::once_flag flags[64];
-  auto kern = cost_cells_kernel<C, MODE, CW, REUSE>;
+  auto kern = cost_cells_kernel<C, MODE, CW, REUSE, IDX>;
   cudaError_t e = set_smem_once(kern, flags, (int)cells_smem_bytes(MAGNET_MAX_PLANES), false);
   if (e != cudaSuccess) return e;
   const size_t smem = cells_smem_bytes(p.D);
   const int chunk = cells_chunk(p.D), nchunks = (p.D + chunk - 1) / chunk;
   dim3 grid(cells_grid_x(p.H, p.W) * nchunks, p.B), block(NT);
-  kern<<<grid, block, smem, st>>>(p, chunk, nchunks);
+  kern<<<grid, block, smem, st>>>(p, chunk, nchunks, src_index);
   return cudaGetLastError();
 }
 
+template <int C, int MODE, bool CW, bool REUSE>
+static cudaError_t launch_cmw(const CostParams& p, const int32_t* src_index, cudaStream_t st) {
+  return src_index ? launch_cmwi<C, MODE, CW, REUSE, true>(p, src_index, st)
+                   : launch_cmwi<C, MODE, CW, REUSE, false>(p, nullptr, st);
+}
+
 template <int C, int MODE, bool REUSE>
-static cudaError_t launch_cm(const CostParams& p, bool cw, cudaStream_t st) {
-  return cw ? launch_cmw<C, MODE, true, REUSE>(p, st) : launch_cmw<C, MODE, false, REUSE>(p, st);
+static cudaError_t launch_cm(const CostParams& p, bool cw, const int32_t* src_index, cudaStream_t st) {
+  return cw ? launch_cmw<C, MODE, true, REUSE>(p, src_index, st) : launch_cmw<C, MODE, false, REUSE>(p, src_index, st);
 }
 
 template <int C>
-static cudaError_t launch_c(const CostParams& p, int mode, bool cw, bool reuse, cudaStream_t st) {
+static cudaError_t launch_c(const CostParams& p, int mode, bool cw, bool reuse, const int32_t* src_index, cudaStream_t st) {
   if (!reuse) {   // diagnostic variant: only the bench configuration is instantiated
-    if (mode == MAGNET_DEPTH_GAUSS) return launch_cm<C, MAGNET_DEPTH_GAUSS, false>(p, cw, st);
+    if (mode == MAGNET_DEPTH_GAUSS) return launch_cm<C, MAGNET_DEPTH_GAUSS, false>(p, cw, src_index, st);
     return cudaErrorInvalidValue;
   }
-  if (mode == MAGNET_DEPTH_VOLUME) return launch_cm<C, MAGNET_DEPTH_VOLUME, true>(p, cw, st);
-  if (mode == MAGNET_DEPTH_GAUSS) return launch_cm<C, MAGNET_DEPTH_GAUSS, true>(p, cw, st);
-  return launch_cm<C, MAGNET_DEPTH_PLANES, true>(p, cw, st);
+  if (mode == MAGNET_DEPTH_VOLUME) return launch_cm<C, MAGNET_DEPTH_VOLUME, true>(p, cw, src_index, st);
+  if (mode == MAGNET_DEPTH_GAUSS) return launch_cm<C, MAGNET_DEPTH_GAUSS, true>(p, cw, src_index, st);
+  return launch_cm<C, MAGNET_DEPTH_PLANES, true>(p, cw, src_index, st);
 }
 
 bool cells_supports(int C, int D, int layout) {
@@ -304,11 +311,12 @@ void cells_launch_info(int B, int H, int W, int D, int* grid, int* block, int* s
   *smem = (int)cells_smem_bytes(D);
 }
 
-cudaError_t launch_cost_cells(const CostParams& p, int mode, int C, bool cw, bool reuse, cudaStream_t st) {
+cudaError_t launch_cost_cells(const CostParams& p, int mode, int C, bool cw, bool reuse, const int32_t* src_index,
+                              cudaStream_t st) {
   switch (C) {
-    case 16: return launch_c<16>(p, mode, cw, reuse, st);
-    case 32: return launch_c<32>(p, mode, cw, reuse, st);
-    case 64: return launch_c<64>(p, mode, cw, reuse, st);
+    case 16: return launch_c<16>(p, mode, cw, reuse, src_index, st);
+    case 32: return launch_c<32>(p, mode, cw, reuse, src_index, st);
+    case 64: return launch_c<64>(p, mode, cw, reuse, src_index, st);
     default: return cudaErrorInvalidValue;
   }
 }

@@ -12,9 +12,10 @@
 
 namespace magnet {
 
-template <bool CW>
+template <bool CW, bool IDX>
 __global__ void __launch_bounds__(128)
-cost_direct_kernel(const CostParams p, const int depth_mode, const int src_layout, const int C) {
+cost_direct_kernel(const CostParams p, const int depth_mode, const int src_layout, const int C,
+                   const int32_t* __restrict__ src_index) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= p.HW) return;
   const int j = blockIdx.y, b = blockIdx.z;
@@ -70,7 +71,7 @@ cost_direct_kernel(const CostParams p, const int depth_mode, const int src_layou
     const bool in_ne = x1 >= 0 && x1 < W && y0 >= 0 && y0 < H;
     const bool in_sw = x0 >= 0 && x0 < W && y1 >= 0 && y1 < H;
     const bool in_se = x1 >= 0 && x1 < W && y1 >= 0 && y1 < H;
-    const int vb = v * p.B + b;                                   // view-major (homography.py:105)
+    const int vb = src_image<IDX>(src_index, b, v, p.B, p.V);    // view-major (homography.py:105) or the frame table
     float cost = 0.0f;
     if (in_nw | in_ne | in_sw | in_se) {
       if (src_layout == MAGNET_SRC_NCHW) {
@@ -144,10 +145,15 @@ cudaError_t launch_softmax_planes(float* vol, int B, int D, int HW, cudaStream_t
 }
 
 cudaError_t launch_cost_direct(const CostParams& p, int depth_mode, int src_layout, int C, bool cw,
-                               bool softmax, cudaStream_t st, int* launches) {
+                               bool softmax, const int32_t* src_index, cudaStream_t st, int* launches) {
   dim3 grid((p.HW + 127) / 128, p.D, p.B), block(128);
-  if (cw) cost_direct_kernel<true><<<grid, block, 0, st>>>(p, depth_mode, src_layout, C);
-  else cost_direct_kernel<false><<<grid, block, 0, st>>>(p, depth_mode, src_layout, C);
+  if (src_index) {
+    if (cw) cost_direct_kernel<true, true><<<grid, block, 0, st>>>(p, depth_mode, src_layout, C, src_index);
+    else cost_direct_kernel<false, true><<<grid, block, 0, st>>>(p, depth_mode, src_layout, C, src_index);
+  } else {
+    if (cw) cost_direct_kernel<true, false><<<grid, block, 0, st>>>(p, depth_mode, src_layout, C, nullptr);
+    else cost_direct_kernel<false, false><<<grid, block, 0, st>>>(p, depth_mode, src_layout, C, nullptr);
+  }
   *launches = 1;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;

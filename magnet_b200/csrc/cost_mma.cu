@@ -134,11 +134,11 @@ enum { PROF_SETUP, PROF_BOX, PROF_TMA, PROF_MMA, PROF_PHASEC, PROF_EPI, PROF_NST
 #endif
 
 // PLANES = 2: MAGNET_SRC_SPLIT16 (hi / lo), 1: MAGNET_SRC_HALF16 (one plane, the hi*hi product only)
-template <int MODE, bool CW, int PLANES>
+template <int MODE, bool CW, int PLANES, bool IDX>
 __global__ void __launch_bounds__(MNT, 2)
 cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CUtensorMap tm_ref,
                 const __grid_constant__ CUtensorMap tm_src, const __grid_constant__ CUtensorMap tm_meta, const int nchunks,
-                const int n_items, const int slot, float* __restrict__ dbg) {
+                const int n_items, const int slot, float* __restrict__ dbg, const int32_t* __restrict__ src_index) {
   extern __shared__ unsigned char smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t padb = (1024u - (raw & 1023u)) & 1023u;
@@ -371,7 +371,7 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
       pixt[2 * lane + 1] = make_float4(cam->a[1], ms.x, ms.y, cam->a[2]);
     }
     __syncwarp();
-    const int vb = v * p.B + b;
+    const int vb = src_image<IDX>(src_index, b, v, p.B, V);
     // sample position of my two hypotheses of pixel i of the row, clamped: anything left of -1 / right of W (above /
     // below likewise) has all four taps out of the image, so cells stay near the image and NaN (fmaxf drops it) maps to
     // "out of bounds"; z = depth in the source camera
@@ -918,14 +918,14 @@ static float* g_mma_dbg = nullptr;
 void mma_set_debug_buffer(float* p) { g_mma_dbg = p; }
 #endif
 
-template <int MODE, bool CW, int PLANES>
-static cudaError_t launch_mma_mw(const CostParams& p, cudaStream_t st) {
+template <int MODE, bool CW, int PLANES, bool IDX>
+static cudaError_t launch_mma_mwi(const CostParams& p, const int32_t* src_index, int n_src, cudaStream_t st) {
   static std::once_flag flags[64];
-  auto kern = cost_mma_kernel<MODE, CW, PLANES>;
+  auto kern = cost_mma_kernel<MODE, CW, PLANES, IDX>;
   int dev = 0;
   cudaError_t e = set_smem_once(kern, flags, M_SMEM_TOTAL, true, &dev);
   if (e != cudaSuccess) return e;
-  const int N = p.B * p.V;
+  const int N = IDX ? n_src : p.B * p.V;               // source images in the buffer
   const unsigned char* refbuf = reinterpret_cast<const unsigned char*>(p.ref_feat);
   const unsigned char* srcbuf = reinterpret_cast<const unsigned char*>(p.src_feat);
   CUtensorMap tm_ref, tm_src, tm_meta;
@@ -949,8 +949,14 @@ static cudaError_t launch_mma_mw(const CostParams& p, cudaStream_t st) {
 #if defined(MAGNET_MMA_DEBUG) || defined(MAGNET_MMA_PROFILE)
   dbg = g_mma_dbg;
 #endif
-  kern<<<grid, block, M_SMEM_TOTAL, st>>>(p, tm_ref, tm_src, tm_meta, nchunks, n_items, slot, dbg);
+  kern<<<grid, block, M_SMEM_TOTAL, st>>>(p, tm_ref, tm_src, tm_meta, nchunks, n_items, slot, dbg, src_index);
   return cudaGetLastError();
+}
+
+template <int MODE, bool CW, int PLANES>
+static cudaError_t launch_mma_mw(const CostParams& p, const int32_t* src_index, int n_src, cudaStream_t st) {
+  return src_index ? launch_mma_mwi<MODE, CW, PLANES, true>(p, src_index, n_src, st)
+                   : launch_mma_mwi<MODE, CW, PLANES, false>(p, nullptr, 0, st);
 }
 
 bool mma_supports(int C, int D, int V, int layout) {
@@ -969,21 +975,24 @@ size_t split16_buffer_bytes(int N, int H, int W) { return split16_bytes((size_t)
 size_t half16_buffer_bytes(int N, int H, int W) { return half16_bytes((size_t)N, (size_t)H, (size_t)W); }
 
 template <int PLANES>
-static cudaError_t launch_cost_mma_planes(const CostParams& p, int mode, bool cw, cudaStream_t st) {
+static cudaError_t launch_cost_mma_planes(const CostParams& p, int mode, bool cw, const int32_t* si, int n_src,
+                                          cudaStream_t st) {
   if (cw) {
-    if (mode == MAGNET_DEPTH_VOLUME) return launch_mma_mw<MAGNET_DEPTH_VOLUME, true, PLANES>(p, st);
-    if (mode == MAGNET_DEPTH_GAUSS) return launch_mma_mw<MAGNET_DEPTH_GAUSS, true, PLANES>(p, st);
-    return launch_mma_mw<MAGNET_DEPTH_PLANES, true, PLANES>(p, st);
+    if (mode == MAGNET_DEPTH_VOLUME) return launch_mma_mw<MAGNET_DEPTH_VOLUME, true, PLANES>(p, si, n_src, st);
+    if (mode == MAGNET_DEPTH_GAUSS) return launch_mma_mw<MAGNET_DEPTH_GAUSS, true, PLANES>(p, si, n_src, st);
+    return launch_mma_mw<MAGNET_DEPTH_PLANES, true, PLANES>(p, si, n_src, st);
   }
-  if (mode == MAGNET_DEPTH_VOLUME) return launch_mma_mw<MAGNET_DEPTH_VOLUME, false, PLANES>(p, st);
-  if (mode == MAGNET_DEPTH_GAUSS) return launch_mma_mw<MAGNET_DEPTH_GAUSS, false, PLANES>(p, st);
-  return launch_mma_mw<MAGNET_DEPTH_PLANES, false, PLANES>(p, st);
+  if (mode == MAGNET_DEPTH_VOLUME) return launch_mma_mw<MAGNET_DEPTH_VOLUME, false, PLANES>(p, si, n_src, st);
+  if (mode == MAGNET_DEPTH_GAUSS) return launch_mma_mw<MAGNET_DEPTH_GAUSS, false, PLANES>(p, si, n_src, st);
+  return launch_mma_mw<MAGNET_DEPTH_PLANES, false, PLANES>(p, si, n_src, st);
 }
 
-// layout: MAGNET_SRC_SPLIT16 (hi / lo planes) or MAGNET_SRC_HALF16 (one plane)
-cudaError_t launch_cost_mma(const CostParams& p, int mode, bool cw, int layout, cudaStream_t st) {
-  if (layout == MAGNET_SRC_HALF16) return launch_cost_mma_planes<1>(p, mode, cw, st);
-  return launch_cost_mma_planes<2>(p, mode, cw, st);
+// layout: MAGNET_SRC_SPLIT16 (hi / lo planes) or MAGNET_SRC_HALF16 (one plane); src_index: NULL (view-major source
+// images, V*B of them) or the (B, V) frame table over n_src images
+cudaError_t launch_cost_mma(const CostParams& p, int mode, bool cw, int layout, const int32_t* src_index, int n_src,
+                            cudaStream_t st) {
+  if (layout == MAGNET_SRC_HALF16) return launch_cost_mma_planes<1>(p, mode, cw, src_index, n_src, st);
+  return launch_cost_mma_planes<2>(p, mode, cw, src_index, n_src, st);
 }
 
 }  // namespace magnet

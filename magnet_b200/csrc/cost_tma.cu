@@ -397,10 +397,10 @@ __device__ __forceinline__ void phase_c(const ViewGeom& g, float4* __restrict__ 
   }
 }
 
-template <int C, int MODE, bool CW>
+template <int C, int MODE, bool CW, bool IDX>
 __global__ void __launch_bounds__(TNT, 2)
 cost_tma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CUtensorMap tmap, const int win_cap,
-                const int nchunks) {
+                const int nchunks, const int32_t* __restrict__ src_index) {
   constexpr int QL = C / 16;
   constexpr int PS = pix_floats(C) * 4;
   constexpr int BOX = tma_box_bytes(C);
@@ -494,7 +494,7 @@ cost_tma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
     g.q0 = __fmaf_rn(cam->A[2], r2, __fmaf_rn(cam->A[1], r1, __fmul_rn(cam->A[0], r0)));
     g.q1 = __fmaf_rn(cam->A[5], r2, __fmaf_rn(cam->A[4], r1, __fmul_rn(cam->A[3], r0)));
     g.q2 = __fmaf_rn(cam->A[8], r2, __fmaf_rn(cam->A[7], r1, __fmul_rn(cam->A[6], r0)));
-    const int vb = v * p.B + b;
+    const int vb = src_image<IDX>(src_index, b, v, p.B, V);
     const unsigned char* img = reinterpret_cast<const unsigned char*>(p.src_feat) + (size_t)vb * HW * PS + h * QL * 16;
 
     // ---------------- phase A + bounding box of the CTA's cells ---------------------------------------------
@@ -643,14 +643,14 @@ static cudaError_t make_pixc_map(CUtensorMap* tm, const float* src, int N, int C
   return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
-template <int C, int MODE, bool CW>
-static cudaError_t launch_tma_cmw(const CostParams& p, cudaStream_t st) {
+template <int C, int MODE, bool CW, bool IDX>
+static cudaError_t launch_tma_cmwi(const CostParams& p, const int32_t* src_index, int n_src, cudaStream_t st) {
   static std::once_flag flags[64];
-  auto kern = cost_tma_kernel<C, MODE, CW>;
+  auto kern = cost_tma_kernel<C, MODE, CW, IDX>;
   cudaError_t e = set_smem_once(kern, flags, TMA_SMEM_TOTAL, true);
   if (e != cudaSuccess) return e;
   CUtensorMap tm;
-  e = make_pixc_map(&tm, p.src_feat, p.B * p.V, C, p.H, p.W);
+  e = make_pixc_map(&tm, p.src_feat, IDX ? n_src : p.B * p.V, C, p.H, p.W);
   if (e != cudaSuccess) return e;
   const int nchunks = (p.D + TCH - 1) / TCH;
   const int tiles = ((p.W + TTW - 1) / TTW) * ((p.H + TTH - 1) / TTH);
@@ -660,20 +660,26 @@ static cudaError_t launch_tma_cmw(const CostParams& p, cudaStream_t st) {
 #else
   const int cap = tma_win_cap(C);
 #endif
-  kern<<<grid, block, TMA_SMEM_TOTAL, st>>>(p, tm, cap, nchunks);
+  kern<<<grid, block, TMA_SMEM_TOTAL, st>>>(p, tm, cap, nchunks, src_index);
   return cudaGetLastError();
 }
 
+template <int C, int MODE, bool CW>
+static cudaError_t launch_tma_cmw(const CostParams& p, const int32_t* src_index, int n_src, cudaStream_t st) {
+  return src_index ? launch_tma_cmwi<C, MODE, CW, true>(p, src_index, n_src, st)
+                   : launch_tma_cmwi<C, MODE, CW, false>(p, nullptr, 0, st);
+}
+
 template <int C>
-static cudaError_t launch_tma_c(const CostParams& p, int mode, bool cw, cudaStream_t st) {
+static cudaError_t launch_tma_c(const CostParams& p, int mode, bool cw, const int32_t* si, int n_src, cudaStream_t st) {
   if (cw) {
-    if (mode == MAGNET_DEPTH_VOLUME) return launch_tma_cmw<C, MAGNET_DEPTH_VOLUME, true>(p, st);
-    if (mode == MAGNET_DEPTH_GAUSS) return launch_tma_cmw<C, MAGNET_DEPTH_GAUSS, true>(p, st);
-    return launch_tma_cmw<C, MAGNET_DEPTH_PLANES, true>(p, st);
+    if (mode == MAGNET_DEPTH_VOLUME) return launch_tma_cmw<C, MAGNET_DEPTH_VOLUME, true>(p, si, n_src, st);
+    if (mode == MAGNET_DEPTH_GAUSS) return launch_tma_cmw<C, MAGNET_DEPTH_GAUSS, true>(p, si, n_src, st);
+    return launch_tma_cmw<C, MAGNET_DEPTH_PLANES, true>(p, si, n_src, st);
   }
-  if (mode == MAGNET_DEPTH_VOLUME) return launch_tma_cmw<C, MAGNET_DEPTH_VOLUME, false>(p, st);
-  if (mode == MAGNET_DEPTH_GAUSS) return launch_tma_cmw<C, MAGNET_DEPTH_GAUSS, false>(p, st);
-  return launch_tma_cmw<C, MAGNET_DEPTH_PLANES, false>(p, st);
+  if (mode == MAGNET_DEPTH_VOLUME) return launch_tma_cmw<C, MAGNET_DEPTH_VOLUME, false>(p, si, n_src, st);
+  if (mode == MAGNET_DEPTH_GAUSS) return launch_tma_cmw<C, MAGNET_DEPTH_GAUSS, false>(p, si, n_src, st);
+  return launch_tma_cmw<C, MAGNET_DEPTH_PLANES, false>(p, si, n_src, st);
 }
 
 bool tma_supports(int C, int D, int V, int layout) {
@@ -686,11 +692,13 @@ void tma_launch_info(int B, int H, int W, int D, int* grid, int* block, int* sme
   *smem = TMA_SMEM_TOTAL;
 }
 
-cudaError_t launch_cost_tma(const CostParams& p, int mode, int C, bool cw, cudaStream_t st) {
+// src_index: NULL (view-major source images, V*B of them) or the (B, V) frame table over n_src images
+cudaError_t launch_cost_tma(const CostParams& p, int mode, int C, bool cw, const int32_t* src_index, int n_src,
+                            cudaStream_t st) {
   switch (C) {
-    case 16: return launch_tma_c<16>(p, mode, cw, st);
-    case 32: return launch_tma_c<32>(p, mode, cw, st);
-    case 64: return launch_tma_c<64>(p, mode, cw, st);
+    case 16: return launch_tma_c<16>(p, mode, cw, src_index, n_src, st);
+    case 32: return launch_tma_c<32>(p, mode, cw, src_index, n_src, st);
+    case 64: return launch_tma_c<64>(p, mode, cw, src_index, n_src, st);
     default: return cudaErrorInvalidValue;
   }
 }

@@ -72,19 +72,33 @@ class MatchingPlan:
     AUTO keeps the global-gather kernel where the drop-in would take the TMA-staged one); a layout is packed on first
     use.  The feature maps may be fp16 / bf16 (torch.autocast): of one half dtype, they go to the single-plane HALF16
     layout wherever the fp32 maps would go to SPLIT16; every other layout reads their fp32 upcast (made once).  The
-    Gaussians are upcast; volumes are fp32."""
+    Gaussians are upcast; volumes are fp32.
 
-    def __init__(self, ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, *, thres: int = 5):
+    With ``src_index`` (B, V), an int32 / int64 frame table on the CPU or the device, ``nghbr_feat`` / ``nghbr_gmms``
+    are per-frame maps (S, C, H, W) / (S, 2, H, W) and view (b, v) reads frame ``src_index[b, v]`` (views with
+    is_valid == 0 too: fill them with any frame).  The frames the table names are packed once each, and ``cost()`` runs
+    the indexed forward (magnet_cost_volume_indexed_f32) of whatever layout ``route`` picks; its volume equals, bit for
+    bit, the one of a plan over the view-major gather ``nghbr_feat[src_index.T.flatten()]``.  Forward only: the table is
+    refused when grad mode is on and a feature map, a Gaussian or a camera tensor requires grad."""
+
+    def __init__(self, ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, *, thres: int = 5,
+                 src_index: Optional[torch.Tensor] = None):
+        if src_index is not None:
+            src_index = self._check_indexed(ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, cam_intrins, src_index)
         if torch.is_grad_enabled() and not geometry_grad_enabled():
             check_geometry_grad(nghbr_poses=nghbr_poses, intM=cam_intrins['intM'],
                                 unit_ray_array_2D=cam_intrins['unit_ray_array_2D'])
         # the caller's camera tensors: a plan built under geometry_grad() is differentiable in them on every cost()
         # call, wherever that call runs (the switch is latched here); a plan built outside never is
         self._cam_in = camera_inputs(nghbr_poses[:, :, :3, :3], nghbr_poses[:, :, :3, 3], cam_intrins) \
-            if geometry_grad_enabled() else (None,) * 4
+            if geometry_grad_enabled() and src_index is None else (None,) * 4
         dev = ref_feat.device
         self.B, self.C, self.H, self.W = ref_feat.shape
         self.V = nghbr_feat.shape[0] // self.B
+        self.src_index = None
+        if src_index is not None:
+            self.V = src_index.shape[1]
+            nghbr_feat, nghbr_gmms, self.src_index = self._source_frames(nghbr_feat, nghbr_gmms, src_index, dev)
         self.kappa = float(thres)
         self.ref_feat = ref_feat.detach().contiguous()
         self.src_gmm = nghbr_gmms.detach().float().contiguous()
@@ -97,6 +111,50 @@ class MatchingPlan:
         self._ref_in, self._src_in = ref_feat, nghbr_feat   # the caller's tensors: cost() is differentiable in them
         self._packed = {}
         self._ref_split = None
+
+    @staticmethod
+    def _check_indexed(ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, cam_intrins, src_index) -> None:
+        """The checks of an indexed plan, all before any launch: no gradient is asked of it, the per-frame maps agree
+        and the table is (B, V) over their S frames.  Returns the table on the host."""
+        if torch.is_grad_enabled():
+            named = dict(ref_feat=ref_feat, nghbr_feat=nghbr_feat, nghbr_gmms=nghbr_gmms, nghbr_poses=nghbr_poses,
+                         intM=cam_intrins['intM'], unit_ray_array_2D=cam_intrins['unit_ray_array_2D'])
+            for name, x in named.items():
+                if isinstance(x, torch.Tensor) and x.requires_grad:
+                    raise _lib.MagnetError(f"{name} requires grad, but a plan with a frame table (src_index) is forward "
+                                           "only: detach it, or use the view-major maps without src_index")
+        B = ref_feat.shape[0]
+        if nghbr_feat.dim() != 4 or tuple(nghbr_feat.shape[1:]) != tuple(ref_feat.shape[1:]):
+            raise _lib.MagnetError(f"with src_index, nghbr_feat must be per-frame maps (S, {', '.join(map(str, ref_feat.shape[1:]))}),"
+                                   f" got {tuple(nghbr_feat.shape)}")
+        S = nghbr_feat.shape[0]
+        if tuple(nghbr_gmms.shape) != (S, 2, *ref_feat.shape[2:]):
+            raise _lib.MagnetError(f"with src_index, nghbr_gmms must be (S, 2, H, W) = {(S, 2, *ref_feat.shape[2:])} "
+                                   f"like nghbr_feat, got {tuple(nghbr_gmms.shape)}")
+        V = src_index.shape[1] if isinstance(src_index, torch.Tensor) and src_index.dim() == 2 else -1
+        ops.check_src_index(src_index, B, V, S, check_range=False)
+        if tuple(nghbr_poses.shape[:2]) != (B, V):
+            raise _lib.MagnetError(f"nghbr_poses must be (B, V, 4, 4) = {(B, V, 4, 4)} like src_index, got "
+                                   f"{tuple(nghbr_poses.shape)}")
+        host = src_index.cpu()
+        ops.check_src_index(host, B, V, S)                 # the range, on the host
+        return host
+
+    @staticmethod
+    def _source_frames(nghbr_feat, nghbr_gmms, src_index, dev):
+        """(source maps, their Gaussians, device table) of an indexed plan: the U distinct frames the table names, in
+        frame order, and the table renumbered over them.  When every frame is named (a sequence, where every frame is
+        some reference's source) the maps are taken as they are, else the U frames are gathered first."""
+        idx = src_index.to(torch.int64)
+        used = torch.unique(idx)
+        S = nghbr_feat.shape[0]
+        if used.numel() < S:
+            pos = torch.full((S,), -1, dtype=torch.int64)
+            pos[used] = torch.arange(used.numel())
+            idx = pos[idx]
+            sel = used.to(nghbr_feat.device)
+            nghbr_feat, nghbr_gmms = nghbr_feat.index_select(0, sel), nghbr_gmms.index_select(0, sel)
+        return nghbr_feat, nghbr_gmms, idx.to(torch.int32).to(dev, non_blocking=True)
 
     def _fp32(self, which: str) -> torch.Tensor:
         """The reference ('ref') or source ('src') features in fp32: the plan's own when they are fp32, else their
@@ -126,6 +184,8 @@ class MatchingPlan:
         otherwise."""
         gmm = gmm.float()                                  # differentiable upcast (a no-op for fp32)
         grad = wants_cw_grad(gmm, self._ref_in, self._src_in, *self._cam_in)
+        if grad and self.src_index is not None:
+            raise _lib.MagnetError("gmm requires grad, but a plan with a frame table (src_index) is forward only")
         if grad:
             if out is not None:
                 raise _lib.MagnetError("cost(out=...) writes into a caller buffer and cannot be differentiated")
@@ -138,7 +198,8 @@ class MatchingPlan:
             packed = layout in PACKED_LAYOUTS
             vol = ops.cost_volume(self._ref_operand(layout), src, self.rays, self.cams, V=self.V, src_layout=layout,
                                   consistency=True, src_gmm=self.src_gmm, kappa=self.kappa, ref_gmm=gmm.detach(),
-                                  k=k, out=out, variant=fv, ref_split=self._ref_split if packed else None)
+                                  k=k, out=out, variant=fv, ref_split=self._ref_split if packed else None,
+                                  src_index=self.src_index, check_index=False)
             return vol, layout, fv, (self._ref_split, src) if packed else None
 
         if grad:
@@ -372,11 +433,14 @@ class MagnetHead(nn.Module):
         c0 = self.mask_head[0]
         return nn.functional.conv2d(x_d3, c0.weight, c0.bias, c0.stride, c0.padding, c0.dilation, c0.groups)
 
-    def forward(self, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins):
+    def forward(self, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins,
+                src_index=None):
+        """The N_iter upsampled predictions.  With ``src_index`` (B, V) the source maps are per-frame (S, ...) and view
+        (b, v) reads frame ``src_index[b, v]`` (``MatchingPlan``); None: view-major maps of V*B images."""
         k = self.downsample_ratio
         if self.fused_upsample:
             preds = self._predictions(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid,
-                                      cam_intrins)
+                                      cam_intrins, src_index)
             if fused_mask_applies(self.mask_head, None, preds, k):
                 pre0 = self.mask_pre(x_d3)
                 if fused_mask_applies(self.mask_head, pre0, preds, k):
@@ -384,20 +448,24 @@ class MagnetHead(nn.Module):
             mask = self.mask_head(x_d3).float()
         else:
             preds, mask = self.forward_quarter(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid,
-                                               cam_intrins)
+                                               cam_intrins, src_index)
         return [self.upsample(pr, mask, k) for pr in preds]
 
-    def _predictions(self, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins):
-        plan = MatchingPlan(ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, thres=self.thres)
+    def _predictions(self, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins,
+                     src_index=None):
+        plan = MatchingPlan(ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, thres=self.thres,
+                            src_index=src_index)
         preds = matching_loop(plan, ref_gmms, x_d3, self.g_net, self.n_iter, self.k_list, detach_cost=self.detach_cost,
                               fused_train=self.fused_train)
         return preds[1:]
 
-    def forward_quarter(self, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins):
+    def forward_quarter(self, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins,
+                        src_index=None):
         """The N_iter quarter-resolution predictions and the upsampling mask, NOT upsampled: what the fused
         upsample + NLL loss (``loss`` below) consumes during training.  Under torch.autocast every input may be half;
-        the predictions and the mask are fp32."""
-        preds = self._predictions(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins)
+        the predictions and the mask are fp32.  ``src_index`` as in ``forward``."""
+        preds = self._predictions(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid, cam_intrins,
+                                  src_index)
         return preds, self.mask_head(x_d3).float()
 
     def loss(self, preds_quarter, mask, gt_depth, gt_depth_mask, gamma: float = 0.8):
@@ -466,6 +534,111 @@ class MAGNET(nn.Module):
         self.head.n_iter = self.train_iter if mode == 'train' else self.test_iter
         return self.head(feat[:B], feat[B:], mono_gmms[:B].detach(), mono_gmms[B:].detach(), x_d3[:B], nghbr_poses,
                          is_valid, cam_intrins)
+
+    def forward_frames(self, imgs, ref_index, src_index, nghbr_poses, is_valid, cam_intrins, mode='test'):
+        """``forward`` over a set of distinct frames: ``imgs`` (S,3,H,W) holds each frame once, ``ref_index`` (B,) names
+        the reference of each sample and ``src_index`` (B, V) its neighbours (int32 / int64, on the CPU or the device;
+        views with is_valid == 0 name any frame).  The backbones run once per frame, under ``no_grad``; the matching
+        reads the sources through the table, so each source frame is also packed once.  Returns what ``forward``
+        returns for the gathered batch ``ref_img = imgs[ref_index]``, ``nghbr_imgs = imgs[src_index.T.flatten()]``
+        (view-major).  Forward only."""
+        S = imgs.shape[0]
+        ref_index = self._frame_index(ref_index, S, imgs.device)
+        with torch.no_grad():
+            mono_gmms, x_d3 = self.d_net(imgs)
+            feat = self.f_net(imgs)
+        return self.forward_sources(feat.index_select(0, ref_index), mono_gmms.index_select(0, ref_index),
+                                    x_d3.index_select(0, ref_index), feat, mono_gmms, src_index, nghbr_poses, is_valid,
+                                    cam_intrins, mode)
+
+    def forward_sources(self, ref_feat, ref_gmms, x_d3, src_feat, src_gmms, src_index, nghbr_poses, is_valid,
+                        cam_intrins, mode='test'):
+        """The head of ``forward_frames`` on backbone outputs already at hand: the B references' F-Net features,
+        mono Gaussians and x_d3, and per-frame source features / Gaussians (S, ...) read through ``src_index`` (B, V)."""
+        self.head.n_iter = self.train_iter if mode == 'train' else self.test_iter
+        return self.head(ref_feat, src_feat, ref_gmms.detach(), src_gmms.detach(), x_d3, nghbr_poses, is_valid,
+                         cam_intrins, src_index=src_index)
+
+    @staticmethod
+    def _frame_index(index, S: int, device) -> torch.Tensor:
+        """ref_index (B,) checked against the S frames, as an int64 device tensor."""
+        if not isinstance(index, torch.Tensor) or index.dim() != 1 or index.dtype not in (torch.int32, torch.int64):
+            raise _lib.MagnetError("ref_index must be a (B,) int32 / int64 tensor")
+        host = index.cpu()
+        if host.numel() == 0 or int(host.min()) < 0 or int(host.max()) >= S:
+            raise _lib.MagnetError(f"ref_index entries must lie in [0, {S}) (the frames of imgs)")
+        return host.to(torch.int64).to(device)
+
+
+class FrameCache:
+    """Sequence evaluation at batch 1 (the reference's test loader): ``MAGNET.forward`` for one sample at a time, with
+    each frame's backbone outputs kept on the device across samples.  In ScanNet's protocol every frame is a reference
+    once and a neighbour of up to four more samples, so the backbones run once per frame instead of about five times.
+
+    ``cache(ref_img, nghbr_imgs, nghbr_poses, is_valid, cam_intrins, ref_ids, nghbr_ids, mode='test')`` takes
+    ``forward``'s arguments plus a hashable id per image: ``ref_ids`` (B ids) and ``nghbr_ids`` (B sequences of V ids,
+    ``nghbr_ids[b][v]`` naming ``nghbr_imgs[v*B + b]``), for example ``(scene_name, img_idx)`` of each view of the
+    reference's ``data_array``.  The backbones run, in one batched call under ``no_grad``, on the ids the cache does not
+    hold; each frame keeps its (mono Gaussian, x_d3, F-Net features) on the device, ``(2 + 256 + C)·h·w`` floats
+    (24.7 MB at 120x160 with C = 64), and the least recently used frames are evicted beyond ``capacity``.  The head
+    then runs as in ``MAGNET.forward_sources``, each distinct source frame packed once.
+
+    An id must name the same image for as long as it is cached: call ``clear()`` when the backbones change (unfrozen,
+    reloaded) or the ids are reused."""
+
+    def __init__(self, model: MAGNET, capacity: int = 32):
+        if capacity < 1:
+            raise ValueError(f"capacity must be at least 1, got {capacity}")
+        from collections import OrderedDict
+        self.model, self.capacity = model, int(capacity)
+        self._frames = OrderedDict()
+        self.backbone_images = 0                           # images the backbones have run on, over the cache's life
+
+    def __len__(self) -> int:
+        return len(self._frames)
+
+    def clear(self) -> None:
+        """Drop every cached frame.  Required whenever the backbones' weights or mode change."""
+        self._frames.clear()
+
+    def __call__(self, ref_img, nghbr_imgs, nghbr_poses, is_valid, cam_intrins, ref_ids, nghbr_ids, mode='test'):
+        B = ref_img.shape[0]
+        V = nghbr_imgs.shape[0] // B
+        ref_ids = list(ref_ids)
+        nghbr_ids = [list(row) for row in nghbr_ids]
+        if len(ref_ids) != B or len(nghbr_ids) != B or any(len(row) != V for row in nghbr_ids) \
+                or nghbr_imgs.shape[0] != V * B:
+            raise _lib.MagnetError(f"ref_ids must name the {B} references and nghbr_ids hold {B} rows of {V} ids")
+        images = {}                                        # id -> image of this call, first occurrence
+        for b, fid in enumerate(ref_ids):
+            images.setdefault(fid, ref_img[b])
+        for b, row in enumerate(nghbr_ids):
+            for v, fid in enumerate(row):
+                images.setdefault(fid, nghbr_imgs[v * B + b])
+        frames = {fid: self._frames[fid] for fid in images if fid in self._frames}
+        missing = [fid for fid in images if fid not in frames]
+        if missing:
+            with torch.no_grad():
+                imgs = torch.stack([images[fid] for fid in missing])
+                mono_gmms, x_d3 = self.model.d_net(imgs)
+                feat = self.model.f_net(imgs)
+            self.backbone_images += len(missing)
+            for i, fid in enumerate(missing):              # own storage per frame, so eviction frees it
+                frames[fid] = (mono_gmms[i].clone(), x_d3[i].clone(), feat[i].clone())
+        for fid in images:
+            self._frames[fid] = frames[fid]
+            self._frames.move_to_end(fid)
+        while len(self._frames) > self.capacity:
+            self._frames.popitem(last=False)
+        src_ids = list(dict.fromkeys(fid for row in nghbr_ids for fid in row))
+        pos = {fid: i for i, fid in enumerate(src_ids)}
+        src_index = torch.tensor([[pos[fid] for fid in row] for row in nghbr_ids], dtype=torch.int32)
+        ref = [frames[fid] for fid in ref_ids]
+        src = [frames[fid] for fid in src_ids]
+        return self.model.forward_sources(torch.stack([f[2] for f in ref]), torch.stack([f[0] for f in ref]),
+                                          torch.stack([f[1] for f in ref]), torch.stack([f[2] for f in src]),
+                                          torch.stack([f[0] for f in src]), src_index, nghbr_poses, is_valid,
+                                          cam_intrins, mode)
 
 
 def sid_planes(min_depth: float, max_depth: float, n: int = 80, device=None) -> torch.Tensor:

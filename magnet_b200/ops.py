@@ -244,16 +244,62 @@ def _cost_args(ref_feat: torch.Tensor, V: int, rays, cams, *, d_volume=None, ref
     return a, gd_shape, (("rays", rays), ("cams", cams), ("d_volume", d_volume), ("ref_gmm", ref_gmm))
 
 
+def check_src_index(src_index, B: int, V: int, n_src: int, *, check_range: bool = True) -> torch.Tensor:
+    """The frame table of an indexed cost volume, checked: an int32 / int64 tensor of shape (B, V) whose entries all
+    lie in [0, n_src), the views with is_valid == 0 included (fill those with any frame of the set).  A CUDA table is
+    read back for the range check (one synchronisation; ``check_range=False`` skips it for a table checked before).
+    Returns the table as contiguous int32 on its device."""
+    if not isinstance(src_index, torch.Tensor):
+        raise TypeError("src_index must be a torch.Tensor")
+    if src_index.dtype not in (torch.int32, torch.int64):
+        raise _lib.MagnetError(f"src_index must be an int32 or int64 tensor, got {src_index.dtype}")
+    if tuple(src_index.shape) != (B, V):
+        raise _lib.MagnetError(f"src_index must have shape (B, V) = {(B, V)}, got {tuple(src_index.shape)}")
+    if n_src < 1:
+        raise _lib.MagnetError(f"an indexed cost volume needs at least one source image, got n_src={n_src}")
+    if check_range and src_index.numel():
+        lo, hi = (int(v) for v in torch.aminmax(src_index))
+        if lo < 0 or hi >= n_src:
+            raise _lib.MagnetError(f"src_index entries must lie in [0, {n_src}) (the source images), got [{lo}, {hi}]")
+    return src_index.to(torch.int32).contiguous()
+
+
+def source_images(src_layout: int, src_feat, C: int, H: int, W: int) -> int:
+    """Images in a source operand of ``src_layout`` for C channels at H x W: the leading dimension of an NCHW / TILED32 /
+    PIXC tensor, or what the size of a SPLIT16 / HALF16 buffer holds (which must be a whole number of images)."""
+    if src_layout in PACKED_LAYOUTS:
+        if not isinstance(src_feat, torch.Tensor):
+            raise TypeError("src_feat must be a torch.Tensor")
+        one = packed_bytes(src_layout, 1, H, W)
+        per = packed_bytes(src_layout, 2, H, W) - one
+        n = (src_feat.numel() - one) // per + 1
+        _check_packed("src_feat", src_feat, src_layout, max(n, 1), H, W)
+        return n
+    shape = {_lib.SRC_NCHW: (C, H, W), _lib.SRC_TILED32: (H, (W + 31) // 32, C // 4, 32, 4),
+             _lib.SRC_PIXC: (H, W, C + 4)}.get(src_layout)
+    if shape is None:
+        raise _lib.MagnetError(f"unknown src_layout {src_layout}")
+    if src_feat.dim() != 1 + len(shape) or tuple(src_feat.shape[1:]) != shape or src_feat.shape[0] < 1:
+        raise _lib.MagnetError(f"src_feat must have shape (n_src, *{shape}), got {tuple(src_feat.shape)}")
+    return int(src_feat.shape[0])
+
+
 def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tensor, cams: torch.Tensor, *,
                 V: int, src_layout: int, consistency: bool, src_gmm: Optional[torch.Tensor] = None,
                 kappa: float = 5.0, d_volume: Optional[torch.Tensor] = None,
                 ref_gmm: Optional[torch.Tensor] = None, k=None, planes: bool = False, softmax: bool = False,
                 variant: int = _lib.VARIANT_AUTO, out: Optional[torch.Tensor] = None,
-                ref_split: Optional[torch.Tensor] = None) -> torch.Tensor:
+                ref_split: Optional[torch.Tensor] = None, src_index: Optional[torch.Tensor] = None,
+                n_src: Optional[int] = None, check_index: bool = True) -> torch.Tensor:
     """One launch of magnet_cost_volume_f32.  Depth source: ``d_volume`` (drop-in), or ``ref_gmm`` + ``k``
     (fused sampler), or ``k`` with ``planes=True`` (fronto-parallel planes).  With ``src_layout=SRC_SPLIT16`` both
     ``src_feat`` and ``ref_split`` are ``repack_split16`` buffers (``ref_feat`` then only supplies the shape); with
-    ``SRC_HALF16`` both are ``repack_half16`` buffers and ``ref_feat`` (any dtype) only supplies the shape."""
+    ``SRC_HALF16`` both are ``repack_half16`` buffers and ``ref_feat`` (any dtype) only supplies the shape.
+
+    With ``src_index`` (B, V) (``check_src_index``) it is one launch of magnet_cost_volume_indexed_f32 instead:
+    ``src_feat`` (and ``src_gmm``) then hold any number of source images, each packed once, and view (b, v) reads image
+    ``src_index[b, v]``; ``n_src``, when given, must be the number of images they hold.  ``check_index=False`` skips the
+    range check of the table (the caller has checked it).  None: the view-major operands of V*B images."""
     ref_feat = _need_cuda("ref_feat", ref_feat) if src_layout == _lib.SRC_HALF16 else _need_cuda_f32("ref_feat", ref_feat)
     if src_layout not in PACKED_LAYOUTS:                   # the packed buffers are checked below, by their size
         src_feat = _need_cuda_f32("src_feat", src_feat)
@@ -262,11 +308,17 @@ def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tens
     B, Cc, H, W = ref_feat.shape
     if V <= 0:
         raise _lib.MagnetError(f"V must be positive, got {V}")
+    n_img = V * B
+    if src_index is not None:
+        n_img = source_images(src_layout, src_feat, Cc, H, W)
+        if n_src is not None and n_src != n_img:
+            raise _lib.MagnetError(f"n_src={n_src} does not match src_feat, which holds {n_img} source images")
+        src_index = check_src_index(src_index, B, V, n_img, check_range=check_index)
     # every operand against (B, V, D, C, H, W): a mismatch would read out of bounds, the reference raises instead
-    src_shape = {_lib.SRC_NCHW: (V * B, Cc, H, W), _lib.SRC_TILED32: (V * B, H, (W + 31) // 32, Cc // 4, 32, 4),
-                 _lib.SRC_PIXC: (V * B, H, W, Cc + 4)}.get(src_layout)
+    src_shape = {_lib.SRC_NCHW: (n_img, Cc, H, W), _lib.SRC_TILED32: (n_img, H, (W + 31) // 32, Cc // 4, 32, 4),
+                 _lib.SRC_PIXC: (n_img, H, W, Cc + 4)}.get(src_layout)
     if src_layout in PACKED_LAYOUTS:
-        _check_packed("src_feat", src_feat, src_layout, V * B, H, W)
+        _check_packed("src_feat", src_feat, src_layout, n_img, H, W)
         _check_packed("ref_split", ref_split, src_layout, B, H, W)
     elif src_shape is None:
         raise _lib.MagnetError(f"unknown src_layout {src_layout}")
@@ -274,7 +326,7 @@ def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tens
         _expect("src_feat", src_feat, src_shape)
     a, _, named = _cost_args(ref_feat, V, rays, cams, d_volume=d_volume, ref_gmm=ref_gmm, k=k, planes=planes)
     dev = _same_device(("ref_feat", ref_feat), ("src_feat", src_feat), ("src_gmm", src_gmm), *named, ("out", out),
-                       ("ref_split", ref_split))
+                       ("ref_split", ref_split), ("src_index", src_index))
     a.src_layout = src_layout
     a.consistency = 1 if consistency else 0
     a.softmax = 1 if softmax else 0
@@ -284,7 +336,7 @@ def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tens
     a.src_feat = src_feat.data_ptr()
     if consistency and src_layout not in (_lib.SRC_PIXC, *PACKED_LAYOUTS):   # those carry the source Gaussians inside src_feat
         src_gmm = _need_cuda_f32("src_gmm", src_gmm)
-        _expect("src_gmm", src_gmm, (V * B, 2, H, W))
+        _expect("src_gmm", src_gmm, (n_img, 2, H, W))
         a.src_gmm = src_gmm.data_ptr()
     if out is None:
         out = torch.empty(B, a.D, H, W, device=ref_feat.device, dtype=torch.float32)
@@ -293,7 +345,11 @@ def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tens
         _expect("out", out, (B, a.D, H, W))
     a.out = out.data_ptr()
     with torch.cuda.device(dev):
-        check(lib().magnet_cost_volume_f32(C.byref(a), _stream(dev)), "magnet_cost_volume_f32")
+        if src_index is None:
+            check(lib().magnet_cost_volume_f32(C.byref(a), _stream(dev)), "magnet_cost_volume_f32")
+        else:
+            check(lib().magnet_cost_volume_indexed_f32(C.byref(a), src_index.data_ptr(), n_img, _stream(dev)),
+                  "magnet_cost_volume_indexed_f32")
     return out
 
 

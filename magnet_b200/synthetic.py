@@ -191,3 +191,51 @@ def make_config(name: str, seed: int = 0, **over) -> MatchingInputs:
     kw = dict(CONFIGS[name])
     kw.update(over)
     return make_inputs(seed=seed, **kw)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Sequences (sequence evaluation, ``MAGNET.forward_frames`` / ``FrameCache``)
+
+def window_neighbours(img_idx: int, last: int, window_radius: int = 20, n_views: int = 4):
+    """The neighbour frames of reference frame ``img_idx`` in a sequence whose frames are 0..last, by the rule of the
+    reference's ScanNet loader (data/dataloader_scannet.py:157-164): offsets k * interval for k in [-n/2, n/2] \\ {0},
+    interval = window_radius // (n/2); an offset i that leaves the sequence is replaced by -i - sign(i) * (interval // 2).
+    Returns the V = n_views frame ids in the loader's order."""
+    interval = window_radius // (n_views // 2)
+    out = []
+    for k in range(-(n_views // 2), n_views // 2 + 1):
+        i = k * interval
+        if i == 0:
+            continue
+        out.append(img_idx + i if 0 <= img_idx + i <= last else img_idx - i - int(np.sign(i)) * int(interval * 0.5))
+    return out
+
+
+def scannet_sequence(n_refs: int, stride: int = 10, window_radius: int = 20, n_views: int = 4):
+    """A test sequence as ScanNet's split lists it: references every ``stride`` frames (frames 0, stride, ...,
+    (n_refs-1)*stride exist, and every frame in between), each with its ``window_neighbours``.  Returns (ref_ids,
+    nghbr_ids): n_refs frame ids and n_refs lists of V ids."""
+    last = (n_refs - 1) * stride
+    refs = [r * stride for r in range(n_refs)]
+    return refs, [window_neighbours(r, last, window_radius, n_views) for r in refs]
+
+
+def trajectory(frames, seed: int = 0, step: float = 0.004, turn_deg: float = 0.12) -> dict:
+    """Camera-to-world extrinsics (4,4) float32 of a smooth hand-held path, one per frame id in ``frames``: per frame
+    a forward-leaning translation of about ``step`` and a rotation of about ``turn_deg`` degrees, with a seeded
+    wobble.  Relative poses come from ``ops.relative_poses`` as in the reference's data_preprocess."""
+    frames = sorted(set(int(f) for f in frames))
+    rng = np.random.default_rng(seed)
+    lo, hi = frames[0], frames[-1]
+    n = hi - lo + 1
+    wob = rng.standard_normal((n, 4)).cumsum(axis=0) * 0.05
+    out = {}
+    for f in frames:
+        i = f - lo
+        yaw = np.deg2rad(turn_deg * i + 2.0 * np.sin(wob[i, 0]))
+        pitch = np.deg2rad(1.5 * np.sin(wob[i, 1]))
+        E = np.eye(4)
+        E[:3, :3] = _rot_y(yaw) @ _rot_x(pitch)
+        E[:3, 3] = [step * i * 0.3 + 0.02 * np.sin(wob[i, 2]), 0.01 * np.sin(wob[i, 3]), step * i]
+        out[f] = E.astype(np.float32)
+    return out
