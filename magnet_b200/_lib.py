@@ -26,31 +26,6 @@ VARIANT_AUTO, VARIANT_DIRECT, VARIANT_CELLS, VARIANT_CELLS_NOREUSE, VARIANT_TMA,
 MAGNET_METRICS_MAX_PRED = 8
 MAGNET_METRICS_COLS = 13
 
-# every symbol include/magnet_b200.h declares (tests check the library exports all of them)
-EXPORTS = (
-    "magnet_abi_version", "magnet_strerror", "magnet_last_cuda_error", "magnet_launch_count",
-    "magnet_cost_launch_info", "magnet_cost_volume_f32", "magnet_cost_volume_f_bwd_f32", "magnet_cost_volume_bwd_f32",
-    "magnet_pack_cameras_f32",
-    "magnet_repack_tiled32_f32", "magnet_repack_pixc_f32", "magnet_repack_split16_f32", "magnet_split16_bytes",
-    "magnet_repack_half16", "magnet_half16_bytes", "magnet_sample_depths_f32", "magnet_gaussian_update_fwd_f32",
-    "magnet_gaussian_update_bwd_f32", "magnet_convex_upsample_fwd_f32", "magnet_convex_upsample_bwd_f32",
-    "magnet_relative_poses_f32", "magnet_camera_rays_f32",
-    "magnet_upsample_nll_partials", "magnet_upsample_nll_fwd_f32", "magnet_upsample_nll_bwd_f32",
-    "magnet_fnet_l1_partials", "magnet_fnet_l1_fwd_f32", "magnet_fnet_l1_bwd_f32",
-    "magnet_depth_metrics_workspace", "magnet_depth_metrics_f32",
-    "magnet_plane_depth_f32", "magnet_depth_metrics_nearest_workspace", "magnet_depth_metrics_nearest_f32",
-    "magnet_gnet_weights_bytes", "magnet_gnet_pack_weights_f32", "magnet_gnet_update_f32",
-    "magnet_gnet_train_weights_bytes", "magnet_gnet_saved_bytes", "magnet_gnet_bwd_workspace_bytes",
-    "magnet_gnet_pack_train_weights_f32", "magnet_gnet_train_fwd_f32", "magnet_gnet_bwd_f32",
-    "magnet_cost_geom_workspace_bytes", "magnet_cost_volume_geom_bwd_f32",
-    "magnet_mask_weights_bytes", "magnet_mask_pack_weights_f32", "magnet_mask_upsample_f32",
-    "magnet_mask_train_weights_bytes", "magnet_mask_saved_bytes", "magnet_mask_bwd_workspace_bytes",
-    "magnet_mask_train_partials", "magnet_mask_pack_train_weights_f32", "magnet_mask_train_fwd_f32",
-    "magnet_mask_bwd_f32",
-    "magnet_dnet_weights_bytes", "magnet_dnet_pack_weights_f32", "magnet_dnet_depth_f32", "magnet_dnet_upsample_f32",
-    "magnet_depth_metrics_var_f32",
-    "magnet_cost_volume_indexed_f32", "magnet_cost_indexed_launch_info",
-)
 MAGNET_HIDDEN_CHANNELS = 128
 MAGNET_GNET_SCRATCH_BYTES = 16
 MAGNET_MASK_MAX_PRED = 8
@@ -138,6 +113,76 @@ class MaskTrainArgs(C.Structure):
         ("grad_pred", C.POINTER(C.c_void_p))]
 
 
+_P, _I32, _I64, _F32, _SZ, _ST = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_size_t, C.c_int
+_OUT = C.POINTER(C.c_int)
+
+# (restype, argtypes) of every symbol include/magnet_b200.h declares; `lib()` checks the library exports each one
+SIGNATURES = {
+    "magnet_abi_version": (C.c_int, []),
+    "magnet_strerror": (C.c_char_p, [C.c_int]),
+    "magnet_last_cuda_error": (C.c_char_p, []),
+    "magnet_launch_count": (C.c_uint64, []),
+    "magnet_cost_launch_info": (_ST, [C.POINTER(CostArgs), _OUT, _OUT, _OUT]),
+    "magnet_cost_volume_f32": (_ST, [C.POINTER(CostArgs), _P]),
+    "magnet_cost_volume_indexed_f32": (_ST, [C.POINTER(CostArgs), _P, _I32, _P]),
+    "magnet_cost_indexed_launch_info": (_ST, [C.POINTER(CostArgs), _P, _I32, _OUT, _OUT, _OUT]),
+    "magnet_cost_volume_f_bwd_f32": (_ST, [C.POINTER(CostFBwdArgs), _P]),
+    "magnet_cost_volume_bwd_f32": (_ST, [C.POINTER(CostBwdArgs), _P]),
+    "magnet_cost_geom_workspace_bytes": (_SZ, [_I32] * 4),
+    "magnet_cost_volume_geom_bwd_f32": (_ST, [C.POINTER(CostGeomBwdArgs), _P]),
+    "magnet_pack_cameras_f32": (_ST, [_P, _P, _I64, _I64, _I64, _I64, _P, _I64, _I64, _I64, _P, _I32, _I32, _P, _P]),
+    "magnet_repack_tiled32_f32": (_ST, [_P, _P] + [_I32] * 4 + [_P]),
+    "magnet_repack_pixc_f32": (_ST, [_P, _P, _P] + [_I32] * 4 + [_P]),
+    "magnet_split16_bytes": (_SZ, [_I32] * 3),
+    "magnet_repack_split16_f32": (_ST, [_P, _P, _P] + [_I32] * 4 + [_P]),
+    "magnet_half16_bytes": (_SZ, [_I32] * 3),
+    "magnet_repack_half16": (_ST, [_P, _I32, _P, _P] + [_I32] * 4 + [_P]),
+    "magnet_sample_depths_f32": (_ST, [_P, _P] + [_I32] * 3 + [_P, _P]),
+    "magnet_gaussian_update_fwd_f32": (_ST, [_P, _P, _I32, _I32, _P, _P]),
+    "magnet_gaussian_update_bwd_f32": (_ST, [_P, _P, _P, _I32, _I32, _P, _P]),
+    "magnet_convex_upsample_fwd_f32": (_ST, [_P, _P] + [_I32] * 5 + [_P, _P]),
+    "magnet_convex_upsample_bwd_f32": (_ST, [_P, _P, _P] + [_I32] * 5 + [_P, _P, _P]),
+    "magnet_relative_poses_f32": (_ST, [_P, _P, _I32, _I32, _P, _P, _P]),
+    "magnet_camera_rays_f32": (_ST, [_P] + [_I32] * 3 + [_P, _P, _P]),
+    "magnet_upsample_nll_partials": (_ST, [_I32] * 4),
+    "magnet_upsample_nll_fwd_f32": (_ST, [_P] * 4 + [_I32] * 4 + [_P, _P]),
+    "magnet_upsample_nll_bwd_f32": (_ST, [_P] * 4 + [_F32] + [_I32] * 4 + [_P, _P, _P]),
+    "magnet_fnet_l1_partials": (_ST, [_I32] * 3),
+    "magnet_fnet_l1_fwd_f32": (_ST, [_P] * 4 + [_I32] * 4 + [_P, _P]),
+    "magnet_fnet_l1_bwd_f32": (_ST, [_P] * 4 + [_F32, _P] + [_I32] * 4 + [_P, _P]),
+    "magnet_plane_depth_f32": (_ST, [_P, _P] + [_I32] * 5 + [_P, _P]),
+    "magnet_depth_metrics_workspace": (C.c_int64, [C.POINTER(DepthMetricsArgs)]),
+    "magnet_depth_metrics_f32": (_ST, [C.POINTER(DepthMetricsArgs), _P]),
+    "magnet_depth_metrics_var_f32": (_ST, [C.POINTER(DepthMetricsArgs), _P]),
+    "magnet_depth_metrics_nearest_workspace": (C.c_int64, [C.POINTER(DepthMetricsNearestArgs)]),
+    "magnet_depth_metrics_nearest_f32": (_ST, [C.POINTER(DepthMetricsNearestArgs), _P]),
+    "magnet_gnet_weights_bytes": (_SZ, [_I32]),
+    "magnet_gnet_pack_weights_f32": (_ST, [_P] * 7 + [_I32, _P, _P]),
+    "magnet_gnet_update_f32": (_ST, [C.POINTER(GnetArgs), _P]),
+    "magnet_gnet_train_weights_bytes": (_SZ, [_I32]),
+    "magnet_gnet_saved_bytes": (_SZ, [_I32] * 3),
+    "magnet_gnet_bwd_workspace_bytes": (_SZ, [_I32] * 4),
+    "magnet_gnet_pack_train_weights_f32": (_ST, [_P] * 7 + [_I32, _P, _P]),
+    "magnet_gnet_train_fwd_f32": (_ST, [C.POINTER(GnetTrainArgs), _P]),
+    "magnet_gnet_bwd_f32": (_ST, [C.POINTER(GnetTrainArgs), _P]),
+    "magnet_mask_weights_bytes": (_SZ, [_I32]),
+    "magnet_mask_pack_weights_f32": (_ST, [_P] * 8),
+    "magnet_mask_upsample_f32": (_ST, [C.POINTER(MaskUpsampleArgs), _P]),
+    "magnet_mask_train_weights_bytes": (_SZ, [_I32]),
+    "magnet_mask_saved_bytes": (_SZ, [_I32] * 4),
+    "magnet_mask_bwd_workspace_bytes": (_SZ, [_I32] * 3),
+    "magnet_mask_train_partials": (_ST, [_I32] * 3),
+    "magnet_mask_pack_train_weights_f32": (_ST, [_P] * 8),
+    "magnet_mask_train_fwd_f32": (_ST, [C.POINTER(MaskTrainArgs), _P]),
+    "magnet_mask_bwd_f32": (_ST, [C.POINTER(MaskTrainArgs), _P]),
+    "magnet_dnet_weights_bytes": (_SZ, [_I32]),
+    "magnet_dnet_pack_weights_f32": (_ST, [_P] * 8 + [_I32, _P, _P]),
+    "magnet_dnet_depth_f32": (_ST, [_P, _P] + [_I32] * 4 + [_P, _P]),
+    "magnet_dnet_upsample_f32": (_ST, [_P] * 3 + [_I32] * 4 + [_P, _P]),
+}
+EXPORTS = tuple(SIGNATURES)
+
+
 class MagnetError(RuntimeError):
     pass
 
@@ -155,140 +200,11 @@ def lib() -> C.CDLL:
             f"{LIB_PATH} not found: build it with `python -m magnet_b200.build` (or __graft_entry__.build()). "
             "magnet_b200 has no CPU / PyTorch fallback for the matching path.")
     L = C.CDLL(str(LIB_PATH))
-    for name in EXPORTS:
+    for name, (restype, argtypes) in SIGNATURES.items():
         if not hasattr(L, name):
             raise MagnetError(f"{LIB_PATH} does not export {name}")
-    L.magnet_abi_version.restype = C.c_int
-    L.magnet_strerror.restype = C.c_char_p
-    L.magnet_strerror.argtypes = [C.c_int]
-    L.magnet_last_cuda_error.restype = C.c_char_p
-    L.magnet_launch_count.restype = C.c_uint64
-    L.magnet_cost_launch_info.restype = C.c_int
-    L.magnet_cost_launch_info.argtypes = [C.POINTER(CostArgs), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    L.magnet_cost_volume_f32.restype = C.c_int
-    L.magnet_cost_volume_f32.argtypes = [C.POINTER(CostArgs), C.c_void_p]
-    L.magnet_cost_volume_indexed_f32.restype = C.c_int
-    L.magnet_cost_volume_indexed_f32.argtypes = [C.POINTER(CostArgs), C.c_void_p, C.c_int32, C.c_void_p]
-    L.magnet_cost_indexed_launch_info.restype = C.c_int
-    L.magnet_cost_indexed_launch_info.argtypes = [C.POINTER(CostArgs), C.c_void_p, C.c_int32, C.POINTER(C.c_int),
-                                                  C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    L.magnet_cost_volume_f_bwd_f32.restype = C.c_int
-    L.magnet_cost_volume_f_bwd_f32.argtypes = [C.POINTER(CostFBwdArgs), C.c_void_p]
-    L.magnet_cost_volume_bwd_f32.restype = C.c_int
-    L.magnet_cost_volume_bwd_f32.argtypes = [C.POINTER(CostBwdArgs), C.c_void_p]
-    L.magnet_pack_cameras_f32.restype = C.c_int
-    L.magnet_pack_cameras_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
-                                          C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int32,
-                                          C.c_int32, C.c_void_p, C.c_void_p]
-    L.magnet_repack_tiled32_f32.restype = C.c_int
-    L.magnet_repack_tiled32_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
-    L.magnet_repack_pixc_f32.restype = C.c_int
-    L.magnet_repack_pixc_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                         C.c_void_p]
-    L.magnet_split16_bytes.restype = C.c_size_t
-    L.magnet_split16_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
-    L.magnet_repack_split16_f32.restype = C.c_int
-    L.magnet_repack_split16_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                            C.c_void_p]
-    L.magnet_half16_bytes.restype = C.c_size_t
-    L.magnet_half16_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
-    L.magnet_repack_half16.restype = C.c_int
-    L.magnet_repack_half16.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                       C.c_int32, C.c_void_p]
-    L.magnet_sample_depths_f32.restype = C.c_int
-    L.magnet_sample_depths_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
-    L.magnet_gaussian_update_fwd_f32.restype = C.c_int
-    L.magnet_gaussian_update_fwd_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
-    L.magnet_gaussian_update_bwd_f32.restype = C.c_int
-    L.magnet_gaussian_update_bwd_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
-    L.magnet_convex_upsample_fwd_f32.restype = C.c_int
-    L.magnet_convex_upsample_fwd_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                                 C.c_int32, C.c_void_p, C.c_void_p]
-    L.magnet_convex_upsample_bwd_f32.restype = C.c_int
-    L.magnet_convex_upsample_bwd_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                                 C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.magnet_relative_poses_f32.restype = C.c_int
-    L.magnet_relative_poses_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.magnet_camera_rays_f32.restype = C.c_int
-    L.magnet_camera_rays_f32.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.magnet_upsample_nll_partials.restype = C.c_int
-    L.magnet_upsample_nll_partials.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32]
-    L.magnet_upsample_nll_fwd_f32.restype = C.c_int
-    L.magnet_upsample_nll_fwd_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                              C.c_int32, C.c_void_p, C.c_void_p]
-    L.magnet_upsample_nll_bwd_f32.restype = C.c_int
-    L.magnet_upsample_nll_bwd_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int32, C.c_int32,
-                                              C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.magnet_fnet_l1_partials.restype = C.c_int
-    L.magnet_fnet_l1_partials.argtypes = [C.c_int32, C.c_int32, C.c_int32]
-    L.magnet_fnet_l1_fwd_f32.restype = C.c_int
-    L.magnet_fnet_l1_fwd_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                         C.c_int32, C.c_void_p, C.c_void_p]
-    L.magnet_fnet_l1_bwd_f32.restype = C.c_int
-    L.magnet_fnet_l1_bwd_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int32,
-                                         C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
-    L.magnet_depth_metrics_workspace.restype = C.c_int64
-    L.magnet_depth_metrics_workspace.argtypes = [C.POINTER(DepthMetricsArgs)]
-    L.magnet_depth_metrics_f32.restype = C.c_int
-    L.magnet_depth_metrics_f32.argtypes = [C.POINTER(DepthMetricsArgs), C.c_void_p]
-    L.magnet_plane_depth_f32.restype = C.c_int
-    L.magnet_plane_depth_f32.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p, C.c_void_p]
-    L.magnet_depth_metrics_nearest_workspace.restype = C.c_int64
-    L.magnet_depth_metrics_nearest_workspace.argtypes = [C.POINTER(DepthMetricsNearestArgs)]
-    L.magnet_depth_metrics_nearest_f32.restype = C.c_int
-    L.magnet_depth_metrics_nearest_f32.argtypes = [C.POINTER(DepthMetricsNearestArgs), C.c_void_p]
-    L.magnet_gnet_weights_bytes.restype = C.c_size_t
-    L.magnet_gnet_weights_bytes.argtypes = [C.c_int32]
-    L.magnet_gnet_pack_weights_f32.restype = C.c_int
-    L.magnet_gnet_pack_weights_f32.argtypes = [C.c_void_p] * 7 + [C.c_int32, C.c_void_p, C.c_void_p]
-    L.magnet_gnet_update_f32.restype = C.c_int
-    L.magnet_gnet_update_f32.argtypes = [C.POINTER(GnetArgs), C.c_void_p]
-    L.magnet_gnet_train_weights_bytes.restype = C.c_size_t
-    L.magnet_gnet_train_weights_bytes.argtypes = [C.c_int32]
-    L.magnet_gnet_saved_bytes.restype = C.c_size_t
-    L.magnet_gnet_saved_bytes.argtypes = [C.c_int32] * 3
-    L.magnet_gnet_bwd_workspace_bytes.restype = C.c_size_t
-    L.magnet_gnet_bwd_workspace_bytes.argtypes = [C.c_int32] * 4
-    L.magnet_gnet_pack_train_weights_f32.restype = C.c_int
-    L.magnet_gnet_pack_train_weights_f32.argtypes = [C.c_void_p] * 7 + [C.c_int32, C.c_void_p, C.c_void_p]
-    L.magnet_gnet_train_fwd_f32.restype = C.c_int
-    L.magnet_gnet_train_fwd_f32.argtypes = [C.POINTER(GnetTrainArgs), C.c_void_p]
-    L.magnet_gnet_bwd_f32.restype = C.c_int
-    L.magnet_gnet_bwd_f32.argtypes = [C.POINTER(GnetTrainArgs), C.c_void_p]
-    L.magnet_cost_geom_workspace_bytes.restype = C.c_size_t
-    L.magnet_cost_geom_workspace_bytes.argtypes = [C.c_int32] * 4
-    L.magnet_cost_volume_geom_bwd_f32.restype = C.c_int
-    L.magnet_cost_volume_geom_bwd_f32.argtypes = [C.POINTER(CostGeomBwdArgs), C.c_void_p]
-    L.magnet_mask_weights_bytes.restype = C.c_size_t
-    L.magnet_mask_weights_bytes.argtypes = [C.c_int32]
-    L.magnet_mask_pack_weights_f32.restype = C.c_int
-    L.magnet_mask_pack_weights_f32.argtypes = [C.c_void_p] * 8
-    L.magnet_mask_upsample_f32.restype = C.c_int
-    L.magnet_mask_upsample_f32.argtypes = [C.POINTER(MaskUpsampleArgs), C.c_void_p]
-    L.magnet_mask_train_weights_bytes.restype = C.c_size_t
-    L.magnet_mask_train_weights_bytes.argtypes = [C.c_int32]
-    L.magnet_mask_saved_bytes.restype = C.c_size_t
-    L.magnet_mask_saved_bytes.argtypes = [C.c_int32] * 4
-    L.magnet_mask_bwd_workspace_bytes.restype = C.c_size_t
-    L.magnet_mask_bwd_workspace_bytes.argtypes = [C.c_int32] * 3
-    L.magnet_mask_train_partials.restype = C.c_int
-    L.magnet_mask_train_partials.argtypes = [C.c_int32] * 3
-    L.magnet_mask_pack_train_weights_f32.restype = C.c_int
-    L.magnet_mask_pack_train_weights_f32.argtypes = [C.c_void_p] * 8
-    L.magnet_mask_train_fwd_f32.restype = C.c_int
-    L.magnet_mask_train_fwd_f32.argtypes = [C.POINTER(MaskTrainArgs), C.c_void_p]
-    L.magnet_mask_bwd_f32.restype = C.c_int
-    L.magnet_mask_bwd_f32.argtypes = [C.POINTER(MaskTrainArgs), C.c_void_p]
-    L.magnet_dnet_weights_bytes.restype = C.c_size_t
-    L.magnet_dnet_weights_bytes.argtypes = [C.c_int32]
-    L.magnet_dnet_pack_weights_f32.restype = C.c_int
-    L.magnet_dnet_pack_weights_f32.argtypes = [C.c_void_p] * 8 + [C.c_int32, C.c_void_p, C.c_void_p]
-    L.magnet_dnet_depth_f32.restype = C.c_int
-    L.magnet_dnet_depth_f32.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p, C.c_void_p]
-    L.magnet_dnet_upsample_f32.restype = C.c_int
-    L.magnet_dnet_upsample_f32.argtypes = [C.c_void_p] * 3 + [C.c_int32] * 4 + [C.c_void_p, C.c_void_p]
-    L.magnet_depth_metrics_var_f32.restype = C.c_int
-    L.magnet_depth_metrics_var_f32.argtypes = [C.POINTER(DepthMetricsArgs), C.c_void_p]
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
     if L.magnet_abi_version() != MAGNET_ABI_VERSION:
         raise MagnetError(f"ABI version mismatch: library {L.magnet_abi_version()} != binding {MAGNET_ABI_VERSION}")
     _lib = L

@@ -20,6 +20,13 @@ def _stream(dev=None) -> int:
     return torch.cuda.current_stream(dev).cuda_stream
 
 
+def _launch(dev, name: str, *args) -> None:
+    """Call the C entry point ``name`` with ``args`` and the current stream of ``dev``, with ``dev`` current; a
+    failed status raises MagnetError."""
+    with torch.cuda.device(dev):
+        check(getattr(lib(), name)(*args, _stream(dev)), name)
+
+
 def _same_device(*named):
     """All operands of one launch must live on one CUDA device; returns it."""
     dev = None
@@ -38,16 +45,39 @@ def _expect(name: str, x: torch.Tensor, shape) -> None:
         raise _lib.MagnetError(f"{name} must have shape {tuple(shape)}, got {tuple(x.shape)}")
 
 
-def _need_cuda_f32(name: str, x: torch.Tensor, contiguous: bool = True) -> torch.Tensor:
-    if not isinstance(x, torch.Tensor):
-        raise TypeError(f"{name} must be a torch.Tensor")
-    if not x.is_cuda:
-        raise _lib.MagnetError(f"{name} must be a CUDA tensor (magnet_b200 has no CPU path)")
+def _need_cuda_f32(name: str, x: torch.Tensor, shape=None, contiguous: bool = True) -> torch.Tensor:
+    """A CUDA float32 operand, of ``shape`` when given; made contiguous unless ``contiguous=False``."""
+    x = _need_cuda(name, x)
     if x.dtype != torch.float32:
         raise _lib.MagnetError(f"{name} must be float32 (the reference path is fp32-only, homography.py:130)")
     if contiguous and not x.is_contiguous():
         x = x.contiguous()
+    if shape is not None:
+        _expect(name, x, shape)
     return x
+
+
+def _need_preds(name: str, preds, shape=None) -> list:
+    """Predictions ``name[i]`` (any iterable, consumed in order), each checked as ``_need_cuda_f32`` does."""
+    return [_need_cuda_f32(f"{name}[{i}]", p, shape) for i, p in enumerate(preds)]
+
+
+def _need_weights(named) -> list:
+    """(name, weight, shape) triples -> the detached weights, each a CUDA float32 tensor of its shape."""
+    return [_need_cuda_f32(nm, t.detach(), shp) for nm, t, shp in named]
+
+
+def _need_cuda_u8_mask(name: str, m: torch.Tensor, shape, shape_text: str) -> torch.Tensor:
+    """A CUDA uint8 mask of ``shape`` (``shape_text`` in the message), made contiguous."""
+    if m.dtype != torch.uint8 or not m.is_cuda or tuple(m.shape) != tuple(shape):
+        raise _lib.MagnetError(f"{name} must be a CUDA uint8 tensor of shape {shape_text}")
+    return m.contiguous()
+
+
+def _is_packed(buf, sizes=None) -> bool:
+    """A packed buffer: a contiguous uint8 CUDA tensor, and, when ``sizes`` is given, of one of those byte counts."""
+    return (isinstance(buf, torch.Tensor) and buf.is_cuda and buf.dtype == torch.uint8 and buf.is_contiguous()
+            and (sizes is None or buf.numel() in sizes))
 
 
 def _need_cuda(name: str, x: torch.Tensor) -> torch.Tensor:
@@ -74,7 +104,7 @@ def _check_packed(name: str, buf, layout: int, N: int, H: int, W: int) -> None:
     """A SPLIT16 / HALF16 buffer of N images: uint8, contiguous, on the device, and exactly the layout's size (the
     kernels cannot tell the two kinds apart, so a buffer of the other kind is refused here, before any launch)."""
     what = "repack_split16" if layout == _lib.SRC_SPLIT16 else "repack_half16"
-    if not (isinstance(buf, torch.Tensor) and buf.is_cuda and buf.dtype == torch.uint8 and buf.is_contiguous()):
+    if not _is_packed(buf):
         raise _lib.MagnetError(f"{name} must be a contiguous uint8 CUDA buffer from {what}")
     nbytes = packed_bytes(layout, N, H, W)
     if buf.numel() != nbytes:
@@ -106,10 +136,8 @@ def pack_cameras(intM: torch.Tensor, R: torch.Tensor, t: torch.Tensor, is_valid:
     cams = torch.empty(B * V, 16, device=intM.device, dtype=torch.float32)
     rs, ts = R.stride(), t.stride()
     dev = _same_device(("intM", intM), ("R", R), ("t", t), ("is_valid", is_valid))
-    with torch.cuda.device(dev):
-        check(lib().magnet_pack_cameras_f32(intM.data_ptr(), R.data_ptr(), rs[0], rs[1], rs[2], rs[3],
-                                            t.data_ptr(), ts[0], ts[1], ts[2], is_valid.data_ptr(), B, V,
-                                            cams.data_ptr(), _stream(dev)), "magnet_pack_cameras_f32")
+    _launch(dev, "magnet_pack_cameras_f32", intM.data_ptr(), R.data_ptr(), rs[0], rs[1], rs[2], rs[3], t.data_ptr(),
+            ts[0], ts[1], ts[2], is_valid.data_ptr(), B, V, cams.data_ptr())
     return cams
 
 
@@ -141,9 +169,7 @@ def repack_tiled32(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch
     N, Cc, H, W = x.shape
     if out is None:
         out = torch.empty(N, H, (W + 31) // 32, Cc // 4, 32, 4, device=x.device, dtype=torch.float32)
-    with torch.cuda.device(x.device):
-        check(lib().magnet_repack_tiled32_f32(x.data_ptr(), out.data_ptr(), N, Cc, H, W, _stream(x.device)),
-              "magnet_repack_tiled32_f32")
+    _launch(x.device, "magnet_repack_tiled32_f32", x.data_ptr(), out.data_ptr(), N, Cc, H, W)
     return out
 
 
@@ -153,9 +179,7 @@ def repack_pixc(x: torch.Tensor, gmm: Optional[torch.Tensor] = None, out: Option
     x = _need_cuda_f32("x", x)
     N, Cc, H, W = x.shape
     gmm, out = _repack_operands(x, gmm, out, (N, H, W, Cc + 4), torch.float32)
-    with torch.cuda.device(x.device):
-        check(lib().magnet_repack_pixc_f32(x.data_ptr(), _ptr(gmm), out.data_ptr(), N, Cc, H, W, _stream(x.device)),
-              "magnet_repack_pixc_f32")
+    _launch(x.device, "magnet_repack_pixc_f32", x.data_ptr(), _ptr(gmm), out.data_ptr(), N, Cc, H, W)
     return out
 
 
@@ -166,9 +190,7 @@ def repack_split16(x: torch.Tensor, gmm: Optional[torch.Tensor] = None, out: Opt
     x = _need_cuda_f32("x", x)
     N, Cc, H, W = x.shape
     gmm, out = _repack_operands(x, gmm, out, (int(lib().magnet_split16_bytes(N, H, W)),))
-    with torch.cuda.device(x.device):
-        check(lib().magnet_repack_split16_f32(x.data_ptr(), _ptr(gmm), out.data_ptr(), N, Cc, H, W, _stream(x.device)),
-              "magnet_repack_split16_f32")
+    _launch(x.device, "magnet_repack_split16_f32", x.data_ptr(), _ptr(gmm), out.data_ptr(), N, Cc, H, W)
     return out
 
 
@@ -176,10 +198,7 @@ def repack_half16(x: torch.Tensor, gmm: Optional[torch.Tensor] = None, out: Opti
     """(N,64,H,W) fp16 / bf16 features [+ (N,2,H,W) fp32 Gaussians] -> HALF16 buffer (uint8): the header and table of
     ``repack_split16(x.float(), gmm)`` around ONE fp16 plane (N,1,H,W,64) = its hi plane (its lo plane is zero for
     every element above the threshold of DESIGN §3.7).  Read by the tensor-core kernels with ``src_layout=SRC_HALF16``."""
-    if not isinstance(x, torch.Tensor):
-        raise TypeError("x must be a torch.Tensor")
-    if not x.is_cuda:
-        raise _lib.MagnetError("x must be a CUDA tensor (magnet_b200 has no CPU path)")
+    x = _need_cuda("x", x)
     if x.dtype not in HALF_DTYPES:
         raise _lib.MagnetError(f"x must be float16 or bfloat16 (repack_split16 takes float32), got {x.dtype}")
     if x.dim() != 4:
@@ -188,9 +207,7 @@ def repack_half16(x: torch.Tensor, gmm: Optional[torch.Tensor] = None, out: Opti
     N, Cc, H, W = x.shape
     gmm, out = _repack_operands(x, gmm, out, (int(lib().magnet_half16_bytes(N, H, W)),))
     _same_device(("x", x), ("gmm", gmm))
-    with torch.cuda.device(x.device):
-        check(lib().magnet_repack_half16(x.data_ptr(), HALF_DTYPES[x.dtype], _ptr(gmm), out.data_ptr(), N, Cc, H, W,
-                                         _stream(x.device)), "magnet_repack_half16")
+    _launch(x.device, "magnet_repack_half16", x.data_ptr(), HALF_DTYPES[x.dtype], _ptr(gmm), out.data_ptr(), N, Cc, H, W)
     return out
 
 
@@ -202,9 +219,8 @@ def sample_depths(gmm: torch.Tensor, k, out: Optional[torch.Tensor] = None) -> t
     D = len(karr)
     if out is None:
         out = torch.empty(B, D, H, W, device=gmm.device, dtype=torch.float32)
-    with torch.cuda.device(gmm.device):
-        check(lib().magnet_sample_depths_f32(gmm.data_ptr(), C.cast(karr, C.c_void_p), B, D, H * W, out.data_ptr(),
-                                             _stream(gmm.device)), "magnet_sample_depths_f32")
+    _launch(gmm.device, "magnet_sample_depths_f32", gmm.data_ptr(), C.cast(karr, C.c_void_p), B, D, H * W,
+            out.data_ptr())
     return out
 
 
@@ -236,8 +252,7 @@ def _cost_args(ref_feat: torch.Tensor, V: int, rays, cams, *, d_volume=None, ref
         if planes:
             a.depth_mode = _lib.DEPTH_PLANES
         else:
-            ref_gmm = _need_cuda_f32("ref_gmm", ref_gmm)
-            _expect("ref_gmm", ref_gmm, (B, 2, H, W))
+            ref_gmm = _need_cuda_f32("ref_gmm", ref_gmm, (B, 2, H, W))
             a.depth_mode, a.ref_gmm = _lib.DEPTH_GAUSS, ref_gmm.data_ptr()
             gd_shape = (B, 2, H, W)
     a._keep = (rays, cams, d_volume, ref_gmm, karr)
@@ -335,21 +350,17 @@ def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tens
     a.ref_feat = ref_split.data_ptr() if src_layout in PACKED_LAYOUTS else ref_feat.data_ptr()
     a.src_feat = src_feat.data_ptr()
     if consistency and src_layout not in (_lib.SRC_PIXC, *PACKED_LAYOUTS):   # those carry the source Gaussians inside src_feat
-        src_gmm = _need_cuda_f32("src_gmm", src_gmm)
-        _expect("src_gmm", src_gmm, (n_img, 2, H, W))
+        src_gmm = _need_cuda_f32("src_gmm", src_gmm, (n_img, 2, H, W))
         a.src_gmm = src_gmm.data_ptr()
     if out is None:
         out = torch.empty(B, a.D, H, W, device=ref_feat.device, dtype=torch.float32)
     else:
-        out = _need_cuda_f32("out", out)
-        _expect("out", out, (B, a.D, H, W))
+        out = _need_cuda_f32("out", out, (B, a.D, H, W))
     a.out = out.data_ptr()
-    with torch.cuda.device(dev):
-        if src_index is None:
-            check(lib().magnet_cost_volume_f32(C.byref(a), _stream(dev)), "magnet_cost_volume_f32")
-        else:
-            check(lib().magnet_cost_volume_indexed_f32(C.byref(a), src_index.data_ptr(), n_img, _stream(dev)),
-                  "magnet_cost_volume_indexed_f32")
+    if src_index is None:
+        _launch(dev, "magnet_cost_volume_f32", C.byref(a))
+    else:
+        _launch(dev, "magnet_cost_volume_indexed_f32", C.byref(a), src_index.data_ptr(), n_img)
     return out
 
 
@@ -374,8 +385,7 @@ def cost_volume_f_bwd(ref_feat, src_feat_nchw, rays, cams, planes, V, prob, grad
     a, _, named = _cost_args(ref_feat, V, rays, cams, k=planes, planes=True)
     _expect("grad_out", grad_out, (B, a.D, H, W))
     if softmax:
-        prob = _need_cuda_f32("prob", prob)
-        _expect("prob", prob, (B, a.D, H, W))
+        prob = _need_cuda_f32("prob", prob, (B, a.D, H, W))
     if split:
         for nm, buf, n in (("src_split", src_split, V * B), ("ref_split", ref_split, B)):
             _check_packed(nm, buf, split_layout, n, H, W)
@@ -392,8 +402,7 @@ def cost_volume_f_bwd(ref_feat, src_feat_nchw, rays, cams, planes, V, prob, grad
     bw.prob = prob.data_ptr() if softmax else None
     bw.grad_out, bw.workspace = grad_out.data_ptr(), work.data_ptr()
     bw.grad_ref, bw.grad_src = g_ref.data_ptr(), g_src.data_ptr()
-    with torch.cuda.device(dev):
-        check(lib().magnet_cost_volume_f_bwd_f32(C.byref(bw), _stream(dev)), "magnet_cost_volume_f_bwd_f32")
+    _launch(dev, "magnet_cost_volume_f_bwd_f32", C.byref(bw))
     return g_ref, g_src
 
 
@@ -429,8 +438,7 @@ def cost_volume_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V: int
     if not shape_only:                             # the NCHW maps are read (CUDA-core kernel)
         bw.ref_feat, bw.src_feat = ref_feat.data_ptr(), src.data_ptr()
     if consistency:
-        src_gmm = _need_cuda_f32("src_gmm", src_gmm)
-        _expect("src_gmm", src_gmm, (V * B, 2, H, W))
+        src_gmm = _need_cuda_f32("src_gmm", src_gmm, (V * B, 2, H, W))
         bw.src_gmm = src_gmm.data_ptr()
     dev = _same_device(("ref_feat", ref_feat), ("src_feat", src), ("src_gmm", src_gmm if consistency else None),
                        *named, ("grad_out", grad_out), ("ref_split", ref_split), ("src_split", src_split))
@@ -440,8 +448,7 @@ def cost_volume_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V: int
     g_d = torch.empty(gd_shape, device=dev, dtype=torch.float32) if need_depth else None
     bw.grad_out, bw.workspace = grad_out.data_ptr(), work.data_ptr()
     bw.grad_ref, bw.grad_src, bw.grad_depth = _ptr(g_ref), _ptr(g_src), _ptr(g_d)
-    with torch.cuda.device(dev):
-        check(lib().magnet_cost_volume_bwd_f32(C.byref(bw), _stream(dev)), "magnet_cost_volume_bwd_f32")
+    _launch(dev, "magnet_cost_volume_bwd_f32", C.byref(bw))
     return g_ref, g_src, g_d
 
 
@@ -473,12 +480,10 @@ def cost_volume_geom_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V
     bw.fwd = C.pointer(a)
     bw.ref_feat, bw.src_feat = ref_feat.data_ptr(), src.data_ptr()
     if a.consistency:
-        src_gmm = _need_cuda_f32("src_gmm", src_gmm)
-        _expect("src_gmm", src_gmm, (V * B, 2, H, W))
+        src_gmm = _need_cuda_f32("src_gmm", src_gmm, (V * B, 2, H, W))
         bw.src_gmm = src_gmm.data_ptr()
     if softmax:
-        prob = _need_cuda_f32("prob", prob)
-        _expect("prob", prob, (B, a.D, H, W))
+        prob = _need_cuda_f32("prob", prob, (B, a.D, H, W))
         bw.prob = prob.data_ptr()
     dev = _same_device(("ref_feat", ref_feat), ("src_feat", src), ("src_gmm", src_gmm if a.consistency else None),
                        *named, ("grad_out", grad_out), ("prob", prob if softmax else None))
@@ -489,8 +494,7 @@ def cost_volume_geom_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V
     g_d = torch.empty(gd_shape, device=dev, dtype=torch.float32) if need_depth else None
     bw.score, bw.workspace, bw.grad_out, bw.grad_cams = score.data_ptr(), work.data_ptr(), grad_out.data_ptr(), g_cams.data_ptr()
     bw.grad_rays, bw.grad_depth = _ptr(g_rays), _ptr(g_d)
-    with torch.cuda.device(dev):
-        check(lib().magnet_cost_volume_geom_bwd_f32(C.byref(bw), _stream(dev)), "magnet_cost_volume_geom_bwd_f32")
+    _launch(dev, "magnet_cost_volume_geom_bwd_f32", C.byref(bw))
     return g_cams, g_rays, g_d
 
 
@@ -531,12 +535,10 @@ class GaussianUpdate(torch.autograd.Function):
         d_output = _need_cuda_f32("d_output", d_output)
         ref_gmm = _need_cuda_f32("ref_gmm", ref_gmm.detach())
         B, _, H, W = d_output.shape
+        _expect("ref_gmm", ref_gmm, d_output.shape)     # after the unpack, which refuses a d_output of another rank
         out = torch.empty_like(d_output)
-        _expect("ref_gmm", ref_gmm, d_output.shape)
         dev = _same_device(("d_output", d_output), ("ref_gmm", ref_gmm))
-        with torch.cuda.device(dev):
-            check(lib().magnet_gaussian_update_fwd_f32(d_output.data_ptr(), ref_gmm.data_ptr(), B, H * W,
-                                                       out.data_ptr(), _stream(dev)), "magnet_gaussian_update_fwd_f32")
+        _launch(dev, "magnet_gaussian_update_fwd_f32", d_output.data_ptr(), ref_gmm.data_ptr(), B, H * W, out.data_ptr())
         ctx.save_for_backward(d_output, ref_gmm)
         return out
 
@@ -546,10 +548,8 @@ class GaussianUpdate(torch.autograd.Function):
         grad_out = _need_cuda_f32("grad_out", grad_out)
         B, _, H, W = d_output.shape
         gin = torch.empty_like(d_output)
-        with torch.cuda.device(d_output.device):
-            check(lib().magnet_gaussian_update_bwd_f32(grad_out.data_ptr(), d_output.data_ptr(), ref_gmm.data_ptr(),
-                                                       B, H * W, gin.data_ptr(), _stream(d_output.device)),
-                  "magnet_gaussian_update_bwd_f32")
+        _launch(d_output.device, "magnet_gaussian_update_bwd_f32", grad_out.data_ptr(), d_output.data_ptr(),
+                ref_gmm.data_ptr(), B, H * W, gin.data_ptr())
         return gin, None
 
 
@@ -582,9 +582,7 @@ def pack_gnet_weights(gnet, D: int) -> torch.Tensor:
                                                          ("b2", c2.bias), ("W3", c3.weight), ("b3", c3.bias))]
     dev = _same_device(*((f"weight {i}", t) for i, t in enumerate(ts)))
     out = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-    with torch.cuda.device(dev):
-        check(lib().magnet_gnet_pack_weights_f32(*(t.data_ptr() for t in ts), int(D), out.data_ptr(), _stream(dev)),
-              "magnet_gnet_pack_weights_f32")
+    _launch(dev, "magnet_gnet_pack_weights_f32", *(t.data_ptr() for t in ts), int(D), out.data_ptr())
     return out
 
 
@@ -597,28 +595,23 @@ def gnet_update(cost: torch.Tensor, invariant: torch.Tensor, packed: torch.Tenso
     if cost.dim() != 4:
         raise _lib.MagnetError(f"cost must be (B,D,H,W), got {tuple(cost.shape)}")
     B, D, H, W = cost.shape
-    invariant = _need_cuda_f32("invariant", invariant)
-    _expect("invariant", invariant, (B, _lib.MAGNET_HIDDEN_CHANNELS, H, W))
-    prev_gmm = _need_cuda_f32("prev_gmm", prev_gmm)
-    _expect("prev_gmm", prev_gmm, (B, 2, H, W))
+    invariant = _need_cuda_f32("invariant", invariant, (B, _lib.MAGNET_HIDDEN_CHANNELS, H, W))
+    prev_gmm = _need_cuda_f32("prev_gmm", prev_gmm, (B, 2, H, W))
     nbytes = gnet_weights_bytes(D)
     if nbytes == 0:
         raise _lib.MagnetError(f"the fused G-Net head takes 1 to {_lib.MAGNET_MAX_PLANES} cost channels, got {D}")
-    if not (isinstance(packed, torch.Tensor) and packed.is_cuda and packed.dtype == torch.uint8
-            and packed.is_contiguous() and packed.numel() == nbytes):
+    if not _is_packed(packed, (nbytes,)):
         raise _lib.MagnetError(f"packed must be a pack_gnet_weights buffer for D = {D} ({nbytes} bytes)")
     if out is None:
         out = torch.empty(B, 2, H, W, device=cost.device, dtype=torch.float32)
     else:
-        out = _need_cuda_f32("out", out)
-        _expect("out", out, (B, 2, H, W))
+        out = _need_cuda_f32("out", out, (B, 2, H, W))
     dev = _same_device(("cost", cost), ("invariant", invariant), ("packed", packed), ("prev_gmm", prev_gmm), ("out", out))
     scratch = torch.empty(_lib.MAGNET_GNET_SCRATCH_BYTES // 4, device=dev, dtype=torch.int32)
     a = _lib.GnetArgs(B=B, D=D, H=H, W=W, cost=cost.data_ptr(), invariant=invariant.data_ptr(),
                       packed_weights=packed.data_ptr(), prev_gmm=prev_gmm.data_ptr(), scratch=scratch.data_ptr(),
                       out=out.data_ptr())
-    with torch.cuda.device(dev):
-        check(lib().magnet_gnet_update_f32(C.byref(a), _stream(dev)), "magnet_gnet_update_f32")
+    _launch(dev, "magnet_gnet_update_f32", C.byref(a))
     return out
 
 
@@ -635,20 +628,14 @@ class GnetHeadTrain(torch.autograd.Function):
         if cost.dim() != 4:
             raise _lib.MagnetError(f"cost must be (B,D,H,W), got {tuple(cost.shape)}")
         B, D, H, W = cost.shape
-        invariant = _need_cuda_f32("invariant", invariant.detach())
-        _expect("invariant", invariant, (B, hid, H, W))
-        prev_gmm = _need_cuda_f32("prev_gmm", prev_gmm.detach())
-        _expect("prev_gmm", prev_gmm, (B, 2, H, W))
+        invariant = _need_cuda_f32("invariant", invariant.detach(), (B, hid, H, W))
+        prev_gmm = _need_cuda_f32("prev_gmm", prev_gmm.detach(), (B, 2, H, W))
         nbytes = int(lib().magnet_gnet_train_weights_bytes(D))
         if nbytes == 0:
             raise _lib.MagnetError(f"the fused G-Net head takes 1 to {_lib.MAGNET_MAX_PLANES} cost channels, got {D}")
         shapes = (("W0", w0, (hid, D, 3, 3)), ("W1", w1, (hid, hid, 1, 1)), ("b1", b1, (hid,)),
                   ("W2", w2, (hid, hid, 1, 1)), ("b2", b2, (hid,)), ("W3", w3, (2, hid, 1, 1)), ("b3", b3, (2,)))
-        ws = []
-        for nm, t, shp in shapes:
-            t = _need_cuda_f32(nm, t.detach())
-            _expect(nm, t, shp)
-            ws.append(t)
+        ws = _need_weights(shapes)
         dev = _same_device(("cost", cost), ("invariant", invariant), ("prev_gmm", prev_gmm),
                            *((nm, t) for (nm, _, _), t in zip(shapes, ws)))
         packed = torch.empty(nbytes, device=dev, dtype=torch.uint8)
@@ -658,10 +645,8 @@ class GnetHeadTrain(torch.autograd.Function):
         a = _lib.GnetTrainArgs(B=B, D=D, H=H, W=W, cost=cost.data_ptr(), invariant=invariant.data_ptr(),
                                packed_weights=packed.data_ptr(), prev_gmm=prev_gmm.data_ptr(), scratch=scratch.data_ptr(),
                                out=out.data_ptr(), saved=saved.data_ptr())
-        with torch.cuda.device(dev):
-            check(lib().magnet_gnet_pack_train_weights_f32(*(t.data_ptr() for t in ws), D, packed.data_ptr(), _stream(dev)),
-                  "magnet_gnet_pack_train_weights_f32")
-            check(lib().magnet_gnet_train_fwd_f32(C.byref(a), _stream(dev)), "magnet_gnet_train_fwd_f32")
+        _launch(dev, "magnet_gnet_pack_train_weights_f32", *(t.data_ptr() for t in ws), D, packed.data_ptr())
+        _launch(dev, "magnet_gnet_train_fwd_f32", C.byref(a))
         ctx.save_for_backward(cost, prev_gmm, packed, saved)
         return out
 
@@ -686,8 +671,7 @@ class GnetHeadTrain(torch.autograd.Function):
                                workspace=ws.data_ptr(), grad_invariant=g_inv.data_ptr(), grad_w0_cost=ptr(g[0]),
                                grad_w1=ptr(g[1]), grad_b1=ptr(g[2]), grad_w2=ptr(g[3]), grad_b2=ptr(g[4]),
                                grad_w3=ptr(g[5]), grad_b3=ptr(g[6]), grad_prev=ptr(g_prev))
-        with torch.cuda.device(dev):
-            check(lib().magnet_gnet_bwd_f32(C.byref(a), _stream(dev)), "magnet_gnet_bwd_f32")
+        _launch(dev, "magnet_gnet_bwd_f32", C.byref(a))
         return (None, g_inv if need[1] else None, *g, g_prev)
 
 
@@ -716,9 +700,8 @@ class ConvexUpsample(torch.autograd.Function):
             raise _lib.MagnetError(f"up_mask must be (B, 9*k*k, H, W) = {(B, 9 * k * k, H, W)}, got {tuple(up_mask.shape)}")
         out = torch.empty(B, CH, k * H, k * W, device=depth.device, dtype=torch.float32)
         dev = _same_device(("depth", depth), ("up_mask", up_mask))
-        with torch.cuda.device(dev):
-            check(lib().magnet_convex_upsample_fwd_f32(depth.data_ptr(), up_mask.data_ptr(), B, CH, H, W, k,
-                                                       out.data_ptr(), _stream(dev)), "magnet_convex_upsample_fwd_f32")
+        _launch(dev, "magnet_convex_upsample_fwd_f32", depth.data_ptr(), up_mask.data_ptr(), B, CH, H, W, k,
+                out.data_ptr())
         ctx.save_for_backward(depth, up_mask)
         ctx.k = k
         return out
@@ -730,10 +713,8 @@ class ConvexUpsample(torch.autograd.Function):
         B, CH, H, W = depth.shape
         g_depth = torch.zeros_like(depth)
         g_mask = torch.empty_like(up_mask)
-        with torch.cuda.device(depth.device):
-            check(lib().magnet_convex_upsample_bwd_f32(grad_out.data_ptr(), depth.data_ptr(), up_mask.data_ptr(), B, CH, H,
-                                                       W, ctx.k, g_depth.data_ptr(), g_mask.data_ptr(),
-                                                       _stream(depth.device)), "magnet_convex_upsample_bwd_f32")
+        _launch(depth.device, "magnet_convex_upsample_bwd_f32", grad_out.data_ptr(), depth.data_ptr(),
+                up_mask.data_ptr(), B, CH, H, W, ctx.k, g_depth.data_ptr(), g_mask.data_ptr())
         return g_depth, g_mask, None
 
 
@@ -746,26 +727,33 @@ def mask_weights_bytes(k: int = 4) -> int:
     return int(lib().magnet_mask_weights_bytes(int(k)))
 
 
+def _is_conv(c, cin, cout, ksize: int) -> bool:
+    """A biased Conv2d cout <- cin (cin None: any) with a ksize x ksize kernel, stride 1, 'same' zero padding."""
+    pad = ksize // 2
+    return (isinstance(c, torch.nn.Conv2d) and c.bias is not None and (cin is None or c.in_channels == cin)
+            and c.out_channels == cout and c.kernel_size == (ksize, ksize) and c.padding == (pad, pad)
+            and c.stride == (1, 1) and c.dilation == (1, 1) and c.groups == 1 and c.padding_mode == "zeros")
+
+
+def _conv_chain(seq, *couts):
+    """The convolutions of Conv(*,128,3), then ReLU, Conv(128,cout,1) for each of ``couts`` (every hidden one 128
+    wide), or None."""
+    hid = _lib.MAGNET_HIDDEN_CHANNELS
+    if not isinstance(seq, torch.nn.Sequential) or len(seq) != 2 * len(couts) + 1:
+        return None
+    if not all(isinstance(seq[i], torch.nn.ReLU) for i in range(1, len(seq), 2)):
+        return None
+    convs = [seq[i] for i in range(0, len(seq), 2)]
+    if not (_is_conv(convs[0], None, hid, 3) and all(_is_conv(c, hid, cout, 1) for c, cout in zip(convs[1:], couts))):
+        return None
+    return convs
+
+
 def mask_head_layers(mask_head):
     """The four convolutions of a mask head with the reference's structure (MAGNET.py:111-118): Conv(*,128,3), ReLU,
     Conv(128,128,1), ReLU, Conv(128,128,1), ReLU, Conv(128,144,1), every convolution with a bias.  None otherwise."""
     hid = _lib.MAGNET_HIDDEN_CHANNELS
-    if not isinstance(mask_head, torch.nn.Sequential) or len(mask_head) != 7:
-        return None
-    convs, relus = [mask_head[i] for i in (0, 2, 4, 6)], [mask_head[i] for i in (1, 3, 5)]
-    if not all(isinstance(c, torch.nn.Conv2d) and c.bias is not None for c in convs):
-        return None
-    if not all(isinstance(r, torch.nn.ReLU) for r in relus):
-        return None
-    c0, c1, c2, c3 = convs
-    if not (c0.out_channels == hid and c0.kernel_size == (3, 3) and c0.padding == (1, 1) and c0.stride == (1, 1)
-            and c0.dilation == (1, 1) and c0.groups == 1 and c0.padding_mode == "zeros"):
-        return None
-    for c, cout in ((c1, hid), (c2, hid), (c3, 9 * 4 * 4)):
-        if not (c.in_channels == hid and c.out_channels == cout and c.kernel_size == (1, 1) and c.padding == (0, 0)
-                and c.stride == (1, 1) and c.groups == 1):
-            return None
-    return convs
+    return _conv_chain(mask_head, hid, hid, 9 * 4 * 4)
 
 
 def pack_mask_weights(mask_head) -> torch.Tensor:
@@ -783,9 +771,7 @@ def pack_mask_weights(mask_head) -> torch.Tensor:
                                                   ("b2", c2.bias), ("W3", c3.weight), ("b3", c3.bias))]
     dev = _same_device(*((f"weight {i}", t) for i, t in enumerate(ts)))
     out = torch.empty(mask_weights_bytes(4), device=dev, dtype=torch.uint8)
-    with torch.cuda.device(dev):
-        check(lib().magnet_mask_pack_weights_f32(*(t.data_ptr() for t in ts), out.data_ptr(), _stream(dev)),
-              "magnet_mask_pack_weights_f32")
+    _launch(dev, "magnet_mask_pack_weights_f32", *(t.data_ptr() for t in ts), out.data_ptr())
     return out
 
 
@@ -806,57 +792,33 @@ def mask_upsample(pre0: torch.Tensor, packed: torch.Tensor, preds, k: int = 4) -
         raise _lib.MagnetError(f"pre0 must be (B,{_lib.MAGNET_HIDDEN_CHANNELS},H,W), got {tuple(pre0.shape)}")
     B, _, H, W = pre0.shape
     nbytes = mask_weights_bytes(4)
-    if not (isinstance(packed, torch.Tensor) and packed.is_cuda and packed.dtype == torch.uint8
-            and packed.is_contiguous() and packed.numel() == nbytes):
+    if not _is_packed(packed, (nbytes,)):
         raise _lib.MagnetError(f"packed must be a pack_mask_weights buffer ({nbytes} bytes)")
-    for i, p in enumerate(preds):
-        preds[i] = _need_cuda_f32(f"preds[{i}]", p)
-        _expect(f"preds[{i}]", preds[i], (B, 2, H, W))
+    preds = _need_preds("preds", preds, (B, 2, H, W))
     dev = _same_device(("pre0", pre0), ("packed", packed), *((f"preds[{i}]", p) for i, p in enumerate(preds)))
     outs = [torch.empty(B, 2, 4 * H, 4 * W, device=dev, dtype=torch.float32) for _ in preds]
     n = _lib.MAGNET_MASK_MAX_PRED
-    with torch.cuda.device(dev):
-        for c in range(0, len(preds), n):
-            ps, os_ = preds[c:c + n], outs[c:c + n]
-            pp = (C.c_void_p * len(ps))(*[p.data_ptr() for p in ps])
-            op = (C.c_void_p * len(os_))(*[o.data_ptr() for o in os_])
-            a = _lib.MaskUpsampleArgs(P=len(ps), B=B, H=H, W=W, k=4, pre0=pre0.data_ptr(), packed_weights=packed.data_ptr(),
-                                      pred=C.cast(pp, C.POINTER(C.c_void_p)), out=C.cast(op, C.POINTER(C.c_void_p)))
-            check(lib().magnet_mask_upsample_f32(C.byref(a), _stream(dev)), "magnet_mask_upsample_f32")
+    for c in range(0, len(preds), n):
+        ps, os_ = preds[c:c + n], outs[c:c + n]
+        pp = (C.c_void_p * len(ps))(*[p.data_ptr() for p in ps])
+        op = (C.c_void_p * len(os_))(*[o.data_ptr() for o in os_])
+        a = _lib.MaskUpsampleArgs(P=len(ps), B=B, H=H, W=W, k=4, pre0=pre0.data_ptr(), packed_weights=packed.data_ptr(),
+                                  pred=C.cast(pp, C.POINTER(C.c_void_p)), out=C.cast(op, C.POINTER(C.c_void_p)))
+        _launch(dev, "magnet_mask_upsample_f32", C.byref(a))
     return outs
-
-
-def _is_conv(c, cin, cout, ksize: int) -> bool:
-    """A biased Conv2d cout <- cin (cin None: any) with a ksize x ksize kernel, stride 1, 'same' zero padding."""
-    pad = ksize // 2
-    return (isinstance(c, torch.nn.Conv2d) and c.bias is not None and (cin is None or c.in_channels == cin)
-            and c.out_channels == cout and c.kernel_size == (ksize, ksize) and c.padding == (pad, pad)
-            and c.stride == (1, 1) and c.dilation == (1, 1) and c.groups == 1 and c.padding_mode == "zeros")
-
-
-def _dnet_chain(seq, cout):
-    """The three convolutions of Conv(*,128,3), ReLU, Conv(128,128,1), ReLU, Conv(128,cout,1), or None."""
-    hid = _lib.MAGNET_HIDDEN_CHANNELS
-    if not isinstance(seq, torch.nn.Sequential) or len(seq) != 5:
-        return None
-    if not (isinstance(seq[1], torch.nn.ReLU) and isinstance(seq[3], torch.nn.ReLU)):
-        return None
-    c0, c1, c2 = seq[0], seq[2], seq[4]
-    if not (_is_conv(c0, None, hid, 3) and _is_conv(c1, hid, hid, 1) and _is_conv(c2, hid, cout, 1)):
-        return None
-    return [c0, c1, c2]
 
 
 def dnet_head_layers(depth_head, mask_head=None):
     """The convolutions of D-Net's heads with the reference's structure (D_dense_depth.py:148-160): depth_head =
     Conv(*,128,3), ReLU, Conv(128,128,1), ReLU, Conv(128,2,1), and, when given, mask_head = the same with a last
     Conv(128,144,1) (k = 4), every convolution with a bias.  -> (depth convs, mask convs or None), or None."""
-    d = _dnet_chain(depth_head, 2)
+    hid = _lib.MAGNET_HIDDEN_CHANNELS
+    d = _conv_chain(depth_head, hid, 2)
     if d is None:
         return None
     if mask_head is None:
         return d, None
-    m = _dnet_chain(mask_head, 9 * 4 * 4)
+    m = _conv_chain(mask_head, hid, 9 * 4 * 4)
     return None if m is None else (d, m)
 
 
@@ -884,16 +846,13 @@ def pack_dnet_weights(depth_head, mask_head=None) -> torch.Tensor:
     dev = _same_device(*zip([nm for nm, _ in named], ts))
     out = torch.empty(dnet_weights_bytes(k), device=dev, dtype=torch.uint8)
     ptrs = [t.data_ptr() for t in ts] + [None] * (8 - len(ts))
-    with torch.cuda.device(dev):
-        check(lib().magnet_dnet_pack_weights_f32(*ptrs, k, out.data_ptr(), _stream(dev)), "magnet_dnet_pack_weights_f32")
+    _launch(dev, "magnet_dnet_pack_weights_f32", *ptrs, k, out.data_ptr())
     return out
 
 
 def _check_dnet_packed(packed, k: int) -> None:
     nbytes = dnet_weights_bytes(k)
-    ok = (isinstance(packed, torch.Tensor) and packed.is_cuda and packed.dtype == torch.uint8 and packed.is_contiguous()
-          and (packed.numel() == nbytes if k == 4 else packed.numel() in (nbytes, dnet_weights_bytes(4))))
-    if not ok:
+    if not _is_packed(packed, (nbytes,) if k == 4 else (nbytes, dnet_weights_bytes(4))):
         what = "with the mask head " if k == 4 else ""
         raise _lib.MagnetError(f"packed must be a pack_dnet_weights buffer {what}({nbytes} bytes"
                                + (")" if k == 4 else f" or {dnet_weights_bytes(4)})"))
@@ -916,9 +875,7 @@ def dnet_depth(pre_d: torch.Tensor, packed: torch.Tensor, sigma: bool) -> torch.
     B, _, H, W = pre_d.shape
     dev = _same_device(("pre_d", pre_d), ("packed", packed))
     out = torch.empty(B, 2, H, W, device=dev, dtype=torch.float32)
-    with torch.cuda.device(dev):
-        check(lib().magnet_dnet_depth_f32(pre_d.data_ptr(), packed.data_ptr(), B, H, W, int(bool(sigma)), out.data_ptr(),
-                                          _stream(dev)), "magnet_dnet_depth_f32")
+    _launch(dev, "magnet_dnet_depth_f32", pre_d.data_ptr(), packed.data_ptr(), B, H, W, int(bool(sigma)), out.data_ptr())
     return out
 
 
@@ -932,13 +889,11 @@ def dnet_upsample(pre_m: torch.Tensor, packed: torch.Tensor, raw: torch.Tensor, 
     pre_m = _dnet_pre("pre_m", pre_m)
     _check_dnet_packed(packed, 4)
     B, _, H, W = pre_m.shape
-    raw = _need_cuda_f32("raw", raw)
-    _expect("raw", raw, (B, 2, H, W))
+    raw = _need_cuda_f32("raw", raw, (B, 2, H, W))
     dev = _same_device(("pre_m", pre_m), ("packed", packed), ("raw", raw))
     out = torch.empty(B, 2, 4 * H, 4 * W, device=dev, dtype=torch.float32)
-    with torch.cuda.device(dev):
-        check(lib().magnet_dnet_upsample_f32(pre_m.data_ptr(), packed.data_ptr(), raw.data_ptr(), B, H, W, 4,
-                                             out.data_ptr(), _stream(dev)), "magnet_dnet_upsample_f32")
+    _launch(dev, "magnet_dnet_upsample_f32", pre_m.data_ptr(), packed.data_ptr(), raw.data_ptr(), B, H, W, 4,
+            out.data_ptr())
     return out
 
 
@@ -970,21 +925,10 @@ class MaskLossTrain(torch.autograd.Function):
         B, _, H, W = pre0.shape
         shapes = (("W1", w1, (hid, hid, 1, 1)), ("b1", b1, (hid,)), ("W2", w2, (hid, hid, 1, 1)), ("b2", b2, (hid,)),
                   ("W3", w3, (nout, hid, 1, 1)), ("b3", b3, (nout,)))
-        ws = []
-        for nm, t, shp in shapes:
-            t = _need_cuda_f32(nm, t.detach())
-            _expect(nm, t, shp)
-            ws.append(t)
-        ps = []
-        for i, p in enumerate(preds):
-            p = _need_cuda_f32(f"preds[{i}]", p.detach())
-            _expect(f"preds[{i}]", p, (B, 2, H, W))
-            ps.append(p)
-        gt = _need_cuda_f32("gt", gt.detach())
-        _expect("gt", gt, (B, 1, 4 * H, 4 * W))
-        if gt_mask_u8.dtype != torch.uint8 or not gt_mask_u8.is_cuda or tuple(gt_mask_u8.shape) != (B, 1, 4 * H, 4 * W):
-            raise _lib.MagnetError("gt_mask must be a CUDA uint8 tensor of shape (B,1,4H,4W)")
-        gt_mask_u8 = gt_mask_u8.contiguous()
+        ws = _need_weights(shapes)
+        ps = _need_preds("preds", (p.detach() for p in preds), (B, 2, H, W))
+        gt = _need_cuda_f32("gt", gt.detach(), (B, 1, 4 * H, 4 * W))
+        gt_mask_u8 = _need_cuda_u8_mask("gt_mask", gt_mask_u8, (B, 1, 4 * H, 4 * W), "(B,1,4H,4W)")
         dev = _same_device(("pre0", pre0), ("gt", gt), ("gt_mask", gt_mask_u8),
                            *((nm, t) for (nm, _, _), t in zip(shapes, ws)), *((f"preds[{i}]", p) for i, p in enumerate(ps)))
         need = ctx.needs_input_grad
@@ -1001,10 +945,8 @@ class MaskLossTrain(torch.autograd.Function):
                                pred=C.cast(pp, C.POINTER(C.c_void_p)), gt=gt.data_ptr(), gt_mask=gt_mask_u8.data_ptr(),
                                pred_scale=C.cast(scale, C.POINTER(C.c_float)), save_maps=int(save_maps),
                                pred_grad=int(pred_grad), partial=partial.data_ptr(), saved=saved.data_ptr())
-        with torch.cuda.device(dev):
-            check(lib().magnet_mask_pack_train_weights_f32(*(t.data_ptr() for t in ws), packed.data_ptr(), _stream(dev)),
-                  "magnet_mask_pack_train_weights_f32")
-            check(lib().magnet_mask_train_fwd_f32(C.byref(a), _stream(dev)), "magnet_mask_train_fwd_f32")
+        _launch(dev, "magnet_mask_pack_train_weights_f32", *(t.data_ptr() for t in ws), packed.data_ptr())
+        _launch(dev, "magnet_mask_train_fwd_f32", C.byref(a))
         ctx.save_for_backward(packed, saved)
         ctx.shape = (P, B, H, W)
         # as magnet_loss sums its terms: per prediction the float64 sum of the partials, in fp32 over count, weighted
@@ -1036,8 +978,7 @@ class MaskLossTrain(torch.autograd.Function):
                                grad_scale=grad_scale.data_ptr(), workspace=ws.data_ptr(), grad_pre0=ptr(g_pre0),
                                grad_w1=ptr(g[0]), grad_b1=ptr(g[1]), grad_w2=ptr(g[2]), grad_b2=ptr(g[3]),
                                grad_w3=ptr(g[4]), grad_b3=ptr(g[5]), grad_pred=C.cast(gp, C.POINTER(C.c_void_p)))
-        with torch.cuda.device(dev):
-            check(lib().magnet_mask_bwd_f32(C.byref(a), _stream(dev)), "magnet_mask_bwd_f32")
+        _launch(dev, "magnet_mask_bwd_f32", C.byref(a))
         return (g_pre0, *g, None, None, None, None, None, *g_preds)
 
 
@@ -1080,14 +1021,11 @@ class UpsampleNLL(torch.autograd.Function):
             raise _lib.MagnetError(f"depth must be (B,2,H,W) [mu, sigma], got {tuple(depth.shape)}")
         _expect("up_mask", up_mask, (B, 9 * k * k, H, W))
         _expect("gt", gt, (B, 1, k * H, k * W))
-        if gt_mask_u8.dtype != torch.uint8 or not gt_mask_u8.is_cuda or tuple(gt_mask_u8.shape) != (B, 1, k * H, k * W):
-            raise _lib.MagnetError("gt_mask must be a CUDA uint8 tensor of shape (B,1,k*H,k*W)")
-        gt_mask_u8 = gt_mask_u8.contiguous()
+        gt_mask_u8 = _need_cuda_u8_mask("gt_mask", gt_mask_u8, (B, 1, k * H, k * W), "(B,1,k*H,k*W)")
         dev = _same_device(("depth", depth), ("up_mask", up_mask), ("gt", gt), ("gt_mask", gt_mask_u8))
         partial = torch.empty(lib().magnet_upsample_nll_partials(B, H, W, k), device=dev, dtype=torch.float32)
-        with torch.cuda.device(dev):
-            check(lib().magnet_upsample_nll_fwd_f32(depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(), gt_mask_u8.data_ptr(),
-                                                    B, H, W, k, partial.data_ptr(), _stream(dev)), "magnet_upsample_nll_fwd_f32")
+        _launch(dev, "magnet_upsample_nll_fwd_f32", depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(),
+                gt_mask_u8.data_ptr(), B, H, W, k, partial.data_ptr())
         ctx.save_for_backward(depth, up_mask, gt, gt_mask_u8)
         ctx.k, ctx.count = k, float(count)
         return partial.sum(dtype=torch.float64).to(torch.float32) / ctx.count
@@ -1099,10 +1037,8 @@ class UpsampleNLL(torch.autograd.Function):
         g_depth = torch.zeros_like(depth)
         g_mask = torch.empty_like(up_mask)
         scale = float(grad_out) / ctx.count
-        with torch.cuda.device(depth.device):
-            check(lib().magnet_upsample_nll_bwd_f32(depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(), gtm.data_ptr(), scale,
-                                                    B, H, W, ctx.k, g_depth.data_ptr(), g_mask.data_ptr(),
-                                                    _stream(depth.device)), "magnet_upsample_nll_bwd_f32")
+        _launch(depth.device, "magnet_upsample_nll_bwd_f32", depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(),
+                gtm.data_ptr(), scale, B, H, W, ctx.k, g_depth.data_ptr(), g_mask.data_ptr())
         return g_depth, g_mask, None, None, None, None
 
 
@@ -1137,15 +1073,11 @@ class FnetL1Loss(torch.autograd.Function):
         if len(karr) != D:
             raise _lib.MagnetError(f"{len(karr)} plane depths for {D} score planes")
         _expect("gt", gt, (B, 1, H, W))
-        if mask_u8.dtype != torch.uint8 or not mask_u8.is_cuda or tuple(mask_u8.shape) != (B, 1, H, W):
-            raise _lib.MagnetError("mask must be a CUDA uint8 tensor of shape (B,1,H,W)")
-        mask_u8 = mask_u8.contiguous()
+        mask_u8 = _need_cuda_u8_mask("mask", mask_u8, (B, 1, H, W), "(B,1,H,W)")
         dev = _same_device(("scores", scores), ("gt", gt), ("mask", mask_u8))
         partial = torch.empty(lib().magnet_fnet_l1_partials(B, H, W), device=dev, dtype=torch.float32)
-        with torch.cuda.device(dev):
-            check(lib().magnet_fnet_l1_fwd_f32(scores.data_ptr(), C.cast(karr, C.c_void_p), gt.data_ptr(),
-                                               mask_u8.data_ptr(), B, D, H, W, partial.data_ptr(), _stream(dev)),
-                  "magnet_fnet_l1_fwd_f32")
+        _launch(dev, "magnet_fnet_l1_fwd_f32", scores.data_ptr(), C.cast(karr, C.c_void_p), gt.data_ptr(),
+                mask_u8.data_ptr(), B, D, H, W, partial.data_ptr())
         ctx.save_for_backward(scores, gt, mask_u8)
         ctx.karr, ctx.count = karr, count
         return partial.sum(dtype=torch.float64).to(torch.float32) / count
@@ -1160,10 +1092,8 @@ class FnetL1Loss(torch.autograd.Function):
             gs, scale = (grad_out / ctx.count).to(torch.float32).contiguous(), 1.0
         else:
             gs, scale = grad_out.to(torch.float32).contiguous(), 1.0 / float(ctx.count)
-        with torch.cuda.device(scores.device):
-            check(lib().magnet_fnet_l1_bwd_f32(scores.data_ptr(), C.cast(ctx.karr, C.c_void_p), gt.data_ptr(),
-                                               mask_u8.data_ptr(), scale, gs.data_ptr(), B, D, H, W, g.data_ptr(),
-                                               _stream(scores.device)), "magnet_fnet_l1_bwd_f32")
+        _launch(scores.device, "magnet_fnet_l1_bwd_f32", scores.data_ptr(), C.cast(ctx.karr, C.c_void_p), gt.data_ptr(),
+                mask_u8.data_ptr(), scale, gs.data_ptr(), B, D, H, W, g.data_ptr())
         return g, None, None, None, None
 
 
@@ -1200,9 +1130,8 @@ def plane_depth(volume: torch.Tensor, planes, *, scores: bool) -> torch.Tensor:
     if len(karr) != D:
         raise _lib.MagnetError(f"{len(karr)} plane depths for {D} planes of the volume")
     out = torch.empty(B, 1, H, W, device=volume.device, dtype=torch.float32)
-    with torch.cuda.device(volume.device):
-        check(lib().magnet_plane_depth_f32(volume.data_ptr(), C.cast(karr, C.c_void_p), B, D, H, W, int(bool(scores)),
-                                           out.data_ptr(), _stream(volume.device)), "magnet_plane_depth_f32")
+    _launch(volume.device, "magnet_plane_depth_f32", volume.data_ptr(), C.cast(karr, C.c_void_p), B, D, H, W,
+            int(bool(scores)), out.data_ptr())
     return out
 
 
@@ -1215,9 +1144,8 @@ def relative_poses(ext_ref: torch.Tensor, ext_nghbr: torch.Tensor):
     poses = torch.empty(B, V, 4, 4, device=ext_ref.device, dtype=torch.float32)
     valid = torch.empty(B, V, device=ext_ref.device, dtype=torch.int32)
     dev = _same_device(("ext_ref", ext_ref), ("ext_nghbr", ext_nghbr))
-    with torch.cuda.device(dev):
-        check(lib().magnet_relative_poses_f32(ext_ref.data_ptr(), ext_nghbr.data_ptr(), B, V, poses.data_ptr(),
-                                              valid.data_ptr(), _stream(dev)), "magnet_relative_poses_f32")
+    _launch(dev, "magnet_relative_poses_f32", ext_ref.data_ptr(), ext_nghbr.data_ptr(), B, V, poses.data_ptr(),
+            valid.data_ptr())
     return poses, valid
 
 
@@ -1235,9 +1163,8 @@ def camera_rays(raw_intrinsics: torch.Tensor, H: int, W: int):
     B = raw_intrinsics.shape[0]
     intM = torch.empty(B, 3, 3, device=raw_intrinsics.device, dtype=torch.float32)
     rays = torch.empty(B, 3, H * W, device=raw_intrinsics.device, dtype=torch.float32)
-    with torch.cuda.device(raw_intrinsics.device):
-        check(lib().magnet_camera_rays_f32(raw_intrinsics.data_ptr(), B, H, W, intM.data_ptr(), rays.data_ptr(),
-                                           _stream(raw_intrinsics.device)), "magnet_camera_rays_f32")
+    _launch(raw_intrinsics.device, "magnet_camera_rays_f32", raw_intrinsics.data_ptr(), B, H, W, intM.data_ptr(),
+            rays.data_ptr())
     return {"intM": intM, "unit_ray_array_2D": rays}
 
 
@@ -1296,14 +1223,11 @@ def depth_metrics(pred_or_list, gt: torch.Tensor, *, min_depth: float, max_depth
         k = int(k)
         if k < 1 or H % k or W % k:
             raise _lib.MagnetError(f"k = {k} must be >= 1 and divide the GT size {H}x{W}")
-        up_mask = _need_cuda_f32("up_mask", up_mask)
-        _expect("up_mask", up_mask, (B, 9 * k * k, H // k, W // k))
+        up_mask = _need_cuda_f32("up_mask", up_mask, (B, 9 * k * k, H // k, W // k))
         pshape = (B, 2, H // k, W // k)
     else:
         pshape = (B, 2, H, W)
-    for i, p in enumerate(preds):
-        preds[i] = _need_cuda_f32(f"pred[{i}]", p)
-        _expect(f"pred[{i}]", preds[i], pshape)
+    preds = _need_preds("pred", preds, pshape)
     dev = _same_device(("gt", gt), ("up_mask", up_mask), *((f"pred[{i}]", p) for i, p in enumerate(preds)))
     r0, r1, c0, c1 = crop_box(crop, H, W)
     ptrs = (C.c_void_p * len(preds))(*[p.data_ptr() for p in preds])
@@ -1311,23 +1235,26 @@ def depth_metrics(pred_or_list, gt: torch.Tensor, *, min_depth: float, max_depth
                               min_depth=float(min_depth), max_depth=float(max_depth),
                               pred=C.cast(ptrs, C.POINTER(C.c_void_p)), up_mask=up_mask.data_ptr() if k else None,
                               gt=gt.data_ptr())
-    n = lib().magnet_depth_metrics_workspace(C.byref(a))
-    if n < 0:
-        check(int(n), "magnet_depth_metrics_workspace")
-    workspace = torch.empty(int(n), device=dev, dtype=torch.float64)
-    out = torch.empty(len(preds), B, _lib.MAGNET_METRICS_COLS, device=dev, dtype=torch.float64)
-    a.workspace, a.out = workspace.data_ptr(), out.data_ptr()
     fn = "magnet_depth_metrics_var_f32" if variance else "magnet_depth_metrics_f32"
-    with torch.cuda.device(dev):
-        check(getattr(lib(), fn)(C.byref(a), _stream(dev)), fn)
+    return _run_depth_metrics(dev, a, "magnet_depth_metrics_workspace", fn)
+
+
+def _run_depth_metrics(dev, a, workspace_fn: str, fn: str) -> torch.Tensor:
+    """The workspace and the (P,B,13) output of the checked metrics arguments ``a``, then the launch of ``fn``."""
+    n = getattr(lib(), workspace_fn)(C.byref(a))
+    if n < 0:
+        check(int(n), workspace_fn)
+    workspace = torch.empty(int(n), device=dev, dtype=torch.float64)
+    out = torch.empty(a.P, a.B, _lib.MAGNET_METRICS_COLS, device=dev, dtype=torch.float64)
+    a.workspace, a.out = workspace.data_ptr(), out.data_ptr()
+    _launch(dev, fn, C.byref(a))
     return out
 
 
 def _depth_metrics_nearest(preds, gt, min_depth, max_depth, crop):
     """The nearest form of ``depth_metrics``: ``preds`` (B,1,h,w) each, ``gt`` the checked (B,1,H,W) GT."""
     B, _, H, W = gt.shape
-    for i, p in enumerate(preds):
-        preds[i] = _need_cuda_f32(f"pred[{i}]", p)
+    preds = _need_preds("pred", preds)
     pshape = tuple(preds[0].shape)
     if len(pshape) != 4 or pshape[:2] != (B, 1) or not (1 <= pshape[2] <= H and 1 <= pshape[3] <= W):
         raise _lib.MagnetError(f"pred[0] must be (B,1,h,w) with B = {B}, h <= {H}, w <= {W}, got {pshape}")
@@ -1339,12 +1266,4 @@ def _depth_metrics_nearest(preds, gt, min_depth, max_depth, crop):
     a = _lib.DepthMetricsNearestArgs(P=len(preds), B=B, H=H, W=W, h=pshape[2], w=pshape[3], row0=r0, row1=r1, col0=c0,
                                      col1=c1, min_depth=float(min_depth), max_depth=float(max_depth),
                                      pred=C.cast(ptrs, C.POINTER(C.c_void_p)), gt=gt.data_ptr())
-    n = lib().magnet_depth_metrics_nearest_workspace(C.byref(a))
-    if n < 0:
-        check(int(n), "magnet_depth_metrics_nearest_workspace")
-    workspace = torch.empty(int(n), device=dev, dtype=torch.float64)
-    out = torch.empty(len(preds), B, _lib.MAGNET_METRICS_COLS, device=dev, dtype=torch.float64)
-    a.workspace, a.out = workspace.data_ptr(), out.data_ptr()
-    with torch.cuda.device(dev):
-        check(lib().magnet_depth_metrics_nearest_f32(C.byref(a), _stream(dev)), "magnet_depth_metrics_nearest_f32")
-    return out
+    return _run_depth_metrics(dev, a, "magnet_depth_metrics_nearest_workspace", "magnet_depth_metrics_nearest_f32")

@@ -27,6 +27,40 @@ def test_library_loads_and_exports_every_declared_symbol():
     assert C.sizeof(CostArgs) == 12 * 4 + 9 * 8
 
 
+def test_struct_mirrors_match_the_header():
+    """Every ctypes mirror names its header struct's fields in the header's order, each an int32, a float or a
+    pointer as the header declares it: a field out of order would pass its size check and corrupt memory silently."""
+    mirrors = {"magnet_cost_args": _lib.CostArgs, "magnet_cost_f_bwd_args": _lib.CostFBwdArgs,
+               "magnet_cost_bwd_args": _lib.CostBwdArgs, "magnet_cost_geom_bwd_args": _lib.CostGeomBwdArgs,
+               "magnet_gnet_args": _lib.GnetArgs, "magnet_gnet_train_args": _lib.GnetTrainArgs,
+               "magnet_mask_upsample_args": _lib.MaskUpsampleArgs, "magnet_mask_train_args": _lib.MaskTrainArgs,
+               "magnet_depth_metrics_args": _lib.DepthMetricsArgs,
+               "magnet_depth_metrics_nearest_args": _lib.DepthMetricsNearestArgs}
+    header = open(os.path.join(ROOT, "include", "magnet_b200.h")).read()
+    header = re.sub(r"/\*.*?\*/", "", header, flags=re.S)
+    structs = dict(re.findall(r"typedef struct (magnet_\w+_args) \{(.*?)\}", header, flags=re.S))
+    assert set(structs) == set(mirrors), set(structs) ^ set(mirrors)
+
+    def kind(ctype):
+        if ctype is C.c_int32:
+            return "int32"
+        if ctype is C.c_float:
+            return "float"
+        assert ctype is C.c_void_p or issubclass(ctype, C._Pointer), ctype
+        return "pointer"
+
+    for name, body in structs.items():
+        declared = []
+        for decl in filter(None, (d.strip() for d in body.split(";"))):
+            m = re.fullmatch(r"(.*?[\s*])(\w+(?:\s*,\s*\w+)*)", decl, flags=re.S)
+            assert m, (name, decl)
+            ctype = m.group(1)
+            k = "pointer" if "*" in ctype else {"int32_t": "int32", "float": "float"}[ctype.split()[-1]]
+            declared += [(f.strip(), k) for f in m.group(2).split(",")]
+        mirrored = [(f, kind(t)) for f, t in mirrors[name]._fields_]
+        assert mirrored == declared, name
+
+
 def test_cost_args_validation_without_gpu():
     L = _lib.lib()
     assert L.magnet_cost_volume_f32(None, None) == _lib.ERR_NULL
