@@ -227,6 +227,7 @@ def matching_loop(plan: MatchingPlan, ref_gmms: torch.Tensor, x_d3: torch.Tensor
     preds = [ref_gmms]
     split = isinstance(g_net_convs, GNET)
     inv = g_net_convs.invariant_part(x_d3, len(karr)) if split else None
+    convs = _split_gnet_convs(g_net_convs, inv, len(karr))    # every cost volume has len(karr) channels
     packed = None
     for _ in range(n_iter):
         cur = preds[-1].detach().float()                   # a half ref_gmms (autocast) enters the update as fp32
@@ -235,12 +236,12 @@ def matching_loop(plan: MatchingPlan, ref_gmms: torch.Tensor, x_d3: torch.Tensor
                 cv = plan.cost(cur, karr, variant=variant)
         else:
             cv = plan.cost(cur, karr, variant=variant)
-        if fused_gnet_applies(g_net_convs, cv, inv):
+        if _fused_rule(convs, (cv, inv), train=False):     # fused_gnet_applies
             if packed is None:                             # the weights are read once per call
                 packed = ops.pack_gnet_weights(g_net_convs, cv.shape[1])
             preds.append(ops.gnet_update(cv, inv, packed, cur))
             continue
-        if fused_train and fused_gnet_trains(g_net_convs, cv, inv):
+        if fused_train and _fused_rule(convs, (cv, inv), train=True, no_grad=(cv,)):   # fused_gnet_trains
             preds.append(ops.gnet_head_train(cv, inv, g_net_convs, cur))
             continue
         raw = g_net_convs.raw_from_parts(cv, inv) if split else g_net_convs(torch.cat([cv, x_d3], dim=1))
@@ -248,38 +249,44 @@ def matching_loop(plan: MatchingPlan, ref_gmms: torch.Tensor, x_d3: torch.Tensor
     return preds
 
 
+def _fused_rule(convs, tensors, *, train: bool, no_grad=()) -> bool:
+    """The policy of every fused head.  ``convs``: the head's recognised convolutions (None: not its structure), whose
+    weights and biases are its parameters; ``tensors``: operands that must be fp32 and whose requires_grad counts.
+    Inference needs nothing to differentiate (grad mode off, or no requires_grad among parameters and tensors); training
+    needs grad mode on, something to differentiate and nothing in ``no_grad`` (operands the fused backward has no
+    gradient for) requiring grad.  Both need CUDA autocast off and fp32 parameters and tensors."""
+    if convs is None:
+        return False
+    params = [p for c in convs for p in (c.weight, c.bias)]
+    grad = torch.is_grad_enabled() and any(t.requires_grad for t in (*params, *tensors))
+    if grad != train or any(t.requires_grad for t in no_grad) or torch.is_autocast_enabled("cuda"):
+        return False
+    return all(t.dtype == torch.float32 for t in (*params, *tensors))
+
+
+def _split_gnet_convs(g_net_convs, inv: Optional[torch.Tensor], D: int):
+    """``ops.gnet_head_layers(g_net_convs, D)`` of a ``GNET`` in the split data flow (``inv`` given) for
+    1 <= D <= MAGNET_MAX_PLANES cost channels, else None."""
+    if not isinstance(g_net_convs, GNET) or inv is None or not 1 <= D <= _lib.MAGNET_MAX_PLANES:
+        return None
+    return ops.gnet_head_layers(g_net_convs, D)
+
+
 def fused_gnet_applies(g_net_convs, cv: torch.Tensor, inv: Optional[torch.Tensor]) -> bool:
     """Whether an iteration of ``matching_loop`` runs the fused G-Net head (``ops.gnet_update``) instead of the module
-    path (``raw_from_parts`` + ``gaussian_update``): the split data flow of a ``GNET``, nothing to differentiate (grad
-    mode off, or no requires_grad among the head's parameters, the cost volume and the invariant), no CUDA autocast,
-    fp32 weights and 1 <= D <= MAGNET_MAX_PLANES cost channels.  The fused head has no backward."""
-    if not isinstance(g_net_convs, GNET) or inv is None:
-        return False
-    params = list(g_net_convs.parameters())
-    if torch.is_grad_enabled() and (cv.requires_grad or inv.requires_grad or any(p.requires_grad for p in params)):
-        return False
-    if torch.is_autocast_enabled("cuda"):
-        return False
-    if any(p.dtype != torch.float32 for p in params) or cv.dtype != torch.float32 or inv.dtype != torch.float32:
-        return False
-    return 1 <= cv.shape[1] <= _lib.MAGNET_MAX_PLANES
+    path (``raw_from_parts`` + ``gaussian_update``): the split data flow of a ``GNET`` that ``ops.gnet_head_layers``
+    recognises for D, nothing to differentiate (grad mode off, or no requires_grad among the head's parameters, the cost
+    volume and the invariant), no CUDA autocast, fp32 weights, volume and invariant and 1 <= D <= MAGNET_MAX_PLANES cost
+    channels.  The fused head has no backward."""
+    return _fused_rule(_split_gnet_convs(g_net_convs, inv, cv.shape[1]), (cv, inv), train=False)
 
 
 def fused_gnet_trains(g_net_convs, cv: torch.Tensor, inv: Optional[torch.Tensor]) -> bool:
     """Whether a training iteration of ``matching_loop(..., fused_train=True)`` runs the differentiable fused head
-    (``ops.gnet_head_train``): the split data flow of a ``GNET``, grad mode on and a head parameter or the invariant
-    requiring grad, a cost volume that does not (the fused backward has no gradient into it), no CUDA autocast, fp32
-    weights and volume and 1 <= D <= MAGNET_MAX_PLANES cost channels."""
-    if not isinstance(g_net_convs, GNET) or inv is None:
-        return False
-    params = list(g_net_convs.parameters())
-    if not torch.is_grad_enabled() or not (inv.requires_grad or any(p.requires_grad for p in params)):
-        return False
-    if cv.requires_grad or torch.is_autocast_enabled("cuda"):
-        return False
-    if any(p.dtype != torch.float32 for p in params) or cv.dtype != torch.float32 or inv.dtype != torch.float32:
-        return False
-    return 1 <= cv.shape[1] <= _lib.MAGNET_MAX_PLANES
+    (``ops.gnet_head_train``): the split data flow of a ``GNET`` that ``ops.gnet_head_layers`` recognises for D, grad
+    mode on and a head parameter or the invariant requiring grad, a cost volume that does not (the fused backward has
+    no gradient into it), no CUDA autocast, fp32 weights, volume and invariant and 1 <= D <= MAGNET_MAX_PLANES."""
+    return _fused_rule(_split_gnet_convs(g_net_convs, inv, cv.shape[1]), (cv, inv), train=True, no_grad=(cv,))
 
 
 def fused_mask_applies(mask_head, pre0: Optional[torch.Tensor], preds, k: int) -> bool:
@@ -287,18 +294,11 @@ def fused_mask_applies(mask_head, pre0: Optional[torch.Tensor], preds, k: int) -
     (``ops.mask_upsample``) instead of ``mask_head(x_d3)`` + ``convex_upsample`` per prediction: a mask head with the
     reference's structure and k == 4, nothing to differentiate (grad mode off, or no requires_grad among the mask
     head's parameters, pre0 and the predictions), no CUDA autocast, fp32 weights, pre0 and predictions.  pre0 may be
-    None when it is not computed yet.  The inference kernel has no backward; training takes the fused path of
-    ``fused_mask_trains``."""
-    if int(k) != 4 or ops.mask_head_layers(mask_head) is None:
-        return False
-    params = list(mask_head.parameters())
-    preds = [preds] if isinstance(preds, torch.Tensor) else list(preds)
-    tensors = preds + ([pre0] if pre0 is not None else [])
-    if torch.is_grad_enabled() and (any(p.requires_grad for p in params) or any(t.requires_grad for t in tensors)):
-        return False
-    if torch.is_autocast_enabled("cuda"):
-        return False
-    return all(p.dtype == torch.float32 for p in params) and all(t.dtype == torch.float32 for t in tensors)
+    None, or the mask head's input x_d3 in its place: without autocast, pre0 = conv(x_d3) is fp32 exactly when x_d3 is
+    and requires grad exactly when x_d3 or a mask-head parameter does.  The inference kernel has no backward; training
+    takes the fused path of ``fused_mask_trains``."""
+    convs = ops.mask_head_layers(mask_head) if int(k) == 4 else None
+    return _fused_rule(convs, ops._pred_list(preds) + ([pre0] if pre0 is not None else []), train=False)
 
 
 def fused_mask_trains(mask_head, pre0: Optional[torch.Tensor], preds, k: int, gt: Optional[torch.Tensor] = None) -> bool:
@@ -306,20 +306,18 @@ def fused_mask_trains(mask_head, pre0: Optional[torch.Tensor], preds, k: int, gt
     loss (``ops.mask_head_loss``) instead of ``mask_head(x_d3)`` + ``magnet_loss``: a mask head with the reference's
     structure and k == 4, grad mode on with something to differentiate (a mask-head parameter, pre0 or a prediction
     requiring grad), 1 <= P <= MAGNET_MASK_MAX_PRED predictions, no CUDA autocast, fp32 weights, pre0, predictions and
-    gt.  pre0 and gt may be None when they are not known yet."""
-    if int(k) != 4 or ops.mask_head_layers(mask_head) is None:
-        return False
-    params = list(mask_head.parameters())
-    preds = [preds] if isinstance(preds, torch.Tensor) else list(preds)
-    if not 1 <= len(preds) <= _lib.MAGNET_MASK_MAX_PRED:
-        return False
-    tensors = preds + ([pre0] if pre0 is not None else [])
-    if not torch.is_grad_enabled() or not (any(p.requires_grad for p in params) or any(t.requires_grad for t in tensors)):
-        return False
-    if torch.is_autocast_enabled("cuda"):
-        return False
-    tensors += [gt] if gt is not None else []
-    return all(p.dtype == torch.float32 for p in params) and all(t.dtype == torch.float32 for t in tensors)
+    gt.  pre0 and gt may be None when they are not known yet; x_d3 may stand for pre0 (``fused_mask_applies``)."""
+    preds = ops._pred_list(preds)
+    fits = int(k) == 4 and 1 <= len(preds) <= _lib.MAGNET_MASK_MAX_PRED and (gt is None or gt.dtype == torch.float32)
+    convs = ops.mask_head_layers(mask_head) if fits else None
+    return _fused_rule(convs, preds + ([pre0] if pre0 is not None else []), train=True)
+
+
+def _dnet_fused_layers(depth_head, mask_head, x_feat: torch.Tensor, k: int):
+    """``ops.dnet_head_layers(depth_head, mask_head)`` where ``fused_dnet_applies`` holds, else None."""
+    layers = ops.dnet_head_layers(depth_head, mask_head) if mask_head is None or int(k) == 4 else None
+    convs = None if layers is None else layers[0] + (layers[1] or [])
+    return layers if _fused_rule(convs, (x_feat,), train=False) else None
 
 
 def fused_dnet_applies(depth_head, mask_head, x_feat: torch.Tensor, k: int) -> bool:
@@ -327,16 +325,7 @@ def fused_dnet_applies(depth_head, mask_head, x_feat: torch.Tensor, k: int) -> b
     the module chain: heads with the reference's structure (``mask_head`` None when it is not run) and k == 4 when the
     mask head is run, nothing to differentiate (grad mode off, or no requires_grad among the heads' parameters and
     x_feat), no CUDA autocast, fp32 weights and x_feat.  The fused kernels have no backward."""
-    if ops.dnet_head_layers(depth_head, mask_head) is None:
-        return False
-    if mask_head is not None and int(k) != 4:
-        return False
-    params = list(depth_head.parameters()) + (list(mask_head.parameters()) if mask_head is not None else [])
-    if torch.is_grad_enabled() and (x_feat.requires_grad or any(p.requires_grad for p in params)):
-        return False
-    if torch.is_autocast_enabled("cuda"):
-        return False
-    return all(p.dtype == torch.float32 for p in params) and x_feat.dtype == torch.float32
+    return _dnet_fused_layers(depth_head, mask_head, x_feat, k) is not None
 
 
 class DnetHead(nn.Module):
@@ -378,8 +367,9 @@ class DnetHead(nn.Module):
     def forward(self, x_feat: torch.Tensor):
         k = self.downsample_ratio
         mask_head = self.mask_head if self.dnet else None
-        if fused_dnet_applies(self.depth_head, mask_head, x_feat, k):
-            packed = ops.pack_dnet_weights(self.depth_head, mask_head)
+        layers = _dnet_fused_layers(self.depth_head, mask_head, x_feat, k)     # fused_dnet_applies
+        if layers is not None:
+            packed = ops._pack_dnet_layers(layers)
             raw = ops.dnet_depth(self._pre(self.depth_head, x_feat), packed, sigma=not self.dnet)
             if not self.dnet:
                 return raw, x_feat
@@ -441,10 +431,8 @@ class MagnetHead(nn.Module):
         if self.fused_upsample:
             preds = self._predictions(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid,
                                       cam_intrins, src_index)
-            if fused_mask_applies(self.mask_head, None, preds, k):
-                pre0 = self.mask_pre(x_d3)
-                if fused_mask_applies(self.mask_head, pre0, preds, k):
-                    return ops.mask_upsample(pre0, ops.pack_mask_weights(self.mask_head), preds, k)
+            if fused_mask_applies(self.mask_head, x_d3, preds, k):
+                return ops.mask_upsample(self.mask_pre(x_d3), ops.pack_mask_weights(self.mask_head), preds, k)
             mask = self.mask_head(x_d3).float()
         else:
             preds, mask = self.forward_quarter(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid,
@@ -482,10 +470,8 @@ class MagnetHead(nn.Module):
         if self.fused_upsample:
             preds = self._predictions(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid,
                                       cam_intrins)
-            if fused_mask_trains(self.mask_head, None, preds, k, gt_depth):
-                pre0 = self.mask_pre(x_d3)
-                if fused_mask_trains(self.mask_head, pre0, preds, k, gt_depth):
-                    return ops.mask_head_loss(pre0, self.mask_head, preds, gt_depth, gt_depth_mask, k, gamma)
+            if fused_mask_trains(self.mask_head, x_d3, preds, k, gt_depth):
+                return ops.mask_head_loss(self.mask_pre(x_d3), self.mask_head, preds, gt_depth, gt_depth_mask, k, gamma)
             mask = self.mask_head(x_d3).float()
         else:
             preds, mask = self.forward_quarter(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, nghbr_poses, is_valid,

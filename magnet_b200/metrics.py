@@ -51,8 +51,7 @@ class DepthMetrics:
         if self._form is not None and form != self._form:
             raise _lib.MagnetError(f"this DepthMetrics scores {self._FORMS[self._form]}; use another instance for "
                                    "another form (its nll column differs)")
-        preds = [pred_or_list] if isinstance(pred_or_list, torch.Tensor) else list(pred_or_list)
-        pred_or_list = [p.float() for p in preds]
+        pred_or_list = [p.float() for p in ops._pred_list(pred_or_list)]
         up_mask = None if up_mask is None else up_mask.float()
         rows = ops.depth_metrics(pred_or_list, gt.float(), min_depth=self.min_depth, max_depth=self.max_depth, crop=self.crop,
                                  up_mask=up_mask, k=k, nearest=nearest, variance=variance)

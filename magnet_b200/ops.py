@@ -562,20 +562,26 @@ def gnet_weights_bytes(D: int) -> int:
     return int(lib().magnet_gnet_weights_bytes(int(D)))
 
 
+def _check_cost_channels(D: int) -> None:
+    if not 1 <= D <= _lib.MAGNET_MAX_PLANES:
+        raise _lib.MagnetError(f"the fused G-Net head takes 1 to {_lib.MAGNET_MAX_PLANES} cost channels, got {D}")
+
+
+def _gnet_convs(gnet, D: int):
+    convs = gnet_head_layers(gnet, D)
+    if convs is None:
+        raise _lib.MagnetError(f"not a G-Net head with the reference's structure and at least {D} cost channels")
+    return convs
+
+
 def pack_gnet_weights(gnet, D: int) -> torch.Tensor:
     """The weights of a ``GNET`` (or its ``gnet`` Sequential) in the fused head's layout, for D cost channels: the
     cost slice W0[:, :D] of the first convolution, the two 128x128 layers and the 128->2 layer, split into fp16 hi/lo
-    with one power-of-two scale per layer.  Read from the module at each call (nothing is cached).  Two launches."""
-    seq = gnet.gnet if hasattr(gnet, "gnet") else gnet
-    c0, c1, c2, c3 = seq[0], seq[2], seq[4], seq[6]
-    hid = _lib.MAGNET_HIDDEN_CHANNELS
-    if not (c0.weight.shape[0] == hid and c0.weight.shape[1] >= D and tuple(c0.weight.shape[2:]) == (3, 3)
-            and tuple(c1.weight.shape) == (hid, hid, 1, 1) and tuple(c2.weight.shape) == (hid, hid, 1, 1)
-            and tuple(c3.weight.shape) == (2, hid, 1, 1)):
-        raise _lib.MagnetError(f"not a G-Net head with {hid} hidden channels and at least {D} cost channels")
+    with one power-of-two scale per layer.  The head must have the structure ``gnet_head_layers`` recognises.  Read
+    from the module at each call (nothing is cached).  Two launches."""
+    c0, c1, c2, c3 = _gnet_convs(gnet, D)
+    _check_cost_channels(D)
     nbytes = gnet_weights_bytes(D)
-    if nbytes == 0:
-        raise _lib.MagnetError(f"the fused G-Net head takes 1 to {_lib.MAGNET_MAX_PLANES} cost channels, got {D}")
     with torch.no_grad():
         w0 = _need_cuda_f32("W0", c0.weight[:, :D])
         ts = [w0] + [_need_cuda_f32(nm, t) for nm, t in (("W1", c1.weight), ("b1", c1.bias), ("W2", c2.weight),
@@ -597,9 +603,8 @@ def gnet_update(cost: torch.Tensor, invariant: torch.Tensor, packed: torch.Tenso
     B, D, H, W = cost.shape
     invariant = _need_cuda_f32("invariant", invariant, (B, _lib.MAGNET_HIDDEN_CHANNELS, H, W))
     prev_gmm = _need_cuda_f32("prev_gmm", prev_gmm, (B, 2, H, W))
+    _check_cost_channels(D)
     nbytes = gnet_weights_bytes(D)
-    if nbytes == 0:
-        raise _lib.MagnetError(f"the fused G-Net head takes 1 to {_lib.MAGNET_MAX_PLANES} cost channels, got {D}")
     if not _is_packed(packed, (nbytes,)):
         raise _lib.MagnetError(f"packed must be a pack_gnet_weights buffer for D = {D} ({nbytes} bytes)")
     if out is None:
@@ -630,12 +635,12 @@ class GnetHeadTrain(torch.autograd.Function):
         B, D, H, W = cost.shape
         invariant = _need_cuda_f32("invariant", invariant.detach(), (B, hid, H, W))
         prev_gmm = _need_cuda_f32("prev_gmm", prev_gmm.detach(), (B, 2, H, W))
+        _check_cost_channels(D)
         nbytes = int(lib().magnet_gnet_train_weights_bytes(D))
-        if nbytes == 0:
-            raise _lib.MagnetError(f"the fused G-Net head takes 1 to {_lib.MAGNET_MAX_PLANES} cost channels, got {D}")
         shapes = (("W0", w0, (hid, D, 3, 3)), ("W1", w1, (hid, hid, 1, 1)), ("b1", b1, (hid,)),
                   ("W2", w2, (hid, hid, 1, 1)), ("b2", b2, (hid,)), ("W3", w3, (2, hid, 1, 1)), ("b3", b3, (2,)))
         ws = _need_weights(shapes)
+        ctx.weight_shapes = [shape for _, _, shape in shapes]
         dev = _same_device(("cost", cost), ("invariant", invariant), ("prev_gmm", prev_gmm),
                            *((nm, t) for (nm, _, _), t in zip(shapes, ws)))
         packed = torch.empty(nbytes, device=dev, dtype=torch.uint8)
@@ -655,22 +660,18 @@ class GnetHeadTrain(torch.autograd.Function):
         cost, prev_gmm, packed, saved = ctx.saved_tensors
         need = ctx.needs_input_grad
         B, D, H, W = cost.shape
-        hid = _lib.MAGNET_HIDDEN_CHANNELS
         dev = cost.device
         grad_out = _need_cuda_f32("grad_out", grad_out)
-        new = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.float32)
-        g_inv = new(B, hid, H, W)
-        g = [new(hid, D, 3, 3) if need[2] else None, new(hid, hid, 1, 1) if need[3] else None,
-             new(hid) if need[4] else None, new(hid, hid, 1, 1) if need[5] else None, new(hid) if need[6] else None,
-             new(2, hid, 1, 1) if need[7] else None, new(2) if need[8] else None]
-        g_prev = new(B, 2, H, W) if need[9] else None
+        new = lambda shape: torch.empty(shape, device=dev, dtype=torch.float32)
+        g_inv = new((B, _lib.MAGNET_HIDDEN_CHANNELS, H, W))
+        g = [new(shape) if n else None for shape, n in zip(ctx.weight_shapes, need[2:9])]
+        g_prev = new((B, 2, H, W)) if need[9] else None
         ws = torch.empty(int(lib().magnet_gnet_bwd_workspace_bytes(B, D, H, W)), device=dev, dtype=torch.uint8)
-        ptr = lambda t: None if t is None else t.data_ptr()
         a = _lib.GnetTrainArgs(B=B, D=D, H=H, W=W, cost=cost.data_ptr(), packed_weights=packed.data_ptr(),
                                prev_gmm=prev_gmm.data_ptr(), saved=saved.data_ptr(), grad_out=grad_out.data_ptr(),
-                               workspace=ws.data_ptr(), grad_invariant=g_inv.data_ptr(), grad_w0_cost=ptr(g[0]),
-                               grad_w1=ptr(g[1]), grad_b1=ptr(g[2]), grad_w2=ptr(g[3]), grad_b2=ptr(g[4]),
-                               grad_w3=ptr(g[5]), grad_b3=ptr(g[6]), grad_prev=ptr(g_prev))
+                               workspace=ws.data_ptr(), grad_invariant=g_inv.data_ptr(), grad_w0_cost=_ptr(g[0]),
+                               grad_w1=_ptr(g[1]), grad_b1=_ptr(g[2]), grad_w2=_ptr(g[3]), grad_b2=_ptr(g[4]),
+                               grad_w3=_ptr(g[5]), grad_b3=_ptr(g[6]), grad_prev=_ptr(g_prev))
         _launch(dev, "magnet_gnet_bwd_f32", C.byref(a))
         return (None, g_inv if need[1] else None, *g, g_prev)
 
@@ -678,12 +679,11 @@ class GnetHeadTrain(torch.autograd.Function):
 def gnet_head_train(cost, invariant, gnet, prev_gmm):
     """``GnetHeadTrain`` on the weights of a ``GNET`` (or its ``gnet`` Sequential): the cost slice W0[:, :D] of the first
     convolution (autograd scatters its gradient into the full weight), the two 128x128 layers and the 128->2 layer.
-    Validates like ``gnet_update``."""
-    seq = gnet.gnet if hasattr(gnet, "gnet") else gnet
-    c0, c1, c2, c3 = seq[0], seq[2], seq[4], seq[6]
-    if cost.dim() != 4 or c0.weight.dim() != 4 or c0.weight.shape[1] < cost.shape[1]:
-        raise _lib.MagnetError(f"not a G-Net head with at least {cost.shape[1] if cost.dim() == 4 else '?'} cost channels")
+    The head must have the structure ``gnet_head_layers`` recognises.  Validates like ``gnet_update``."""
+    if cost.dim() != 4:
+        raise _lib.MagnetError(f"cost must be (B,D,H,W), got {tuple(cost.shape)}")
     D = cost.shape[1]
+    c0, c1, c2, c3 = _gnet_convs(gnet, D)
     return GnetHeadTrain.apply(cost, invariant, c0.weight[:, :D], c1.weight, c1.bias, c2.weight, c2.bias, c3.weight,
                                c3.bias, prev_gmm)
 
@@ -749,6 +749,15 @@ def _conv_chain(seq, *couts):
     return convs
 
 
+def gnet_head_layers(gnet, D: int):
+    """The four convolutions of a ``GNET`` (or its ``gnet`` Sequential) with the reference's structure (MAGNET.py:53-60):
+    Conv(*,128,3), ReLU, Conv(128,128,1), ReLU, Conv(128,128,1), ReLU, Conv(128,2,1), every convolution with a bias,
+    the first with at least D input channels (the cost channels come first).  None otherwise."""
+    hid = _lib.MAGNET_HIDDEN_CHANNELS
+    convs = _conv_chain(gnet.gnet if hasattr(gnet, "gnet") else gnet, hid, hid, 2)
+    return None if convs is None or convs[0].in_channels < D else convs
+
+
 def mask_head_layers(mask_head):
     """The four convolutions of a mask head with the reference's structure (MAGNET.py:111-118): Conv(*,128,3), ReLU,
     Conv(128,128,1), ReLU, Conv(128,128,1), ReLU, Conv(128,144,1), every convolution with a bias.  None otherwise."""
@@ -756,16 +765,37 @@ def mask_head_layers(mask_head):
     return _conv_chain(mask_head, hid, hid, 9 * 4 * 4)
 
 
+def _mask_convs(mask_head):
+    convs = mask_head_layers(mask_head)
+    if convs is None:
+        raise _lib.MagnetError("not a mask head with the reference's structure (Conv(*,128,3), ReLU, Conv(128,128,1), "
+                               "ReLU, Conv(128,128,1), ReLU, Conv(128,144,1))")
+    return convs
+
+
+def _check_k4(k, head: str = "mask head") -> None:
+    if int(k) != 4:
+        raise _lib.MagnetError(f"the fused {head} takes k = 4 only (144 mask channels), got {k}")
+
+
+def _need_hidden(name: str, x: torch.Tensor) -> torch.Tensor:
+    """A (B,128,H,W) hidden map: a first convolution's output before its ReLU, checked as ``_need_cuda_f32`` does."""
+    x = _need_cuda_f32(name, x)
+    if x.dim() != 4 or x.shape[1] != _lib.MAGNET_HIDDEN_CHANNELS:
+        raise _lib.MagnetError(f"{name} must be (B,{_lib.MAGNET_HIDDEN_CHANNELS},H,W), got {tuple(x.shape)}")
+    return x
+
+
+def _pred_list(preds) -> list:
+    return [preds] if isinstance(preds, torch.Tensor) else list(preds)
+
+
 def pack_mask_weights(mask_head) -> torch.Tensor:
     """The weights of the mask head's last three layers in the fused kernel's layout (``mask_upsample``): the two
     128x128 layers and the 128->144 layer, split into fp16 hi/lo with one power-of-two scale per layer, and the fp32
     biases.  The first (3x3) layer stays outside (``MagnetHead.mask_pre``).  Read from the module at each call (nothing
     is cached).  Two launches."""
-    convs = mask_head_layers(mask_head)
-    if convs is None:
-        raise _lib.MagnetError("not a mask head with the reference's structure (Conv(*,128,3), ReLU, Conv(128,128,1), "
-                               "ReLU, Conv(128,128,1), ReLU, Conv(128,144,1))")
-    _, c1, c2, c3 = convs
+    _, c1, c2, c3 = _mask_convs(mask_head)
     with torch.no_grad():
         ts = [_need_cuda_f32(nm, t) for nm, t in (("W1", c1.weight), ("b1", c1.bias), ("W2", c2.weight),
                                                   ("b2", c2.bias), ("W3", c3.weight), ("b3", c3.bias))]
@@ -782,14 +812,11 @@ def mask_upsample(pre0: torch.Tensor, packed: torch.Tensor, preds, k: int = 4) -
     (B,2,k*H,k*W) tensors, as ``convex_upsample(pred, mask_head(x_d3), k)`` gives them.  The 144-channel mask is never
     written.  k = 4 only.  Not differentiable (forward only): training runs the mask head, the upsampling and the
     loss through ``mask_head_loss``, which has a backward."""
-    preds = [preds] if isinstance(preds, torch.Tensor) else list(preds)
+    preds = _pred_list(preds)
     if not preds:
         raise _lib.MagnetError("mask_upsample needs at least one prediction")
-    if int(k) != 4:
-        raise _lib.MagnetError(f"the fused mask head takes k = 4 only (144 mask channels), got {k}")
-    pre0 = _need_cuda_f32("pre0", pre0)
-    if pre0.dim() != 4 or pre0.shape[1] != _lib.MAGNET_HIDDEN_CHANNELS:
-        raise _lib.MagnetError(f"pre0 must be (B,{_lib.MAGNET_HIDDEN_CHANNELS},H,W), got {tuple(pre0.shape)}")
+    _check_k4(k)
+    pre0 = _need_hidden("pre0", pre0)
     B, _, H, W = pre0.shape
     nbytes = mask_weights_bytes(4)
     if not _is_packed(packed, (nbytes,)):
@@ -836,6 +863,11 @@ def pack_dnet_weights(depth_head, mask_head=None) -> torch.Tensor:
     if layers is None:
         raise _lib.MagnetError("not D-Net heads with the reference's structure (Conv(*,128,3), ReLU, Conv(128,128,1), "
                                "ReLU, Conv(128,2,1); mask head: the same ending in Conv(128,144,1))")
+    return _pack_dnet_layers(layers)
+
+
+def _pack_dnet_layers(layers) -> torch.Tensor:
+    """``pack_dnet_weights`` of the heads' convolutions as ``dnet_head_layers`` returns them."""
     (_, d1, d2), m = layers
     k = 0 if m is None else 4
     named = [("depth W1", d1.weight), ("depth b1", d1.bias), ("depth W2", d2.weight), ("depth b2", d2.bias)]
@@ -858,19 +890,12 @@ def _check_dnet_packed(packed, k: int) -> None:
                                + (")" if k == 4 else f" or {dnet_weights_bytes(4)})"))
 
 
-def _dnet_pre(name: str, pre: torch.Tensor) -> torch.Tensor:
-    pre = _need_cuda_f32(name, pre)
-    if pre.dim() != 4 or pre.shape[1] != _lib.MAGNET_HIDDEN_CHANNELS:
-        raise _lib.MagnetError(f"{name} must be (B,{_lib.MAGNET_HIDDEN_CHANNELS},H,W), got {tuple(pre.shape)}")
-    return pre
-
-
 def dnet_depth(pre_d: torch.Tensor, packed: torch.Tensor, sigma: bool) -> torch.Tensor:
     """D-Net's depth head after its first convolution in one kernel: pre_d (B,128,H,W) = that convolution's output
     before its ReLU, packed = ``pack_dnet_weights(depth_head[, mask_head])`` -> (B,2,H,W): with ``sigma`` [mu, sigma] as
     activation_G_magnet gives it (DNET.py:62-67, MaGNet's mono_gmms), else the raw [mu, v] that ``dnet_upsample``
     reads.  Forward only."""
-    pre_d = _dnet_pre("pre_d", pre_d)
+    pre_d = _need_hidden("pre_d", pre_d)
     _check_dnet_packed(packed, 0)
     B, _, H, W = pre_d.shape
     dev = _same_device(("pre_d", pre_d), ("packed", packed))
@@ -884,9 +909,8 @@ def dnet_upsample(pre_m: torch.Tensor, packed: torch.Tensor, raw: torch.Tensor, 
     one kernel: pre_m (B,128,H,W) = the mask head's first convolution before its ReLU, packed = ``pack_dnet_weights(
     depth_head, mask_head)``, raw = ``dnet_depth(..., sigma=False)`` -> (B,2,4H,4W) [mu, var], what DNET(args)
     returns (DNET.py:56-60).  The 144-channel mask is never written.  k = 4 only.  Forward only."""
-    if int(k) != 4:
-        raise _lib.MagnetError(f"the fused D-Net mask head takes k = 4 only (144 mask channels), got {k}")
-    pre_m = _dnet_pre("pre_m", pre_m)
+    _check_k4(k, "D-Net mask head")
+    pre_m = _need_hidden("pre_m", pre_m)
     _check_dnet_packed(packed, 4)
     B, _, H, W = pre_m.shape
     raw = _need_cuda_f32("raw", raw, (B, 2, H, W))
@@ -917,15 +941,13 @@ class MaskLossTrain(torch.autograd.Function):
         P = len(preds)
         if not 1 <= P <= _lib.MAGNET_MASK_MAX_PRED:
             raise _lib.MagnetError(f"the fused mask-head loss takes 1 to {_lib.MAGNET_MASK_MAX_PRED} predictions, got {P}")
-        if int(k) != 4:
-            raise _lib.MagnetError(f"the fused mask head takes k = 4 only (144 mask channels), got {k}")
-        pre0 = _need_cuda_f32("pre0", pre0.detach())
-        if pre0.dim() != 4 or pre0.shape[1] != hid:
-            raise _lib.MagnetError(f"pre0 must be (B,{hid},H,W), got {tuple(pre0.shape)}")
+        _check_k4(k)
+        pre0 = _need_hidden("pre0", pre0.detach())
         B, _, H, W = pre0.shape
         shapes = (("W1", w1, (hid, hid, 1, 1)), ("b1", b1, (hid,)), ("W2", w2, (hid, hid, 1, 1)), ("b2", b2, (hid,)),
                   ("W3", w3, (nout, hid, 1, 1)), ("b3", b3, (nout,)))
         ws = _need_weights(shapes)
+        ctx.weight_shapes = [shape for _, _, shape in shapes]
         ps = _need_preds("preds", (p.detach() for p in preds), (B, 2, H, W))
         gt = _need_cuda_f32("gt", gt.detach(), (B, 1, 4 * H, 4 * W))
         gt_mask_u8 = _need_cuda_u8_mask("gt_mask", gt_mask_u8, (B, 1, 4 * H, 4 * W), "(B,1,4H,4W)")
@@ -961,23 +983,19 @@ class MaskLossTrain(torch.autograd.Function):
         packed, saved = ctx.saved_tensors
         need = ctx.needs_input_grad
         P, B, H, W = ctx.shape
-        hid, nout = _lib.MAGNET_HIDDEN_CHANNELS, 9 * 4 * 4
         dev = saved.device
-        new = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.float32)
-        g_pre0 = new(B, hid, H, W) if need[0] else None
-        g = [new(hid, hid, 1, 1) if need[1] else None, new(hid) if need[2] else None,
-             new(hid, hid, 1, 1) if need[3] else None, new(hid) if need[4] else None,
-             new(nout, hid, 1, 1) if need[5] else None, new(nout) if need[6] else None]
-        g_preds = [new(B, 2, H, W) if need[12 + i] else None for i in range(P)]
+        new = lambda shape: torch.empty(shape, device=dev, dtype=torch.float32)
+        g_pre0 = new((B, _lib.MAGNET_HIDDEN_CHANNELS, H, W)) if need[0] else None
+        g = [new(shape) if n else None for shape, n in zip(ctx.weight_shapes, need[1:7])]
+        g_preds = [new((B, 2, H, W)) if need[12 + i] else None for i in range(P)]
         grad_scale = grad_loss.detach().to(device=dev, dtype=torch.float32).reshape(1).contiguous()
         nws = int(lib().magnet_mask_bwd_workspace_bytes(B, H, W)) if any(need[:7]) else 256
         ws = torch.empty(nws, device=dev, dtype=torch.uint8)
-        ptr = lambda t: None if t is None else t.data_ptr()
-        gp = (C.c_void_p * P)(*[ptr(t) for t in g_preds])
+        gp = (C.c_void_p * P)(*[_ptr(t) for t in g_preds])
         a = _lib.MaskTrainArgs(P=P, B=B, H=H, W=W, k=4, packed_weights=packed.data_ptr(), saved=saved.data_ptr(),
-                               grad_scale=grad_scale.data_ptr(), workspace=ws.data_ptr(), grad_pre0=ptr(g_pre0),
-                               grad_w1=ptr(g[0]), grad_b1=ptr(g[1]), grad_w2=ptr(g[2]), grad_b2=ptr(g[3]),
-                               grad_w3=ptr(g[4]), grad_b3=ptr(g[5]), grad_pred=C.cast(gp, C.POINTER(C.c_void_p)))
+                               grad_scale=grad_scale.data_ptr(), workspace=ws.data_ptr(), grad_pre0=_ptr(g_pre0),
+                               grad_w1=_ptr(g[0]), grad_b1=_ptr(g[1]), grad_w2=_ptr(g[2]), grad_b2=_ptr(g[3]),
+                               grad_w3=_ptr(g[4]), grad_b3=_ptr(g[5]), grad_pred=C.cast(gp, C.POINTER(C.c_void_p)))
         _launch(dev, "magnet_mask_bwd_f32", C.byref(a))
         return (g_pre0, *g, None, None, None, None, None, *g_preds)
 
@@ -988,20 +1006,15 @@ def mask_head_loss(pre0, mask_head, preds, gt, gt_mask, k: int = 4, gamma: float
     through ``MaskLossTrain``, differentiable in pre0, the last three layers' weights and biases and every prediction.
     k = 4 and 1 to MAGNET_MASK_MAX_PRED predictions; gt_mask bool / uint8.  Validates like ``mask_upsample`` and
     ``UpsampleNLL``; reads the number of supervised pixels with one host read, as ``magnet_loss``."""
-    convs = mask_head_layers(mask_head)
-    if convs is None:
-        raise _lib.MagnetError("not a mask head with the reference's structure (Conv(*,128,3), ReLU, Conv(128,128,1), "
-                               "ReLU, Conv(128,128,1), ReLU, Conv(128,144,1))")
-    preds = [preds] if isinstance(preds, torch.Tensor) else list(preds)
+    _, c1, c2, c3 = _mask_convs(mask_head)
+    preds = _pred_list(preds)
     if not preds:
         raise _lib.MagnetError("mask_head_loss needs at least one prediction")
-    if int(k) != 4:
-        raise _lib.MagnetError(f"the fused mask head takes k = 4 only (144 mask channels), got {k}")
+    _check_k4(k)
     gtm = gt_mask.to(torch.uint8)
     count = int(gtm.sum().item())          # one host read per step, as magnet_loss
     if count == 0:
         raise _lib.MagnetError("gt_mask selects no pixel")
-    _, c1, c2, c3 = convs
     return MaskLossTrain.apply(pre0, c1.weight, c1.bias, c2.weight, c2.bias, c3.weight, c3.bias, gt, gtm, 4, gamma,
                                count, *preds)
 
@@ -1203,7 +1216,7 @@ def depth_metrics(pred_or_list, gt: torch.Tensor, *, min_depth: float, max_depth
     crop: None, 'garg' or 'eigen'.  Returns a (P,B,13) float64 device tensor: the number of valid pixels, then the
     metrics in METRIC_KEYS order (NaN for an image without a valid pixel; nll 0.0 there in the nearest form).  Two
     kernel launches, no host sync."""
-    preds = [pred_or_list] if isinstance(pred_or_list, torch.Tensor) else list(pred_or_list)
+    preds = _pred_list(pred_or_list)
     if not 1 <= len(preds) <= _lib.MAGNET_METRICS_MAX_PRED:
         raise _lib.MagnetError(f"1 to {_lib.MAGNET_METRICS_MAX_PRED} predictions per call, got {len(preds)}")
     if nearest and (up_mask is not None or k is not None):

@@ -5,8 +5,9 @@ import ctypes as C
 import numpy as np
 import pytest
 import torch
+import torch.nn as nn
 
-from magnet_b200 import _lib
+from magnet_b200 import _lib, ops
 from magnet_b200.matcher import GNET, fused_gnet_applies
 
 
@@ -108,7 +109,7 @@ def test_three_product_gemm_error(scale, K):
 
 
 # ---- dispatch rule ------------------------------------------------------------------------------------------------
-def test_dispatch_rule_truth_table():
+def test_dispatch_rule_truth_table_with_head_width():
     g = GNET(ch_in=8 + 4)
     cv, inv = torch.zeros(1, 8, 4, 4), torch.zeros(1, 128, 4, 4)
     with torch.no_grad():
@@ -117,7 +118,10 @@ def test_dispatch_rule_truth_table():
         assert not fused_gnet_applies(g, cv, None)
         assert not fused_gnet_applies(g, torch.zeros(1, 0, 4, 4), inv)  # D = 0
         assert not fused_gnet_applies(g, torch.zeros(1, 257, 4, 4), inv)
-        assert fused_gnet_applies(g, torch.zeros(1, 256, 4, 4), inv)
+        assert not fused_gnet_applies(g, torch.zeros(1, 13, 4, 4), inv)  # D above the head's 12 input channels
+        wide = GNET(ch_in=300)
+        assert fused_gnet_applies(wide, torch.zeros(1, 256, 4, 4), inv)
+        assert not fused_gnet_applies(wide, torch.zeros(1, 257, 4, 4), inv)
         assert not fused_gnet_applies(g, cv.half(), inv)
         g.half()
         assert not fused_gnet_applies(g, cv, inv)                       # weights not fp32
@@ -130,3 +134,21 @@ def test_dispatch_rule_truth_table():
     assert not fused_gnet_applies(g, cv, inv.clone().requires_grad_(True))
     with torch.no_grad():
         assert fused_gnet_applies(g, cv.clone().requires_grad_(True), inv)
+
+
+def test_structure_recognition():
+    g = GNET(ch_in=8 + 4)
+    convs = ops.gnet_head_layers(g, 8)
+    assert convs == [g.gnet[0], g.gnet[2], g.gnet[4], g.gnet[6]]
+    assert ops.gnet_head_layers(g.gnet, 8) == convs                     # a GNET and its Sequential
+    assert ops.gnet_head_layers(g, 12) == convs and ops.gnet_head_layers(g, 13) is None
+    unpadded = GNET(ch_in=8 + 4)
+    unpadded.gnet[0] = nn.Conv2d(12, 128, 3, padding=0)
+    assert ops.gnet_head_layers(unpadded, 8) is None
+    with torch.no_grad():
+        assert not fused_gnet_applies(unpadded, torch.zeros(1, 8, 4, 4), torch.zeros(1, 128, 4, 4))
+    # refused on the CPU, before any device check
+    with pytest.raises(_lib.MagnetError, match="not a G-Net head"):
+        ops.pack_gnet_weights(unpadded, 8)
+    with pytest.raises(_lib.MagnetError, match="not a G-Net head"):
+        ops.gnet_head_train(torch.zeros(1, 8, 4, 4), torch.zeros(1, 128, 4, 4), unpadded, torch.zeros(1, 2, 4, 4))

@@ -95,7 +95,7 @@ def test_train_size_formulas():
 
 
 # ---- dispatch rule ------------------------------------------------------------------------------------------------
-def test_train_dispatch_rule_truth_table():
+def test_train_dispatch_rule_truth_table_with_head_width():
     g = GNET(ch_in=8 + 4)
     cv, inv = torch.zeros(1, 8, 4, 4), torch.zeros(1, 128, 4, 4)
     assert fused_gnet_trains(g, cv, inv)                                # grad mode on, trainable parameters
@@ -106,7 +106,10 @@ def test_train_dispatch_rule_truth_table():
     assert not fused_gnet_trains(g, cv, None)
     assert not fused_gnet_trains(g, torch.zeros(1, 0, 4, 4), inv)       # D = 0
     assert not fused_gnet_trains(g, torch.zeros(1, 257, 4, 4), inv)
-    assert fused_gnet_trains(g, torch.zeros(1, 256, 4, 4), inv)
+    assert not fused_gnet_trains(g, torch.zeros(1, 13, 4, 4), inv)    # D above the head's 12 input channels
+    wide = GNET(ch_in=300)
+    assert fused_gnet_trains(wide, torch.zeros(1, 256, 4, 4), inv)
+    assert not fused_gnet_trains(wide, torch.zeros(1, 257, 4, 4), inv)
     assert not fused_gnet_trains(g, cv.half(), inv)
     # (CUDA autocast cannot be entered without a GPU: its case is in test_gpu_gnet_train)
     g.half()
