@@ -42,8 +42,9 @@ class _PrepCache:
     passed (never to a ``detach()`` temporary), so a freed-and-reallocated tensor at the same address cannot alias a
     stale entry.  Writers that do not bump ``_version`` (a CUDA-graph replay, NCCL, a non-torch kernel) are invisible
     to this key; therefore the cache is BYPASSED while the current stream is being captured (the preparation kernels
-    then become part of the graph and replay with the data), and ``clear_cache()`` / ``prep_cache(False)`` exist for
-    callers that refill buffers behind torch's back."""
+    then become part of the graph and replay with the data) and while torch.compile traces (the key reads data
+    pointers, and a compiled graph replays its preparations with the data too), and ``clear_cache()`` /
+    ``prep_cache(False)`` exist for callers that refill buffers behind torch's back."""
 
     def __init__(self, capacity: int = 8):
         self.capacity = capacity
@@ -55,7 +56,7 @@ class _PrepCache:
         return tuple((t.data_ptr(), t._version, tuple(t.shape), tuple(t.stride()), str(t.device)) for t in tensors)
 
     def _usable(self, tensors) -> bool:
-        if not self.enabled:
+        if not self.enabled or torch.compiler.is_compiling():
             return False
         if any(t.is_cuda for t in tensors) and torch.cuda.is_current_stream_capturing():
             return False
@@ -116,6 +117,8 @@ def _camera_table(cam_intrins, R, t, is_valid, device):
     """K*R, K*t per (b, v): 2 KB, one 3 us kernel.  Cached on the tensors R and t are views OF (MAGNET.py:147-148
     slices nghbr_poses once per forward) — both bases, with their version counters — plus the views' geometry."""
     intM_d, _ = _device_intrinsics(cam_intrins, device)
+    if torch.compiler.is_compiling():                  # no cache while tracing, and its key reads data pointers
+        return ops.pack_cameras(intM_d, R, t, is_valid.to(device=device, dtype=torch.int32))
     rbase = R._base if R._base is not None else R
     tbase = t._base if t._base is not None else t
     src = (rbase, tbase, is_valid, cam_intrins['intM'])
@@ -377,8 +380,24 @@ def est_costvolume_CW(d_volume, ref_feat, nghbr_feat, ref_gmms, nghbr_gmms,
 
 def _plane_list(d_center):
     """The D plane depths as host floats.  ``d_center`` is a constant of the training run (train_FNet.py:56-66): the
-    device -> host read happens once per tensor, not once per step."""
+    device -> host read happens once per tensor, not once per step.  A sequence of floats is taken as it is; under
+    torch.compile it is required (a tensor is refused rather than read in the compiled graph)."""
+    if torch.compiler.is_compiling():
+        return ops.k_array(d_center)                   # the list of floats; a tensor is refused
+    if not isinstance(d_center, torch.Tensor):
+        return [float(v) for v in d_center]
     return _cached("planes", (d_center,), lambda: d_center.detach().reshape(-1).cpu().tolist())
+
+
+def _f_forward(ref_feat, nghbr_feat, planes, rays_d, cams, V, variant, softmax):
+    """The F volume's forward: (volume, source layout, source maps, reference split)."""
+    layout, fv = route(int(ref_feat.shape[1]), V, len(planes), variant, _lib.DEPTH_PLANES, ref_feat.dtype,
+                       nghbr_feat.dtype)
+    src, ref_split = _packed_source(layout, nghbr_feat, None, ref_feat)
+    ref = (ref_feat if layout == _lib.SRC_HALF16 else _f32(ref_feat)).detach()
+    out = ops.cost_volume(ref, src, rays_d, cams, V=V, src_layout=layout, consistency=False,
+                          k=planes, planes=True, softmax=softmax, variant=fv, ref_split=ref_split)
+    return out, layout, src, ref_split
 
 
 class _CostVolumeF(torch.autograd.Function):
@@ -390,12 +409,7 @@ class _CostVolumeF(torch.autograd.Function):
     @staticmethod
     def forward(ctx, ref_feat, nghbr_feat, planes, rays_d, cams, V, variant, softmax, tc_bwd,
                 R=None, t=None, intM=None, rays=None):
-        layout, fv = route(int(ref_feat.shape[1]), V, len(planes), variant, _lib.DEPTH_PLANES, ref_feat.dtype,
-                           nghbr_feat.dtype)
-        src, ref_split = _packed_source(layout, nghbr_feat, None, ref_feat)
-        ref = (ref_feat if layout == _lib.SRC_HALF16 else _f32(ref_feat)).detach()
-        out = ops.cost_volume(ref, src, rays_d, cams, V=V, src_layout=layout, consistency=False,
-                              k=planes, planes=True, softmax=softmax, variant=fv, ref_split=ref_split)
+        out, layout, src, ref_split = _f_forward(ref_feat, nghbr_feat, planes, rays_d, cams, V, variant, softmax)
         ctx.save_for_backward(ref_feat.detach(), nghbr_feat.detach(), out if softmax else None, rays_d, cams,
                               *_detached(R, t, intM, rays))
         ctx.layout = layout if tc_bwd else _lib.SRC_NCHW   # what the feature gradients read
@@ -440,6 +454,8 @@ def _f_volume(d_center, ref_feat, nghbr_feat, R, t, is_valid, cam_intrins, varia
     planes = _plane_list(d_center)
     _, rays_d = _device_intrinsics(cam_intrins, device)
     cams = _camera_table(cam_intrins, R, t, is_valid, device)
+    if torch.compiler.is_compiling() and not wants_cw_grad(ref_feat, nghbr_feat, *cam_in):
+        return _f_forward(ref_feat, nghbr_feat, planes, rays_d, cams, V, variant, softmax)[0]   # traced inference
     return _CostVolumeF.apply(ref_feat, nghbr_feat, planes, rays_d, cams, V, variant, softmax, tc_bwd, *cam_in)
 
 

@@ -2,12 +2,32 @@
 train_MaGNet.py:153-180) and its ``utils.RunningAverageDict`` (utils/utils.py:160-174)."""
 from __future__ import annotations
 
+import sys
 from typing import Optional
 
 import torch
 
 from . import _lib, dist, ops
 from .ops import METRIC_KEYS
+
+
+def accumulate(acc: torch.Tensor, rows: torch.Tensor) -> None:
+    """Add the (P,B,13) rows of ``ops.depth_metrics`` into the (P,14) accumulator: images seen, then the column sums."""
+    acc[:, 0] += rows.shape[1]
+    acc[:, 1:] += rows.sum(dim=1)
+
+
+def _new_accumulator(P: int, device) -> torch.Tensor:
+    """A zero (P,14) float64 accumulator.  In a program that uses torch.compile (dynamo loaded) it is marked as a static
+    address, so that CUDA-graph trees (mode="reduce-overhead") capture a compiled update's in-place write into it
+    instead of skipping the graph; an eager program does not pay the seconds of importing dynamo."""
+    acc = torch.zeros(P, 1 + _lib.MAGNET_METRICS_COLS, device=device, dtype=torch.float64)
+    if "torch._dynamo" in sys.modules:
+        torch._dynamo.mark_static_address(acc)
+    return acc
+
+
+_new_accumulator_outside_graph = torch._disable_dynamo(_new_accumulator)   # torch.compiler.disable, imported lazily
 
 
 class DepthMetrics:
@@ -21,7 +41,10 @@ class DepthMetrics:
     An instance scores one of three forms: Gaussian predictions [mu, sigma] (full resolution or fused upsampling; nll
     is the Gaussian NLL), with ``nearest=True`` F-Net depth maps (train_FNet.py's validate(); nll is 0.0), or with
     ``variance=True`` D-Net's [mu, var] (test_DNet.py's validate(); nll of the variance itself).  The form is fixed at
-    the first update and the others are refused, because the nll column means something different in each."""
+    the first update and the others are refused, because the nll column means something different in each.
+
+    Under torch.compile ``update`` is one registered op (``magnet_b200::depth_metrics_update``) that writes into the
+    accumulator, which the first update allocates outside the graph."""
 
     _FORMS = {"gaussian": "Gaussian predictions (nearest=False, variance=False)",
               "nearest": "F-Net depth maps (nearest=True)", "variance": "D-Net [mu, var] predictions (variance=True)"}
@@ -53,17 +76,30 @@ class DepthMetrics:
                                    "another form (its nll column differs)")
         pred_or_list = [p.float() for p in ops._pred_list(pred_or_list)]
         up_mask = None if up_mask is None else up_mask.float()
+        if torch.compiler.is_compiling():
+            return self._update_traced(pred_or_list, gt.float(), up_mask, k, nearest, variance, form)
         rows = ops.depth_metrics(pred_or_list, gt.float(), min_depth=self.min_depth, max_depth=self.max_depth, crop=self.crop,
                                  up_mask=up_mask, k=k, nearest=nearest, variance=variance)
         self._form = form
-        P, B = rows.shape[0], rows.shape[1]
+        self._check_acc(rows.shape[0], rows.device)
+        accumulate(self._acc, rows)
+        return rows
+
+    def _check_acc(self, P: int, device) -> None:
+        """Allocate the accumulator for P predictions on ``device`` at the first update; refuse another P or device."""
         if self._acc is None:
-            self._acc = torch.zeros(P, 1 + _lib.MAGNET_METRICS_COLS, device=rows.device, dtype=torch.float64)
-        elif self._acc.shape[0] != P or self._acc.device != rows.device:
+            self._acc = (_new_accumulator_outside_graph if torch.compiler.is_compiling() else _new_accumulator)(P, device)
+        elif self._acc.shape[0] != P or self._acc.device != device:
             raise _lib.MagnetError(f"this DepthMetrics accumulates {self._acc.shape[0]} predictions on "
-                                   f"{self._acc.device}, got {P} on {rows.device}")
-        self._acc[:, 0] += B
-        self._acc[:, 1:] += rows.sum(dim=1)
+                                   f"{self._acc.device}, got {P} on {device}")
+
+    def _update_traced(self, preds, gt, up_mask, k, nearest, variance, form):
+        """``update`` as torch.compile traces it: the accumulator first (the op writes into it), then the op."""
+        self._check_acc(len(preds), gt.device)
+        rows = torch.ops.magnet_b200.depth_metrics_update(self._acc, preds, gt, self.min_depth, self.max_depth,
+                                                          self.crop, up_mask, None if k is None else int(k), nearest,
+                                                          variance)
+        self._form = form
         return rows
 
     def all_reduce(self) -> None:

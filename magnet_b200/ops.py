@@ -20,6 +20,23 @@ def _stream(dev=None) -> int:
     return torch.cuda.current_stream(dev).cuda_stream
 
 
+def _traced() -> bool:
+    """Whether torch.compile is tracing the call.  A traced call goes through its registered op
+    (``magnet_b200.library``), whose implementation is the eager call; an eager call goes to the C entry point directly,
+    without the dispatcher (DESIGN §3.18)."""
+    return torch.compiler.is_compiling()
+
+
+def _op(name: str):
+    return getattr(torch.ops.magnet_b200, name)
+
+
+def _no_out_traced(out) -> None:
+    if out is not None:
+        raise _lib.MagnetError("out= writes into a caller buffer by address: under torch.compile the ops allocate "
+                               "their outputs (pass out=None)")
+
+
 def _launch(dev, name: str, *args) -> None:
     """Call the C entry point ``name`` with ``args`` and the current stream of ``dev``, with ``dev`` current; a
     failed status raises MagnetError."""
@@ -114,7 +131,14 @@ def _check_packed(name: str, buf, layout: int, N: int, H: int, W: int) -> None:
 
 def k_array(k: Sequence[float]):
     """Python / numpy / tensor sequence -> host float[D] (rounded to fp32 like torch does for
-    tensor * python-scalar, MAGNET.py:155)."""
+    tensor * python-scalar, MAGNET.py:155).  While torch.compile traces: the list of Python floats the registered ops
+    take instead (they round it the same way), and a tensor is refused, because reading it would put a device-to-host
+    copy in the compiled graph."""
+    if _traced():
+        if isinstance(k, torch.Tensor):
+            raise _lib.MagnetError("under torch.compile the hypotheses / plane depths must be a sequence of Python "
+                                   "floats, not a tensor (read it to the host once, outside the compiled function)")
+        return [float(v) for v in k]
     if isinstance(k, torch.Tensor):
         k = k.detach().cpu().flatten().tolist()
     vals = [float(v) for v in k]
@@ -126,6 +150,8 @@ def k_array(k: Sequence[float]):
 def pack_cameras(intM: torch.Tensor, R: torch.Tensor, t: torch.Tensor, is_valid: torch.Tensor) -> torch.Tensor:
     """(B,3,3) intrinsics, (B,V,3,3) / (B,V,3) pose views (any strides), (B,V) int32 validity — all on the
     device — -> (B*V, 16) float32 camera-constant table (struct magnet_camera)."""
+    if _traced():
+        return _op("pack_cameras")(intM, R, t, is_valid)
     intM = _need_cuda_f32("intM", intM)
     R = _need_cuda_f32("R", R, contiguous=False)
     t = _need_cuda_f32("t", t, contiguous=False)
@@ -165,6 +191,9 @@ def _ptr(x: Optional[torch.Tensor]):
 def repack_tiled32(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """(N,C,H,W) -> TILED32 (N, H, ceil(W/32), C/4, 32, 4): the source-feature layout the tap-sharing
     kernel gathers from (channel quads of a pixel 512 B apart, 32 neighbouring pixels contiguous)."""
+    if _traced():
+        _no_out_traced(out)
+        return _op("repack_tiled32")(x)
     x = _need_cuda_f32("x", x)
     N, Cc, H, W = x.shape
     if out is None:
@@ -176,6 +205,9 @@ def repack_tiled32(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch
 def repack_pixc(x: torch.Tensor, gmm: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """(N,C,H,W) features [+ (N,2,H,W) Gaussians] -> PIXC (N, H, W, C+4): pixel-major, per pixel the C channels then
     (mu, sigma, 0, 0) — the layout the TMA-staged CUDA-core kernel fetches its windows from.  C in {16, 32, 64}."""
+    if _traced():
+        _no_out_traced(out)
+        return _op("repack_pixc")(x, gmm)
     x = _need_cuda_f32("x", x)
     N, Cc, H, W = x.shape
     gmm, out = _repack_operands(x, gmm, out, (N, H, W, Cc + 4), torch.float32)
@@ -187,6 +219,9 @@ def repack_split16(x: torch.Tensor, gmm: Optional[torch.Tensor] = None, out: Opt
     """(N,64,H,W) features [+ (N,2,H,W) Gaussians] -> SPLIT16 buffer (uint8): header with the power-of-two scale s, fp16
     planes (N,2,H,W,64) with x*s = hi + lo, table (N,H,W,4) = (mu, sigma, 0, 0) — what the tensor-core kernel's TMA boxes
     fetch (reference features: gmm=None)."""
+    if _traced():
+        _no_out_traced(out)
+        return _op("repack_split16")(x, gmm)
     x = _need_cuda_f32("x", x)
     N, Cc, H, W = x.shape
     gmm, out = _repack_operands(x, gmm, out, (int(lib().magnet_split16_bytes(N, H, W)),))
@@ -198,6 +233,9 @@ def repack_half16(x: torch.Tensor, gmm: Optional[torch.Tensor] = None, out: Opti
     """(N,64,H,W) fp16 / bf16 features [+ (N,2,H,W) fp32 Gaussians] -> HALF16 buffer (uint8): the header and table of
     ``repack_split16(x.float(), gmm)`` around ONE fp16 plane (N,1,H,W,64) = its hi plane (its lo plane is zero for
     every element above the threshold of DESIGN §3.7).  Read by the tensor-core kernels with ``src_layout=SRC_HALF16``."""
+    if _traced():
+        _no_out_traced(out)
+        return _op("repack_half16")(x, gmm)
     x = _need_cuda("x", x)
     if x.dtype not in HALF_DTYPES:
         raise _lib.MagnetError(f"x must be float16 or bfloat16 (repack_split16 takes float32), got {x.dtype}")
@@ -213,6 +251,9 @@ def repack_half16(x: torch.Tensor, gmm: Optional[torch.Tensor] = None, out: Opti
 
 def sample_depths(gmm: torch.Tensor, k, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Sampler alone (MAGNET.py:154-156): gmm (B,2,H,W) -> d_volume (B,D,H,W)."""
+    if _traced():
+        _no_out_traced(out)
+        return _op("sample_depths")(gmm, k_array(k))
     gmm = _need_cuda_f32("gmm", gmm)
     karr = k if isinstance(k, C.Array) else k_array(k)
     B, _, H, W = gmm.shape
@@ -314,7 +355,14 @@ def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tens
     With ``src_index`` (B, V) (``check_src_index``) it is one launch of magnet_cost_volume_indexed_f32 instead:
     ``src_feat`` (and ``src_gmm``) then hold any number of source images, each packed once, and view (b, v) reads image
     ``src_index[b, v]``; ``n_src``, when given, must be the number of images they hold.  ``check_index=False`` skips the
-    range check of the table (the caller has checked it).  None: the view-major operands of V*B images."""
+    range check of the table (the caller has checked it).  None: the view-major operands of V*B images.
+    Under torch.compile the view-major form is the registered op ``magnet_b200::cost_volume``; the indexed form is not
+    registered (its table is range-checked on the host)."""
+    if _traced() and src_index is None:
+        _no_out_traced(out)
+        return _op("cost_volume")(ref_feat, src_feat, rays, cams, int(V), int(src_layout), bool(consistency), src_gmm,
+                                  float(kappa), d_volume, ref_gmm, None if k is None else k_array(k), bool(planes),
+                                  bool(softmax), int(variant), ref_split)
     ref_feat = _need_cuda("ref_feat", ref_feat) if src_layout == _lib.SRC_HALF16 else _need_cuda_f32("ref_feat", ref_feat)
     if src_layout not in PACKED_LAYOUTS:                   # the packed buffers are checked below, by their size
         src_feat = _need_cuda_f32("src_feat", src_feat)
@@ -554,6 +602,8 @@ class GaussianUpdate(torch.autograd.Function):
 
 
 def gaussian_update(d_output: torch.Tensor, ref_gmm: torch.Tensor) -> torch.Tensor:
+    if _traced() and not (torch.is_grad_enabled() and d_output.requires_grad):
+        return _op("gaussian_update")(d_output, ref_gmm.detach())
     return GaussianUpdate.apply(d_output, ref_gmm)
 
 
@@ -581,11 +631,16 @@ def pack_gnet_weights(gnet, D: int) -> torch.Tensor:
     from the module at each call (nothing is cached).  Two launches."""
     c0, c1, c2, c3 = _gnet_convs(gnet, D)
     _check_cost_channels(D)
+    ws = [t.detach() for t in (c0.weight[:, :D], c1.weight, c1.bias, c2.weight, c2.bias, c3.weight, c3.bias)]
+    if _traced():
+        return _op("pack_gnet_weights")(ws, int(D))
+    return _pack_gnet(ws, D)
+
+
+def _pack_gnet(ws, D: int) -> torch.Tensor:
+    """``pack_gnet_weights`` of the detached tensors W0[:, :D], W1, b1, W2, b2, W3, b3."""
     nbytes = gnet_weights_bytes(D)
-    with torch.no_grad():
-        w0 = _need_cuda_f32("W0", c0.weight[:, :D])
-        ts = [w0] + [_need_cuda_f32(nm, t) for nm, t in (("W1", c1.weight), ("b1", c1.bias), ("W2", c2.weight),
-                                                         ("b2", c2.bias), ("W3", c3.weight), ("b3", c3.bias))]
+    ts = [_need_cuda_f32(nm, t) for nm, t in zip(("W0", "W1", "b1", "W2", "b2", "W3", "b3"), ws)]
     dev = _same_device(*((f"weight {i}", t) for i, t in enumerate(ts)))
     out = torch.empty(nbytes, device=dev, dtype=torch.uint8)
     _launch(dev, "magnet_gnet_pack_weights_f32", *(t.data_ptr() for t in ts), int(D), out.data_ptr())
@@ -597,6 +652,9 @@ def gnet_update(cost: torch.Tensor, invariant: torch.Tensor, packed: torch.Tenso
     """One inference iteration of the G-Net head and the Gaussian update in one fused kernel: cost (B,D,H,W),
     invariant (B,128,H,W) = ``GNET.invariant_part(x_d3, D)``, packed = ``pack_gnet_weights(g_net, D)``, prev_gmm
     (B,2,H,W) -> the updated (B,2,H,W) Gaussian.  Not differentiable (forward only)."""
+    if _traced():
+        _no_out_traced(out)
+        return _op("gnet_update")(cost, invariant, packed, prev_gmm)
     cost = _need_cuda_f32("cost", cost)
     if cost.dim() != 4:
         raise _lib.MagnetError(f"cost must be (B,D,H,W), got {tuple(cost.shape)}")
@@ -719,6 +777,8 @@ class ConvexUpsample(torch.autograd.Function):
 
 
 def convex_upsample(depth: torch.Tensor, up_mask: torch.Tensor, k: int) -> torch.Tensor:
+    if _traced() and not (torch.is_grad_enabled() and (depth.requires_grad or up_mask.requires_grad)):
+        return _op("convex_upsample")(depth, up_mask, int(k))
     return ConvexUpsample.apply(depth, up_mask, k)
 
 
@@ -796,9 +856,15 @@ def pack_mask_weights(mask_head) -> torch.Tensor:
     biases.  The first (3x3) layer stays outside (``MagnetHead.mask_pre``).  Read from the module at each call (nothing
     is cached).  Two launches."""
     _, c1, c2, c3 = _mask_convs(mask_head)
-    with torch.no_grad():
-        ts = [_need_cuda_f32(nm, t) for nm, t in (("W1", c1.weight), ("b1", c1.bias), ("W2", c2.weight),
-                                                  ("b2", c2.bias), ("W3", c3.weight), ("b3", c3.bias))]
+    ws = [t.detach() for t in (c1.weight, c1.bias, c2.weight, c2.bias, c3.weight, c3.bias)]
+    if _traced():
+        return _op("pack_mask_weights")(ws)
+    return _pack_mask(ws)
+
+
+def _pack_mask(ws) -> torch.Tensor:
+    """``pack_mask_weights`` of the detached tensors W1, b1, W2, b2, W3, b3."""
+    ts = [_need_cuda_f32(nm, t) for nm, t in zip(("W1", "b1", "W2", "b2", "W3", "b3"), ws)]
     dev = _same_device(*((f"weight {i}", t) for i, t in enumerate(ts)))
     out = torch.empty(mask_weights_bytes(4), device=dev, dtype=torch.uint8)
     _launch(dev, "magnet_mask_pack_weights_f32", *(t.data_ptr() for t in ts), out.data_ptr())
@@ -813,6 +879,8 @@ def mask_upsample(pre0: torch.Tensor, packed: torch.Tensor, preds, k: int = 4) -
     written.  k = 4 only.  Not differentiable (forward only): training runs the mask head, the upsampling and the
     loss through ``mask_head_loss``, which has a backward."""
     preds = _pred_list(preds)
+    if _traced():
+        return _op("mask_upsample")(pre0, packed, preds, int(k))
     if not preds:
         raise _lib.MagnetError("mask_upsample needs at least one prediction")
     _check_k4(k)
@@ -870,12 +938,18 @@ def _pack_dnet_layers(layers) -> torch.Tensor:
     """``pack_dnet_weights`` of the heads' convolutions as ``dnet_head_layers`` returns them."""
     (_, d1, d2), m = layers
     k = 0 if m is None else 4
-    named = [("depth W1", d1.weight), ("depth b1", d1.bias), ("depth W2", d2.weight), ("depth b2", d2.bias)]
-    if m is not None:
-        named += [("mask W1", m[1].weight), ("mask b1", m[1].bias), ("mask W3", m[2].weight), ("mask b3", m[2].bias)]
-    with torch.no_grad():
-        ts = [_need_cuda_f32(nm, t) for nm, t in named]
-    dev = _same_device(*zip([nm for nm, _ in named], ts))
+    ws = [d1.weight, d1.bias, d2.weight, d2.bias] + ([] if m is None else [m[1].weight, m[1].bias, m[2].weight, m[2].bias])
+    ws = [t.detach() for t in ws]
+    if _traced():
+        return _op("pack_dnet_weights")(ws, k)
+    return _pack_dnet(ws, k)
+
+
+def _pack_dnet(ws, k: int) -> torch.Tensor:
+    """``pack_dnet_weights`` of the detached tensors depth W1, b1, W2, b2 and, for k = 4, mask W1, b1, W3, b3."""
+    names = ["depth W1", "depth b1", "depth W2", "depth b2", "mask W1", "mask b1", "mask W3", "mask b3"][:len(ws)]
+    ts = [_need_cuda_f32(nm, t) for nm, t in zip(names, ws)]
+    dev = _same_device(*zip(names, ts))
     out = torch.empty(dnet_weights_bytes(k), device=dev, dtype=torch.uint8)
     ptrs = [t.data_ptr() for t in ts] + [None] * (8 - len(ts))
     _launch(dev, "magnet_dnet_pack_weights_f32", *ptrs, k, out.data_ptr())
@@ -895,6 +969,8 @@ def dnet_depth(pre_d: torch.Tensor, packed: torch.Tensor, sigma: bool) -> torch.
     before its ReLU, packed = ``pack_dnet_weights(depth_head[, mask_head])`` -> (B,2,H,W): with ``sigma`` [mu, sigma] as
     activation_G_magnet gives it (DNET.py:62-67, MaGNet's mono_gmms), else the raw [mu, v] that ``dnet_upsample``
     reads.  Forward only."""
+    if _traced():
+        return _op("dnet_depth")(pre_d, packed, bool(sigma))
     pre_d = _need_hidden("pre_d", pre_d)
     _check_dnet_packed(packed, 0)
     B, _, H, W = pre_d.shape
@@ -909,6 +985,8 @@ def dnet_upsample(pre_m: torch.Tensor, packed: torch.Tensor, raw: torch.Tensor, 
     one kernel: pre_m (B,128,H,W) = the mask head's first convolution before its ReLU, packed = ``pack_dnet_weights(
     depth_head, mask_head)``, raw = ``dnet_depth(..., sigma=False)`` -> (B,2,4H,4W) [mu, var], what DNET(args)
     returns (DNET.py:56-60).  The 144-channel mask is never written.  k = 4 only.  Forward only."""
+    if _traced():
+        return _op("dnet_upsample")(pre_m, packed, raw, int(k))
     _check_k4(k, "D-Net mask head")
     pre_m = _need_hidden("pre_m", pre_m)
     _check_dnet_packed(packed, 4)
@@ -1129,9 +1207,12 @@ def plane_depth(volume: torch.Tensor, planes, *, scores: bool) -> torch.Tensor:
     ``plane_sweep_f(softmax=False)``; the softmax over the planes is fused in and the prediction is bit for bit the one
     ``fnet_l1_loss`` supervises.  ``scores=False``: ``volume`` is the probability volume of ``est_costvolume_F`` /
     ``MAGNET_F.forward``.  ``planes``: the D plane depths, a sequence of floats or the (1,D,1,1) ``d_center`` tensor
-    (read to the host once per tensor).  Half-precision volumes (torch.autocast) are upcast."""
+    (read to the host once per tensor; under torch.compile it must be the sequence of floats).  Half-precision volumes
+    (torch.autocast) are upcast."""
     if isinstance(volume, torch.Tensor) and volume.dtype in (torch.float16, torch.bfloat16):
         volume = volume.float()
+    if _traced():
+        return _op("plane_depth")(volume, k_array(planes), bool(scores))
     volume = _need_cuda_f32("volume", volume)
     if volume.dim() != 4:
         raise _lib.MagnetError(f"volume must be (B,D,H,W), got {tuple(volume.shape)}")
@@ -1151,6 +1232,8 @@ def plane_depth(volume: torch.Tensor, planes, *, scores: bool) -> torch.Tensor:
 def relative_poses(ext_ref: torch.Tensor, ext_nghbr: torch.Tensor):
     """data_preprocess (utils/utils.py:72-98) on the device: ext_ref (B,4,4), ext_nghbr (V,B,4,4) ->
     (nghbr_poses (B,V,4,4), is_valid (B,V) int32)."""
+    if _traced():
+        return tuple(_op("relative_poses")(ext_ref, ext_nghbr))
     ext_ref = _need_cuda_f32("ext_ref", ext_ref)
     ext_nghbr = _need_cuda_f32("ext_nghbr", ext_nghbr)
     V, B = ext_nghbr.shape[0], ext_nghbr.shape[1]
@@ -1167,6 +1250,9 @@ def camera_rays(raw_intrinsics: torch.Tensor, H: int, W: int):
     raw_intrinsics (B,8) float64 [fx, fy, cx, cy, img_W, img_H, left_margin, top_margin] (a (B,6) tensor
     [fx, fy, cx, cy, raw_W, raw_H] is accepted as the ScanNet case: no crop) -> cam_intrins dict
     {'intM' (B,3,3), 'unit_ray_array_2D' (B,3,H*W)} (device)."""
+    if _traced():
+        intM, rays = _op("camera_rays")(raw_intrinsics, int(H), int(W))
+        return {"intM": intM, "unit_ray_array_2D": rays}
     if not raw_intrinsics.is_cuda or raw_intrinsics.dtype != torch.float64 or raw_intrinsics.dim() != 2 \
             or raw_intrinsics.shape[1] not in (6, 8):
         raise _lib.MagnetError("raw_intrinsics must be a CUDA float64 tensor (B,8) (or (B,6) without crop margins)")
@@ -1217,6 +1303,9 @@ def depth_metrics(pred_or_list, gt: torch.Tensor, *, min_depth: float, max_depth
     metrics in METRIC_KEYS order (NaN for an image without a valid pixel; nll 0.0 there in the nearest form).  Two
     kernel launches, no host sync."""
     preds = _pred_list(pred_or_list)
+    if _traced():
+        return _op("depth_metrics")(preds, gt, float(min_depth), float(max_depth), crop, up_mask,
+                                    None if k is None else int(k), bool(nearest), bool(variance))
     if not 1 <= len(preds) <= _lib.MAGNET_METRICS_MAX_PRED:
         raise _lib.MagnetError(f"1 to {_lib.MAGNET_METRICS_MAX_PRED} predictions per call, got {len(preds)}")
     if nearest and (up_mask is not None or k is not None):
