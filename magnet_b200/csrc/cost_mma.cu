@@ -62,6 +62,7 @@ constexpr int MTW = 8, MTH = 8;        // CTA tile in reference pixels
 constexpr int MPX = MTW * MTH;         // 64 = rows of the accumulator that are used
 constexpr int MCH = 64;                // hypotheses per CTA (two per lane)
 constexpr int MSEG = 32;               // 8-cell segments per window: N <= 256 accumulator columns
+constexpr int MBATCH = 4;              // pixels of a tile row evaluated together in phase C (see there)
 constexpr int MMAXV = 16;              // views whose camera constants are staged in shared memory
 constexpr int SEG_BYTES = 2048;        // hi atom (8 cells x 128 B) + lo atom
 constexpr int META_SEG_BYTES = 128;    // 8 cells x (mu, sigma of the cell and of its right neighbour)
@@ -372,15 +373,6 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
     }
     __syncwarp();
     const int vb = src_image<IDX>(src_index, b, v, p.B, V);
-    // sample position of my two hypotheses of pixel i of the row, clamped: anything left of -1 / right of W (above /
-    // below likewise) has all four taps out of the image, so cells stay near the image and NaN (fmaxf drops it) maps to
-    // "out of bounds"; z = depth in the source camera
-    auto project_px = [&](const int i, float2& ix, float2& iy, float2& z) {
-      const float4 t1 = pixt[2 * i], t2 = pixt[2 * i + 1];   // same address on every lane: broadcast
-      project2(depth2(i, t2.y, t2.z), t1.w, t2.x, t2.w, t1.x, t1.y, t1.z, ix, iy, z);
-      ix.x = clamp_coord(ix.x, xmax); ix.y = clamp_coord(ix.y, xmax);
-      iy.x = clamp_coord(iy.x, ymax); iy.y = clamp_coord(iy.y, ymax);
-    };
 
     // the box of this view was completed by the barrier that ended the previous pass (or the item set-up)
     const int* bb = bbox + (it & 1) * 4;
@@ -487,8 +479,16 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
         }
 #endif
         // ---------------- per hypothesis: 4 G reads, 4 table reads, 3 bilinear interpolations -------------------
-        // byte offset of cell (x0, y0) in a G row = 4 * ((y0 - sy) * pitch + (x0 - sx)), evaluated in fp32 (small
-        // integers, exact) on top of 1.5 * 2^23 so that the integer sits in the mantissa
+        // The pixels of the row go in batches of MBATCH, stage by stage: the batch's pixel constants and depths, then
+        // its projections and cell offsets, then all its G and table reads, then the interpolations and adds, so the
+        // chains of the batch's pixels overlap.  Inside a batch there is no branch: a dead pixel reads cells inside
+        // the window like any other (the min / select below) and liveness only predicates its adds.  A warp-uniform
+        // branch skips a batch
+        // without a live pixel; it also bounds the block ptxas schedules as one.  With the whole row in one block,
+        // ptxas (CUDA 12.9) needs more than 128 registers and serialises the wgmma of <GAUSS, true> (C7511); with
+        // blocks of 4 pixels no instantiation has more spills or C7511 / C7520 warnings than with one pixel per
+        // block.  Each hypothesis sees the same operations in the same order as with one pixel at a time, so the
+        // accumulators are the same bit for bit.
         const bool single = nseg_all * rows_all <= MSEG;    // every cell origin lies in this (only) window
         auto phase_c = [&](auto single_tag) {
           constexpr bool SINGLE = decltype(single_tag)::value;
@@ -498,60 +498,101 @@ cost_mma_kernel(const __grid_constant__ CostParams p, const __grid_constant__ CU
           const float pitch4f = (float)(nseg * 32);
           const float c0f = MAGIC - 4.0f * sxf - pitch4f * syf;   // exact: integers below 2^24
           const uint32_t pitch4 = (uint32_t)nseg * 32u;
-          uint32_t rowaddr = g_row0 + (uint32_t)(warp * 8 * gp) * 4u;
+          uint32_t rowaddr = g_row0 + (uint32_t)(warp * 8 * gp) * 4u;   // G row of pixel i0 (one running address)
           const uint32_t cmax = pitch4 * (uint32_t)(rows - 1) - 8u;   // last cell origin of the window (bytes)
+          const float2 m1 = make_float2(-1.0f, -1.0f);
 #pragma unroll
-          for (int i = 0; i < MTW; ++i, rowaddr += (uint32_t)gp * 4u) {
-            if (!((livemask >> i) & 1u)) continue;         // warp-uniform
-            float2 x, y, z;
-            project_px(i, x, y, z);
-            float2 x0, y0, fx, fy;                         // cell origins and fractions (cw_mask.cuh)
-            cell_split(x.x, x0.x, fx.x); cell_split(x.y, x0.y, fx.y);
-            cell_split(y.x, y0.x, fy.x); cell_split(y.y, y0.y, fy.y);
-            const float2 m1 = make_float2(-1.0f, -1.0f);
-            // byte offset of the cell in a G row = 4 * ((y0 - sy) * pitch + (x0 - sx)), in fp32 (small integers, exact)
-            // on top of 1.5 * 2^23 so that the integer sits in the mantissa
-            const float2 o = ffma2_rn(y0, make_float2(pitch4f, pitch4f), ffma2_rn(x0, make_float2(4.0f, 4.0f), make_float2(c0f, c0f)));
-            uint32_t ca = __float_as_uint(o.x) & 0x3fffffu, cb = __float_as_uint(o.y) & 0x3fffffu;
-            bool pa = true, pb = true;
-            if (!SINGLE) {                                 // evaluated in the sub-window that holds the cell origin
-              pa = x0.x >= sxf && x0.x < xend && y0.x >= syf && y0.x < yend;
-              pb = x0.y >= sxf && x0.y < xend && y0.y >= syf && y0.y < yend;
-              ca = pa ? ca : 0u;                           // the others read cell 0
-              cb = pb ? cb : 0u;
-            } else {                                       // a wrong box can never address outside the window
-              ca = min(ca, cmax);
-              cb = min(cb, cmax);
+          for (int i0 = 0; i0 < MTW; i0 += MBATCH, rowaddr += (uint32_t)(MBATCH * gp) * 4u) {
+            if (!((livemask >> i0) & ((1u << MBATCH) - 1u))) continue;   // warp-uniform
+            float4 t1[MBATCH], t2[MBATCH];                 // pixel table: same address on every lane, broadcast
+            float2 d[MBATCH];
+#pragma unroll
+            for (int u = 0; u < MBATCH; ++u) {
+              t1[u] = pixt[2 * (i0 + u)];
+              t2[u] = pixt[2 * (i0 + u) + 1];
             }
+#pragma unroll
+            for (int u = 0; u < MBATCH; ++u) d[u] = depth2(i0 + u, t2[u].y, t2[u].z);
+            float2 z[MBATCH], fx[MBATCH], fy[MBATCH];
+            uint32_t ca[MBATCH], cb[MBATCH];
+            bool pa[MBATCH], pb[MBATCH];
+#pragma unroll
+            for (int u = 0; u < MBATCH; ++u) {
+              // sample position of my two hypotheses, clamped: anything left of -1 / right of W (above / below
+              // likewise) has all four taps out of the image, so cells stay near the image and NaN (fmaxf drops it)
+              // maps to "out of bounds"; z = depth in the source camera
+              float2 x, y;
+              project2(d[u], t1[u].w, t2[u].x, t2[u].w, t1[u].x, t1[u].y, t1[u].z, x, y, z[u]);
+              x.x = clamp_coord(x.x, xmax); x.y = clamp_coord(x.y, xmax);
+              y.x = clamp_coord(y.x, ymax); y.y = clamp_coord(y.y, ymax);
+              float2 x0, y0;                               // cell origins and fractions (cw_mask.cuh)
+              cell_split(x.x, x0.x, fx[u].x); cell_split(x.y, x0.y, fx[u].y);
+              cell_split(y.x, y0.x, fy[u].x); cell_split(y.y, y0.y, fy[u].y);
+              // byte offset of the cell in a G row = 4 * ((y0 - sy) * pitch + (x0 - sx)), in fp32 (small integers,
+              // exact) on top of 1.5 * 2^23 so that the integer sits in the mantissa
+              const float2 o = ffma2_rn(y0, make_float2(pitch4f, pitch4f), ffma2_rn(x0, make_float2(4.0f, 4.0f), make_float2(c0f, c0f)));
+              ca[u] = __float_as_uint(o.x) & 0x3fffffu;
+              cb[u] = __float_as_uint(o.y) & 0x3fffffu;
+              const bool live = (livemask >> (i0 + u)) & 1u;
+              pa[u] = live;
+              pb[u] = live;
+              if (!SINGLE) {                               // evaluated in the sub-window that holds the cell origin
+                pa[u] = live && x0.x >= sxf && x0.x < xend && y0.x >= syf && y0.x < yend;
+                pb[u] = live && x0.y >= sxf && x0.y < xend && y0.y >= syf && y0.y < yend;
+                ca[u] = pa[u] ? ca[u] : 0u;                // the others (dead pixels too) read cell 0
+                cb[u] = pb[u] ? cb[u] : 0u;
+              } else {                                     // a wrong box can never address outside the window
+                ca[u] = min(ca[u], cmax);
+                cb[u] = min(cb[u], cmax);
+              }
 #ifdef MAGNET_MMA_DEBUG
-            if (dbg != nullptr && sy == wy0 && sx == wx0) {  // hypotheses whose cell origin fell outside the box
-              const bool outa = lane < Dc && (x0.x < (float)wx0 || x0.x > (float)wx1 || y0.x < (float)wy0 || y0.x > (float)wy1);
-              const bool outb = lane + 32 < Dc && (x0.y < (float)wx0 || x0.y > (float)wx1 || y0.y < (float)wy0 || y0.y > (float)wy1);
-              const unsigned nout = __popc(__ballot_sync(FULL, outa)) + __popc(__ballot_sync(FULL, outb));
-              if (lane == 0 && nout != 0u) atomicAdd(reinterpret_cast<unsigned*>(dbg + MMA_DBG_OUTSIDE), nout);
-            }
+              if (dbg != nullptr && sy == wy0 && sx == wx0) {   // hypotheses whose cell origin fell outside the box
+                const bool outa = live && lane < Dc && (x0.x < (float)wx0 || x0.x > (float)wx1 || y0.x < (float)wy0 || y0.x > (float)wy1);
+                const bool outb = live && lane + 32 < Dc && (x0.y < (float)wx0 || x0.y > (float)wx1 || y0.y < (float)wy0 || y0.y > (float)wy1);
+                const unsigned nout = __popc(__ballot_sync(FULL, outa)) + __popc(__ballot_sync(FULL, outb));
+                if (lane == 0 && nout != 0u) atomicAdd(reinterpret_cast<unsigned*>(dbg + MMA_DBG_OUTSIDE), nout);
+              }
 #endif
-            const uint32_t ga = rowaddr + ca, gb = rowaddr + cb;
-            const float2 g00 = make_float2(lds_f32(ga), lds_f32(gb)), g01 = make_float2(lds_f32(ga + 4), lds_f32(gb + 4));
-            const float2 g10 = make_float2(lds_f32(ga + pitch4), lds_f32(gb + pitch4));
-            const float2 g11 = make_float2(lds_f32(ga + pitch4 + 4), lds_f32(gb + pitch4 + 4));
-            const float2 ct = ffma2_rn(fx, ffma2_rn(g00, m1, g01), g00), cu = ffma2_rn(fx, ffma2_rn(g10, m1, g11), g10);
-            const float2 cost = ffma2_rn(fy, ffma2_rn(ct, m1, cu), ct);            // both hypotheses at once
-            const float costa = cost.x, costb = cost.y;
-            bool oka, okb;
-            if (CW) {
-              const uint32_t ma = m_base + ca * 4u, mb = m_base + cb * 4u;
-              // table entry of a cell = (mu, sigma) of the cell and of its right neighbour: two 16-byte reads per hypothesis
-              const float2 msa = lerp2d_x2(lds_f32x4(ma), lds_f32x4(ma + pitch4 * 4u), fx.x, fy.x);
-              const float2 msb = lerp2d_x2(lds_f32x4(mb), lds_f32x4(mb + pitch4 * 4u), fx.y, fy.y);
-              oka = cw_keep(z.x, msa, kappa);               // homography.py:157-158 (cw_mask.cuh)
-              okb = cw_keep(z.y, msb, kappa);
-            } else {
-              oka = fabsf(costa) < 3.0e38f;
-              okb = fabsf(costb) < 3.0e38f;
             }
-            if (pa && oka) accr[i].x += costa;
-            if (pb && okb) accr[i].y += costb;
+            float2 g00[MBATCH], g01[MBATCH], g10[MBATCH], g11[MBATCH];
+            float4 mta[MBATCH], mba[MBATCH], mtb[MBATCH], mbb[MBATCH];   // (CW) table: top / bottom row x hypothesis a / b
+            uint32_t ra = rowaddr;
+#pragma unroll
+            for (int u = 0; u < MBATCH; ++u, ra += (uint32_t)gp * 4u) {
+              const uint32_t ga = ra + ca[u], gb = ra + cb[u];
+              g00[u] = make_float2(lds_f32(ga), lds_f32(gb));
+              g01[u] = make_float2(lds_f32(ga + 4), lds_f32(gb + 4));
+              g10[u] = make_float2(lds_f32(ga + pitch4), lds_f32(gb + pitch4));
+              g11[u] = make_float2(lds_f32(ga + pitch4 + 4), lds_f32(gb + pitch4 + 4));
+              if (CW) {
+                // table entry of a cell = (mu, sigma) of the cell and of its right neighbour: two 16-byte reads per
+                // hypothesis
+                const uint32_t ma = m_base + ca[u] * 4u, mb = m_base + cb[u] * 4u;
+                mta[u] = lds_f32x4(ma);
+                mba[u] = lds_f32x4(ma + pitch4 * 4u);
+                mtb[u] = lds_f32x4(mb);
+                mbb[u] = lds_f32x4(mb + pitch4 * 4u);
+              }
+            }
+#pragma unroll
+            for (int u = 0; u < MBATCH; ++u) {
+              const float2 ct = ffma2_rn(fx[u], ffma2_rn(g00[u], m1, g01[u]), g00[u]);
+              const float2 cu = ffma2_rn(fx[u], ffma2_rn(g10[u], m1, g11[u]), g10[u]);
+              const float2 cost = ffma2_rn(fy[u], ffma2_rn(ct, m1, cu), ct);        // both hypotheses at once
+              const float costa = cost.x, costb = cost.y;
+              bool oka, okb;
+              if (CW) {
+                const float2 msa = lerp2d_x2(mta[u], mba[u], fx[u].x, fy[u].x);
+                const float2 msb = lerp2d_x2(mtb[u], mbb[u], fx[u].y, fy[u].y);
+                oka = cw_keep(z[u].x, msa, kappa);          // homography.py:157-158 (cw_mask.cuh)
+                okb = cw_keep(z[u].y, msb, kappa);
+              } else {
+                oka = fabsf(costa) < 3.0e38f;
+                okb = fabsf(costb) < 3.0e38f;
+              }
+              if (pa[u] && oka) accr[i0 + u].x += costa;
+              if (pb[u] && okb) accr[i0 + u].y += costb;
+            }
           }
         };
         if (single) phase_c(std::true_type{});
