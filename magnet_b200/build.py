@@ -17,9 +17,10 @@ PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 BUILD = PKG / "_build"
 LIB = PKG / "libmagnet_b200.so"
-SOURCES = ["api.cu", "cost_mma.cu", "cost_tma.cu", "cost_cells.cu", "cost_direct.cu", "cost_f_bwd.cu", "cost_f_bwd_mma.cu", "cost_cw_bwd.cu", "fnet_l1.cu",
+SOURCES = ["api.cu", "launch_common.cu", "split16.cu", "cost_mma.cu", "cost_tma.cu", "cost_cells.cu", "cost_direct.cu", "cost_f_bwd.cu", "cost_f_bwd_mma.cu", "cost_cw_bwd.cu", "fnet_l1.cu",
            "plane_depth.cu", "aux_kernels.cu", "depth_metrics.cu", "gnet_head.cu", "mask_head.cu", "dnet_head.cu", "head_pack.cu"]
-HEADERS = [CSRC / "common.cuh", CSRC / "cells_common.cuh", CSRC / "tma_common.cuh", CSRC / "cw_mask.cuh",
+HEADERS = [CSRC / "common.cuh", CSRC / "launchers.h", CSRC / "packed_layout.cuh", CSRC / "cells_common.cuh",
+           CSRC / "tma_common.cuh", CSRC / "cw_mask.cuh",
            CSRC / "upsample_common.cuh", CSRC / "gaussian_common.cuh", CSRC / "head_common.cuh", CSRC / "soft_argmin.cuh", PKG.parent / "include" / "magnet_b200.h"]
 ARCH = "arch=compute_90a,code=sm_90a"
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", ARCH, "-lineinfo",
@@ -67,7 +68,7 @@ def build(force: bool = False, verbose: bool = False, defines=(), tag: str = "")
 
     with ThreadPoolExecutor(max_workers=len(SOURCES)) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    cmd = [nvcc, "-shared", "-gencode", ARCH, "-o", str(lib), *map(str, objs)]
+    cmd = [nvcc, "-shared", "-gencode", ARCH, "-Xlinker", "--no-undefined", "-o", str(lib), *map(str, objs)]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

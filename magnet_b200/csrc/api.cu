@@ -5,123 +5,7 @@
 #include <cstring>
 
 #include "common.cuh"
-
-namespace magnet {
-cudaError_t launch_cost_direct(const CostParams& p, int depth_mode, int src_layout, int C, bool cw,
-                               bool softmax, const int32_t* src_index, cudaStream_t st, int* launches);
-cudaError_t launch_cost_cells(const CostParams& p, int mode, int C, bool cw, bool reuse, const int32_t* src_index,
-                              cudaStream_t st);
-cudaError_t launch_softmax_planes(float* vol, int B, int D, int HW, cudaStream_t st);
-bool cells_supports(int C, int D, int layout);
-cudaError_t launch_cost_tma(const CostParams& p, int mode, int C, bool cw, const int32_t* src_index, int n_src,
-                            cudaStream_t st);
-bool tma_supports(int C, int D, int V, int layout);
-void tma_launch_info(int B, int H, int W, int D, int* grid, int* block, int* smem);
-cudaError_t launch_cost_mma(const CostParams& p, int mode, bool cw, int layout, const int32_t* src_index, int n_src,
-                            cudaStream_t st);
-bool mma_supports(int C, int D, int V, int layout);
-void mma_launch_info(int B, int H, int W, int D, int* grid, int* block, int* smem);
-size_t split16_buffer_bytes(int N, int H, int W);
-size_t half16_buffer_bytes(int N, int H, int W);
-cudaError_t launch_repack_split16(const float* src, const float* gmm, void* dst, int N, int C, int H, int W,
-                                  cudaStream_t st, int* launches);
-cudaError_t launch_repack_half16(const void* src, int dtype, const float* gmm, void* dst, int N, int C, int H, int W,
-                                 cudaStream_t st, int* launches);
-#if defined(MAGNET_MMA_DEBUG) || defined(MAGNET_MMA_PROFILE)
-void mma_set_debug_buffer(float* p);
-#endif
-cudaError_t launch_repack_pixc(const float* src, const float* gmm, float* dst, int N, int C, int H, int W,
-                               cudaStream_t st);
-void cells_launch_info(int B, int H, int W, int D, int* grid, int* block, int* smem);
-cudaError_t launch_pack_cameras(const float* intM, const float* R, int64_t r_sb, int64_t r_sv, int64_t r_si,
-                                int64_t r_sj, const float* t, int64_t t_sb, int64_t t_sv, int64_t t_si,
-                                const int32_t* is_valid, int B, int V, magnet_camera* out, cudaStream_t st);
-cudaError_t launch_repack(const float* src, float* dst, int N, int C, int H, int W, cudaStream_t st);
-cudaError_t launch_sample(const float* gmm, const float* k_host, int B, int D, int HW, float* dvol,
-                          cudaStream_t st);
-cudaError_t launch_update_fwd(const float* dout, const float* gmm0, int B, int HW, float* out, cudaStream_t st);
-cudaError_t launch_update_bwd(const float* gout, const float* dout, const float* gmm0, int B, int HW, float* gin,
-                              cudaStream_t st);
-cudaError_t launch_relative_poses(const float* ext_ref, const float* ext_nghbr, int B, int V, float* poses,
-                                  int32_t* valid, cudaStream_t st);
-cudaError_t launch_camera_rays(const double* raw, int B, int H, int W, float* intM, float* rays, cudaStream_t st);
-cudaError_t launch_upsample_fwd(const float* depth, const float* mask, int B, int CH, int H, int W, int k, float* out,
-                                cudaStream_t st);
-cudaError_t launch_upsample_bwd(const float* gout, const float* depth, const float* mask, int B, int CH, int H, int W,
-                                int k, float* gdepth, float* gmask, cudaStream_t st);
-cudaError_t launch_cost_f_bwd(const BwdParams& p, cudaStream_t st, int* launches);
-cudaError_t launch_cost_f_bwd_mma(const BwdParams& p, int layout, cudaStream_t st, int* launches);
-bool f_bwd_mma_supports(int C, int V);
-cudaError_t launch_cost_cw_bwd(const CwBwdParams& p, const CwBwdParams* split, int split_layout, int C, int mode,
-                               bool mask_mma, const float* grad_out, cudaStream_t st, int* launches);
-bool cw_bwd_supports(int C);
-size_t geom_workspace_bytes(int B, int V, int H, int W);
-cudaError_t launch_cost_geom_bwd(const CwBwdParams& p, int C, int mode, bool mask_mma, int softmax, const float* prob,
-                                 const float* grad_out, float* partials, float* grad_rays, float* grad_cams,
-                                 cudaStream_t st, int* launches);
-#ifdef MAGNET_MMA_DEBUG
-void f_bwd_mma_set_debug_buffer(float* p);
-#endif
-int fnet_l1_partials(int B, int HW);
-cudaError_t launch_fnet_l1_fwd(const float* scores, const float* planes, const float* gt, const uint8_t* mask, int B,
-                               int D, int HW, float* partial, cudaStream_t st);
-cudaError_t launch_fnet_l1_bwd(const float* scores, const float* planes, const float* gt, const uint8_t* mask,
-                               float scale, const float* grad_scale, int B, int D, int HW, float* grad_scores,
-                               cudaStream_t st);
-cudaError_t launch_upsample_nll_fwd(const float* depth, const float* mask, const float* gt, const uint8_t* gtm, int B,
-                                    int H, int W, int k, float* partial, cudaStream_t st);
-cudaError_t launch_upsample_nll_bwd(const float* depth, const float* mask, const float* gt, const uint8_t* gtm, float scale,
-                                    int B, int H, int W, int k, float* gdepth, float* gmask, cudaStream_t st);
-cudaError_t launch_plane_depth(const float* vol, const float* planes, int B, int D, int HW, bool scores, float* out,
-                               cudaStream_t st);
-size_t depth_metrics_workspace(int P, int B, int rows, int cols);
-cudaError_t launch_depth_metrics(const float* const* preds, int P, const float* up_mask, const float* gt, int B, int H,
-                                 int W, int k, int h, int w, bool variance, int r0, int r1, int c0, int c1, float min_d,
-                                 float max_d, double* partial, double* out, cudaStream_t st);
-size_t dnet_weights_bytes(bool with_mask);
-cudaError_t launch_dnet_pack(const float* dw1, const float* db1, const float* dw2, const float* db2, const float* mw1,
-                             const float* mb1, const float* mw3, const float* mb3, bool with_mask, void* dst,
-                             cudaStream_t st);
-cudaError_t launch_dnet_depth(int B, int H, int W, const float* pre_d, const void* weights, bool sigma, float* out,
-                              cudaStream_t st);
-cudaError_t launch_dnet_upsample_packed(int B, int H, int W, const float* pre_m, const void* weights, const float* raw,
-                                        float* out, cudaStream_t st);
-size_t gnet_weights_bytes(int D);
-cudaError_t launch_gnet_pack(const float* w0, const float* w1, const float* b1, const float* w2, const float* b2,
-                             const float* w3, const float* b3, int D, void* dst, cudaStream_t st);
-cudaError_t launch_gnet_update(int B, int D, int H, int W, const float* cost, const float* inv, const void* weights,
-                               const float* prev, unsigned* scratch, float* out, cudaStream_t st);
-size_t gnet_train_weights_bytes(int D);
-size_t mask_weights_bytes();
-cudaError_t launch_mask_pack(const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
-                             const float* b3, void* dst, cudaStream_t st);
-cudaError_t launch_mask_upsample(int P, int B, int H, int W, const float* pre0, const void* weights,
-                                 const float* const* pred, float* const* out, cudaStream_t st);
-size_t mask_train_weights_bytes();
-int mask_train_partials(int B, int H, int W);
-size_t mask_saved_bytes(int P, int B, int H, int W);
-size_t mask_bwd_workspace_bytes(int B, int H, int W);
-cudaError_t launch_mask_pack_train(const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
-                                   const float* b3, void* dst, cudaStream_t st);
-cudaError_t launch_mask_train_fwd(int P, int B, int H, int W, const float* pre0, const void* weights,
-                                  const float* const* pred, const float* gt, const unsigned char* gtm,
-                                  const float* scale, bool save_maps, bool pred_grad, float* partial, float* saved,
-                                  cudaStream_t st, int* launches);
-cudaError_t launch_mask_bwd(int P, int B, int H, int W, const void* weights, const float* saved, const float* gscale,
-                            void* workspace, float* grad_pre0, float* gw1, float* gb1, float* gw2, float* gb2,
-                            float* gw3, float* gb3, float* const* grad_pred, cudaStream_t st, int* launches);
-size_t gnet_saved_bytes(int B, int H, int W);
-size_t gnet_bwd_workspace_bytes(int B, int D, int H, int W);
-cudaError_t launch_gnet_pack_train(const float* w0, const float* w1, const float* b1, const float* w2, const float* b2,
-                                   const float* w3, const float* b3, int D, void* dst, cudaStream_t st);
-cudaError_t launch_gnet_train_fwd(int B, int D, int H, int W, const float* cost, const float* inv, const void* weights,
-                                  const float* prev, unsigned* scratch, float* out, float* saved, cudaStream_t st);
-cudaError_t launch_gnet_bwd(int B, int D, int H, int W, const float* cost, const float* prev, const void* weights,
-                            const float* saved, const float* grad, void* workspace, float* grad_inv, float* gw0,
-                            float* gw1, float* gb1, float* gw2, float* gb2, float* gw3, float* gb3, float* grad_prev,
-                            cudaStream_t st, int* launches);
-}  // namespace magnet
-
+#include "launchers.h"
 
 namespace {
 std::atomic<uint64_t> g_launches{0};
@@ -303,22 +187,19 @@ int run_cost(const magnet_cost_args* a, const int32_t* src_index, int n_src, voi
   int launches = 0;
   cudaError_t e;
   const cudaStream_t st = (cudaStream_t)stream;
-  if (use_mma(a) || use_tma(a) || use_cells(a)) {
-    if (use_mma(a))
-      e = magnet::launch_cost_mma(p, a->depth_mode, a->consistency != 0, a->src_layout, src_index, n_src, st);
-    else if (use_tma(a))
-      e = magnet::launch_cost_tma(p, a->depth_mode, a->C, a->consistency != 0, src_index, n_src, st);
-    else
-      e = magnet::launch_cost_cells(p, a->depth_mode, a->C, a->consistency != 0,
-                                    a->variant != MAGNET_VARIANT_CELLS_NOREUSE, src_index, st);
-    launches = 1;
-    if (e == cudaSuccess && a->softmax) {          // homography.py:46, in place on the 1/V-averaged scores
-      e = magnet::launch_softmax_planes(a->out, a->B, a->D, a->H * a->W, st);
-      launches = 2;
-    }
-  } else {
-    e = magnet::launch_cost_direct(p, a->depth_mode, a->src_layout, a->C, a->consistency != 0, a->softmax != 0,
-                                   src_index, st, &launches);
+  const bool cw = a->consistency != 0;
+  if (use_mma(a))
+    e = magnet::launch_cost_mma(p, a->depth_mode, cw, a->src_layout, src_index, n_src, st, &launches);
+  else if (use_tma(a))
+    e = magnet::launch_cost_tma(p, a->depth_mode, a->C, cw, src_index, n_src, st, &launches);
+  else if (use_cells(a))
+    e = magnet::launch_cost_cells(p, a->depth_mode, a->C, cw, a->variant != MAGNET_VARIANT_CELLS_NOREUSE, src_index, st,
+                                  &launches);
+  else
+    e = magnet::launch_cost_direct(p, a->depth_mode, a->src_layout, a->C, cw, src_index, st, &launches);
+  if (e == cudaSuccess && a->softmax) {            // homography.py:46, in place on the 1/V-averaged scores
+    e = magnet::launch_softmax_planes(a->out, a->B, a->D, a->H * a->W, st);
+    ++launches;
   }
   return finish(e, launches);
 }

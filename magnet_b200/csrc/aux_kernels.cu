@@ -1,5 +1,6 @@
 // Small kernels around the cost volume: camera constants, source repack, sampler, Gaussian update.
 #include "common.cuh"
+#include "launchers.h"
 #include "gaussian_common.cuh"
 #include "upsample_common.cuh"
 

@@ -4,12 +4,12 @@
 #include <stdint.h>
 
 #include <mutex>
+#include <type_traits>
 
 #include "../../include/magnet_b200.h"
 
 namespace magnet {
 
-int sm_count(int dev);                                                  // cost_mma.cu
 inline size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
 
 // Opt-in shared memory (and, with max_carveout, the largest carveout): set once per (kernel, device), not on every
@@ -26,6 +26,58 @@ cudaError_t set_smem_once(K kern, std::once_flag (&flags)[64], int bytes, bool m
       e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   });
   return e;
+}
+
+// Runtime value -> compile-time constant.  A Choice<T, Vs...> holds a value that is one of Vs; dispatch(f, c...) calls
+// f(std::integral_constant<T, V>{}...) with the V that each choice holds, and returns cudaErrorInvalidValue when one
+// holds none of its Vs.  Every combination of the Vs is instantiated: a launcher whose kernel exists for only part of
+// the product says so with `if constexpr` in f.
+template <class T, T... Vs>
+struct Choice {
+  T value;
+};
+using DepthMode = Choice<int, MAGNET_DEPTH_VOLUME, MAGNET_DEPTH_GAUSS, MAGNET_DEPTH_PLANES>;
+using Flag = Choice<bool, false, true>;
+
+template <class F>
+cudaError_t dispatch(F&& f) {
+  return f();
+}
+template <class F, class T, T... Vs, class... Rest>
+cudaError_t dispatch(F&& f, Choice<T, Vs...> c, Rest... rest);
+template <class T, T V, class F, class... Rest>
+cudaError_t dispatch_fixed(F& f, Rest... rest) {   // f with its first argument bound to V
+  return dispatch([&f](auto... cs) { return f(std::integral_constant<T, V>{}, cs...); }, rest...);
+}
+template <class F, class T, T... Vs, class... Rest>
+cudaError_t dispatch(F&& f, Choice<T, Vs...> c, Rest... rest) {
+  cudaError_t e = cudaErrorInvalidValue;
+  (void)((c.value == Vs && ((e = dispatch_fixed<T, Vs>(f, rest...)), true)) || ...);
+  return e;
+}
+
+// Work slots of the persistent kernels: each launch takes one slot of its family's arrays (host ticket, work_slot() in
+// launchers.h); `next` counts the work items handed out, `done` the CTAs that finished, and the launch's last CTA
+// re-arms the slot, so a captured launch can be replayed and no memset precedes a launch.  Launches that share a slot
+// must not run concurrently: WORK_SLOTS / 2 eager launches or as many captured ones would have to be in flight at once.
+constexpr int WORK_SLOTS = 1024;
+
+// the next work item of the launch (0, 1, ... in claim order)
+__device__ __forceinline__ unsigned slot_claim(unsigned* next, int slot) { return atomicAdd(&next[slot], 1u); }
+
+// once per CTA, after its last global write: true in the launch's last CTA to finish
+__device__ __forceinline__ bool slot_last_cta(unsigned* done, int slot) {
+  __threadfence();
+  return atomicAdd(&done[slot], 1u) == gridDim.x - 1;
+}
+
+// once per CTA at exit: the last CTA re-arms the work counter
+__device__ __forceinline__ void slot_finish(unsigned* next, unsigned* done, int slot) {
+  if (slot_last_cta(done, slot)) {
+    next[slot] = 0u;
+    done[slot] = 0u;
+    __threadfence();
+  }
 }
 
 // Kernel-side view of magnet_cost_args; k values travel in the launch parameters

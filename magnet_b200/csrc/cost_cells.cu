@@ -41,6 +41,7 @@
 #include <mutex>
 
 #include "cells_common.cuh"
+#include "launchers.h"
 
 namespace magnet {
 
@@ -266,7 +267,7 @@ cost_cells_kernel(const __grid_constant__ CostParams p, const int chunk, const i
 static int cells_grid_x(int H, int W) { return ((W + TILE_W - 1) / TILE_W) * ((H + TILE_H - 1) / TILE_H); }
 
 template <int C, int MODE, bool CW, bool REUSE, bool IDX>
-static cudaError_t launch_cmwi(const CostParams& p, const int32_t* src_index, cudaStream_t st) {
+static cudaError_t launch_cells(const CostParams& p, const int32_t* src_index, cudaStream_t st) {
   static std::once_flag flags[64];
   auto kern = cost_cells_kernel<C, MODE, CW, REUSE, IDX>;
   cudaError_t e = set_smem_once(kern, flags, (int)cells_smem_bytes(MAGNET_MAX_PLANES), false);
@@ -276,28 +277,6 @@ static cudaError_t launch_cmwi(const CostParams& p, const int32_t* src_index, cu
   dim3 grid(cells_grid_x(p.H, p.W) * nchunks, p.B), block(NT);
   kern<<<grid, block, smem, st>>>(p, chunk, nchunks, src_index);
   return cudaGetLastError();
-}
-
-template <int C, int MODE, bool CW, bool REUSE>
-static cudaError_t launch_cmw(const CostParams& p, const int32_t* src_index, cudaStream_t st) {
-  return src_index ? launch_cmwi<C, MODE, CW, REUSE, true>(p, src_index, st)
-                   : launch_cmwi<C, MODE, CW, REUSE, false>(p, nullptr, st);
-}
-
-template <int C, int MODE, bool REUSE>
-static cudaError_t launch_cm(const CostParams& p, bool cw, const int32_t* src_index, cudaStream_t st) {
-  return cw ? launch_cmw<C, MODE, true, REUSE>(p, src_index, st) : launch_cmw<C, MODE, false, REUSE>(p, src_index, st);
-}
-
-template <int C>
-static cudaError_t launch_c(const CostParams& p, int mode, bool cw, bool reuse, const int32_t* src_index, cudaStream_t st) {
-  if (!reuse) {   // diagnostic variant: only the bench configuration is instantiated
-    if (mode == MAGNET_DEPTH_GAUSS) return launch_cm<C, MAGNET_DEPTH_GAUSS, false>(p, cw, src_index, st);
-    return cudaErrorInvalidValue;
-  }
-  if (mode == MAGNET_DEPTH_VOLUME) return launch_cm<C, MAGNET_DEPTH_VOLUME, true>(p, cw, src_index, st);
-  if (mode == MAGNET_DEPTH_GAUSS) return launch_cm<C, MAGNET_DEPTH_GAUSS, true>(p, cw, src_index, st);
-  return launch_cm<C, MAGNET_DEPTH_PLANES, true>(p, cw, src_index, st);
 }
 
 bool cells_supports(int C, int D, int layout) {
@@ -312,13 +291,15 @@ void cells_launch_info(int B, int H, int W, int D, int* grid, int* block, int* s
 }
 
 cudaError_t launch_cost_cells(const CostParams& p, int mode, int C, bool cw, bool reuse, const int32_t* src_index,
-                              cudaStream_t st) {
-  switch (C) {
-    case 16: return launch_c<16>(p, mode, cw, reuse, src_index, st);
-    case 32: return launch_c<32>(p, mode, cw, reuse, src_index, st);
-    case 64: return launch_c<64>(p, mode, cw, reuse, src_index, st);
-    default: return cudaErrorInvalidValue;
-  }
+                              cudaStream_t st, int* launches) {
+  *launches = 1;
+  return dispatch(
+      [&](auto c, auto m, auto w, auto r, auto idx) -> cudaError_t {
+        // !REUSE is a diagnostic variant: only the bench configuration, GAUSS, is instantiated
+        if constexpr (!r && m != MAGNET_DEPTH_GAUSS) return cudaErrorInvalidValue;
+        else return launch_cells<c, m, w, r, idx>(p, src_index, st);
+      },
+      Choice<int, 16, 32, 64>{C}, DepthMode{mode}, Flag{cw}, Flag{reuse}, Flag{src_index != nullptr});
 }
 
 }  // namespace magnet

@@ -34,10 +34,9 @@
 // The GEOM flag sits on the shared body so that the existing kernels keep their parameter block and their code.
 #include "cells_common.cuh"
 #include "cw_mask.cuh"
+#include "launchers.h"
 
 namespace magnet {
-
-cudaError_t launch_score_grad(const BwdParams& p, cudaStream_t st);   // cost_f_bwd.cu
 
 constexpr int MASK_MMA = 0, MASK_DIRECT = 1;
 
@@ -347,32 +346,11 @@ size_t geom_workspace_bytes(int B, int V, int H, int W) {
   return (size_t)B * V * 12 * nblk * sizeof(float);
 }
 
-template <int CPL>
-static void launch_cpl(const CwBwdParams& p, int C, int mode, int mask, dim3 grid, cudaStream_t st) {
-  if (mode == MAGNET_DEPTH_VOLUME) {
-    if (mask == MASK_MMA) cost_cw_bwd_kernel<CPL, MAGNET_DEPTH_VOLUME, MASK_MMA><<<grid, 128, 0, st>>>(p, C);
-    else cost_cw_bwd_kernel<CPL, MAGNET_DEPTH_VOLUME, MASK_DIRECT><<<grid, 128, 0, st>>>(p, C);
-  } else {
-    if (mask == MASK_MMA) cost_cw_bwd_kernel<CPL, MAGNET_DEPTH_GAUSS, MASK_MMA><<<grid, 128, 0, st>>>(p, C);
-    else cost_cw_bwd_kernel<CPL, MAGNET_DEPTH_GAUSS, MASK_DIRECT><<<grid, 128, 0, st>>>(p, C);
-  }
+// channels per lane of C <= 64 channels (4 lanes per pixel)
+static Choice<int, 1, 2, 4, 8, 16> channels_per_lane(int C) {
+  return {C <= 4 ? 1 : C <= 8 ? 2 : C <= 16 ? 4 : C <= 32 ? 8 : C <= 64 ? 16 : 0};
 }
-
-cudaError_t launch_cost_cw_bwd_mma(const CwBwdParams& p, int mode, int layout, cudaStream_t st);   // cost_f_bwd_mma.cu
-
-template <int CPL>
-static void launch_geom_cpl(const CwBwdParams& p, const GeomOut& go, int C, int mode, int mask, dim3 grid,
-                            cudaStream_t st) {
-  if (mode == MAGNET_DEPTH_PLANES) {
-    cost_geom_bwd_kernel<CPL, MAGNET_DEPTH_PLANES, MASK_MMA><<<grid, 128, 0, st>>>(p, C, go);
-  } else if (mode == MAGNET_DEPTH_VOLUME) {
-    if (mask == MASK_MMA) cost_geom_bwd_kernel<CPL, MAGNET_DEPTH_VOLUME, MASK_MMA><<<grid, 128, 0, st>>>(p, C, go);
-    else cost_geom_bwd_kernel<CPL, MAGNET_DEPTH_VOLUME, MASK_DIRECT><<<grid, 128, 0, st>>>(p, C, go);
-  } else {
-    if (mask == MASK_MMA) cost_geom_bwd_kernel<CPL, MAGNET_DEPTH_GAUSS, MASK_MMA><<<grid, 128, 0, st>>>(p, C, go);
-    else cost_geom_bwd_kernel<CPL, MAGNET_DEPTH_GAUSS, MASK_DIRECT><<<grid, 128, 0, st>>>(p, C, go);
-  }
-}
+using Mask = Choice<int, MASK_MMA, MASK_DIRECT>;
 
 // Camera (and optionally ray and depth) gradients: g_score (softmax or not) into p.g_score, the GEOM walk with
 // per-block partials into `partials`, then the fixed-order reduction into grad_cams (B*V, 12).  Three launches.
@@ -396,13 +374,18 @@ cudaError_t launch_cost_geom_bwd(const CwBwdParams& p, int C, int mode, bool mas
   go.grad_rays = grad_rays;
   const dim3 grid((4 * p.HW + 127) / 128, p.B);
   const int mask = mask_mma || mode == MAGNET_DEPTH_PLANES ? MASK_MMA : MASK_DIRECT;
-  if (C <= 4) launch_geom_cpl<1>(p, go, C, mode, mask, grid, st);
-  else if (C <= 8) launch_geom_cpl<2>(p, go, C, mode, mask, grid, st);
-  else if (C <= 16) launch_geom_cpl<4>(p, go, C, mode, mask, grid, st);
-  else if (C <= 32) launch_geom_cpl<8>(p, go, C, mode, mask, grid, st);
-  else if (C <= 64) launch_geom_cpl<16>(p, go, C, mode, mask, grid, st);
-  else return cudaErrorInvalidValue;
-  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  e = dispatch(
+      [&](auto cpl, auto m, auto k) -> cudaError_t {
+        // the F volume (PLANES) has no mask: its positions are the tensor-core forward's
+        if constexpr (m == MAGNET_DEPTH_PLANES && k != MASK_MMA) {
+          return cudaErrorInvalidValue;
+        } else {
+          cost_geom_bwd_kernel<cpl, m, k><<<grid, 128, 0, st>>>(p, C, go);
+          return cudaGetLastError();
+        }
+      },
+      channels_per_lane(C), DepthMode{mode}, Mask{mask});
+  if (e != cudaSuccess) return e;
   geom_reduce_kernel<<<p.B * p.V, 384, 0, st>>>(partials, p.cams, (int)grid.x, grad_cams);
   *launches = 3;
   return cudaGetLastError();
@@ -437,15 +420,15 @@ cudaError_t launch_cost_cw_bwd(const CwBwdParams& p, const CwBwdParams* split, i
   }
   if (cc.grad_ref == nullptr && cc.grad_src == nullptr && cc.grad_depth == nullptr) return cudaSuccess;
   const dim3 grid((4 * p.HW + 127) / 128, p.B);
-  const int mask = mask_mma ? MASK_MMA : MASK_DIRECT;
-  if (C <= 4) launch_cpl<1>(cc, C, mode, mask, grid, st);
-  else if (C <= 8) launch_cpl<2>(cc, C, mode, mask, grid, st);
-  else if (C <= 16) launch_cpl<4>(cc, C, mode, mask, grid, st);
-  else if (C <= 32) launch_cpl<8>(cc, C, mode, mask, grid, st);
-  else if (C <= 64) launch_cpl<16>(cc, C, mode, mask, grid, st);
-  else return cudaErrorInvalidValue;
-  ++*launches;
-  return cudaGetLastError();
+  e = dispatch(
+      [&](auto cpl, auto m, auto k) {
+        cost_cw_bwd_kernel<cpl, m, k><<<grid, 128, 0, st>>>(cc, C);
+        return cudaGetLastError();
+      },
+      channels_per_lane(C), Choice<int, MAGNET_DEPTH_VOLUME, MAGNET_DEPTH_GAUSS>{mode},
+      Mask{mask_mma ? MASK_MMA : MASK_DIRECT});
+  if (e == cudaSuccess) ++*launches;
+  return e;
 }
 
 }  // namespace magnet

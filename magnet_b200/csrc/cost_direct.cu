@@ -9,6 +9,7 @@
 // cross-check for the tap-sharing kernel, (2) the fallback for channel counts the tap-sharing
 // kernel is not instantiated for.
 #include "common.cuh"
+#include "launchers.h"
 
 namespace magnet {
 
@@ -127,7 +128,7 @@ cost_direct_kernel(const CostParams p, const int depth_mode, const int src_layou
   p.out[((size_t)b * p.D + j) * HW + n] = __fdiv_rn(s, p.vf);      // :120 / float(n_views)
 }
 
-// softmax over the D planes, in place (homography.py:46) — used by the DIRECT variant only.
+// softmax over the D planes, in place (homography.py:46), after any cost-volume forward that asks for it
 __global__ void softmax_planes_kernel(float* __restrict__ vol, int D, int HW) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= HW) return;
@@ -145,24 +146,15 @@ cudaError_t launch_softmax_planes(float* vol, int B, int D, int HW, cudaStream_t
 }
 
 cudaError_t launch_cost_direct(const CostParams& p, int depth_mode, int src_layout, int C, bool cw,
-                               bool softmax, const int32_t* src_index, cudaStream_t st, int* launches) {
-  dim3 grid((p.HW + 127) / 128, p.D, p.B), block(128);
-  if (src_index) {
-    if (cw) cost_direct_kernel<true, true><<<grid, block, 0, st>>>(p, depth_mode, src_layout, C, src_index);
-    else cost_direct_kernel<false, true><<<grid, block, 0, st>>>(p, depth_mode, src_layout, C, src_index);
-  } else {
-    if (cw) cost_direct_kernel<true, false><<<grid, block, 0, st>>>(p, depth_mode, src_layout, C, nullptr);
-    else cost_direct_kernel<false, false><<<grid, block, 0, st>>>(p, depth_mode, src_layout, C, nullptr);
-  }
+                               const int32_t* src_index, cudaStream_t st, int* launches) {
   *launches = 1;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  if (softmax) {
-    softmax_planes_kernel<<<dim3((p.HW + 127) / 128, p.B), 128, 0, st>>>(p.out, p.D, p.HW);
-    *launches = 2;
-    e = cudaGetLastError();
-  }
-  return e;
+  return dispatch(
+      [&](auto w, auto idx) {
+        cost_direct_kernel<w, idx><<<dim3((p.HW + 127) / 128, p.D, p.B), 128, 0, st>>>(p, depth_mode, src_layout, C,
+                                                                                       src_index);
+        return cudaGetLastError();
+      },
+      Flag{cw}, Flag{src_index != nullptr});
 }
 
 }  // namespace magnet

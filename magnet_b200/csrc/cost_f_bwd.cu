@@ -10,6 +10,7 @@
 // (4 gathers + 4 red.add per channel).  One thread per (b, pixel); exact per-plane walk (any plane order).
 // Correctness-first implementation: it is not on the frames/s path (F-Net training only).
 #include "cells_common.cuh"
+#include "launchers.h"
 
 namespace magnet {
 
@@ -116,16 +117,13 @@ cudaError_t launch_score_grad(const BwdParams& p, cudaStream_t st) {
 cudaError_t launch_cost_f_bwd(const BwdParams& p, cudaStream_t st, int* launches) {
   cudaError_t e = launch_score_grad(p, st);
   if (e != cudaSuccess) return e;
-  dim3 grid((p.HW + 127) / 128, p.B);
-  switch (p.C) {
-    case 8: cost_f_bwd_kernel<8><<<grid, 128, 0, st>>>(p); break;
-    case 16: cost_f_bwd_kernel<16><<<grid, 128, 0, st>>>(p); break;
-    case 32: cost_f_bwd_kernel<32><<<grid, 128, 0, st>>>(p); break;
-    case 64: cost_f_bwd_kernel<64><<<grid, 128, 0, st>>>(p); break;
-    default: return cudaErrorInvalidValue;
-  }
   *launches = 2;
-  return cudaGetLastError();
+  return dispatch(
+      [&](auto c) {
+        cost_f_bwd_kernel<c><<<dim3((p.HW + 127) / 128, p.B), 128, 0, st>>>(p);
+        return cudaGetLastError();
+      },
+      Choice<int, 8, 16, 32, 64>{p.C});
 }
 
 }  // namespace magnet

@@ -10,8 +10,8 @@
 //     g_ref[p][:]   += sum_v Gc_v[p][:] S_v[window][:]                       GEMM 1: M = 64 pixels, N = 64 channels, K = cells
 //     g_src_v[cell][:] += sum_p Gc_v[p][cell] R[p][:]                         GEMM 2: M = cells, N = 64 channels, K = 64 pixels
 //
-//   * work item = (batch element, 8x8 tile) on persistent CTAs (two per SM) with a graph-replay-safe work counter (the
-//     scheme of cost_mma.cu, own slots).  The item loops over the valid views and all D planes, so g_ref of the tile has
+//   * work item = (batch element, 8x8 tile) on persistent CTAs (two per SM) with a graph-replay-safe work counter (work
+//     slots of common.cuh, own arrays).  The item loops over the valid views and all D planes, so g_ref of the tile has
 //     one owner and is written once, without atomics.
 //   * window: positions are clamped to [-2, W+1] x [-2, H+1] as in the forward; only (pixel, plane) pairs whose cell
 //     touches the image and whose g is nonzero can contribute, so the bounding box (warp reduction) is taken over those.
@@ -43,11 +43,12 @@
 #include <cuda_fp16.h>
 
 #include <algorithm>
-#include <atomic>
 #include <mutex>
 
 #include "cells_common.cuh"
 #include "cw_mask.cuh"
+#include "launchers.h"
+#include "packed_layout.cuh"
 #include "tma_common.cuh"
 
 namespace magnet {
@@ -70,9 +71,8 @@ constexpr int B_SMEM_TOTAL = B_SMEM_USED + 1024;   // slack for the 1024-byte al
 static_assert(BSEG * BSEG_BYTES == 32768 && 128 * 64 * 4 == 32768 && 64 * 65 * 4 <= 32768, "region WIN");
 static_assert(2 * (B_SMEM_TOTAL + 1024) <= 227 * 1024, "two CTAs per SM");
 
-constexpr int FB_SLOTS = 1024;
-__device__ unsigned g_fbwd_next[FB_SLOTS];
-__device__ unsigned g_fbwd_done[FB_SLOTS];
+__device__ unsigned g_fbwd_next[WORK_SLOTS];
+__device__ unsigned g_fbwd_done[WORK_SLOTS];
 
 // debug dump (MAGNET_MMA_DEBUG builds): header, fp32 Gc, GEMM 2 and both warpgroups' GEMM 1 accumulators of the first
 // processed sub-window of work item 0, handed in through magnet_f_bwd_mma_debug_buffer
@@ -148,7 +148,7 @@ cost_f_bwd_mma_kernel(const __grid_constant__ P p, const __grid_constant__ CUten
     mbar_arrive_expect_tx(bar_ref, 8192u * PLANES);
     tma_load_5d(sbase + BOFF_REF, &tm_ref, bar_ref, 0, tx0, ty0, 0, b);
     misc[8] = 0;
-    misc[9] = (int)gridDim.x + (int)atomicAdd(&g_fbwd_next[slot], 1u);
+    misc[9] = (int)gridDim.x + (int)slot_claim(g_fbwd_next, slot);
   }
   const int px = tx0 + (pp & 7), py = ty0 + (pp >> 3);
   const bool live = px < W && py < H;
@@ -192,8 +192,7 @@ cost_f_bwd_mma_kernel(const __grid_constant__ P p, const __grid_constant__ CUten
     const int vb = v * p.B + b;
     const float4* meta = nullptr;                          // (mu, sigma) table of the source split buffer (CW)
     if constexpr (CW)
-      meta = reinterpret_cast<const float4*>(reinterpret_cast<const unsigned char*>(p.src_feat) + SPLIT16_HEADER +
-                                             (size_t)p.B * V * HW * 128 * PLANES);
+      meta = packed_table(p.src_feat, (size_t)p.B * V, HW, PLANES);
     // cell origin of plane j at my pixel, and whether it can contribute (a tap in the image, g != 0)
     auto cell = [&](const int j, float& g, float& ix, float& iy, int& x0, int& y0) -> bool {
       g = ldg_f(gs + (size_t)j * HW);
@@ -447,23 +446,12 @@ cost_f_bwd_mma_kernel(const __grid_constant__ P p, const __grid_constant__ CUten
   item = nxt;
   }  // work items
 
-  if (tid == 0) {                                          // the last CTA to finish re-arms the work counter
-    __threadfence();
-    if (atomicAdd(&g_fbwd_done[slot], 1u) == gridDim.x - 1) {
-      g_fbwd_next[slot] = 0u;
-      g_fbwd_done[slot] = 0u;
-      __threadfence();
-    }
-  }
+  if (tid == 0) slot_finish(g_fbwd_next, g_fbwd_done, slot);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------
-cudaError_t make_planes_map(CUtensorMap* tm, const void* planes, int N, int H, int W, int box_rows,
-                            int nplanes);                                                              // cost_mma.cu
-cudaError_t launch_score_grad(const BwdParams& p, cudaStream_t st);                                    // cost_f_bwd.cu
-
 #ifdef MAGNET_MMA_DEBUG
 static float* g_fbwd_dbg = nullptr;
 void f_bwd_mma_set_debug_buffer(float* p) { g_fbwd_dbg = p; }
@@ -471,16 +459,7 @@ void f_bwd_mma_set_debug_buffer(float* p) { g_fbwd_dbg = p; }
 
 bool f_bwd_mma_supports(int C, int V) { return C == 64 && V >= 1 && V <= 16; }
 
-void f_bwd_mma_launch_info(int B, int H, int W, int* grid, int* block, int* smem) {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  *grid = std::min(((W + BTW - 1) / BTW) * ((H + BTH - 1) / BTH) * B, 2 * sm_count(dev));
-  *block = BNT;
-  *smem = B_SMEM_TOTAL;
-}
-
-// work-counter tickets shared by every instantiation (they share the slots of g_fbwd_next / g_fbwd_done)
-static std::atomic<unsigned> ticket{0}, graph_ticket{0};
+static SlotTickets fbwd_tickets;
 
 // p.ref_feat / p.src_feat point to the SPLIT16 (PLANES = 2) or HALF16 (PLANES = 1) buffers of the forward (B and V*B
 // images); p.g_score is written
@@ -491,44 +470,38 @@ static cudaError_t launch_bwd_mma(const P& p, cudaStream_t st) {
   int dev = 0;
   cudaError_t e = set_smem_once(kern, flags, B_SMEM_TOTAL, true, &dev);
   if (e != cudaSuccess) return e;
-  const unsigned char* refbuf = reinterpret_cast<const unsigned char*>(p.ref_feat);
-  const unsigned char* srcbuf = reinterpret_cast<const unsigned char*>(p.src_feat);
   CUtensorMap tm_ref, tm_src;
-  if ((e = make_planes_map(&tm_ref, refbuf + SPLIT16_HEADER, p.B, p.H, p.W, 8, PLANES)) != cudaSuccess) return e;
-  if ((e = make_planes_map(&tm_src, srcbuf + SPLIT16_HEADER, p.B * p.V, p.H, p.W, 1, PLANES)) != cudaSuccess) return e;
+  if ((e = make_planes_map(&tm_ref, p.ref_feat, p.B, p.H, p.W, 8, PLANES)) != cudaSuccess) return e;
+  if ((e = make_planes_map(&tm_src, p.src_feat, p.B * p.V, p.H, p.W, 1, PLANES)) != cudaSuccess) return e;
   const int n_items = ((p.W + BTW - 1) / BTW) * ((p.H + BTH - 1) / BTH) * p.B;
-  // work-counter slot: eager launches cycle through the lower half, captured launches own one of the upper half for
-  // the life of their graph (cost_mma.cu)
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  if (cudaStreamIsCapturing(st, &cap) != cudaSuccess) cap = cudaStreamCaptureStatusNone;
-  const int slot = cap == cudaStreamCaptureStatusActive ? FB_SLOTS / 2 + (int)(graph_ticket.fetch_add(1) % (FB_SLOTS / 2))
-                                                        : (int)(ticket.fetch_add(1) % (FB_SLOTS / 2));
   float* dbg = nullptr;
 #ifdef MAGNET_MMA_DEBUG
   dbg = g_fbwd_dbg;
 #endif
-  kern<<<std::min(n_items, 2 * sm_count(dev)), BNT, B_SMEM_TOTAL, st>>>(p, tm_ref, tm_src, n_items, slot, dbg);
+  kern<<<std::min(n_items, 2 * sm_count(dev)), BNT, B_SMEM_TOTAL, st>>>(p, tm_ref, tm_src, n_items,
+                                                                        work_slot(fbwd_tickets, st), dbg);
   return cudaGetLastError();
 }
 
 // layout: MAGNET_SRC_SPLIT16 or MAGNET_SRC_HALF16, the buffers' layout
+// the planes of a buffer of `layout`: 2 for SPLIT16 (hi / lo), 1 for HALF16
+static Choice<int, 1, 2> planes_of(int layout) { return {layout == MAGNET_SRC_HALF16 ? 1 : 2}; }
+
+// F volume: two instantiations (PLANES)
 cudaError_t launch_cost_f_bwd_mma(const BwdParams& p, int layout, cudaStream_t st, int* launches) {
   cudaError_t e = launch_score_grad(p, st);
   if (e != cudaSuccess) return e;
   *launches = 2;
-  if (layout == MAGNET_SRC_HALF16) return launch_bwd_mma<BwdParams, MAGNET_DEPTH_PLANES, false, 1>(p, st);
-  return launch_bwd_mma<BwdParams, MAGNET_DEPTH_PLANES, false, 2>(p, st);
+  return dispatch([&](auto planes) { return launch_bwd_mma<BwdParams, MAGNET_DEPTH_PLANES, false, planes>(p, st); },
+                  planes_of(layout));
 }
 
 // CW volume, feature gradients on the tensor cores: p.ref_feat / p.src_feat are the forward's split buffers (layout
-// SPLIT16 or HALF16), p.g_score already holds grad_out / V (cost_cw_bwd.cu)
+// SPLIT16 or HALF16), p.g_score already holds grad_out / V (cost_cw_bwd.cu).  Four instantiations: the per-pixel
+// depth modes VOLUME and GAUSS (mode), by PLANES.
 cudaError_t launch_cost_cw_bwd_mma(const CwBwdParams& p, int mode, int layout, cudaStream_t st) {
-  if (layout == MAGNET_SRC_HALF16) {
-    if (mode == MAGNET_DEPTH_VOLUME) return launch_bwd_mma<CwBwdParams, MAGNET_DEPTH_VOLUME, true, 1>(p, st);
-    return launch_bwd_mma<CwBwdParams, MAGNET_DEPTH_GAUSS, true, 1>(p, st);
-  }
-  if (mode == MAGNET_DEPTH_VOLUME) return launch_bwd_mma<CwBwdParams, MAGNET_DEPTH_VOLUME, true, 2>(p, st);
-  return launch_bwd_mma<CwBwdParams, MAGNET_DEPTH_GAUSS, true, 2>(p, st);
+  return dispatch([&](auto m, auto planes) { return launch_bwd_mma<CwBwdParams, m, true, planes>(p, st); },
+                  Choice<int, MAGNET_DEPTH_VOLUME, MAGNET_DEPTH_GAUSS>{mode}, planes_of(layout));
 }
 
 }  // namespace magnet

@@ -38,6 +38,7 @@
 #include <mutex>
 
 #include "common.cuh"
+#include "launchers.h"
 #include "tma_common.cuh"
 
 namespace magnet {
@@ -612,22 +613,6 @@ cudaError_t launch_repack_pixc(const float* src, const float* gmm, float* dst, i
 // ---------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn encode_tiled_fn() {   // shared with cost_mma.cu
-  static EncodeTiledFn fn = [] {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-      f = nullptr;
-    return reinterpret_cast<EncodeTiledFn>(f);
-  }();
-  return fn;
-}
-
 // rank-4 map over the PIXC buffer: (C+4 floats, W, H, N), box = one row of 8 pixels, zero fill outside
 static cudaError_t make_pixc_map(CUtensorMap* tm, const float* src, int N, int C, int H, int W) {
   EncodeTiledFn enc = encode_tiled_fn();
@@ -644,7 +629,7 @@ static cudaError_t make_pixc_map(CUtensorMap* tm, const float* src, int N, int C
 }
 
 template <int C, int MODE, bool CW, bool IDX>
-static cudaError_t launch_tma_cmwi(const CostParams& p, const int32_t* src_index, int n_src, cudaStream_t st) {
+static cudaError_t launch_tma(const CostParams& p, const int32_t* src_index, int n_src, cudaStream_t st) {
   static std::once_flag flags[64];
   auto kern = cost_tma_kernel<C, MODE, CW, IDX>;
   cudaError_t e = set_smem_once(kern, flags, TMA_SMEM_TOTAL, true);
@@ -664,24 +649,6 @@ static cudaError_t launch_tma_cmwi(const CostParams& p, const int32_t* src_index
   return cudaGetLastError();
 }
 
-template <int C, int MODE, bool CW>
-static cudaError_t launch_tma_cmw(const CostParams& p, const int32_t* src_index, int n_src, cudaStream_t st) {
-  return src_index ? launch_tma_cmwi<C, MODE, CW, true>(p, src_index, n_src, st)
-                   : launch_tma_cmwi<C, MODE, CW, false>(p, nullptr, 0, st);
-}
-
-template <int C>
-static cudaError_t launch_tma_c(const CostParams& p, int mode, bool cw, const int32_t* si, int n_src, cudaStream_t st) {
-  if (cw) {
-    if (mode == MAGNET_DEPTH_VOLUME) return launch_tma_cmw<C, MAGNET_DEPTH_VOLUME, true>(p, si, n_src, st);
-    if (mode == MAGNET_DEPTH_GAUSS) return launch_tma_cmw<C, MAGNET_DEPTH_GAUSS, true>(p, si, n_src, st);
-    return launch_tma_cmw<C, MAGNET_DEPTH_PLANES, true>(p, si, n_src, st);
-  }
-  if (mode == MAGNET_DEPTH_VOLUME) return launch_tma_cmw<C, MAGNET_DEPTH_VOLUME, false>(p, si, n_src, st);
-  if (mode == MAGNET_DEPTH_GAUSS) return launch_tma_cmw<C, MAGNET_DEPTH_GAUSS, false>(p, si, n_src, st);
-  return launch_tma_cmw<C, MAGNET_DEPTH_PLANES, false>(p, si, n_src, st);
-}
-
 bool tma_supports(int C, int D, int V, int layout) {
   return (C == 16 || C == 32 || C == 64) && layout == MAGNET_SRC_PIXC && D >= 1 && V <= TMAXV;
 }
@@ -694,13 +661,10 @@ void tma_launch_info(int B, int H, int W, int D, int* grid, int* block, int* sme
 
 // src_index: NULL (view-major source images, V*B of them) or the (B, V) frame table over n_src images
 cudaError_t launch_cost_tma(const CostParams& p, int mode, int C, bool cw, const int32_t* src_index, int n_src,
-                            cudaStream_t st) {
-  switch (C) {
-    case 16: return launch_tma_c<16>(p, mode, cw, src_index, n_src, st);
-    case 32: return launch_tma_c<32>(p, mode, cw, src_index, n_src, st);
-    case 64: return launch_tma_c<64>(p, mode, cw, src_index, n_src, st);
-    default: return cudaErrorInvalidValue;
-  }
+                            cudaStream_t st, int* launches) {
+  *launches = 1;
+  return dispatch([&](auto c, auto m, auto w, auto idx) { return launch_tma<c, m, w, idx>(p, src_index, n_src, st); },
+                  Choice<int, 16, 32, 64>{C}, DepthMode{mode}, Flag{cw}, Flag{src_index != nullptr});
 }
 
 }  // namespace magnet

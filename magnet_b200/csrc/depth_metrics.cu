@@ -11,6 +11,7 @@
 // Build note: this file relies on IEEE float32 division and full-precision logf / log10f; the library is compiled
 // without --use_fast_math, and the explicit __f*_rn intrinsics keep nvcc from contracting terms into FMAs.
 #include "common.cuh"
+#include "launchers.h"
 #include "upsample_common.cuh"
 
 namespace magnet {

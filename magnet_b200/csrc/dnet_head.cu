@@ -7,13 +7,9 @@
 #include <mutex>
 
 #include "head_common.cuh"
+#include "launchers.h"
 
 namespace magnet {
-
-size_t dnet_mask_weights_bytes();                                                                   // mask_head.cu
-void add_dnet_mask_pack(HeadPack& p, const float* w1, const float* b1, const float* w3, const float* b3, size_t base);
-cudaError_t launch_dnet_upsample(int B, int H, int W, const float* pre_m, const void* weights, const float* raw,
-                                 float* out, cudaStream_t st);
 
 namespace {
 constexpr int NT = 256;

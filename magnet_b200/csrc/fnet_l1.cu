@@ -5,6 +5,7 @@
 //   forward: one partial sum of |pred - gt| per CTA of 128 pixels (the caller adds them and divides by the count)
 //   backward: dL/dscore_j = prob_j (d_j - pred) sign(pred - gt) mask scale, sign(0) = 0 (torch's abs backward)
 #include "common.cuh"
+#include "launchers.h"
 #include "soft_argmin.cuh"
 
 namespace magnet {

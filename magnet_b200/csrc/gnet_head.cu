@@ -12,10 +12,9 @@
 
 #include "gaussian_common.cuh"
 #include "head_common.cuh"
+#include "launchers.h"
 
 namespace magnet {
-
-cudaError_t launch_absmax_f32(const float* x, size_t n, unsigned* out, cudaStream_t st);  // cost_mma.cu
 
 namespace {
 constexpr int TY = 8, TX = 16;                 // pixel tile of a CTA: warp w owns row w (16 pixels = the MMA's M)

@@ -242,5 +242,7 @@ struct HeadPack {
   }
 };
 cudaError_t launch_head_pack(const HeadPack& p, void* dst, cudaStream_t st);
+// the mask-head part of D-Net's pack, at byte `base` of it
+void add_dnet_mask_pack(HeadPack& p, const float* w1, const float* b1, const float* w3, const float* b3, size_t base);
 
 }  // namespace magnet

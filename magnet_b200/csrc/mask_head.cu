@@ -10,6 +10,7 @@
 #include <mutex>
 
 #include "head_common.cuh"
+#include "launchers.h"
 #include "upsample_common.cuh"
 
 namespace magnet {
@@ -258,9 +259,6 @@ cudaError_t launch_dnet_upsample(int B, int H, int W, const float* pre_m, const 
 // The mask head, the upsampling and the Gaussian NLL of MagnetLoss (utils/losses.py:34-50) in one forward kernel that
 // also forms the loss's gradient with respect to the 144 logits and the predictions while they are on chip; a
 // tensor-core backward chain through the three 1x1 layers; the weight gradients on the G-Net head's fixed-order GEMMs.
-size_t head_wgrad_partial_floats(int B, int H, int W, int Ma, int Nw);                          // gnet_head.cu
-cudaError_t launch_head_wgrad(int B, int H, int W, int Ma, const float* a, int Nw, const float* b, float* part,
-                              float* out_w, float* out_b, cudaStream_t st);
 
 namespace {
 // d_logits is stored as channels 0..127 (B,128,H,W) followed by channels 128..143 (B,16,H,W): the weight-gradient GEMM

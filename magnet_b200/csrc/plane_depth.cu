@@ -4,6 +4,7 @@
 //     fused in (soft_argmin.cuh, the same code as the training loss), the probability volume is never written.
 //   probabilities form: the output of est_costvolume_F / MAGNET_F.forward; pred = sum_j p_j d_j in plane order.
 #include "common.cuh"
+#include "launchers.h"
 #include "soft_argmin.cuh"
 
 namespace magnet {

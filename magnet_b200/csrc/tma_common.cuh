@@ -44,14 +44,6 @@ __device__ __forceinline__ void mbar_wait_or_trap(uint32_t bar, uint32_t parity)
   __trap();
 }
 
-// header of a MAGNET_SRC_SPLIT16 buffer (256 bytes)
-struct Split16Header {
-  float scale;       // s = 2^k
-  float inv_scale;   // 2^-k
-  unsigned absmax;   // bits of max |x|
-};
-constexpr size_t SPLIT16_HEADER = 256;
-
 // TMA tiled load of one box of a rank-4 tensor map into shared memory (UTMALDG); out-of-range elements are
 // zero-filled by the copy engine, coordinates are signed.
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tmap, uint32_t bar, int c0, int c1, int c2,
