@@ -11,7 +11,10 @@ upsampled predictions (utils/losses.py:34-50), AdamW, gradient clipping at 1.0, 
 all-reduce per step (magnet_b200.dist.FlatGradAllReduce) instead of DistributedDataParallel.  The frozen
 D-Net / F-Net are replaced by fixed random tensors of their output shapes (they need torch.hub + checkpoints in
 the reference and are out of scope): features (B,64,h,w) / (V*B,64,h,w), Gaussians, x_d3 (B,256,h,w).
-The matching loop runs on the H100 kernels (sampler fused, update kernel with backward)."""
+The matching loop runs on the H100 kernels (sampler fused, update kernel with backward).
+
+--compile default / reduce-overhead compiles the function that returns the loss (torch.compile, or CUDA-graph trees);
+its backward is compiled with it and runs at loss.backward().  The all-reduce, clipping and AdamW step stay eager."""
 import argparse, json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -48,6 +51,8 @@ def main():
                     help="run the mask head after its first convolution, the upsampling and the loss as one fused "
                          "tensor-core op with its backward (MagnetHead.train_loss with fused_upsample, DESIGN §3.13) "
                          "instead of the cuDNN mask head and the fused upsample+NLL kernels")
+    ap.add_argument("--compile", choices=("none", "default", "reduce-overhead"), default="none",
+                    help="compile the loss function (the training kernels are custom ops with registered backwards)")
     args = ap.parse_args()
     if args.fused_mask and args.unfused_loss:
         raise SystemExit("--fused-mask and --unfused-loss exclude each other")
@@ -73,6 +78,25 @@ def main():
     reducer.broadcast_parameters(0)
     opt = torch.optim.AdamW(head.parameters(), lr=3.57e-4, weight_decay=1e-2)
 
+    def loss_fn(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, poses, is_valid, intM, rays, gt, mask):
+        cam = {"intM": intM, "unit_ray_array_2D": rays}
+        if args.unfused_loss:
+            return gaussian_nll(head(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, poses, is_valid, cam), gt, mask)
+        if args.fused_mask:
+            return head.train_loss(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, poses, is_valid, cam, gt, mask)
+        preds_q, up_mask = head.forward_quarter(ref_feat, nghbr_feat, ref_gmms, nghbr_gmms, x_d3, poses, is_valid, cam)
+        return head.loss(preds_q, up_mask, gt, mask)         # f-2: no (B,2,4H,4W) tensors, fwd or bwd
+
+    if args.compile != "none" and args.unfused_loss:
+        raise SystemExit("--compile needs a loss without boolean indexing (drop --unfused-loss)")
+    step_loss = loss_fn if args.compile == "none" else torch.compile(loss_fn, mode=None if args.compile == "default"
+                                                                     else args.compile)
+    # the eager step takes is_valid and cam_intrins on the host, as the reference's loaders give them; a compiled one
+    # takes them on the device (CUDA-graph trees do not capture a graph with host inputs)
+    host = (inp.is_valid, inp.cam_intrins["intM"], inp.cam_intrins["unit_ray_array_2D"])
+    step_args = (inp.ref_feat, inp.nghbr_feat, inp.ref_gmms, inp.nghbr_gmms, x_d3, inp.nghbr_poses,
+                 *(host if args.compile == "none" else (t.to(dev) for t in host)), gt, mask)
+
     WARM = 5                                                               # cuDNN autotuning, NCCL lazy init, allocator growth
     losses, t0, marks = [], None, []
     for step in range(args.steps + WARM):
@@ -80,18 +104,8 @@ def main():
             torch.cuda.synchronize(); md.barrier(); t0 = time.perf_counter()
         if step >= WARM:
             ev = torch.cuda.Event(enable_timing=True); ev.record(); marks.append(ev)
-        if args.unfused_loss:
-            preds = head(inp.ref_feat, inp.nghbr_feat, inp.ref_gmms, inp.nghbr_gmms, x_d3, inp.nghbr_poses,
-                         inp.is_valid, inp.cam_intrins)
-            loss = gaussian_nll(preds, gt, mask)
-        elif args.fused_mask:
-            loss = head.train_loss(inp.ref_feat, inp.nghbr_feat, inp.ref_gmms, inp.nghbr_gmms, x_d3, inp.nghbr_poses,
-                                   inp.is_valid, inp.cam_intrins, gt, mask)
-        else:                                                              # f-2: no (B,2,4H,4W) tensors, fwd or bwd
-            preds_q, up_mask = head.forward_quarter(inp.ref_feat, inp.nghbr_feat, inp.ref_gmms, inp.nghbr_gmms, x_d3,
-                                                    inp.nghbr_poses, inp.is_valid, inp.cam_intrins)
-            loss = head.loss(preds_q, up_mask, gt, mask)
         opt.zero_grad(set_to_none=True)
+        loss = step_loss(*step_args)
         loss.backward()
         reducer()                                                          # one 3 MB all-reduce
         torch.nn.utils.clip_grad_norm_(head.parameters(), 1.0)
@@ -106,7 +120,7 @@ def main():
                           "head_path": "fused G-Net kernels" if args.fused_head else "cuDNN module chain",
                           "loss_path": "unfused (torch NLL on upsampled predictions)" if args.unfused_loss else
                                        "fused mask head + upsample + NLL kernel" if args.fused_mask else "fused upsample+NLL kernels",
-                          "ms_per_step": 1e3 * dt / args.steps, "frames_per_s": gb * args.steps / dt,
+                          "compile": args.compile, "ms_per_step": 1e3 * dt / args.steps, "frames_per_s": gb * args.steps / dt,
                           "rank0_step_ms_median": per_step[len(per_step) // 2], "rank0_step_ms_max": per_step[-1],
                           "loss_first": losses[0], "loss_last": losses[-1], "trainable_params": reducer.bucket.numel()}))
     md.shutdown()

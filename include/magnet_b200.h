@@ -472,6 +472,9 @@ int magnet_mask_train_partials(int32_t B, int32_t H, int32_t W);
 int magnet_mask_pack_train_weights_f32(const float* w1, const float* b1, const float* w2, const float* b2,
                                        const float* w3, const float* b3, void* packed, void* stream);
 int magnet_mask_train_fwd_f32(const magnet_mask_train_args* args, void* stream);
+/* magnet_mask_train_fwd_f32 with the P prediction scales read from the DEVICE array pred_scale (args->pred_scale is not
+ * read) when the kernel runs, so that a captured CUDA graph takes them from memory.  Same arithmetic otherwise. */
+int magnet_mask_train_fwd_dev_f32(const magnet_mask_train_args* args, const float* pred_scale, void* stream);
 int magnet_mask_bwd_f32(const magnet_mask_train_args* args, void* stream);
 
 /*
@@ -557,6 +560,10 @@ int magnet_upsample_nll_fwd_f32(const float* depth, const float* up_mask, const 
 int magnet_upsample_nll_bwd_f32(const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
                                 float scale, int32_t B, int32_t H, int32_t W, int32_t k, float* grad_depth,
                                 float* grad_mask, void* stream);
+/* magnet_upsample_nll_bwd_f32 with the scale read from the DEVICE float *scale when the kernel runs (for CUDA graphs). */
+int magnet_upsample_nll_bwd_dev_f32(const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
+                                    const float* scale, int32_t B, int32_t H, int32_t W, int32_t k, float* grad_depth,
+                                    float* grad_mask, void* stream);
 
 /*
  * F-Net training loss, fused — replaces train_FNet.py:96-108 on the 1/V-averaged scores of the plane-sweep volume

@@ -147,6 +147,7 @@ SIGNATURES = {
     "magnet_upsample_nll_partials": (_ST, [_I32] * 4),
     "magnet_upsample_nll_fwd_f32": (_ST, [_P] * 4 + [_I32] * 4 + [_P, _P]),
     "magnet_upsample_nll_bwd_f32": (_ST, [_P] * 4 + [_F32] + [_I32] * 4 + [_P, _P, _P]),
+    "magnet_upsample_nll_bwd_dev_f32": (_ST, [_P] * 5 + [_I32] * 4 + [_P, _P, _P]),
     "magnet_fnet_l1_partials": (_ST, [_I32] * 3),
     "magnet_fnet_l1_fwd_f32": (_ST, [_P] * 4 + [_I32] * 4 + [_P, _P]),
     "magnet_fnet_l1_bwd_f32": (_ST, [_P] * 4 + [_F32, _P] + [_I32] * 4 + [_P, _P]),
@@ -174,6 +175,7 @@ SIGNATURES = {
     "magnet_mask_train_partials": (_ST, [_I32] * 3),
     "magnet_mask_pack_train_weights_f32": (_ST, [_P] * 8),
     "magnet_mask_train_fwd_f32": (_ST, [C.POINTER(MaskTrainArgs), _P]),
+    "magnet_mask_train_fwd_dev_f32": (_ST, [C.POINTER(MaskTrainArgs), _P, _P]),
     "magnet_mask_bwd_f32": (_ST, [C.POINTER(MaskTrainArgs), _P]),
     "magnet_dnet_weights_bytes": (_SZ, [_I32]),
     "magnet_dnet_pack_weights_f32": (_ST, [_P] * 8 + [_I32, _P, _P]),

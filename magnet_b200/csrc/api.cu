@@ -569,8 +569,17 @@ int magnet_upsample_nll_bwd_f32(const float* depth, const float* up_mask, const 
                                 float* grad_mask, void* stream) {
   if (!depth || !up_mask || !gt || !gt_mask || !grad_depth || !grad_mask) return MAGNET_ERR_NULL;
   if (B <= 0 || H <= 0 || W <= 0 || k <= 0 || B > 65535 || H * k > 65535) return MAGNET_ERR_SHAPE;
-  return finish(magnet::launch_upsample_nll_bwd(depth, up_mask, gt, gt_mask, scale, B, H, W, k, grad_depth, grad_mask,
-                                                (cudaStream_t)stream), 1);
+  return finish(magnet::launch_upsample_nll_bwd(depth, up_mask, gt, gt_mask, scale, nullptr, B, H, W, k, grad_depth,
+                                                grad_mask, (cudaStream_t)stream), 1);
+}
+
+int magnet_upsample_nll_bwd_dev_f32(const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
+                                    const float* scale, int32_t B, int32_t H, int32_t W, int32_t k, float* grad_depth,
+                                    float* grad_mask, void* stream) {
+  if (!depth || !up_mask || !gt || !gt_mask || !scale || !grad_depth || !grad_mask) return MAGNET_ERR_NULL;
+  if (B <= 0 || H <= 0 || W <= 0 || k <= 0 || B > 65535 || H * k > 65535) return MAGNET_ERR_SHAPE;
+  return finish(magnet::launch_upsample_nll_bwd(depth, up_mask, gt, gt_mask, 0.0f, scale, B, H, W, k, grad_depth,
+                                                grad_mask, (cudaStream_t)stream), 1);
 }
 
 int magnet_fnet_l1_partials(int32_t B, int32_t H, int32_t W) {
@@ -722,20 +731,29 @@ int magnet_mask_pack_train_weights_f32(const float* w1, const float* b1, const f
   return finish(magnet::launch_mask_pack_train(w1, b1, w2, b2, w3, b3, packed, (cudaStream_t)stream), 2);
 }
 
-int magnet_mask_train_fwd_f32(const magnet_mask_train_args* a, void* stream) {
+// the fused mask-loss forward with its prediction scales from `scale` (host or device, `on_device`)
+static int mask_train_fwd(const magnet_mask_train_args* a, const float* scale, bool on_device, void* stream) {
   const int st = validate_mask_train(a);
   if (st != MAGNET_OK) return st;
-  if (!a->pre0 || !a->pred || !a->gt || !a->gt_mask || !a->pred_scale || !a->partial) return MAGNET_ERR_NULL;
+  if (!a->pre0 || !a->pred || !a->gt || !a->gt_mask || !scale || !a->partial) return MAGNET_ERR_NULL;
   if (preds_null(a->pred, a->P)) return MAGNET_ERR_NULL;
   if (misaligned16(a->pre0)) return MAGNET_ERR_ALIGN;
   for (int p = 0; p < a->P; ++p)
     if (misaligned16(a->pred[p])) return MAGNET_ERR_ALIGN;
   int launches = 0;
   const cudaError_t e = magnet::launch_mask_train_fwd(a->P, a->B, a->H, a->W, a->pre0, a->packed_weights, a->pred,
-                                                      a->gt, a->gt_mask, a->pred_scale, a->save_maps != 0,
+                                                      a->gt, a->gt_mask, scale, on_device, a->save_maps != 0,
                                                       a->pred_grad != 0, a->partial, a->saved, (cudaStream_t)stream,
                                                       &launches);
   return finish(e, launches);
+}
+
+int magnet_mask_train_fwd_f32(const magnet_mask_train_args* a, void* stream) {
+  return mask_train_fwd(a, a ? a->pred_scale : nullptr, false, stream);
+}
+
+int magnet_mask_train_fwd_dev_f32(const magnet_mask_train_args* a, const float* pred_scale, void* stream) {
+  return mask_train_fwd(a, pred_scale, true, stream);
 }
 
 int magnet_mask_bwd_f32(const magnet_mask_train_args* a, void* stream) {

@@ -284,10 +284,13 @@ __global__ void __launch_bounds__(128) upsample_nll_fwd_kernel(const float* __re
     partial[(b * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = (red[0] + red[1]) + (red[2] + red[3]);
 }
 
-// scale = upstream gradient * iteration weight / number of supervised pixels
+// scale = upstream gradient * iteration weight / number of supervised pixels: the argument, or with DEV_SCALE the
+// device float *scale_dev (read at run time, so a captured graph takes it from memory)
+template <bool DEV_SCALE>
 __global__ void __launch_bounds__(128) upsample_nll_bwd_kernel(const float* __restrict__ depth, const float* __restrict__ mask,
                                                                 const float* __restrict__ gt, const uint8_t* __restrict__ gtm,
-                                                                float scale, int H, int W, int k, float* __restrict__ gdepth,
+                                                                float scale_arg, const float* __restrict__ scale_dev, int H,
+                                                                int W, int k, float* __restrict__ gdepth,
                                                                 float* __restrict__ gmask) {
   const int X = blockIdx.x * blockDim.x + threadIdx.x, Y = blockIdx.y;
   const size_t b = blockIdx.z;
@@ -301,6 +304,7 @@ __global__ void __launch_bounds__(128) upsample_nll_bwd_kernel(const float* __re
     for (int i = 0; i < 9; ++i) gmask[moff + (size_t)i * k * k * HW] = 0.0f;
     return;
   }
+  const float scale = DEV_SCALE ? __ldg(scale_dev) : scale_arg;
   float w[9], mu, sg;
   upsampled_gaussian(depth, mask, b, H, W, k, x, y, kx, ky, w, mu, sg);
   const float var = fmaxf(sg * sg, 1e-10f), d = mu - gt[o];
@@ -334,9 +338,13 @@ cudaError_t launch_upsample_nll_fwd(const float* depth, const float* mask, const
 }
 
 cudaError_t launch_upsample_nll_bwd(const float* depth, const float* mask, const float* gt, const uint8_t* gtm, float scale,
-                                    int B, int H, int W, int k, float* gdepth, float* gmask, cudaStream_t st) {
+                                    const float* scale_dev, int B, int H, int W, int k, float* gdepth, float* gmask,
+                                    cudaStream_t st) {
   dim3 grid((W * k + 127) / 128, H * k, B);
-  upsample_nll_bwd_kernel<<<grid, 128, 0, st>>>(depth, mask, gt, gtm, scale, H, W, k, gdepth, gmask);
+  if (scale_dev)
+    upsample_nll_bwd_kernel<true><<<grid, 128, 0, st>>>(depth, mask, gt, gtm, 0.0f, scale_dev, H, W, k, gdepth, gmask);
+  else
+    upsample_nll_bwd_kernel<false><<<grid, 128, 0, st>>>(depth, mask, gt, gtm, scale, nullptr, H, W, k, gdepth, gmask);
   return cudaGetLastError();
 }
 

@@ -95,8 +95,10 @@ cudaError_t launch_upsample_bwd(const float* gout, const float* depth, const flo
                                 int k, float* gdepth, float* gmask, cudaStream_t st);
 cudaError_t launch_upsample_nll_fwd(const float* depth, const float* mask, const float* gt, const uint8_t* gtm, int B,
                                     int H, int W, int k, float* partial, cudaStream_t st);
+// scale_dev: a DEVICE float read in place of `scale` when not NULL
 cudaError_t launch_upsample_nll_bwd(const float* depth, const float* mask, const float* gt, const uint8_t* gtm, float scale,
-                                    int B, int H, int W, int k, float* gdepth, float* gmask, cudaStream_t st);
+                                    const float* scale_dev, int B, int H, int W, int k, float* gdepth, float* gmask,
+                                    cudaStream_t st);
 
 // ---- F-Net loss, plane depth, depth metrics ---------------------------------------------------------------------------
 int fnet_l1_partials(int B, int HW);
@@ -156,8 +158,8 @@ cudaError_t launch_mask_pack_train(const float* w1, const float* b1, const float
                                    const float* b3, void* dst, cudaStream_t st);
 cudaError_t launch_mask_train_fwd(int P, int B, int H, int W, const float* pre0, const void* weights,
                                   const float* const* pred, const float* gt, const unsigned char* gtm,
-                                  const float* scale, bool save_maps, bool pred_grad, float* partial, float* saved,
-                                  cudaStream_t st, int* launches);
+                                  const float* scale, bool scale_on_device, bool save_maps, bool pred_grad,
+                                  float* partial, float* saved, cudaStream_t st, int* launches);
 cudaError_t launch_mask_bwd(int P, int B, int H, int W, const void* weights, const float* saved, const float* gscale,
                             void* workspace, float* grad_pre0, float* gw1, float* gb1, float* gw2, float* gb2,
                             float* gw3, float* gb3, float* const* grad_pred, cudaStream_t st, int* launches);

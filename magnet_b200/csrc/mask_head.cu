@@ -286,12 +286,16 @@ struct MaskTrainParams {
   float* __restrict__ saved;          // h0, h1, h2 (B,128,H,W) each, or NULL
   float* __restrict__ dlog;           // d_logits (B,128,H,W) + (B,16,H,W), or NULL
   float* __restrict__ gpred;          // P x (B,2,H,W) prediction gradients, accumulated; or NULL
+  const float* __restrict__ scale_dev;  // DEV_SCALE: P device floats read in place of `scale`
 };
 
 // The inference kernel's tiles, layers and logits (bit for bit), then per full-resolution sub-pixel where gt_mask is
 // set: the convex upsampling of every prediction, its NLL and the NLL's derivative (upsample_nll_fwd / bwd_kernel's
 // expressions), the logits' gradient d = sum_p w (t_p - <w, t_p>) in prediction order, and the gradient into each
 // prediction's 3x3 neighbourhood, gathered per tile in shared memory and added to global memory once per tile.
+// DEV_SCALE: the prediction scales are read from device memory (p.scale_dev) at run time, so that a captured graph takes
+// them from memory; otherwise they are the kernel parameters p.scale.
+template <bool DEV_SCALE>
 __global__ void __launch_bounds__(NT, 1) mask_train_fwd_kernel(const MaskTrainParams p) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ float red[NT / 32][MAX_PRED];
@@ -416,7 +420,7 @@ __global__ void __launch_bounds__(NT, 1) mask_train_fwd_kernel(const MaskTrainPa
               else convex_combine(w, tap, mu, sg);
               const float var = fmaxf(sg * sg, 1e-10f), d = mu - gt;
               nll[pp] += (d * d) / (2.0f * var) + 0.5f * logf(var);
-              const float s = p.scale[pp];
+              const float s = DEV_SCALE ? __ldg(p.scale_dev + pp) : p.scale[pp];
               const float g_mu = s * d / var;
               // var[var < 1e-10] = 1e-10 (losses.py:45) cuts the gradient to sigma where it clamps
               const float g_sg = (sg * sg < 1e-10f) ? 0.0f : s * (1.0f / sg - (d * d) / (var * sg));
@@ -598,11 +602,12 @@ cudaError_t launch_mask_pack_train(const float* w1, const float* b1, const float
 
 cudaError_t launch_mask_train_fwd(int P, int B, int H, int W, const float* pre0, const void* weights,
                                   const float* const* pred, const float* gt, const unsigned char* gtm,
-                                  const float* scale, bool save_maps, bool pred_grad, float* partial, float* saved,
-                                  cudaStream_t st, int* launches) {
-  static std::once_flag flags[64];
+                                  const float* scale, bool scale_on_device, bool save_maps, bool pred_grad,
+                                  float* partial, float* saved, cudaStream_t st, int* launches) {
+  static std::once_flag flags[2][64];
   int dev = 0;
-  cudaError_t e = set_smem_once(mask_train_fwd_kernel, flags, (int)smem_train(MAX_PRED), false, &dev);
+  const auto kern = scale_on_device ? mask_train_fwd_kernel<true> : mask_train_fwd_kernel<false>;
+  cudaError_t e = set_smem_once(kern, flags[scale_on_device], (int)smem_train(MAX_PRED), false, &dev);
   if (e != cudaSuccess) return e;
   const size_t map = (size_t)B * H * W;
   MaskTrainParams p;
@@ -615,8 +620,9 @@ cudaError_t launch_mask_train_fwd(int P, int B, int H, int W, const float* pre0,
   p.gt = gt; p.gtm = gtm;
   for (int i = 0; i < MAX_PRED; ++i) {
     p.pred[i] = i < P ? pred[i] : nullptr;
-    p.scale[i] = i < P ? scale[i] : 0.0f;
+    p.scale[i] = i < P && !scale_on_device ? scale[i] : 0.0f;
   }
+  p.scale_dev = scale_on_device ? scale : nullptr;
   p.partial = partial;
   // saved: P x (B,2,H,W) prediction gradients, then h0, h1, h2 and d_logits (mask_saved_floats)
   float* maps = saved + (size_t)2 * P * map;
@@ -628,7 +634,7 @@ cudaError_t launch_mask_train_fwd(int P, int B, int H, int W, const float* pre0,
     if ((e = cudaMemsetAsync(p.gpred, 0, (size_t)P * 2 * map * 4, st)) != cudaSuccess) return e;
     ++*launches;
   }
-  mask_train_fwd_kernel<<<std::min(p.ntiles, sm_count(dev)), NT, smem_train(P), st>>>(p);   // persistent
+  kern<<<std::min(p.ntiles, sm_count(dev)), NT, smem_train(P), st>>>(p);   // persistent
   return cudaGetLastError();
 }
 

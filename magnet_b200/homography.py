@@ -456,6 +456,12 @@ def _f_volume(d_center, ref_feat, nghbr_feat, R, t, is_valid, cam_intrins, varia
     cams = _camera_table(cam_intrins, R, t, is_valid, device)
     if torch.compiler.is_compiling() and not wants_cw_grad(ref_feat, nghbr_feat, *cam_in):
         return _f_forward(ref_feat, nghbr_feat, planes, rays_d, cams, V, variant, softmax)[0]   # traced inference
+    if torch.compiler.is_compiling() and not cam_in:       # traced training: the op with a backward
+        layout, fv = route(int(ref_feat.shape[1]), V, len(planes), variant, _lib.DEPTH_PLANES, ref_feat.dtype,
+                           nghbr_feat.dtype)
+        src, ref_split = _packed_source(layout, nghbr_feat, None, ref_feat)
+        return ops._op("cost_volume_f")(ref_feat, nghbr_feat, src, ref_split, rays_d, cams, V, layout, fv, planes,
+                                        softmax, tc_bwd)
     return _CostVolumeF.apply(ref_feat, nghbr_feat, planes, rays_d, cams, V, variant, softmax, tc_bwd, *cam_in)
 
 

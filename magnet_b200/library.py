@@ -7,7 +7,11 @@ in ``ops.py``, in one place.  The ``ops`` functions call the op only while torch
 its outputs; the one that writes into an argument, ``depth_metrics_update``, declares it in ``mutates_args``.  Each
 ``register_fake`` states the output shapes and dtypes the eager function returns, from shapes and host arithmetic only.
 
-Training entry points stay ``torch.autograd.Function``s and are not registered.
+The training launches are ops too (``TRAIN_OPS``), tied to their backward ops with ``register_autograd``: the G-Net
+head, the fused mask loss, the upsample-NLL and F-Net losses, the F volume, and the backwards of ``gaussian_update`` and
+``convex_upsample``.  What an autograd Function keeps on ``ctx`` (packed weights, saved maps) is an op output here.
+The loss ops take the number of supervised pixels as a device tensor and normalise on the device, with the eager
+arithmetic inside the op (DESIGN §3.18), so a compiled step has no host read and can be captured in a CUDA graph.
 """
 from __future__ import annotations
 
@@ -23,6 +27,11 @@ _NS = "magnet_b200"
 
 def _op(name: str, mutates_args=()):
     return torch.library.custom_op(f"{_NS}::{name}", mutates_args=mutates_args, device_types="cuda")
+
+
+def _grads(ctx, need_from: int, grads):
+    """``grads`` with None where ``ctx.needs_input_grad[need_from + i]`` is False."""
+    return [g if n else None for g, n in zip(grads, ctx.needs_input_grad[need_from:])]
 
 
 def _f32(x: Tensor, *shape) -> Tensor:
@@ -290,7 +299,313 @@ def _(acc, preds, gt, min_depth, max_depth, crop, up_mask, k, nearest, variance)
     return _metric_rows(preds, gt)
 
 
+# --- training: backwards of the update and the upsampling -------------------------------------------------------------
+
+@_op("gaussian_update_bwd")
+def gaussian_update_bwd(grad_out: Tensor, d_output: Tensor, ref_gmm: Tensor) -> Tensor:
+    return ops.gaussian_update_bwd(grad_out, d_output, ref_gmm)
+
+
+@gaussian_update_bwd.register_fake
+def _(grad_out, d_output, ref_gmm):
+    return d_output.new_empty(d_output.shape, dtype=torch.float32)
+
+
+def _gaussian_update_setup(ctx, inputs, output):
+    ctx.save_for_backward(*inputs)
+
+
+def _gaussian_update_backward(ctx, grad):
+    d_output, ref_gmm = ctx.saved_tensors
+    return gaussian_update_bwd(grad, d_output, ref_gmm), None
+
+
+gaussian_update.register_autograd(_gaussian_update_backward, setup_context=_gaussian_update_setup)
+
+
+@_op("convex_upsample_bwd")
+def convex_upsample_bwd(grad_out: Tensor, depth: Tensor, up_mask: Tensor, k: int) -> Tuple[Tensor, Tensor]:
+    return ops.convex_upsample_bwd(grad_out, depth, up_mask, k)
+
+
+@convex_upsample_bwd.register_fake
+def _(grad_out, depth, up_mask, k):
+    return _f32(depth, *depth.shape), _f32(up_mask, *up_mask.shape)
+
+
+def _convex_upsample_setup(ctx, inputs, output):
+    depth, up_mask, ctx.k = inputs
+    ctx.save_for_backward(depth, up_mask)
+
+
+def _convex_upsample_backward(ctx, grad):
+    depth, up_mask = ctx.saved_tensors
+    return (*convex_upsample_bwd(grad, depth, up_mask, ctx.k), None)
+
+
+convex_upsample.register_autograd(_convex_upsample_backward, setup_context=_convex_upsample_setup)
+
+
+# --- training: G-Net head --------------------------------------------------------------------------------------------
+
+@_op("gnet_train_fwd")
+def gnet_train_fwd(cost: Tensor, invariant: Tensor, w0: Tensor, w1: Tensor, b1: Tensor, w2: Tensor, b2: Tensor,
+                   w3: Tensor, b3: Tensor, prev_gmm: Tensor) -> Tuple[Tensor, Tensor, Tensor]:
+    """``GnetHeadTrain``'s forward: (updated Gaussian, packed training weights, saved hidden maps)."""
+    out, packed, saved, _, _ = ops.gnet_train_fwd(cost, invariant, (w0, w1, b1, w2, b2, w3, b3), prev_gmm)
+    return out, packed, saved
+
+
+@gnet_train_fwd.register_fake
+def _(cost, invariant, w0, w1, b1, w2, b2, w3, b3, prev_gmm):
+    B, D, H, W = cost.shape
+    L = _lib.lib()
+    return (_f32(cost, B, 2, H, W), _bytes(cost, int(L.magnet_gnet_train_weights_bytes(D))),
+            _f32(cost, int(L.magnet_gnet_saved_bytes(B, H, W)) // 4))
+
+
+@_op("gnet_bwd")
+def gnet_bwd(grad_out: Tensor, cost: Tensor, prev_gmm: Tensor, packed: Tensor, saved: Tensor,
+             need: List[bool]) -> List[Tensor]:
+    """[grad of the invariant, of W0[:, :D], W1, b1, W2, b2, W3, b3, of prev_gmm]; an empty tensor where ``need`` (8
+    flags: the weights and prev_gmm) is False."""
+    return [_empty_if_none(g, cost) for g in ops.gnet_bwd(grad_out, cost, prev_gmm, packed, saved, need)]
+
+
+def _empty_if_none(g, like):
+    return like.new_empty((0,), dtype=torch.float32) if g is None else g
+
+
+@gnet_bwd.register_fake
+def _(grad_out, cost, prev_gmm, packed, saved, need):
+    B, D, H, W = cost.shape
+    shapes = [s for _, s in ops.gnet_weight_shapes(D)] + [(B, 2, H, W)]
+    return [_f32(cost, B, _lib.MAGNET_HIDDEN_CHANNELS, H, W)] + [_f32(cost, *(s if n else (0,))) for s, n in zip(shapes, need)]
+
+
+def _gnet_train_setup(ctx, inputs, output):
+    cost, prev_gmm = inputs[0], inputs[9]
+    ctx.save_for_backward(cost, prev_gmm, output[1], output[2])
+
+
+def _gnet_train_backward(ctx, grad, _packed, _saved):
+    cost, prev_gmm, packed, saved = ctx.saved_tensors
+    need = [bool(n) for n in ctx.needs_input_grad[2:10]]
+    return (None, *_grads(ctx, 1, gnet_bwd(grad, cost, prev_gmm, packed, saved, need)))
+
+
+gnet_train_fwd.register_autograd(_gnet_train_backward, setup_context=_gnet_train_setup)
+
+
+# --- training: the fused mask head, upsampling and loss --------------------------------------------------------------
+
+@_op("mask_train_fwd")
+def mask_train_fwd(pre0: Tensor, w1: Tensor, b1: Tensor, w2: Tensor, b2: Tensor, w3: Tensor, b3: Tensor, gt: Tensor,
+                   gt_mask: Tensor, count: Tensor, preds: List[Tensor], gamma: float, save_maps: bool,
+                   pred_grad: bool) -> Tuple[Tensor, Tensor, Tensor]:
+    """``MaskLossTrain``'s forward with the number of supervised pixels ``count`` on the device: (loss, packed training
+    weights, saved).  The prediction scales gamma_p / count are formed on the device and read by the kernel when it
+    runs; the loss is formed from the partials as the eager forward forms it (NaN for count 0)."""
+    P = len(preds)
+    gammas = ops.loss_weights(gamma, P)
+    # the weights are filled on the device (a host-to-device copy could not be captured in a CUDA graph)
+    num = torch.stack([torch.full((), g, dtype=torch.float64, device=pre0.device) for g in gammas])
+    scales = ops.device_scales(num, count)
+    partial, packed, saved = ops.mask_train_fwd(pre0, (w1, b1, w2, b2, w3, b3), preds, gt, gt_mask, save_maps,
+                                                pred_grad, scales)
+    terms = ops.loss_term(partial.view(-1, P).sum(0, dtype=torch.float64), count)
+    loss = 0.0
+    for i in range(P):
+        loss = loss + gammas[i] * terms[i]
+    return loss, packed, saved
+
+
+@mask_train_fwd.register_fake
+def _(pre0, w1, b1, w2, b2, w3, b3, gt, gt_mask, count, preds, gamma, save_maps, pred_grad):
+    B, _, H, W = pre0.shape
+    return (pre0.new_empty((), dtype=torch.float32), _bytes(pre0, int(_lib.lib().magnet_mask_train_weights_bytes(4))),
+            _f32(pre0, ops.mask_saved_floats(len(preds), B, H, W, save_maps)))
+
+
+@_op("mask_bwd")
+def mask_bwd(grad_loss: Tensor, packed: Tensor, saved: Tensor, P: int, B: int, H: int, W: int,
+             need_layers: List[bool], pred_grad: bool) -> List[Tensor]:
+    """[grad of pre0, of W1, b1, W2, b2, W3, b3, then of each of the P predictions]; an empty tensor where
+    ``need_layers`` (7 flags: pre0 and the six tensors) or ``pred_grad`` is False."""
+    g = ops.mask_bwd(grad_loss, packed, saved, (P, B, H, W), need_layers, [pred_grad] * P)
+    return [_empty_if_none(t, saved) for t in g]
+
+
+@mask_bwd.register_fake
+def _(grad_loss, packed, saved, P, B, H, W, need_layers, pred_grad):
+    shapes = [(B, _lib.MAGNET_HIDDEN_CHANNELS, H, W)] + [s for _, s in ops.mask_weight_shapes()]
+    return ([_f32(saved, *(s if n else (0,))) for s, n in zip(shapes, need_layers)]
+            + [_f32(saved, *((B, 2, H, W) if pred_grad else (0,))) for _ in range(P)])
+
+
+def _mask_train_setup(ctx, inputs, output):
+    pre0, preds, pred_grad = inputs[0], inputs[10], inputs[13]
+    B, _, H, W = pre0.shape
+    ctx.shape, ctx.pred_grad = (len(preds), B, H, W), pred_grad
+    ctx.save_for_backward(output[1], output[2])
+
+
+def _mask_train_backward(ctx, grad, _packed, _saved):
+    packed, saved = ctx.saved_tensors
+    P = ctx.shape[0]
+    need = [bool(n) for n in ctx.needs_input_grad[:7]]
+    g = mask_bwd(grad, packed, saved, *ctx.shape, need, ctx.pred_grad)
+    preds = list(g[7:]) if ctx.pred_grad else [None] * P
+    return (*_grads(ctx, 0, g[:7]), None, None, None, preds, None, None, None)
+
+
+mask_train_fwd.register_autograd(_mask_train_backward, setup_context=_mask_train_setup)
+
+
+# --- training: the module path's upsample-NLL loss -------------------------------------------------------------------
+
+@_op("upsample_nll_fwd")
+def upsample_nll_fwd(depth: Tensor, up_mask: Tensor, gt: Tensor, gt_mask: Tensor, k: int, count: Tensor,
+                     weight: float) -> Tensor:
+    """``weight * UpsampleNLL(depth, up_mask, gt, gt_mask, k, count)`` with ``count`` on the device: one term of
+    ``magnet_loss``, weighted as the eager sum weights it (NaN for count 0)."""
+    partial, _ = ops.upsample_nll_fwd(depth, up_mask, gt, gt_mask, k)
+    return ops.loss_term(partial.sum(dtype=torch.float64), count) * weight
+
+
+@upsample_nll_fwd.register_fake
+def _(depth, up_mask, gt, gt_mask, k, count, weight):
+    return depth.new_empty((), dtype=torch.float32)
+
+
+@_op("upsample_nll_bwd")
+def upsample_nll_bwd(grad: Tensor, depth: Tensor, up_mask: Tensor, gt: Tensor, gt_mask: Tensor, k: int, count: Tensor,
+                     weight: float) -> Tuple[Tensor, Tensor]:
+    """The gradients of ``upsample_nll_fwd`` w.r.t. (depth, up_mask): the term's upstream gradient ``grad * weight``
+    over ``count`` in float64, rounded once to fp32 (0 for count 0), read by the kernel from device memory."""
+    scale = ops.device_scales(grad.to(torch.float32) * weight, count)
+    return ops.upsample_nll_bwd(depth, up_mask, gt, gt_mask, k, scale)
+
+
+@upsample_nll_bwd.register_fake
+def _(grad, depth, up_mask, gt, gt_mask, k, count, weight):
+    return _f32(depth, *depth.shape), _f32(up_mask, *up_mask.shape)
+
+
+def _upsample_nll_setup(ctx, inputs, output):
+    depth, up_mask, gt, gt_mask, ctx.k, count, ctx.weight = inputs
+    ctx.save_for_backward(depth, up_mask, gt, gt_mask, count)
+
+
+def _upsample_nll_backward(ctx, grad):
+    depth, up_mask, gt, gt_mask, count = ctx.saved_tensors
+    g_depth, g_mask = upsample_nll_bwd(grad, depth, up_mask, gt, gt_mask, ctx.k, count, ctx.weight)
+    return g_depth, g_mask, None, None, None, None, None
+
+
+upsample_nll_fwd.register_autograd(_upsample_nll_backward, setup_context=_upsample_nll_setup)
+
+
+# --- training: F-Net's L1 loss and the F volume ----------------------------------------------------------------------
+
+@_op("fnet_l1_fwd")
+def fnet_l1_fwd(scores: Tensor, planes: List[float], gt: Tensor, mask: Tensor, count: Tensor) -> Tensor:
+    """``FnetL1Loss`` with ``count`` on the device (NaN for count 0)."""
+    partial = ops.fnet_l1_fwd(scores, planes, gt, mask)[0]
+    return ops.loss_term(partial.sum(dtype=torch.float64), count)
+
+
+@fnet_l1_fwd.register_fake
+def _(scores, planes, gt, mask, count):
+    return scores.new_empty((), dtype=torch.float32)
+
+
+@_op("fnet_l1_bwd")
+def fnet_l1_bwd(grad: Tensor, scores: Tensor, planes: List[float], gt: Tensor, mask: Tensor, count: Tensor) -> Tensor:
+    """The gradient of ``fnet_l1_fwd`` w.r.t. the scores: the eager kernel scale fp32(1 / count) (0 for count 0) times
+    the upstream gradient, one fp32 product as the kernel forms it, read from device memory."""
+    grad_scale = ops.device_scales(torch.ones_like(count, dtype=torch.float64), count) * grad.to(torch.float32)
+    return ops.fnet_l1_bwd(scores, planes, gt, mask, 1.0, grad_scale)
+
+
+@fnet_l1_bwd.register_fake
+def _(grad, scores, planes, gt, mask, count):
+    return _f32(scores, *scores.shape)
+
+
+def _fnet_l1_setup(ctx, inputs, output):
+    scores, ctx.planes, gt, mask, count = inputs
+    ctx.save_for_backward(scores, gt, mask, count)
+
+
+def _fnet_l1_backward(ctx, grad):
+    scores, gt, mask, count = ctx.saved_tensors
+    return fnet_l1_bwd(grad, scores, ctx.planes, gt, mask, count), None, None, None, None
+
+
+fnet_l1_fwd.register_autograd(_fnet_l1_backward, setup_context=_fnet_l1_setup)
+
+
+@_op("cost_volume_f")
+def cost_volume_f(ref_feat: Tensor, nghbr_feat: Tensor, src: Tensor, ref_split: Optional[Tensor], rays: Tensor,
+                  cams: Tensor, V: int, layout: int, variant: int, planes: List[float], softmax: bool,
+                  tc_bwd: bool) -> Tensor:
+    """The F volume of training (``_CostVolumeF``): ``src`` / ``ref_split`` are the source maps in ``layout`` and the
+    reference split the forward reads (``homography.repack_source``); ``ref_feat`` / ``nghbr_feat`` the NCHW maps it is
+    differentiable in.  With ``tc_bwd`` and a SPLIT16 / HALF16 layout the backward runs on the tensor cores on the same
+    buffers, otherwise on the CUDA cores on the NCHW maps."""
+    ref = ref_feat if layout == _lib.SRC_HALF16 else ref_feat.float()
+    return ops.cost_volume(ref.detach(), src, rays, cams, V=V, src_layout=layout, consistency=False, k=planes,
+                           planes=True, softmax=softmax, variant=variant, ref_split=ref_split)
+
+
+@cost_volume_f.register_fake
+def _(ref_feat, nghbr_feat, src, ref_split, rays, cams, V, layout, variant, planes, softmax, tc_bwd):
+    B, _, H, W = ref_feat.shape
+    return _f32(ref_feat, B, len(planes), H, W)
+
+
+@_op("cost_volume_f_bwd")
+def cost_volume_f_bwd(grad_out: Tensor, ref_feat: Tensor, nghbr_feat: Tensor, rays: Tensor, cams: Tensor, V: int,
+                      planes: List[float], prob: Optional[Tensor], softmax: bool, ref_split: Optional[Tensor],
+                      src_split: Optional[Tensor], layout: int) -> Tuple[Tensor, Tensor]:
+    """The gradients of ``cost_volume_f`` w.r.t. (ref_feat, nghbr_feat), in their dtypes: the tensor-core kernel on the
+    forward's buffers for a SPLIT16 / HALF16 ``layout``, else the CUDA-core kernel on the fp32 NCHW maps."""
+    shape_only = layout == _lib.SRC_HALF16
+    ref, src = (ref_feat, nghbr_feat) if shape_only else (ref_feat.float(), nghbr_feat.float())
+    g_ref, g_src = ops.cost_volume_f_bwd(ref, src, rays, cams, planes, V, prob, grad_out.contiguous(), softmax=softmax,
+                                         ref_split=ref_split, src_split=src_split,
+                                         split_layout=layout if layout in ops.PACKED_LAYOUTS else _lib.SRC_SPLIT16)
+    return g_ref.to(ref_feat.dtype), g_src.to(nghbr_feat.dtype)
+
+
+@cost_volume_f_bwd.register_fake
+def _(grad_out, ref_feat, nghbr_feat, rays, cams, V, planes, prob, softmax, ref_split, src_split, layout):
+    return ref_feat.new_empty(ref_feat.shape), nghbr_feat.new_empty(nghbr_feat.shape)
+
+
+def _cost_volume_f_setup(ctx, inputs, output):
+    ref_feat, nghbr_feat, src, ref_split, rays, cams, V, layout, _, planes, softmax, tc_bwd = inputs
+    ctx.layout = layout if tc_bwd and layout in ops.PACKED_LAYOUTS else _lib.SRC_NCHW
+    packed = ctx.layout in ops.PACKED_LAYOUTS
+    ctx.V, ctx.planes, ctx.softmax = V, planes, softmax
+    ctx.save_for_backward(ref_feat, nghbr_feat, rays, cams, output if softmax else None, ref_split if packed else None,
+                          src if packed else None)
+
+
+def _cost_volume_f_backward(ctx, grad):
+    ref_feat, nghbr_feat, rays, cams, prob, ref_split, src_split = ctx.saved_tensors
+    g_ref, g_src = cost_volume_f_bwd(grad, ref_feat, nghbr_feat, rays, cams, ctx.V, ctx.planes, prob, ctx.softmax,
+                                     ref_split, src_split, ctx.layout)
+    return (g_ref, g_src) + (None,) * 10
+
+
+cost_volume_f.register_autograd(_cost_volume_f_backward, setup_context=_cost_volume_f_setup)
+
+
 OPS = ("pack_cameras", "relative_poses", "camera_rays", "sample_depths", "repack_tiled32", "repack_pixc",
        "repack_split16", "repack_half16", "cost_volume", "gaussian_update", "pack_gnet_weights", "gnet_update",
        "convex_upsample", "pack_mask_weights", "mask_upsample", "pack_dnet_weights", "dnet_depth", "dnet_upsample",
        "plane_depth", "depth_metrics", "depth_metrics_update")
+TRAIN_OPS = ("gaussian_update_bwd", "convex_upsample_bwd", "gnet_train_fwd", "gnet_bwd", "mask_train_fwd", "mask_bwd",
+             "upsample_nll_fwd", "upsample_nll_bwd", "fnet_l1_fwd", "fnet_l1_bwd", "cost_volume_f", "cost_volume_f_bwd")

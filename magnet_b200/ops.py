@@ -593,16 +593,22 @@ class GaussianUpdate(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out: torch.Tensor):
         d_output, ref_gmm = ctx.saved_tensors
-        grad_out = _need_cuda_f32("grad_out", grad_out)
-        B, _, H, W = d_output.shape
-        gin = torch.empty_like(d_output)
-        _launch(d_output.device, "magnet_gaussian_update_bwd_f32", grad_out.data_ptr(), d_output.data_ptr(),
-                ref_gmm.data_ptr(), B, H * W, gin.data_ptr())
-        return gin, None
+        return gaussian_update_bwd(grad_out, d_output, ref_gmm), None
+
+
+def gaussian_update_bwd(grad_out, d_output, ref_gmm) -> torch.Tensor:
+    """The gradient of ``gaussian_update`` w.r.t. d_output: one magnet_gaussian_update_bwd_f32 launch."""
+    grad_out = _need_cuda_f32("grad_out", grad_out)
+    d_output, ref_gmm = _need_cuda_f32("d_output", d_output), _need_cuda_f32("ref_gmm", ref_gmm)
+    B, _, H, W = d_output.shape
+    gin = torch.empty_like(d_output)
+    _launch(d_output.device, "magnet_gaussian_update_bwd_f32", grad_out.data_ptr(), d_output.data_ptr(),
+            ref_gmm.data_ptr(), B, H * W, gin.data_ptr())
+    return gin
 
 
 def gaussian_update(d_output: torch.Tensor, ref_gmm: torch.Tensor) -> torch.Tensor:
-    if _traced() and not (torch.is_grad_enabled() and d_output.requires_grad):
+    if _traced():                                  # the op has a backward (magnet_b200.library)
         return _op("gaussian_update")(d_output, ref_gmm.detach())
     return GaussianUpdate.apply(d_output, ref_gmm)
 
@@ -686,30 +692,7 @@ class GnetHeadTrain(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, cost, invariant, w0, w1, b1, w2, b2, w3, b3, prev_gmm):
-        hid = _lib.MAGNET_HIDDEN_CHANNELS
-        cost = _need_cuda_f32("cost", cost.detach())
-        if cost.dim() != 4:
-            raise _lib.MagnetError(f"cost must be (B,D,H,W), got {tuple(cost.shape)}")
-        B, D, H, W = cost.shape
-        invariant = _need_cuda_f32("invariant", invariant.detach(), (B, hid, H, W))
-        prev_gmm = _need_cuda_f32("prev_gmm", prev_gmm.detach(), (B, 2, H, W))
-        _check_cost_channels(D)
-        nbytes = int(lib().magnet_gnet_train_weights_bytes(D))
-        shapes = (("W0", w0, (hid, D, 3, 3)), ("W1", w1, (hid, hid, 1, 1)), ("b1", b1, (hid,)),
-                  ("W2", w2, (hid, hid, 1, 1)), ("b2", b2, (hid,)), ("W3", w3, (2, hid, 1, 1)), ("b3", b3, (2,)))
-        ws = _need_weights(shapes)
-        ctx.weight_shapes = [shape for _, _, shape in shapes]
-        dev = _same_device(("cost", cost), ("invariant", invariant), ("prev_gmm", prev_gmm),
-                           *((nm, t) for (nm, _, _), t in zip(shapes, ws)))
-        packed = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-        saved = torch.empty(int(lib().magnet_gnet_saved_bytes(B, H, W)) // 4, device=dev, dtype=torch.float32)
-        out = torch.empty(B, 2, H, W, device=dev, dtype=torch.float32)
-        scratch = torch.empty(_lib.MAGNET_GNET_SCRATCH_BYTES // 4, device=dev, dtype=torch.int32)
-        a = _lib.GnetTrainArgs(B=B, D=D, H=H, W=W, cost=cost.data_ptr(), invariant=invariant.data_ptr(),
-                               packed_weights=packed.data_ptr(), prev_gmm=prev_gmm.data_ptr(), scratch=scratch.data_ptr(),
-                               out=out.data_ptr(), saved=saved.data_ptr())
-        _launch(dev, "magnet_gnet_pack_train_weights_f32", *(t.data_ptr() for t in ws), D, packed.data_ptr())
-        _launch(dev, "magnet_gnet_train_fwd_f32", C.byref(a))
+        out, packed, saved, cost, prev_gmm = gnet_train_fwd(cost, invariant, (w0, w1, b1, w2, b2, w3, b3), prev_gmm)
         ctx.save_for_backward(cost, prev_gmm, packed, saved)
         return out
 
@@ -717,21 +700,64 @@ class GnetHeadTrain(torch.autograd.Function):
     def backward(ctx, grad_out):
         cost, prev_gmm, packed, saved = ctx.saved_tensors
         need = ctx.needs_input_grad
-        B, D, H, W = cost.shape
-        dev = cost.device
-        grad_out = _need_cuda_f32("grad_out", grad_out)
-        new = lambda shape: torch.empty(shape, device=dev, dtype=torch.float32)
-        g_inv = new((B, _lib.MAGNET_HIDDEN_CHANNELS, H, W))
-        g = [new(shape) if n else None for shape, n in zip(ctx.weight_shapes, need[2:9])]
-        g_prev = new((B, 2, H, W)) if need[9] else None
-        ws = torch.empty(int(lib().magnet_gnet_bwd_workspace_bytes(B, D, H, W)), device=dev, dtype=torch.uint8)
-        a = _lib.GnetTrainArgs(B=B, D=D, H=H, W=W, cost=cost.data_ptr(), packed_weights=packed.data_ptr(),
-                               prev_gmm=prev_gmm.data_ptr(), saved=saved.data_ptr(), grad_out=grad_out.data_ptr(),
-                               workspace=ws.data_ptr(), grad_invariant=g_inv.data_ptr(), grad_w0_cost=_ptr(g[0]),
-                               grad_w1=_ptr(g[1]), grad_b1=_ptr(g[2]), grad_w2=_ptr(g[3]), grad_b2=_ptr(g[4]),
-                               grad_w3=_ptr(g[5]), grad_b3=_ptr(g[6]), grad_prev=_ptr(g_prev))
-        _launch(dev, "magnet_gnet_bwd_f32", C.byref(a))
+        g_inv, *g, g_prev = gnet_bwd(grad_out, cost, prev_gmm, packed, saved, need[2:10])
         return (None, g_inv if need[1] else None, *g, g_prev)
+
+
+def gnet_weight_shapes(D: int):
+    """(name, shape) of the fused head's trained tensors W0[:, :D], W1, b1, W2, b2, W3, b3."""
+    hid = _lib.MAGNET_HIDDEN_CHANNELS
+    return (("W0", (hid, D, 3, 3)), ("W1", (hid, hid, 1, 1)), ("b1", (hid,)), ("W2", (hid, hid, 1, 1)), ("b2", (hid,)),
+            ("W3", (2, hid, 1, 1)), ("b3", (2,)))
+
+
+def gnet_train_fwd(cost, invariant, weights, prev_gmm):
+    """The forward of ``GnetHeadTrain``: the weights W0[:, :D], W1, b1, W2, b2, W3, b3 packed for training, then the
+    training forward (two launches).  Returns (out (B,2,H,W), packed weights, saved hidden maps, and the checked cost
+    and prev_gmm the backward reads)."""
+    cost = _need_cuda_f32("cost", cost.detach())
+    if cost.dim() != 4:
+        raise _lib.MagnetError(f"cost must be (B,D,H,W), got {tuple(cost.shape)}")
+    B, D, H, W = cost.shape
+    invariant = _need_cuda_f32("invariant", invariant.detach(), (B, _lib.MAGNET_HIDDEN_CHANNELS, H, W))
+    prev_gmm = _need_cuda_f32("prev_gmm", prev_gmm.detach(), (B, 2, H, W))
+    _check_cost_channels(D)
+    nbytes = int(lib().magnet_gnet_train_weights_bytes(D))
+    shapes = gnet_weight_shapes(D)
+    ws = _need_weights([(nm, t, shp) for (nm, shp), t in zip(shapes, weights)])
+    dev = _same_device(("cost", cost), ("invariant", invariant), ("prev_gmm", prev_gmm),
+                       *((nm, t) for (nm, _), t in zip(shapes, ws)))
+    packed = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+    saved = torch.empty(int(lib().magnet_gnet_saved_bytes(B, H, W)) // 4, device=dev, dtype=torch.float32)
+    out = torch.empty(B, 2, H, W, device=dev, dtype=torch.float32)
+    scratch = torch.empty(_lib.MAGNET_GNET_SCRATCH_BYTES // 4, device=dev, dtype=torch.int32)
+    a = _lib.GnetTrainArgs(B=B, D=D, H=H, W=W, cost=cost.data_ptr(), invariant=invariant.data_ptr(),
+                           packed_weights=packed.data_ptr(), prev_gmm=prev_gmm.data_ptr(), scratch=scratch.data_ptr(),
+                           out=out.data_ptr(), saved=saved.data_ptr())
+    _launch(dev, "magnet_gnet_pack_train_weights_f32", *(t.data_ptr() for t in ws), D, packed.data_ptr())
+    _launch(dev, "magnet_gnet_train_fwd_f32", C.byref(a))
+    return out, packed, saved, cost, prev_gmm
+
+
+def gnet_bwd(grad_out, cost, prev_gmm, packed, saved, need):
+    """The backward of ``GnetHeadTrain`` (one magnet_gnet_bwd_f32 call): -> [grad of the invariant, of W0[:, :D], W1, b1,
+    W2, b2, W3, b3, of prev_gmm].  ``need``: 8 flags, whether the gradient of each weight and of prev_gmm is written
+    (None where not); the invariant's gradient is always written."""
+    B, D, H, W = cost.shape
+    dev = cost.device
+    grad_out = _need_cuda_f32("grad_out", grad_out)
+    new = lambda shape: torch.empty(shape, device=dev, dtype=torch.float32)
+    g_inv = new((B, _lib.MAGNET_HIDDEN_CHANNELS, H, W))
+    g = [new(shape) if n else None for (_, shape), n in zip(gnet_weight_shapes(D), need[:7])]
+    g_prev = new((B, 2, H, W)) if need[7] else None
+    ws = torch.empty(int(lib().magnet_gnet_bwd_workspace_bytes(B, D, H, W)), device=dev, dtype=torch.uint8)
+    a = _lib.GnetTrainArgs(B=B, D=D, H=H, W=W, cost=cost.data_ptr(), packed_weights=packed.data_ptr(),
+                           prev_gmm=prev_gmm.data_ptr(), saved=saved.data_ptr(), grad_out=grad_out.data_ptr(),
+                           workspace=ws.data_ptr(), grad_invariant=g_inv.data_ptr(), grad_w0_cost=_ptr(g[0]),
+                           grad_w1=_ptr(g[1]), grad_b1=_ptr(g[2]), grad_w2=_ptr(g[3]), grad_b2=_ptr(g[4]),
+                           grad_w3=_ptr(g[5]), grad_b3=_ptr(g[6]), grad_prev=_ptr(g_prev))
+    _launch(dev, "magnet_gnet_bwd_f32", C.byref(a))
+    return [g_inv, *g, g_prev]
 
 
 def gnet_head_train(cost, invariant, gnet, prev_gmm):
@@ -742,8 +768,10 @@ def gnet_head_train(cost, invariant, gnet, prev_gmm):
         raise _lib.MagnetError(f"cost must be (B,D,H,W), got {tuple(cost.shape)}")
     D = cost.shape[1]
     c0, c1, c2, c3 = _gnet_convs(gnet, D)
-    return GnetHeadTrain.apply(cost, invariant, c0.weight[:, :D], c1.weight, c1.bias, c2.weight, c2.bias, c3.weight,
-                               c3.bias, prev_gmm)
+    ws = (c0.weight[:, :D], c1.weight, c1.bias, c2.weight, c2.bias, c3.weight, c3.bias)
+    if _traced():
+        return _op("gnet_train_fwd")(cost, invariant, *ws, prev_gmm)[0]
+    return GnetHeadTrain.apply(cost, invariant, *ws, prev_gmm)
 
 
 class ConvexUpsample(torch.autograd.Function):
@@ -767,17 +795,23 @@ class ConvexUpsample(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out: torch.Tensor):
         depth, up_mask = ctx.saved_tensors
-        grad_out = _need_cuda_f32("grad_out", grad_out)
-        B, CH, H, W = depth.shape
-        g_depth = torch.zeros_like(depth)
-        g_mask = torch.empty_like(up_mask)
-        _launch(depth.device, "magnet_convex_upsample_bwd_f32", grad_out.data_ptr(), depth.data_ptr(),
-                up_mask.data_ptr(), B, CH, H, W, ctx.k, g_depth.data_ptr(), g_mask.data_ptr())
-        return g_depth, g_mask, None
+        return (*convex_upsample_bwd(grad_out, depth, up_mask, ctx.k), None)
+
+
+def convex_upsample_bwd(grad_out, depth, up_mask, k: int):
+    """The gradients of ``convex_upsample`` w.r.t. (depth, up_mask): one magnet_convex_upsample_bwd_f32 launch."""
+    grad_out = _need_cuda_f32("grad_out", grad_out)
+    depth, up_mask = _need_cuda_f32("depth", depth), _need_cuda_f32("up_mask", up_mask)
+    B, CH, H, W = depth.shape
+    g_depth = torch.zeros_like(depth)
+    g_mask = torch.empty_like(up_mask)
+    _launch(depth.device, "magnet_convex_upsample_bwd_f32", grad_out.data_ptr(), depth.data_ptr(),
+            up_mask.data_ptr(), B, CH, H, W, k, g_depth.data_ptr(), g_mask.data_ptr())
+    return g_depth, g_mask
 
 
 def convex_upsample(depth: torch.Tensor, up_mask: torch.Tensor, k: int) -> torch.Tensor:
-    if _traced() and not (torch.is_grad_enabled() and (depth.requires_grad or up_mask.requires_grad)):
+    if _traced():                                  # the op has a backward (magnet_b200.library)
         return _op("convex_upsample")(depth, up_mask, int(k))
     return ConvexUpsample.apply(depth, up_mask, k)
 
@@ -1015,40 +1049,15 @@ class MaskLossTrain(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, pre0, w1, b1, w2, b2, w3, b3, gt, gt_mask_u8, k, gamma, count, *preds):
-        hid, nout = _lib.MAGNET_HIDDEN_CHANNELS, 9 * 4 * 4
-        P = len(preds)
-        if not 1 <= P <= _lib.MAGNET_MASK_MAX_PRED:
-            raise _lib.MagnetError(f"the fused mask-head loss takes 1 to {_lib.MAGNET_MASK_MAX_PRED} predictions, got {P}")
         _check_k4(k)
-        pre0 = _need_hidden("pre0", pre0.detach())
-        B, _, H, W = pre0.shape
-        shapes = (("W1", w1, (hid, hid, 1, 1)), ("b1", b1, (hid,)), ("W2", w2, (hid, hid, 1, 1)), ("b2", b2, (hid,)),
-                  ("W3", w3, (nout, hid, 1, 1)), ("b3", b3, (nout,)))
-        ws = _need_weights(shapes)
-        ctx.weight_shapes = [shape for _, _, shape in shapes]
-        ps = _need_preds("preds", (p.detach() for p in preds), (B, 2, H, W))
-        gt = _need_cuda_f32("gt", gt.detach(), (B, 1, 4 * H, 4 * W))
-        gt_mask_u8 = _need_cuda_u8_mask("gt_mask", gt_mask_u8, (B, 1, 4 * H, 4 * W), "(B,1,4H,4W)")
-        dev = _same_device(("pre0", pre0), ("gt", gt), ("gt_mask", gt_mask_u8),
-                           *((nm, t) for (nm, _, _), t in zip(shapes, ws)), *((f"preds[{i}]", p) for i, p in enumerate(ps)))
         need = ctx.needs_input_grad
         save_maps, pred_grad = any(need[:7]), any(need[12:])
-        gammas = [gamma ** (P - i - 1) for i in range(P)]
-        scale = (C.c_float * P)(*[g / float(count) for g in gammas])
-        pp = (C.c_void_p * P)(*[p.data_ptr() for p in ps])
-        packed = torch.empty(int(lib().magnet_mask_train_weights_bytes(4)), device=dev, dtype=torch.uint8)
-        partial = torch.empty(int(lib().magnet_mask_train_partials(B, H, W)) * P, device=dev, dtype=torch.float32)
-        # the prediction gradients come first in `saved`; the maps after them only when a layer gradient needs them
-        nsaved = int(lib().magnet_mask_saved_bytes(P, B, H, W)) // 4 if save_maps else 2 * P * B * H * W
-        saved = torch.empty(nsaved, device=dev, dtype=torch.float32)
-        a = _lib.MaskTrainArgs(P=P, B=B, H=H, W=W, k=4, pre0=pre0.data_ptr(), packed_weights=packed.data_ptr(),
-                               pred=C.cast(pp, C.POINTER(C.c_void_p)), gt=gt.data_ptr(), gt_mask=gt_mask_u8.data_ptr(),
-                               pred_scale=C.cast(scale, C.POINTER(C.c_float)), save_maps=int(save_maps),
-                               pred_grad=int(pred_grad), partial=partial.data_ptr(), saved=saved.data_ptr())
-        _launch(dev, "magnet_mask_pack_train_weights_f32", *(t.data_ptr() for t in ws), packed.data_ptr())
-        _launch(dev, "magnet_mask_train_fwd_f32", C.byref(a))
+        P = len(preds)
+        gammas = loss_weights(gamma, P)
+        partial, packed, saved = mask_train_fwd(pre0, (w1, b1, w2, b2, w3, b3), preds, gt, gt_mask_u8, save_maps,
+                                                pred_grad, [g / float(count) for g in gammas])
         ctx.save_for_backward(packed, saved)
-        ctx.shape = (P, B, H, W)
+        ctx.shape = (P, *pre0.shape[:1], *pre0.shape[2:])
         # as magnet_loss sums its terms: per prediction the float64 sum of the partials, in fp32 over count, weighted
         terms = partial.view(-1, P).sum(0, dtype=torch.float64).to(torch.float32) / float(count)
         loss = 0.0
@@ -1060,22 +1069,106 @@ class MaskLossTrain(torch.autograd.Function):
     def backward(ctx, grad_loss):
         packed, saved = ctx.saved_tensors
         need = ctx.needs_input_grad
-        P, B, H, W = ctx.shape
-        dev = saved.device
-        new = lambda shape: torch.empty(shape, device=dev, dtype=torch.float32)
-        g_pre0 = new((B, _lib.MAGNET_HIDDEN_CHANNELS, H, W)) if need[0] else None
-        g = [new(shape) if n else None for shape, n in zip(ctx.weight_shapes, need[1:7])]
-        g_preds = [new((B, 2, H, W)) if need[12 + i] else None for i in range(P)]
-        grad_scale = grad_loss.detach().to(device=dev, dtype=torch.float32).reshape(1).contiguous()
-        nws = int(lib().magnet_mask_bwd_workspace_bytes(B, H, W)) if any(need[:7]) else 256
-        ws = torch.empty(nws, device=dev, dtype=torch.uint8)
-        gp = (C.c_void_p * P)(*[_ptr(t) for t in g_preds])
-        a = _lib.MaskTrainArgs(P=P, B=B, H=H, W=W, k=4, packed_weights=packed.data_ptr(), saved=saved.data_ptr(),
-                               grad_scale=grad_scale.data_ptr(), workspace=ws.data_ptr(), grad_pre0=_ptr(g_pre0),
-                               grad_w1=_ptr(g[0]), grad_b1=_ptr(g[1]), grad_w2=_ptr(g[2]), grad_b2=_ptr(g[3]),
-                               grad_w3=_ptr(g[4]), grad_b3=_ptr(g[5]), grad_pred=C.cast(gp, C.POINTER(C.c_void_p)))
-        _launch(dev, "magnet_mask_bwd_f32", C.byref(a))
-        return (g_pre0, *g, None, None, None, None, None, *g_preds)
+        g_pre0, *g = mask_bwd(grad_loss, packed, saved, ctx.shape, need[:7], need[12:])
+        return (g_pre0, *g[:6], None, None, None, None, None, *g[6:])
+
+
+MASK_WEIGHT_NAMES = ("W1", "b1", "W2", "b2", "W3", "b3")
+
+
+def mask_weight_shapes():
+    """(name, shape) of the fused mask head's trained tensors W1, b1, W2, b2, W3, b3."""
+    hid, nout = _lib.MAGNET_HIDDEN_CHANNELS, 9 * 4 * 4
+    return tuple(zip(MASK_WEIGHT_NAMES, ((hid, hid, 1, 1), (hid,), (hid, hid, 1, 1), (hid,), (nout, hid, 1, 1), (nout,))))
+
+
+def loss_weights(gamma: float, P: int) -> list:
+    """MagnetLoss's weight gamma^(P-i-1) of prediction i (utils/losses.py:50), as Python floats."""
+    return [gamma ** (P - i - 1) for i in range(P)]
+
+
+def mask_saved_floats(P: int, B: int, H: int, W: int, save_maps: bool) -> int:
+    """Floats of the `saved` buffer of the fused mask-loss forward: the prediction gradients, then the maps only when a
+    layer gradient needs them."""
+    return int(lib().magnet_mask_saved_bytes(P, B, H, W)) // 4 if save_maps else 2 * P * B * H * W
+
+
+def mask_train_fwd(pre0, weights, preds, gt, gt_mask_u8, save_maps: bool, pred_grad: bool, scales):
+    """The forward of ``MaskLossTrain``: the weights W1, b1, W2, b2, W3, b3 packed for training, then the fused forward
+    (two launches).  ``scales``: the P prediction scales gamma_p / count, a list of host floats, or a (P,) float32 device
+    tensor that the kernel reads when it runs (magnet_mask_train_fwd_dev_f32).  Returns (loss partials
+    [tiles x P], packed weights, saved)."""
+    P = len(preds)
+    if not 1 <= P <= _lib.MAGNET_MASK_MAX_PRED:
+        raise _lib.MagnetError(f"the fused mask-head loss takes 1 to {_lib.MAGNET_MASK_MAX_PRED} predictions, got {P}")
+    pre0 = _need_hidden("pre0", pre0.detach())
+    B, _, H, W = pre0.shape
+    shapes = mask_weight_shapes()
+    ws = _need_weights([(nm, t, shp) for (nm, shp), t in zip(shapes, weights)])
+    ps = _need_preds("preds", (p.detach() for p in preds), (B, 2, H, W))
+    gt = _need_cuda_f32("gt", gt.detach(), (B, 1, 4 * H, 4 * W))
+    gt_mask_u8 = _need_cuda_u8_mask("gt_mask", gt_mask_u8, (B, 1, 4 * H, 4 * W), "(B,1,4H,4W)")
+    dev = _same_device(("pre0", pre0), ("gt", gt), ("gt_mask", gt_mask_u8),
+                       *((nm, t) for (nm, _), t in zip(shapes, ws)), *((f"preds[{i}]", p) for i, p in enumerate(ps)))
+    on_device = isinstance(scales, torch.Tensor)
+    if on_device:
+        scales = _need_cuda_f32("scales", scales, (P,))
+        _same_device(("pre0", pre0), ("scales", scales))
+        host_scale = None
+    else:
+        host_scale = (C.c_float * P)(*scales)
+    pp = (C.c_void_p * P)(*[p.data_ptr() for p in ps])
+    packed = torch.empty(int(lib().magnet_mask_train_weights_bytes(4)), device=dev, dtype=torch.uint8)
+    partial = torch.empty(int(lib().magnet_mask_train_partials(B, H, W)) * P, device=dev, dtype=torch.float32)
+    saved = torch.empty(mask_saved_floats(P, B, H, W, save_maps), device=dev, dtype=torch.float32)
+    a = _lib.MaskTrainArgs(P=P, B=B, H=H, W=W, k=4, pre0=pre0.data_ptr(), packed_weights=packed.data_ptr(),
+                           pred=C.cast(pp, C.POINTER(C.c_void_p)), gt=gt.data_ptr(), gt_mask=gt_mask_u8.data_ptr(),
+                           pred_scale=None if on_device else C.cast(host_scale, C.POINTER(C.c_float)),
+                           save_maps=int(save_maps), pred_grad=int(pred_grad), partial=partial.data_ptr(),
+                           saved=saved.data_ptr())
+    _launch(dev, "magnet_mask_pack_train_weights_f32", *(t.data_ptr() for t in ws), packed.data_ptr())
+    if on_device:
+        _launch(dev, "magnet_mask_train_fwd_dev_f32", C.byref(a), scales.data_ptr())
+    else:
+        _launch(dev, "magnet_mask_train_fwd_f32", C.byref(a))
+    return partial, packed, saved
+
+
+def mask_bwd(grad_loss, packed, saved, shape, need_layers, need_preds):
+    """The backward of ``MaskLossTrain`` (one magnet_mask_bwd_f32 call) for (P, B, H, W) = ``shape``: -> [grad of pre0,
+    of W1, b1, W2, b2, W3, b3, then of each prediction].  ``need_layers``: 7 flags (pre0 and the six tensors),
+    ``need_preds``: P flags; a gradient not needed is None.  The upstream gradient stays on the device."""
+    P, B, H, W = shape
+    dev = saved.device
+    new = lambda shp: torch.empty(shp, device=dev, dtype=torch.float32)
+    g_pre0 = new((B, _lib.MAGNET_HIDDEN_CHANNELS, H, W)) if need_layers[0] else None
+    g = [new(shp) if n else None for (_, shp), n in zip(mask_weight_shapes(), need_layers[1:7])]
+    g_preds = [new((B, 2, H, W)) if need_preds[i] else None for i in range(P)]
+    grad_scale = grad_loss.detach().to(device=dev, dtype=torch.float32).reshape(1).contiguous()
+    nws = int(lib().magnet_mask_bwd_workspace_bytes(B, H, W)) if any(need_layers) else 256
+    ws = torch.empty(nws, device=dev, dtype=torch.uint8)
+    gp = (C.c_void_p * P)(*[_ptr(t) for t in g_preds])
+    a = _lib.MaskTrainArgs(P=P, B=B, H=H, W=W, k=4, packed_weights=packed.data_ptr(), saved=saved.data_ptr(),
+                           grad_scale=grad_scale.data_ptr(), workspace=ws.data_ptr(), grad_pre0=_ptr(g_pre0),
+                           grad_w1=_ptr(g[0]), grad_b1=_ptr(g[1]), grad_w2=_ptr(g[2]), grad_b2=_ptr(g[3]),
+                           grad_w3=_ptr(g[4]), grad_b3=_ptr(g[5]), grad_pred=C.cast(gp, C.POINTER(C.c_void_p)))
+    _launch(dev, "magnet_mask_bwd_f32", C.byref(a))
+    return [g_pre0, *g, *g_preds]
+
+
+def device_scales(num: torch.Tensor, count: torch.Tensor) -> torch.Tensor:
+    """num / count on the device, as the host forms float(num / float(count)): a float64 division rounded once to
+    float32; 0 where count is 0, so that an empty mask gives exactly zero gradients."""
+    count = count.to(torch.float64)
+    q = num.to(torch.float64) / torch.where(count > 0, count, torch.ones_like(count))
+    return torch.where(count > 0, q, torch.zeros_like(q)).to(torch.float32)
+
+
+def loss_term(partial_sum: torch.Tensor, count: torch.Tensor) -> torch.Tensor:
+    """The float64 sum of a loss's partials over the device count of supervised pixels, with the arithmetic of the eager
+    ``partial_sum.to(float32) / float(count)``: torch divides a CUDA tensor by a host scalar as a product with the scalar's
+    fp32 reciprocal.  NaN for a count of 0 (0 * inf), as a mean over an empty selection."""
+    return partial_sum.to(torch.float32) * torch.reciprocal(count.to(torch.float32))
 
 
 def mask_head_loss(pre0, mask_head, preds, gt, gt_mask, k: int = 4, gamma: float = 0.8):
@@ -1090,11 +1183,16 @@ def mask_head_loss(pre0, mask_head, preds, gt, gt_mask, k: int = 4, gamma: float
         raise _lib.MagnetError("mask_head_loss needs at least one prediction")
     _check_k4(k)
     gtm = gt_mask.to(torch.uint8)
+    ws = (c1.weight, c1.bias, c2.weight, c2.bias, c3.weight, c3.bias)
+    if _traced():                          # the count stays on the device; an empty mask gives a NaN loss
+        grad = torch.is_grad_enabled()
+        save_maps = grad and any(t.requires_grad for t in (pre0, *ws))
+        pred_grad = grad and any(p.requires_grad for p in preds)
+        return _op("mask_train_fwd")(pre0, *ws, gt, gtm, gtm.sum(), preds, float(gamma), save_maps, pred_grad)[0]
     count = int(gtm.sum().item())          # one host read per step, as magnet_loss
     if count == 0:
         raise _lib.MagnetError("gt_mask selects no pixel")
-    return MaskLossTrain.apply(pre0, c1.weight, c1.bias, c2.weight, c2.bias, c3.weight, c3.bias, gt, gtm, 4, gamma,
-                               count, *preds)
+    return MaskLossTrain.apply(pre0, *ws, gt, gtm, 4, gamma, count, *preds)
 
 
 class UpsampleNLL(torch.autograd.Function):
@@ -1107,16 +1205,7 @@ class UpsampleNLL(torch.autograd.Function):
         depth = _need_cuda_f32("depth", depth)
         up_mask = _need_cuda_f32("up_mask", up_mask)
         gt = _need_cuda_f32("gt", gt)
-        B, CH, H, W = depth.shape
-        if CH != 2:
-            raise _lib.MagnetError(f"depth must be (B,2,H,W) [mu, sigma], got {tuple(depth.shape)}")
-        _expect("up_mask", up_mask, (B, 9 * k * k, H, W))
-        _expect("gt", gt, (B, 1, k * H, k * W))
-        gt_mask_u8 = _need_cuda_u8_mask("gt_mask", gt_mask_u8, (B, 1, k * H, k * W), "(B,1,k*H,k*W)")
-        dev = _same_device(("depth", depth), ("up_mask", up_mask), ("gt", gt), ("gt_mask", gt_mask_u8))
-        partial = torch.empty(lib().magnet_upsample_nll_partials(B, H, W, k), device=dev, dtype=torch.float32)
-        _launch(dev, "magnet_upsample_nll_fwd_f32", depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(),
-                gt_mask_u8.data_ptr(), B, H, W, k, partial.data_ptr())
+        partial, gt_mask_u8 = upsample_nll_fwd(depth, up_mask, gt, gt_mask_u8, k)
         ctx.save_for_backward(depth, up_mask, gt, gt_mask_u8)
         ctx.k, ctx.count = k, float(count)
         return partial.sum(dtype=torch.float64).to(torch.float32) / ctx.count
@@ -1124,24 +1213,59 @@ class UpsampleNLL(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out):
         depth, up_mask, gt, gtm = ctx.saved_tensors
-        B, _, H, W = depth.shape
-        g_depth = torch.zeros_like(depth)
-        g_mask = torch.empty_like(up_mask)
-        scale = float(grad_out) / ctx.count
+        return (*upsample_nll_bwd(depth, up_mask, gt, gtm, ctx.k, float(grad_out) / ctx.count), None, None, None, None)
+
+
+def upsample_nll_fwd(depth, up_mask, gt, gt_mask_u8, k: int):
+    """The forward kernel of ``UpsampleNLL`` on checked fp32 operands: -> (per-CTA NLL partial sums, the checked mask)."""
+    depth, up_mask, gt = _need_cuda_f32("depth", depth), _need_cuda_f32("up_mask", up_mask), _need_cuda_f32("gt", gt)
+    B, CH, H, W = depth.shape
+    if CH != 2:
+        raise _lib.MagnetError(f"depth must be (B,2,H,W) [mu, sigma], got {tuple(depth.shape)}")
+    _expect("up_mask", up_mask, (B, 9 * k * k, H, W))
+    _expect("gt", gt, (B, 1, k * H, k * W))
+    gt_mask_u8 = _need_cuda_u8_mask("gt_mask", gt_mask_u8, (B, 1, k * H, k * W), "(B,1,k*H,k*W)")
+    dev = _same_device(("depth", depth), ("up_mask", up_mask), ("gt", gt), ("gt_mask", gt_mask_u8))
+    partial = torch.empty(lib().magnet_upsample_nll_partials(B, H, W, k), device=dev, dtype=torch.float32)
+    _launch(dev, "magnet_upsample_nll_fwd_f32", depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(),
+            gt_mask_u8.data_ptr(), B, H, W, k, partial.data_ptr())
+    return partial, gt_mask_u8
+
+
+def upsample_nll_bwd(depth, up_mask, gt, gt_mask_u8, k: int, scale):
+    """The gradients of ``UpsampleNLL`` w.r.t. (depth, up_mask) at ``scale`` = upstream gradient / count: a host float
+    (magnet_upsample_nll_bwd_f32), or a 1-element float32 device tensor the kernel reads when it runs
+    (magnet_upsample_nll_bwd_dev_f32)."""
+    depth, up_mask, gt = _need_cuda_f32("depth", depth), _need_cuda_f32("up_mask", up_mask), _need_cuda_f32("gt", gt)
+    B, _, H, W = depth.shape
+    g_depth = torch.zeros_like(depth)
+    g_mask = torch.empty_like(up_mask)
+    if isinstance(scale, torch.Tensor):
+        scale = _need_cuda_f32("scale", scale.reshape(1))
+        _launch(depth.device, "magnet_upsample_nll_bwd_dev_f32", depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(),
+                gt_mask_u8.data_ptr(), scale.data_ptr(), B, H, W, k, g_depth.data_ptr(), g_mask.data_ptr())
+    else:
         _launch(depth.device, "magnet_upsample_nll_bwd_f32", depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(),
-                gtm.data_ptr(), scale, B, H, W, ctx.k, g_depth.data_ptr(), g_mask.data_ptr())
-        return g_depth, g_mask, None, None, None, None
+                gt_mask_u8.data_ptr(), scale, B, H, W, k, g_depth.data_ptr(), g_mask.data_ptr())
+    return g_depth, g_mask
 
 
 def magnet_loss(pred_list, up_mask, gt, gt_mask, k: int, gamma: float = 0.8):
     """MagnetLoss 'gaussian' (utils/losses.py:34-50) on the QUARTER-RESOLUTION predictions of the matching loop and the
     shared upsampling mask: sum_i gamma^(n-i-1) * mean NLL(upsample(pred_i)), each term one fused kernel (f-2).
-    pred_list: the (B,2,H,W) Gaussians pred_1..pred_n; gt (B,1,kH,kW); gt_mask bool / uint8 of the same shape."""
+    pred_list: the (B,2,H,W) Gaussians pred_1..pred_n; gt (B,1,kH,kW); gt_mask bool / uint8 of the same shape.
+    Under torch.compile the count stays on the device and an empty mask gives a NaN loss (eager raises)."""
     gtm = gt_mask.to(torch.uint8)
+    n = len(pred_list)
+    if _traced():
+        count = gtm.sum()
+        loss = 0.0
+        for i, pred in enumerate(pred_list):
+            loss = loss + _op("upsample_nll_fwd")(pred, up_mask, gt, gtm, int(k), count, gamma ** (n - i - 1))
+        return loss
     count = int(gtm.sum().item())          # one host read per step; the reference's boolean indexing syncs 3x per term
     if count == 0:
         raise _lib.MagnetError("gt_mask selects no pixel")
-    n = len(pred_list)
     loss = 0.0
     for i, pred in enumerate(pred_list):
         loss = loss + gamma ** (n - i - 1) * UpsampleNLL.apply(pred, up_mask, gt, gtm, k, count)
@@ -1159,16 +1283,7 @@ class FnetL1Loss(torch.autograd.Function):
         gt = _need_cuda_f32("gt", gt)
         if scores.dim() != 4:
             raise _lib.MagnetError(f"scores must be (B,D,H,W), got {tuple(scores.shape)}")
-        B, D, H, W = scores.shape
-        karr = planes if isinstance(planes, C.Array) else k_array(planes)
-        if len(karr) != D:
-            raise _lib.MagnetError(f"{len(karr)} plane depths for {D} score planes")
-        _expect("gt", gt, (B, 1, H, W))
-        mask_u8 = _need_cuda_u8_mask("mask", mask_u8, (B, 1, H, W), "(B,1,H,W)")
-        dev = _same_device(("scores", scores), ("gt", gt), ("mask", mask_u8))
-        partial = torch.empty(lib().magnet_fnet_l1_partials(B, H, W), device=dev, dtype=torch.float32)
-        _launch(dev, "magnet_fnet_l1_fwd_f32", scores.data_ptr(), C.cast(karr, C.c_void_p), gt.data_ptr(),
-                mask_u8.data_ptr(), B, D, H, W, partial.data_ptr())
+        partial, karr, scores, gt, mask_u8 = fnet_l1_fwd(scores, planes, gt, mask_u8)
         ctx.save_for_backward(scores, gt, mask_u8)
         ctx.karr, ctx.count = karr, count
         return partial.sum(dtype=torch.float64).to(torch.float32) / count
@@ -1176,24 +1291,58 @@ class FnetL1Loss(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out):
         scores, gt, mask_u8 = ctx.saved_tensors
-        B, D, H, W = scores.shape
-        g = torch.empty_like(scores)
         # the upstream gradient stays on the device (no host read: the step can be captured in a CUDA graph)
         if isinstance(ctx.count, torch.Tensor):
-            gs, scale = (grad_out / ctx.count).to(torch.float32).contiguous(), 1.0
+            gs, scale = (grad_out / ctx.count).to(torch.float32), 1.0
         else:
-            gs, scale = grad_out.to(torch.float32).contiguous(), 1.0 / float(ctx.count)
-        _launch(scores.device, "magnet_fnet_l1_bwd_f32", scores.data_ptr(), C.cast(ctx.karr, C.c_void_p), gt.data_ptr(),
-                mask_u8.data_ptr(), scale, gs.data_ptr(), B, D, H, W, g.data_ptr())
-        return g, None, None, None, None
+            gs, scale = grad_out.to(torch.float32), 1.0 / float(ctx.count)
+        return fnet_l1_bwd(scores, ctx.karr, gt, mask_u8, scale, gs), None, None, None, None
+
+
+def fnet_l1_fwd(scores, planes, gt, mask_u8):
+    """The forward kernel of ``FnetL1Loss``: -> (per-CTA L1 partial sums, the host plane array, and the checked scores,
+    gt and mask the backward reads)."""
+    scores = _need_cuda_f32("scores", scores)
+    gt = _need_cuda_f32("gt", gt)
+    if scores.dim() != 4:
+        raise _lib.MagnetError(f"scores must be (B,D,H,W), got {tuple(scores.shape)}")
+    B, D, H, W = scores.shape
+    karr = planes if isinstance(planes, C.Array) else k_array(planes)
+    if len(karr) != D:
+        raise _lib.MagnetError(f"{len(karr)} plane depths for {D} score planes")
+    _expect("gt", gt, (B, 1, H, W))
+    mask_u8 = _need_cuda_u8_mask("mask", mask_u8, (B, 1, H, W), "(B,1,H,W)")
+    dev = _same_device(("scores", scores), ("gt", gt), ("mask", mask_u8))
+    partial = torch.empty(lib().magnet_fnet_l1_partials(B, H, W), device=dev, dtype=torch.float32)
+    _launch(dev, "magnet_fnet_l1_fwd_f32", scores.data_ptr(), C.cast(karr, C.c_void_p), gt.data_ptr(),
+            mask_u8.data_ptr(), B, D, H, W, partial.data_ptr())
+    return partial, karr, scores, gt, mask_u8
+
+
+def fnet_l1_bwd(scores, planes, gt, mask_u8, scale: float, grad_scale: torch.Tensor) -> torch.Tensor:
+    """The gradient of ``FnetL1Loss`` w.r.t. the scores: one magnet_fnet_l1_bwd_f32 launch with the host ``scale`` and
+    the 1-element device ``grad_scale`` (read when the kernel runs)."""
+    scores = _need_cuda_f32("scores", scores)
+    B, D, H, W = scores.shape
+    karr = planes if isinstance(planes, C.Array) else k_array(planes)
+    gs = grad_scale.to(torch.float32).reshape(1).contiguous()
+    g = torch.empty_like(scores)
+    _launch(scores.device, "magnet_fnet_l1_bwd_f32", scores.data_ptr(), C.cast(karr, C.c_void_p), gt.data_ptr(),
+            mask_u8.data_ptr(), scale, gs.data_ptr(), B, D, H, W, g.data_ptr())
+    return g
 
 
 def fnet_l1_loss(scores, planes, gt_q, mask_q, count=None):
     """F-Net's L1 loss (train_FNet.py:96-108) on the 1/V-averaged plane-sweep scores (B,D,H,W): softmax over the D
     planes, soft-argmin depth with the plane depths ``planes``, mean |pred - gt_q| where ``mask_q`` (B,1,H,W) is set.
     ``count`` = number of supervised pixels; by default it is read from the mask (one host read, which also rejects an
-    empty mask — pass it explicitly to capture the step in a CUDA graph)."""
+    empty mask — pass it explicitly to capture the step in a CUDA graph).  Under torch.compile the count is formed on
+    the device (``count`` must then be None) and an empty mask gives a NaN loss."""
     mask_u8 = mask_q.to(torch.uint8)
+    if _traced():
+        if count is not None:
+            raise _lib.MagnetError("under torch.compile fnet_l1_loss counts the mask on the device (pass count=None)")
+        return _op("fnet_l1_fwd")(scores, k_array(planes), gt_q, mask_u8, mask_u8.sum())
     if count is None:
         count = int(mask_u8.sum().item())
         if count == 0:
