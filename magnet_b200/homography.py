@@ -26,6 +26,7 @@ magnet_cost_volume_geom_bwd_f32).
 from __future__ import annotations
 
 import contextlib
+import threading
 import weakref
 from typing import Dict, Tuple
 
@@ -44,16 +45,34 @@ class _PrepCache:
     to this key; therefore the cache is BYPASSED while the current stream is being captured (the preparation kernels
     then become part of the graph and replay with the data) and while torch.compile traces (the key reads data
     pointers, and a compiled graph replays its preparations with the data too), and ``clear_cache()`` /
-    ``prep_cache(False)`` exist for callers that refill buffers behind torch's back."""
+    ``prep_cache(False)`` exist for callers that refill buffers behind torch's back.
+
+    Entries are per stream: the key also holds the current stream of the device the preparation is made on (``device``,
+    else the first CUDA source tensor's).  A preparation is enqueued and allocated on that stream, so only calls on the
+    same stream may read it: they are ordered after its kernels, and once the entry is dropped the caching allocator
+    hands its memory only to later work of that stream.  A call on another stream prepares again.  ``capacity`` counts
+    per stream (one CW call holds four or five entries), so streams that alternate do not evict each other's entries.
+    The dict is guarded by a lock, so host threads may share the cache; the preparations themselves run outside it."""
 
     def __init__(self, capacity: int = 8):
         self.capacity = capacity
         self.enabled = True
         self._items: Dict[Tuple, Tuple[tuple, object]] = {}
+        self._lock = threading.Lock()
 
     @staticmethod
-    def _sig(tensors):
-        return tuple((t.data_ptr(), t._version, tuple(t.shape), tuple(t.stride()), str(t.device)) for t in tensors)
+    def _key(kind, tensors, extra, device):
+        if device is None:
+            device = next((t.device for t in tensors if t.is_cuda), None)
+        elif not isinstance(device, torch.device):
+            device = torch.device(device)
+        stream = None
+        if device is not None and device.type == "cuda":
+            # the raw handle: torch.cuda.current_stream builds a Stream object, several microseconds per lookup
+            index = torch.cuda.current_device() if device.index is None else device.index
+            stream = (index, torch._C._cuda_getCurrentRawStream(index))
+        sig = tuple((t.data_ptr(), t._version, tuple(t.shape), tuple(t.stride()), str(t.device)) for t in tensors)
+        return (kind, stream) + sig + tuple(extra)
 
     def _usable(self, tensors) -> bool:
         if not self.enabled or torch.compiler.is_compiling():
@@ -62,31 +81,36 @@ class _PrepCache:
             return False
         return True
 
-    def get(self, kind: str, tensors, extra=()):
+    def get(self, kind: str, tensors, extra=(), device=None):
         if not self._usable(tensors):
             return None
-        key = (kind,) + self._sig(tensors) + tuple(extra)
-        hit = self._items.get(key)
-        if hit is not None:
-            refs, value = hit
-            if all(r() is t for r, t in zip(refs, tensors)):
-                return value
-            del self._items[key]
+        key = self._key(kind, tensors, extra, device)
+        with self._lock:
+            hit = self._items.get(key)
+            if hit is not None:
+                refs, value = hit
+                if all(r() is t for r, t in zip(refs, tensors)):
+                    return value
+                del self._items[key]
         return None
 
-    def put(self, kind: str, tensors, value, extra=()):
+    def put(self, kind: str, tensors, value, extra=(), device=None):
         if not self._usable(tensors):
             return value
-        key = (kind,) + self._sig(tensors) + tuple(extra)
-        for dead in [k for k, (refs, _) in self._items.items() if any(r() is None for r in refs)]:
-            del self._items[dead]                      # drop preparations whose source tensor is gone
-        if len(self._items) >= self.capacity:
-            self._items.pop(next(iter(self._items)))
-        self._items[key] = (tuple(weakref.ref(t) for t in tensors), value)
+        key = self._key(kind, tensors, extra, device)
+        refs = tuple(weakref.ref(t) for t in tensors)
+        with self._lock:
+            for dead in [k for k, (rs, _) in self._items.items() if any(r() is None for r in rs)]:
+                del self._items[dead]                  # drop preparations whose source tensor is gone
+            same = [k for k in self._items if k[1] == key[1]]
+            if len(same) >= self.capacity:
+                del self._items[same[0]]               # the stream's oldest entry (dicts keep insertion order)
+            self._items[key] = (refs, value)
         return value
 
     def clear(self):
-        self._items.clear()
+        with self._lock:
+            self._items.clear()
 
 
 _cache = _PrepCache()
@@ -105,12 +129,12 @@ def prep_cache(enabled: bool) -> None:
 
 def _device_intrinsics(cam_intrins, device):
     intM, rays = cam_intrins['intM'], cam_intrins['unit_ray_array_2D']
-    hit = _cache.get("intr", (intM, rays), (str(device),))
+    hit = _cache.get("intr", (intM, rays), (str(device),), device)
     if hit is not None:
         return hit
     value = (intM.detach().to(device=device, dtype=torch.float32).contiguous(),
              rays.detach().to(device=device, dtype=torch.float32).contiguous())
-    return _cache.put("intr", (intM, rays), value, (str(device),))
+    return _cache.put("intr", (intM, rays), value, (str(device),), device)
 
 
 def _camera_table(cam_intrins, R, t, is_valid, device):
@@ -123,11 +147,11 @@ def _camera_table(cam_intrins, R, t, is_valid, device):
     tbase = t._base if t._base is not None else t
     src = (rbase, tbase, is_valid, cam_intrins['intM'])
     extra = (R.data_ptr(), tuple(R.shape), tuple(R.stride()), t.data_ptr(), tuple(t.shape), tuple(t.stride()))
-    hit = _cache.get("cams", src, extra)
+    hit = _cache.get("cams", src, extra, device)
     if hit is not None:
         return hit
     valid_d = is_valid.to(device=device, dtype=torch.int32)
-    return _cache.put("cams", src, ops.pack_cameras(intM_d, R, t, valid_d), extra)
+    return _cache.put("cams", src, ops.pack_cameras(intM_d, R, t, valid_d), extra, device)
 
 
 MMA_MIN_PLANES = 32   # below half a 64-hypothesis chunk the all-pairs GEMM is wasted: the gather kernel does only the needed taps

@@ -561,8 +561,12 @@ def camera_chain(grad_cams, intM, R, t):
     return grad_R, grad_t, grad_K
 
 
-def cost_launch_info(B, V, D, Cc, H, W, variant=_lib.VARIANT_AUTO):
-    """(grid CTAs, threads per CTA, dynamic smem bytes) the cost kernel would use for these sizes."""
+def cost_launch_info(B, V, D, Cc, H, W, variant=_lib.VARIANT_AUTO, device=None):
+    """(grid CTAs, threads per CTA, dynamic smem bytes) the cost kernel would use for these sizes on ``device`` (a CUDA
+    device; None: the current one).  The persistent kernels size their grid by that device's SM count."""
+    if device is not None:
+        with torch.cuda.device(device):
+            return cost_launch_info(B, V, D, Cc, H, W, variant)
     a = CostArgs()
     a.B, a.V, a.D, a.C, a.H, a.W = B, V, D, Cc, H, W
     layout = {_lib.VARIANT_TMA: _lib.SRC_PIXC, _lib.VARIANT_MMA: _lib.SRC_SPLIT16}.get(variant, _lib.SRC_TILED32)
