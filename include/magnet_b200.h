@@ -145,7 +145,8 @@ int magnet_cost_volume_f32(const magnet_cost_args* args, void* stream);
  * HALF16 buffers) hold n_src source images in any order, and view (b, v) reads image src_index[b*V + v] instead of
  * v*B + b.  The cameras stay per (b, v) and the reference operands per b.
  *   src_index: DEVICE int32 array (B, V), b*V + v order.  Every entry, also those of views with is_valid == 0, must lie
- *              in [0, n_src): the kernels do not check them (the Python layer does, on the host, before any launch).
+ *              in [0, n_src): the kernels do not check them (the Python layer does, on the host before any launch,
+ *              or on the device with magnet_check_src_index while torch.compile traces).
  *   n_src:     images in src_feat, >= 1; a SPLIT16 / HALF16 buffer is magnet_split16_bytes(n_src, H, W) /
  *              magnet_half16_bytes(n_src, H, W) bytes.
  * MAGNET_ERR_NULL for a NULL src_index, MAGNET_ERR_SHAPE for n_src < 1, MAGNET_ERR_ALIGN for a misaligned src_index.
@@ -155,6 +156,26 @@ int magnet_cost_volume_indexed_f32(const magnet_cost_args* args, const int32_t* 
 /* magnet_cost_launch_info for magnet_cost_volume_indexed_f32 (the same kernels and grid; the arguments checked alike). */
 int magnet_cost_indexed_launch_info(const magnet_cost_args* args, const int32_t* src_index, int32_t n_src,
                                     int* grid_ctas, int* block_threads, int* smem_bytes);
+
+/* Element type of the frame table magnet_check_src_index reads. */
+typedef enum magnet_index_dtype {
+  MAGNET_INDEX_I32 = 0,   /* int32_t */
+  MAGNET_INDEX_I64 = 1    /* int64_t, read as 64-bit: an entry >= 2^31 is out of range, never wrapped */
+} magnet_index_dtype;
+
+/*
+ * The range check of a frame table on the device, for callers that cannot read the table back (a CUDA graph, a
+ * torch.compile graph).  src_index: DEVICE (B, V) array, b*V + v order, of element type `dtype` (magnet_index_dtype).
+ *   index_out: DEVICE int32 (B, V), the table magnet_cost_volume_indexed_f32 may read: each entry in [0, n_src) copied,
+ *              every other entry replaced by 0.
+ *   bad:       DEVICE int32 (B,), nonzero for each b with at least one entry outside [0, n_src) (views with
+ *              is_valid == 0 count too), 0 otherwise.
+ * One kernel launch, no allocation, no host synchronisation.  MAGNET_ERR_NULL for a NULL pointer, MAGNET_ERR_SHAPE for
+ * B < 1, V < 1, n_src < 1 or B*V >= 2^31, MAGNET_ERR_UNSUPPORTED for an unknown dtype, MAGNET_ERR_ALIGN for a pointer
+ * not aligned to its element size.
+ */
+int magnet_check_src_index(const void* src_index, int32_t dtype, int32_t B, int32_t V, int32_t n_src,
+                           int32_t* index_out, int32_t* bad, void* stream);
 
 /*
  * Backward of the plane-sweep volume (est_costvolume_F) w.r.t. both feature maps — what autograd derives for

@@ -22,6 +22,7 @@ OK, ERR_NULL, ERR_SHAPE, ERR_UNSUPPORTED, ERR_CUDA, ERR_ALIGN = 0, -1, -2, -3, -
 DEPTH_VOLUME, DEPTH_GAUSS, DEPTH_PLANES = 0, 1, 2
 SRC_NCHW, SRC_TILED32, SRC_PIXC, SRC_SPLIT16, SRC_HALF16 = 0, 1, 2, 3, 4
 DTYPE_F16, DTYPE_BF16 = 0, 1
+INDEX_I32, INDEX_I64 = 0, 1
 VARIANT_AUTO, VARIANT_DIRECT, VARIANT_CELLS, VARIANT_CELLS_NOREUSE, VARIANT_TMA, VARIANT_MMA = 0, 1, 2, 3, 4, 5
 MAGNET_METRICS_MAX_PRED = 8
 MAGNET_METRICS_COLS = 13
@@ -126,6 +127,7 @@ SIGNATURES = {
     "magnet_cost_volume_f32": (_ST, [C.POINTER(CostArgs), _P]),
     "magnet_cost_volume_indexed_f32": (_ST, [C.POINTER(CostArgs), _P, _I32, _P]),
     "magnet_cost_indexed_launch_info": (_ST, [C.POINTER(CostArgs), _P, _I32, _OUT, _OUT, _OUT]),
+    "magnet_check_src_index": (_ST, [_P] + [_I32] * 4 + [_P, _P, _P]),
     "magnet_cost_volume_f_bwd_f32": (_ST, [C.POINTER(CostFBwdArgs), _P]),
     "magnet_cost_volume_bwd_f32": (_ST, [C.POINTER(CostBwdArgs), _P]),
     "magnet_cost_geom_workspace_bytes": (_SZ, [_I32] * 4),

@@ -312,6 +312,18 @@ int magnet_cost_volume_indexed_f32(const magnet_cost_args* a, const int32_t* src
   return run_cost(a, src_index, n_src, stream);
 }
 
+int magnet_check_src_index(const void* src_index, int32_t dtype, int32_t B, int32_t V, int32_t n_src,
+                           int32_t* index_out, int32_t* bad, void* stream) {
+  if (!src_index || !bad) return MAGNET_ERR_NULL;
+  int st = validate_index(index_out, n_src);       // the table the indexed forward will read
+  if (st != MAGNET_OK) return st;
+  if (B < 1 || V < 1 || (int64_t)B * V >= ((int64_t)1 << 31)) return MAGNET_ERR_SHAPE;
+  if (dtype != MAGNET_INDEX_I32 && dtype != MAGNET_INDEX_I64) return MAGNET_ERR_UNSUPPORTED;
+  const bool wide = dtype == MAGNET_INDEX_I64;
+  if (reinterpret_cast<uintptr_t>(src_index) % (wide ? 8 : 4) != 0 || misaligned4(bad)) return MAGNET_ERR_ALIGN;
+  return finish(magnet::launch_check_src_index(src_index, wide, B, V, n_src, index_out, bad, (cudaStream_t)stream), 1);
+}
+
 int magnet_cost_volume_f_bwd_f32(const magnet_cost_f_bwd_args* b, void* stream) {
   if (!b || !b->fwd) return MAGNET_ERR_NULL;
   const magnet_cost_args* a = b->fwd;

@@ -412,4 +412,32 @@ cudaError_t launch_update_bwd(const float* gout, const float* dout, const float*
   return cudaGetLastError();
 }
 
+// The frame table's range check on the device (magnet_check_src_index): one CTA per row b.  Each entry is compared in
+// its own width, so an int64 entry >= 2^31 is out of range rather than wrapped; out-of-range entries become 0 in `out`
+// and set bad[b].  Every entry and every bad[b] is written, so no memset precedes the launch.
+template <class T>
+__global__ void __launch_bounds__(128) check_src_index_kernel(const T* __restrict__ idx, int V, int n_src,
+                                                              int32_t* __restrict__ out, int32_t* __restrict__ bad) {
+  const size_t row = (size_t)blockIdx.x * V;
+  int any = 0;
+  for (int v = threadIdx.x; v < V; v += blockDim.x) {
+    const T e = idx[row + v];
+    const bool ok = e >= 0 && e < (T)n_src;
+    out[row + v] = ok ? (int32_t)e : 0;
+    any |= !ok;
+  }
+  any = __syncthreads_or(any);
+  if (threadIdx.x == 0) bad[blockIdx.x] = any;
+}
+
+cudaError_t launch_check_src_index(const void* idx, bool wide, int B, int V, int n_src, int32_t* out, int32_t* bad,
+                                   cudaStream_t st) {
+  const int threads = V >= 128 ? 128 : (V + 31) / 32 * 32;
+  if (wide)
+    check_src_index_kernel<int64_t><<<B, threads, 0, st>>>(static_cast<const int64_t*>(idx), V, n_src, out, bad);
+  else
+    check_src_index_kernel<int32_t><<<B, threads, 0, st>>>(static_cast<const int32_t*>(idx), V, n_src, out, bad);
+  return cudaGetLastError();
+}
+
 }  // namespace magnet

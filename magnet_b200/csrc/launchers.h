@@ -47,6 +47,9 @@ void cells_launch_info(int B, int H, int W, int D, int* grid, int* block, int* s
 cudaError_t launch_cost_direct(const CostParams& p, int depth_mode, int src_layout, int C, bool cw,
                                const int32_t* src_index, cudaStream_t st, int* launches);
 cudaError_t launch_softmax_planes(float* vol, int B, int D, int HW, cudaStream_t st);
+// the frame table's range check (aux_kernels.cu): `idx` int64 when `wide`, else int32
+cudaError_t launch_check_src_index(const void* idx, bool wide, int B, int V, int n_src, int32_t* out, int32_t* bad,
+                                   cudaStream_t st);
 
 // ---- source layouts ---------------------------------------------------------------------------------------------------
 size_t split16_buffer_bytes(int N, int H, int W);

@@ -154,6 +154,57 @@ def _(ref_feat, src_feat, rays, cams, V, src_layout, consistency, src_gmm, kappa
     return ref_feat.new_empty((B, D, H, W), dtype=torch.float32)
 
 
+@_op("check_src_index")
+def check_src_index(src_index: Tensor, n_src: int) -> Tuple[Tensor, Tensor]:
+    """``ops.check_src_index_device``: (int32 table with out-of-range entries replaced by 0, (B,) int32 flags)."""
+    return ops.check_src_index_device(src_index, n_src)
+
+
+@check_src_index.register_fake
+def _(src_index, n_src):
+    B, V = src_index.shape
+    return src_index.new_empty((B, V), dtype=torch.int32), src_index.new_empty((B,), dtype=torch.int32)
+
+
+@_op("cost_volume_indexed")
+def cost_volume_indexed(ref_feat: Tensor, src_feat: Tensor, rays: Tensor, cams: Tensor, V: int, src_layout: int,
+                        consistency: bool, src_gmm: Optional[Tensor], kappa: float, d_volume: Optional[Tensor],
+                        ref_gmm: Optional[Tensor], k: Optional[List[float]], planes: bool, softmax: bool, variant: int,
+                        ref_split: Optional[Tensor], src_index: Tensor, n_src: Optional[int]) -> Tensor:
+    """``cost_volume`` with view (b, v) reading source image ``src_index[b, v]`` of the n_src images the source operand
+    holds (None: as many as it holds, ``ops.source_images``).  The table is range-checked on the device, never read
+    back: the forward reads the sanitised table, and the (D, H, W) block of every sample with an entry outside
+    [0, n_src) is then set to NaN."""
+    B, C, H, W = ref_feat.shape
+    n_img = _source_images(src_layout, src_feat, C, H, W, n_src)
+    if src_index.dim() != 2 or tuple(src_index.shape) != (B, V):
+        raise _lib.MagnetError(f"src_index must have shape (B, V) = {(B, V)}, got {tuple(src_index.shape)}")
+    table, bad = ops.check_src_index_device(src_index, n_img)
+    vol = ops.cost_volume(ref_feat, src_feat, rays, cams, V=V, src_layout=src_layout, consistency=consistency,
+                          src_gmm=src_gmm, kappa=kappa, d_volume=d_volume, ref_gmm=ref_gmm, k=k, planes=planes,
+                          softmax=softmax, variant=variant, ref_split=ref_split, src_index=table, n_src=n_img,
+                          check_index=False)
+    return vol.masked_fill_((bad != 0).view(B, 1, 1, 1), float("nan"))
+
+
+def _source_images(src_layout: int, src_feat: Tensor, C, H, W, n_src: Optional[int]) -> int:
+    """The source images of an indexed volume: those the operand holds (a packed buffer's count from its size), which
+    ``n_src`` must equal when given."""
+    n_img = ops.source_images(src_layout, src_feat, int(C), int(H), int(W))
+    if n_src is not None and n_src != n_img:
+        raise _lib.MagnetError(f"n_src={n_src} does not match src_feat, which holds {n_img} source images")
+    return n_img
+
+
+@cost_volume_indexed.register_fake
+def _(ref_feat, src_feat, rays, cams, V, src_layout, consistency, src_gmm, kappa, d_volume, ref_gmm, k, planes,
+      softmax, variant, ref_split, src_index, n_src):
+    B, C, H, W = ref_feat.shape
+    _source_images(src_layout, src_feat, C, H, W, n_src)
+    D = d_volume.shape[1] if d_volume is not None else len(k)
+    return ref_feat.new_empty((B, D, H, W), dtype=torch.float32)
+
+
 @_op("gaussian_update")
 def gaussian_update(d_output: Tensor, ref_gmm: Tensor) -> Tensor:
     return ops.GaussianUpdate.apply(d_output, ref_gmm)
@@ -607,5 +658,7 @@ OPS = ("pack_cameras", "relative_poses", "camera_rays", "sample_depths", "repack
        "repack_split16", "repack_half16", "cost_volume", "gaussian_update", "pack_gnet_weights", "gnet_update",
        "convex_upsample", "pack_mask_weights", "mask_upsample", "pack_dnet_weights", "dnet_depth", "dnet_upsample",
        "plane_depth", "depth_metrics", "depth_metrics_update")
+# the frame-table path of sequence evaluation (DESIGN §3.17 / §3.18): the device-side range check and the indexed volume
+SEQUENCE_OPS = ("check_src_index", "cost_volume_indexed")
 TRAIN_OPS = ("gaussian_update_bwd", "convex_upsample_bwd", "gnet_train_fwd", "gnet_bwd", "mask_train_fwd", "mask_bwd",
              "upsample_nll_fwd", "upsample_nll_bwd", "fnet_l1_fwd", "fnet_l1_bwd", "cost_volume_f", "cost_volume_f_bwd")

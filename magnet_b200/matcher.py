@@ -79,7 +79,14 @@ class MatchingPlan:
     is_valid == 0 too: fill them with any frame).  The frames the table names are packed once each, and ``cost()`` runs
     the indexed forward (magnet_cost_volume_indexed_f32) of whatever layout ``route`` picks; its volume equals, bit for
     bit, the one of a plan over the view-major gather ``nghbr_feat[src_index.T.flatten()]``.  Forward only: the table is
-    refused when grad mode is on and a feature map, a Gaussian or a camera tensor requires grad."""
+    refused when grad mode is on and a feature map, a Gaussian or a camera tensor requires grad.
+
+    While torch.compile traces, the table is never read on the host: all S frames are packed, the table goes to the
+    device as it is and every ``cost()`` is the op ``cost_volume_indexed``, which range-checks it on the device; a
+    sample with an entry outside [0, S) gets a NaN volume (eager raises MagnetError).  The packed layouts' power-of-two
+    scale then comes from all S frames instead of the named ones, so the traced volume is the eager plan's bit for bit
+    when every frame is named (``FrameCache``, a whole sequence) and otherwise the one of ``ops.cost_volume`` on the
+    same S-frame buffer (DESIGN §3.18)."""
 
     def __init__(self, ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, is_valid, cam_intrins, *, thres: int = 5,
                  src_index: Optional[torch.Tensor] = None):
@@ -115,7 +122,8 @@ class MatchingPlan:
     @staticmethod
     def _check_indexed(ref_feat, nghbr_feat, nghbr_gmms, nghbr_poses, cam_intrins, src_index) -> None:
         """The checks of an indexed plan, all before any launch: no gradient is asked of it, the per-frame maps agree
-        and the table is (B, V) over their S frames.  Returns the table on the host."""
+        and the table is (B, V) over their S frames.  Returns the table on the host; while tracing, the table as it is
+        (its range is checked on the device, by the op each ``cost()`` runs)."""
         if torch.is_grad_enabled():
             named = dict(ref_feat=ref_feat, nghbr_feat=nghbr_feat, nghbr_gmms=nghbr_gmms, nghbr_poses=nghbr_poses,
                          intM=cam_intrins['intM'], unit_ray_array_2D=cam_intrins['unit_ray_array_2D'])
@@ -136,6 +144,8 @@ class MatchingPlan:
         if tuple(nghbr_poses.shape[:2]) != (B, V):
             raise _lib.MagnetError(f"nghbr_poses must be (B, V, 4, 4) = {(B, V, 4, 4)} like src_index, got "
                                    f"{tuple(nghbr_poses.shape)}")
+        if ops._traced():
+            return src_index
         host = src_index.cpu()
         ops.check_src_index(host, B, V, S)                 # the range, on the host
         return host
@@ -144,7 +154,10 @@ class MatchingPlan:
     def _source_frames(nghbr_feat, nghbr_gmms, src_index, dev):
         """(source maps, their Gaussians, device table) of an indexed plan: the U distinct frames the table names, in
         frame order, and the table renumbered over them.  When every frame is named (a sequence, where every frame is
-        some reference's source) the maps are taken as they are, else the U frames are gathered first."""
+        some reference's source) the maps are taken as they are, else the U frames are gathered first.  While tracing:
+        all S maps and the table as it is, on the device (one copy of a CPU table, no read)."""
+        if ops._traced():
+            return nghbr_feat, nghbr_gmms, src_index.to(dev)
         idx = src_index.to(torch.int64)
         used = torch.unique(idx)
         S = nghbr_feat.shape[0]
@@ -527,15 +540,21 @@ class MAGNET(nn.Module):
         views with is_valid == 0 name any frame).  The backbones run once per frame, under ``no_grad``; the matching
         reads the sources through the table, so each source frame is also packed once.  Returns what ``forward``
         returns for the gathered batch ``ref_img = imgs[ref_index]``, ``nghbr_imgs = imgs[src_index.T.flatten()]``
-        (view-major).  Forward only."""
+        (view-major).  Forward only.  While torch.compile traces, ``ref_index`` is range-checked on the device like
+        ``src_index`` (a (B, 1) table over the S frames): a sample with an entry outside [0, S) in either gets NaN
+        predictions, where eager raises MagnetError."""
         S = imgs.shape[0]
-        ref_index = self._frame_index(ref_index, S, imgs.device)
+        ref_index, bad = self._frame_index(ref_index, S, imgs.device)
         with torch.no_grad():
             mono_gmms, x_d3 = self.d_net(imgs)
             feat = self.f_net(imgs)
-        return self.forward_sources(feat.index_select(0, ref_index), mono_gmms.index_select(0, ref_index),
-                                    x_d3.index_select(0, ref_index), feat, mono_gmms, src_index, nghbr_poses, is_valid,
-                                    cam_intrins, mode)
+        preds = self.forward_sources(feat.index_select(0, ref_index), mono_gmms.index_select(0, ref_index),
+                                     x_d3.index_select(0, ref_index), feat, mono_gmms, src_index, nghbr_poses, is_valid,
+                                     cam_intrins, mode)
+        if bad is None:
+            return preds
+        flagged = (bad != 0).view(-1, 1, 1, 1)
+        return [p.masked_fill(flagged, float("nan")) for p in preds]
 
     def forward_sources(self, ref_feat, ref_gmms, x_d3, src_feat, src_gmms, src_index, nghbr_poses, is_valid,
                         cam_intrins, mode='test'):
@@ -546,14 +565,18 @@ class MAGNET(nn.Module):
                          cam_intrins, src_index=src_index)
 
     @staticmethod
-    def _frame_index(index, S: int, device) -> torch.Tensor:
-        """ref_index (B,) checked against the S frames, as an int64 device tensor."""
+    def _frame_index(index, S: int, device):
+        """(ref_index (B,) checked against the S frames as a device tensor, None): int64, checked on the host.  While
+        tracing: (the int32 table of ``ops.check_src_index_device``, its (B,) flags), nothing read back."""
         if not isinstance(index, torch.Tensor) or index.dim() != 1 or index.dtype not in (torch.int32, torch.int64):
             raise _lib.MagnetError("ref_index must be a (B,) int32 / int64 tensor")
+        if ops._traced():
+            table, bad = ops.check_src_index_device(index.to(device).view(-1, 1), S)
+            return table.view(-1), bad
         host = index.cpu()
         if host.numel() == 0 or int(host.min()) < 0 or int(host.max()) >= S:
             raise _lib.MagnetError(f"ref_index entries must lie in [0, {S}) (the frames of imgs)")
-        return host.to(torch.int64).to(device)
+        return host.to(torch.int64).to(device), None
 
 
 class FrameCache:
@@ -570,13 +593,21 @@ class FrameCache:
     then runs as in ``MAGNET.forward_sources``, each distinct source frame packed once.
 
     An id must name the same image for as long as it is cached: call ``clear()`` when the backbones change (unfrozen,
-    reloaded) or the ids are reused."""
+    reloaded) or the ids are reused.
 
-    def __init__(self, model: MAGNET, capacity: int = 32):
+    ``head`` replaces ``model.forward_sources`` as the head each call runs, with the same arguments: typically
+    ``torch.compile(model.forward_sources, mode="reduce-overhead")``, so the head of every sample replays one CUDA graph
+    while the cache's bookkeeping stays eager Python.  With a ``head`` the frame table is handed to it on the device
+    (copied from pinned memory without a synchronisation), since a compiled graph with a host tensor cannot be
+    captured; without one it stays on the host, where the eager plan checks it."""
+
+    def __init__(self, model: MAGNET, capacity: int = 32, head: Optional[Callable] = None):
         if capacity < 1:
             raise ValueError(f"capacity must be at least 1, got {capacity}")
         from collections import OrderedDict
         self.model, self.capacity = model, int(capacity)
+        self.head = model.forward_sources if head is None else head
+        self._table_on_device = head is not None
         self._frames = OrderedDict()
         self.backbone_images = 0                           # images the backbones have run on, over the cache's life
 
@@ -619,12 +650,13 @@ class FrameCache:
         src_ids = list(dict.fromkeys(fid for row in nghbr_ids for fid in row))
         pos = {fid: i for i, fid in enumerate(src_ids)}
         src_index = torch.tensor([[pos[fid] for fid in row] for row in nghbr_ids], dtype=torch.int32)
+        if self._table_on_device:
+            src_index = src_index.pin_memory().to(ref_img.device, non_blocking=True)
         ref = [frames[fid] for fid in ref_ids]
         src = [frames[fid] for fid in src_ids]
-        return self.model.forward_sources(torch.stack([f[2] for f in ref]), torch.stack([f[0] for f in ref]),
-                                          torch.stack([f[1] for f in ref]), torch.stack([f[2] for f in src]),
-                                          torch.stack([f[0] for f in src]), src_index, nghbr_poses, is_valid,
-                                          cam_intrins, mode)
+        return self.head(torch.stack([f[2] for f in ref]), torch.stack([f[0] for f in ref]),
+                         torch.stack([f[1] for f in ref]), torch.stack([f[2] for f in src]),
+                         torch.stack([f[0] for f in src]), src_index, nghbr_poses, is_valid, cam_intrins, mode)
 
 
 def sid_planes(min_depth: float, max_depth: float, n: int = 80, device=None) -> torch.Tensor:

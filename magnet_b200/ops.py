@@ -320,6 +320,35 @@ def check_src_index(src_index, B: int, V: int, n_src: int, *, check_range: bool 
     return src_index.to(torch.int32).contiguous()
 
 
+# element types magnet_check_src_index reads
+INDEX_DTYPES = {torch.int32: _lib.INDEX_I32, torch.int64: _lib.INDEX_I64}
+
+
+def check_src_index_device(src_index: torch.Tensor, n_src: int):
+    """The range check of a (B, V) int32 / int64 frame table on its device, without reading it back: one launch of
+    magnet_check_src_index.  Returns (table, bad): the contiguous int32 (B, V) table with every entry outside
+    [0, n_src) replaced by 0, which the indexed cost volume may read, and a (B,) int32 flag, nonzero for each row that
+    held such an entry (views with is_valid == 0 count too, as in ``check_src_index``).  An int64 entry is compared in
+    64 bits, so 2**31 is out of range rather than wrapped.  This is the check of the traced indexed path
+    (DESIGN §3.18); eager calls check on the host and never launch it."""
+    if _traced():
+        return _op("check_src_index")(src_index, int(n_src))
+    src_index = _need_cuda("src_index", src_index)
+    if src_index.dtype not in INDEX_DTYPES:
+        raise _lib.MagnetError(f"src_index must be an int32 or int64 tensor, got {src_index.dtype}")
+    if src_index.dim() != 2:
+        raise _lib.MagnetError(f"src_index must have shape (B, V), got {tuple(src_index.shape)}")
+    if n_src < 1:
+        raise _lib.MagnetError(f"an indexed cost volume needs at least one source image, got n_src={n_src}")
+    src_index = src_index.contiguous()
+    B, V = src_index.shape
+    table = torch.empty((B, V), device=src_index.device, dtype=torch.int32)
+    bad = torch.empty((B,), device=src_index.device, dtype=torch.int32)
+    _launch(src_index.device, "magnet_check_src_index", src_index.data_ptr(), INDEX_DTYPES[src_index.dtype], B, V,
+            int(n_src), table.data_ptr(), bad.data_ptr())
+    return table, bad
+
+
 def source_images(src_layout: int, src_feat, C: int, H: int, W: int) -> int:
     """Images in a source operand of ``src_layout`` for C channels at H x W: the leading dimension of an NCHW / TILED32 /
     PIXC tensor, or what the size of a SPLIT16 / HALF16 buffer holds (which must be a whole number of images)."""
@@ -328,7 +357,7 @@ def source_images(src_layout: int, src_feat, C: int, H: int, W: int) -> int:
             raise TypeError("src_feat must be a torch.Tensor")
         one = packed_bytes(src_layout, 1, H, W)
         per = packed_bytes(src_layout, 2, H, W) - one
-        n = (src_feat.numel() - one) // per + 1
+        n = (int(src_feat.numel()) - one) // per + 1      # int(): a symbolic size (a traced op's fake) is specialised
         _check_packed("src_feat", src_feat, src_layout, max(n, 1), H, W)
         return n
     shape = {_lib.SRC_NCHW: (C, H, W), _lib.SRC_TILED32: (H, (W + 31) // 32, C // 4, 32, 4),
@@ -356,13 +385,18 @@ def cost_volume(ref_feat: torch.Tensor, src_feat: torch.Tensor, rays: torch.Tens
     ``src_feat`` (and ``src_gmm``) then hold any number of source images, each packed once, and view (b, v) reads image
     ``src_index[b, v]``; ``n_src``, when given, must be the number of images they hold.  ``check_index=False`` skips the
     range check of the table (the caller has checked it).  None: the view-major operands of V*B images.
-    Under torch.compile the view-major form is the registered op ``magnet_b200::cost_volume``; the indexed form is not
-    registered (its table is range-checked on the host)."""
-    if _traced() and src_index is None:
+    Under torch.compile the view-major form is the registered op ``magnet_b200::cost_volume`` and the indexed form
+    ``magnet_b200::cost_volume_indexed``, which checks the table on the device (``check_src_index_device``) whatever
+    ``check_index`` says: a sample with an entry outside [0, n_src) gets a NaN volume instead of an exception, the
+    others are unaffected (DESIGN §3.18).  A table on the CPU is copied to the device once, in the graph."""
+    if _traced():
         _no_out_traced(out)
-        return _op("cost_volume")(ref_feat, src_feat, rays, cams, int(V), int(src_layout), bool(consistency), src_gmm,
-                                  float(kappa), d_volume, ref_gmm, None if k is None else k_array(k), bool(planes),
-                                  bool(softmax), int(variant), ref_split)
+        args = (ref_feat, src_feat, rays, cams, int(V), int(src_layout), bool(consistency), src_gmm, float(kappa),
+                d_volume, ref_gmm, None if k is None else k_array(k), bool(planes), bool(softmax), int(variant),
+                ref_split)
+        if src_index is None:
+            return _op("cost_volume")(*args)
+        return _op("cost_volume_indexed")(*args, src_index.to(ref_feat.device), None if n_src is None else int(n_src))
     ref_feat = _need_cuda("ref_feat", ref_feat) if src_layout == _lib.SRC_HALF16 else _need_cuda_f32("ref_feat", ref_feat)
     if src_layout not in PACKED_LAYOUTS:                   # the packed buffers are checked below, by their size
         src_feat = _need_cuda_f32("src_feat", src_feat)
