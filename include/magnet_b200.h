@@ -587,6 +587,25 @@ int magnet_upsample_nll_bwd_dev_f32(const float* depth, const float* up_mask, co
                                     float* grad_mask, void* stream);
 
 /*
+ * D-Net's training loss, fused — replaces, on the output of D-Net's depth and mask heads, upsample_depth_via_mask
+ * (models/submodules/D_dense_depth.py:86-100), activation_G (models/DNET.py:56-60) and DnetLoss (utils/losses.py:13-22):
+ *   var = elu(v_up) + 1 + 1e-10, var[var < 1e-10] = 1e-10, nll = (mu - gt)^2 / (2 var) + 0.5 log(var),
+ * with [mu, v_up] the convex upsampling of the RAW depth-head output raw (B,2,H,W) [mu, v], over the pixels where
+ * gt_mask != 0.  The clamp never fires for a non-NaN v (elu(v) + 1 >= 0).  Arguments, outputs, partial sums and their
+ * count (magnet_upsample_nll_partials) as the magnet_upsample_nll_* trio, with raw in place of depth and grad_raw
+ * (B,2,H,W, ACCUMULATED: the caller zeroes it) in place of grad_depth; scale = upstream gradient / number of supervised
+ * pixels.  The _dev form reads the scale from the DEVICE float *scale when the kernel runs (for CUDA graphs).  One
+ * kernel each.
+ */
+int magnet_dnet_nll_fwd_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask, int32_t B,
+                            int32_t H, int32_t W, int32_t k, float* partial, void* stream);
+int magnet_dnet_nll_bwd_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask, float scale,
+                            int32_t B, int32_t H, int32_t W, int32_t k, float* grad_raw, float* grad_mask, void* stream);
+int magnet_dnet_nll_bwd_dev_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask,
+                                const float* scale, int32_t B, int32_t H, int32_t W, int32_t k, float* grad_raw,
+                                float* grad_mask, void* stream);
+
+/*
  * F-Net training loss, fused — replaces train_FNet.py:96-108 on the 1/V-averaged scores of the plane-sweep volume
  * (magnet_cost_volume_f32 with softmax == 0, depth_mode MAGNET_DEPTH_PLANES):
  *   prob = softmax over the D planes, pred = sum_j prob_j * planes_host[j], l1 = |pred - gt| where mask != 0.

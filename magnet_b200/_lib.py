@@ -150,6 +150,9 @@ SIGNATURES = {
     "magnet_upsample_nll_fwd_f32": (_ST, [_P] * 4 + [_I32] * 4 + [_P, _P]),
     "magnet_upsample_nll_bwd_f32": (_ST, [_P] * 4 + [_F32] + [_I32] * 4 + [_P, _P, _P]),
     "magnet_upsample_nll_bwd_dev_f32": (_ST, [_P] * 5 + [_I32] * 4 + [_P, _P, _P]),
+    "magnet_dnet_nll_fwd_f32": (_ST, [_P] * 4 + [_I32] * 4 + [_P, _P]),
+    "magnet_dnet_nll_bwd_f32": (_ST, [_P] * 4 + [_F32] + [_I32] * 4 + [_P, _P, _P]),
+    "magnet_dnet_nll_bwd_dev_f32": (_ST, [_P] * 5 + [_I32] * 4 + [_P, _P, _P]),
     "magnet_fnet_l1_partials": (_ST, [_I32] * 3),
     "magnet_fnet_l1_fwd_f32": (_ST, [_P] * 4 + [_I32] * 4 + [_P, _P]),
     "magnet_fnet_l1_bwd_f32": (_ST, [_P] * 4 + [_F32, _P] + [_I32] * 4 + [_P, _P]),

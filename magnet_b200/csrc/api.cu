@@ -229,6 +229,31 @@ int validate_depth_metrics_nearest_shape(const magnet_depth_metrics_nearest_args
   return validate_box(a->H, a->W, a->row0, a->row1, a->col0, a->col1);
 }
 
+// The upsample + NLL losses (magnet_upsample_nll_* with MagnetLoss's variance, magnet_dnet_nll_* with DnetLoss's):
+// one launch each, checked the same way.  Grid: W*k / 128 x H*k x B.
+bool upsample_nll_shape_ok(int32_t B, int32_t H, int32_t W, int32_t k) {
+  return B > 0 && H > 0 && W > 0 && k > 0 && B <= 65535 && (int64_t)H * k <= 65535;
+}
+
+int upsample_nll_fwd(bool dnet, const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
+                     int32_t B, int32_t H, int32_t W, int32_t k, float* partial, void* stream) {
+  if (!depth || !up_mask || !gt || !gt_mask || !partial) return MAGNET_ERR_NULL;
+  if (!upsample_nll_shape_ok(B, H, W, k)) return MAGNET_ERR_SHAPE;
+  return finish(magnet::launch_upsample_nll_fwd(dnet, depth, up_mask, gt, gt_mask, B, H, W, k, partial,
+                                                (cudaStream_t)stream), 1);
+}
+
+// scale_dev (on_device): a DEVICE float read in place of `scale` when the kernel runs
+int upsample_nll_bwd(bool dnet, const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
+                     float scale, const float* scale_dev, bool on_device, int32_t B, int32_t H, int32_t W, int32_t k,
+                     float* grad_depth, float* grad_mask, void* stream) {
+  if (!depth || !up_mask || !gt || !gt_mask || (on_device && !scale_dev) || !grad_depth || !grad_mask)
+    return MAGNET_ERR_NULL;
+  if (!upsample_nll_shape_ok(B, H, W, k)) return MAGNET_ERR_SHAPE;
+  return finish(magnet::launch_upsample_nll_bwd(dnet, depth, up_mask, gt, gt_mask, scale, scale_dev, B, H, W, k,
+                                                grad_depth, grad_mask, (cudaStream_t)stream), 1);
+}
+
 // P prediction pointers, none NULL
 bool preds_null(const float* const* pred, int P) {
   for (int p = 0; p < P; ++p)
@@ -570,28 +595,38 @@ int magnet_upsample_nll_partials(int32_t B, int32_t H, int32_t W, int32_t k) {
 
 int magnet_upsample_nll_fwd_f32(const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
                                 int32_t B, int32_t H, int32_t W, int32_t k, float* partial, void* stream) {
-  if (!depth || !up_mask || !gt || !gt_mask || !partial) return MAGNET_ERR_NULL;
-  if (B <= 0 || H <= 0 || W <= 0 || k <= 0 || B > 65535 || H * k > 65535) return MAGNET_ERR_SHAPE;
-  return finish(magnet::launch_upsample_nll_fwd(depth, up_mask, gt, gt_mask, B, H, W, k, partial, (cudaStream_t)stream),
-                1);
+  return upsample_nll_fwd(false, depth, up_mask, gt, gt_mask, B, H, W, k, partial, stream);
 }
 
 int magnet_upsample_nll_bwd_f32(const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
                                 float scale, int32_t B, int32_t H, int32_t W, int32_t k, float* grad_depth,
                                 float* grad_mask, void* stream) {
-  if (!depth || !up_mask || !gt || !gt_mask || !grad_depth || !grad_mask) return MAGNET_ERR_NULL;
-  if (B <= 0 || H <= 0 || W <= 0 || k <= 0 || B > 65535 || H * k > 65535) return MAGNET_ERR_SHAPE;
-  return finish(magnet::launch_upsample_nll_bwd(depth, up_mask, gt, gt_mask, scale, nullptr, B, H, W, k, grad_depth,
-                                                grad_mask, (cudaStream_t)stream), 1);
+  return upsample_nll_bwd(false, depth, up_mask, gt, gt_mask, scale, nullptr, false, B, H, W, k, grad_depth, grad_mask,
+                          stream);
 }
 
 int magnet_upsample_nll_bwd_dev_f32(const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
                                     const float* scale, int32_t B, int32_t H, int32_t W, int32_t k, float* grad_depth,
                                     float* grad_mask, void* stream) {
-  if (!depth || !up_mask || !gt || !gt_mask || !scale || !grad_depth || !grad_mask) return MAGNET_ERR_NULL;
-  if (B <= 0 || H <= 0 || W <= 0 || k <= 0 || B > 65535 || H * k > 65535) return MAGNET_ERR_SHAPE;
-  return finish(magnet::launch_upsample_nll_bwd(depth, up_mask, gt, gt_mask, 0.0f, scale, B, H, W, k, grad_depth,
-                                                grad_mask, (cudaStream_t)stream), 1);
+  return upsample_nll_bwd(false, depth, up_mask, gt, gt_mask, 0.0f, scale, true, B, H, W, k, grad_depth, grad_mask,
+                          stream);
+}
+
+int magnet_dnet_nll_fwd_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask, int32_t B,
+                            int32_t H, int32_t W, int32_t k, float* partial, void* stream) {
+  return upsample_nll_fwd(true, raw, up_mask, gt, gt_mask, B, H, W, k, partial, stream);
+}
+
+int magnet_dnet_nll_bwd_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask, float scale,
+                            int32_t B, int32_t H, int32_t W, int32_t k, float* grad_raw, float* grad_mask, void* stream) {
+  return upsample_nll_bwd(true, raw, up_mask, gt, gt_mask, scale, nullptr, false, B, H, W, k, grad_raw, grad_mask,
+                          stream);
+}
+
+int magnet_dnet_nll_bwd_dev_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask,
+                                const float* scale, int32_t B, int32_t H, int32_t W, int32_t k, float* grad_raw,
+                                float* grad_mask, void* stream) {
+  return upsample_nll_bwd(true, raw, up_mask, gt, gt_mask, 0.0f, scale, true, B, H, W, k, grad_raw, grad_mask, stream);
 }
 
 int magnet_fnet_l1_partials(int32_t B, int32_t H, int32_t W) {

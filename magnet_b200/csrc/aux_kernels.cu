@@ -260,6 +260,22 @@ __global__ void camera_rays_kernel(const double* __restrict__ raw, int H, int W,
 // var = max(sigma^2, 1e-10).  The (B,2,kH,kW) prediction is never written: forward emits one partial sum per CTA
 // (summed by the caller: deterministic), backward scatters straight into grad_depth / grad_mask.
 // The upsampled (mu, sigma) come from upsampled_gaussian (upsample_common.cuh), shared with the depth metrics.
+//
+// NllForm::DNET is DnetLoss (utils/losses.py:13-22) on D-Net's output (DESIGN §3.19): the second channel is the raw v
+// of the depth head, upsampled the same way, and var = activation_G(v_up) (DNET.py:56-60, activation_g) before the same
+// clamp var[var < 1e-10] = 1e-10 (dnet_var).
+enum class NllForm { MAGNET, DNET };
+
+// DnetLoss's variance of the upsampled raw v.  The clamp cannot fire unless v is NaN (which passes, as in torch):
+// expm1f is within 1 ulp, so expm1f(v) >= -1 (the float below -1 is 2 ulps of [-1, -0.5) away from any e^v - 1 > -1);
+// then expm1f(v) + 1 >= +0 exactly and activation_g(v) >= 0 + 1e-10f = 1e-10f, while torch compares the fp32 var with
+// the fp32 1e-10f.  For v <= -17.4 expm1f(v) is -1 and var is exactly 1e-10f, unclamped, with its gradient.
+__device__ __forceinline__ float dnet_var(float v) {
+  const float a = activation_g(v);
+  return a < 1e-10f ? 1e-10f : a;
+}
+
+template <NllForm F>
 __global__ void __launch_bounds__(128) upsample_nll_fwd_kernel(const float* __restrict__ depth, const float* __restrict__ mask,
                                                                 const float* __restrict__ gt, const uint8_t* __restrict__ gtm,
                                                                 int H, int W, int k, float* __restrict__ partial) {
@@ -269,9 +285,9 @@ __global__ void __launch_bounds__(128) upsample_nll_fwd_kernel(const float* __re
   if (X < W * k) {
     const size_t o = (b * H * k + Y) * (size_t)(W * k) + X;
     if (gtm[o]) {
-      float w[9], mu, sg;
+      float w[9], mu, sg;                                   // sg: sigma (MAGNET) or the raw v (DNET)
       upsampled_gaussian(depth, mask, b, H, W, k, X / k, Y / k, X % k, Y % k, w, mu, sg);
-      const float var = fmaxf(sg * sg, 1e-10f), d = mu - gt[o];
+      const float var = F == NllForm::MAGNET ? fmaxf(sg * sg, 1e-10f) : dnet_var(sg), d = mu - gt[o];
       nll = (d * d) / (2.0f * var) + 0.5f * logf(var);
     }
   }
@@ -286,7 +302,7 @@ __global__ void __launch_bounds__(128) upsample_nll_fwd_kernel(const float* __re
 
 // scale = upstream gradient * iteration weight / number of supervised pixels: the argument, or with DEV_SCALE the
 // device float *scale_dev (read at run time, so a captured graph takes it from memory)
-template <bool DEV_SCALE>
+template <NllForm F, bool DEV_SCALE>
 __global__ void __launch_bounds__(128) upsample_nll_bwd_kernel(const float* __restrict__ depth, const float* __restrict__ mask,
                                                                 const float* __restrict__ gt, const uint8_t* __restrict__ gtm,
                                                                 float scale_arg, const float* __restrict__ scale_dev, int H,
@@ -305,12 +321,22 @@ __global__ void __launch_bounds__(128) upsample_nll_bwd_kernel(const float* __re
     return;
   }
   const float scale = DEV_SCALE ? __ldg(scale_dev) : scale_arg;
-  float w[9], mu, sg;
+  float w[9], mu, sg;                                       // sg: sigma (MAGNET) or the raw v (DNET)
   upsampled_gaussian(depth, mask, b, H, W, k, x, y, kx, ky, w, mu, sg);
-  const float var = fmaxf(sg * sg, 1e-10f), d = mu - gt[o];
-  const float g_mu = scale * d / var;
-  // var[var < 1e-10] = 1e-10 (losses.py:45) cuts the gradient to sigma where it clamps
-  const float g_sg = (sg * sg < 1e-10f) ? 0.0f : scale * (1.0f / sg - (d * d) / (var * sg));
+  float g_mu, g_sg;
+  if constexpr (F == NllForm::MAGNET) {
+    const float var = fmaxf(sg * sg, 1e-10f), d = mu - gt[o];
+    g_mu = scale * d / var;
+    // var[var < 1e-10] = 1e-10 (losses.py:45) cuts the gradient to sigma where it clamps
+    g_sg = (sg * sg < 1e-10f) ? 0.0f : scale * (1.0f / sg - (d * d) / (var * sg));
+  } else {
+    const float var = dnet_var(sg), d = mu - gt[o];
+    g_mu = scale * d / var;
+    // d nll / d var times elu'(v) as ATen's elu backward forms it (exp(v) for v <= 0); zero where the clamp of
+    // losses.py:20 fires (never for a non-NaN v, dnet_var)
+    const float delu = sg <= 0.0f ? expf(sg) : 1.0f;
+    g_sg = (activation_g(sg) < 1e-10f) ? 0.0f : scale * (0.5f / var - (d * d) / (2.0f * var * var)) * delu;
+  }
   float t[9];
 #pragma unroll
   for (int i = 0; i < 9; ++i) {
@@ -330,21 +356,34 @@ __global__ void __launch_bounds__(128) upsample_nll_bwd_kernel(const float* __re
   for (int i = 0; i < 9; ++i) gmask[moff + (size_t)i * k * k * HW] = w[i] * (t[i] - dot);
 }
 
-cudaError_t launch_upsample_nll_fwd(const float* depth, const float* mask, const float* gt, const uint8_t* gtm, int B,
-                                    int H, int W, int k, float* partial, cudaStream_t st) {
+cudaError_t launch_upsample_nll_fwd(bool dnet, const float* depth, const float* mask, const float* gt, const uint8_t* gtm,
+                                    int B, int H, int W, int k, float* partial, cudaStream_t st) {
   dim3 grid((W * k + 127) / 128, H * k, B);
-  upsample_nll_fwd_kernel<<<grid, 128, 0, st>>>(depth, mask, gt, gtm, H, W, k, partial);
+  if (dnet)
+    upsample_nll_fwd_kernel<NllForm::DNET><<<grid, 128, 0, st>>>(depth, mask, gt, gtm, H, W, k, partial);
+  else
+    upsample_nll_fwd_kernel<NllForm::MAGNET><<<grid, 128, 0, st>>>(depth, mask, gt, gtm, H, W, k, partial);
   return cudaGetLastError();
 }
 
-cudaError_t launch_upsample_nll_bwd(const float* depth, const float* mask, const float* gt, const uint8_t* gtm, float scale,
-                                    const float* scale_dev, int B, int H, int W, int k, float* gdepth, float* gmask,
-                                    cudaStream_t st) {
-  dim3 grid((W * k + 127) / 128, H * k, B);
+template <NllForm F>
+static void upsample_nll_bwd(dim3 grid, const float* depth, const float* mask, const float* gt, const uint8_t* gtm,
+                             float scale, const float* scale_dev, int H, int W, int k, float* gdepth, float* gmask,
+                             cudaStream_t st) {
   if (scale_dev)
-    upsample_nll_bwd_kernel<true><<<grid, 128, 0, st>>>(depth, mask, gt, gtm, 0.0f, scale_dev, H, W, k, gdepth, gmask);
+    upsample_nll_bwd_kernel<F, true><<<grid, 128, 0, st>>>(depth, mask, gt, gtm, 0.0f, scale_dev, H, W, k, gdepth, gmask);
   else
-    upsample_nll_bwd_kernel<false><<<grid, 128, 0, st>>>(depth, mask, gt, gtm, scale, nullptr, H, W, k, gdepth, gmask);
+    upsample_nll_bwd_kernel<F, false><<<grid, 128, 0, st>>>(depth, mask, gt, gtm, scale, nullptr, H, W, k, gdepth, gmask);
+}
+
+cudaError_t launch_upsample_nll_bwd(bool dnet, const float* depth, const float* mask, const float* gt, const uint8_t* gtm,
+                                    float scale, const float* scale_dev, int B, int H, int W, int k, float* gdepth,
+                                    float* gmask, cudaStream_t st) {
+  dim3 grid((W * k + 127) / 128, H * k, B);
+  if (dnet)
+    upsample_nll_bwd<NllForm::DNET>(grid, depth, mask, gt, gtm, scale, scale_dev, H, W, k, gdepth, gmask, st);
+  else
+    upsample_nll_bwd<NllForm::MAGNET>(grid, depth, mask, gt, gtm, scale, scale_dev, H, W, k, gdepth, gmask, st);
   return cudaGetLastError();
 }
 

@@ -1,5 +1,6 @@
 // Device code of the Gaussian update shared by the stand-alone update kernel (aux_kernels.cu) and the fused G-Net
-// head (gnet_head.cu), so both produce the same bits from the same G-Net output.
+// head (gnet_head.cu), so both produce the same bits from the same G-Net output; and D-Net's variance activation,
+// shared by the fused D-Net heads (dnet_head.cu, mask_head.cu) and the D-Net loss (aux_kernels.cu).
 #pragma once
 #include <cmath>
 
@@ -28,6 +29,13 @@ __device__ __forceinline__ void gaussian_update_bwd_prev(float g_mu, float g_sg,
   const float elu = s1 > 0.0f ? s1 : __fsub_rn(expf(s1), 1.0f);
   d_mu0 = g_mu;
   d_s0 = __fadd_rn(__fmul_rn(g_mu, mu1), __fmul_rn(g_sg, __fadd_rn(__fadd_rn(elu, 1.0f), 1e-10f)));
+}
+
+// D-Net's activation_G (models/DNET.py:56-60) on the raw variance channel, in torch's order: F.elu as ATen's CUDA kernel
+// evaluates it (x <= 0 ? expm1(x) : x), then + 1.0 and + 1e-10 as two fp32 additions.  NaN stays NaN.
+__device__ __forceinline__ float activation_g(float v) {
+  const float e = v <= 0.0f ? expm1f(v) : v;
+  return __fadd_rn(__fadd_rn(e, 1.0f), 1e-10f);
 }
 
 }  // namespace magnet

@@ -5,6 +5,7 @@
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "gaussian_common.cuh"        // activation_g
 
 namespace magnet {
 
@@ -119,13 +120,6 @@ __device__ __forceinline__ void out2_layer(const float (&acc)[NTILE][4], const f
 #pragma unroll
     for (int i = 0; i < 4; ++i) r[i] = __fadd_rn(r[i], __shfl_xor_sync(0xffffffffu, r[i], o));
   }
-}
-
-// D-Net's activation_G (models/DNET.py:56-60) on the raw variance channel, in torch's order: F.elu as ATen's CUDA kernel
-// evaluates it (x <= 0 ? expm1(x) : x), then + 1.0 and + 1e-10 as two fp32 additions.  NaN stays NaN.
-__device__ __forceinline__ float activation_g(float v) {
-  const float e = v <= 0.0f ? expm1f(v) : v;
-  return __fadd_rn(__fadd_rn(e, 1.0f), 1e-10f);
 }
 
 // ---- training (DESIGN §3.10, §3.13) --------------------------------------------------------------------------------

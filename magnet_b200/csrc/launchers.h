@@ -96,12 +96,13 @@ cudaError_t launch_upsample_fwd(const float* depth, const float* mask, int B, in
                                 cudaStream_t st);
 cudaError_t launch_upsample_bwd(const float* gout, const float* depth, const float* mask, int B, int CH, int H, int W,
                                 int k, float* gdepth, float* gmask, cudaStream_t st);
-cudaError_t launch_upsample_nll_fwd(const float* depth, const float* mask, const float* gt, const uint8_t* gtm, int B,
-                                    int H, int W, int k, float* partial, cudaStream_t st);
+// dnet: DnetLoss (var = activation_G of the upsampled raw v) instead of MagnetLoss (var = sigma^2)
+cudaError_t launch_upsample_nll_fwd(bool dnet, const float* depth, const float* mask, const float* gt, const uint8_t* gtm,
+                                    int B, int H, int W, int k, float* partial, cudaStream_t st);
 // scale_dev: a DEVICE float read in place of `scale` when not NULL
-cudaError_t launch_upsample_nll_bwd(const float* depth, const float* mask, const float* gt, const uint8_t* gtm, float scale,
-                                    const float* scale_dev, int B, int H, int W, int k, float* gdepth, float* gmask,
-                                    cudaStream_t st);
+cudaError_t launch_upsample_nll_bwd(bool dnet, const float* depth, const float* mask, const float* gt, const uint8_t* gtm,
+                                    float scale, const float* scale_dev, int B, int H, int W, int k, float* gdepth,
+                                    float* gmask, cudaStream_t st);
 
 // ---- F-Net loss, plane depth, depth metrics ---------------------------------------------------------------------------
 int fnet_l1_partials(int B, int HW);

@@ -9,7 +9,8 @@ its outputs; the one that writes into an argument, ``depth_metrics_update``, dec
 
 The training launches are ops too (``TRAIN_OPS``), tied to their backward ops with ``register_autograd``: the G-Net
 head, the fused mask loss, the upsample-NLL and F-Net losses, the F volume, and the backwards of ``gaussian_update`` and
-``convex_upsample``.  What an autograd Function keeps on ``ctx`` (packed weights, saved maps) is an op output here.
+``convex_upsample``; D-Net's loss is the pair in ``DNET_TRAIN_OPS``.  What an autograd Function keeps on ``ctx``
+(packed weights, saved maps) is an op output here.
 The loss ops take the number of supervised pixels as a device tensor and normalise on the device, with the eager
 arithmetic inside the op (DESIGN §3.18), so a compiled step has no host read and can be captured in a CUDA graph.
 """
@@ -557,6 +558,49 @@ def _upsample_nll_backward(ctx, grad):
 upsample_nll_fwd.register_autograd(_upsample_nll_backward, setup_context=_upsample_nll_setup)
 
 
+# --- training: D-Net's upsample-NLL loss (DnetLoss) ------------------------------------------------------------------
+
+@_op("dnet_nll_fwd")
+def dnet_nll_fwd(raw: Tensor, up_mask: Tensor, gt: Tensor, gt_mask: Tensor, k: int, count: Tensor) -> Tensor:
+    """``UpsampleNLL(raw, up_mask, gt, gt_mask, k, count, dnet=True)`` with ``count`` on the device (NaN for count
+    0)."""
+    partial, _ = ops.upsample_nll_fwd(raw, up_mask, gt, gt_mask, k, dnet=True)
+    return ops.loss_term(partial.sum(dtype=torch.float64), count)
+
+
+@dnet_nll_fwd.register_fake
+def _(raw, up_mask, gt, gt_mask, k, count):
+    return raw.new_empty((), dtype=torch.float32)
+
+
+@_op("dnet_nll_bwd")
+def dnet_nll_bwd(grad: Tensor, raw: Tensor, up_mask: Tensor, gt: Tensor, gt_mask: Tensor, k: int,
+                 count: Tensor) -> Tuple[Tensor, Tensor]:
+    """The gradients of ``dnet_nll_fwd`` w.r.t. (raw, up_mask): the upstream gradient over ``count`` in float64, rounded
+    once to fp32 (0 for count 0), read by the kernel from device memory."""
+    scale = ops.device_scales(grad.to(torch.float32), count)
+    return ops.upsample_nll_bwd(raw, up_mask, gt, gt_mask, k, scale, dnet=True)
+
+
+@dnet_nll_bwd.register_fake
+def _(grad, raw, up_mask, gt, gt_mask, k, count):
+    return _f32(raw, *raw.shape), _f32(up_mask, *up_mask.shape)
+
+
+def _dnet_nll_setup(ctx, inputs, output):
+    raw, up_mask, gt, gt_mask, ctx.k, count = inputs
+    ctx.save_for_backward(raw, up_mask, gt, gt_mask, count)
+
+
+def _dnet_nll_backward(ctx, grad):
+    raw, up_mask, gt, gt_mask, count = ctx.saved_tensors
+    g_raw, g_mask = dnet_nll_bwd(grad, raw, up_mask, gt, gt_mask, ctx.k, count)
+    return g_raw, g_mask, None, None, None, None
+
+
+dnet_nll_fwd.register_autograd(_dnet_nll_backward, setup_context=_dnet_nll_setup)
+
+
 # --- training: F-Net's L1 loss and the F volume ----------------------------------------------------------------------
 
 @_op("fnet_l1_fwd")
@@ -662,3 +706,6 @@ OPS = ("pack_cameras", "relative_poses", "camera_rays", "sample_depths", "repack
 SEQUENCE_OPS = ("check_src_index", "cost_volume_indexed")
 TRAIN_OPS = ("gaussian_update_bwd", "convex_upsample_bwd", "gnet_train_fwd", "gnet_bwd", "mask_train_fwd", "mask_bwd",
              "upsample_nll_fwd", "upsample_nll_bwd", "fnet_l1_fwd", "fnet_l1_bwd", "cost_volume_f", "cost_volume_f_bwd")
+# D-Net training (DESIGN §3.19): the fused DnetLoss and its backward.  Training ops like TRAIN_OPS, listed apart so
+# that TRAIN_OPS stays the set of MaGNet and F-Net training launches its registration tests enumerate.
+DNET_TRAIN_OPS = ("dnet_nll_fwd", "dnet_nll_bwd")

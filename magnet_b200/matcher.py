@@ -395,6 +395,20 @@ class DnetHead(nn.Module):
         mu, v = torch.split(up, 1, dim=1)                   # activation_G (DNET.py:56-60)
         return torch.cat([mu, nn.functional.elu(v) + 1.0 + 1e-10], dim=1)
 
+    def loss(self, x_feat: torch.Tensor, gt_dmap: torch.Tensor, gt_dmap_mask: torch.Tensor) -> torch.Tensor:
+        """D-Net's training loss, ``DnetLoss(DnetHead(dnet=True)(x_feat), gt_dmap, gt_dmap_mask)`` (train_DNet.py's
+        step, utils/losses.py:13-22): both heads on cuDNN, then the learned upsampling, activation_G and the NLL as one
+        fused kernel each way (``ops.dnet_loss``, DESIGN §3.19), so the full-resolution prediction is never written.
+        Differentiable in both heads' parameters and x_feat.  gt_dmap / gt_dmap_mask (B,1,kh,kw); under torch.autocast
+        the half head outputs are upcast once here.  Eager raises ``MagnetError`` on an empty mask; compiled, that step
+        gives a NaN loss and zero gradients.  ``dnet=False`` (MaGNet's frozen D-Net) is not trained this way."""
+        if not self.dnet:
+            raise _lib.MagnetError("DnetHead.loss trains D-Net's own output (dnet=True); a dnet=False head is not "
+                                   "trained through DnetLoss")
+        raw = self.depth_head(x_feat)
+        up_mask = self.mask_head(x_feat)
+        return ops.dnet_loss(raw.float(), up_mask.float(), gt_dmap.float(), gt_dmap_mask, self.downsample_ratio)
+
 
 class MagnetHead(nn.Module):
     """G-Net + mask head + convex upsampling of the reference's ``MAGNET`` (models/MAGNET.py:100-118,

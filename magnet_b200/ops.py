@@ -1236,56 +1236,88 @@ def mask_head_loss(pre0, mask_head, preds, gt, gt_mask, k: int = 4, gamma: float
 class UpsampleNLL(torch.autograd.Function):
     """mean over the supervised pixels of the Gaussian NLL of ONE convex-upsampled prediction — upsample_depth_via_mask
     (MAGNET.py:15-27) + the per-prediction term of MagnetLoss (utils/losses.py:39-49) in one kernel each way; the
-    (B,2,kH,kW) prediction never reaches HBM.  Differentiable in depth (B,2,H,W) and up_mask (B,9k^2,H,W)."""
+    (B,2,kH,kW) prediction never reaches HBM.  Differentiable in depth (B,2,H,W) and up_mask (B,9k^2,H,W).
+    With ``dnet``: DnetLoss (utils/losses.py:13-22) instead, ``depth`` being D-Net's raw depth-head output [mu, v],
+    upsampled and passed through activation_G (DNET.py:56-60) inside the kernel (DESIGN §3.19)."""
 
     @staticmethod
-    def forward(ctx, depth, up_mask, gt, gt_mask_u8, k, count):
-        depth = _need_cuda_f32("depth", depth)
+    def forward(ctx, depth, up_mask, gt, gt_mask_u8, k, count, dnet=False):
+        depth = _need_cuda_f32("raw" if dnet else "depth", depth)
         up_mask = _need_cuda_f32("up_mask", up_mask)
         gt = _need_cuda_f32("gt", gt)
-        partial, gt_mask_u8 = upsample_nll_fwd(depth, up_mask, gt, gt_mask_u8, k)
+        partial, gt_mask_u8 = upsample_nll_fwd(depth, up_mask, gt, gt_mask_u8, k, dnet)
         ctx.save_for_backward(depth, up_mask, gt, gt_mask_u8)
-        ctx.k, ctx.count = k, float(count)
+        ctx.k, ctx.count, ctx.dnet = k, float(count), dnet
         return partial.sum(dtype=torch.float64).to(torch.float32) / ctx.count
 
     @staticmethod
     def backward(ctx, grad_out):
         depth, up_mask, gt, gtm = ctx.saved_tensors
-        return (*upsample_nll_bwd(depth, up_mask, gt, gtm, ctx.k, float(grad_out) / ctx.count), None, None, None, None)
+        grads = upsample_nll_bwd(depth, up_mask, gt, gtm, ctx.k, float(grad_out) / ctx.count, ctx.dnet)
+        return (*grads, None, None, None, None, None)
 
 
-def upsample_nll_fwd(depth, up_mask, gt, gt_mask_u8, k: int):
-    """The forward kernel of ``UpsampleNLL`` on checked fp32 operands: -> (per-CTA NLL partial sums, the checked mask)."""
-    depth, up_mask, gt = _need_cuda_f32("depth", depth), _need_cuda_f32("up_mask", up_mask), _need_cuda_f32("gt", gt)
+# the entry points (forward, backward, backward with a device scale) of the two upsample + NLL loss forms: MagnetLoss
+# of an upsampled [mu, sigma] and, with dnet=True, DnetLoss of the upsampled raw [mu, v] through activation_G
+_NLL_ENTRY = {False: ("magnet_upsample_nll_fwd_f32", "magnet_upsample_nll_bwd_f32", "magnet_upsample_nll_bwd_dev_f32"),
+              True: ("magnet_dnet_nll_fwd_f32", "magnet_dnet_nll_bwd_f32", "magnet_dnet_nll_bwd_dev_f32")}
+
+
+def upsample_nll_fwd(depth, up_mask, gt, gt_mask_u8, k: int, dnet: bool = False):
+    """The forward kernel of ``UpsampleNLL`` (DnetLoss's with ``dnet``; ``depth`` is then D-Net's raw [mu, v]) on
+    checked fp32 operands: -> (per-CTA NLL partial sums, the checked mask)."""
+    name = "raw" if dnet else "depth"
+    depth, up_mask, gt = _need_cuda_f32(name, depth), _need_cuda_f32("up_mask", up_mask), _need_cuda_f32("gt", gt)
     B, CH, H, W = depth.shape
     if CH != 2:
-        raise _lib.MagnetError(f"depth must be (B,2,H,W) [mu, sigma], got {tuple(depth.shape)}")
+        raise _lib.MagnetError(f"{name} must be (B,2,H,W) [mu, {'v' if dnet else 'sigma'}], got {tuple(depth.shape)}")
     _expect("up_mask", up_mask, (B, 9 * k * k, H, W))
     _expect("gt", gt, (B, 1, k * H, k * W))
     gt_mask_u8 = _need_cuda_u8_mask("gt_mask", gt_mask_u8, (B, 1, k * H, k * W), "(B,1,k*H,k*W)")
-    dev = _same_device(("depth", depth), ("up_mask", up_mask), ("gt", gt), ("gt_mask", gt_mask_u8))
+    dev = _same_device((name, depth), ("up_mask", up_mask), ("gt", gt), ("gt_mask", gt_mask_u8))
     partial = torch.empty(lib().magnet_upsample_nll_partials(B, H, W, k), device=dev, dtype=torch.float32)
-    _launch(dev, "magnet_upsample_nll_fwd_f32", depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(),
+    _launch(dev, _NLL_ENTRY[bool(dnet)][0], depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(),
             gt_mask_u8.data_ptr(), B, H, W, k, partial.data_ptr())
     return partial, gt_mask_u8
 
 
-def upsample_nll_bwd(depth, up_mask, gt, gt_mask_u8, k: int, scale):
-    """The gradients of ``UpsampleNLL`` w.r.t. (depth, up_mask) at ``scale`` = upstream gradient / count: a host float
-    (magnet_upsample_nll_bwd_f32), or a 1-element float32 device tensor the kernel reads when it runs
-    (magnet_upsample_nll_bwd_dev_f32)."""
-    depth, up_mask, gt = _need_cuda_f32("depth", depth), _need_cuda_f32("up_mask", up_mask), _need_cuda_f32("gt", gt)
+def upsample_nll_bwd(depth, up_mask, gt, gt_mask_u8, k: int, scale, dnet: bool = False):
+    """The gradients of ``UpsampleNLL`` (DnetLoss's with ``dnet``) w.r.t. (depth, up_mask) at ``scale`` = upstream
+    gradient / count: a host float (magnet_upsample_nll_bwd_f32 / magnet_dnet_nll_bwd_f32), or a 1-element float32
+    device tensor the kernel reads when it runs (the _dev_f32 entry points)."""
+    name = "raw" if dnet else "depth"
+    depth, up_mask, gt = _need_cuda_f32(name, depth), _need_cuda_f32("up_mask", up_mask), _need_cuda_f32("gt", gt)
     B, _, H, W = depth.shape
+    # the kernel reads the mask by address: a traced caller's mask may be strided (a permuted or channels-last bool)
+    gt_mask_u8 = _need_cuda_u8_mask("gt_mask", gt_mask_u8, (B, 1, k * H, k * W), "(B,1,k*H,k*W)")
     g_depth = torch.zeros_like(depth)
     g_mask = torch.empty_like(up_mask)
+    _, host, on_device = _NLL_ENTRY[bool(dnet)]
     if isinstance(scale, torch.Tensor):
         scale = _need_cuda_f32("scale", scale.reshape(1))
-        _launch(depth.device, "magnet_upsample_nll_bwd_dev_f32", depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(),
+        _launch(depth.device, on_device, depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(),
                 gt_mask_u8.data_ptr(), scale.data_ptr(), B, H, W, k, g_depth.data_ptr(), g_mask.data_ptr())
     else:
-        _launch(depth.device, "magnet_upsample_nll_bwd_f32", depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(),
+        _launch(depth.device, host, depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(),
                 gt_mask_u8.data_ptr(), scale, B, H, W, k, g_depth.data_ptr(), g_mask.data_ptr())
     return g_depth, g_mask
+
+
+def dnet_loss(raw, up_mask, gt, gt_mask, k: int = 4):
+    """DnetLoss 'gaussian' (utils/losses.py:13-22) of ``DNET(args)``'s output, from the heads' outputs BEFORE the
+    upsampling: raw (B,2,h,w) = the depth head's [mu, v], up_mask (B,9k^2,h,w) = the mask head's logits, gt / gt_mask
+    (B,1,kh,kw), gt_mask bool / uint8; any k >= 1.  Through ``UpsampleNLL`` with ``dnet``; fp32 operands.  Eager reads the number of
+    supervised pixels with one host read and raises on an empty mask; under torch.compile the count stays on the device
+    and an empty mask gives a NaN loss and zero gradients."""
+    if int(k) < 1:
+        raise _lib.MagnetError(f"the upsampling ratio k must be >= 1, got {k}")
+    gtm = gt_mask.to(torch.uint8)
+    if _traced():
+        return _op("dnet_nll_fwd")(raw, up_mask, gt, gtm, int(k), gtm.sum())
+    count = int(gtm.sum().item())          # one host read per step; the reference's boolean indexing syncs 3x
+    if count == 0:
+        raise _lib.MagnetError("gt_mask selects no pixel")
+    return UpsampleNLL.apply(raw, up_mask, gt, gtm, int(k), count, True)
 
 
 def magnet_loss(pred_list, up_mask, gt, gt_mask, k: int, gamma: float = 0.8):
@@ -1306,7 +1338,7 @@ def magnet_loss(pred_list, up_mask, gt, gt_mask, k: int, gamma: float = 0.8):
         raise _lib.MagnetError("gt_mask selects no pixel")
     loss = 0.0
     for i, pred in enumerate(pred_list):
-        loss = loss + gamma ** (n - i - 1) * UpsampleNLL.apply(pred, up_mask, gt, gtm, k, count)
+        loss = loss + gamma ** (n - i - 1) * UpsampleNLL.apply(pred, up_mask, gt, gtm, k, count, False)
     return loss
 
 
