@@ -187,7 +187,8 @@ int magnet_check_src_index(const void* src_index, int32_t dtype, int32_t B, int3
  *   - src_layout MAGNET_SRC_SPLIT16, variant AUTO or MMA, C == 64, V <= 16: ref_feat / src_feat are the split buffers
  *     the forward read (tensor-core kernel: both gradients as GEMMs on the fp16 hi/lo planes).  MAGNET_SRC_HALF16 in
  *     the same way, on HALF16 buffers.
- * grad_src is accumulated with atomics in either form, so results are not bit-deterministic from run to run.
+ * grad_src is accumulated with atomics in either form, so results are not bit-deterministic from run to run (the
+ * package refuses this backward under torch.use_deterministic_algorithms; DESIGN §3.20).
  */
 typedef struct magnet_cost_f_bwd_args {
   const magnet_cost_args* fwd;
@@ -213,7 +214,9 @@ int magnet_cost_volume_f_bwd_f32(const magnet_cost_f_bwd_args* args, void* strea
  *   - variant MAGNET_VARIANT_DIRECT (src_layout NCHW or TILED32): everything from the NCHW maps below, C <= 64.
  * Other forward kernels (CELLS, TMA) are rejected with MAGNET_ERR_UNSUPPORTED.  The depth gradient always comes from
  * the CUDA-core kernel; fwd->out is ignored.  Each of grad_ref, grad_src and grad_depth may be NULL when it is not wanted.
- * grad_src is accumulated with atomics, so results are not bit-deterministic from run to run.
+ * grad_src is accumulated with atomics, and the tensor-core form's coefficients with shared-memory atomics, so those
+ * results are not bit-deterministic from run to run (the package refuses them under torch.use_deterministic_algorithms;
+ * DESIGN §3.20).  grad_depth and the CUDA-core grad_ref are written in a fixed order.
  */
 typedef struct magnet_cost_bwd_args {
   const magnet_cost_args* fwd;
@@ -452,6 +455,12 @@ int magnet_mask_upsample_f32(const magnet_mask_upsample_args* args, void* stream
  * prediction and no mask is written.  Loss partials and saved maps are bit-identical from run to run; the prediction
  * gradients are sums of atomic adds.  One memset (pred_grad) and one kernel.
  *
+ * magnet_mask_train_fwd_det_f32 / magnet_mask_train_fwd_dev_det_f32 (DESIGN §3.20): the same calls with the prediction
+ * gradients (pred_grad) summed in a fixed order, so every output is bit-identical from run to run.  The kernel writes
+ * the softmax weights and the per-pixel gradients of each supervised pixel to `workspace`
+ * (magnet_mask_train_det_workspace_bytes(P,B,H,W) bytes, 16-byte aligned; required only with pred_grad) and a second
+ * kernel sums them; no memset.  P*B <= 65535 with pred_grad.  Without pred_grad they are the calls above.
+ *
  * magnet_mask_bwd_f32: given grad_scale = dL/d loss (a DEVICE float), writes grad_pre0 (B,128,H,W) = dL/d pre0,
  * grad_w1 / grad_w2 (128,128), grad_b1 / grad_b2 (128), grad_w3 (144,128), grad_b3 (144) and grad_pred[p] (B,2,H,W);
  * each may be NULL (not computed), as may grad_pred itself.  Each output is its unit-gradient value times grad_scale
@@ -476,7 +485,8 @@ typedef struct magnet_mask_train_args {
   float* partial;            /* forward: magnet_mask_train_partials(B, H, W) x P floats                              */
   float* saved;              /* magnet_mask_saved_bytes(P, B, H, W): written by the forward, read by the backward    */
   const float* grad_scale;   /* DEVICE float, the loss's upstream gradient; backward                                */
-  void* workspace;           /* magnet_mask_bwd_workspace_bytes(B, H, W); backward                                  */
+  void* workspace;           /* magnet_mask_bwd_workspace_bytes(B, H, W); backward.  _det forward with pred_grad:     */
+                             /* magnet_mask_train_det_workspace_bytes(P, B, H, W)                                   */
   float* grad_pre0;          /* (B, 128, H, W) or NULL                                                              */
   float* grad_w1;            /* (128, 128) or NULL                                                                  */
   float* grad_b1;            /* (128) or NULL                                                                       */
@@ -489,6 +499,8 @@ typedef struct magnet_mask_train_args {
 size_t magnet_mask_train_weights_bytes(int32_t k);
 size_t magnet_mask_saved_bytes(int32_t P, int32_t B, int32_t H, int32_t W);
 size_t magnet_mask_bwd_workspace_bytes(int32_t B, int32_t H, int32_t W);
+/* (9 + 2 P) * 16 * B*H*W floats; 0 for arguments the forward rejects */
+size_t magnet_mask_train_det_workspace_bytes(int32_t P, int32_t B, int32_t H, int32_t W);
 int magnet_mask_train_partials(int32_t B, int32_t H, int32_t W);
 int magnet_mask_pack_train_weights_f32(const float* w1, const float* b1, const float* w2, const float* b2,
                                        const float* w3, const float* b3, void* packed, void* stream);
@@ -496,6 +508,8 @@ int magnet_mask_train_fwd_f32(const magnet_mask_train_args* args, void* stream);
 /* magnet_mask_train_fwd_f32 with the P prediction scales read from the DEVICE array pred_scale (args->pred_scale is not
  * read) when the kernel runs, so that a captured CUDA graph takes them from memory.  Same arithmetic otherwise. */
 int magnet_mask_train_fwd_dev_f32(const magnet_mask_train_args* args, const float* pred_scale, void* stream);
+int magnet_mask_train_fwd_det_f32(const magnet_mask_train_args* args, void* stream);
+int magnet_mask_train_fwd_dev_det_f32(const magnet_mask_train_args* args, const float* pred_scale, void* stream);
 int magnet_mask_bwd_f32(const magnet_mask_train_args* args, void* stream);
 
 /*
@@ -559,10 +573,16 @@ int magnet_camera_rays_f32(const double* raw_intrinsics, int32_t B, int32_t H, i
  */
 int magnet_convex_upsample_fwd_f32(const float* depth, const float* up_mask, int32_t B, int32_t CH, int32_t H,
                                    int32_t W, int32_t k, float* out, void* stream);
-/* Backward: grad_mask (B,9*k*k,H,W) is written; grad_depth (B,CH,H,W) is ACCUMULATED (caller zeroes it). */
+/* Backward: grad_mask (B,9*k*k,H,W) is written; grad_depth (B,CH,H,W) is ACCUMULATED (caller zeroes it) with atomics,
+ * so it is not bit-deterministic from run to run (magnet_convex_upsample_bwd_det_f32 is). */
 int magnet_convex_upsample_bwd_f32(const float* grad_out, const float* depth, const float* up_mask, int32_t B,
                                    int32_t CH, int32_t H, int32_t W, int32_t k, float* grad_depth, float* grad_mask,
                                    void* stream);
+/* The fixed-order backward (DESIGN §3.20): the same arguments and grad_mask; grad_depth is WRITTEN, each element summed
+ * over its 9*k*k terms in one order, so both outputs are bit-identical from run to run.  No workspace.  Two kernels. */
+int magnet_convex_upsample_bwd_det_f32(const float* grad_out, const float* depth, const float* up_mask, int32_t B,
+                                       int32_t CH, int32_t H, int32_t W, int32_t k, float* grad_depth,
+                                       float* grad_mask, void* stream);
 
 /*
  * Convex upsampling fused with the Gaussian negative log-likelihood — replaces, per prediction of pred_list,
@@ -573,7 +593,12 @@ int magnet_convex_upsample_bwd_f32(const float* grad_out, const float* depth, co
  * forward: partial[magnet_upsample_nll_partials(B,H,W,k)] receives one partial sum of nll per CTA (the caller adds
  *   them — deterministic — and divides by the number of supervised pixels).
  * backward: scale = upstream gradient * gamma^(n-i-1) / number of supervised pixels; grad_depth (B,2,H,W) is
- *   ACCUMULATED (the caller zeroes it), grad_mask (B,9*k*k,H,W) is written.
+ *   ACCUMULATED (the caller zeroes it) with atomics, so it is not bit-deterministic from run to run; grad_mask
+ *   (B,9*k*k,H,W) is written.
+ * _det backward (DESIGN §3.20): the same arithmetic per term, with grad_depth WRITTEN and each element summed over its
+ *   terms in one order, so both outputs are bit-identical from run to run.  `workspace` holds
+ *   magnet_upsample_nll_bwd_det_workspace_bytes(B,H,W,k) bytes (the per-pixel gradients, (B,2,k*H,k*W) floats;
+ *   4-byte aligned).  Two kernels.
  */
 int magnet_upsample_nll_partials(int32_t B, int32_t H, int32_t W, int32_t k);
 int magnet_upsample_nll_fwd_f32(const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
@@ -585,6 +610,15 @@ int magnet_upsample_nll_bwd_f32(const float* depth, const float* up_mask, const 
 int magnet_upsample_nll_bwd_dev_f32(const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
                                     const float* scale, int32_t B, int32_t H, int32_t W, int32_t k, float* grad_depth,
                                     float* grad_mask, void* stream);
+/* 0 for a shape the upsample + NLL calls reject; shared by the MagnetLoss and DnetLoss _det backwards. */
+size_t magnet_upsample_nll_bwd_det_workspace_bytes(int32_t B, int32_t H, int32_t W, int32_t k);
+int magnet_upsample_nll_bwd_det_f32(const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
+                                    float scale, int32_t B, int32_t H, int32_t W, int32_t k, float* workspace,
+                                    float* grad_depth, float* grad_mask, void* stream);
+int magnet_upsample_nll_bwd_dev_det_f32(const float* depth, const float* up_mask, const float* gt,
+                                        const uint8_t* gt_mask, const float* scale, int32_t B, int32_t H, int32_t W,
+                                        int32_t k, float* workspace, float* grad_depth, float* grad_mask,
+                                        void* stream);
 
 /*
  * D-Net's training loss, fused — replaces, on the output of D-Net's depth and mask heads, upsample_depth_via_mask
@@ -595,7 +629,8 @@ int magnet_upsample_nll_bwd_dev_f32(const float* depth, const float* up_mask, co
  * count (magnet_upsample_nll_partials) as the magnet_upsample_nll_* trio, with raw in place of depth and grad_raw
  * (B,2,H,W, ACCUMULATED: the caller zeroes it) in place of grad_depth; scale = upstream gradient / number of supervised
  * pixels.  The _dev form reads the scale from the DEVICE float *scale when the kernel runs (for CUDA graphs).  One
- * kernel each.
+ * kernel each.  The _det backwards are the fixed-order forms of the magnet_upsample_nll_*_det pair, with grad_raw
+ * WRITTEN and the same workspace (magnet_upsample_nll_bwd_det_workspace_bytes); two kernels each.
  */
 int magnet_dnet_nll_fwd_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask, int32_t B,
                             int32_t H, int32_t W, int32_t k, float* partial, void* stream);
@@ -604,6 +639,12 @@ int magnet_dnet_nll_bwd_f32(const float* raw, const float* up_mask, const float*
 int magnet_dnet_nll_bwd_dev_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask,
                                 const float* scale, int32_t B, int32_t H, int32_t W, int32_t k, float* grad_raw,
                                 float* grad_mask, void* stream);
+int magnet_dnet_nll_bwd_det_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask,
+                                float scale, int32_t B, int32_t H, int32_t W, int32_t k, float* workspace,
+                                float* grad_raw, float* grad_mask, void* stream);
+int magnet_dnet_nll_bwd_dev_det_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask,
+                                    const float* scale, int32_t B, int32_t H, int32_t W, int32_t k, float* workspace,
+                                    float* grad_raw, float* grad_mask, void* stream);
 
 /*
  * F-Net training loss, fused — replaces train_FNet.py:96-108 on the 1/V-averaged scores of the plane-sweep volume

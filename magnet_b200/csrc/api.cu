@@ -243,15 +243,27 @@ int upsample_nll_fwd(bool dnet, const float* depth, const float* up_mask, const 
                                                 (cudaStream_t)stream), 1);
 }
 
-// scale_dev (on_device): a DEVICE float read in place of `scale` when the kernel runs
-int upsample_nll_bwd(bool dnet, const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
-                     float scale, const float* scale_dev, bool on_device, int32_t B, int32_t H, int32_t W, int32_t k,
-                     float* grad_depth, float* grad_mask, void* stream) {
+// scale_dev (on_device): a DEVICE float read in place of `scale` when the kernel runs; det: the fixed-order form,
+// which needs `workspace` (magnet_upsample_nll_bwd_det_workspace_bytes)
+int upsample_nll_bwd(bool dnet, bool det, const float* depth, const float* up_mask, const float* gt,
+                     const uint8_t* gt_mask, float scale, const float* scale_dev, bool on_device, int32_t B, int32_t H,
+                     int32_t W, int32_t k, float* workspace, float* grad_depth, float* grad_mask, void* stream) {
   if (!depth || !up_mask || !gt || !gt_mask || (on_device && !scale_dev) || !grad_depth || !grad_mask)
     return MAGNET_ERR_NULL;
+  if (det && !workspace) return MAGNET_ERR_NULL;
   if (!upsample_nll_shape_ok(B, H, W, k)) return MAGNET_ERR_SHAPE;
-  return finish(magnet::launch_upsample_nll_bwd(dnet, depth, up_mask, gt, gt_mask, scale, scale_dev, B, H, W, k,
-                                                grad_depth, grad_mask, (cudaStream_t)stream), 1);
+  if (det && misaligned4(workspace)) return MAGNET_ERR_ALIGN;
+  return finish(magnet::launch_upsample_nll_bwd(dnet, det, depth, up_mask, gt, gt_mask, scale, scale_dev, B, H, W, k,
+                                                workspace, grad_depth, grad_mask, (cudaStream_t)stream), det ? 2 : 1);
+}
+
+int convex_upsample_bwd(bool det, const float* grad_out, const float* depth, const float* up_mask, int32_t B, int32_t CH,
+                        int32_t H, int32_t W, int32_t k, float* grad_depth, float* grad_mask, void* stream) {
+  if (!grad_out || !depth || !up_mask || !grad_depth || !grad_mask) return MAGNET_ERR_NULL;
+  if (B <= 0 || H <= 0 || W <= 0 || k <= 0 || B > 65535 || H * k > 65535) return MAGNET_ERR_SHAPE;
+  if (CH != 1 && CH != 2) return MAGNET_ERR_UNSUPPORTED;
+  return finish(magnet::launch_upsample_bwd(grad_out, depth, up_mask, B, CH, H, W, k, det, grad_depth, grad_mask,
+                                            (cudaStream_t)stream), det ? 2 : 1);
 }
 
 // P prediction pointers, none NULL
@@ -581,11 +593,13 @@ int magnet_convex_upsample_fwd_f32(const float* depth, const float* up_mask, int
 int magnet_convex_upsample_bwd_f32(const float* grad_out, const float* depth, const float* up_mask, int32_t B,
                                    int32_t CH, int32_t H, int32_t W, int32_t k, float* grad_depth, float* grad_mask,
                                    void* stream) {
-  if (!grad_out || !depth || !up_mask || !grad_depth || !grad_mask) return MAGNET_ERR_NULL;
-  if (B <= 0 || H <= 0 || W <= 0 || k <= 0 || B > 65535 || H * k > 65535) return MAGNET_ERR_SHAPE;
-  if (CH != 1 && CH != 2) return MAGNET_ERR_UNSUPPORTED;
-  return finish(magnet::launch_upsample_bwd(grad_out, depth, up_mask, B, CH, H, W, k, grad_depth, grad_mask,
-                                            (cudaStream_t)stream), 1);
+  return convex_upsample_bwd(false, grad_out, depth, up_mask, B, CH, H, W, k, grad_depth, grad_mask, stream);
+}
+
+int magnet_convex_upsample_bwd_det_f32(const float* grad_out, const float* depth, const float* up_mask, int32_t B,
+                                       int32_t CH, int32_t H, int32_t W, int32_t k, float* grad_depth,
+                                       float* grad_mask, void* stream) {
+  return convex_upsample_bwd(true, grad_out, depth, up_mask, B, CH, H, W, k, grad_depth, grad_mask, stream);
 }
 
 int magnet_upsample_nll_partials(int32_t B, int32_t H, int32_t W, int32_t k) {
@@ -601,15 +615,35 @@ int magnet_upsample_nll_fwd_f32(const float* depth, const float* up_mask, const 
 int magnet_upsample_nll_bwd_f32(const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
                                 float scale, int32_t B, int32_t H, int32_t W, int32_t k, float* grad_depth,
                                 float* grad_mask, void* stream) {
-  return upsample_nll_bwd(false, depth, up_mask, gt, gt_mask, scale, nullptr, false, B, H, W, k, grad_depth, grad_mask,
-                          stream);
+  return upsample_nll_bwd(false, false, depth, up_mask, gt, gt_mask, scale, nullptr, false, B, H, W, k, nullptr,
+                          grad_depth, grad_mask, stream);
 }
 
 int magnet_upsample_nll_bwd_dev_f32(const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
                                     const float* scale, int32_t B, int32_t H, int32_t W, int32_t k, float* grad_depth,
                                     float* grad_mask, void* stream) {
-  return upsample_nll_bwd(false, depth, up_mask, gt, gt_mask, 0.0f, scale, true, B, H, W, k, grad_depth, grad_mask,
-                          stream);
+  return upsample_nll_bwd(false, false, depth, up_mask, gt, gt_mask, 0.0f, scale, true, B, H, W, k, nullptr,
+                          grad_depth, grad_mask, stream);
+}
+
+size_t magnet_upsample_nll_bwd_det_workspace_bytes(int32_t B, int32_t H, int32_t W, int32_t k) {
+  if (!upsample_nll_shape_ok(B, H, W, k)) return 0;
+  return (size_t)B * 2 * H * W * k * k * 4;
+}
+
+int magnet_upsample_nll_bwd_det_f32(const float* depth, const float* up_mask, const float* gt, const uint8_t* gt_mask,
+                                    float scale, int32_t B, int32_t H, int32_t W, int32_t k, float* workspace,
+                                    float* grad_depth, float* grad_mask, void* stream) {
+  return upsample_nll_bwd(false, true, depth, up_mask, gt, gt_mask, scale, nullptr, false, B, H, W, k, workspace,
+                          grad_depth, grad_mask, stream);
+}
+
+int magnet_upsample_nll_bwd_dev_det_f32(const float* depth, const float* up_mask, const float* gt,
+                                        const uint8_t* gt_mask, const float* scale, int32_t B, int32_t H, int32_t W,
+                                        int32_t k, float* workspace, float* grad_depth, float* grad_mask,
+                                        void* stream) {
+  return upsample_nll_bwd(false, true, depth, up_mask, gt, gt_mask, 0.0f, scale, true, B, H, W, k, workspace,
+                          grad_depth, grad_mask, stream);
 }
 
 int magnet_dnet_nll_fwd_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask, int32_t B,
@@ -619,14 +653,29 @@ int magnet_dnet_nll_fwd_f32(const float* raw, const float* up_mask, const float*
 
 int magnet_dnet_nll_bwd_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask, float scale,
                             int32_t B, int32_t H, int32_t W, int32_t k, float* grad_raw, float* grad_mask, void* stream) {
-  return upsample_nll_bwd(true, raw, up_mask, gt, gt_mask, scale, nullptr, false, B, H, W, k, grad_raw, grad_mask,
-                          stream);
+  return upsample_nll_bwd(true, false, raw, up_mask, gt, gt_mask, scale, nullptr, false, B, H, W, k, nullptr, grad_raw,
+                          grad_mask, stream);
 }
 
 int magnet_dnet_nll_bwd_dev_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask,
                                 const float* scale, int32_t B, int32_t H, int32_t W, int32_t k, float* grad_raw,
                                 float* grad_mask, void* stream) {
-  return upsample_nll_bwd(true, raw, up_mask, gt, gt_mask, 0.0f, scale, true, B, H, W, k, grad_raw, grad_mask, stream);
+  return upsample_nll_bwd(true, false, raw, up_mask, gt, gt_mask, 0.0f, scale, true, B, H, W, k, nullptr, grad_raw,
+                          grad_mask, stream);
+}
+
+int magnet_dnet_nll_bwd_det_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask,
+                                float scale, int32_t B, int32_t H, int32_t W, int32_t k, float* workspace,
+                                float* grad_raw, float* grad_mask, void* stream) {
+  return upsample_nll_bwd(true, true, raw, up_mask, gt, gt_mask, scale, nullptr, false, B, H, W, k, workspace, grad_raw,
+                          grad_mask, stream);
+}
+
+int magnet_dnet_nll_bwd_dev_det_f32(const float* raw, const float* up_mask, const float* gt, const uint8_t* gt_mask,
+                                    const float* scale, int32_t B, int32_t H, int32_t W, int32_t k, float* workspace,
+                                    float* grad_raw, float* grad_mask, void* stream) {
+  return upsample_nll_bwd(true, true, raw, up_mask, gt, gt_mask, 0.0f, scale, true, B, H, W, k, workspace, grad_raw,
+                          grad_mask, stream);
 }
 
 int magnet_fnet_l1_partials(int32_t B, int32_t H, int32_t W) {
@@ -766,6 +815,11 @@ size_t magnet_mask_bwd_workspace_bytes(int32_t B, int32_t H, int32_t W) {
   return magnet::mask_bwd_workspace_bytes(B, H, W);
 }
 
+size_t magnet_mask_train_det_workspace_bytes(int32_t P, int32_t B, int32_t H, int32_t W) {
+  if (P < 1 || P > MAGNET_MASK_MAX_PRED || !pixels_ok(B, H, W) || (int64_t)P * B > 65535) return 0;
+  return magnet::mask_train_det_workspace_bytes(P, B, H, W);
+}
+
 int magnet_mask_train_partials(int32_t B, int32_t H, int32_t W) {
   if (!pixels_ok(B, H, W)) return MAGNET_ERR_SHAPE;
   return magnet::mask_train_partials(B, H, W);
@@ -778,29 +832,43 @@ int magnet_mask_pack_train_weights_f32(const float* w1, const float* b1, const f
   return finish(magnet::launch_mask_pack_train(w1, b1, w2, b2, w3, b3, packed, (cudaStream_t)stream), 2);
 }
 
-// the fused mask-loss forward with its prediction scales from `scale` (host or device, `on_device`)
-static int mask_train_fwd(const magnet_mask_train_args* a, const float* scale, bool on_device, void* stream) {
+// the fused mask-loss forward with its prediction scales from `scale` (host or device, `on_device`); det: the prediction
+// gradients in a fixed order through a->workspace (magnet_mask_train_det_workspace_bytes) when a->pred_grad is set
+static int mask_train_fwd(const magnet_mask_train_args* a, const float* scale, bool on_device, bool det, void* stream) {
   const int st = validate_mask_train(a);
   if (st != MAGNET_OK) return st;
   if (!a->pre0 || !a->pred || !a->gt || !a->gt_mask || !scale || !a->partial) return MAGNET_ERR_NULL;
   if (preds_null(a->pred, a->P)) return MAGNET_ERR_NULL;
+  const bool det_pg = det && a->pred_grad != 0;
+  if (det_pg && !a->workspace) return MAGNET_ERR_NULL;
+  if (det_pg && (int64_t)a->P * a->B > 65535) return MAGNET_ERR_SHAPE;
   if (misaligned16(a->pre0)) return MAGNET_ERR_ALIGN;
   for (int p = 0; p < a->P; ++p)
     if (misaligned16(a->pred[p])) return MAGNET_ERR_ALIGN;
+  if (det_pg && misaligned16(a->workspace)) return MAGNET_ERR_ALIGN;
   int launches = 0;
   const cudaError_t e = magnet::launch_mask_train_fwd(a->P, a->B, a->H, a->W, a->pre0, a->packed_weights, a->pred,
                                                       a->gt, a->gt_mask, scale, on_device, a->save_maps != 0,
-                                                      a->pred_grad != 0, a->partial, a->saved, (cudaStream_t)stream,
-                                                      &launches);
+                                                      a->pred_grad != 0, a->partial, a->saved,
+                                                      det_pg ? static_cast<float*>(a->workspace) : nullptr,
+                                                      (cudaStream_t)stream, &launches);
   return finish(e, launches);
 }
 
 int magnet_mask_train_fwd_f32(const magnet_mask_train_args* a, void* stream) {
-  return mask_train_fwd(a, a ? a->pred_scale : nullptr, false, stream);
+  return mask_train_fwd(a, a ? a->pred_scale : nullptr, false, false, stream);
 }
 
 int magnet_mask_train_fwd_dev_f32(const magnet_mask_train_args* a, const float* pred_scale, void* stream) {
-  return mask_train_fwd(a, pred_scale, true, stream);
+  return mask_train_fwd(a, pred_scale, true, false, stream);
+}
+
+int magnet_mask_train_fwd_det_f32(const magnet_mask_train_args* a, void* stream) {
+  return mask_train_fwd(a, a ? a->pred_scale : nullptr, false, true, stream);
+}
+
+int magnet_mask_train_fwd_dev_det_f32(const magnet_mask_train_args* a, const float* pred_scale, void* stream) {
+  return mask_train_fwd(a, pred_scale, true, true, stream);
 }
 
 int magnet_mask_bwd_f32(const magnet_mask_train_args* a, void* stream) {

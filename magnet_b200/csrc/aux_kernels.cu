@@ -133,8 +133,9 @@ __global__ void convex_upsample_fwd_kernel(const float* __restrict__ depth, cons
 }
 
 // Backward of the above w.r.t. the mask logits (softmax backward, written) and the low-resolution map
-// (scatter-add with red.add into grad_depth, which the caller zeroes).
-template <int CH>
+// (scatter-add with red.add into grad_depth, which the caller zeroes).  DET: the mask gradient only; the low-resolution
+// map's gradient is then summed in a fixed order by upsample_gather_kernel.
+template <int CH, bool DET>
 __global__ void convex_upsample_bwd_kernel(const float* __restrict__ gout, const float* __restrict__ depth,
                                            const float* __restrict__ mask, int H, int W, int k,
                                            float* __restrict__ gdepth, float* __restrict__ gmask) {
@@ -164,7 +165,7 @@ __global__ void convex_upsample_bwd_kernel(const float* __restrict__ gout, const
       const int yy = y + i / 3 - 1, xx = x + i % 3 - 1;
       if (yy >= 0 && yy < H && xx >= 0 && xx < W) {
         t[i] = __fmaf_rn(g, dp[(size_t)yy * W + xx], t[i]);
-        atomicAdd(gd + (size_t)yy * W + xx, g * w[i]);
+        if (!DET) atomicAdd(gd + (size_t)yy * W + xx, g * w[i]);
       }
     }
   }
@@ -173,6 +174,72 @@ __global__ void convex_upsample_bwd_kernel(const float* __restrict__ gout, const
   for (int i = 0; i < 9; ++i) dot = __fmaf_rn(w[i], t[i], dot);
 #pragma unroll
   for (int i = 0; i < 9; ++i) gmask[moff + (size_t)i * k * k * HW] = w[i] * (t[i] - dot);
+}
+
+// The fixed-order form of the three scatters into the quarter-resolution map (DESIGN §3.20): one thread per (image z,
+// quarter-resolution pixel q) and all CH channels sums g(sub-pixel) * w(sub-pixel, tap n -> q) over the 3x3 neighbours n
+// of q in tap order and their k x k sub-pixels in row order, so the sum has one order whatever the schedule.  Each term
+// is the rounded product the scatter adds.  Image z of g (Z,CH,kH,kW) and out (Z,CH,H,W) takes the weights and gt mask of
+// image z % B.  LOGITS: w is the mask-logit tensor (B,9k^2,H,W) and each weight is its softmax, formed as the forward
+// forms it; otherwise w holds the softmax weights in that layout.  MASKED: sub-pixels where gtm (B,1,kH,kW) is 0 add
+// nothing (g is not read there).
+template <int CH, bool LOGITS, bool MASKED>
+__global__ void __launch_bounds__(128) upsample_gather_kernel(const float* __restrict__ g, const float* __restrict__ w,
+                                                              const uint8_t* __restrict__ gtm, int B, int H, int W,
+                                                              int k, float* __restrict__ out) {
+  const size_t HW = (size_t)H * W, n = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= HW) return;
+  const size_t z = blockIdx.y, b = z % B, kk = (size_t)k * k, full = HW * kk, wk = (size_t)W * k;
+  const int y = (int)(n / W), x = (int)(n % W);
+  float acc[CH];
+#pragma unroll
+  for (int c = 0; c < CH; ++c) acc[c] = 0.0f;
+#pragma unroll
+  for (int i = 0; i < 9; ++i) {
+    const int ny = y - (i / 3 - 1), nx = x - (i % 3 - 1);       // the neighbour whose tap i is q
+    if (ny < 0 || ny >= H || nx < 0 || nx >= W) continue;
+    for (int ky = 0; ky < k; ++ky) {
+      for (int kx = 0; kx < k; ++kx) {
+        const size_t o = ((size_t)ny * k + ky) * wk + (size_t)nx * k + kx;
+        if (MASKED && !gtm[b * full + o]) continue;
+        const float* wp = w + (b * 9 * kk + (size_t)ky * k + kx) * HW + (size_t)ny * W + nx;
+        float wi;
+        if constexpr (LOGITS) {
+          float m = -INFINITY;
+#pragma unroll
+          for (int j = 0; j < 9; ++j) m = fmaxf(m, wp[(size_t)j * kk * HW]);
+          float s = 0.0f, e = 0.0f;
+#pragma unroll
+          for (int j = 0; j < 9; ++j) {
+            const float t = expf(wp[(size_t)j * kk * HW] - m);
+            s += t;
+            if (j == i) e = t;
+          }
+          wi = e * (1.0f / s);
+        } else {
+          wi = wp[(size_t)i * kk * HW];
+        }
+#pragma unroll
+        for (int c = 0; c < CH; ++c) acc[c] = __fadd_rn(acc[c], __fmul_rn(g[(z * CH + c) * full + o], wi));
+      }
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < CH; ++c) out[(z * CH + c) * HW + n] = acc[c];
+}
+
+template <int CH, bool LOGITS, bool MASKED>
+static cudaError_t upsample_gather(const float* g, const float* w, const uint8_t* gtm, int Z, int B, int H, int W,
+                                   int k, float* out, cudaStream_t st) {
+  const size_t HW = (size_t)H * W;
+  upsample_gather_kernel<CH, LOGITS, MASKED><<<dim3((unsigned)((HW + 127) / 128), Z), 128, 0, st>>>(g, w, gtm, B, H, W,
+                                                                                                    k, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_mask_pred_gather(const float* g, const float* w, const uint8_t* gtm, int P, int B, int H, int W,
+                                    int k, float* gpred, cudaStream_t st) {
+  return upsample_gather<2, false, true>(g, w, gtm, P * B, B, H, W, k, gpred, st);
 }
 
 // SURVEY §8 f-4 — caller-side camera prep on the device.
@@ -302,7 +369,9 @@ __global__ void __launch_bounds__(128) upsample_nll_fwd_kernel(const float* __re
 
 // scale = upstream gradient * iteration weight / number of supervised pixels: the argument, or with DEV_SCALE the
 // device float *scale_dev (read at run time, so a captured graph takes it from memory)
-template <NllForm F, bool DEV_SCALE>
+// DET: instead of scattering into the quarter-resolution map, the per-pixel (g_mu, g_sg) are written where gt_mask is
+// set to gdepth, which then points to a (B,2,kH,kW) workspace, and upsample_gather_kernel sums them in a fixed order.
+template <NllForm F, bool DEV_SCALE, bool DET>
 __global__ void __launch_bounds__(128) upsample_nll_bwd_kernel(const float* __restrict__ depth, const float* __restrict__ mask,
                                                                 const float* __restrict__ gt, const uint8_t* __restrict__ gtm,
                                                                 float scale_arg, const float* __restrict__ scale_dev, int H,
@@ -337,6 +406,11 @@ __global__ void __launch_bounds__(128) upsample_nll_bwd_kernel(const float* __re
     const float delu = sg <= 0.0f ? expf(sg) : 1.0f;
     g_sg = (activation_g(sg) < 1e-10f) ? 0.0f : scale * (0.5f / var - (d * d) / (2.0f * var * var)) * delu;
   }
+  if constexpr (DET) {
+    const size_t full = HW * k * k, oi = (size_t)Y * (W * k) + X;
+    gdepth[(b * 2 + 0) * full + oi] = g_mu;
+    gdepth[(b * 2 + 1) * full + oi] = g_sg;
+  }
   float t[9];
 #pragma unroll
   for (int i = 0; i < 9; ++i) {
@@ -345,8 +419,10 @@ __global__ void __launch_bounds__(128) upsample_nll_bwd_kernel(const float* __re
     if (yy >= 0 && yy < H && xx >= 0 && xx < W) {
       const size_t q = (size_t)yy * W + xx;
       t[i] = __fmaf_rn(g_sg, depth[(b * 2 + 1) * HW + q], g_mu * depth[(b * 2 + 0) * HW + q]);
-      atomicAdd(gdepth + (b * 2 + 0) * HW + q, g_mu * w[i]);
-      atomicAdd(gdepth + (b * 2 + 1) * HW + q, g_sg * w[i]);
+      if constexpr (!DET) {
+        atomicAdd(gdepth + (b * 2 + 0) * HW + q, g_mu * w[i]);
+        atomicAdd(gdepth + (b * 2 + 1) * HW + q, g_sg * w[i]);
+      }
     }
   }
   float dot = 0.0f;
@@ -366,24 +442,37 @@ cudaError_t launch_upsample_nll_fwd(bool dnet, const float* depth, const float* 
   return cudaGetLastError();
 }
 
-template <NllForm F>
+template <NllForm F, bool DET>
 static void upsample_nll_bwd(dim3 grid, const float* depth, const float* mask, const float* gt, const uint8_t* gtm,
                              float scale, const float* scale_dev, int H, int W, int k, float* gdepth, float* gmask,
                              cudaStream_t st) {
   if (scale_dev)
-    upsample_nll_bwd_kernel<F, true><<<grid, 128, 0, st>>>(depth, mask, gt, gtm, 0.0f, scale_dev, H, W, k, gdepth, gmask);
+    upsample_nll_bwd_kernel<F, true, DET><<<grid, 128, 0, st>>>(depth, mask, gt, gtm, 0.0f, scale_dev, H, W, k, gdepth,
+                                                                gmask);
   else
-    upsample_nll_bwd_kernel<F, false><<<grid, 128, 0, st>>>(depth, mask, gt, gtm, scale, nullptr, H, W, k, gdepth, gmask);
+    upsample_nll_bwd_kernel<F, false, DET><<<grid, 128, 0, st>>>(depth, mask, gt, gtm, scale, nullptr, H, W, k, gdepth,
+                                                                 gmask);
 }
 
-cudaError_t launch_upsample_nll_bwd(bool dnet, const float* depth, const float* mask, const float* gt, const uint8_t* gtm,
-                                    float scale, const float* scale_dev, int B, int H, int W, int k, float* gdepth,
-                                    float* gmask, cudaStream_t st) {
+// workspace (det only): (B,2,kH,kW) floats, the per-pixel gradients the gather reads
+cudaError_t launch_upsample_nll_bwd(bool dnet, bool det, const float* depth, const float* mask, const float* gt,
+                                    const uint8_t* gtm, float scale, const float* scale_dev, int B, int H, int W, int k,
+                                    float* workspace, float* gdepth, float* gmask, cudaStream_t st) {
   dim3 grid((W * k + 127) / 128, H * k, B);
+  if (det) {
+    if (dnet)
+      upsample_nll_bwd<NllForm::DNET, true>(grid, depth, mask, gt, gtm, scale, scale_dev, H, W, k, workspace, gmask, st);
+    else
+      upsample_nll_bwd<NllForm::MAGNET, true>(grid, depth, mask, gt, gtm, scale, scale_dev, H, W, k, workspace, gmask,
+                                              st);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    return upsample_gather<2, true, true>(workspace, mask, gtm, B, B, H, W, k, gdepth, st);
+  }
   if (dnet)
-    upsample_nll_bwd<NllForm::DNET>(grid, depth, mask, gt, gtm, scale, scale_dev, H, W, k, gdepth, gmask, st);
+    upsample_nll_bwd<NllForm::DNET, false>(grid, depth, mask, gt, gtm, scale, scale_dev, H, W, k, gdepth, gmask, st);
   else
-    upsample_nll_bwd<NllForm::MAGNET>(grid, depth, mask, gt, gtm, scale, scale_dev, H, W, k, gdepth, gmask, st);
+    upsample_nll_bwd<NllForm::MAGNET, false>(grid, depth, mask, gt, gtm, scale, scale_dev, H, W, k, gdepth, gmask, st);
   return cudaGetLastError();
 }
 
@@ -407,13 +496,25 @@ cudaError_t launch_upsample_fwd(const float* depth, const float* mask, int B, in
   return cudaGetLastError();
 }
 
+template <int CH>
+static cudaError_t upsample_bwd(dim3 grid, const float* gout, const float* depth, const float* mask, int B, int H, int W,
+                                int k, bool det, float* gdepth, float* gmask, cudaStream_t st) {
+  if (!det) {
+    convex_upsample_bwd_kernel<CH, false><<<grid, 128, 0, st>>>(gout, depth, mask, H, W, k, gdepth, gmask);
+    return cudaGetLastError();
+  }
+  convex_upsample_bwd_kernel<CH, true><<<grid, 128, 0, st>>>(gout, depth, mask, H, W, k, gdepth, gmask);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  return upsample_gather<CH, true, false>(gout, mask, nullptr, B, B, H, W, k, gdepth, st);
+}
+
 cudaError_t launch_upsample_bwd(const float* gout, const float* depth, const float* mask, int B, int CH, int H, int W,
-                                int k, float* gdepth, float* gmask, cudaStream_t st) {
+                                int k, bool det, float* gdepth, float* gmask, cudaStream_t st) {
   dim3 grid((W * k + 127) / 128, H * k, B);
-  if (CH == 1) convex_upsample_bwd_kernel<1><<<grid, 128, 0, st>>>(gout, depth, mask, H, W, k, gdepth, gmask);
-  else if (CH == 2) convex_upsample_bwd_kernel<2><<<grid, 128, 0, st>>>(gout, depth, mask, H, W, k, gdepth, gmask);
-  else return cudaErrorInvalidValue;
-  return cudaGetLastError();
+  if (CH == 1) return upsample_bwd<1>(grid, gout, depth, mask, B, H, W, k, det, gdepth, gmask, st);
+  if (CH == 2) return upsample_bwd<2>(grid, gout, depth, mask, B, H, W, k, det, gdepth, gmask, st);
+  return cudaErrorInvalidValue;
 }
 
 cudaError_t launch_pack_cameras(const float* intM, const float* R, int64_t r_sb, int64_t r_sv, int64_t r_si,

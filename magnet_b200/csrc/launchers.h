@@ -94,15 +94,21 @@ cudaError_t launch_relative_poses(const float* ext_ref, const float* ext_nghbr, 
 cudaError_t launch_camera_rays(const double* raw, int B, int H, int W, float* intM, float* rays, cudaStream_t st);
 cudaError_t launch_upsample_fwd(const float* depth, const float* mask, int B, int CH, int H, int W, int k, float* out,
                                 cudaStream_t st);
+// det: grad_depth summed in a fixed order (written, 2 launches) instead of accumulated with atomics (1 launch)
 cudaError_t launch_upsample_bwd(const float* gout, const float* depth, const float* mask, int B, int CH, int H, int W,
-                                int k, float* gdepth, float* gmask, cudaStream_t st);
+                                int k, bool det, float* gdepth, float* gmask, cudaStream_t st);
 // dnet: DnetLoss (var = activation_G of the upsampled raw v) instead of MagnetLoss (var = sigma^2)
 cudaError_t launch_upsample_nll_fwd(bool dnet, const float* depth, const float* mask, const float* gt, const uint8_t* gtm,
                                     int B, int H, int W, int k, float* partial, cudaStream_t st);
-// scale_dev: a DEVICE float read in place of `scale` when not NULL
-cudaError_t launch_upsample_nll_bwd(bool dnet, const float* depth, const float* mask, const float* gt, const uint8_t* gtm,
-                                    float scale, const float* scale_dev, int B, int H, int W, int k, float* gdepth,
-                                    float* gmask, cudaStream_t st);
+// scale_dev: a DEVICE float read in place of `scale` when not NULL.  det: grad_depth written in a fixed order through
+// `workspace` ((B,2,kH,kW) floats, 2 launches) instead of accumulated with atomics (1 launch)
+cudaError_t launch_upsample_nll_bwd(bool dnet, bool det, const float* depth, const float* mask, const float* gt,
+                                    const uint8_t* gtm, float scale, const float* scale_dev, int B, int H, int W, int k,
+                                    float* workspace, float* gdepth, float* gmask, cudaStream_t st);
+// the fixed-order prediction gradients of the fused mask-loss forward: gpred (P*B,2,H,W) from the per-pixel gradients
+// g (P*B,2,kH,kW) and softmax weights w (B,9k^2,H,W) where gtm (B,1,kH,kW) is set
+cudaError_t launch_mask_pred_gather(const float* g, const float* w, const uint8_t* gtm, int P, int B, int H, int W,
+                                    int k, float* gpred, cudaStream_t st);
 
 // ---- F-Net loss, plane depth, depth metrics ---------------------------------------------------------------------------
 int fnet_l1_partials(int B, int HW);
@@ -158,12 +164,13 @@ size_t mask_train_weights_bytes();
 int mask_train_partials(int B, int H, int W);
 size_t mask_saved_bytes(int P, int B, int H, int W);
 size_t mask_bwd_workspace_bytes(int B, int H, int W);
+size_t mask_train_det_workspace_bytes(int P, int B, int H, int W);
 cudaError_t launch_mask_pack_train(const float* w1, const float* b1, const float* w2, const float* b2, const float* w3,
                                    const float* b3, void* dst, cudaStream_t st);
 cudaError_t launch_mask_train_fwd(int P, int B, int H, int W, const float* pre0, const void* weights,
                                   const float* const* pred, const float* gt, const unsigned char* gtm,
                                   const float* scale, bool scale_on_device, bool save_maps, bool pred_grad,
-                                  float* partial, float* saved, cudaStream_t st, int* launches);
+                                  float* partial, float* saved, float* det_workspace, cudaStream_t st, int* launches);
 cudaError_t launch_mask_bwd(int P, int B, int H, int W, const void* weights, const float* saved, const float* gscale,
                             void* workspace, float* grad_pre0, float* gw1, float* gb1, float* gw2, float* gb2,
                             float* gw3, float* gb3, float* const* grad_pred, cudaStream_t st, int* launches);

@@ -285,7 +285,7 @@ struct MaskTrainParams {
   float* __restrict__ partial;        // [ntiles][P] loss partials
   float* __restrict__ saved;          // h0, h1, h2 (B,128,H,W) each, or NULL
   float* __restrict__ dlog;           // d_logits (B,128,H,W) + (B,16,H,W), or NULL
-  float* __restrict__ gpred;          // P x (B,2,H,W) prediction gradients, accumulated; or NULL
+  float* __restrict__ gpred;          // P x (B,2,H,W) prediction gradients, accumulated; or NULL.  DET: the workspace
   const float* __restrict__ scale_dev;  // DEV_SCALE: P device floats read in place of `scale`
 };
 
@@ -295,7 +295,10 @@ struct MaskTrainParams {
 // prediction's 3x3 neighbourhood, gathered per tile in shared memory and added to global memory once per tile.
 // DEV_SCALE: the prediction scales are read from device memory (p.scale_dev) at run time, so that a captured graph takes
 // them from memory; otherwise they are the kernel parameters p.scale.
-template <bool DEV_SCALE>
+// DET: no neighbourhood gradients; p.gpred is a workspace to which each supervised sub-pixel writes its softmax weights
+// (B,144,H,W) and, after them, per prediction its (d mu, d sigma) (P*B,2,4H,4W); upsample_gather_kernel then sums them
+// into the prediction gradients in a fixed order.
+template <bool DEV_SCALE, bool DET>
 __global__ void __launch_bounds__(NT, 1) mask_train_fwd_kernel(const MaskTrainParams p) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ float red[NT / 32][MAX_PRED];
@@ -311,7 +314,9 @@ __global__ void __launch_bounds__(NT, 1) mask_train_fwd_kernel(const MaskTrainPa
     const float* vs = reinterpret_cast<const float*>(p.weights + M_VEC);
     for (int i = tid; i < M_NVEC; i += NT) vec[i] = __ldg(vs + i);
   }
-  const bool want_pg = p.gpred != nullptr;
+  const bool want_pg = !DET && p.gpred != nullptr;
+  float* const det_w = p.gpred;
+  float* const det_g = p.gpred + (size_t)NOUT * p.B * p.H * p.W;
   if (want_pg)
     for (int i = tid; i < p.P * 2 * HP; i += NT) gacc[i] = 0.0f;
   const int* shw = reinterpret_cast<const int*>(p.weights + M_HDR);
@@ -424,6 +429,11 @@ __global__ void __launch_bounds__(NT, 1) mask_train_fwd_kernel(const MaskTrainPa
               const float g_mu = s * d / var;
               // var[var < 1e-10] = 1e-10 (losses.py:45) cuts the gradient to sigma where it clamps
               const float g_sg = (sg * sg < 1e-10f) ? 0.0f : s * (1.0f / sg - (d * d) / (var * sg));
+              if constexpr (DET) {
+                const size_t full = (size_t)HW * K_UP * K_UP, og = ((size_t)pp * p.B + b) * 2 * full + o + e - b * full;
+                det_g[og] = g_mu;
+                det_g[og + full] = g_sg;
+              }
               float tt[9];
 #pragma unroll
               for (int i = 0; i < 9; ++i) {
@@ -443,6 +453,11 @@ __global__ void __launch_bounds__(NT, 1) mask_train_fwd_kernel(const MaskTrainPa
               for (int i = 0; i < 9; ++i) dot = __fmaf_rn(w[i], tt[i], dot);
 #pragma unroll
               for (int i = 0; i < 9; ++i) dl[i] = __fadd_rn(dl[i], w[i] * (tt[i] - dot));
+            }
+            if constexpr (DET) {
+              float* wp = det_w + ((size_t)b * NOUT + ky * K_UP + kx + e) * HW + (size_t)y * W + x;
+#pragma unroll
+              for (int i = 0; i < 9; ++i) wp[(size_t)i * K_UP * K_UP * HW] = w[i];
             }
           }
 #pragma unroll
@@ -585,6 +600,9 @@ __global__ void __launch_bounds__(256) scale_grads_kernel(const ScaleList l, con
 size_t mask_train_weights_bytes() { return M_BYTES + S_WT; }
 int mask_train_partials(int B, int H, int W) { return B * ((H + TY - 1) / TY) * ((W + TX - 1) / TX); }
 size_t mask_saved_bytes(int P, int B, int H, int W) { return (size_t)(3 * HID + NOUT + 2 * P) * B * H * W * 4; }
+size_t mask_train_det_workspace_bytes(int P, int B, int H, int W) {
+  return (size_t)(9 + 2 * P) * K_UP * K_UP * B * H * W * 4;
+}
 size_t mask_bwd_workspace_bytes(int B, int H, int W) {
   return align256((size_t)2 * HID * B * H * W * 4) + head_wgrad_partial_floats(B, H, W, HID, HID) * 4;
 }
@@ -603,11 +621,13 @@ cudaError_t launch_mask_pack_train(const float* w1, const float* b1, const float
 cudaError_t launch_mask_train_fwd(int P, int B, int H, int W, const float* pre0, const void* weights,
                                   const float* const* pred, const float* gt, const unsigned char* gtm,
                                   const float* scale, bool scale_on_device, bool save_maps, bool pred_grad,
-                                  float* partial, float* saved, cudaStream_t st, int* launches) {
-  static std::once_flag flags[2][64];
+                                  float* partial, float* saved, float* det_workspace, cudaStream_t st, int* launches) {
+  static std::once_flag flags[2][2][64];
   int dev = 0;
-  const auto kern = scale_on_device ? mask_train_fwd_kernel<true> : mask_train_fwd_kernel<false>;
-  cudaError_t e = set_smem_once(kern, flags[scale_on_device], (int)smem_train(MAX_PRED), false, &dev);
+  const bool det = pred_grad && det_workspace;
+  const auto kern = det ? (scale_on_device ? mask_train_fwd_kernel<true, true> : mask_train_fwd_kernel<false, true>)
+                        : (scale_on_device ? mask_train_fwd_kernel<true, false> : mask_train_fwd_kernel<false, false>);
+  cudaError_t e = set_smem_once(kern, flags[det][scale_on_device], (int)smem_train(MAX_PRED), false, &dev);
   if (e != cudaSuccess) return e;
   const size_t map = (size_t)B * H * W;
   MaskTrainParams p;
@@ -628,14 +648,16 @@ cudaError_t launch_mask_train_fwd(int P, int B, int H, int W, const float* pre0,
   float* maps = saved + (size_t)2 * P * map;
   p.saved = save_maps ? maps : nullptr;
   p.dlog = save_maps ? maps + 3 * HID * map : nullptr;
-  p.gpred = pred_grad ? saved : nullptr;
+  p.gpred = det ? det_workspace : pred_grad ? saved : nullptr;
   *launches = 1;
-  if (pred_grad) {
+  if (pred_grad && !det) {
     if ((e = cudaMemsetAsync(p.gpred, 0, (size_t)P * 2 * map * 4, st)) != cudaSuccess) return e;
     ++*launches;
   }
   kern<<<std::min(p.ntiles, sm_count(dev)), NT, smem_train(P), st>>>(p);   // persistent
-  return cudaGetLastError();
+  if ((e = cudaGetLastError()) != cudaSuccess || !det) return e;
+  ++*launches;
+  return launch_mask_pred_gather(det_workspace + (size_t)NOUT * map, det_workspace, gtm, P, B, H, W, K_UP, saved, st);
 }
 
 // Launches: the chain kernel (when a gradient below the logits is asked for), per requested (weight, bias) pair of

@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import warnings
 from typing import Optional, Sequence
 
 import torch
@@ -29,6 +30,26 @@ def _traced() -> bool:
 
 def _op(name: str):
     return getattr(torch.ops.magnet_b200, name)
+
+
+def _deterministic() -> bool:
+    """Whether torch.use_deterministic_algorithms is on.  The backward wrappers then run the fixed-order ``_det`` entry
+    points, whose results are bit-identical from run to run (DESIGN §3.20); with the flag off they run the atomic ones.
+    Read when the wrapper runs: a CUDA graph keeps the choice made when it was captured."""
+    return torch.are_deterministic_algorithms_enabled()
+
+
+def _alert_not_deterministic(what: str) -> None:
+    """What torch does for an op without a deterministic form under torch.use_deterministic_algorithms: raise, or warn
+    with ``warn_only=True``.  Nothing with the flag off."""
+    if not _deterministic():
+        return
+    msg = (f"{what} accumulates with float atomics and has no deterministic implementation, but "
+           "torch.use_deterministic_algorithms(True) is set (DESIGN §3.20)")
+    if torch.is_deterministic_algorithms_warn_only_enabled():
+        warnings.warn(msg)
+    else:
+        raise RuntimeError(msg)
 
 
 def _no_out_traced(out) -> None:
@@ -473,6 +494,7 @@ def cost_volume_f_bwd(ref_feat, src_feat_nchw, rays, cams, planes, V, prob, grad
             _check_packed(nm, buf, split_layout, n, H, W)
     dev = _same_device(("ref_feat", ref_feat), ("src_feat", src), *named, ("prob", prob if softmax else None),
                        ("grad_out", grad_out), ("ref_split", ref_split), ("src_split", src_split))
+    _alert_not_deterministic("magnet_cost_volume_f_bwd_f32 (grad_src)")
     a.consistency, a.softmax = 0, 1 if softmax else 0
     a.src_layout = split_layout if split else _lib.SRC_NCHW
     a.ref_feat, a.src_feat = (ref_split.data_ptr(), src_split.data_ptr()) if split else (ref_feat.data_ptr(), src.data_ptr())
@@ -511,10 +533,15 @@ def cost_volume_bwd(ref_feat, src_feat, src_gmm, rays, cams, grad_out, *, V: int
     a, gd_shape, named = _cost_args(ref_feat, V, rays, cams, d_volume=d_volume, ref_gmm=ref_gmm, k=k)
     a.src_layout, a.variant, a.consistency, a.softmax, a.kappa = fwd_layout, fwd_variant, 1 if consistency else 0, 0, float(kappa)
     _expect("grad_out", grad_out, (B, a.D, H, W))
-    if fwd_layout in PACKED_LAYOUTS and (ref_split is not None or src_split is not None):
+    tensor_cores = fwd_layout in PACKED_LAYOUTS and (ref_split is not None or src_split is not None)
+    if tensor_cores:
         for nm, buf, nimg in (("src_split", src_split, V * B), ("ref_split", ref_split, B)):
             _check_packed(nm, buf, fwd_layout, nimg, H, W)
         a.ref_feat, a.src_feat = ref_split.data_ptr(), src_split.data_ptr()
+    if need_src:
+        _alert_not_deterministic("magnet_cost_volume_bwd_f32 (grad_src)")
+    elif need_ref and tensor_cores:
+        _alert_not_deterministic("magnet_cost_volume_bwd_f32 (tensor-core grad_ref)")
     bw = _lib.CostBwdArgs()
     bw.fwd = C.pointer(a)
     if not shape_only:                             # the NCHW maps are read (CUDA-core kernel)
@@ -837,14 +864,17 @@ class ConvexUpsample(torch.autograd.Function):
 
 
 def convex_upsample_bwd(grad_out, depth, up_mask, k: int):
-    """The gradients of ``convex_upsample`` w.r.t. (depth, up_mask): one magnet_convex_upsample_bwd_f32 launch."""
+    """The gradients of ``convex_upsample`` w.r.t. (depth, up_mask): magnet_convex_upsample_bwd_f32, or under
+    torch.use_deterministic_algorithms its fixed-order form magnet_convex_upsample_bwd_det_f32."""
     grad_out = _need_cuda_f32("grad_out", grad_out)
     depth, up_mask = _need_cuda_f32("depth", depth), _need_cuda_f32("up_mask", up_mask)
     B, CH, H, W = depth.shape
-    g_depth = torch.zeros_like(depth)
+    det = _deterministic()
+    g_depth = torch.empty_like(depth) if det else torch.zeros_like(depth)
     g_mask = torch.empty_like(up_mask)
-    _launch(depth.device, "magnet_convex_upsample_bwd_f32", grad_out.data_ptr(), depth.data_ptr(),
-            up_mask.data_ptr(), B, CH, H, W, k, g_depth.data_ptr(), g_mask.data_ptr())
+    name = "magnet_convex_upsample_bwd_det_f32" if det else "magnet_convex_upsample_bwd_f32"
+    _launch(depth.device, name, grad_out.data_ptr(), depth.data_ptr(), up_mask.data_ptr(), B, CH, H, W, k,
+            g_depth.data_ptr(), g_mask.data_ptr())
     return g_depth, g_mask
 
 
@@ -1134,7 +1164,8 @@ def mask_saved_floats(P: int, B: int, H: int, W: int, save_maps: bool) -> int:
 def mask_train_fwd(pre0, weights, preds, gt, gt_mask_u8, save_maps: bool, pred_grad: bool, scales):
     """The forward of ``MaskLossTrain``: the weights W1, b1, W2, b2, W3, b3 packed for training, then the fused forward
     (two launches).  ``scales``: the P prediction scales gamma_p / count, a list of host floats, or a (P,) float32 device
-    tensor that the kernel reads when it runs (magnet_mask_train_fwd_dev_f32).  Returns (loss partials
+    tensor that the kernel reads when it runs (magnet_mask_train_fwd_dev_f32).  With ``pred_grad`` under
+    torch.use_deterministic_algorithms, the fixed-order forms (the _det entry points) run.  Returns (loss partials
     [tiles x P], packed weights, saved)."""
     P = len(preds)
     if not 1 <= P <= _lib.MAGNET_MASK_MAX_PRED:
@@ -1159,16 +1190,20 @@ def mask_train_fwd(pre0, weights, preds, gt, gt_mask_u8, save_maps: bool, pred_g
     packed = torch.empty(int(lib().magnet_mask_train_weights_bytes(4)), device=dev, dtype=torch.uint8)
     partial = torch.empty(int(lib().magnet_mask_train_partials(B, H, W)) * P, device=dev, dtype=torch.float32)
     saved = torch.empty(mask_saved_floats(P, B, H, W, save_maps), device=dev, dtype=torch.float32)
+    det = pred_grad and _deterministic()
+    work = (torch.empty(int(lib().magnet_mask_train_det_workspace_bytes(P, B, H, W)), device=dev, dtype=torch.uint8)
+            if det else None)
     a = _lib.MaskTrainArgs(P=P, B=B, H=H, W=W, k=4, pre0=pre0.data_ptr(), packed_weights=packed.data_ptr(),
                            pred=C.cast(pp, C.POINTER(C.c_void_p)), gt=gt.data_ptr(), gt_mask=gt_mask_u8.data_ptr(),
                            pred_scale=None if on_device else C.cast(host_scale, C.POINTER(C.c_float)),
                            save_maps=int(save_maps), pred_grad=int(pred_grad), partial=partial.data_ptr(),
-                           saved=saved.data_ptr())
+                           saved=saved.data_ptr(), workspace=_ptr(work))
     _launch(dev, "magnet_mask_pack_train_weights_f32", *(t.data_ptr() for t in ws), packed.data_ptr())
+    suffix = "_det_f32" if det else "_f32"
     if on_device:
-        _launch(dev, "magnet_mask_train_fwd_dev_f32", C.byref(a), scales.data_ptr())
+        _launch(dev, "magnet_mask_train_fwd_dev" + suffix, C.byref(a), scales.data_ptr())
     else:
-        _launch(dev, "magnet_mask_train_fwd_f32", C.byref(a))
+        _launch(dev, "magnet_mask_train_fwd" + suffix, C.byref(a))
     return partial, packed, saved
 
 
@@ -1261,6 +1296,9 @@ class UpsampleNLL(torch.autograd.Function):
 # of an upsampled [mu, sigma] and, with dnet=True, DnetLoss of the upsampled raw [mu, v] through activation_G
 _NLL_ENTRY = {False: ("magnet_upsample_nll_fwd_f32", "magnet_upsample_nll_bwd_f32", "magnet_upsample_nll_bwd_dev_f32"),
               True: ("magnet_dnet_nll_fwd_f32", "magnet_dnet_nll_bwd_f32", "magnet_dnet_nll_bwd_dev_f32")}
+# their fixed-order backwards (host scale, device scale), which take a workspace
+_NLL_DET_ENTRY = {False: ("magnet_upsample_nll_bwd_det_f32", "magnet_upsample_nll_bwd_dev_det_f32"),
+                  True: ("magnet_dnet_nll_bwd_det_f32", "magnet_dnet_nll_bwd_dev_det_f32")}
 
 
 def upsample_nll_fwd(depth, up_mask, gt, gt_mask_u8, k: int, dnet: bool = False):
@@ -1284,22 +1322,32 @@ def upsample_nll_fwd(depth, up_mask, gt, gt_mask_u8, k: int, dnet: bool = False)
 def upsample_nll_bwd(depth, up_mask, gt, gt_mask_u8, k: int, scale, dnet: bool = False):
     """The gradients of ``UpsampleNLL`` (DnetLoss's with ``dnet``) w.r.t. (depth, up_mask) at ``scale`` = upstream
     gradient / count: a host float (magnet_upsample_nll_bwd_f32 / magnet_dnet_nll_bwd_f32), or a 1-element float32
-    device tensor the kernel reads when it runs (the _dev_f32 entry points)."""
+    device tensor the kernel reads when it runs (the _dev_f32 entry points).  Under
+    torch.use_deterministic_algorithms the fixed-order forms (the _det entry points) run."""
     name = "raw" if dnet else "depth"
     depth, up_mask, gt = _need_cuda_f32(name, depth), _need_cuda_f32("up_mask", up_mask), _need_cuda_f32("gt", gt)
     B, _, H, W = depth.shape
     # the kernel reads the mask by address: a traced caller's mask may be strided (a permuted or channels-last bool)
     gt_mask_u8 = _need_cuda_u8_mask("gt_mask", gt_mask_u8, (B, 1, k * H, k * W), "(B,1,k*H,k*W)")
-    g_depth = torch.zeros_like(depth)
     g_mask = torch.empty_like(up_mask)
-    _, host, on_device = _NLL_ENTRY[bool(dnet)]
     if isinstance(scale, torch.Tensor):
         scale = _need_cuda_f32("scale", scale.reshape(1))
+    if _deterministic():
+        g_depth = torch.empty_like(depth)
+        work = torch.empty(int(lib().magnet_upsample_nll_bwd_det_workspace_bytes(B, H, W, k)) // 4,
+                           device=depth.device, dtype=torch.float32)
+        host, on_device = _NLL_DET_ENTRY[bool(dnet)]
+        outs = (work.data_ptr(), g_depth.data_ptr(), g_mask.data_ptr())
+    else:
+        g_depth = torch.zeros_like(depth)
+        _, host, on_device = _NLL_ENTRY[bool(dnet)]
+        outs = (g_depth.data_ptr(), g_mask.data_ptr())
+    if isinstance(scale, torch.Tensor):
         _launch(depth.device, on_device, depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(),
-                gt_mask_u8.data_ptr(), scale.data_ptr(), B, H, W, k, g_depth.data_ptr(), g_mask.data_ptr())
+                gt_mask_u8.data_ptr(), scale.data_ptr(), B, H, W, k, *outs)
     else:
         _launch(depth.device, host, depth.data_ptr(), up_mask.data_ptr(), gt.data_ptr(),
-                gt_mask_u8.data_ptr(), scale, B, H, W, k, g_depth.data_ptr(), g_mask.data_ptr())
+                gt_mask_u8.data_ptr(), scale, B, H, W, k, *outs)
     return g_depth, g_mask
 
 
